@@ -1,20 +1,21 @@
 #!/usr/bin/env python
-"""bench.py — samples/s of PERSIA's sparse-embedding hot path on B200 (BASELINE.json metric).
+"""bench.py — samples/s of PERSIA's sparse-embedding hot path on H100 (BASELINE.json metric).
 
 A "step" is one pass of the hot path over one batch of synthetic Criteo-shaped ids: training forward
 (prefix -> per-slot dedup -> find-or-admit over the distinct signs -> gather+pool -> f16) and backward (NaN rule ->
 in-order gradient reduce per sign -> Adagrad update).
 
 BASELINE.json names two things, measured by two legs:
-  * metric leg — "samples/sec (26 slots, dim128) at 1/2/4/8 B200": dim 128, 8192 samples per GPU (configs[3]'s
-    65536 / 8), 1e8 resident rows per GPU, Adagrad.  This is `value` / `e2e` at every N (weak scaling: per-GPU work is
+  * metric leg — "samples/sec (26 slots, dim128) at 1/2/4/8 GPUs": dim 128, 8192 samples per GPU (configs[3]'s
+    65536 / 8), 5e7 resident rows per GPU (51 GB of rows + optimizer state: what fits in an 80 GB H100), Adagrad.  This is `value` / `e2e` at every N (weak scaling: per-GPU work is
     fixed).  At N >= 2 the rows are hash-sharded over the GPUs and the exchange runs inside the kernels (configs[2]); at
     N = 8 the ids are drawn from a 1e10 key space over a capacity-bounded table with eviction on (configs[3]).
-  * roofline leg — configs[1], "1xB200: 26 slots, 1e8 rows, dim-64, batch 4096, GPU hash lookup + sparse Adagrad,
-    HBM GB/s vs roofline": run at N = 1 only; `roofline` comes from it.
+  * roofline leg — configs[1]'s shape, "26 slots, dim-64, batch 4096, GPU hash lookup + sparse Adagrad, HBM GB/s vs
+    roofline", over the same --rows resident rows: run at N = 1 only; `roofline` comes from it.
 
   python bench.py [--gpus N --steps K --warmup W]            our arm (CUDA, through the C ABI)
   python bench.py --impl reference [...]                     the reference's CPU path (oracle port) on host cores
+  python bench.py --dump-outputs DIR [...]                   also writes what the last timed step computed (DIR/*.npy)
 
 Prints ONE JSON line (rank 0).  See DESIGN.md §Measurement for every field.
 """
@@ -44,7 +45,7 @@ def parse_args():
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--rows", type=float, default=float(os.environ.get("PB_BENCH_ROWS", 1e8)),
+    ap.add_argument("--rows", type=float, default=float(os.environ.get("PB_BENCH_ROWS", 5e7)),
                     help="resident rows per GPU (weak scaling: the table grows with N)")
     ap.add_argument("--batch", type=int, default=8192, help="samples per GPU per step (metric leg)")
     ap.add_argument("--dim", type=int, default=128, help="embedding dim of the metric leg")
@@ -62,6 +63,9 @@ def parse_args():
     ap.add_argument("--no-staleness", action="store_true", help="skip the 2 / 4 batches-in-flight measurement")
     ap.add_argument("--no-kernel-table", action="store_true", help="N > 1: skip the per-kernel-family timing pass")
     ap.add_argument("--no-graph", action="store_true", help="launch kernel by kernel instead of replaying CUDA graphs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="N = 1: after the metric leg's timed steps, write a fixed sample of what its last step computed "
+                         "(forward output, updated table rows) as DIR/<name>.npy, float32")
     return ap.parse_args()
 
 
@@ -89,7 +93,7 @@ def workload_config(args):
 
 
 # ------------------------------------------------------------------------------------------------------
-# clocks: nvidia-smi sampled DURING the timed region (B200_PROFILING.md recipe)
+# clocks: nvidia-smi sampled DURING the timed region
 # ------------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -276,13 +280,38 @@ def b200_main(args):
 
 
 def peak_hbm():
-    peaks = {}
+    return 3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 (not a measured peak)"
+
+
+def gpu_info(torch, gpu_index=0):
+    """Name, power limit and top SM clock of the card the numbers were measured on (a power-limited card clocks lower)."""
+    info = {"name": torch.cuda.get_device_name(gpu_index), "power_limit": None, "max_sm_clock": None}
     try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    return peak, ("MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)")
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader",
+                              "-i", str(gpu_index)], capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+    except (OSError, subprocess.SubprocessError):
+        return info
+    if len(out) == 2:
+        info["power_limit"], info["max_sm_clock"] = out[0].strip(), out[1].strip()
+    return info
+
+
+def dump_outputs(out_dir, torch, sh, out, ids, pf, S, B, dev):
+    """Writes what one training step computed, as float32 .npy files (about 44 MB at the default sizes):
+    forward_output.npy  [S, n, dim]  the pooled f16 embeddings of a fixed sample of n <= 2048 samples of every slot;
+    updated_rows.npy    [m, entry]   embedding ++ Adagrad state of a fixed sample of m <= 16384 of the distinct signs
+                                     of the step, read back after its update (signs in ascending order)."""
+    from persia_b200 import shard as SH
+
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(0)
+    samples = torch.from_numpy(np.sort(rng.choice(B, size=min(B, 2048), replace=False))).to(dev)
+    np.save(os.path.join(out_dir, "forward_output.npy"), out[:, samples].float().cpu().numpy())
+    signs = torch.unique(SH.add_prefix(torch.from_numpy(ids.view(np.int64)).to(dev), [s * B for s in range(S + 1)], pf))
+    pick = torch.from_numpy(np.sort(rng.choice(signs.numel(), size=min(signs.numel(), 16384), replace=False))).to(dev)
+    ent, found = sh.get_entries(signs[pick])
+    assert bool(found.all()), "a sign of the last step has no row"
+    np.save(os.path.join(out_dir, "updated_rows.npy"), ent.float().cpu().numpy())
 
 
 def fill_table(torch, SH, sh, card, pf, dev, dim, owner=None):
@@ -326,7 +355,7 @@ def kernel_bytes(stats, dim, state):
     }
 
 
-def run_leg(args, torch, dim, B, rows, name, want_kernels, want_parity):
+def run_leg(args, torch, dim, B, rows, name, want_kernels, want_parity, dump_dir=None):
     """One single-GPU leg: table of `rows` resident rows of `dim`, batches of B samples."""
     import ctypes as C
 
@@ -410,6 +439,8 @@ def run_leg(args, torch, dim, B, rows, name, want_kernels, want_parity):
         t1 = time.time()
         ms = e0.elapsed_time(e1)
         clocks = sampler.stop(t0, t1)
+        if dump_dir:
+            dump_outputs(dump_dir, torch, sh, outs[(K - 1) % n_sets], ids_host[(K - 1) % n_sets], pf, S, B, dev)
         reps = []
         for _ in range(3):  # run-to-run spread of the same K steps
             e0.record(stream)
@@ -635,8 +666,8 @@ def roofline_from(leg, peak, peak_src, label):
         "achieved": ach, "peak": peak, "unit": "GB/s", "frac": (ach / peak) if ach else None,
         "frac_worst_case": by["whole_step_worst_case"] / step_s / 1e9 / peak,
         "traffic": None,
-        "traffic_note": "not measured by this run: profiles/ holds the ncu --set full capture of this command "
-                        "(dram__bytes_read.sum + dram__bytes_write.sum per kernel) and its command line",
+        "traffic_note": "not measured by this run: DRAM bytes actually moved need a hardware-counter profiler "
+                        "(dram__bytes_read.sum + dram__bytes_write.sum per kernel)",
         "peak_source": peak_src,
         "bytes_model": "measured multiplicities of the batch: N occurrences, U distinct (slot, sign) pairs, of which `cold` occur "
                        "once, `warm` 2..32 times (their occurrences are counted), `hot` more.  k_reduce_cold = cold x (8 + "
@@ -716,14 +747,14 @@ def single_gpu(args, torch):
     roof_leg = None
     if not args.no_roofline_leg:
         roof_leg = run_leg(args, torch, 64, 4096, rows, "roofline leg (configs[1])", True, not args.no_parity)
-    leg = run_leg(args, torch, args.dim, args.batch, rows, "metric leg", True, not args.no_parity)
+    leg = run_leg(args, torch, args.dim, args.batch, rows, "metric leg", True, not args.no_parity, args.dump_outputs)
     B, K = args.batch, args.steps
     S = args.slots
     n_occ = S * B
     value = B / (leg["ms_per_step"] * 1e-3)
     metric_roof = roofline_from(leg, peak, peak_src, f"the metric leg: dim {args.dim}, batch {B}, {rows:.3g} rows")
     if roof_leg:
-        roofline = roofline_from(roof_leg, peak, peak_src, "configs[1]: dim 64, batch 4096, 1e8 rows")
+        roofline = roofline_from(roof_leg, peak, peak_src, f"configs[1] shape: dim 64, batch 4096, {rows:.3g} rows")
         roofline["metric_leg"] = {k: metric_roof[k] for k in ("achieved", "frac", "frac_worst_case", "kernels", "whole_step",
                                                               "unique_fraction", "batch_stats")}
     else:
@@ -750,10 +781,10 @@ def single_gpu(args, torch):
                                       **leg["in_flight"],
                                       "roofline_leg": roof_leg["in_flight"] if roof_leg else None},
                 "roofline_leg": None if not roof_leg else {
-                    "workload": "configs[1]: 26 slots, 1e8 rows, dim 64, batch 4096, Adagrad", "ms_per_step": roof_leg["ms_per_step"],
+                    "workload": f"configs[1] shape: 26 slots, {rows:.3g} rows, dim 64, batch 4096, Adagrad", "ms_per_step": roof_leg["ms_per_step"],
                     "samples_per_s": 4096 / (roof_leg["ms_per_step"] * 1e-3), "ms_per_step_repetitions": roof_leg["ms_per_step_reps"],
                     "e2e_samples_per_s": 4096 / (roof_leg["ms_e2e"] * 1e-3), "parity": roof_leg["parity"]}},
-        "clocks": leg["clocks"],
+        "gpu": gpu_info(torch, torch.cuda.current_device()), "clocks": leg["clocks"],
         "e2e": {"value": B / (leg["ms_e2e"] * 1e-3), "unit": UNIT, "h2d_bytes_per_step": n_occ * 8,
                 "d2h_bytes_per_step": S * 4, "ms_per_step": leg["ms_e2e"],
                 "path": "pinned host ids -> H2D (copy stream, one step ahead) -> pb_forward -> pb_backward -> D2H slot status read by the host every step, one step behind the launches"},

@@ -1,4 +1,4 @@
-/* persia_b200.h — C ABI of libpersia_b200.so: PERSIA's sparse-embedding hot path on B200 (sm_100a).
+/* persia_b200.h — C ABI of libpersia_b200.so: PERSIA's sparse-embedding hot path on H100 (sm_90a).
  *
  * The reference (PersiaML/PERSIA @ ff754b8) has no FFI for this path: its NN-worker engine
  * (rust/persia-core) talks to an embedding worker and R parameter servers over HTTP.  These entry

@@ -5,8 +5,8 @@
 // cpu_baseline / --impl reference legs of bench.py use it, as the checker and
 // as the timed CPU baseline.
 //
-// The reference (PersiaML/PERSIA @ ff754b8) is Rust and cannot be compiled in
-// this image (no cargo/rustc), so this is a C++17 restatement, function by
+// The reference (PersiaML/PERSIA @ ff754b8) is Rust, which this project does
+// not build, so this is a C++17 restatement, function by
 // function, of the files cited below (paths relative to the reference root).
 // It is pinned against every golden vector the reference's own unit tests hold
 // for this path (tests/test_oracle_golden.py):

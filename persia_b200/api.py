@@ -1,9 +1,9 @@
 """The `persia` Python API over libpersia_b200 — host-side mirror of the reference's user-facing layer.
 
 The reference's `persia/ctx.py`, `persia/embedding/{__init__,optim,data}.py` sit on the PyO3 module `persia_core`.
-persia_b200.persia_core re-exposes that module surface, and the reference's own `persia` package runs unchanged on
-it where /root/reference exists (tests/test_persia_core_surface.py).  On a box without the reference tree this module
-provides the same names, arguments and behaviour, written from scratch against the same surface, so that a user script
+persia_b200.persia_core re-exposes that module surface (tests/test_persia_core_surface.py).  This module provides
+the same names, arguments and behaviour as the reference's `persia` package, written from scratch against the same
+surface, so that a user script
 
     from persia_b200.api import TrainCtx, PersiaBatch, IDTypeFeatureWithSingleID, Label, NonIDTypeFeature, Adagrad, EmbeddingConfig
 

@@ -1,4 +1,4 @@
-"""Builds libpersia_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo)."""
+"""Builds libpersia_b200.so in-tree with nvcc for H100 (sm_90a); no JIT cache: the .so travels with the repo."""
 import os
 import shutil
 import subprocess
@@ -22,7 +22,7 @@ def stale():
     if not os.path.exists(SO):
         return True
     t = os.path.getmtime(SO)
-    deps = [os.path.join(CSRC, s) for s in SOURCES] + [h if os.path.isabs(h) else os.path.join(CSRC, h) for h in HEADERS]
+    deps = [os.path.abspath(__file__)] + [os.path.join(CSRC, s) for s in SOURCES] + [h if os.path.isabs(h) else os.path.join(CSRC, h) for h in HEADERS]
     return any(os.path.getmtime(d) > t for d in deps)
 
 
@@ -30,7 +30,7 @@ def build(force=False, verbose=False):
     if not force and not stale():
         return SO
     cmd = [
-        nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+        nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
         "--fmad=false",  # the optimizer reproduces the reference's fused / unfused structure explicitly
         "-Xcompiler", "-fPIC", "-shared", "-cudart", "shared",
         "-I", os.path.join(ROOT, "include"), "-I", CSRC,

@@ -1,4 +1,4 @@
-// pb_common.cuh — shared device helpers for libpersia_b200 (sm_100a only).
+// pb_common.cuh — shared device helpers for libpersia_b200 (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -15,6 +15,7 @@ constexpr uint32_t ROW_PENDING = 0xFFFFFFFFu;  // key claimed, row not yet publi
 constexpr uint32_t ROW_NONE = 0xFFFFFFFEu;     // key present but no storage (shard was full when it was admitted)
 constexpr uint32_t BUCKET = 8;                 // cells per bucket
 constexpr uint64_t PB_NULL_SIGN = 0xFFFFFFFFFFFFFFFEULL;  // padding of a framed shard exchange (owner-mode contexts only)
+constexpr uint32_t PB_NUM_SMS = 132;           // SMs of an H100 SXM: grid-stride kernels launch a small multiple of it
 
 // One cell of the index: 16 B.  Cells are grouped in buckets of BUCKET = 8 (one 128 B line): a sign's home
 // bucket is mix64(sign) & bucket_mask; a lookup reads whole buckets with 8 lanes, so the probe length is

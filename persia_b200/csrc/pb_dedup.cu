@@ -270,7 +270,7 @@ __global__ void k_fill_set(DCell* set, uint64_t n) {
 // ------------------------------------------------------------------------------------------------
 // launchers (host)
 // ------------------------------------------------------------------------------------------------
-void launch_fill_set(DCell* set, uint64_t n, cudaStream_t st) { PB_LAUNCH(k_fill_set, 148 * 4, 256, 0, st, set, n); }
+void launch_fill_set(DCell* set, uint64_t n, cudaStream_t st) { PB_LAUNCH(k_fill_set, PB_NUM_SMS * 4, 256, 0, st, set, n); }
 
 void launch_dedup(const SlotsDev& sl, const BatchDev& b, const uint64_t* ids, cudaStream_t st) {
   if (b.n) PB_LAUNCH_F(FAM_DEDUP, (k_dedup<true>), cdiv(b.n, 256), 256, 0, st, sl, b, ids);
@@ -280,7 +280,7 @@ void launch_probe_items(bool training, const TableDev& t, const HyperDev& hy, co
                         const BatchDev& b, cudaStream_t st) {
   if (!b.n) return;
   uint32_t grid = cdiv((uint64_t)b.n * BUCKET, 256);  // worst case U = N
-  if (grid > 148u * 4u) grid = 148u * 4u;              // the blocks stride over the items
+  if (grid > PB_NUM_SMS * 4u) grid = PB_NUM_SMS * 4u;  // the blocks stride over the items
   if (training) PB_LAUNCH_F(FAM_PROBE, (k_probe_items<MODE_TRAIN>), grid, 256, 0, st, t, hy, op, sl, b);
   else PB_LAUNCH_F(FAM_PROBE, (k_probe_items<MODE_FIND>), grid, 256, 0, st, t, hy, op, sl, b);
 }
@@ -314,12 +314,12 @@ void launch_gather_items(const TableDev& t, const SlotsDev& sl, const BatchDev& 
   }
 }
 
-void launch_clear_hot_bits(const BatchDev& b, cudaStream_t st) { PB_LAUNCH(k_clear_hot_bits, 148, 256, 0, st, b); }
+void launch_clear_hot_bits(const BatchDev& b, cudaStream_t st) { PB_LAUNCH(k_clear_hot_bits, PB_NUM_SMS, 256, 0, st, b); }
 
 void launch_clear_items(const BatchDev& b, cudaStream_t st) {
   if (!b.n) return;
   const uint32_t full = cdiv(b.n, 256);
-  PB_LAUNCH(k_clear_items, full < 148u * 4u ? full : 148u * 4u, 256, 0, st, b);
+  PB_LAUNCH(k_clear_items, full < PB_NUM_SMS * 4u ? full : PB_NUM_SMS * 4u, 256, 0, st, b);
 }
 
 }  // namespace pb

@@ -236,7 +236,7 @@ __global__ void __launch_bounds__(256) k_evict_sweep_spill(TableDev t, uint32_t*
 // ------------------------------------------------------------------------------------------------
 // launchers (host)
 // ------------------------------------------------------------------------------------------------
-void launch_fill_cells(Cell* cells, uint64_t n, cudaStream_t st) { PB_LAUNCH(k_fill_cells, 148 * 8, 256, 0, st, cells, n); }
+void launch_fill_cells(Cell* cells, uint64_t n, cudaStream_t st) { PB_LAUNCH(k_fill_cells, PB_NUM_SMS * 8, 256, 0, st, cells, n); }
 
 void launch_begin_batch(const TableDev& t, uint32_t* ctx_tick, uint32_t* batch_cnt, cudaStream_t st, bool bump) {
   PB_LAUNCH(k_begin_batch, 1, batch_cnt ? 256 : 32, 0, st, t.counters, ctx_tick, batch_cnt, bump ? 1 : 0);
@@ -310,22 +310,22 @@ __global__ void __launch_bounds__(256) k_export_signs(TableDev t, uint64_t* __re
 void launch_export_signs(const TableDev& t, uint64_t* signs, uint32_t* recency, uint32_t max_n, uint32_t* count,
                          cudaStream_t st) {
   cudaMemsetAsync(count, 0, sizeof(uint32_t), st);
-  PB_LAUNCH(k_export_signs, 148 * 8, 256, 0, st, t, signs, recency, max_n, count);
+  PB_LAUNCH(k_export_signs, PB_NUM_SMS * 8, 256, 0, st, t, signs, recency, max_n, count);
 }
 
 void launch_spill(const TableDev& t, uint32_t want_free, uint32_t keep, uint32_t* ev, uint64_t* signs, float* entries,
                   uint32_t max_n, uint32_t* count, cudaStream_t st) {
   PB_LAUNCH(k_evict_plan, 1, 256, 0, st, t, want_free, want_free, ev);
-  PB_LAUNCH(k_evict_hist, 148 * 8, 256, 0, st, t, ev);
+  PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, t, ev);
   PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
-  PB_LAUNCH(k_evict_sweep_spill, 148 * 8, 256, 0, st, t, ev, signs, entries, max_n, count);
+  PB_LAUNCH(k_evict_sweep_spill, PB_NUM_SMS * 8, 256, 0, st, t, ev, signs, entries, max_n, count);
 }
 
 void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, cudaStream_t st) {
   PB_LAUNCH(k_evict_plan, 1, 256, 0, st, t, low_water, target_free, ev);
-  PB_LAUNCH(k_evict_hist, 148 * 8, 256, 0, st, t, ev);
+  PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, t, ev);
   PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
-  PB_LAUNCH(k_evict_sweep, 148 * 8, 256, 0, st, t, ev);
+  PB_LAUNCH(k_evict_sweep, PB_NUM_SMS * 8, 256, 0, st, t, ev);
 }
 
 void launch_shard_of(const uint64_t* signs, uint32_t n, uint32_t R, uint32_t* shard, uint64_t* hash, cudaStream_t st) {

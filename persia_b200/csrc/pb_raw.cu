@@ -283,14 +283,14 @@ void launch_raw_forward(const TableDev& t, const SlotsDev& sl, const uint64_t* i
 
 void launch_raw_nan(const void* grad, bool f16, const uint32_t* n_distinct, uint32_t dim, const uint32_t* tick,
                     uint32_t* nan_tick, cudaStream_t st) {
-  if (f16) PB_LAUNCH_F(FAM_NAN, k_raw_nan<true>, 148 * 2, 256, 0, st, grad, n_distinct, dim, tick, nan_tick);
-  else PB_LAUNCH_F(FAM_NAN, k_raw_nan<false>, 148 * 2, 256, 0, st, grad, n_distinct, dim, tick, nan_tick);
+  if (f16) PB_LAUNCH_F(FAM_NAN, k_raw_nan<true>, PB_NUM_SMS * 2, 256, 0, st, grad, n_distinct, dim, tick, nan_tick);
+  else PB_LAUNCH_F(FAM_NAN, k_raw_nan<false>, PB_NUM_SMS * 2, 256, 0, st, grad, n_distinct, dim, tick, nan_tick);
 }
 
 void launch_raw_stage(const void* grad, bool f16, const uint32_t* n_distinct, uint32_t dim, float inv_scale,
                       bool do_scale, float* out, cudaStream_t st) {
-  if (f16) PB_LAUNCH(k_raw_stage<true>, 148 * 4, 256, 0, st, grad, n_distinct, dim, inv_scale, do_scale ? 1 : 0, out);
-  else PB_LAUNCH(k_raw_stage<false>, 148 * 4, 256, 0, st, grad, n_distinct, dim, inv_scale, do_scale ? 1 : 0, out);
+  if (f16) PB_LAUNCH(k_raw_stage<true>, PB_NUM_SMS * 4, 256, 0, st, grad, n_distinct, dim, inv_scale, do_scale ? 1 : 0, out);
+  else PB_LAUNCH(k_raw_stage<false>, PB_NUM_SMS * 4, 256, 0, st, grad, n_distinct, dim, inv_scale, do_scale ? 1 : 0, out);
 }
 
 }  // namespace pb

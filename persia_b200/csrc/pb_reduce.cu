@@ -351,7 +351,7 @@ __global__ void __launch_bounds__(256) k_reduce_cold(TableDev t, OptimDev op, Hy
 //              sample, no scaling) has its own lean loop: ~25 instructions per 16 bytes is what bounds a producer.
 //   chain      (CH warps, 32 * EPL columns each) waits for the slot and adds its rows in order: one LDS and EPL
 //              dependent FADDs per row — nothing else — then arrives on `empty`; finally the optimizer step.
-// Measured alternatives (profiles/r2_hot_ubench_*.txt): cp.async.bulk of the rows into a raw ring + converter warps is
+// Measured alternatives (scripts/ubench/hot_ubench.cu): cp.async.bulk of the rows into a raw ring + converter warps is
 // bound by the copy engine's issue rate (~60 cycles per 128-byte copy and SM), a single warp doing load + convert + add
 // by the instruction stream (~40 cycles per row).
 // ------------------------------------------------------------------------------------------------
@@ -810,8 +810,8 @@ static void items_dispatch(const TableDev& t, const OptimDev& op, const HyperDev
   // grids sized for the worst case (every occurrence its own item); blocks past the list lengths return at once
   const uint32_t per_block = 256u / G;
   uint32_t grid_cold = cdiv(a.b.n, per_block), grid_warm = cdiv(a.b.n / 2 + 1, per_block);
-  if (grid_cold > 148u * 6u) grid_cold = 148u * 6u;  // groups stride over their list
-  if (grid_warm > 148u * 3u) grid_warm = 148u * 3u;
+  if (grid_cold > PB_NUM_SMS * 6u) grid_cold = PB_NUM_SMS * 6u;  // groups stride over their list
+  if (grid_warm > PB_NUM_SMS * 3u) grid_warm = PB_NUM_SMS * 3u;
   if (send) {
     PB_LAUNCH_F(FAM_WARM, (k_reduce_warm<VEC, F16, PB_OPT_SGD, true>), grid_warm, 256, 0, st_warm, t, op, hy, sl, gr, a, G);
     PB_LAUNCH_F(FAM_UPDATE, (k_reduce_cold<VEC, F16, PB_OPT_SGD, true>), grid_cold, 256, 0, st, t, op, hy, sl, gr, a, G);
@@ -872,7 +872,7 @@ static void hot_launch(const TableDev& t, const OptimDev& op, const HyperDev& hy
   uint32_t per_sm = 1;
   if (getenv("PB_HOT_PER_SM")) per_sm = (uint32_t)atoi(getenv("PB_HOT_PER_SM"));
   const uint32_t cap_blocks = cdiv(a.b.n, PB_WARM_MAX + 1);  // at most this many hot items exist
-  uint32_t grid = 148u * per_sm;
+  uint32_t grid = PB_NUM_SMS * per_sm;
   if (grid > cap_blocks) grid = cap_blocks ? cap_blocks : 1;
   PB_LAUNCH_F(FAM_HOT, kern, grid, HOT_THREADS, smem, st, t, op, hy, sl, gr, a, g, g_hot_trace);
 }

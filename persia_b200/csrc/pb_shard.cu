@@ -359,7 +359,7 @@ __global__ void k_owner_adam_pows(XchgDev x, float* table_pow, float b1, float b
 }
 void launch_owner_adam(const XchgDev& x, float* table_pow, float b1, float b2, cudaStream_t st) {
   const uint32_t full = cdiv((uint64_t)x.R * x.cap, 256);
-  PB_LAUNCH(k_owner_adam_present, full < 148u * 2u ? full : 148u * 2u, 256, 0, st, x);
+  PB_LAUNCH(k_owner_adam_present, full < PB_NUM_SMS * 2u ? full : PB_NUM_SMS * 2u, 256, 0, st, x);
   PB_LAUNCH(k_owner_adam_pows, 1, PB_ADAM_KEYS, 0, st, x, table_pow, b1, b2);
 }
 
@@ -577,7 +577,7 @@ void launch_wait(const XchgDev& x, int phase, int src, cudaStream_t st) {
 void launch_owner_lookup(bool training, const TableDev& t, const HyperDev& hy, const OptimDev& op, const XchgDev& x,
                          cudaStream_t st) {
   const uint32_t full = cdiv((uint64_t)x.R * x.cap * BUCKET, 256);
-  const uint32_t grid = full < 148u * PB_PROBE_BLOCKS ? full : 148u * PB_PROBE_BLOCKS;
+  const uint32_t grid = full < PB_NUM_SMS * PB_PROBE_BLOCKS ? full : PB_NUM_SMS * PB_PROBE_BLOCKS;
   if (training) {
     if (x.row_f32) PB_LAUNCH_F(FAM_PROBE, (k_owner_lookup<MODE_TRAIN, true>), grid, 256, 0, st, t, hy, op, x);
     else PB_LAUNCH_F(FAM_PROBE, (k_owner_lookup<MODE_TRAIN, false>), grid, 256, 0, st, t, hy, op, x);
@@ -615,7 +615,7 @@ void launch_expand_items(const TableDev& t, const SlotsDev& sl, const BatchDev& 
 #undef PB_E
 }
 
-void launch_uclear(const XchgDev& x, cudaStream_t st) { PB_LAUNCH(k_uclear, 148 * 4, 256, 0, st, x); }
+void launch_uclear(const XchgDev& x, cudaStream_t st) { PB_LAUNCH(k_uclear, PB_NUM_SMS * 4, 256, 0, st, x); }
 
 void launch_owner_update(const TableDev& t, const OptimDev& op, const HyperDev& hy, const XchgDev& x, uint32_t src,
                          cudaStream_t st);
@@ -632,7 +632,7 @@ void launch_owner_update_all(const TableDev& t, const OptimDev& op, const HyperD
   int vec, Gi;
   vec_group(t.dim, vec, Gi);  // Gi lanes cover a row with one chunk each (a power of two <= 32)
   const uint32_t full = cdiv((uint64_t)x.R * x.cap * 4u, 256);  // a warp per eight requests
-  const uint32_t grid = full < 148u * 6u ? full : 148u * 6u;
+  const uint32_t grid = full < PB_NUM_SMS * 6u ? full : PB_NUM_SMS * 6u;
   const uint32_t nvec = t.dim / (uint32_t)vec;
   const bool exact = (uint32_t)Gi == nvec;  // (rows longer than 32 chunks keep one chunk per lane and stride)
   if (vec == 4 && exact) owner_update_all_kind<4, 1>(t, op, hy, x, (uint32_t)Gi, grid, st);
@@ -649,7 +649,7 @@ void launch_owner_update(const TableDev& t, const OptimDev& op, const HyperDev& 
   vec_group(t.dim, vec, Gi);
   const uint32_t G = (uint32_t)Gi;
   const uint32_t full = cdiv((uint64_t)cdiv(x.cap, 2) * G, 256);
-  const uint32_t grid = full < 148u * 6u ? full : 148u * 6u;
+  const uint32_t grid = full < PB_NUM_SMS * 6u ? full : PB_NUM_SMS * 6u;
   if (vec == 4) PB_LAUNCH_F(FAM_UPDATE, (k_owner_update<4>), grid, 256, 0, st, t, op, hy, x, src, G);
   else PB_LAUNCH_F(FAM_UPDATE, (k_owner_update<1>), grid, 256, 0, st, t, op, hy, x, src, G);
 }

@@ -59,7 +59,7 @@ __global__ void k_zero_words(uint32_t* p, uint32_t n) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) p[i] = 0;
 }
 void launch_zero_words(uint32_t* p, uint32_t n_words, cudaStream_t st) {
-  if (n_words) PB_LAUNCH(k_zero_words, cdiv(n_words, 1024) < 148 ? cdiv(n_words, 1024) : 148, 256, 0, st, p, n_words);
+  if (n_words) PB_LAUNCH(k_zero_words, cdiv(n_words, 1024) < PB_NUM_SMS ? cdiv(n_words, 1024) : PB_NUM_SMS, 256, 0, st, p, n_words);
 }
 
 // d_work layout: [one pass's histogram region][n materialised shard ids]

@@ -98,7 +98,7 @@ void launch_nan_scan(const GradsDev& gr, uint32_t n_slots, uint32_t elems_per_sl
                      uint32_t* nan_tick, int32_t* status, cudaStream_t st) {
   uint32_t per = f16 ? elems_per_slot / 8 : elems_per_slot;
   uint32_t gx = cdiv(per ? per : 1, 256 * 4);
-  if (gx > 148 * 4) gx = 148 * 4;
+  if (gx > PB_NUM_SMS * 4) gx = PB_NUM_SMS * 4;
   dim3 grid(gx, n_slots);
   if (f16) PB_LAUNCH_F(FAM_NAN, k_nan_scan<true>, grid, 256, 0, st, gr, elems_per_slot, tick, nan_tick);
   else PB_LAUNCH_F(FAM_NAN, k_nan_scan<false>, grid, 256, 0, st, gr, elems_per_slot, tick, nan_tick);

@@ -1,5 +1,5 @@
 // micro-benchmarks behind k_reduce_hot's design: what one warp sustains for each pipeline role, alone and beside
-// warps parked on an mbarrier.  nvcc -O3 -gencode arch=compute_100a,code=sm_100a hot_ubench.cu -o hot_ubench
+// warps parked on an mbarrier.  nvcc -O3 -gencode arch=compute_90a,code=sm_90a hot_ubench.cu -o hot_ubench
 #include <cuda_fp16.h>
 #include <cstdio>
 #include <cstdlib>
@@ -374,7 +374,7 @@ int main(int argc, char** argv) {
   cudaFuncSetAttribute(k_bench2<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
   cudaFuncSetAttribute(k_bench2<512>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
   cudaFuncSetAttribute(k_bench2<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
-  for (int g_blocks : {1, 148}) {
+  for (int g_blocks : {1, 132}) {
     for (int mode : {7, 11, 8, 9}) {
       if (only >= 0 && mode != only) continue;
       for (int nt : {256, 512, 1024}) {
@@ -397,7 +397,7 @@ int main(int argc, char** argv) {
     }
   }
   cudaFuncSetAttribute(k_bench3, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
-  for (int g_blocks : {1, 148, 296}) {
+  for (int g_blocks : {1, 132, 264}) {
     for (int mode : {12, 13}) {
       if (only >= 0 && mode != only) continue;
       std::vector<long long> h(grid);

@@ -1,16 +1,17 @@
 """Extracts the little-endian golden vectors of persia-speedy's own test suite
-(/root/reference/rust/persia-speedy/tests/serialization_tests.rs, `symmetric_tests!` blocks) into
-tests/golden/speedy_vectors.json.  Run in the build container (the reference tree does not travel to the GPU box):
+(rust/persia-speedy/tests/serialization_tests.rs of a PERSIA checkout, `symmetric_tests!` blocks) into
+tests/golden/speedy_vectors.json, which the tests read:
 
-    python tests/golden/make_speedy_vectors.py
+    python tests/golden/make_speedy_vectors.py <path to the PERSIA checkout>
 
 Only the literal byte lists are copied (test data, not code); the `in = ...` expressions are kept as text so that
 tests/test_speedy_codec.py can show which Rust value each vector encodes."""
 import json
 import os
 import re
+import sys
 
-SRC = "/root/reference/rust/persia-speedy/tests/serialization_tests.rs"
+SRC = "rust/persia-speedy/tests/serialization_tests.rs"
 WANT = ["vec_u8", "vec_u16", "vec_u32", "vec_u64", "bool_false", "bool_true", "u16", "i16", "u32", "i32", "u64", "i64", "usize",
         "f32", "f64", "string", "tuple_u16_u16", "option_u16_some", "option_u16_none", "hashmap", "system_time", "derived_struct",
         "derived_simple_enum_a", "derived_simple_enum_b", "derived_simple_enum_c", "derived_enum_unit_variant",
@@ -18,7 +19,7 @@ WANT = ["vec_u8", "vec_u16", "vec_u32", "vec_u64", "bool_false", "bool_true", "u
 
 
 def main():
-    txt = open(SRC).read()
+    txt = open(os.path.join(sys.argv[1], SRC)).read()
     out = {}
     for name in WANT:
         m = re.search(r"\n\s*%s for ([^{]+?)\{\s*in = (.*?),\s*le = \[(.*?)\]" % re.escape(name), txt, re.S)

@@ -25,7 +25,7 @@ def torch_cuda():
     if not torch.cuda.is_available():
         pytest.fail("GPU tests need a CUDA device (there is no CPU fallback)")
     if torch.cuda.get_device_properties(0).total_memory < 70e9:
-        pytest.skip("the full-size shard needs a 180 GB-class GPU")
+        pytest.skip("the full-size shard needs an 80 GB-class GPU")
     return torch
 
 
