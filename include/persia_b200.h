@@ -9,8 +9,8 @@
  * negative pb_status; pb_last_error() gives the message for the calling thread.
  *
  * Conventions: `d_` = device pointer, `h_` = host pointer.  Gradient, output and update buffers (the gradients of
- * pb_backward, pb_backward_sharded, pb_backward_raw and pb_update; d_out_f16 of pb_forward and pb_forward_sharded;
- * d_table_f16 of pb_forward_raw) must be 16-byte aligned: the kernels access them with vector loads and stores.  A
+ * pb_backward, pb_backward_sharded, pb_backward_raw(_sharded) and pb_update; d_out_f16 of pb_forward and
+ * pb_forward_sharded; d_table_f16 of pb_forward_raw(_sharded)) must be 16-byte aligned: the kernels access them with vector loads and stores.  A
  * call given a pointer that is not returns PB_ERR_INVALID before it enqueues anything.  (A contiguous tensor view at
  * a storage offset, e.g. one slot of an [S, B, dim] tensor when B * dim * 2 is not a multiple of 16, can break the
  * rule; the Python wrappers pass a copy of such views.)  A "sign" is a prefixed u64 feature id
@@ -236,7 +236,7 @@ int pb_xchg_status(pb_xchg* x, uint32_t h_out[2], void* stream);
 #define PB_PHASE_FINISH 4 /* requester, forward only: rows in -> output */
 #define PB_PHASE_ALL 7
 /* forward_batched_direct over R shards: arguments as pb_forward.  Not supported here yet: slots sharing a
- * feature group, raw slots. */
+ * feature group (raw slots: pb_forward_raw_sharded below). */
 int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
                        const uint32_t* h_slot_occ_off, uint32_t batch, int training, void* d_out_f16, void* stream,
                        int phases);
@@ -244,6 +244,27 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
  * rank, before anything is sent (mod.rs:731-746). */
 int pb_backward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* const* h_grads, int is_f16, const float* h_scale,
                         int32_t* d_slot_status, void* stream, int phases);
+/* A raw (embedding_summation: false) slot over R shards: arguments and outputs as pb_forward_raw / pb_backward_raw, plus
+ * the exchange and `phases`.  Each call is one request per owner (the slot's distinct signs, sharded by
+ * farmhash64(sign) % R); the owner serves and applies them like the summation calls' (R requests, rank order).
+ *   - The exchange must be created with rows_f32 != 0, and its dim must be the table's.  The owner returns f32 rows and
+ *     the requester rounds them once: table row u+1 is f16(row) bit for bit, so a -0 element stays -0 (an f16 exchange
+ *     would give f16(0 + row)).  Signs over `cap` read as zeros, take no gradient and raise pb_xchg_status' h_out[0].
+ *   - The context serves one slot; the exchange serves this slot only (one exchange per raw slot and rank).  Its rows
+ *     may live in the same pb_table as the summation slots of that dim.
+ *   - Backward: d_grad is the [U, dim] gradient (U = d_counts[0] of the forward), NULL = add_skipped_gradient.  The NaN
+ *     rule (the whole request is dropped), the f16 +-inf clamp and 1/scale are applied on the requesting rank before
+ *     anything is sent; *d_status as pb_backward_raw.  Without a pending raw training forward: PB_ERR_STATE.
+ *   - Both are collective, also for an empty batch (U = 0): every rank calls them once per step, and every rank must
+ *     issue the step's collective calls (raw and summation, over all exchanges) in the same order — a rank waiting on
+ *     one exchange blocks its stream while a peer may be waiting on another.
+ * U stays on the device: no host sync and no allocation after the first call of a context, so a step is capturable. */
+int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids, uint32_t n_occ,
+                           const uint32_t* d_row_off, uint32_t batch, uint32_t sample_fixed_size, int training,
+                           void* d_table_f16, int64_t* d_index, int64_t* d_non_empty, uint32_t* d_sample_id_num,
+                           uint32_t* d_counts, void* stream, int phases);
+int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_grad, int is_f16, float scale,
+                            int32_t* d_status, void* stream, int phases);
 
 /* Number of kernels the library has launched on behalf of the caller since load (bench bookkeeping). */
 uint64_t pb_launch_count(void);

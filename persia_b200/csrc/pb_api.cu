@@ -119,6 +119,7 @@ struct pb_ctx {
   uint32_t* occ_cell = nullptr;
   RawWork raw{};
   bool raw_ready = false, raw_pending = false;
+  pb_table* raw_table = nullptr;  // sharded raw forward pending on this table: counted in its pending_batches
   float* raw_stage = nullptr;
   size_t raw_stage_floats = 0;
 };
@@ -240,6 +241,13 @@ void drop_pending(pb_ctx* c) {
   if (c->pending && c->pending_table && c->pending_table->pending_batches) c->pending_table->pending_batches--;
   c->pending = false;
   c->pending_table = nullptr;
+}
+
+// a sharded raw forward's rows stay protected from eviction until its gradients are applied, like a summation batch's
+void drop_raw_pending(pb_ctx* c) {
+  if (c->raw_table && c->raw_table->pending_batches) c->raw_table->pending_batches--;
+  c->raw_table = nullptr;
+  c->raw_pending = false;
 }
 
 }  // namespace
@@ -611,9 +619,11 @@ int pb_ctx_destroy(pb_ctx* c) {
   DeviceGuard g(c->device);
   cudaDeviceSynchronize();
   drop_pending(c);
+  drop_raw_pending(c);
   void* ptrs[] = {c->b.set,   c->b.occ_set, c->b.item_cell, c->b.seg_occ, c->b.cold, c->b.warm, c->b.hot, c->b.hot_bits, c->b.cnt,
                   c->occ_cell, c->occ_outrow, c->row_off, c->nan_tick, c->vw_stage, c->dev_tick, c->raw.set,
-                  c->raw.occ_set, c->raw.flag, c->raw.rank, c->raw.tiles, c->raw.distinct_cell, c->raw.counts, c->raw_stage};
+                  c->raw.occ_set, c->raw.flag, c->raw.rank, c->raw.tiles, c->raw.distinct_cell, c->raw.counts, c->raw.target,
+                  c->raw.peer,    c->raw_stage};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   if (c->side) cudaStreamDestroy(c->side);
@@ -839,6 +849,37 @@ void xchg_layout(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32, uint64_t 
   off[2] = off[1] + round256((uint64_t)R * cap * dim * (rows_f32 ? 4 : 2));        // grad
   off[3] = off[2] + round256((uint64_t)R * cap * dim * 4);                         // gok
   off[4] = off[3] + round256((uint64_t)R * cap * 4);                               // end
+}
+
+// The owner's part of a sharded backward (PB_PHASE_SERVE), shared by the summation and the raw calls: the step's R
+// gradient requests, every row stepped once per request in rank order.  prefix[n_prefix]: the feature groups of the
+// slots the exchange serves (Adam beta powers).
+int owner_backward(pb_table* t, pb_xchg* x, const uint64_t* prefix, uint32_t n_prefix, uint64_t spacing, int phases,
+                   cudaStream_t st) {
+  if (t->op.kind == PB_OPT_ADAGRAD_VW) {  // (needs the whole gradient's dot per step) one request after another
+    for (uint32_t src = 0; src < x->d.R; ++src) {
+      launch_wait(x->d, XC_FLAG_GRAD, (int)src, st);
+      launch_owner_update(t->d, t->op, t->hy, x->d, src, st);
+    }
+    launch_uclear(x->d, st);
+  } else {  // owner: the R requests in one launch, every row stepped in rank order
+    if (phases != PB_PHASE_ALL) launch_wait(x->d, XC_FLAG_GRAD, -1, st);
+    if (t->op.kind == PB_OPT_ADAM) {  // every request advances the beta powers of the feature groups it holds here
+      for (uint32_t s = 0; s < n_prefix; ++s)
+        if (adam_index(t, prefix[s]) < 0) return fail(PB_ERR_CAPACITY, "more feature groups than Adam beta-power pairs");
+      if (x->akeys_uploaded != t->adam_keys.size()) {  // (first steps only: not inside a graph capture)
+        PB_CUDA(cudaStreamSynchronize(st));
+        PB_CUDA(cudaMemcpy(x->akeys, t->adam_keys.data(), sizeof(uint64_t) * t->adam_keys.size(), cudaMemcpyHostToDevice));
+        x->akeys_uploaded = t->adam_keys.size();
+      }
+      x->d.n_akeys = (uint32_t)t->adam_keys.size();
+      x->d.amask = ~spacing;
+      launch_owner_adam(x->d, t->adam_dev, t->op.b1, t->op.b2, st);
+    }
+    launch_owner_update_all(t->d, t->op, t->hy, x->d, st);
+  }
+  x->u_dirty = false;
+  return PB_OK;
 }
 }  // namespace
 
@@ -1066,29 +1107,7 @@ int pb_backward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* const* h
     PB_CUDA(cudaGetLastError());
     return PB_OK;
   }
-  if (t->op.kind == PB_OPT_ADAGRAD_VW) {  // (needs the whole gradient's dot per step) one request after another
-    for (uint32_t src = 0; src < x->d.R; ++src) {
-      launch_wait(x->d, XC_FLAG_GRAD, (int)src, st);
-      launch_owner_update(t->d, t->op, t->hy, x->d, src, st);
-    }
-    launch_uclear(x->d, st);
-  } else {  // owner: the R requests in one launch, every row stepped in rank order
-    if (phases != PB_PHASE_ALL) launch_wait(x->d, XC_FLAG_GRAD, -1, st);
-    if (t->op.kind == PB_OPT_ADAM) {  // every request advances the beta powers of the feature groups it holds here
-      for (uint32_t s = 0; s < S; ++s)
-        if (adam_index(t, c->slots.prefix[s]) < 0) return fail(PB_ERR_CAPACITY, "more feature groups than Adam beta-power pairs");
-      if (x->akeys_uploaded != t->adam_keys.size()) {  // (first steps only: not inside a graph capture)
-        PB_CUDA(cudaStreamSynchronize(st));
-        PB_CUDA(cudaMemcpy(x->akeys, t->adam_keys.data(), sizeof(uint64_t) * t->adam_keys.size(), cudaMemcpyHostToDevice));
-        x->akeys_uploaded = t->adam_keys.size();
-      }
-      x->d.n_akeys = (uint32_t)t->adam_keys.size();
-      x->d.amask = ~sl.spacing;
-      launch_owner_adam(x->d, t->adam_dev, t->op.b1, t->op.b2, st);
-    }
-    launch_owner_update_all(t->d, t->op, t->hy, x->d, st);
-  }
-  x->u_dirty = false;
+  if ((rc = owner_backward(t, x, c->slots.prefix, S, sl.spacing, phases, st))) return rc;
   drop_pending(c);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
@@ -1110,6 +1129,8 @@ static int ensure_raw(pb_ctx* c) {
   PB_CUDA(cudaMalloc(&w.distinct_cell, 4 * n));
   PB_CUDA(cudaMalloc(&w.counts, 8));
   PB_CUDA(cudaMemset(w.counts, 0, 8));
+  PB_CUDA(cudaMalloc(&w.target, 4 * n));
+  PB_CUDA(cudaMalloc(&w.peer, 4 * PB_MAX_RANKS));
   c->raw_ready = true;
   return PB_OK;
 }
@@ -1216,6 +1237,120 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
   }
   launch_update_direct(t->d, t->op, t->hy, c->raw.distinct_cell, g32, c->n_occ, pair, st, c->raw.counts,
                        c->dev_tick, c->nan_tick);
+  PB_CUDA(cudaGetLastError());
+  return PB_OK;
+}
+
+int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids, uint32_t n_occ,
+                           const uint32_t* d_row_off, uint32_t batch, uint32_t sample_fixed_size, int training,
+                           void* d_table_f16, int64_t* d_index, int64_t* d_non_empty, uint32_t* d_sample_id_num,
+                           uint32_t* d_counts, void* stream, int phases) {
+  if (phases == 0) phases = PB_PHASE_ALL;
+  const bool all = phases == PB_PHASE_ALL;
+  if (!t || !c || !x || !d_table_f16 || !d_index || !d_non_empty || !d_sample_id_num || !d_counts || (n_occ && !d_ids))
+    return fail(PB_ERR_INVALID, "null argument");
+  if (misaligned(d_table_f16)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
+  if (!c->has_slots || c->slots.n_slots != 1) return fail(PB_ERR_STATE, "a raw context serves exactly one slot (pb_ctx_set_slots)");
+  if (t->device != c->device || t->device != x->device) return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
+  if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
+  if (!x->d.row_f32) return fail(PB_ERR_INVALID, "raw slots need an exchange created with f32 rows (the requester rounds them)");
+  if (batch > 65535) return fail(PB_ERR_BATCH, "batch size cannot be larger than 65535");
+  if (sample_fixed_size == 0) return fail(PB_ERR_INVALID, "sample_fixed_size must be positive");
+  if (n_occ > c->max_occ || batch > c->max_out || (uint64_t)batch * sample_fixed_size > (1ull << 31))
+    return fail(PB_ERR_CAPACITY, "batch exceeds the context's capacity");
+  if (!d_row_off && n_occ != batch) return fail(PB_ERR_INVALID, "row offsets are required unless every sample has one id");
+  int rc;
+  // every rank serves lookups whether or not its own batch trains: the shard must be usable (a collective call)
+  if ((rc = ready_for_training(t))) return rc;
+  DeviceGuard g(t->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = ensure_alloc(t))) return rc;
+  if ((rc = ensure_raw(c))) return rc;
+  if (phases & PB_PHASE_SEND) {
+    const uint32_t occ_off[2] = {0, n_occ};
+    SlotsDev sl;
+    if ((rc = make_slots(c->slots, occ_off, sl))) return rc;
+    sl.uniform = 0;
+    drop_raw_pending(c);  // the numbering below replaces the pending batch's
+    if (training) {
+      if ((rc = maybe_evict(t, st))) return rc;
+      launch_begin_batch(t->d, c->dev_tick, nullptr, st);
+    }
+    const uint32_t* occ_sample = nullptr;
+    if (d_row_off) {
+      PB_CUDA(cudaMemcpyAsync(c->row_off, d_row_off, 4 * ((size_t)batch + 1), cudaMemcpyDeviceToDevice, st));
+      launch_expand_rows(c->row_off, batch, c->occ_outrow, st);
+      occ_sample = c->occ_outrow;
+    }
+    launch_raw_number(sl, d_ids, n_occ, d_row_off ? c->row_off : nullptr, occ_sample, batch, sample_fixed_size, nullptr,
+                      c->raw, (long long*)d_index, (long long*)d_non_empty, d_sample_id_num, st);
+    PB_CUDA(cudaMemcpyAsync(d_counts, c->raw.counts, 8, cudaMemcpyDeviceToDevice, st));
+    PB_CUDA(cudaMemsetAsync(c->raw.peer, 0, 4 * PB_MAX_RANKS, st));
+    launch_raw_route(c->raw, n_occ, x->d, st);  // requester: distinct signs -> owners' areas
+    if (all) launch_signal_wait(x->d, XC_FLAG_SIGN, c->raw.peer, st);
+    else launch_signal(x->d, XC_FLAG_SIGN, c->raw.peer, st);
+  }
+  if (phases & PB_PHASE_SERVE) {
+    if (!all) launch_wait(x->d, XC_FLAG_SIGN, -1, st);
+    if (training && x->u_dirty) launch_uclear(x->d, st);  // a training batch whose gradients never came left its rows noted
+    launch_owner_lookup(training != 0, t->d, t->hy, t->op, x->d, st);  // owner: f32 rows -> requesters' areas
+    if (training) x->u_dirty = true;
+    if (all) launch_signal_wait(x->d, XC_FLAG_ROW, nullptr, st);
+    else launch_signal(x->d, XC_FLAG_ROW, nullptr, st);
+  }
+  if (!(phases & PB_PHASE_FINISH)) {
+    PB_CUDA(cudaGetLastError());
+    return PB_OK;
+  }
+  if (!all) launch_wait(x->d, XC_FLAG_ROW, -1, st);
+  launch_raw_fill(c->raw, n_occ, t->d.dim, x->d, d_table_f16, st);  // requester: rows in -> distinct-sign table
+  if (training) {
+    c->n_occ = n_occ;
+    c->batch = batch;
+    c->raw_pending = true;
+    c->raw_table = t;
+    t->pending_batches++;
+  }
+  PB_CUDA(cudaGetLastError());
+  return PB_OK;
+}
+
+int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_grad, int is_f16, float scale,
+                            int32_t* d_status, void* stream, int phases) {
+  if (phases == 0) phases = PB_PHASE_ALL;
+  if (!t || !c || !x) return fail(PB_ERR_INVALID, "null argument");
+  if (!c->has_slots || c->slots.n_slots != 1) return fail(PB_ERR_STATE, "a raw context serves exactly one slot (pb_ctx_set_slots)");
+  if (t->device != c->device || t->device != x->device) return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
+  if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
+  if (!c->raw_pending) return fail(PB_ERR_STATE, "no raw forward batch is pending in this context (backward_ref_id not found)");
+  if (d_grad && misaligned(d_grad)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
+  int rc = ready_for_training(t);
+  if (rc) return rc;
+  const bool do_scale = std::fabs(scale - 1.0f) > 1.1920929e-07f;
+  const float inv = 1.0f / scale;
+  if (d_grad && do_scale && !std::isfinite(inv)) return fail(PB_ERR_INVALID, "scale on gradient must be finite");
+  DeviceGuard g(t->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const uint32_t dim = t->d.dim;
+  if (phases & PB_PHASE_SEND) {  // the NaN rule, add_skipped_gradient, the clamp and 1/scale: on the requester
+    GradsDev gr;
+    std::memset(&gr, 0, sizeof(gr));
+    gr.ptr[0] = d_grad;
+    if (d_grad) launch_raw_nan(d_grad, is_f16 != 0, c->raw.counts, dim, c->dev_tick, c->nan_tick, st);
+    if (d_status) launch_slot_status(gr, 1, c->dev_tick, c->nan_tick, d_status, st);
+    launch_raw_send(d_grad, is_f16 != 0, c->raw, c->n_occ, dim, inv, do_scale, c->dev_tick, c->nan_tick, x->d, st);
+    if (phases == PB_PHASE_ALL && t->op.kind != PB_OPT_ADAGRAD_VW) launch_signal_wait(x->d, XC_FLAG_GRAD, nullptr, st);
+    else launch_signal(x->d, XC_FLAG_GRAD, nullptr, st);
+  }
+  if (!(phases & PB_PHASE_SERVE)) {
+    PB_CUDA(cudaGetLastError());
+    return PB_OK;
+  }
+  const uint32_t occ_off[2] = {0, c->n_occ};
+  SlotsDev sl;
+  if ((rc = make_slots(c->slots, occ_off, sl))) return rc;
+  if ((rc = owner_backward(t, x, c->slots.prefix, 1, sl.spacing, phases, st))) return rc;
+  drop_raw_pending(c);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }

@@ -127,8 +127,11 @@ struct RawWork {
   uint32_t* flag;           // scan input / second scan output
   uint32_t* rank;           // scan output
   uint32_t* tiles;          // scan spine
-  uint32_t* distinct_cell;  // index cell of every distinct sign (forward -> backward)
+  uint32_t* distinct_cell;  // index cell of every distinct sign (forward -> backward); sharded: its scratch-set cell
   uint32_t* counts;         // [0] distinct signs, [1] ids placed in `index`
+  // sharded path (pb_forward_raw_sharded): where every distinct sign went, owner * cap + slot (ROW_NONE: over cap)
+  uint32_t* target;         // [n]
+  uint32_t* peer;           // [PB_MAX_RANKS] distinct signs routed to each owner
 };
 
 void launch_fill_cells(Cell* cells, uint64_t n, cudaStream_t st);
@@ -184,6 +187,16 @@ void launch_adam_fill(float* pow, float b1, float b2, cudaStream_t st);
 void launch_adam_advance(float* pow, const AdamKeys& keys, float b1, float b2, cudaStream_t st, const GradsDev* gr = nullptr,
                          uint32_t n_slots = 0, const uint32_t* tick = nullptr, const uint32_t* nan_tick = nullptr);
 uint32_t raw_scan_tiles(uint32_t n);
+// numbering of the distinct signs, index / non_empty / sample_id_num; occ_cell null: distinct_cell = scratch-set cells
+void launch_raw_number(const SlotsDev& sl, const uint64_t* ids, uint32_t n, const uint32_t* row_off,
+                       const uint32_t* occ_sample, uint32_t batch, uint32_t fixed, const uint32_t* occ_cell,
+                       const RawWork& w, long long* index, long long* non_empty, uint32_t* sample_id_num,
+                       cudaStream_t st);
+// pb_shard.cu, raw slot over R shards: requester's route, table fill and gradient send (n: worst-case U)
+void launch_raw_route(const RawWork& w, uint32_t n, const XchgDev& x, cudaStream_t st);
+void launch_raw_fill(const RawWork& w, uint32_t n, uint32_t dim, const XchgDev& x, void* table_f16, cudaStream_t st);
+void launch_raw_send(const void* grad, bool f16, const RawWork& w, uint32_t n, uint32_t dim, float inv_scale,
+                     bool do_scale, const uint32_t* tick, const uint32_t* nan_tick, const XchgDev& x, cudaStream_t st);
 void launch_raw_forward(const TableDev& t, const SlotsDev& sl, const uint64_t* ids, uint32_t n,
                         const uint32_t* row_off, const uint32_t* occ_sample, uint32_t batch, uint32_t fixed,
                         const uint32_t* occ_cell, const RawWork& w, void* table_f16, long long* index,

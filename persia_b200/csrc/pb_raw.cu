@@ -136,7 +136,9 @@ __global__ void __launch_bounds__(256) k_raw_flag(const RawCell* __restrict__ se
   if (i < n) flag[i] = set[occ_set[i]].first == i ? 1u : 0u;
 }
 
-// first occurrences publish their sign's number and remember the sign's index cell for the backward
+// first occurrences publish their sign's number and remember, per distinct sign, its index cell for the backward
+// (occ_cell given: the local table's probe) or its cell of the scratch set (occ_cell null: the sharded path, whose
+// route kernel reads the sign from there)
 __global__ void __launch_bounds__(256) k_raw_assign(RawCell* __restrict__ set, const uint32_t* __restrict__ occ_set,
                                                     const uint32_t* __restrict__ flag,
                                                     const uint32_t* __restrict__ rank,
@@ -145,7 +147,7 @@ __global__ void __launch_bounds__(256) k_raw_assign(RawCell* __restrict__ set, c
   uint32_t i = blockIdx.x * 256 + threadIdx.x;
   if (i >= n || !flag[i]) return;
   set[occ_set[i]].rank = rank[i];
-  distinct_cell[rank[i]] = occ_cell[i];
+  distinct_cell[rank[i]] = occ_cell ? occ_cell[i] : occ_set[i];
 }
 
 // mod.rs:593-620: index[b * fixed + col] = number + 1 for col < fixed (0 = padding).  The reference's
@@ -247,10 +249,10 @@ __global__ void __launch_bounds__(256) k_raw_stage(const void* __restrict__ grad
 
 uint32_t raw_scan_tiles(uint32_t n) { return cdiv(n ? n : 1, SCAN_TILE) + 1; }
 
-void launch_raw_forward(const TableDev& t, const SlotsDev& sl, const uint64_t* ids, uint32_t n,
-                        const uint32_t* row_off, const uint32_t* occ_sample, uint32_t batch, uint32_t fixed,
-                        const uint32_t* occ_cell, const RawWork& w, void* table_f16, long long* index,
-                        long long* non_empty, uint32_t* sample_id_num, cudaStream_t st) {
+void launch_raw_number(const SlotsDev& sl, const uint64_t* ids, uint32_t n, const uint32_t* row_off,
+                       const uint32_t* occ_sample, uint32_t batch, uint32_t fixed, const uint32_t* occ_cell,
+                       const RawWork& w, long long* index, long long* non_empty, uint32_t* sample_id_num,
+                       cudaStream_t st) {
   cudaMemsetAsync(w.set, 0xFF, sizeof(RawCell) * ((size_t)w.set_mask + 2), st);
   cudaMemsetAsync(index, 0, sizeof(long long) * (size_t)batch * fixed, st);
   if (n) {
@@ -271,6 +273,13 @@ void launch_raw_forward(const TableDev& t, const SlotsDev& sl, const uint64_t* i
   } else {
     cudaMemsetAsync(w.counts + 1, 0, 4, st);
   }
+}
+
+void launch_raw_forward(const TableDev& t, const SlotsDev& sl, const uint64_t* ids, uint32_t n,
+                        const uint32_t* row_off, const uint32_t* occ_sample, uint32_t batch, uint32_t fixed,
+                        const uint32_t* occ_cell, const RawWork& w, void* table_f16, long long* index,
+                        long long* non_empty, uint32_t* sample_id_num, cudaStream_t st) {
+  launch_raw_number(sl, ids, n, row_off, occ_sample, batch, fixed, occ_cell, w, index, non_empty, sample_id_num, st);
   int vec, G;
   vec_group(t.dim, vec, G);
   const uint32_t grid = cdiv((uint64_t)(n ? n : 1) * G, 256);

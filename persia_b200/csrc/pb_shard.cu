@@ -531,6 +531,11 @@ __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, H
       g0[u] = grads + (size_t)(act[u] ? k : 0u) * t.dim;
       sc[u].vw_state = (act[u] && op.kind == PB_OPT_ADAGRAD_VW) ? prow[u][t.dim] : 0.0f;
       sc[u].r1 = sc[u].r2 = 0.0f;
+      if (act[u] && op.kind == PB_OPT_ADAM) {  // this request's (beta1^t, beta2^t) of the row's feature group
+        const float* pw = x.apow + ((size_t)src * PB_ADAM_KEYS + adam_key_of(x, x_sign(x, x.rank)[(size_t)src * x.cap + k])) * 2u;
+        sc[u].r1 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[0]));
+        sc[u].r2 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[1]));
+      }
     }
     for (uint32_t c = lane; c < nvec; c += G) {
       RowElems<-1, VEC> rc[2];
@@ -557,6 +562,121 @@ __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, H
         }
     }
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// raw slot over R shards (pb_forward_raw_sharded / pb_backward_raw_sharded).  The requester numbers the slot's distinct
+// signs like pb_forward_raw (pb_raw.cu), then every distinct sign is one entry of its owner's request:
+//   k_raw_route  sign -> owner's area; target[u] = owner * cap + slot, kept for the fill and the backward
+//   k_raw_fill   received f32 row -> table row u + 1, rounded once (f16(row): a -0 stays -0); row 0 and misses zeros
+//   k_raw_send   the [U, dim] gradient, +-inf clamped and unscaled, -> owner's gradient area with its apply word
+// The owner's side is the summation path's: k_owner_lookup, then k_owner_update_all / k_owner_update.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_raw_route(RawWork w, XchgDev x) {
+  const uint32_t n_items = w.counts[0];
+  if (blockIdx.x * blockDim.x >= n_items) return;  // whole block (the grid is sized for the worst case)
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool valid = u < n_items;
+  uint32_t owner = 0xFFFFFFFFu;
+  uint64_t sign = 0;
+  if (valid) {
+    sign = w.set[w.distinct_cell[u]].key;  // (the sign 2^64-1 has the set's extra cell, whose key stays 2^64-1)
+    owner = (uint32_t)(farmhash64_u64(sign) % x.R);  // sign_to_shard_modulo, mod.rs:341-345
+  }
+  __shared__ uint32_t s_n[PB_MAX_RANKS], s_g[PB_MAX_RANKS];
+  if (threadIdx.x < PB_MAX_RANKS) s_n[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t peers = __match_any_sync(0xffffffffu, owner);
+  const uint32_t leader = __ffs(peers) - 1;
+  uint32_t k = 0;
+  if (valid && lane == leader) k = atomicAdd(&s_n[owner], (uint32_t)__popc(peers));
+  k = __shfl_sync(0xffffffffu, k, leader) + __popc(peers & ((1u << lane) - 1u));
+  __syncthreads();
+  if (threadIdx.x < x.R && s_n[threadIdx.x]) s_g[threadIdx.x] = atomicAdd(&w.peer[threadIdx.x], s_n[threadIdx.x]);
+  __syncthreads();
+  if (!valid) return;
+  k += s_g[owner];
+  uint32_t target = ROW_NONE;
+  if (k < x.cap) {
+    target = owner * x.cap + k;
+    x_sign(x, owner)[(size_t)x.rank * x.cap + k] = sign;  // over NVLink when owner != rank
+  } else {
+    x.err[0] = 1u;  // the pair needs more than cap slots: the caller re-runs the batch with a larger cap
+  }
+  w.target[u] = target;
+}
+
+__global__ void __launch_bounds__(256) k_raw_fill(const uint32_t* __restrict__ counts, const uint32_t* __restrict__ target,
+                                                  uint32_t dim, XchgDev x, __half* __restrict__ out, uint32_t G) {
+  const uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) / G;  // table row
+  const uint32_t lane = threadIdx.x % G;
+  if (r > counts[0]) return;
+  const uint32_t tg = r ? target[r - 1] : ROW_NONE;
+  const float* src = reinterpret_cast<const float*>(x_row(x, x.rank)) + (size_t)(tg == ROW_NONE ? 0u : tg) * dim;
+  __half* o = out + (size_t)r * dim;
+  for (uint32_t e = lane; e < dim; e += G) o[e] = __float2half_rn(tg == ROW_NONE ? 0.0f : src[e]);  // ndarray_f32_to_f16: RNE
+}
+
+template <bool F16>
+__global__ void __launch_bounds__(256) k_raw_send(const void* __restrict__ grad, const uint32_t* __restrict__ counts,
+                                                  const uint32_t* __restrict__ target, uint32_t dim, float inv_scale,
+                                                  int do_scale, const uint32_t* __restrict__ tick,
+                                                  const uint32_t* __restrict__ nan_tick, XchgDev x, uint32_t G) {
+  const uint32_t U = counts[0];
+  // add_skipped_gradient, or a NaN anywhere in the gradient (mod.rs:731-746): the whole request is dropped
+  const bool drop = grad == nullptr || nan_tick[0] == *tick;
+  const uint32_t lane = threadIdx.x % G;
+  const uint32_t n_groups = gridDim.x * (blockDim.x / G);
+  for (uint32_t u = (blockIdx.x * blockDim.x + threadIdx.x) / G; u < U; u += n_groups) {
+    const uint32_t tg = target[u];
+    if (tg == ROW_NONE) continue;  // over cap: the sign was never looked up
+    const uint32_t owner = tg / x.cap;
+    const size_t j = (size_t)x.rank * x.cap + tg % x.cap;  // this request's entry in the owner's area
+    if (!drop) {
+      float* dst = reinterpret_cast<float*>(x.base[owner] + x.off_grad) + j * dim;
+      for (uint32_t e = lane; e < dim; e += G) {
+        const size_t i = (size_t)u * dim + e;
+        float v;
+        if (F16) {  // f16 -> f32 with +-inf -> +-65504 (persia-common lib.rs:163-180)
+          v = __half2float(reinterpret_cast<const __half*>(grad)[i]);
+          if (v == INFINITY) v = 65504.0f;
+          else if (v == -INFINITY) v = -65504.0f;
+        } else {
+          v = reinterpret_cast<const float*>(grad)[i];
+        }
+        dst[e] = do_scale ? __fmul_rn(v, inv_scale) : v;  // x 1/scale_factor (mod.rs:751-755)
+      }
+    }
+    if (lane == 0) reinterpret_cast<uint32_t*>(x.base[owner] + x.off_gok)[j] = drop ? 0u : 1u;
+  }
+}
+
+static uint32_t lanes_for(uint32_t dim) {
+  uint32_t G = 1;
+  while (G < dim && G < 32) G <<= 1;
+  return G;
+}
+
+void launch_raw_route(const RawWork& w, uint32_t n, const XchgDev& x, cudaStream_t st) {
+  if (!n) return;
+  PB_LAUNCH_F(FAM_ROUTE, k_raw_route, cdiv(n, 256), 256, 0, st, w, x);
+}
+
+void launch_raw_fill(const RawWork& w, uint32_t n, uint32_t dim, const XchgDev& x, void* table_f16, cudaStream_t st) {
+  const uint32_t G = lanes_for(dim);
+  PB_LAUNCH_F(FAM_GATHER, k_raw_fill, cdiv((uint64_t)(n + 1) * G, 256), 256, 0, st, w.counts, w.target, dim, x,
+              reinterpret_cast<__half*>(table_f16), G);
+}
+
+void launch_raw_send(const void* grad, bool f16, const RawWork& w, uint32_t n, uint32_t dim, float inv_scale,
+                     bool do_scale, const uint32_t* tick, const uint32_t* nan_tick, const XchgDev& x, cudaStream_t st) {
+  if (!n) return;
+  const uint32_t G = lanes_for(dim);
+  const uint32_t full = cdiv((uint64_t)n * G, 256);
+  const uint32_t grid = full < PB_NUM_SMS * 4u ? full : PB_NUM_SMS * 4u;
+  if (f16) PB_LAUNCH_F(FAM_ROUTE, k_raw_send<true>, grid, 256, 0, st, grad, w.counts, w.target, dim, inv_scale, do_scale ? 1 : 0, tick, nan_tick, x, G);
+  else PB_LAUNCH_F(FAM_ROUTE, k_raw_send<false>, grid, 256, 0, st, grad, w.counts, w.target, dim, inv_scale, do_scale ? 1 : 0, tick, nan_tick, x, G);
 }
 
 // ------------------------------------------------------------------------------------------------

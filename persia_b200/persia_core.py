@@ -7,8 +7,12 @@ process's GPU, `get_embedding_from_data` / `Forward.get_batch` run pb_forward, `
 the raw device pointers `GradientBatch.add_gradient` receives.  `install()` registers it (and its submodules)
 in `sys.modules` as `persia_core`, after which the reference's own `persia` package runs unchanged on top.
 
-Scope of round 1: summation and raw slots (no hash-stack on raw slots), one process / one GPU (`replica_size == 1`; the sharded
-multi-GPU worker is persia_b200.worker); `Forward` prefetches on worker threads with the reference's ordering and
+Scope: summation and raw slots (no hash-stack on raw slots), one process per GPU.  With `replica_size > 1` every dim
+group is served by a ShardedEmbeddingWorker and every raw slot by its own ShardedRawWorker (persia_b200.worker), all
+of one dim on the rank's one table; there a raw slot may not share its feature group with another slot of the batch.
+Their calls are collective, so every rank issues them in one fixed order: the raw slots in batch order, then the
+summation dims in ascending order, in the forward and again in the backward; every batch must carry the same raw
+slots in the same order.  `Forward` prefetches on worker threads with the reference's ordering and
 staleness rules (persia_b200/engine.py), `Backward` applies updates in the caller's thread; `to_bytes()` is a private encoding (the speedy wire format is N4); `dump`/`load`
 write and read the reference's `.emb` checkpoint files (persia_b200/checkpoint.py).
 """
@@ -83,6 +87,7 @@ class _State:
         self.dataflow_sender = None
         self.next_batch_id = 0
         self.forward_id_buffer = {}
+        self.raw_order = None  # replica_size > 1: the raw slots of the first batch, in order (every batch must match)
 
     def set_config(self, cfg):
         self.prefix_bit, self.slots = parse_embedding_config(cfg)
@@ -464,8 +469,17 @@ def _forward_locked(batch, device_id, training):
         sc = _S.by_name[name]
         if not sc.embedding_summation and sc.hash_stack_rounds > 0:
             raise RuntimeError(f"slot {name}: a raw (embedding_summation: false) slot with hash_stack is not supported")
-        if not sc.embedding_summation and (_S.replica_size or 1) > 1:
-            raise RuntimeError(f"slot {name}: raw (embedding_summation: false) slots are not supported on replica_size > 1 yet")
+    sharded = (_S.replica_size or 1) > 1
+    if sharded:  # the collective calls of a step must come in the same order on every rank
+        raw_names = tuple(n for n, _ in feats if not _S.by_name[n].embedding_summation)
+        for n in raw_names:
+            if sum(_S.by_name[m].index_prefix == _S.by_name[n].index_prefix for m, _ in feats) > 1:
+                raise RuntimeError(f"slot {n}: on R GPUs a raw slot cannot share its feature group with another slot "
+                                   "of the batch")
+        if _S.raw_order is None:
+            _S.raw_order = raw_names
+        elif _S.raw_order != raw_names:
+            raise RuntimeError("on R GPUs every batch must carry the same raw slots, in the same order")
     pending = _Pending()
     by_slot = {}
     raw_out = {}
@@ -475,6 +489,23 @@ def _forward_locked(batch, device_id, training):
             continue
         with _STATE_LOCK:
             g = _S.group(sc.dim)
+        if sharded:  # R GPUs: one request per owner, through the slot's raw worker
+            with g["lock"]:
+                ids, row_off, _ = _flatten([(n, x)], B)
+                wk = _sharded_raw_worker(g, sc, B, ids, row_off, dev)
+                d_ids = torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True)
+                d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
+                table, index, non_empty, num, counts = wk.forward_raw(d_ids, B, sc.sample_fixed_size, row_off=d_off,
+                                                                      training=training)
+                if wk.status()[0]:
+                    raise RuntimeError("a batch requested more distinct signs of one shard than the exchange holds: raise "
+                                       "PERSIA_B200_XCHG_CAP")
+                U, ne = counts.tolist()
+            raw_out[n] = (Tensor(table[:U + 1], n), Tensor(index, f"{n}_index"),
+                          Tensor(non_empty[:ne], f"{n}_non_empty_index"), num.tolist())
+            if training:
+                pending.parts.append((g, None, [n], True))
+            continue
         key = ("raw", n)
         pool = g["ctx"].setdefault(key, [])
         ids, row_off, _ = _flatten([(n, x)], B)
@@ -562,30 +593,63 @@ def _sharded_worker(g, dim, names, B, ids, row_off, slot_off, dev):
 
     if not dist.is_initialized():
         raise RuntimeError("replica_size > 1 needs torch.distributed (TrainCtx initialises it; else call init_process_group)")
-    R = dist.get_world_size()
     slots = [_S.by_name[n] for n in names]
-    cap = int(os.environ.get("PERSIA_B200_XCHG_CAP", 0))
-    if not cap:  # from this first batch: distinct signs per owner, largest over the ranks, with a generous margin
-        counts = np.zeros(R, np.int64)
-        spacing = np.uint64((1 << (64 - _S.prefix_bit)) - 1)
-        for i, sc in enumerate(slots):
-            x = ids[slot_off[i]:slot_off[i + 1]]
-            u = np.unique(x % spacing + np.uint64(sc.index_prefix) if sc.index_prefix else x)
-            counts += np.bincount((farmhash64_np(u) % np.uint64(R)).astype(np.int64), minlength=R)
-        t = torch.tensor([int(counts.max())], dtype=torch.int64, device=dev)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        cap = (int(int(t) * 1.5) + 1024 + 7) // 8 * 8
+    cap = _exchange_cap([(ids[slot_off[i]:slot_off[i + 1]], sc.index_prefix) for i, sc in enumerate(slots)], dev)
     ragged = row_off is not None
     per_sample = max(1, -(-len(ids) // max(1, len(names) * B)))
     max_batch = int(os.environ.get("PERSIA_B200_MAX_BATCH", B))
+    # the group's table is the rank's shard: raw workers of this dim serve it too
     wk = W.distributed(len(names), dim, [sc.index_prefix for sc in slots], _S.capacity, cap, _S.optimizer or {}, dev,
                        hyper=_S.hyper, max_batch=max(B, max_batch), sqrt_scaling=[sc.sqrt_scaling for sc in slots],
-                       rows_f32=ragged, prefix_bit=_S.prefix_bit, max_ids_per_sample=2 * per_sample if ragged else 1)
+                       rows_f32=ragged, prefix_bit=_S.prefix_bit, max_ids_per_sample=2 * per_sample if ragged else 1,
+                       shard=g["shard"])
     wk.names = tuple(names)
-    wk.shard.set_eviction()
-    g["shard"].close()
-    g["shard"], g["worker"] = wk.shard, wk
+    g["worker"] = wk
     return wk
+
+
+def _sharded_raw_worker(g, sc, B, ids, row_off, dev):
+    """Raw slot `sc`'s ShardedRawWorker (persia_b200/worker.py) over the rank's table of its dim, created by the first
+    batch that carries the slot: a collective, like _sharded_worker."""
+    wk = g.setdefault("raw_workers", {}).get(sc.name)
+    if wk is not None:
+        return wk
+    import torch.distributed as dist
+
+    from .worker import ShardedRawWorker
+
+    if not dist.is_initialized():
+        raise RuntimeError("replica_size > 1 needs torch.distributed (TrainCtx initialises it; else call init_process_group)")
+    cap = _exchange_cap([(ids, sc.index_prefix)], dev)
+    ragged = row_off is not None
+    per_sample = max(1, -(-len(ids) // max(1, B)))
+    max_batch = int(os.environ.get("PERSIA_B200_MAX_BATCH", B))
+    wk = ShardedRawWorker.distributed(1, sc.dim, [sc.index_prefix], _S.capacity, cap, _S.optimizer or {}, dev,
+                                      hyper=_S.hyper, max_batch=max(B, max_batch, 1), prefix_bit=_S.prefix_bit,
+                                      max_ids_per_sample=2 * per_sample if ragged else 1, shard=g["shard"])
+    g["raw_workers"][sc.name] = wk
+    return wk
+
+
+def _exchange_cap(slot_ids, dev):
+    """Slots per (source, owner) pair of a new exchange: PERSIA_B200_XCHG_CAP, else from this first batch — the
+    distinct signs it requests of one owner, largest over the ranks (a collective), with a generous margin.
+    slot_ids: [(flat ids of one slot, its index_prefix)]."""
+    import torch
+    import torch.distributed as dist
+
+    cap = int(os.environ.get("PERSIA_B200_XCHG_CAP", 0))
+    if cap:
+        return cap
+    R = dist.get_world_size()
+    counts = np.zeros(R, np.int64)
+    spacing = np.uint64((1 << (64 - _S.prefix_bit)) - 1)
+    for x, prefix in slot_ids:
+        u = np.unique(x % spacing + np.uint64(prefix) if prefix else x)
+        counts += np.bincount((farmhash64_np(u) % np.uint64(R)).astype(np.int64), minlength=R)
+    t = torch.tensor([int(counts.max())], dtype=torch.int64, device=dev)
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    return (int(int(t) * 1.5) + 1024 + 7) // 8 * 8
 
 
 class PersiaTrainingBatch:  # forward.rs:256-306, #[pyclass(dict)]: python attaches attributes to it
@@ -711,7 +775,14 @@ class Backward:  # backward.rs:203-405
                 with g["lock"]:
                     if is_raw:  # [U, dim] gradient of the distinct-sign table (persia/ctx.py:970-980)
                         item = grads.get(names[0])
-                        if item is None:
+                        if ctx is None:  # R GPUs: the slot's raw worker (a collective, even when skipped)
+                            wk = g["raw_workers"][names[0]]
+                            if item is None:
+                                wk.backward_raw(None)
+                            else:
+                                ptr, shape, is16, sc = item
+                                wk.backward_raw(ptr, scale=sc, is_f16=is16)
+                        elif item is None:
                             ctx.backward_raw(g["shard"], None)
                         else:
                             ptr, shape, is16, sc = item

@@ -48,15 +48,21 @@ def distinct_per_owner(ids, batch, prefixes, R, prefix_bit=8):
 class ShardedEmbeddingWorker:
     def __init__(self, n_slots, dim, prefixes, capacity, device, rank, world, cap, area, peer_bases, optimizer,
                  hyper=None, max_batch=4096, sqrt_scaling=None, rows_f32=False, prefix_bit=8, stream=None,
-                 max_ids_per_sample=1):
+                 max_ids_per_sample=1, shard=None):
+        """shard: an existing EmbeddingShard of this rank to serve (configured by its owner, who also closes it), so
+        that the workers of one dim — summation slots and raw slots — share one table; None: a new one."""
         self.S, self.dim, self.rank, self.R, self.cap = n_slots, dim, rank, world, int(cap)
         self.device = device if isinstance(device, torch.device) else torch.device("cuda", device)
         self.lib = N.load()
         self.stream = stream
         self.area = area  # keeps the receive area alive
-        self.shard = SH.EmbeddingShard(dim, capacity, self.device)
-        self.shard.set_optimizer(**optimizer)
-        self.shard.configure(**(hyper or {}))
+        self._own_shard = shard is None
+        if shard is None:
+            shard = SH.EmbeddingShard(dim, capacity, self.device)
+            shard.set_optimizer(**optimizer)
+            shard.configure(**(hyper or {}))
+        assert shard.dim == dim, "the shard holds another embedding dim"
+        self.shard = shard
         n = n_slots * max_batch * max_ids_per_sample
         self.ctx = SH.BatchContext(n, n_slots * max_batch, prefixes, sqrt_scaling, prefix_bit, self.device)
         bases = (C.c_uint64 * world)(*[int(p) for p in peer_bases])
@@ -72,15 +78,17 @@ class ShardedEmbeddingWorker:
         return b
 
     @classmethod
-    def local_group(cls, world, n_slots, dim, prefixes, capacity, cap, optimizer, device=0, **kw):
-        """R virtual ranks on one GPU (tests; also a way to exercise the protocol without a multi-GPU box)."""
+    def local_group(cls, world, n_slots, dim, prefixes, capacity, cap, optimizer, device=0, shards=None, **kw):
+        """R virtual ranks on one GPU (tests; also a way to exercise the protocol without a multi-GPU box).
+        shards: the R ranks' existing EmbeddingShards (e.g. `[w.shard for w in group]` of another group of this dim)."""
         dev = torch.device("cuda", device)
         nbytes = cls.area_bytes(world, cap, dim, kw.get("rows_f32", False))
         areas = [torch.zeros(nbytes + 256, dtype=torch.uint8, device=dev) for _ in range(world)]
         bases = [(a.data_ptr() + 255) // 256 * 256 for a in areas]
         torch.cuda.synchronize(dev)
         return [cls(n_slots, dim, prefixes, capacity, dev, r, world, cap, areas[r], bases, optimizer,
-                    stream=torch.cuda.Stream(device=dev), **kw) for r in range(world)]
+                    stream=torch.cuda.Stream(device=dev), shard=shards[r] if shards else None, **kw)
+                for r in range(world)]
 
     @classmethod
     def distributed(cls, n_slots, dim, prefixes, capacity, cap, optimizer, device, group=None, **kw):
@@ -209,10 +217,96 @@ class ShardedEmbeddingWorker:
             self.lib.pb_xchg_destroy(self.h)
             self.h = None
         self.ctx.close()
-        self.shard.close()
+        if self._own_shard:
+            self.shard.close()
 
     def __del__(self):
         try:
             self.close()
         except Exception:
             pass
+
+
+class ShardedRawWorker(ShardedEmbeddingWorker):
+    """One raw (embedding_summation: false) slot over the R GPUs of one box: pb_forward_raw_sharded /
+    pb_backward_raw_sharded.  Built like ShardedEmbeddingWorker with n_slots == 1 (its one prefix is the slot's
+    index_prefix); its exchange always carries f32 rows, which the requester rounds to the f16 table.  Pass `shard=` /
+    `shards=` to serve the table of the rank's summation worker of the same dim.  Every call is collective, including
+    batches without ids; each raw slot of a model has its own worker (its own exchange)."""
+
+    def __init__(self, n_slots, dim, prefixes, capacity, device, rank, world, cap, area, peer_bases, optimizer, **kw):
+        assert n_slots == 1 and len(prefixes) == 1, "a raw worker serves one slot"
+        kw["rows_f32"] = True
+        kw.pop("sqrt_scaling", None)  # (a raw slot's sqrt_scaling only matters with hash-stack, which it cannot have)
+        super().__init__(1, dim, prefixes, capacity, device, rank, world, cap, area, peer_bases, optimizer, **kw)
+        self._dummy = None
+
+    @staticmethod
+    def area_bytes(world, cap, dim, rows_f32=True):
+        return ShardedEmbeddingWorker.area_bytes(world, cap, dim, True)
+
+    def forward_raw(self, ids, batch, sample_fixed_size, row_off=None, training=True, out=None, phases=0):
+        """What BatchContext.forward_raw returns: (table f16 [n_occ+1, dim] of which rows [0, U] are valid, index i64
+        [batch*fixed], non_empty i64 of which counts[1] entries are valid, sample_id_num i32 [batch], counts i32 [2] =
+        (U, non-empty entries)), on the device.  out: those five buffers from an earlier call (phase-split and
+        captured calls reuse them)."""
+        ids = SH._as_i64_bits(ids)
+        n, fixed = ids.numel(), int(sample_fixed_size)
+        if out is None:
+            out = (torch.empty((n + 1, self.dim), dtype=torch.float16, device=self.device),
+                   torch.empty(batch * fixed, dtype=torch.int64, device=self.device),
+                   torch.empty(max(batch * fixed, 1), dtype=torch.int64, device=self.device),
+                   torch.empty(max(batch, 1), dtype=torch.int32, device=self.device),
+                   torch.empty(2, dtype=torch.int32, device=self.device))
+        table, index, non_empty, num, counts = out
+        if row_off is not None:
+            assert row_off.dtype == torch.int32 and row_off.is_contiguous() and row_off.numel() == batch + 1
+        N.check(self.lib.pb_forward_raw_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), n, SH._ptr(row_off),
+                                                int(batch), fixed, int(training), SH._ptr(table), SH._ptr(index),
+                                                SH._ptr(non_empty), SH._ptr(num), SH._ptr(counts), self._st(),
+                                                int(phases)))
+        return table, index, non_empty, num[:batch], counts
+
+    def backward_raw(self, grad, scale=1.0, want_status=False, is_f16=None, phases=0, status=None):
+        """grad: device tensor [U, dim] (f32 as persia/ctx.py:970-980 builds it, or f16), a raw device pointer (then
+        pass is_f16), or None (add_skipped_gradient).  A tensor that is not 16-byte aligned is copied first."""
+        ptr = None
+        if grad is not None and not isinstance(grad, int):
+            st = self.stream if self.stream is not None else torch.cuda.current_stream(self.device)
+            grad = SH.aligned(grad, st)
+            assert grad.is_contiguous() and grad.dtype in (torch.float16, torch.float32)
+            is_f16 = grad.dtype == torch.float16
+            if grad.numel():
+                ptr = grad.data_ptr()
+            else:  # U = 0: nothing is read, but the request is not a skipped one
+                if self._dummy is None:
+                    self._dummy = torch.zeros(4, dtype=torch.float32, device=self.device)
+                ptr = self._dummy.data_ptr()
+        elif grad is not None:
+            ptr = grad
+        if status is None and want_status:
+            status = torch.empty(1, dtype=torch.int32, device=self.device)
+        N.check(self.lib.pb_backward_raw_sharded(self.shard.h, self.ctx.h, self.h, ptr, int(bool(is_f16)), float(scale),
+                                                 SH._ptr(status), self._st(), int(phases)))
+        return status
+
+    @staticmethod
+    def group_forward_raw(workers, ids, batch, sample_fixed_size, training=True, row_offs=None, outs=None):
+        """Virtual ranks of one GPU, driven by one host thread: every phase is enqueued for all ranks before the next.
+        Returns one forward_raw result per rank."""
+        R = len(workers)
+        outs = list(outs) if outs is not None else [None] * R
+        for ph in (N.PHASE_SEND, N.PHASE_SERVE, N.PHASE_FINISH):
+            for r, w in enumerate(workers):
+                outs[r] = w.forward_raw(ids[r], batch, sample_fixed_size, row_offs[r] if row_offs else None, training,
+                                        out=outs[r], phases=ph)
+        return outs
+
+    @staticmethod
+    def group_backward_raw(workers, grads, scales=None, want_status=False):
+        """grads: per rank a [U_r, dim] tensor or None (add_skipped_gradient); scales: per rank (default 1)."""
+        sts = [torch.empty(1, dtype=torch.int32, device=w.device) if want_status else None for w in workers]
+        for ph in (N.PHASE_SEND, N.PHASE_SERVE):
+            for r, w in enumerate(workers):
+                w.backward_raw(grads[r], scales[r] if scales is not None else 1.0, phases=ph, status=sts[r])
+        return sts
