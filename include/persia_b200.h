@@ -235,8 +235,9 @@ int pb_xchg_status(pb_xchg* x, uint32_t h_out[2], void* stream);
 #define PB_PHASE_SERVE 2  /* owner: forward lookups + rows out; backward optimizer steps */
 #define PB_PHASE_FINISH 4 /* requester, forward only: rows in -> output */
 #define PB_PHASE_ALL 7
-/* forward_batched_direct over R shards: arguments as pb_forward.  Not supported here yet: slots sharing a
- * feature group (raw slots: pb_forward_raw_sharded below). */
+/* forward_batched_direct over R shards: arguments as pb_forward (raw slots: pb_forward_raw_sharded below).  Slots that
+ * share a feature group (equal prefixes) are supported: a sign held by several of them is one entry per slot of the
+ * request, and the owner steps a row rank by rank, each rank's entries in slot order, as the reference does. */
 int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
                        const uint32_t* h_slot_occ_off, uint32_t batch, int training, void* d_out_f16, void* stream,
                        int phases);

@@ -108,6 +108,7 @@ struct pb_ctx {
   // slots of one feature group take turns in the backward (mod.rs:720-822): round of every slot
   uint32_t n_rounds = 1;
   uint8_t round_of[PB_MAX_SLOTS];
+  GroupLinks links;  // sharded path: previous / next slot of every slot's group (k_link_items)
   // backward workspace
   uint32_t* nan_tick = nullptr;
   float* vw_stage = nullptr;
@@ -646,10 +647,15 @@ int pb_ctx_set_slots(pb_ctx* c, const pb_slots_cfg* cfg) {
   // two slots with the same prefix share a key space (one feature group): a sign may sit in both, and the reference
   // steps it once per slot, in slot order (mod.rs:720-822).  Slot s runs in round = number of earlier slots of its group.
   c->n_rounds = 1;
+  std::memset(&c->links, 0xFF, sizeof(c->links));
   for (uint32_t i = 0; i < cfg->n_slots; ++i) {
     uint32_t r = 0;
     for (uint32_t k = 0; k < i; ++k)
-      if (cfg->prefix[i] == cfg->prefix[k]) ++r;
+      if (cfg->prefix[i] == cfg->prefix[k]) {
+        ++r;
+        c->links.prev[i] = (uint8_t)k;  // (the nearest earlier slot of the group is the last one found)
+      }
+    if (c->links.prev[i] != 0xFF) c->links.next[c->links.prev[i]] = (uint8_t)i;
     c->round_of[i] = (uint8_t)r;
     if (r + 1 > c->n_rounds) c->n_rounds = r + 1;
   }
@@ -843,12 +849,13 @@ struct pb_xchg {
 
 namespace {
 uint64_t round256(uint64_t v) { return (v + 255u) & ~(uint64_t)255u; }
-void xchg_layout(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32, uint64_t off[5]) {
+void xchg_layout(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32, uint64_t off[6]) {
   off[0] = round256((uint64_t)XC_WORDS * PB_MAX_RANKS * 4);                        // sign
   off[1] = off[0] + round256((uint64_t)R * cap * 8);                               // row
   off[2] = off[1] + round256((uint64_t)R * cap * dim * (rows_f32 ? 4 : 2));        // grad
   off[3] = off[2] + round256((uint64_t)R * cap * dim * 4);                         // gok
-  off[4] = off[3] + round256((uint64_t)R * cap * 4);                               // end
+  off[4] = off[3] + round256((uint64_t)R * cap * 4);                               // chain
+  off[5] = off[4] + round256((uint64_t)R * cap * 4);                               // end
 }
 
 // The owner's part of a sharded backward (PB_PHASE_SERVE), shared by the summation and the raw calls: the step's R
@@ -885,9 +892,9 @@ int owner_backward(pb_table* t, pb_xchg* x, const uint64_t* prefix, uint32_t n_p
 
 uint64_t pb_xchg_bytes(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32) {
   if (R == 0 || R > PB_MAX_RANKS || cap == 0 || dim == 0) return 0;
-  uint64_t off[5];
+  uint64_t off[6];
   xchg_layout(R, cap, dim, rows_f32, off);
-  return off[4];
+  return off[5];
 }
 
 int pb_xchg_create(int device, uint32_t R, uint32_t rank, uint32_t cap, uint32_t dim, int rows_f32,
@@ -895,13 +902,14 @@ int pb_xchg_create(int device, uint32_t R, uint32_t rank, uint32_t cap, uint32_t
   if (!out || !h_peer_base || R == 0 || R > PB_MAX_RANKS || rank >= R || cap == 0 || dim == 0)
     return fail(PB_ERR_INVALID, "bad argument");
   if ((uint64_t)R * cap >= 0xFFFFFFF0ull) return fail(PB_ERR_INVALID, "R * cap must stay below 2^32 - 16");
+  if (cap >= CHAIN_END) return fail(PB_ERR_INVALID, "cap must stay below 2^31 - 1");
   for (uint32_t q = 0; q < R; ++q)
     if (!h_peer_base[q] || (h_peer_base[q] & 255u)) return fail(PB_ERR_INVALID, "receive areas must be mapped and 256-byte aligned");
   DeviceGuard g(device);
   pb_xchg* x = new pb_xchg();
   x->device = device;
   x->dim = dim;
-  uint64_t off[5];
+  uint64_t off[6];
   xchg_layout(R, cap, dim, rows_f32, off);
   XchgDev& d = x->d;
   std::memset(&d, 0, sizeof(d));
@@ -910,11 +918,12 @@ int pb_xchg_create(int device, uint32_t R, uint32_t rank, uint32_t cap, uint32_t
   d.off_row = off[1];
   d.off_grad = off[2];
   d.off_gok = off[3];
+  d.off_chain = off[4];
   d.R = R;
   d.rank = rank;
   d.cap = cap;
   d.row_f32 = rows_f32 ? 1 : 0;
-  const size_t words = XC_WORDS + (size_t)XC_WORDS * PB_MAX_RANKS + PB_MAX_RANKS + 4 + 2 * (size_t)R * cap;
+  const size_t words = XC_WORDS + (size_t)XC_WORDS * PB_MAX_RANKS + PB_MAX_RANKS + 4 + 3 * (size_t)R * cap + 1;
   cudaError_t e = cudaMalloc(&x->mem, 4 * words);
   if (e == cudaSuccess) e = cudaMemset(x->mem, 0, 4 * words);
   uint32_t ucells = 1024;
@@ -935,6 +944,8 @@ int pb_xchg_create(int device, uint32_t R, uint32_t rank, uint32_t cap, uint32_t
   d.err = d.own_cnt + PB_MAX_RANKS;
   d.own_row = d.err + 4;
   d.uwin = d.own_row + (size_t)R * cap;
+  d.own_link = d.uwin + (size_t)R * cap;
+  d.chained = d.own_link + (size_t)R * cap;
   d.ucell = x->ucell;
   d.ucells = ucells;
   d.akeys = x->akeys;
@@ -978,7 +989,6 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
   if (t->device != c->device || t->device != x->device) return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
   if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
   if (batch > 65535) return fail(PB_ERR_BATCH, "batch size cannot be larger than 65535");
-  if (c->n_rounds != 1) return fail(PB_ERR_INVALID, "slots sharing a feature group are not supported on the sharded path");
   if (d_row_off && !x->d.row_f32) return fail(PB_ERR_INVALID, "ragged layouts need an exchange created with f32 rows");
   uint32_t S = c->slots.n_slots;
   uint64_t n_out = (uint64_t)S * batch;
@@ -1009,6 +1019,7 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
     c->b.n = n_occ;
     launch_dedup(sl, c->b, d_ids, st);
     launch_route_items(training != 0, sl, c->b, x->d, st);               // requester: signs -> owners' areas
+    if (training && c->n_rounds > 1) launch_link_items(sl, c->b, x->d, c->links, st);  // a sign's entries, slot order
     if (all) launch_signal_wait(x->d, XC_FLAG_SIGN, c->b.cnt + BC_PEER, st);  // (one launch when no phase split is asked for)
     else launch_signal(x->d, XC_FLAG_SIGN, c->b.cnt + BC_PEER, st);
   }

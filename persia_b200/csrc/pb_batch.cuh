@@ -5,6 +5,12 @@
 
 namespace pb {
 
+// the scratch set's region of a slot (k_dedup, pb_dedup.cu): linear probing from a hash over `size` cells
+__device__ __forceinline__ uint32_t set_region(const SlotsDev& sl, uint32_t slot, uint32_t& size) {
+  size = 2u * (sl.occ_off[slot + 1] - sl.occ_off[slot]) + 1u;  // the reserved cell (sign == KEY_EMPTY) follows
+  return 2u * sl.occ_off[slot] + 2u * slot;
+}
+
 // block-level list bookkeeping shared by k_probe_items and k_route_items (pb_shard.cu): every thread of the block
 // calls it once, converged.  `head`: this thread speaks for an item; cnt its multiplicity (0 = keep nothing);
 // returns through the references the item's list position and the base of its occurrence list.

@@ -17,11 +17,6 @@
 
 namespace pb {
 
-__device__ __forceinline__ uint32_t set_region(const SlotsDev& sl, uint32_t slot, uint32_t& size) {
-  size = 2u * (sl.occ_off[slot + 1] - sl.occ_off[slot]) + 1u;  // the reserved cell (sign == KEY_EMPTY) follows
-  return 2u * sl.occ_off[slot] + 2u * slot;
-}
-
 // ------------------------------------------------------------------------------------------------
 // A0 + A2.  One thread per id occurrence: prefix, insert-or-find in the slot's region (linear probing, CAS on
 // the key), count.  Counting and item numbering are aggregated per warp (__match_any_sync / ballot): a sign

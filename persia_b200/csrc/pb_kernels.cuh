@@ -70,7 +70,19 @@ struct BatchDev {
 //   row    [R][cap][dim]        rows returned to this rank, by owner (f16, or f32 for ragged layouts)
 //   grad   [R][cap][dim] f32    reduced gradients sent to this rank, by source
 //   gok    [R][cap] u32         1 = apply the gradient, 0 = the slot was skipped / held a NaN
-enum { XC_FLAG_SIGN = 0, XC_FLAG_ROW, XC_FLAG_GRAD, XC_COUNT, XC_WORDS };
+//   chain  [R][cap] u32         requests with slots sharing a feature group: CHAIN_CONT | the sign's next entry
+// ctrl word XC_CHAIN of a source equals its XC_FLAG_SIGN word when that source's request of the step carries chain words.
+enum { XC_FLAG_SIGN = 0, XC_FLAG_ROW, XC_FLAG_GRAD, XC_COUNT, XC_CHAIN, XC_WORDS };
+// chain word of an entry: a sign that several slots of one feature group hold is one entry per slot; the first (the
+// head, in slot order) carries the step, the others follow it.  CHAIN_CONT: not a head; low bits: the request's next
+// entry of the sign (CHAIN_END: none).
+constexpr uint32_t CHAIN_CONT = 0x80000000u;
+constexpr uint32_t CHAIN_END = 0x7FFFFFFFu;
+// the slots of a context's feature groups in slot order: prev / next slot of the same group (0xFF: none)
+struct GroupLinks {
+  uint8_t prev[PB_MAX_SLOTS];
+  uint8_t next[PB_MAX_SLOTS];
+};
 constexpr uint32_t PB_MAX_RANKS = 16;
 constexpr uint32_t PB_ADAM_KEYS = 256;  // beta-power pairs per table; the last one serves pb_update
 // owner side, one step: the distinct rows the R requests touch (k_owner_lookup fills it, k_owner_update_all empties it)
@@ -82,7 +94,7 @@ struct __align__(16) UCell {
 };
 struct XchgDev {
   uint64_t base[PB_MAX_RANKS];
-  uint64_t off_sign, off_row, off_grad, off_gok;  // byte offsets inside an area (ctrl at 0)
+  uint64_t off_sign, off_row, off_grad, off_gok, off_chain;  // byte offsets inside an area (ctrl at 0)
   uint32_t R, rank, cap, row_f32;
   uint32_t* epoch;     // [XC_WORDS] phases signalled so far (device side: CUDA-graph safe)
   uint32_t* waited;    // [XC_WORDS][PB_MAX_RANKS] phases waited for so far, per source
@@ -92,6 +104,8 @@ struct XchgDev {
   UCell* ucell;        // [ucells] rows of the step's requests, hashed by row number
   uint32_t* uwin;      // [R][cap] the cell a request's sign opened (it was the first to ask for the row), else ROW_NONE
   uint32_t ucells;     // a power of two >= 2 R cap
+  uint32_t* chained;   // [1] bit per source: its request of this step carries chain words (forward -> backward)
+  uint32_t* own_link;  // [R][cap] chain word of every received sign of such a request (forward -> backward)
   // Adam on the owner: feature groups (index prefixes) of the table, the groups each request holds, and the (beta1^t,
   // beta2^t) pair every request's signs of a group use (get_batch_level_state, optim.rs:151-197)
   const uint64_t* akeys;  // [n_akeys] prefixes, position = pair number of the table
@@ -160,6 +174,7 @@ void launch_reduce_items(const TableDev& t, const OptimDev& op, const HyperDev& 
                          bool send = false);
 // pb_shard.cu
 void launch_route_items(bool training, const SlotsDev& sl, const BatchDev& b, const XchgDev& x, cudaStream_t st);
+void launch_link_items(const SlotsDev& sl, const BatchDev& b, const XchgDev& x, const GroupLinks& gl, cudaStream_t st);
 void launch_signal(const XchgDev& x, int phase, const uint32_t* counts, cudaStream_t st);
 void launch_wait(const XchgDev& x, int phase, int src /* -1: every source */, cudaStream_t st);
 void launch_signal_wait(const XchgDev& x, int phase, const uint32_t* counts, cudaStream_t st);

@@ -12,6 +12,7 @@
 //
 // There is no separate exchange step: the kernel that produces data writes it where its consumer lives.
 //   k_route_items    (requester) owner of every distinct sign, sign stored straight into the owner's receive area
+//   k_link_items     (requester, slots sharing a feature group only) a sign's entries of one request linked in slot order
 //   k_owner_lookup   (owner) find / admit / initialise, row gathered, converted and stored straight into the
 //                    requester's receive area
 //   k_expand_items   (requester) received rows -> output rows in batch order (+ pooling for ragged layouts)
@@ -34,6 +35,9 @@ __device__ __forceinline__ uint64_t* x_sign(const XchgDev& x, uint32_t q) {
 }
 __device__ __forceinline__ unsigned char* x_row(const XchgDev& x, uint32_t q) {
   return reinterpret_cast<unsigned char*>(x.base[q] + x.off_row);
+}
+__device__ __forceinline__ uint32_t* x_chain(const XchgDev& x, uint32_t q) {
+  return reinterpret_cast<uint32_t*>(x.base[q] + x.off_chain);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -92,6 +96,60 @@ __global__ void __launch_bounds__(256) k_route_items(SlotsDev sl, BatchDev b, Xc
     if (is.cls == 1) b.cold[is.pos] = make_uint2(target, first);
     else if (is.cls == 2) b.warm[is.pos] = make_uint4(target, is.base, cnt, 0u);
     else if (is.cls == 3) b.hot[is.pos] = make_uint4(target, is.base, cnt, slot);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// requester, forward, slots sharing a feature group (launched only then): a sign that several slots of one group hold
+// is one entry per slot in its owner's request, and the reference steps them one after another in slot order
+// (mod.rs:703-872).  Every routed item looks for its sign in the regions of the other slots of its group, nearest
+// first, and writes its entry's chain word: CHAIN_CONT if an earlier slot holds the sign (the owner steps it after
+// that one), and the entry of the next later slot that does (or CHAIN_END).  Items over cap take no part.  Block 0
+// also marks this request as carrying chain words: the owner compares ctrl[XC_CHAIN] with the SIGN flag about to be
+// raised, so a mark left from an earlier step never counts.
+// ------------------------------------------------------------------------------------------------
+// target of `sign` in the scratch-set region of `slot` (k_dedup's probe sequence), ROW_NONE if absent or over cap
+__device__ __forceinline__ uint32_t find_in_slot(const SlotsDev& sl, const BatchDev& b, uint32_t slot, uint64_t sign) {
+  uint32_t size;
+  const uint32_t off = set_region(sl, slot, size);
+  if (sign == KEY_EMPTY) {  // the reserved cell: key 0 when the slot holds the sign
+    const DCell& c = b.set[off + size];
+    return c.key != KEY_EMPTY ? c.target : ROW_NONE;
+  }
+  uint32_t idx = off + __umulhi((uint32_t)(mix64(sign) >> 32), size);
+  for (;;) {  // the region has more cells than the slot has ids: ends on an empty cell
+    const uint64_t k = b.set[idx].key;
+    if (k == sign) return b.set[idx].target;
+    if (k == KEY_EMPTY) return ROW_NONE;
+    idx = (idx + 1 == off + size) ? off : idx + 1;
+  }
+}
+
+__global__ void __launch_bounds__(256) k_link_items(SlotsDev sl, BatchDev b, XchgDev x, GroupLinks gl) {
+  if (blockIdx.x == 0 && threadIdx.x < x.R) x_ctrl(x, threadIdx.x)[XC_CHAIN * PB_MAX_RANKS + x.rank] = x.epoch[XC_FLAG_SIGN] + 1u;
+  const uint32_t n_items = b.cnt[BC_ITEMS];
+  for (uint32_t u = blockIdx.x * blockDim.x + threadIdx.x; u < n_items; u += gridDim.x * blockDim.x) {
+    const uint32_t cell = b.item_cell[u];
+    const uint4 lo = *reinterpret_cast<const uint4*>(&b.set[cell]);
+    const uint4 hi = *(reinterpret_cast<const uint4*>(&b.set[cell]) + 1);  // target, base, first, item
+    const uint32_t target = hi.x;
+    if (target == ROW_NONE) continue;
+    const uint64_t sign = (hi.w >> 31) ? KEY_EMPTY : ((uint64_t)lo.x | ((uint64_t)lo.y << 32));
+    const uint32_t slot = slot_of_occ(sl, hi.z);
+    uint32_t word = CHAIN_END;
+    for (uint32_t s = gl.prev[slot]; s != 0xFFu; s = gl.prev[s])
+      if (find_in_slot(sl, b, s, sign) != ROW_NONE) {
+        word |= CHAIN_CONT;
+        break;
+      }
+    for (uint32_t s = gl.next[slot]; s != 0xFFu; s = gl.next[s]) {
+      const uint32_t t2 = find_in_slot(sl, b, s, sign);
+      if (t2 != ROW_NONE) {
+        word = (word & CHAIN_CONT) | (t2 % x.cap);  // (same sign, same owner)
+        break;
+      }
+    }
+    x_chain(x, target / x.cap)[(size_t)x.rank * x.cap + target % x.cap] = word;  // over NVLink when the owner is a peer
   }
 }
 
@@ -159,6 +217,19 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_owner_lookup(TableDev 
   const uint32_t* ctrl = x_ctrl(x, x.rank);
   const uint32_t warp_first = ((blockIdx.x * blockDim.x + threadIdx.x) / 32) * (32 / BUCKET);
   if (blockIdx.x == 0 && threadIdx.x < x.R) x.own_cnt[threadIdx.x] = ctrl[XC_COUNT * PB_MAX_RANKS + threadIdx.x];
+  uint32_t chained = 0;  // sources whose request carries chain words (k_link_items)
+  if (MODE == MODE_TRAIN) {
+    __shared__ uint32_t s_chained;
+    if (threadIdx.x == 0) s_chained = 0u;
+    __syncthreads();
+    if (threadIdx.x < x.R) {
+      const uint32_t f = ctrl[XC_FLAG_SIGN * PB_MAX_RANKS + threadIdx.x];
+      if (f != 0u && ctrl[XC_CHAIN * PB_MAX_RANKS + threadIdx.x] == f) atomicOr(&s_chained, 1u << threadIdx.x);
+    }
+    __syncthreads();
+    chained = s_chained;
+    if (blockIdx.x == 0 && threadIdx.x == 0) *x.chained = chained;
+  }
   for (uint32_t j0 = warp_first; j0 < total; j0 += groups) {  // uniform per warp
     const uint32_t j = j0 + lane / BUCKET;
     const uint32_t src = j / x.cap, k = j % x.cap;
@@ -175,9 +246,14 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_owner_lookup(TableDev 
       x.own_row[j] = r.row;
       if (r.row == ROW_NONE) atomicAdd(&t.counters[CTR_MISS], 1u);
       if (MODE == MODE_TRAIN) {
-        // the backward steps every row ONCE for all the requests that hold it (in rank order): note who asked
-        uint32_t won = ROW_NONE;
-        if (r.row < t.capacity) {
+        // the backward steps every row ONCE for all the requests that hold it (in rank order): note who asked.  A
+        // chained request notes the head of each sign's chain; the other entries are reached through the links.
+        uint32_t won = ROW_NONE, link = CHAIN_END;
+        if ((chained >> src) & 1u) {
+          link = x_chain(x, x.rank)[j];
+          x.own_link[j] = link;  // (the area's word may be overwritten by the source's next request before the backward)
+        }
+        if (r.row < t.capacity && !(link & CHAIN_CONT)) {
           uint32_t idx = (r.row * 0x9E3779B1u) & (x.ucells - 1u);
           for (;;) {
             const uint32_t old = atomicCAS(&x.ucell[idx].row, ROW_NONE, r.row);
@@ -383,8 +459,9 @@ template <int VEC, int CPL, int KIND>
 __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(TableDev t, OptimDev op, HyperDev hy, XchgDev x, uint32_t G) {
   // G lanes per row, CPL chunks of VEC floats per lane (G * CPL * VEC == dim): few lanes per row keep the per-row
   // bookkeeping off most of the warp, and a lane has CPL independent loads in flight
-  __shared__ uint32_t s_cnt[PB_MAX_RANKS];
+  __shared__ uint32_t s_cnt[PB_MAX_RANKS], s_chained;
   if (threadIdx.x < PB_MAX_RANKS) s_cnt[threadIdx.x] = threadIdx.x < x.R ? x.own_cnt[threadIdx.x] : 0u;
+  if (threadIdx.x == 0) s_chained = *x.chained;
   __syncthreads();
   const uint32_t wl = threadIdx.x & 31u, lane = wl % G, gi = wl / G, n_g = 32u / G;
   const uint32_t gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (gi * G));
@@ -440,7 +517,8 @@ __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(Tabl
         rc[u].load(prow, e, t, op);
         load_vec<VEC>(grads + (size_t)j * t.dim + e, g1[u]);
       }
-      if (mask == (1u << me)) {  // the opener is the only holder (the rule)
+      const uint32_t chained = mask & s_chained;  // holders whose request may hold the row more than once
+      if (mask == (1u << me) && !chained) {  // the opener is the only holder, with one entry (the rule)
         if (ok1) {
           PB_ADAM_CTX(me)
 #pragma unroll
@@ -450,6 +528,29 @@ __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(Tabl
             rc[u].store(prow, e, t, op);
           }
         }
+      } else if (chained) {
+        // slots sharing a feature group: every holder in rank order, and within its request the sign's entries in
+        // slot order — the head (the cell's index), then the chain; a skipped entry is passed over, the walk goes on
+        for (uint32_t m = mask; m; m &= m - 1u) {
+          const uint32_t s = (uint32_t)__ffs(m) - 1u;
+          uint32_t k = cell->k[s];
+          for (uint32_t d = 0; d < PB_MAX_SLOTS; ++d) {  // (a chain holds at most one entry per slot)
+            const uint32_t at = s * x.cap + k;
+            if (gok[at]) {
+              float g[CPL][VEC];
+#pragma unroll
+              for (int u = 0; u < CPL; ++u) load_vec<VEC>(grads + (size_t)at * t.dim + ((uint32_t)u * G + lane) * VEC, g[u]);
+              PB_ADAM_CTX(s)
+#pragma unroll
+              for (int u = 0; u < CPL; ++u) rc[u].step(((uint32_t)u * G + lane) * VEC, g[u], t, op, hy, sc);
+            }
+            if (!((chained >> s) & 1u)) break;
+            k = x.own_link[at] & CHAIN_END;
+            if (k >= s_cnt[s]) break;  // CHAIN_END
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < CPL; ++u) rc[u].store(prow, ((uint32_t)u * G + lane) * VEC, t, op);
       } else {
         for (uint32_t m = mask; m;) {  // holders in rank order, two at a time: index, apply word, gradient — each stage
           uint32_t at[2], ok[2];       // issued for both before the next
@@ -512,6 +613,52 @@ __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, H
   const float* grads = reinterpret_cast<const float*>(x.base[x.rank] + x.off_grad) + (size_t)src * x.cap * t.dim;
   const uint32_t* gok = reinterpret_cast<const uint32_t*>(x.base[x.rank] + x.off_gok) + (size_t)src * x.cap;
   const uint32_t* own_row = x.own_row + (size_t)src * x.cap;
+  if ((*x.chained >> src) & 1u) {
+    // slots sharing a feature group: a lane group takes a chain's head and steps the sign's entries one after another in
+    // slot order (so no two groups hold one row); the entries after the head only count their misses here
+    const uint32_t* link = x.own_link + (size_t)src * x.cap;
+    const uint32_t wl = threadIdx.x & 31u;
+    const uint32_t gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (wl / G * G));
+    for (uint32_t k0 = blockIdx.x * (blockDim.x / G) + threadIdx.x / G; k0 < n; k0 += n_groups) {
+      const uint32_t row = own_row[k0];
+      if (row >= t.capacity) {
+        if (lane == 0 && gok[k0] != 0u) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);
+        continue;
+      }
+      if (link[k0] & CHAIN_CONT) continue;
+      float* prow = t.rows + (size_t)row * t.stride;
+      StepCtx sc;
+      sc.r1 = sc.r2 = 0.0f;
+      if (op.kind == PB_OPT_ADAM) {  // this request's (beta1^t, beta2^t) of the row's feature group
+        const float* pw = x.apow + ((size_t)src * PB_ADAM_KEYS + adam_key_of(x, x_sign(x, x.rank)[(size_t)src * x.cap + k0])) * 2u;
+        sc.r1 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[0]));
+        sc.r2 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[1]));
+      }
+      uint32_t k = k0;
+      for (uint32_t d = 0; d < PB_MAX_SLOTS; ++d) {  // (a chain holds at most one entry per slot)
+        if (gok[k] != 0u) {
+          const float* g0 = grads + (size_t)k * t.dim;
+          sc.vw_state = op.kind == PB_OPT_ADAGRAD_VW ? prow[t.dim] : 0.0f;
+          for (uint32_t c = lane; c < nvec; c += G) {
+            RowElems<-1, VEC> rc;
+            float g[VEC];
+            rc.load(prow, c * VEC, t, op);
+            load_vec<VEC>(g0 + c * VEC, g);
+            rc.step(c * VEC, g, t, op, hy, sc);
+            rc.store(prow, c * VEC, t, op);
+          }
+          if (op.kind == PB_OPT_ADAGRAD_VW) {  // every lane has read the state before lane 0 writes the next one
+            __syncwarp(gmask);
+            if (lane == 0) prow[t.dim] = __fadd_rn(__fmul_rn(sc.vw_state, op.mom), __fdiv_rn(vw_dot(g0, t.dim), (float)t.dim));
+            __syncwarp(gmask);
+          }
+        }
+        k = link[k] & CHAIN_END;
+        if (k >= n) break;  // CHAIN_END
+      }
+    }
+    return;
+  }
   for (uint32_t k0 = (blockIdx.x * (blockDim.x / G) + threadIdx.x / G) * 2; k0 < n; k0 += n_groups * 2) {
     // two requests' worth of loads in flight per lane group
     float* prow[2];
@@ -687,6 +834,12 @@ void launch_route_items(bool training, const SlotsDev& sl, const BatchDev& b, co
   const uint32_t grid = cdiv(b.n, 256);  // worst case U = N; blocks past the item count return at once
   if (training) PB_LAUNCH_F(FAM_ROUTE, (k_route_items<true>), grid, 256, 0, st, sl, b, x);
   else PB_LAUNCH_F(FAM_ROUTE, (k_route_items<false>), grid, 256, 0, st, sl, b, x);
+}
+
+void launch_link_items(const SlotsDev& sl, const BatchDev& b, const XchgDev& x, const GroupLinks& gl, cudaStream_t st) {
+  if (!b.n) return;
+  const uint32_t full = cdiv(b.n, 256);  // worst case U = N; the blocks stride over the items
+  PB_LAUNCH_F(FAM_ROUTE, k_link_items, full < PB_NUM_SMS * 4u ? full : PB_NUM_SMS * 4u, 256, 0, st, sl, b, x, gl);
 }
 
 void launch_signal(const XchgDev& x, int phase, const uint32_t* counts, cudaStream_t st) {

@@ -9,7 +9,9 @@ in `sys.modules` as `persia_core`, after which the reference's own `persia` pack
 
 Scope: summation and raw slots (no hash-stack on raw slots), one process per GPU.  With `replica_size > 1` every dim
 group is served by a ShardedEmbeddingWorker and every raw slot by its own ShardedRawWorker (persia_b200.worker), all
-of one dim on the rank's one table; there a raw slot may not share its feature group with another slot of the batch.
+of one dim on the rank's one table; summation slots there may share a feature group (each rank's entries of a shared
+sign are applied in slot order, the ranks in rank order), but a raw slot may not share its feature group with another
+slot of the batch.
 Their calls are collective, so every rank issues them in one fixed order: the raw slots in batch order, then the
 summation dims in ascending order, in the forward and again in the backward; every batch must carry the same raw
 slots in the same order.  `Forward` prefetches on worker threads with the reference's ordering and
