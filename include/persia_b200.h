@@ -100,6 +100,11 @@ int pb_table_spill(pb_table* t, uint64_t want_free, uint32_t keep_batches, uint6
  * refused because the shard is full, [4] in-kernel waits that gave up (must stay 0: a non-zero value voids the batch
  * that raised it).  Synchronises `stream`. */
 int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream);
+/* Diagnostic: the state of the hash index's n_cells normal cells (the three cells reserved for the marker-valued signs
+ * are not counted): [0] live (a resident sign), [1] tombstones (an evicted sign), [2] EMPTY.  An admission needs an
+ * EMPTY cell on its probe path; every eviction check rebuilds the index (tombstones dropped) once fewer than 1/8 of the
+ * cells are EMPTY.  Synchronises `stream`. */
+int pb_table_index_stats(pb_table* t, uint64_t h_out[3], void* stream);
 
 /* ---- single-request entry points (the PS RPCs) ------------------------------------------------- */
 /* lookup_mixed -> batched_lookup (embedding_parameter_service/mod.rs:162-262, 344-357).

@@ -84,6 +84,9 @@ struct pb_table {
   uint32_t evict_every = 0, evict_low = 0, evict_target = 0, evict_keep = 2;
   uint32_t train_calls = 0;
   uint32_t* evict_ws = nullptr;
+  uint64_t* rebuild_keys = nullptr;  // the index rebuild's compacted (sign, row) pairs, `capacity` each
+  uint32_t* rebuild_rows = nullptr;
+  uint32_t* stats_ws = nullptr;      // pb_table_index_stats
   uint32_t pending_batches = 0;  // training forwards whose backward has not been enqueued yet
 };
 
@@ -120,7 +123,7 @@ struct pb_ctx {
   uint32_t* occ_cell = nullptr;
   RawWork raw{};
   bool raw_ready = false, raw_pending = false;
-  pb_table* raw_table = nullptr;  // sharded raw forward pending on this table: counted in its pending_batches
+  pb_table* raw_table = nullptr;  // raw forward pending on this table: counted in its pending_batches
   float* raw_stage = nullptr;
   size_t raw_stage_floats = 0;
 };
@@ -174,17 +177,27 @@ int ensure_scratch(pb_table* t, uint32_t n) {
   return PB_OK;
 }
 
-// Between two training requests: release the least recently used rows when free storage runs low.
+// the free-row stack, the sweep's workspace and the rebuild's pair buffer, allocated by the first sweep
+int ensure_evict_ws(pb_table* t) {
+  if (t->d.free_rows) return PB_OK;
+  const size_t cap = t->d.capacity;
+  PB_CUDA(cudaMalloc(&t->evict_ws, sizeof(uint32_t) * EVICT_WS_WORDS));
+  PB_CUDA(cudaMalloc(&t->rebuild_keys, sizeof(uint64_t) * cap));
+  PB_CUDA(cudaMalloc(&t->rebuild_rows, sizeof(uint32_t) * cap));
+  PB_CUDA(cudaMalloc(&t->d.free_rows, sizeof(uint32_t) * cap));
+  return PB_OK;
+}
+
+// Between two training requests: release the least recently used rows when free storage runs low, and rebuild the
+// index when its EMPTY cells run short.
 int maybe_evict(pb_table* t, cudaStream_t st) {
   if (!t->evict_every || (++t->train_calls % t->evict_every)) return PB_OK;
-  if (!t->d.free_rows) {
-    PB_CUDA(cudaMalloc(&t->d.free_rows, sizeof(uint32_t) * (size_t)t->d.capacity));
-    PB_CUDA(cudaMalloc(&t->evict_ws, sizeof(uint32_t) * (3 + 1024)));
-  }
+  int rc = ensure_evict_ws(t);
+  if (rc) return rc;
   // rows of batches whose gradients are still to come are never released: a row used by a pending batch was
   // refreshed by its forward, i.e. at most `pending_batches` requests ago
   const uint32_t keep = t->evict_keep > t->pending_batches + 1 ? t->evict_keep : t->pending_batches + 1;
-  launch_evict(t->d, t->evict_low, t->evict_target, keep, t->evict_ws, st);
+  launch_evict(t->d, t->evict_low, t->evict_target, keep, t->evict_ws, t->rebuild_keys, t->rebuild_rows, st);
   return PB_OK;
 }
 
@@ -244,7 +257,7 @@ void drop_pending(pb_ctx* c) {
   c->pending_table = nullptr;
 }
 
-// a sharded raw forward's rows stay protected from eviction until its gradients are applied, like a summation batch's
+// a raw forward's rows stay protected from eviction until its gradients are applied, like a summation batch's
 void drop_raw_pending(pb_ctx* c) {
   if (c->raw_table && c->raw_table->pending_batches) c->raw_table->pending_batches--;
   c->raw_table = nullptr;
@@ -298,7 +311,10 @@ int pb_table_destroy(pb_table* t) {
     cudaFree(t->d.row_tick);
     if (t->d.free_rows) cudaFree(t->d.free_rows);
     if (t->evict_ws) cudaFree(t->evict_ws);
+    if (t->rebuild_keys) cudaFree(t->rebuild_keys);
+    if (t->rebuild_rows) cudaFree(t->rebuild_rows);
   }
+  if (t->stats_ws) cudaFree(t->stats_ws);
   if (t->scratch) cudaFree(t->scratch);
   if (t->adam_dev) cudaFree(t->adam_dev);
   delete t;
@@ -345,14 +361,13 @@ int pb_table_spill(pb_table* t, uint64_t want_free, uint32_t keep_batches, uint6
   if (!t || !d_count || (max_n && (!d_signs || !d_entries))) return fail(PB_ERR_INVALID, "null argument");
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
-  if (!t->d.free_rows) {
-    PB_CUDA(cudaMalloc(&t->d.free_rows, sizeof(uint32_t) * (size_t)t->d.capacity));
-    PB_CUDA(cudaMalloc(&t->evict_ws, sizeof(uint32_t) * (3 + 1024)));
-  }
+  int rc = ensure_evict_ws(t);
+  if (rc) return rc;
   if (want_free > t->d.capacity) want_free = t->d.capacity;
   const uint32_t keep = keep_batches > t->pending_batches + 1 ? keep_batches : t->pending_batches + 1;
   PB_CUDA(cudaMemsetAsync(d_count, 0, sizeof(uint32_t), st));
-  launch_spill(t->d, (uint32_t)want_free, keep, t->evict_ws, d_signs, d_entries, max_n, d_count, st);
+  launch_spill(t->d, (uint32_t)want_free, keep, t->evict_ws, t->rebuild_keys, t->rebuild_rows, d_signs, d_entries, max_n,
+               d_count, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -389,6 +404,21 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream) {
   h_out[2] = c[CTR_GRAD_MISS];
   h_out[3] = c[CTR_FULL];
   h_out[4] = c[CTR_ERR];
+  return PB_OK;
+}
+
+int pb_table_index_stats(pb_table* t, uint64_t h_out[3], void* stream) {
+  if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
+  h_out[0] = h_out[1] = h_out[2] = 0;
+  if (!t->allocated) return PB_OK;
+  DeviceGuard g(t->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (!t->stats_ws) PB_CUDA(cudaMalloc(&t->stats_ws, 3 * sizeof(uint32_t)));
+  launch_index_stats(t->d, t->stats_ws, st);
+  uint32_t c[3];
+  PB_CUDA(cudaMemcpyAsync(c, t->stats_ws, sizeof(c), cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  for (int i = 0; i < 3; ++i) h_out[i] = c[i];
   return PB_OK;
 }
 
@@ -1188,6 +1218,7 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   SlotsDev sl;
   if ((rc = make_slots(c->slots, occ_off, sl))) return rc;
   sl.uniform = 0;
+  drop_raw_pending(c);  // the numbering below replaces the pending batch's
   if (training) {
     if ((rc = maybe_evict(t, st))) return rc;
     launch_begin_batch(t->d, c->dev_tick, nullptr, st);
@@ -1208,6 +1239,8 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
     c->n_occ = n_occ;
     c->batch = batch;
     c->raw_pending = true;
+    c->raw_table = t;
+    t->pending_batches++;
   }
   PB_CUDA(cudaGetLastError());
   return PB_OK;
@@ -1217,12 +1250,13 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
                     void* stream) {
   if (!t || !c) return fail(PB_ERR_INVALID, "null argument");
   if (!c->raw_pending) return fail(PB_ERR_STATE, "no raw forward batch is pending in this context (backward_ref_id not found)");
+  if (c->raw_table != t) return fail(PB_ERR_INVALID, "the pending raw batch was looked up in another table");
   if (d_grad && misaligned(d_grad)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
   int rc = ready_for_training(t);
   if (rc) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
-  c->raw_pending = false;
+  drop_raw_pending(c);  // enqueued below: the sweep of the next training call runs after these gradients
   GradsDev gr;
   std::memset(&gr, 0, sizeof(gr));
   gr.ptr[0] = d_grad;
@@ -1251,8 +1285,8 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
   // The pending training forward allocated the buffer for this table's dim; only another table's larger dim allocates.
   if ((rc = ensure_raw_stage(c, dim, st))) return rc;
   launch_raw_stage(d_grad, is_f16 != 0, c->raw.counts, dim, inv, do_scale, c->raw_stage, st);
-  launch_update_direct(t->d, t->op, t->hy, c->raw.distinct_cell, c->raw_stage, c->n_occ, pair, st, c->raw.counts,
-                       c->dev_tick, c->nan_tick);
+  launch_update_direct(t->d, t->op, t->hy, c->raw.target, c->raw_stage, c->n_occ, pair, st, c->raw.counts,
+                       c->dev_tick, c->nan_tick, true);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }

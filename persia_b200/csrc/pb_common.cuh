@@ -88,6 +88,7 @@ enum {
   CTR_ADMIT = 6,     // rows admitted
   CTR_EVICT = 7,     // rows evicted
   CTR_ERR = 8,       // an in-kernel wait gave up (mbarrier / peer flag): results of that batch are void
+  CTR_USED = 9,      // normal index cells that are not EMPTY (live or tombstone): the index is rebuilt before it fills
   CTR_COUNT = 16
 };
 

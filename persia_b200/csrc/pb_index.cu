@@ -221,7 +221,7 @@ __global__ void __launch_bounds__(256) k_evict_sweep_spill(TableDev t, uint32_t*
     if (age < thr) continue;
     const uint32_t at = atomicAdd(count, 1u);
     if (at >= max_n) continue;  // no room to write it out: it stays resident (count tells the caller)
-    signs[at] = (i < t.n_cells) ? c.key : KEY_EMPTY;  // (the reserved cell holds the sign KEY_EMPTY)
+    signs[at] = (i < t.n_cells) ? c.key : KEY_EMPTY - (i - t.n_cells);  // the three marker-valued signs
     const float* row = t.rows + (size_t)c.row * t.stride;
     for (uint32_t e = 0; e < entry_len; ++e) entries[(size_t)at * entry_len + e] = row[e];
     t.cells[i].key = (i < t.n_cells) ? KEY_TOMB : KEY_EMPTY;
@@ -234,8 +234,103 @@ __global__ void __launch_bounds__(256) k_evict_sweep_spill(TableDev t, uint32_t*
 }
 
 // ------------------------------------------------------------------------------------------------
+// Index rebuild (pb_probe.cuh): EMPTY cells only get fewer between rebuilds, so after every eviction check, swept or
+// not, the index is rebuilt once more than 7/8 of its normal cells are used (CTR_USED).  Every step is gated on the
+// flag the plan sets (no host sync; a captured step stays capturable).  The live (sign, row) pairs of the normal cells
+// are compacted into a buffer of `capacity` entries, the normal cells refilled with EMPTY and every pair re-inserted
+// at the first EMPTY cell of its probe sequence; the reserved cells stay as they are.  Rows and row_tick do not move,
+// so rows held by pending batches stay valid.  After a rebuild at most capacity <= 2/3 n_cells cells are used.
+// ev[EV_RB] = rebuild flag, ev[EV_RB + 1] = pairs compacted.
+// ------------------------------------------------------------------------------------------------
+constexpr uint32_t EV_RB = 3 + EV_BINS;
+static_assert(EV_RB + 2 <= EVICT_WS_WORDS, "eviction workspace too small");
+
+__global__ void k_rebuild_plan(TableDev t, uint32_t* __restrict__ ev) {
+  if (threadIdx.x) return;
+  ev[EV_RB] = t.counters[CTR_USED] > t.n_cells - t.n_cells / 8 ? 1u : 0u;
+  ev[EV_RB + 1] = 0u;
+}
+
+__global__ void __launch_bounds__(256) k_rebuild_compact(TableDev t, uint32_t* __restrict__ ev, uint64_t* __restrict__ keys,
+                                                         uint32_t* __restrict__ rows) {
+  if (!ev[EV_RB]) return;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < t.n_cells; i += gridDim.x * blockDim.x) {
+    const Cell c = t.cells[i];
+    if (c.key >= KEY_TOMB || c.row >= t.capacity) continue;
+    const uint32_t at = atomicAdd(&ev[EV_RB + 1], 1u);
+    if (at < t.capacity) {  // (always: every live cell holds a row of its own)
+      keys[at] = c.key;
+      rows[at] = c.row;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) k_rebuild_clear(TableDev t, const uint32_t* __restrict__ ev) {
+  if (!ev[EV_RB]) return;
+  Cell e;
+  e.key = KEY_EMPTY;
+  e.row = ROW_PENDING;
+  e.aux = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < t.n_cells; i += gridDim.x * blockDim.x) t.cells[i] = e;
+}
+
+// keys are distinct and no cell is a tombstone: a CAS on EMPTY is all an insertion needs
+__global__ void __launch_bounds__(256) k_rebuild_insert(TableDev t, const uint32_t* __restrict__ ev,
+                                                        const uint64_t* __restrict__ keys, const uint32_t* __restrict__ rows) {
+  if (!ev[EV_RB]) return;
+  const uint32_t n = min(ev[EV_RB + 1], t.capacity);
+  if (blockIdx.x == 0 && threadIdx.x == 0) t.counters[CTR_USED] = n;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const unsigned long long key = keys[i];
+    uint32_t bucket = (uint32_t)mix64(key) & t.bucket_mask;
+    for (bool done = false; !done; bucket = (bucket + 1) & t.bucket_mask) {  // n < n_cells: an EMPTY cell exists
+      for (uint32_t s = 0; s < BUCKET && !done; ++s) {
+        Cell* c = t.cells + (size_t)bucket * BUCKET + s;
+        if (c->key == KEY_EMPTY && atomicCAS(&c->key, KEY_EMPTY, key) == KEY_EMPTY) {
+          c->row = rows[i];
+          done = true;
+        }
+      }
+    }
+  }
+}
+
+// diagnostic (pb_table_index_stats): live, tombstone and EMPTY cells among the n_cells normal cells
+__global__ void __launch_bounds__(256) k_index_stats(TableDev t, uint32_t* __restrict__ out) {
+  uint32_t live = 0, tomb = 0, empty = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < t.n_cells; i += gridDim.x * blockDim.x) {
+    const Cell c = t.cells[i];
+    if (c.key == KEY_EMPTY) ++empty;
+    else if (c.key == KEY_TOMB) ++tomb;
+    else if (c.row < t.capacity) ++live;
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    live += __shfl_down_sync(0xffffffffu, live, o);
+    tomb += __shfl_down_sync(0xffffffffu, tomb, o);
+    empty += __shfl_down_sync(0xffffffffu, empty, o);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    atomicAdd(&out[0], live);
+    atomicAdd(&out[1], tomb);
+    atomicAdd(&out[2], empty);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // launchers (host)
 // ------------------------------------------------------------------------------------------------
+static void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st) {
+  PB_LAUNCH(k_rebuild_plan, 1, 32, 0, st, t, ev);
+  PB_LAUNCH(k_rebuild_compact, PB_NUM_SMS * 8, 256, 0, st, t, ev, keys, rows);
+  PB_LAUNCH(k_rebuild_clear, PB_NUM_SMS * 8, 256, 0, st, t, ev);
+  PB_LAUNCH(k_rebuild_insert, PB_NUM_SMS * 8, 256, 0, st, t, ev, keys, rows);
+}
+
+void launch_index_stats(const TableDev& t, uint32_t* out, cudaStream_t st) {
+  cudaMemsetAsync(out, 0, 3 * sizeof(uint32_t), st);
+  PB_LAUNCH(k_index_stats, PB_NUM_SMS * 8, 256, 0, st, t, out);
+}
+
 void launch_fill_cells(Cell* cells, uint64_t n, cudaStream_t st) { PB_LAUNCH(k_fill_cells, PB_NUM_SMS * 8, 256, 0, st, cells, n); }
 
 void launch_begin_batch(const TableDev& t, uint32_t* ctx_tick, uint32_t* batch_cnt, cudaStream_t st, bool bump) {
@@ -313,19 +408,22 @@ void launch_export_signs(const TableDev& t, uint64_t* signs, uint32_t* recency, 
   PB_LAUNCH(k_export_signs, PB_NUM_SMS * 8, 256, 0, st, t, signs, recency, max_n, count);
 }
 
-void launch_spill(const TableDev& t, uint32_t want_free, uint32_t keep, uint32_t* ev, uint64_t* signs, float* entries,
-                  uint32_t max_n, uint32_t* count, cudaStream_t st) {
+void launch_spill(const TableDev& t, uint32_t want_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys, uint32_t* rb_rows,
+                  uint64_t* signs, float* entries, uint32_t max_n, uint32_t* count, cudaStream_t st) {
   PB_LAUNCH(k_evict_plan, 1, 256, 0, st, t, want_free, want_free, ev);
   PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, t, ev);
   PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
   PB_LAUNCH(k_evict_sweep_spill, PB_NUM_SMS * 8, 256, 0, st, t, ev, signs, entries, max_n, count);
+  launch_rebuild(t, ev, rb_keys, rb_rows, st);
 }
 
-void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, cudaStream_t st) {
+void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys,
+                  uint32_t* rb_rows, cudaStream_t st) {
   PB_LAUNCH(k_evict_plan, 1, 256, 0, st, t, low_water, target_free, ev);
   PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, t, ev);
   PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
   PB_LAUNCH(k_evict_sweep, PB_NUM_SMS * 8, 256, 0, st, t, ev);
+  launch_rebuild(t, ev, rb_keys, rb_rows, st);
 }
 
 void launch_shard_of(const uint64_t* signs, uint32_t n, uint32_t R, uint32_t* shard, uint64_t* hash, cudaStream_t st) {

@@ -143,7 +143,8 @@ struct RawWork {
   uint32_t* tiles;          // scan spine
   uint32_t* distinct_cell;  // index cell of every distinct sign (forward -> backward); sharded: its scratch-set cell
   uint32_t* counts;         // [0] distinct signs, [1] ids placed in `index`
-  // sharded path (pb_forward_raw_sharded): where every distinct sign went, owner * cap + slot (ROW_NONE: over cap)
+  // sharded path (pb_forward_raw_sharded): where every distinct sign went, owner * cap + slot (ROW_NONE: over cap);
+  // local path (pb_forward_raw): the table row of every distinct sign (ROW_NONE: no storage), forward -> backward
   uint32_t* target;         // [n]
   uint32_t* peer;           // [PB_MAX_RANKS] distinct signs routed to each owner
 };
@@ -189,11 +190,12 @@ void launch_uclear(const XchgDev& x, cudaStream_t st);
 void launch_owner_update_all(const TableDev& t, const OptimDev& op, const HyperDev& hy, const XchgDev& x, cudaStream_t st);
 void launch_owner_update(const TableDev& t, const OptimDev& op, const HyperDev& hy, const XchgDev& x, uint32_t src,
                          cudaStream_t st);
-// n_ptr (optional): the live count on the device (<= n); tick/nan_tick (optional): skip everything when equal
-void launch_update_direct(const TableDev& t, const OptimDev& op, const HyperDev& hy, const uint32_t* occ_cell,
+// n_ptr (optional): the live count on the device (<= n); tick/nan_tick (optional): skip everything when equal;
+// by_row: `where` holds table rows (ROW_NONE: no storage) rather than index cells
+void launch_update_direct(const TableDev& t, const OptimDev& op, const HyperDev& hy, const uint32_t* where,
                           const float* grads, uint32_t n, const float* adam_pair, cudaStream_t st,
                           const uint32_t* n_ptr = nullptr, const uint32_t* tick = nullptr,
-                          const uint32_t* nan_tick = nullptr);
+                          const uint32_t* nan_tick = nullptr, bool by_row = false);
 struct AdamKeys {
   uint8_t idx[PB_MAX_SLOTS];
   uint32_t n;
@@ -234,9 +236,14 @@ void launch_add_prefix(const SlotsDev& sl, const uint64_t* ids, uint32_t n, uint
 void launch_shard_of(const uint64_t* signs, uint32_t n, uint32_t R, uint32_t* shard, uint64_t* hash, cudaStream_t st);
 void launch_export_signs(const TableDev& t, uint64_t* signs, uint32_t* recency, uint32_t max_n, uint32_t* count,
                          cudaStream_t st);
-void launch_spill(const TableDev& t, uint32_t want_free, uint32_t keep, uint32_t* ev, uint64_t* signs, float* entries,
-                  uint32_t max_n, uint32_t* count, cudaStream_t st);
-void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, cudaStream_t st);
+// capacity sweeps (pb_index.cu): ev = EVICT_WS_WORDS words; rb_keys / rb_rows = `capacity` entries each, where the index
+// rebuild that follows every sweep check compacts the live pairs
+constexpr uint32_t EVICT_WS_WORDS = 3 + 1024 + 2;
+void launch_spill(const TableDev& t, uint32_t want_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys, uint32_t* rb_rows,
+                  uint64_t* signs, float* entries, uint32_t max_n, uint32_t* count, cudaStream_t st);
+void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys,
+                  uint32_t* rb_rows, cudaStream_t st);
+void launch_index_stats(const TableDev& t, uint32_t* out, cudaStream_t st);
 uint64_t launch_count();
 enum { FAM_PROBE = 0, FAM_DEDUP, FAM_GATHER, FAM_NAN, FAM_HOT, FAM_UPDATE, FAM_OTHER, FAM_WARM, FAM_WAIT, FAM_ROUTE, FAM_OWNER, FAM_COUNT };
 bool profiling();  // a kernel family is being timed: the backward then runs its kernels one after another

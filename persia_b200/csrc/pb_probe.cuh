@@ -61,11 +61,15 @@ static __device__ __noinline__ void init_row(const TableDev& t, const HyperDev& 
 // Returns, to every lane of the group, the index cell (n_cells + N_SPECIAL = the sign has no storage) and the row
 // (ROW_NONE likewise).
 // Invariant that makes "an empty cell in the bucket => the sign is absent" true: a sign is stored no later
-// in its probe sequence than the first bucket that had an EMPTY cell when it was admitted, and a cell never
-// returns to EMPTY: eviction leaves a tombstone, which lookups walk past and admissions reuse (after having
-// seen an EMPTY cell further on, i.e. knowing the sign is absent).  A sign admitted when the shard is out of row
-// storage is rolled back to a tombstone (the reference would have evicted its LRU entry; here the sweep between
+// in its probe sequence than the first bucket that had an EMPTY cell when it was admitted, and between rebuilds
+// a cell never returns to EMPTY: eviction leaves a tombstone, which lookups walk past and admissions reuse (after
+// having seen an EMPTY cell further on, i.e. knowing the sign is absent).  A sign admitted when the shard is out of
+// row storage is rolled back to a tombstone (the reference would have evicted its LRU entry; here the sweep between
 // batches does), so it can be admitted again later.
+// So EMPTY cells only ever get fewer: an admission whose probe path holds no tombstone uses one up, and under
+// eviction churn they would run out (every admission then fails, every miss walks the whole index).  CTR_USED counts
+// the normal cells that are not EMPTY; every eviction check rebuilds the index when it passes 7/8 of them
+// (pb_index.cu, k_rebuild_*): live signs are re-inserted into an index of EMPTY cells, tombstones are dropped.
 // ------------------------------------------------------------------------------------------------
 struct ProbeOut {
   uint32_t cell, row;
@@ -113,6 +117,7 @@ __device__ __forceinline__ ProbeOut probe_group(const TableDev& t, const HyperDe
     const bool won_cas = try_ins && old == (use_tomb ? KEY_TOMB : KEY_EMPTY);  // lane `le` of this group admitted the sign
     uint32_t row = 0;
     if (won_cas && sub == le) {
+      if (!use_tomb && !special) atomicAdd(&t.counters[CTR_USED], 1u);  // an EMPTY cell is used up (rollback leaves a tombstone)
       // storage: a row released by eviction if there is one, else the next never-used row
       uint32_t f = atomicSub(&t.counters[CTR_FREE], 1u);
       if (f > 0 && f <= t.capacity) {

@@ -182,10 +182,13 @@ __global__ void __launch_bounds__(256) k_raw_non_empty(const uint32_t* __restric
   for (uint32_t j = 0; j < m; ++j) non_empty[o + j] = (long long)b * fixed + j;
 }
 
-// table row d + 1 = f16(embedding of distinct sign d); zeros when the sign has no storage (lookup miss)
+// table row d + 1 = f16(embedding of distinct sign d); zeros when the sign has no storage (lookup miss).  The row
+// itself goes to distinct_row[d] for the backward: a cell may move (index rebuild) before the gradients come, a row
+// held by a pending batch does not
 template <int VEC, int G>
 __global__ void __launch_bounds__(256) k_raw_table(TableDev t, const uint32_t* __restrict__ distinct_cell,
-                                                   const uint32_t* __restrict__ n_distinct, __half* __restrict__ out) {
+                                                   const uint32_t* __restrict__ n_distinct, __half* __restrict__ out,
+                                                   uint32_t* __restrict__ distinct_row) {
   const uint32_t d = (blockIdx.x * 256 + threadIdx.x) / G;
   const uint32_t lane = threadIdx.x % G;
   if (d == 0 && blockIdx.x == 0)  // row 0: padding target of index == 0
@@ -193,6 +196,7 @@ __global__ void __launch_bounds__(256) k_raw_table(TableDev t, const uint32_t* _
   if (d >= *n_distinct) return;
   const uint32_t h = distinct_cell[d];
   const uint32_t row = (h < t.n_cells + N_SPECIAL) ? t.cells[h].row : ROW_NONE;
+  if (lane == 0) distinct_row[d] = row < t.capacity ? row : ROW_NONE;
   __half* o = out + (size_t)(d + 1) * t.dim;
   const float* prow = t.rows + (size_t)(row < t.capacity ? row : 0) * t.stride;
   for (uint32_t c = lane; c < t.dim / VEC; c += G) {
@@ -286,7 +290,7 @@ void launch_raw_forward(const TableDev& t, const SlotsDev& sl, const uint64_t* i
   vec_group(t.dim, vec, G);
   const uint32_t grid = cdiv((uint64_t)(n ? n : 1) * G, 256);
 #define PB_T(V, GG) \
-  if (vec == V && G == GG) PB_LAUNCH((k_raw_table<V, GG>), grid, 256, 0, st, t, w.distinct_cell, w.counts, (__half*)table_f16);
+  if (vec == V && G == GG) PB_LAUNCH((k_raw_table<V, GG>), grid, 256, 0, st, t, w.distinct_cell, w.counts, (__half*)table_f16, w.target);
   PB_T(4, 1) PB_T(4, 2) PB_T(4, 4) PB_T(4, 8) PB_T(4, 16) PB_T(4, 32)
   PB_T(1, 1) PB_T(1, 2) PB_T(1, 4) PB_T(1, 8) PB_T(1, 16) PB_T(1, 32)
 #undef PB_T

@@ -47,9 +47,10 @@ __global__ void k_slot_status(GradsDev gr, uint32_t n_slots, const uint32_t* __r
   if (s < n_slots) status[s] = !gr.ptr[s] ? 1 : (nan_tick[s] == tick ? 2 : 0);
 }
 
-// pb_update: distinct signs with explicit f32 gradients (update_gradient_mixed, PS mod.rs:359-427).
+// pb_update: distinct signs with explicit f32 gradients (update_gradient_mixed, PS mod.rs:359-427); the raw backward
+// (by_row: the rows its forward found).
 template <int VEC, int G>
-__global__ void __launch_bounds__(256) k_update_direct(TableDev t, OptimDev op, HyperDev hy,
+__global__ void __launch_bounds__(256) k_update_direct(TableDev t, OptimDev op, HyperDev hy, int by_row,
                                                        const uint32_t* __restrict__ occ_cell,
                                                        const float* __restrict__ grads, uint32_t n,
                                                        const float* __restrict__ adam_pair,
@@ -62,7 +63,7 @@ __global__ void __launch_bounds__(256) k_update_direct(TableDev t, OptimDev op, 
   if (gid >= n) return;
   if (nan_tick && nan_tick[0] == *tick_ptr) return;  // NaN rule: the whole gradient is dropped
   uint32_t h = occ_cell[gid];
-  uint32_t row = (h < t.n_cells + N_SPECIAL) ? t.cells[h].row : ROW_NONE;
+  uint32_t row = by_row ? h : (h < t.n_cells + N_SPECIAL) ? t.cells[h].row : ROW_NONE;
   if (row >= t.capacity) {
     if (lane == 0) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);
     return;
@@ -144,17 +145,17 @@ void launch_slot_status(const GradsDev& gr, uint32_t n_slots, const uint32_t* ti
   PB_LAUNCH(k_slot_status, 1, PB_MAX_SLOTS, 0, st, gr, n_slots, tick, nan_tick, status);
 }
 
-void launch_update_direct(const TableDev& t, const OptimDev& op, const HyperDev& hy, const uint32_t* occ_cell,
+void launch_update_direct(const TableDev& t, const OptimDev& op, const HyperDev& hy, const uint32_t* where,
                           const float* grads, uint32_t n, const float* adam_pair, cudaStream_t st,
-                          const uint32_t* n_ptr, const uint32_t* tick, const uint32_t* nan_tick) {
+                          const uint32_t* n_ptr, const uint32_t* tick, const uint32_t* nan_tick, bool by_row) {
   if (!n) return;
   int vec, G;
   vec_group(t.dim, vec, G);
   uint32_t grid = cdiv((uint64_t)n * G, 256);
 #define PB_U(V, GG)                                                                                          \
   if (vec == V && G == GG)                                                                                   \
-    PB_LAUNCH_F(FAM_UPDATE, (k_update_direct<V, GG>), grid, 256, 0, st, t, op, hy, occ_cell, grads, n, adam_pair, n_ptr, \
-                tick, nan_tick);
+    PB_LAUNCH_F(FAM_UPDATE, (k_update_direct<V, GG>), grid, 256, 0, st, t, op, hy, by_row ? 1 : 0, where, grads, n,  \
+                adam_pair, n_ptr, tick, nan_tick);
   PB_U(4, 1) PB_U(4, 2) PB_U(4, 4) PB_U(4, 8) PB_U(4, 16) PB_U(4, 32)
   PB_U(1, 1) PB_U(1, 2) PB_U(1, 4) PB_U(1, 8) PB_U(1, 16) PB_U(1, 32)
 #undef PB_U

@@ -58,6 +58,7 @@ SYMBOLS = {
     "pb_table_set_eviction": (_i32, [_vp, _u32, _u64, _u64, _u32]),
     "pb_table_spill": (_i32, [_vp, _u64, _u32, _vp, _vp, _u32, _vp, _vp]),
     "pb_table_counters": (_i32, [_vp, C.POINTER(_u64 * 5), _vp]),
+    "pb_table_index_stats": (_i32, [_vp, C.POINTER(_u64 * 3), _vp]),
     "pb_lookup": (_i32, [_vp, _vp, _u32, _i32, _vp, _vp]),
     "pb_update": (_i32, [_vp, _vp, _vp, _u32, _vp]),
     "pb_set_rows": (_i32, [_vp, _vp, _vp, _u32, _vp]),

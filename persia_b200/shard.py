@@ -86,6 +86,12 @@ class EmbeddingShard:
         return {"admitted": out[0], "lookup_miss": out[1], "gradient_id_miss": out[2], "capacity_refused": out[3],
                 "wait_errors": out[4]}
 
+    def index_stats(self):
+        """Cells of the hash index (host sync): live signs, tombstones of evicted signs, and EMPTY cells."""
+        out = (C.c_uint64 * 3)()
+        N.check(self.lib.pb_table_index_stats(self.h, C.byref(out), _stream(self.device)))
+        return {"live": out[0], "tomb": out[1], "empty": out[2]}
+
     def __len__(self):
         return int(self.counters()["admitted"])
 
