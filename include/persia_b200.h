@@ -100,6 +100,42 @@ int pb_table_spill(pb_table* t, uint64_t want_free, uint32_t keep_batches, uint6
  * refused because the shard is full, [4] in-kernel waits that gave up (must stay 0: a non-zero value voids the batch
  * that raised it).  Synchronises `stream`. */
 int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream);
+/* ---- host-memory tier: a table larger than HBM on one GPU ----------------------------------------------------------
+ * The reference's parameter server keeps every entry in host DRAM, bounded by `capacity`.  A tier is a second table
+ * whose rows (embedding ++ optimizer state) live in mapped pinned host memory (cudaHostAllocMapped | Portable, not
+ * write-combined); its index cells, row recency, free-row stack and counters live in HBM like any table's.  So HBM
+ * bounds the tier too, at 44-68 B of HBM per host row: 16 B index cells, n_cells = next_pow2(1.5 x rows) (24-48 B per
+ * row), plus row recency 4, free-row stack 4 and the rebuild's pairs 12.  That is about 1.2e8-1.8e8 host rows per 8 GB.
+ * (The HBM table itself adds 4 B per HBM row for the move's victim list.)
+ *
+ * Attached behind an HBM table (same dim and optimizer kind: one entry layout), the tier is never trained directly; the
+ * kernels only move or read whole entries, stream-ordered, without host synchronisation (a step stays capturable in a
+ * CUDA graph):
+ *   - out: every eviction check of the HBM table (pb_table_set_eviction) moves its victims into the tier instead of
+ *     dropping them.  The tier first drops its own oldest entries until it can hold them (counted as dropped: the
+ *     reference's LRU bound on the whole table), then each victim is written to a tier row and published there before
+ *     its HBM cell is released.  Rows of pending batches (raw ones included) are never victims.
+ *   - restore: training requests — pb_forward (over the batch's distinct signs), pb_forward_raw, pb_lookup — and
+ *     pb_set_rows first move every tier-held sign of the request back into a free HBM row (a pending batch holds HBM rows).
+ *   - in place: inference requests (training == 0) of pb_forward, pb_forward_raw and pb_lookup read tier-held signs where
+ *     they are and move nothing, so an inference pass of any size returns every value; pb_update steps a tier-held row
+ *     where it is; pb_get_rows reads the tier in place; pb_set_rows stores the entries the HBM table has no row for in
+ *     the tier (entries neither table has a row for are counted as dropped).
+ * Invariants: a sign lives in at most one of the two tables.  A tier-held sign is never re-initialised: if a training
+ * request finds no free HBM row for it (e.g. pending batches protect every row) its restore is refused and counted, it
+ * reads as zeros and its gradient counts as a gradient miss (as an admission refused for capacity does), and its tier
+ * entry stays as it was.  A moved entry keeps its recency, and the tier ages rows by the HBM table's training-request
+ * number: the union evicts least recently used first, and pb_table_export_signs of both tables merges into the
+ * reference's list order.
+ * pb_table_clear of the table clears its tier too.  Destroy the table before its tier.  The sharded calls and
+ * pb_table_spill refuse a table with a tier. */
+int pb_table_create_host(int device, const pb_table_cfg* cfg, pb_table** out);
+/* Both tables need their optimizer registered; checks dim, optimizer kind and row stride. */
+int pb_table_attach_tier(pb_table* t, pb_table* tier);
+/* The tier behind `t` (zeros without one): [0] entries it holds, [1] entries moved out of HBM into it, [2] entries
+ * restored into HBM, [3] entries dropped: by its own sweep, or because neither table had a row for them (an eviction
+ * victim or a pb_set_rows entry), [4] training restores refused for want of a free HBM row.  Synchronises `stream`. */
+int pb_tier_stats(pb_table* t, uint64_t h_out[5], void* stream);
 /* Diagnostic: the state of the hash index's n_cells normal cells (the three cells reserved for the marker-valued signs
  * are not counted): [0] live (a resident sign), [1] tombstones (an evicted sign), [2] EMPTY.  An admission needs an
  * EMPTY cell on its probe path; every eviction check rebuilds the index (tombstones dropped) once fewer than 1/8 of the

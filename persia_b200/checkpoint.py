@@ -237,6 +237,10 @@ def load_shards(src_dir, shards_by_dim, replica_index=0, replica_size=1, chunk=1
                 if lens != {sh.entry_len}:
                     raise RuntimeError(f"dim-{int(dim)} entries of {sorted(lens)} floats, the registered optimizer needs "
                                        f"{sh.entry_len} (embedding ++ state)")
+                if getattr(sh, "host_tier", None) is not None:
+                    # HBM rows + a host tier: the newest entries take the HBM rows, the oldest overflow to the tier (the
+                    # reference's LRU map, filled in list order beyond its capacity, would keep the newest)
+                    pick = pick[::-1]
                 for lo in range(0, pick.size, chunk):
                     sel = pick[lo:lo + chunk]
                     ent = torch.from_numpy(np.stack([entries[i] for i in sel])).to(sh.device)

@@ -88,6 +88,13 @@ struct pb_table {
   uint32_t* rebuild_rows = nullptr;
   uint32_t* stats_ws = nullptr;      // pb_table_index_stats
   uint32_t pending_batches = 0;  // training forwards whose backward has not been enqueued yet
+  // host-memory tier (pb_tier.cu): `host` = this table's rows are mapped pinned host memory (pb_table_create_host);
+  // `tier` = the host table attached behind this one, `tier_of` = the table this one is attached behind
+  bool host = false;
+  float* host_rows = nullptr;  // host address of d.rows (cudaFreeHost)
+  pb_table* tier = nullptr;
+  pb_table* tier_of = nullptr;
+  uint32_t* move_cells = nullptr;  // the eviction check's victim list (with rebuild_keys / rebuild_rows), `capacity` words
 };
 
 struct pb_ctx {
@@ -154,7 +161,13 @@ int ensure_alloc(pb_table* t) {
   d.cell_mask = d.n_cells - 1;
   d.bucket_mask = d.n_cells / BUCKET - 1;
   PB_CUDA(cudaMalloc(&d.cells, sizeof(Cell) * ((size_t)d.n_cells + N_SPECIAL)));
-  PB_CUDA(cudaMalloc(&d.rows, sizeof(float) * (size_t)d.capacity * d.stride));
+  if (t->host) {  // not write-combined: the host reads these rows back (checkpoints)
+    PB_CUDA(cudaHostAlloc((void**)&t->host_rows, sizeof(float) * (size_t)d.capacity * d.stride,
+                          cudaHostAllocMapped | cudaHostAllocPortable));
+    PB_CUDA(cudaHostGetDevicePointer((void**)&d.rows, t->host_rows, 0));
+  } else {
+    PB_CUDA(cudaMalloc(&d.rows, sizeof(float) * (size_t)d.capacity * d.stride));
+  }
   PB_CUDA(cudaMalloc(&d.counters, sizeof(uint32_t) * CTR_COUNT));
   PB_CUDA(cudaMalloc(&d.row_tick, sizeof(uint32_t) * (size_t)d.capacity));
   PB_CUDA(cudaMemset(d.row_tick, 0, sizeof(uint32_t) * (size_t)d.capacity));
@@ -197,11 +210,23 @@ int maybe_evict(pb_table* t, cudaStream_t st) {
   // rows of batches whose gradients are still to come are never released: a row used by a pending batch was
   // refreshed by its forward, i.e. at most `pending_batches` requests ago
   const uint32_t keep = t->evict_keep > t->pending_batches + 1 ? t->evict_keep : t->pending_batches + 1;
+  if (t->tier) {  // the victims move into the tier
+    pb_table* h = t->tier;
+    launch_evict_tier(t->d, h->d, t->hy, t->op, t->evict_low, t->evict_target, keep, t->evict_ws, t->rebuild_keys,
+                      t->rebuild_rows, h->evict_ws, h->rebuild_keys, h->rebuild_rows, t->move_cells, st);
+    return PB_OK;
+  }
   launch_evict(t->d, t->evict_low, t->evict_target, keep, t->evict_ws, t->rebuild_keys, t->rebuild_rows, st);
   return PB_OK;
 }
 
+// signs the HBM table lacks and its tier holds are moved back into HBM rows before they are probed
+void restore_ids(pb_table* t, bool prefix, const SlotsDev& sl, const uint64_t* ids, uint32_t n, cudaStream_t st) {
+  if (t->tier) launch_tier_restore(t->d, t->tier->d, t->hy, t->op, sl, prefix, ids, n, st);
+}
+
 int ready_for_training(pb_table* t) {
+  if (t->tier_of) return fail(PB_ERR_STATE, "a host tier is not trained directly: use the table it is attached to");
   if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered (OptimizerNotFoundError)");
   if (!t->has_hy) return fail(PB_ERR_STATE, "embedding server not configured (NotConfiguredError)");
   return PB_OK;
@@ -300,13 +325,59 @@ int pb_table_create(int device, const pb_table_cfg* cfg, pb_table** out) {
   return PB_OK;
 }
 
+int pb_table_create_host(int device, const pb_table_cfg* cfg, pb_table** out) {
+  int rc = pb_table_create(device, cfg, out);
+  if (rc) return rc;
+  (*out)->host = true;
+  return PB_OK;
+}
+
+int pb_table_attach_tier(pb_table* t, pb_table* tier) {
+  if (!t || !tier) return fail(PB_ERR_INVALID, "null argument");
+  if (t->host || !tier->host) return fail(PB_ERR_INVALID, "the tier must be a host table (pb_table_create_host) behind an HBM table");
+  if (t->tier || t->tier_of || tier->tier_of || tier->tier) return fail(PB_ERR_STATE, "one of the tables already has a tier or is one");
+  if (t->device != tier->device) return fail(PB_ERR_INVALID, "the tables live on different devices");
+  if (!t->has_op || !tier->has_op) return fail(PB_ERR_STATE, "register the optimizer of both tables before attaching the tier");
+  if (t->cfg.dim != tier->cfg.dim || t->op.kind != tier->op.kind)
+    return fail(PB_ERR_INVALID, "the tier must have the table's dim and optimizer (one entry layout)");
+  DeviceGuard g(t->device);
+  int rc;
+  if ((rc = ensure_alloc(t)) || (rc = ensure_alloc(tier))) return rc;
+  if (t->d.stride != tier->d.stride) return fail(PB_ERR_INVALID, "the tier's row stride differs from the table's");
+  if ((rc = ensure_evict_ws(t)) || (rc = ensure_evict_ws(tier))) return rc;
+  PB_CUDA(cudaMalloc(&t->move_cells, sizeof(uint32_t) * (size_t)t->d.capacity));
+  t->tier = tier;
+  tier->tier_of = t;
+  return PB_OK;
+}
+
+int pb_tier_stats(pb_table* t, uint64_t h_out[5], void* stream) {
+  if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
+  for (int i = 0; i < 5; ++i) h_out[i] = 0;
+  if (!t->tier) return PB_OK;
+  DeviceGuard g(t->device);
+  uint32_t c[CTR_COUNT];
+  PB_CUDA(cudaMemcpyAsync(c, t->tier->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  h_out[0] = c[CTR_ADMIT] - c[CTR_EVICT] - c[CTR_TIER_IN];
+  h_out[1] = c[CTR_TIER_OUT];
+  h_out[2] = c[CTR_TIER_IN];
+  h_out[3] = (uint64_t)c[CTR_EVICT] + c[CTR_TIER_LOST];
+  h_out[4] = c[CTR_TIER_REFUSED];
+  return PB_OK;
+}
+
 int pb_table_destroy(pb_table* t) {
   if (!t) return PB_OK;
   DeviceGuard g(t->device);
+  if (t->tier) t->tier->tier_of = nullptr;
+  if (t->tier_of) t->tier_of->tier = nullptr;
+  if (t->move_cells) cudaFree(t->move_cells);
   if (t->allocated) {
     cudaDeviceSynchronize();
     cudaFree(t->d.cells);
-    cudaFree(t->d.rows);
+    if (t->host) cudaFreeHost(t->host_rows);
+    else cudaFree(t->d.rows);
     cudaFree(t->d.counters);
     cudaFree(t->d.row_tick);
     if (t->d.free_rows) cudaFree(t->d.free_rows);
@@ -359,6 +430,7 @@ int pb_table_configure(pb_table* t, const pb_hyper_cfg* c) {
 int pb_table_spill(pb_table* t, uint64_t want_free, uint32_t keep_batches, uint64_t* d_signs, float* d_entries, uint32_t max_n,
                    uint32_t* d_count, void* stream) {
   if (!t || !d_count || (max_n && (!d_signs || !d_entries))) return fail(PB_ERR_INVALID, "null argument");
+  if (t->tier || t->tier_of) return fail(PB_ERR_STATE, "a table with a host tier (or a tier) moves its rows itself: no spill");
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   int rc = ensure_evict_ws(t);
@@ -399,7 +471,7 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream) {
   uint32_t c[CTR_COUNT];
   PB_CUDA(cudaMemcpyAsync(c, t->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
-  h_out[0] = c[CTR_ADMIT] - c[CTR_EVICT];  // resident rows
+  h_out[0] = c[CTR_ADMIT] - c[CTR_EVICT] - c[CTR_TIER_IN];  // resident rows (a tier's restored rows left it)
   h_out[1] = c[CTR_MISS];
   h_out[2] = c[CTR_GRAD_MISS];
   h_out[3] = c[CTR_FULL];
@@ -439,7 +511,7 @@ int pb_table_clear(pb_table* t, void* stream) {
   launch_fill_cells(t->d.cells, (uint64_t)t->d.n_cells + N_SPECIAL, st);
   PB_CUDA(cudaMemsetAsync(t->d.counters, 0, sizeof(uint32_t) * CTR_COUNT, st));
   PB_CUDA(cudaMemsetAsync(t->d.row_tick, 0, sizeof(uint32_t) * (size_t)t->d.capacity, st));
-  return PB_OK;
+  return t->tier ? pb_table_clear(t->tier, stream) : PB_OK;
 }
 
 int pb_lookup(pb_table* t, const uint64_t* d_signs, uint32_t n, int training, float* d_out, void* stream) {
@@ -461,11 +533,14 @@ int pb_lookup(pb_table* t, const uint64_t* d_signs, uint32_t n, int training, fl
   if (training) {
     if ((rc = maybe_evict(t, st))) return rc;
     launch_begin_batch(t->d, nullptr, nullptr, st);
+    restore_ids(t, false, sl, d_signs, n, st);
     launch_probe(MODE_TRAIN, false, t->d, t->hy, t->op, sl, d_signs, n, t->scratch, st);
   } else {
     launch_probe(MODE_FIND, false, t->d, t->hy, t->op, sl, d_signs, n, t->scratch, st);
   }
   launch_gather(t->d, t->scratch, n, d_out, st);
+  if (!training && t->tier)  // inference moves nothing: a tier-held sign is read where it is
+    launch_tier_get(t->d, t->tier->d, d_signs, t->scratch, n, t->d.dim, d_out, nullptr, t->d.counters + CTR_MISS, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -481,6 +556,10 @@ int pb_update(pb_table* t, const uint64_t* d_signs, const float* d_grads, uint32
   if ((rc = ensure_scratch(t, n))) return rc;
   SlotsDev sl = no_slots();
   launch_probe(MODE_FIND, false, t->d, t->hy, t->op, sl, d_signs, n, t->scratch, st);
+  if (t->tier) {  // a tier-held sign's row is stepped where it is (no HBM row is needed)
+    if ((rc = ensure_scratch(t->tier, n))) return rc;
+    launch_tier_where(t->d, t->tier->d, d_signs, t->scratch, n, t->tier->scratch, st);
+  }
   const float* pair = nullptr;
   if (t->op.kind == PB_OPT_ADAM) {  // get_batch_level_state: one power step per request (optim.rs:155-197)
     AdamKeys k{};
@@ -490,6 +569,7 @@ int pb_update(pb_table* t, const uint64_t* d_signs, const float* d_grads, uint32
     pair = t->adam_dev + 2 * (PB_ADAM_KEYS - 1);
   }
   launch_update_direct(t->d, t->op, t->hy, t->scratch, d_grads, n, pair, st);
+  if (t->tier) launch_update_direct(t->tier->d, t->op, t->hy, t->tier->scratch, d_grads, n, pair, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -503,8 +583,12 @@ int pb_set_rows(pb_table* t, const uint64_t* d_signs, const float* d_entries, ui
   if (rc) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
   SlotsDev sl = no_slots();
+  // with a tier: a tier-held sign is first moved back (it then lives in one table), and an entry the HBM table has no
+  // row for goes to the tier
+  restore_ids(t, false, sl, d_signs, n, st);
   launch_probe(MODE_SET, false, t->d, t->hy, t->op, sl, d_signs, n, t->scratch, st);
   launch_copy_entries(true, t->d, t->scratch, n, const_cast<float*>(d_entries), nullptr, st);
+  if (t->tier) launch_tier_set(t->d, t->tier->d, t->hy, t->op, d_signs, t->scratch, n, d_entries, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -520,6 +604,8 @@ int pb_get_rows(pb_table* t, const uint64_t* d_signs, uint32_t n, float* d_entri
   SlotsDev sl = no_slots();
   launch_probe(MODE_FIND, false, t->d, t->hy, t->op, sl, d_signs, n, t->scratch, st);
   launch_copy_entries(false, t->d, t->scratch, n, d_entries, d_found, st);
+  if (t->tier)  // read in place
+    launch_tier_get(t->d, t->tier->d, d_signs, t->scratch, n, t->d.dim + t->d.state_floats, d_entries, d_found, nullptr, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -747,8 +833,16 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   launch_begin_batch(t->d, training ? c->dev_tick : nullptr, c->b.cnt, st, training != 0);
   c->b.n = n_occ;
   launch_dedup(sl, c->b, d_ids, st);
+  // a training batch moves its tier-held signs into HBM rows (each distinct sign once); inference reads them in place
+  if (t->tier && training) launch_tier_restore_items(t->d, t->tier->d, t->hy, t->op, c->b, st);
   launch_probe_items(training != 0, t->d, t->hy, t->op, sl, c->b, st);
-  launch_gather_items(t->d, sl, c->b, d_row_off, (uint32_t)n_out, batch, training != 0, d_out_f16, st);
+  if (t->tier && !training) {
+    launch_tier_find_items(t->d, t->tier->d, c->b, st);
+    launch_gather_items(t->d, sl, c->b, d_row_off, (uint32_t)n_out, batch, false, d_out_f16, st, t->tier->d.rows,
+                        t->tier->d.capacity);
+  } else {
+    launch_gather_items(t->d, sl, c->b, d_row_off, (uint32_t)n_out, batch, training != 0, d_out_f16, st);
+  }
   if (training) {
     c->n_occ = n_occ;
     c->batch = batch;
@@ -1014,6 +1108,7 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
   if (phases == 0) phases = PB_PHASE_ALL;
   const bool all = phases == PB_PHASE_ALL;
   if (!t || !c || !x || !h_slot_occ_off || !d_out_f16 || (n_occ && !d_ids)) return fail(PB_ERR_INVALID, "null argument");
+  if (t->tier) return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no sharded calls)");
   if (misaligned(d_out_f16)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
   if (!c->has_slots) return fail(PB_ERR_STATE, "pb_ctx_set_slots not called");
   if (t->device != c->device || t->device != x->device) return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
@@ -1222,6 +1317,7 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   if (training) {
     if ((rc = maybe_evict(t, st))) return rc;
     launch_begin_batch(t->d, c->dev_tick, nullptr, st);
+    restore_ids(t, true, sl, d_ids, n_occ, st);
     launch_probe(MODE_TRAIN, true, t->d, t->hy, t->op, sl, d_ids, n_occ, c->occ_cell, st);
   } else {
     launch_probe(MODE_FIND, true, t->d, t->hy, t->op, sl, d_ids, n_occ, c->occ_cell, st);
@@ -1234,6 +1330,8 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   }
   launch_raw_forward(t->d, sl, d_ids, n_occ, d_row_off ? c->row_off : nullptr, occ_sample, batch, sample_fixed_size,
                      c->occ_cell, c->raw, d_table_f16, (long long*)d_index, (long long*)d_non_empty, d_sample_id_num, st);
+  if (!training && t->tier)  // inference moves nothing: tier-held signs are read where they are
+    launch_tier_raw_fill(t->d, t->tier->d, sl, d_ids, n_occ, c->occ_cell, c->raw, d_table_f16, st);
   PB_CUDA(cudaMemcpyAsync(d_counts, c->raw.counts, 8, cudaMemcpyDeviceToDevice, st));
   if (training) {
     c->n_occ = n_occ;
@@ -1299,6 +1397,7 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
   const bool all = phases == PB_PHASE_ALL;
   if (!t || !c || !x || !d_table_f16 || !d_index || !d_non_empty || !d_sample_id_num || !d_counts || (n_occ && !d_ids))
     return fail(PB_ERR_INVALID, "null argument");
+  if (t->tier) return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no sharded calls)");
   if (misaligned(d_table_f16)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
   if (!c->has_slots || c->slots.n_slots != 1) return fail(PB_ERR_STATE, "a raw context serves exactly one slot (pb_ctx_set_slots)");
   if (t->device != c->device || t->device != x->device) return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");

@@ -89,6 +89,11 @@ enum {
   CTR_EVICT = 7,     // rows evicted
   CTR_ERR = 8,       // an in-kernel wait gave up (mbarrier / peer flag): results of that batch are void
   CTR_USED = 9,      // normal index cells that are not EMPTY (live or tombstone): the index is rebuilt before it fills
+  // a host-memory tier's own counters (pb_tier.cu; zero on every other table)
+  CTR_TIER_OUT = 10,      // entries moved in from the HBM table by its eviction checks
+  CTR_TIER_IN = 11,       // entries restored into the HBM table (their tier rows are free again)
+  CTR_TIER_REFUSED = 12,  // restores that found no free HBM row (the entry stayed in the tier)
+  CTR_TIER_LOST = 13,     // victims of an HBM sweep that found no tier row (dropped, like a plain sweep's)
   CTR_COUNT = 16
 };
 

@@ -154,10 +154,13 @@ __device__ __forceinline__ void store_f16(__half* dst, const float (&acc)[VEC], 
 
 constexpr int GATHER_ITEM_ROWS = 4;  // output rows per group in the one-id-per-sample layout (independent loads in flight)
 
-template <int VEC, int G, bool TRAIN>
+// TIER (inference with a host tier attached, pb_tier.cu): an item whose target is capacity + r reads row r of the tier
+// in place, tier_rows = the tier's mapped rows (same stride), tier_cap its rows
+template <int VEC, int G, bool TRAIN, bool TIER>
 __global__ void __launch_bounds__(256) k_gather_items(TableDev t, SlotsDev sl, BatchDev b,
                                                       const uint32_t* __restrict__ row_off, uint32_t n_out,
-                                                      uint32_t batch, __half* __restrict__ out) {
+                                                      uint32_t batch, __half* __restrict__ out,
+                                                      const float* __restrict__ tier_rows, uint32_t tier_cap) {
   const uint32_t group = (blockIdx.x * blockDim.x + threadIdx.x) / G;
   const uint32_t lane = threadIdx.x % G;
   const uint32_t nvec = t.dim / VEC;
@@ -189,6 +192,8 @@ __global__ void __launch_bounds__(256) k_gather_items(TableDev t, SlotsDev sl, B
       for (int k = 0; k < GATHER_ITEM_ROWS; ++k) {
         if (ref[k].row < t.capacity) {
           load_vec<VEC>(t.rows + (size_t)ref[k].row * t.stride + c * VEC, v[k]);
+        } else if (TIER && ref[k].row - t.capacity < tier_cap) {
+          load_vec<VEC>(tier_rows + (size_t)(ref[k].row - t.capacity) * t.stride + c * VEC, v[k]);
         } else {
 #pragma unroll
           for (int e = 0; e < VEC; ++e) v[k][e] = 0.0f;
@@ -224,9 +229,10 @@ __global__ void __launch_bounds__(256) k_gather_items(TableDev t, SlotsDev sl, B
     for (int k = 0; k < VEC; ++k) acc[k] = 0.0f;
     for (uint32_t j = beg; j < end; ++j) {
       const uint32_t row = b.set[b.occ_set[j]].target;
-      if (row >= t.capacity) continue;
       float v[VEC];
-      load_vec<VEC>(t.rows + (size_t)row * t.stride + c * VEC, v);
+      if (row < t.capacity) load_vec<VEC>(t.rows + (size_t)row * t.stride + c * VEC, v);
+      else if (TIER && row - t.capacity < tier_cap) load_vec<VEC>(tier_rows + (size_t)(row - t.capacity) * t.stride + c * VEC, v);
+      else continue;
 #pragma unroll
       for (int k = 0; k < VEC; ++k) acc[k] = __fadd_rn(acc[k], v[k]);
     }
@@ -280,32 +286,38 @@ void launch_probe_items(bool training, const TableDev& t, const HyperDev& hy, co
   else PB_LAUNCH_F(FAM_PROBE, (k_probe_items<MODE_FIND>), grid, 256, 0, st, t, hy, op, sl, b);
 }
 
-template <int VEC, bool TRAIN>
+template <int VEC, bool TRAIN, bool TIER>
 static void gather_items_dispatch(int G, const TableDev& t, const SlotsDev& sl, const BatchDev& b, const uint32_t* row_off,
-                                  uint32_t n_out, uint32_t batch, __half* out, cudaStream_t st) {
+                                  uint32_t n_out, uint32_t batch, __half* out, const float* tier_rows, uint32_t tier_cap,
+                                  cudaStream_t st) {
   uint32_t grid;
 #define PB_G(GG)                                                                                                  \
   case GG:                                                                                                        \
     grid = cdiv((uint64_t)(row_off ? n_out : cdiv(n_out, GATHER_ITEM_ROWS)) * GG, 256);                           \
     if (!row_off && grid < cdiv(n_out, 256)) grid = cdiv(n_out, 256);                                             \
-    PB_LAUNCH_F(FAM_GATHER, (k_gather_items<VEC, GG, TRAIN>), grid, 256, 0, st, t, sl, b, row_off, n_out, batch, out); \
+    PB_LAUNCH_F(FAM_GATHER, (k_gather_items<VEC, GG, TRAIN, TIER>), grid, 256, 0, st, t, sl, b, row_off, n_out, batch, out, \
+                tier_rows, tier_cap);                                                                              \
     break;
   switch (G) { PB_G(1) PB_G(2) PB_G(4) PB_G(8) PB_G(16) PB_G(32) }
 #undef PB_G
 }
 
 void launch_gather_items(const TableDev& t, const SlotsDev& sl, const BatchDev& b, const uint32_t* row_off,
-                         uint32_t n_out, uint32_t batch, bool training, void* out_f16, cudaStream_t st) {
+                         uint32_t n_out, uint32_t batch, bool training, void* out_f16, cudaStream_t st,
+                         const float* tier_rows, uint32_t tier_cap) {
   if (!n_out) return;
   int vec, G;
   vec_group(t.dim, vec, G);
   __half* out = reinterpret_cast<__half*>(out_f16);
+  const bool tier = !training && tier_rows;
   if (vec == 4) {
-    if (training) gather_items_dispatch<4, true>(G, t, sl, b, row_off, n_out, batch, out, st);
-    else gather_items_dispatch<4, false>(G, t, sl, b, row_off, n_out, batch, out, st);
+    if (training) gather_items_dispatch<4, true, false>(G, t, sl, b, row_off, n_out, batch, out, nullptr, 0, st);
+    else if (tier) gather_items_dispatch<4, false, true>(G, t, sl, b, row_off, n_out, batch, out, tier_rows, tier_cap, st);
+    else gather_items_dispatch<4, false, false>(G, t, sl, b, row_off, n_out, batch, out, nullptr, 0, st);
   } else {
-    if (training) gather_items_dispatch<1, true>(G, t, sl, b, row_off, n_out, batch, out, st);
-    else gather_items_dispatch<1, false>(G, t, sl, b, row_off, n_out, batch, out, st);
+    if (training) gather_items_dispatch<1, true, false>(G, t, sl, b, row_off, n_out, batch, out, nullptr, 0, st);
+    else if (tier) gather_items_dispatch<1, false, true>(G, t, sl, b, row_off, n_out, batch, out, tier_rows, tier_cap, st);
+    else gather_items_dispatch<1, false, false>(G, t, sl, b, row_off, n_out, batch, out, nullptr, 0, st);
   }
 }
 

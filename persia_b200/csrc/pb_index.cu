@@ -147,7 +147,6 @@ __global__ void k_fill_cells(Cell* cells, uint64_t n) {
 // (3) tombstone those cells and push their rows on the free stack.  ev[0] = threshold age, ev[1] = want,
 // ev[2] = go flag, ev[3..] = age histogram (EV_BINS bins, last bin = older).
 // ------------------------------------------------------------------------------------------------
-constexpr uint32_t EV_BINS = 1024;
 __global__ void k_evict_plan(TableDev t, uint32_t low_water, uint32_t target_free, uint32_t* __restrict__ ev) {
   // one block: decide whether a sweep is needed and clear the histogram
   uint32_t used = min(t.counters[CTR_ROWS], t.capacity);
@@ -242,7 +241,6 @@ __global__ void __launch_bounds__(256) k_evict_sweep_spill(TableDev t, uint32_t*
 // so rows held by pending batches stay valid.  After a rebuild at most capacity <= 2/3 n_cells cells are used.
 // ev[EV_RB] = rebuild flag, ev[EV_RB + 1] = pairs compacted.
 // ------------------------------------------------------------------------------------------------
-constexpr uint32_t EV_RB = 3 + EV_BINS;
 static_assert(EV_RB + 2 <= EVICT_WS_WORDS, "eviction workspace too small");
 
 __global__ void k_rebuild_plan(TableDev t, uint32_t* __restrict__ ev) {
@@ -319,7 +317,7 @@ __global__ void __launch_bounds__(256) k_index_stats(TableDev t, uint32_t* __res
 // ------------------------------------------------------------------------------------------------
 // launchers (host)
 // ------------------------------------------------------------------------------------------------
-static void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st) {
+void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st) {
   PB_LAUNCH(k_rebuild_plan, 1, 32, 0, st, t, ev);
   PB_LAUNCH(k_rebuild_compact, PB_NUM_SMS * 8, 256, 0, st, t, ev, keys, rows);
   PB_LAUNCH(k_rebuild_clear, PB_NUM_SMS * 8, 256, 0, st, t, ev);
@@ -424,6 +422,24 @@ void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, u
   PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
   PB_LAUNCH(k_evict_sweep, PB_NUM_SMS * 8, 256, 0, st, t, ev);
   launch_rebuild(t, ev, rb_keys, rb_rows, st);
+}
+
+// The HBM table's plan and threshold count its victims; the tier's own sweep (gated on the flag launch_tier_plan sets)
+// drops as many of the tier's oldest entries as it takes to hold them; the victims then move (launch_tier_move) instead
+// of being swept.  Every step reads its sizes from the device: no host sync, a captured step stays capturable.
+void launch_evict_tier(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, uint32_t low_water,
+                       uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys, uint32_t* rb_rows, uint32_t* tev,
+                       uint64_t* trb_keys, uint32_t* trb_rows, uint32_t* move_cells, cudaStream_t st) {
+  PB_LAUNCH(k_evict_plan, 1, 256, 0, st, h, low_water, target_free, ev);
+  PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, h, ev);
+  PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
+  launch_tier_plan(h, t, ev, tev, st);
+  PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, t, tev);
+  PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, 0u, tev);  // no batch holds a tier row: only the current batch number's stay
+  PB_LAUNCH(k_evict_sweep, PB_NUM_SMS * 8, 256, 0, st, t, tev);
+  launch_tier_move(h, t, hy, op, ev, tev, rb_keys, rb_rows, move_cells, st);  // (the rebuild buffers are free until below)
+  launch_rebuild(h, ev, rb_keys, rb_rows, st);
+  launch_rebuild(t, tev, trb_keys, trb_rows, st);
 }
 
 void launch_shard_of(const uint64_t* signs, uint32_t n, uint32_t R, uint32_t* shard, uint64_t* hash, cudaStream_t st) {

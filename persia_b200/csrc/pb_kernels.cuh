@@ -160,8 +160,10 @@ void launch_gather(const TableDev& t, const uint32_t* occ_cell, uint32_t n_out, 
 void launch_dedup(const SlotsDev& sl, const BatchDev& b, const uint64_t* ids, cudaStream_t st);
 void launch_probe_items(bool training, const TableDev& t, const HyperDev& hy, const OptimDev& op, const SlotsDev& sl,
                         const BatchDev& b, cudaStream_t st);
+// tier_rows / tier_cap (inference with a host tier): targets >= capacity name tier rows, read in place
 void launch_gather_items(const TableDev& t, const SlotsDev& sl, const BatchDev& b, const uint32_t* row_off,
-                         uint32_t n_out, uint32_t batch, bool training, void* out_f16, cudaStream_t st);
+                         uint32_t n_out, uint32_t batch, bool training, void* out_f16, cudaStream_t st,
+                         const float* tier_rows = nullptr, uint32_t tier_cap = 0);
 void launch_clear_items(const BatchDev& b, cudaStream_t st);
 void launch_clear_hot_bits(const BatchDev& b, cudaStream_t st);  // of a batch whose backward never came
 void launch_copy_entries(bool write, const TableDev& t, const uint32_t* occ_cell, uint32_t n, float* entries,
@@ -238,18 +240,55 @@ void launch_export_signs(const TableDev& t, uint64_t* signs, uint32_t* recency, 
                          cudaStream_t st);
 // capacity sweeps (pb_index.cu): ev = EVICT_WS_WORDS words; rb_keys / rb_rows = `capacity` entries each, where the index
 // rebuild that follows every sweep check compacts the live pairs
-constexpr uint32_t EVICT_WS_WORDS = 3 + 1024 + 2;
+constexpr uint32_t EV_BINS = 1024;        // ev[3..]: age histogram (last bin = older)
+constexpr uint32_t EV_RB = 3 + EV_BINS;   // ev[EV_RB] rebuild flag, ev[EV_RB + 1] pairs compacted
+constexpr uint32_t EV_MOVE = EV_RB + 2;   // a tier's ev[EV_MOVE]: HBM victims listed for the move (pb_tier.cu)
+constexpr uint32_t EVICT_WS_WORDS = EV_MOVE + 1;
 void launch_spill(const TableDev& t, uint32_t want_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys, uint32_t* rb_rows,
                   uint64_t* signs, float* entries, uint32_t max_n, uint32_t* count, cudaStream_t st);
 void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys,
                   uint32_t* rb_rows, cudaStream_t st);
 void launch_index_stats(const TableDev& t, uint32_t* out, cudaStream_t st);
+// host-memory tier (pb_tier.cu).  h: the HBM table, t: its tier (rows in mapped pinned host memory).
+// The eviction check of a table with a tier: the HBM sweep's victims move into the tier (whose own sweep first drops its
+// oldest entries to make room) instead of being dropped.  ev / rb_*: the HBM table's workspaces, tev / trb_*: the tier's,
+// move_cells: `h.capacity` words.
+void launch_evict_tier(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, uint32_t low_water,
+                       uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys, uint32_t* rb_rows, uint32_t* tev,
+                       uint64_t* trb_keys, uint32_t* trb_rows, uint32_t* move_cells, cudaStream_t st);
+void launch_tier_plan(const TableDev& h, const TableDev& t, const uint32_t* ev, uint32_t* tev, cudaStream_t st);
+void launch_tier_move(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const uint32_t* ev,
+                      uint32_t* tev, uint64_t* keys, uint32_t* rows, uint32_t* cells, cudaStream_t st);
+// before a probe: every sign the HBM index lacks and the tier holds is moved into a free HBM row (flat ids, prefixed by
+// slot when `prefix`; or the distinct items of a batch)
+void launch_tier_restore(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const SlotsDev& sl,
+                         bool prefix, const uint64_t* ids, uint32_t n, cudaStream_t st);
+void launch_tier_restore_items(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op,
+                               const BatchDev& b, cudaStream_t st);
+// Reads in place (no move): signs the HBM probe missed (occ_cell = none) that the tier holds.
+//   pb_get_rows: whole entries (len = entry length) + found;  inference pb_lookup: embeddings (len = dim), and the
+//   HBM table's CTR_MISS gives back the misses it counted for them (miss_ctr = that counter)
+void launch_tier_get(const TableDev& h, const TableDev& t, const uint64_t* signs, const uint32_t* occ_cell, uint32_t n,
+                     uint32_t len, float* entries, uint8_t* found, uint32_t* miss_ctr, cudaStream_t st);
+// inference pb_forward: items the HBM probe missed get target = h.capacity + tier row (launch_gather_items reads it)
+void launch_tier_find_items(const TableDev& h, const TableDev& t, const BatchDev& b, cudaStream_t st);
+// inference pb_forward_raw: distinct signs the HBM probe missed are filled into the f16 table from the tier
+void launch_tier_raw_fill(const TableDev& h, const TableDev& t, const SlotsDev& sl, const uint64_t* ids, uint32_t n,
+                          const uint32_t* occ_cell, const RawWork& w, void* table_f16, cudaStream_t st);
+// pb_update: where[i] = the tier cell of every sign the HBM probe missed and the tier holds (else none); the HBM table's
+// CTR_GRAD_MISS gives back the miss its update will count for it
+void launch_tier_where(const TableDev& h, const TableDev& t, const uint64_t* signs, const uint32_t* occ_cell, uint32_t n,
+                       uint32_t* where, cudaStream_t st);
+// pb_set_rows: entries the HBM table had no row for are stored in the tier
+void launch_tier_set(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const uint64_t* signs,
+                     const uint32_t* occ_cell, uint32_t n, const float* entries, cudaStream_t st);
+void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st);
 uint64_t launch_count();
 enum { FAM_PROBE = 0, FAM_DEDUP, FAM_GATHER, FAM_NAN, FAM_HOT, FAM_UPDATE, FAM_OTHER, FAM_WARM, FAM_WAIT, FAM_ROUTE, FAM_OWNER, FAM_COUNT };
 bool profiling();  // a kernel family is being timed: the backward then runs its kernels one after another
 void profile_enable(uint32_t family_mask);
 void profile_read(double* ms, uint64_t* count, int n_families);
 
-enum { MODE_FIND = 0, MODE_TRAIN = 1, MODE_SET = 2 };
+enum { MODE_FIND = 0, MODE_TRAIN = 1, MODE_SET = 2, MODE_MOVE = 3 };
 
 }  // namespace pb

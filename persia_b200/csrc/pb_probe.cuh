@@ -57,6 +57,9 @@ static __device__ __noinline__ void init_row(const TableDev& t, const HyperDev& 
 //   MODE_TRAIN  find, refresh recency (get_refresh, eviction_map.rs:48-60), admit + initialise on miss
 //               (emb_entry.rs:28-68 + optim.rs:299-302)
 //   MODE_SET    find or force-admit without initialisation (set_embedding)
+//   MODE_MOVE   admit an entry that moves between an HBM table and its host tier (pb_tier.cu): as MODE_SET, but the
+//               row number stays unpublished (ROW_PENDING) for the caller to store once the entry is copied, and a
+//               refusal is not counted as CTR_FULL (the caller counts it)
 // Must be called by all 32 lanes of a warp (four groups, each with its own sign; `valid` false = no work).
 // Returns, to every lane of the group, the index cell (n_cells + N_SPECIAL = the sign has no storage) and the row
 // (ROW_NONE likewise).
@@ -128,7 +131,7 @@ __device__ __forceinline__ ProbeOut probe_group(const TableDev& t, const HyperDe
       }
       if (row >= t.capacity) {
         row = ROW_NONE;
-        atomicAdd(&t.counters[CTR_FULL], 1u);
+        if (MODE != MODE_MOVE) atomicAdd(&t.counters[CTR_FULL], 1u);
       } else {
         atomicAdd(&t.counters[CTR_ADMIT], 1u);
         t.row_tick[row] = tick;  // recency of a fresh row
@@ -137,7 +140,7 @@ __device__ __forceinline__ ProbeOut probe_group(const TableDev& t, const HyperDe
         *reinterpret_cast<volatile uint32_t*>(&t.cells[free_cell].row) = row;
         __threadfence();
         *reinterpret_cast<volatile unsigned long long*>(&t.cells[free_cell].key) = special ? KEY_EMPTY : KEY_TOMB;
-      } else if (MODE != MODE_TRAIN) {
+      } else if (MODE == MODE_SET) {
         *reinterpret_cast<volatile uint32_t*>(&t.cells[free_cell].row) = row;  // set_embedding: the caller fills the row
       }
     }

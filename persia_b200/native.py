@@ -59,6 +59,9 @@ SYMBOLS = {
     "pb_table_spill": (_i32, [_vp, _u64, _u32, _vp, _vp, _u32, _vp, _vp]),
     "pb_table_counters": (_i32, [_vp, C.POINTER(_u64 * 5), _vp]),
     "pb_table_index_stats": (_i32, [_vp, C.POINTER(_u64 * 3), _vp]),
+    "pb_table_create_host": (_i32, [_i32, C.POINTER(TableCfg), C.POINTER(_vp)]),
+    "pb_table_attach_tier": (_i32, [_vp, _vp]),
+    "pb_tier_stats": (_i32, [_vp, C.POINTER(_u64 * 5), _vp]),
     "pb_lookup": (_i32, [_vp, _vp, _u32, _i32, _vp, _vp]),
     "pb_update": (_i32, [_vp, _vp, _vp, _u32, _vp]),
     "pb_set_rows": (_i32, [_vp, _vp, _vp, _u32, _vp]),

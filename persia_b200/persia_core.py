@@ -74,6 +74,24 @@ def parse_embedding_config(cfg):
     return bits, slots
 
 
+def hbm_split(capacity, hbm_rows, replica_size=1):
+    """(rows in HBM, rows of the host-memory tier behind them) of a table of `capacity` entries.  hbm_rows
+    (PERSIA_B200_HBM_ROWS; None or "" = unset): a table larger than that keeps the rest in host memory, moved in and out
+    by the kernels (include/persia_b200.h, pb_table_attach_tier); unset or >= capacity: everything in HBM, no tier."""
+    capacity = int(capacity)
+    if hbm_rows is None or str(hbm_rows).strip() == "":
+        return capacity, 0
+    hbm_rows = int(hbm_rows)
+    if hbm_rows <= 0:
+        raise RuntimeError(f"PERSIA_B200_HBM_ROWS must be positive, got {hbm_rows}")
+    if hbm_rows >= capacity:
+        return capacity, 0
+    if (replica_size or 1) > 1:
+        raise RuntimeError("PERSIA_B200_HBM_ROWS (a host-memory tier behind the HBM rows) is supported on one GPU only "
+                           f"(replica_size = 1, got {replica_size}): unset it or raise it to the capacity ({capacity})")
+    return hbm_rows, capacity - hbm_rows
+
+
 class _State:
     def __init__(self):
         self.reset()
@@ -120,7 +138,8 @@ class _State:
             from . import shard as SH
 
             dev = self.device_id if self.device_id is not None else 0
-            sh = SH.EmbeddingShard(dim, self.capacity, dev)
+            hbm, tier = hbm_split(self.capacity, os.environ.get("PERSIA_B200_HBM_ROWS"), self.replica_size)
+            sh = SH.EmbeddingShard(dim, hbm, dev, tier_rows=tier)
             sh.set_eviction()  # the reference's holder is an LRU map bounded by `capacity` (eviction_map.rs:76-97)
             if self.optimizer is not None:
                 sh.set_optimizer(**self.optimizer)

@@ -43,15 +43,21 @@ def _as_i64_bits(t):
 
 
 class EmbeddingShard:
-    def __init__(self, dim, capacity, device=0):
+    def __init__(self, dim, capacity, device=0, tier_rows=0, host=False):
+        """capacity: rows in HBM.  tier_rows > 0: a host-memory tier of that many rows behind them (include/persia_b200.h,
+        pb_table_attach_tier), attached once the optimizer is registered.  host: this table's rows live in host memory
+        (the tier itself)."""
         self.lib = N.load()
         self.dim, self.capacity = int(dim), int(capacity)
         self.device = torch.device("cuda", device) if not isinstance(device, torch.device) else device
         h = C.c_void_p()
         cfg = N.TableCfg(self.dim, self.capacity)
-        N.check(self.lib.pb_table_create(self.device.index or 0, C.byref(cfg), C.byref(h)))
+        create = self.lib.pb_table_create_host if host else self.lib.pb_table_create
+        N.check(create(self.device.index or 0, C.byref(cfg), C.byref(h)))
         self.h = h
         self._entry_len = None
+        self.host_tier = EmbeddingShard(dim, tier_rows, device, host=True) if tier_rows else None
+        self._tier_attached = False
 
     # register_optimizer (PS mod.rs:429-438)
     def set_optimizer(self, kind, lr=0.01, wd=0.0, g_square_momentum=1.0, initialization=0.01, eps=1e-10,
@@ -59,6 +65,11 @@ class EmbeddingShard:
         cfg = N.OptimCfg(kind, lr, wd, g_square_momentum, initialization, eps, beta1, beta2)
         N.check(self.lib.pb_table_set_optimizer(self.h, C.byref(cfg)))
         self._entry_len = None
+        if self.host_tier is not None:  # one entry layout in both tables
+            N.check(self.lib.pb_table_set_optimizer(self.host_tier.h, C.byref(cfg)))
+            if not self._tier_attached:
+                N.check(self.lib.pb_table_attach_tier(self.h, self.host_tier.h))
+                self._tier_attached = True
 
     # configure (PS mod.rs:440-451)
     def configure(self, init_lower=-0.01, init_upper=0.01, admit_probability=1.0, enable_weight_bound=True,
@@ -92,8 +103,16 @@ class EmbeddingShard:
         N.check(self.lib.pb_table_index_stats(self.h, C.byref(out), _stream(self.device)))
         return {"live": out[0], "tomb": out[1], "empty": out[2]}
 
+    def tier_stats(self):
+        """The host tier's counters (host sync); all zero without a tier."""
+        out = (C.c_uint64 * 5)()
+        N.check(self.lib.pb_tier_stats(self.h, C.byref(out), _stream(self.device)))
+        return {"host_rows": out[0], "moved_out": out[1], "restored": out[2], "dropped": out[3], "refused": out[4]}
+
     def __len__(self):
-        return int(self.counters()["admitted"])
+        """Entries held: the HBM rows plus the host tier's."""
+        n = int(self.counters()["admitted"])
+        return n + int(self.tier_stats()["host_rows"]) if self.host_tier is not None else n
 
     def clear(self):
         N.check(self.lib.pb_table_clear(self.h, _stream(self.device)))
@@ -141,17 +160,26 @@ class EmbeddingShard:
         n = min(int(count), max_n)
         return signs[:n].cpu().numpy().view(np.uint64), ent[:n].cpu().numpy()
 
-    def export_signs(self):
-        """Resident signs (int64 bit patterns) and the training-request number each was last used in, on the device,
-        sorted oldest first (ties by sign): the order the reference's LRU list is dumped in."""
+    def _export_table(self, h):
         count = torch.zeros(1, dtype=torch.int32, device=self.device)
-        N.check(self.lib.pb_table_export_signs(self.h, None, None, 0, _ptr(count), _stream(self.device)))
+        N.check(self.lib.pb_table_export_signs(h, None, None, 0, _ptr(count), _stream(self.device)))
         n = int(count)
         signs = torch.empty(n, dtype=torch.int64, device=self.device)
         rec = torch.empty(n, dtype=torch.int32, device=self.device)
         if n:
-            N.check(self.lib.pb_table_export_signs(self.h, _ptr(signs), _ptr(rec), n, _ptr(count), _stream(self.device)))
+            N.check(self.lib.pb_table_export_signs(h, _ptr(signs), _ptr(rec), n, _ptr(count), _stream(self.device)))
             assert int(count) == n, "the table changed during the export"
+        return signs, rec
+
+    def export_signs(self):
+        """Resident signs (int64 bit patterns) and the training-request number each was last used in, on the device,
+        sorted oldest first (ties by sign): the order the reference's LRU list is dumped in.  With a host tier, the
+        signs of both tables (they share one clock)."""
+        signs, rec = self._export_table(self.h)
+        if self.host_tier is not None:
+            ts, tr = self._export_table(self.host_tier.h)
+            signs, rec = torch.cat([signs, ts]), torch.cat([rec, tr])
+        if signs.numel():
             order = torch.argsort(signs, stable=True)           # deterministic file: by sign ...
             order = order[torch.argsort(rec[order].to(torch.int64) & 0xFFFFFFFF, stable=True)]  # ... inside a request
             signs, rec = signs[order], rec[order]
@@ -161,6 +189,8 @@ class EmbeddingShard:
         if getattr(self, "h", None):
             self.lib.pb_table_destroy(self.h)
             self.h = None
+        if getattr(self, "host_tier", None) is not None:  # after the table it stands behind
+            self.host_tier.close()
 
     def __del__(self):
         try:
