@@ -87,14 +87,6 @@ int pb_table_clear(pb_table* t, void* stream);
 int pb_table_set_eviction(pb_table* t, uint32_t check_every, uint64_t low_water, uint64_t target_free, uint32_t keep_batches);
 /* floats per resident row: dim + optimizer state (emb_entry.rs:17-25 `inner`). */
 int pb_table_entry_len(pb_table* t, uint32_t* h_out);
-/* Host-DRAM tier (BASELINE.json configs[4]: the embedding holder's DRAM behind a GPU-resident working set): release the
- * least recently used rows until `want_free` rows are free, like the capacity sweep (rows touched by the last
- * max(keep_batches, pending batches + 1) requests stay), but WRITE EVERY VICTIM OUT first: its sign to d_signs[k] and its
- * whole entry (embedding ++ optimizer state, pb_entry_len floats) to d_entries[k].  Victims beyond max_n stay resident;
- * *d_count = victims found (<= max_n were released).  The caller keeps the pairs (persia_b200/tier.py) and brings a sign
- * back with pb_set_rows before its next lookup.  Enqueued on `stream`. */
-int pb_table_spill(pb_table* t, uint64_t want_free, uint32_t keep_batches, uint64_t* d_signs, float* d_entries, uint32_t max_n,
-                   uint32_t* d_count, void* stream);
 /* counters since creation / clear: [0] resident rows (admitted - evicted), [1] distinct signs of a request that missed
  * (infer) or were not admitted (index_miss_count), [2] gradient ids not found (gradient_id_miss_count), [3] admissions
  * refused because the shard is full, [4] in-kernel waits that gave up (must stay 0: a non-zero value voids the batch
@@ -127,8 +119,8 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream);
  * entry stays as it was.  A moved entry keeps its recency, and the tier ages rows by the HBM table's training-request
  * number: the union evicts least recently used first, and pb_table_export_signs of both tables merges into the
  * reference's list order.
- * pb_table_clear of the table clears its tier too.  Destroy the table before its tier.  The sharded calls and
- * pb_table_spill refuse a table with a tier. */
+ * pb_table_clear of the table clears its tier too.  Destroy the table before its tier.  The sharded calls refuse a
+ * table with a tier. */
 int pb_table_create_host(int device, const pb_table_cfg* cfg, pb_table** out);
 /* Both tables need their optimizer registered; checks dim, optimizer kind and row stride. */
 int pb_table_attach_tier(pb_table* t, pb_table* tier);

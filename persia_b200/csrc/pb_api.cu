@@ -427,23 +427,6 @@ int pb_table_configure(pb_table* t, const pb_hyper_cfg* c) {
   return PB_OK;
 }
 
-int pb_table_spill(pb_table* t, uint64_t want_free, uint32_t keep_batches, uint64_t* d_signs, float* d_entries, uint32_t max_n,
-                   uint32_t* d_count, void* stream) {
-  if (!t || !d_count || (max_n && (!d_signs || !d_entries))) return fail(PB_ERR_INVALID, "null argument");
-  if (t->tier || t->tier_of) return fail(PB_ERR_STATE, "a table with a host tier (or a tier) moves its rows itself: no spill");
-  DeviceGuard g(t->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  int rc = ensure_evict_ws(t);
-  if (rc) return rc;
-  if (want_free > t->d.capacity) want_free = t->d.capacity;
-  const uint32_t keep = keep_batches > t->pending_batches + 1 ? keep_batches : t->pending_batches + 1;
-  PB_CUDA(cudaMemsetAsync(d_count, 0, sizeof(uint32_t), st));
-  launch_spill(t->d, (uint32_t)want_free, keep, t->evict_ws, t->rebuild_keys, t->rebuild_rows, d_signs, d_entries, max_n,
-               d_count, st);
-  PB_CUDA(cudaGetLastError());
-  return PB_OK;
-}
-
 int pb_table_set_eviction(pb_table* t, uint32_t check_every, uint64_t low_water, uint64_t target_free, uint32_t keep_batches) {
   if (!t) return fail(PB_ERR_INVALID, "null argument");
   if (check_every && (target_free < low_water || target_free > t->cfg.capacity))

@@ -166,8 +166,7 @@ __global__ void __launch_bounds__(256) k_evict_hist(TableDev t, uint32_t* __rest
   const uint64_t n = (uint64_t)t.n_cells + N_SPECIAL;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     Cell c = t.cells[i];
-    bool occupied = (i < t.n_cells) ? (c.key < KEY_TOMB) : (c.key == 0ULL);
-    if (!occupied || c.row >= t.capacity) continue;
+    if (!cell_live(t, i, c)) continue;
     uint32_t age = tick - t.row_tick[c.row];
     atomicAdd(&ev[3 + min(age, EV_BINS - 1)], 1u);
   }
@@ -190,40 +189,10 @@ __global__ void __launch_bounds__(256) k_evict_sweep(TableDev t, uint32_t* __res
   const uint64_t n = (uint64_t)t.n_cells + N_SPECIAL;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     Cell c = t.cells[i];
-    bool occupied = (i < t.n_cells) ? (c.key < KEY_TOMB) : (c.key == 0ULL);
-    if (!occupied || c.row >= t.capacity) continue;
+    if (!cell_live(t, i, c)) continue;
     uint32_t age = tick - t.row_tick[c.row];
     if (age < thr) continue;
     t.cells[i].key = (i < t.n_cells) ? KEY_TOMB : KEY_EMPTY;  // reserved cells have no probe chain behind them
-    t.cells[i].row = ROW_PENDING;
-    t.row_tick[c.row] = 0u;
-    uint32_t f = atomicAdd(&t.counters[CTR_FREE], 1u);
-    t.free_rows[f] = c.row;
-    atomicAdd(&t.counters[CTR_EVICT], 1u);
-  }
-}
-
-// the same sweep for a table backed by a host tier (pb_table_spill): every released row is first written out — sign
-// and whole entry (embedding ++ optimizer state) — and only the victims that fit the caller's buffers are released
-__global__ void __launch_bounds__(256) k_evict_sweep_spill(TableDev t, uint32_t* __restrict__ ev, uint64_t* __restrict__ signs,
-                                                           float* __restrict__ entries, uint32_t max_n,
-                                                           uint32_t* __restrict__ count) {
-  if (!ev[2] || ev[0] == 0xFFFFFFFFu) return;
-  const uint32_t tick = t.counters[CTR_TICK], thr = ev[0];
-  const uint64_t n = (uint64_t)t.n_cells + N_SPECIAL;
-  const uint32_t entry_len = t.dim + t.state_floats;
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    Cell c = t.cells[i];
-    bool occupied = (i < t.n_cells) ? (c.key < KEY_TOMB) : (c.key == 0ULL);
-    if (!occupied || c.row >= t.capacity) continue;
-    uint32_t age = tick - t.row_tick[c.row];
-    if (age < thr) continue;
-    const uint32_t at = atomicAdd(count, 1u);
-    if (at >= max_n) continue;  // no room to write it out: it stays resident (count tells the caller)
-    signs[at] = (i < t.n_cells) ? c.key : KEY_EMPTY - (i - t.n_cells);  // the three marker-valued signs
-    const float* row = t.rows + (size_t)c.row * t.stride;
-    for (uint32_t e = 0; e < entry_len; ++e) entries[(size_t)at * entry_len + e] = row[e];
-    t.cells[i].key = (i < t.n_cells) ? KEY_TOMB : KEY_EMPTY;
     t.cells[i].row = ROW_PENDING;
     t.row_tick[c.row] = 0u;
     uint32_t f = atomicAdd(&t.counters[CTR_FREE], 1u);
@@ -390,11 +359,10 @@ __global__ void __launch_bounds__(256) k_export_signs(TableDev t, uint64_t* __re
   const uint64_t n = (uint64_t)t.n_cells + N_SPECIAL;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     Cell c = t.cells[i];
-    const bool occupied = (i < t.n_cells) ? (c.key < KEY_TOMB) : (c.key == 0ULL);
-    if (!occupied || c.row >= t.capacity) continue;
+    if (!cell_live(t, i, c)) continue;
     const uint32_t k = atomicAdd(count, 1u);
     if (k < max_n) {
-      signs[k] = (i < t.n_cells) ? c.key : KEY_EMPTY - (i - t.n_cells);  // the three marker-valued signs
+      signs[k] = cell_sign(t, i, c);
       recency[k] = t.row_tick[c.row];
     }
   }
@@ -404,15 +372,6 @@ void launch_export_signs(const TableDev& t, uint64_t* signs, uint32_t* recency, 
                          cudaStream_t st) {
   cudaMemsetAsync(count, 0, sizeof(uint32_t), st);
   PB_LAUNCH(k_export_signs, PB_NUM_SMS * 8, 256, 0, st, t, signs, recency, max_n, count);
-}
-
-void launch_spill(const TableDev& t, uint32_t want_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys, uint32_t* rb_rows,
-                  uint64_t* signs, float* entries, uint32_t max_n, uint32_t* count, cudaStream_t st) {
-  PB_LAUNCH(k_evict_plan, 1, 256, 0, st, t, want_free, want_free, ev);
-  PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, t, ev);
-  PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
-  PB_LAUNCH(k_evict_sweep_spill, PB_NUM_SMS * 8, 256, 0, st, t, ev, signs, entries, max_n, count);
-  launch_rebuild(t, ev, rb_keys, rb_rows, st);
 }
 
 void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys,

@@ -244,8 +244,6 @@ constexpr uint32_t EV_BINS = 1024;        // ev[3..]: age histogram (last bin = 
 constexpr uint32_t EV_RB = 3 + EV_BINS;   // ev[EV_RB] rebuild flag, ev[EV_RB + 1] pairs compacted
 constexpr uint32_t EV_MOVE = EV_RB + 2;   // a tier's ev[EV_MOVE]: HBM victims listed for the move (pb_tier.cu)
 constexpr uint32_t EVICT_WS_WORDS = EV_MOVE + 1;
-void launch_spill(const TableDev& t, uint32_t want_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys, uint32_t* rb_rows,
-                  uint64_t* signs, float* entries, uint32_t max_n, uint32_t* count, cudaStream_t st);
 void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys,
                   uint32_t* rb_rows, cudaStream_t st);
 void launch_index_stats(const TableDev& t, uint32_t* out, cudaStream_t st);

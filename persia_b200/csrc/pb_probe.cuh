@@ -201,4 +201,15 @@ __device__ __forceinline__ ProbeOut probe_group(const TableDev& t, const HyperDe
   return o;
 }
 
+// Whole-index scans (eviction, checkpoint export, the tier's move) visit all n_cells + N_SPECIAL cells `i` holding `c`.
+// live: the cell holds a sign with a row (a reserved cell holds 0 for its sign, KEY_EMPTY when it is free)
+__device__ __forceinline__ bool cell_live(const TableDev& t, uint64_t i, const Cell& c) {
+  return (i < t.n_cells ? c.key < KEY_TOMB : c.key == 0ULL) && c.row < t.capacity;
+}
+
+// the sign a live cell holds: reserved cell n_cells + k holds the marker-valued sign KEY_EMPTY - k
+__device__ __forceinline__ uint64_t cell_sign(const TableDev& t, uint64_t i, const Cell& c) {
+  return i < t.n_cells ? c.key : KEY_EMPTY - (i - t.n_cells);
+}
+
 }  // namespace pb

@@ -148,11 +148,10 @@ __global__ void __launch_bounds__(256) k_tier_collect(TableDev h, const uint32_t
   const uint64_t n = (uint64_t)h.n_cells + N_SPECIAL;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
     const Cell c = h.cells[i];
-    const bool occupied = (i < h.n_cells) ? (c.key < KEY_TOMB) : (c.key == 0ULL);
-    if (!occupied || c.row >= h.capacity) continue;
+    if (!cell_live(h, i, c)) continue;
     if (tick - h.row_tick[c.row] < thr) continue;
     const uint32_t at = atomicAdd(&tev[EV_MOVE], 1u);  // < capacity: every live cell holds a row of its own
-    keys[at] = (i < h.n_cells) ? c.key : KEY_EMPTY - (i - h.n_cells);  // the three marker-valued signs
+    keys[at] = cell_sign(h, i, c);
     rows[at] = c.row;
     cells[at] = (uint32_t)i;
   }

@@ -56,7 +56,6 @@ SYMBOLS = {
     "pb_table_clear": (_i32, [_vp, _vp]),
     "pb_table_entry_len": (_i32, [_vp, C.POINTER(_u32)]),
     "pb_table_set_eviction": (_i32, [_vp, _u32, _u64, _u64, _u32]),
-    "pb_table_spill": (_i32, [_vp, _u64, _u32, _vp, _vp, _u32, _vp, _vp]),
     "pb_table_counters": (_i32, [_vp, C.POINTER(_u64 * 5), _vp]),
     "pb_table_index_stats": (_i32, [_vp, C.POINTER(_u64 * 3), _vp]),
     "pb_table_create_host": (_i32, [_i32, C.POINTER(TableCfg), C.POINTER(_vp)]),

@@ -8,7 +8,6 @@ memory and the current stream here; all compute is in libpersia_b200.so.
 """
 import ctypes as C
 
-import numpy as np
 import torch
 
 from . import native as N
@@ -148,18 +147,6 @@ class EmbeddingShard:
         N.check(self.lib.pb_get_rows(self.h, _ptr(signs), n, _ptr(ent), _ptr(found), _stream(self.device)))
         return ent, found.bool()
 
-    def spill(self, want_free, keep_batches=1, max_n=None):
-        """pb_table_spill: release least recently used rows until `want_free` are free, returning what was released as
-        (signs uint64 numpy, entries float32 numpy [n, entry_len]) — the host tier's input."""
-        max_n = int(max_n if max_n is not None else min(self.capacity, max(int(want_free), 1)))
-        signs = torch.empty(max_n, dtype=torch.int64, device=self.device)
-        ent = torch.empty((max_n, self.entry_len), dtype=torch.float32, device=self.device)
-        count = torch.zeros(1, dtype=torch.int32, device=self.device)
-        N.check(self.lib.pb_table_spill(self.h, int(want_free), int(keep_batches), _ptr(signs), _ptr(ent), max_n, _ptr(count),
-                                        _stream(self.device)))
-        n = min(int(count), max_n)
-        return signs[:n].cpu().numpy().view(np.uint64), ent[:n].cpu().numpy()
-
     def _export_table(self, h):
         count = torch.zeros(1, dtype=torch.int32, device=self.device)
         N.check(self.lib.pb_table_export_signs(h, None, None, 0, _ptr(count), _stream(self.device)))
@@ -234,8 +221,6 @@ class BatchContext:
         off = (C.c_uint32 * (self.n_slots + 1))(*[int(x) for x in slot_occ_off])
         if row_off is not None:
             assert row_off.dtype == torch.int32 and row_off.is_contiguous()
-        if getattr(shard, "tier", None) is not None:  # host-DRAM tier: make room, bring the batch's spilled signs back
-            shard.tier.before_lookup(add_prefix(ids, slot_occ_off, self.prefixes, self.prefix_bit))
         N.check(self.lib.pb_forward(shard.h, self.h, _ptr(ids), ids.numel(), _ptr(row_off), off, int(batch),
                                     int(training), _ptr(out), _stream(self.device)))
         return out

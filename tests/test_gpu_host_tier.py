@@ -124,6 +124,56 @@ def test_tier_parity_over_churn(torch_cuda, pb, oracle, kind_name, dim, kw):
         oracle.set_rsqrt_exact(False)
 
 
+@pytest.mark.parametrize("kind_name,dim,kw", [("ADAGRAD", 16, {"lr": 0.02, "init_acc": 0.01, "eps": 1e-10}),
+                                               ("SGD", 32, {"lr": 0.05, "wd": 0.001})])
+def test_tier_parity_with_warm_signs(torch_cuda, pb, oracle, kind_name, dim, kw):
+    """Three slots of cardinality 40, 3000 and 40000 at batch 200 over C = 2500 HBM rows and ~10^4 signs: slot 0's
+    signs recur about 5 times per batch, so warm items go through restores too.  Every training forward starts with at
+    least S x B free HBM rows.  Outputs and every entry seen equal the unbounded oracle's bit for bit."""
+    torch = torch_cuda
+    kind = getattr(oracle, kind_name)
+    rng = np.random.default_rng(17 + dim)
+    S, B, card, steps, C = 3, 200, [40, 3000, 40000], 40, 2500
+    pf = [oracle.index_prefix(i) for i in range(S)]
+    s = pb.EmbeddingShard(dim, C, 0, tier_rows=1 << 14)
+    s.set_optimizer(kind, **_optim_kw(kw))
+    s.configure()
+    s.set_eviction(check_every=1, low_water=S * B, target_free=S * B, keep_batches=1)
+    ctx = pb.BatchContext(4 * S * B, 4 * S * B, pf)
+    w = oracle.Worker([oracle.SlotCfg(dim, prefix=pf[i]) for i in range(S)], n_ps=1)  # never evicts
+    w.configure()
+    w.set_optimizer(oracle.Optim(kind, **kw))
+    oracle.set_rsqrt_exact(True)
+    try:
+        seen = set()
+        for step in range(steps):
+            ids, _, slot_off = make_batch(rng, S, B, card)
+            got = ctx.forward(s, to_dev_ids(ids, DEV), slot_off, B, training=True).cpu().numpy()
+            want, octx = w.forward(ids, full_row_off(S, B), B, training=True)
+            for i in range(S):
+                assert got[i].tobytes() == want[i].tobytes(), (step, i)
+                seen.update(w.ctx_signs(octx, i).tolist())
+            g = (rng.standard_normal((S, B, dim)) * 1e-2).astype(np.float16)
+            ctx.backward(s, [torch.from_numpy(g[i]).to(DEV) for i in range(S)])
+            w.backward(octx, [g[i] for i in range(S)])
+        torch.cuda.synchronize()
+        ts = s.tier_stats()
+        assert len(seen) > 2 * C and ts["moved_out"] > 0 and ts["restored"] > 0, (len(seen), ts)
+        assert ts["dropped"] == 0 and ts["refused"] == 0, ts
+        assert len(s) == len(seen)  # every sign lives in exactly one of the two tables
+        assert s.counters()["capacity_refused"] == 0
+        signs = np.array(sorted(seen), np.uint64)
+        ent, found = s.get_entries(to_dev_ids(signs, DEV))
+        ent, found = ent.cpu().numpy(), found.cpu().numpy()
+        assert found.all()
+        for k, sign in enumerate(signs):
+            assert ent[k].tobytes() == w.get_entry(int(sign)).tobytes(), int(sign)
+    finally:
+        oracle.set_rsqrt_exact(False)
+        ctx.close()
+        s.close()
+
+
 # ---------------------------------------------------------------------------------------------- 2. union LRU
 class UnionModel:
     """The resident sets of an HBM table of C rows and its tier of T rows under pb_table_set_eviction's policy with a

@@ -160,9 +160,9 @@ def optim_pair(oracle, kind):
     return dict(lr=0.02, initialization=0.01, eps=1e-10), oracle.Optim(oracle.ADAGRAD, lr=0.02, init_acc=0.01, eps=1e-10)
 
 
-def new_shard(pb, oracle, dim, cap, kind):
+def new_shard(pb, oracle, dim, cap, kind, tier_rows=0):
     gpu, cpu = optim_pair(oracle, kind)
-    s = pb.EmbeddingShard(dim, cap, 0)
+    s = pb.EmbeddingShard(dim, cap, 0, tier_rows=tier_rows)
     s.set_optimizer(kind, **gpu)
     s.configure(init_lower=LO, init_upper=HI)
     return s, cpu
@@ -458,12 +458,12 @@ def test_refusal_then_sweep_admits(torch_cuda, oracle):
     assert c["capacity_refused"] == 200 and c["admitted"] == 100 + 200, c
 
 
-def test_marker_signs_through_eviction_spill_and_tier(torch_cuda, oracle):
-    """2^64-1, 2^64-2 and 2^64-3 equal the index's cell markers and live in reserved cells: they are evicted, re-admitted,
-    exported, spilled under their own values and brought back by the host tier; their cells return to EMPTY."""
+def test_marker_signs_through_eviction_and_the_tier(torch_cuda, oracle):
+    """2^64-1, 2^64-2 and 2^64-3 equal the index's cell markers and live in reserved cells: they are evicted, re-admitted
+    and exported.  On a table with a host tier, an eviction check moves them into the tier's reserved cells under their
+    own values, reads use them there, and a training lookup brings them back bit for bit."""
     torch = torch_cuda
     from persia_b200 import shard as pb
-    from persia_b200.tier import HostTier
 
     cap, dim = 64, 8
     markers = np.array([M64, M64 - 1, M64 - 2], np.uint64)
@@ -496,20 +496,45 @@ def test_marker_signs_through_eviction_spill_and_tier(torch_cuda, oracle):
     call(other[5:6], "age 1")
     call(other[6:7], "age 2")
     assert set(m.res) == {int(x) for x in markers} | {int(other[5]), int(other[6])}
-    tier = HostTier(s, reserve=8)
-    sg, ent = s.spill(cap, keep_batches=1, max_n=cap)  # releases the rows at least two requests old: the markers
-    assert sorted(int(x) for x in sg) == sorted(int(x) for x in markers), sg
-    by = {int(x): e for x, e in zip(sg, ent)}
-    np.testing.assert_array_equal(np.stack([by[int(x)] for x in markers]), before)
-    assert len(s) == 2 and s.index_stats()["live"] == 2
-    np.testing.assert_array_equal(s.lookup(to_dev_ids(markers, DEV), training=False).cpu().numpy(), 0)
-    tier.store.add(sg, ent)
-    tier.before_lookup(to_dev_ids(markers, DEV))  # the tier puts them back under their own signs
-    e2, found = s.get_entries(to_dev_ids(markers, DEV))
-    assert found.all()
-    np.testing.assert_array_equal(e2.cpu().numpy(), before)
     got, _ = s.export_signs()
     assert set(int(x) for x in got.cpu().numpy().view(np.uint64)) == set(m.res)
+
+    # the same signs on a table with a host tier (IndexModel counts HBM rows only: the tier is checked directly)
+    t, _ = new_shard(pb, oracle, dim, cap, oracle.SGD, tier_rows=256)
+    t.set_eviction(check_every=1, low_water=cap, target_free=cap, keep_batches=1)
+
+    def signs_of(h):
+        return set(t._export_table(h)[0].cpu().numpy().view(np.uint64).tolist())
+
+    try:
+        t.lookup(to_dev_ids(markers, DEV), training=True)
+        t.update(to_dev_ids(markers, DEV), torch.from_numpy(g).to(DEV))  # the entries `before` holds: init + one step
+        np.testing.assert_array_equal(t.get_entries(to_dev_ids(markers, DEV))[0].cpu().numpy(), before)
+        for _ in range(3):  # the check before the third releases the rows two requests old: the markers move out
+            t.lookup(to_dev_ids(other[:1], DEV), training=True)
+        ts = t.tier_stats()
+        assert ts["moved_out"] == 3 and ts["host_rows"] == 3 and ts["restored"] == 0, ts
+        assert t.index_stats()["live"] == 1 and signs_of(t.h) == {int(other[0])}
+        # in the tier's reserved cells, not its normal ones
+        assert t.host_tier.index_stats()["live"] == 0 and signs_of(t.host_tier.h) == {int(x) for x in markers}
+        got, _ = t.export_signs()
+        assert set(got.cpu().numpy().view(np.uint64).tolist()) == {int(x) for x in markers} | {int(other[0])}
+        e2, found = t.get_entries(to_dev_ids(markers, DEV))
+        assert found.all()
+        np.testing.assert_array_equal(e2.cpu().numpy(), before)
+        np.testing.assert_array_equal(t.lookup(to_dev_ids(markers, DEV), training=False).cpu().numpy(), before[:, :dim])
+        assert t.tier_stats()["restored"] == 0  # read in place
+        t.lookup(to_dev_ids(markers, DEV), training=True)  # restored under their own signs
+        ts = t.tier_stats()
+        assert ts["restored"] == 3 and ts["moved_out"] == 3 and ts["host_rows"] == 0, ts
+        assert t.host_tier.index_stats()["live"] == 0 and not signs_of(t.host_tier.h)
+        assert signs_of(t.h) == {int(x) for x in markers} | {int(other[0])}
+        e2, found = t.get_entries(to_dev_ids(markers, DEV))
+        assert found.all()
+        np.testing.assert_array_equal(e2.cpu().numpy(), before)
+        assert t.counters()["capacity_refused"] == 0
+    finally:
+        t.close()
 
 
 # ---- a pending local raw forward keeps its rows ---------------------------------------------------------------------
