@@ -19,8 +19,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-from util import (DEV, EDGE_COUNTS, EDGE_PATHS, batch_with_multiplicities, full_row_off, run_edge_path,  # noqa: E402
-                  same_bits, to_dev_i32, to_dev_ids)
+from util import (DEV, EDGE_COUNTS, EDGE_PATHS, batch_with_multiplicities, full_row_off, pool_lists,  # noqa: E402
+                  run_edge_path, same_bits, to_dev_i32, to_dev_ids)
 
 pytestmark = pytest.mark.gpu
 FLT_MIN = np.float32(np.finfo(np.float32).tiny)
@@ -280,20 +280,6 @@ def _edge_rows(signs, dim):
     return EDGE_VALUES[(k[:, None] + np.arange(dim)[None, :]) % len(EDGE_VALUES)]
 
 
-def _pooled(rows, lists, sqrt):
-    """The EW's forward: sum into zeros in f32, x 1/sqrt(max(n, 1)), RNE to f16 (mod.rs:547-579)."""
-    out = np.zeros((len(lists), rows.shape[1]), np.float32)
-    for b, ks in enumerate(lists):
-        acc = np.zeros(rows.shape[1], np.float32)
-        for k in ks:
-            acc = acc + rows[k]
-        if sqrt:
-            acc = acc * (np.float32(1) / np.sqrt(np.float32(max(len(ks), 1))))
-        out[b] = acc
-    with np.errstate(over="ignore"):
-        return out.astype(np.float16)
-
-
 def _seed(torch, oracle, shards, w, signs, dim, R):
     ent = _edge_rows(signs, dim)
     owner = oracle.shard_of(signs, R) if R > 1 else np.zeros(signs.size, np.uint32)
@@ -341,8 +327,8 @@ def test_forward_f16_rounding_edges(torch_cuda, oracle, dim):
                           training=False).cpu().numpy()
         want, _ = w.forward(ids, row_off, B, training=False)
         assert same_bits(got[0], want[0]) and same_bits(got[1], want[1])
-        assert same_bits(got[0], _pooled(rows, [[int(k)] for k in ids1], False))
-        assert same_bits(got[1], _pooled(rows, lists, sqrt))
+        assert same_bits(got[0], pool_lists(rows, [[int(k)] for k in ids1], False))
+        assert same_bits(got[1], pool_lists(rows, lists, sqrt))
         assert np.isposinf(got[0]).any() and not (got[0].view(np.uint16) == 0x8000).any()
     # the raw table: f16(row), -0 kept
     s = SH.EmbeddingShard(dim, 1 << 12, 0)
@@ -381,7 +367,7 @@ def test_forward_f16_rounding_edges(torch_cuda, oracle, dim):
             want, _ = w.forward(batches[r], full_row_off(1, B), B, training=False)
             got = outs[r][0].cpu().numpy()
             assert same_bits(got, want[0]), (rows_f32, r)
-            assert same_bits(got, _pooled(rows, [[int(k)] for k in batches[r]], False)), (rows_f32, r)
+            assert same_bits(got, pool_lists(rows, [[int(k)] for k in batches[r]], False)), (rows_f32, r)
 
 
 # ---- init range -------------------------------------------------------------------------------------------------------

@@ -7,7 +7,8 @@ import os
 import numpy as np
 import pytest
 
-from util import f16_ulp_diff, full_row_off, make_batch, same_bits, to_dev_i32, to_dev_ids
+from util import (f16_ulp_diff, full_row_off, held_rows, make_batch, pool_model, same_bits, slot_signs, to_dev_i32,
+                  to_dev_ids)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -90,8 +91,11 @@ def test_tier_parity_over_churn(torch_cuda, pb, oracle, kind_name, dim, kw):
             got = ctx.forward(s, to_dev_ids(ids, DEV), slot_off, B, row_off=ro_dev, training=True).cpu().numpy()
             ro = row_off if row_off is not None else full_row_off(S, B)
             want, octx = w.forward(ids, ro, B, training=True)
+            signs = slot_signs(oracle, ids, slot_off, pf)  # the forward admits and restores, it steps nothing
+            model = pool_model(held_rows(torch, oracle, [s], signs), signs, row_off, B, None, dim=dim)
             counts = np.diff(ro).reshape(S, B)
             for i in range(S):
+                assert same_bits(got[i], model[i]), step
                 one = counts[i] <= 1  # a sample of several ids may differ by 1 f16 ulp: f32 sum order (test_gpu_parity)
                 np.testing.assert_array_equal(got[i][one].view(np.uint16), want[i][one].view(np.uint16), err_msg=str(step))
                 assert f16_ulp_diff(got[i][~one], want[i][~one]) <= 1, step
@@ -442,6 +446,9 @@ def test_tier_inference_and_direct_update_read_in_place(torch_cuda, pb, oracle):
     ids, row_off, slot_off = make_batch(rng, 1, 300, card, max_ids=4)
     got = ctx.forward(s, to_dev_ids(ids, DEV), slot_off, 300, row_off=to_dev_i32(row_off, DEV), training=False)
     want, _ = w.forward(ids, row_off, 300, training=False)
+    signs = oracle.add_prefix(ids, 8, pf)  # tier-held signs read in place: the model reads them from the tier too
+    model = pool_model(held_rows(torch, oracle, [s], signs), signs, row_off, 300, None, dim=dim)
+    assert same_bits(got.cpu().numpy()[0], model[0])
     assert f16_ulp_diff(got.cpu().numpy()[0], want[0]) <= 1
     # pb_lookup
     signs = oracle.add_prefix(held, 8, pf)
@@ -625,6 +632,13 @@ def test_tier_through_persia_core(torch_cuda, oracle, tmp_path, monkeypatch):
             embs = {t.name: t for t in (e.get_sum_embedding() for e in tb.consume_all_id_type_feature_embedding_tensors())}
             ids, off = csr(user, tags)
             want, octx = w.forward(ids, off, B, training=training)
+            # rows after the forward (it admits and restores, it steps nothing), wherever they live
+            signs = np.concatenate([oracle.add_prefix(np.array(user, np.uint64), 8, by["user"].index_prefix),
+                                    oracle.add_prefix(ids[B:], 8, by["tags"].index_prefix)])
+            torch.cuda.synchronize()
+            ent = ctx.get_entries(signs, 16, missing_ok=True)
+            rows = {int(x): e[:16] for x, e in zip(signs, ent) if e is not None}
+            model = pool_model(rows, signs, off, B, [by["user"].sqrt_scaling, by["tags"].sqrt_scaling], dim=16)
             xs = {}
             for k, n in enumerate(("user", "tags")):
                 t = embs[n]
@@ -634,6 +648,7 @@ def test_tier_through_persia_core(torch_cuda, oracle, tmp_path, monkeypatch):
                     np.testing.assert_array_equal(got.view(np.uint16), want[k].view(np.uint16))
                 else:  # several ids per sample: 1 f16 ulp of f32 sum order (test_gpu_parity)
                     assert f16_ulp_diff(got, want[k]) <= 1
+                assert same_bits(got, model[k]), n
                 xs[n] = (t, x)
             return xs, octx
 

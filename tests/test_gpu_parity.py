@@ -2,14 +2,15 @@
 
 Bar (SURVEY.md §8c): bit-exact for hashes, prefixes, shard ids, partitions, looked-up rows, single-id
 pooled f16 outputs, SGD and (against the oracle's exact-rsqrt mode) Adagrad updates; <= 1 f16 ulp for
-multi-id pooled sums (f32 summation order differs); Adagrad vs the reference's _mm256_rsqrt_ps mode within
-3.7e-4 of the step.
+multi-id pooled sums (f32 summation order differs), which are bit-exact against util.pool_model; Adagrad vs
+the reference's _mm256_rsqrt_ps mode within 3.7e-4 of the step.
 """
 import numpy as np
 import pytest
 
 from util import entries_equal as _entries_equal
-from util import f16_ulp_diff, full_row_off, make_batch, to_dev_i32, to_dev_ids
+from util import (f16_ulp_diff, full_row_off, held_rows, make_batch, pool_model, same_bits, slot_signs, to_dev_i32,
+                  to_dev_ids)
 from util import fwd_both as _fwd_both
 from util import pair as _pair
 from util import train_steps as _train_steps
@@ -283,12 +284,16 @@ def test_forward_multi_id_ragged(torch_cuda, pb, oracle, dim):
     torch = torch_cuda
     rng = np.random.default_rng(dim)
     S, B = 5, 257
-    s, ctx, w, _ = _pair(pb, oracle, S, dim, oracle.ADAGRAD, sqrt=[False, True, False, True, True])
+    sqrt = [False, True, False, True, True]
+    s, ctx, w, pf = _pair(pb, oracle, S, dim, oracle.ADAGRAD, sqrt=sqrt)
     for it in range(4):
         ids, row_off, slot_off = make_batch(rng, S, B, [3, 50, 1000, 100000, 7], max_ids=6, allow_empty=True)
         training = it != 2
         got, want, _ = _fwd_both(torch, s, ctx, w, ids, row_off, slot_off, B, training=training)
+        signs = slot_signs(oracle, ids, slot_off, pf)
+        model = pool_model(held_rows(torch, oracle, [s], signs), signs, row_off, B, sqrt, dim=dim)
         for i in range(S):
+            assert same_bits(got[i], model[i])  # sample order, bit for bit
             assert f16_ulp_diff(got[i], want[i]) <= 1  # f32 sum order differs for multi-id samples
         assert len(s) == w.ps_len(0)
         counts = np.diff(row_off)

@@ -16,7 +16,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-from util import full_row_off, make_batch, to_dev_i32, to_dev_ids  # noqa: E402
+from util import (full_row_off, held_rows, make_batch, pool_model, same_bits, slot_signs, to_dev_i32,  # noqa: E402
+                  to_dev_ids)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -182,12 +183,17 @@ def test_groups_ragged_sqrt_scale(torch_cuda, oracle):
             outs = W.group_forward(ws, [d[0] for d in dev_in], B, training=True, row_offs=[d[1] for d in dev_in],
                                    slot_occ_offs=[b[2] for b in batches], outs=pre)
             torch.cuda.synchronize()
+            # every rank's rows after the forward (it admits, it steps nothing), each from its owner
+            signs = [slot_signs(oracle, b[0], b[2], pf) for b in batches]
+            rows = held_rows(torch, oracle, [x.shard for x in ws], np.concatenate(signs))
             octx = []
             for r in range(R):
                 want, c = w.forward(batches[r][0], batches[r][1], B, training=True)
+                model = pool_model(rows, signs[r], batches[r][1], B, sqrt, dim=dim)
                 octx.append(c)
                 got = outs[r].cpu().numpy()
                 for i in range(S):
+                    assert same_bits(got[i], model[i]), (step, r, i)  # sample order, bit for bit
                     # (a sample's ids are summed in sample order here, in shard order there: one f16 step apart at most)
                     np.testing.assert_allclose(got[i].astype(np.float32), want[i].astype(np.float32), rtol=2e-3, atol=8e-3)
                     seen.update(w.ctx_signs(c, i).tolist())

@@ -117,6 +117,103 @@ def entries_equal(torch, s, w, signs, exact=True, rtol=0.0, atol=0.0):
             np.testing.assert_allclose(ent[k], ref, rtol=rtol, atol=atol)
 
 
+def slot_signs(oracle, ids, slot_off, prefixes, prefix_bit=8):
+    """The signs of slot-major ids: every slot's index prefix added (indices_add_prefix)."""
+    ids = np.asarray(ids, np.uint64)
+    out = np.empty(ids.size, np.uint64)
+    for s, p in enumerate(prefixes):
+        lo, hi = int(slot_off[s]), int(slot_off[s + 1])
+        out[lo:hi] = oracle.add_prefix(ids[lo:hi], prefix_bit, p)
+    return out
+
+
+def held_rows(torch, oracle, shards, signs):
+    """{sign: f32 [dim]} of the signs the table holds now (HBM or tier); with R > 1 shards each sign is read from its
+    owner.  A sign without a row is absent."""
+    signs = np.unique(np.asarray(signs, np.uint64))
+    R, dim = len(shards), shards[0].dim
+    owner = oracle.shard_of(signs, R) if R > 1 else np.zeros(signs.size, np.uint32)
+    rows = {}
+    for r, s in enumerate(shards):
+        mine = signs[owner == r]
+        if not mine.size:
+            continue
+        ent, found = s.get_entries(to_dev_ids(mine, DEV))
+        ent, found = ent.cpu().numpy(), found.cpu().numpy().astype(bool)
+        rows.update((int(x), ent[k, :dim]) for k, x in enumerate(mine) if found[k])
+    return rows
+
+
+def pool_model(rows, ids, row_off, batch, sqrt, dim=None, order="sample", per_row=False, factor=None):
+    """The pooled forward of summation slots (k_gather_items, k_expand_pool), step by step in f32: every output row
+    sums the rows of its sample's signs into +0 in ascending occurrence order, skipping signs without a row; a slot with
+    sqrt scaling then multiplies by f32(1 / f32(sqrt(max(n, 1)))); the result rounds to f16 (RNE).  One-id layouts
+    (row_off None) give f16(0 + row).
+      rows     {sign: f32 [dim]}: what the table held at forward time
+      ids      u64 [N] signs (prefixed), slot-major;  row_off  u32 [S*B+1] or None;  sqrt  per-slot bools or None
+    Variants that the kernels must NOT match (tests use them to show their inputs discriminate):
+      order    "reversed" / "sorted" (by sign) within each sample;  per_row  scale every row before adding it;
+      factor   n (int array) -> f32 sqrt factor, instead of the double-rounded one.
+    Returns f16 [S, B, dim]."""
+    ids = np.asarray(ids, np.uint64)
+    keys = np.array(sorted(rows), np.uint64)
+    if dim is None:
+        dim = len(next(iter(rows.values())))
+    table = np.zeros((keys.size + 1, dim), np.float32)  # the last row stands for "no row" (never added)
+    for k, x in enumerate(keys):
+        table[k] = np.asarray(rows[int(x)], np.float32)[:dim]
+    pos = np.searchsorted(keys, ids)
+    hit = pos < keys.size
+    hit[hit] = keys[pos[hit]] == ids[hit]
+    idx = np.where(hit, pos, keys.size)
+    n_out = ids.size if row_off is None else len(row_off) - 1
+    S = n_out // batch if batch else 0
+    with np.errstate(over="ignore", invalid="ignore"):
+        if row_off is None:
+            return (np.float32(0) + table[idx]).astype(np.float16).reshape(S, batch, dim)
+        ro = np.asarray(row_off, np.int64)
+        cnt = np.diff(ro)
+        sample = np.repeat(np.arange(n_out), cnt)
+        first = ro[:-1][sample]
+        if order == "sample":
+            perm = np.arange(ids.size)
+        elif order == "reversed":
+            perm = 2 * first + cnt[sample] - 1 - np.arange(ids.size)
+        else:
+            assert order == "sorted", order
+            perm = np.lexsort((ids, sample))
+        scale = np.ones(n_out, np.float32)
+        sq = np.repeat(np.asarray(sqrt if sqrt is not None else [False] * S, bool), batch)
+        if sq.any():
+            n = np.maximum(cnt[sq], 1)
+            scale[sq] = factor(n) if factor else np.float32(1) / np.sqrt(n.astype(np.float32))
+        acc = np.zeros((n_out, dim), np.float32)
+        for k in range(int(cnt.max(initial=0))):
+            m = np.flatnonzero(cnt > k)
+            j = perm[ro[m] + k]
+            sel, j = m[hit[j]], j[hit[j]]
+            v = table[idx[j]]
+            acc[sel] = acc[sel] + (v * scale[sel, None] if per_row else v)
+        if not per_row:
+            acc = acc * scale[:, None]
+        return acc.astype(np.float16).reshape(S, batch, dim)
+
+
+def pool_lists(rows, lists, sqrt):
+    """The EW's forward over one slot, in closed form: rows f32 [n, dim], lists the row numbers of every sample; sum into
+    zeros in f32, x 1/sqrt(max(n, 1)), RNE to f16 (mod.rs:547-579)."""
+    out = np.zeros((len(lists), rows.shape[1]), np.float32)
+    for b, ks in enumerate(lists):
+        acc = np.zeros(rows.shape[1], np.float32)
+        for k in ks:
+            acc = acc + rows[k]
+        if sqrt:
+            acc = acc * (np.float32(1) / np.sqrt(np.float32(max(len(ks), 1))))
+        out[b] = acc
+    with np.errstate(over="ignore"):
+        return out.astype(np.float16)
+
+
 def same_bits(a, b):
     """Bit equality of two float arrays, except that NaN matches any NaN (CUDA's canonical NaN and x86's default NaN
     differ in payload and sign)."""
