@@ -620,8 +620,9 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
       skip = slot_dead(dead, slot) || row >= t.capacity;
       if (!slot_dead(dead, slot) && row >= t.capacity && tid == 0 && !a.quiet_miss) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);
     }
-    if (skip) {  // the item's bits must still go back to zero for the next batch
-      if (bm_mode)
+    if (skip) {  // the item's bits must still go back to zero for the next batch, unless a later round reads them
+      const bool other_round = !((a.round_mask[slot >> 5] >> (slot & 31)) & 1u);  // (an earlier one zeroed them already)
+      if (bm_mode && !other_round)
         for (uint32_t w = tid; w < (hi - lo + 31u) / 32u; w += HOT_THREADS) a.b.hot_bits[base + w] = 0u;
       continue;
     }
@@ -691,7 +692,11 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
         }
         __syncthreads();
         const uint32_t nwin = s_nwin;
-        const uint32_t n_chunks = (nwin + g.R - 1u) / g.R;
+        // rows per chunk: a chunk is one producer warp's, so a window that does not give every producer a chunk of R
+        // rows is cut into chunks of one or two parts, all loaded at once by different warps (one load round trip
+        // before the chain starts instead of two).  The slots keep their place in the ring (R rows apart).
+        const uint32_t cr = nwin <= PW * g.R1 ? g.R1 : (2u * g.R1 <= g.R && nwin <= 2u * PW * g.R1 ? 2u * g.R1 : g.R);
+        const uint32_t n_chunks = (nwin + cr - 1u) / cr;
         if (trace && tid == 0) trace[8 * h + 1] = globaltimer_ns();
         if (warp >= CH) {
           // ---- producers: chunk c belongs to warp CH + (it % PW)
@@ -702,9 +707,9 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
           // a chunk is one or two halves of R1 rows; a producer has both halves' loads in flight before it converts
           for (uint32_t c = me < PW ? (me + PW - it % PW) % PW : n_chunks; c < n_chunks; c += PW) {  // (warps past PW idle)
             const uint32_t i = it + c, stage = i % g.S, par = (i / g.S) & 1u;
-            const uint32_t nv = min(g.R, nwin - c * g.R);
+            const uint32_t nv = min(cr, nwin - c * cr);
             float* slotp = ring + (size_t)stage * g.R * g.stride;
-            const uint16_t* srt = sorted + c * g.R;
+            const uint16_t* srt = sorted + c * cr;
             if (lean) {
               // the chunk's parts of R1 rows ping-pong between two register sets: part k + 2 is loaded as soon as part k has
               // been converted, so two parts' loads are always in flight
@@ -722,7 +727,7 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
             } else {
               if (!failed && !mbar_wait(empty0 + 8u * stage, par ^ 1u)) failed = true;
               for (uint32_t r0 = 0; r0 < nv; r0 += g.R1)
-                produce_chunk<F16>(slotp + (size_t)r0 * g.stride, g, src, a, sorted, c * g.R + r0, min(g.R1, nv - r0), wbase, col0, t.dim, lane);
+                produce_chunk<F16>(slotp + (size_t)r0 * g.stride, g, src, a, sorted, c * cr + r0, min(g.R1, nv - r0), wbase, col0, t.dim, lane);
             }
             mbar_arrive(full0 + 8u * stage);
           }
@@ -731,20 +736,20 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
           long long tw = 0, ta = 0;
           for (uint32_t c = 0; c < n_chunks; ++c) {
             const uint32_t i = it + c;
-            const uint32_t nv = min(g.R, nwin - c * g.R), stage = i % g.S, par = (i / g.S) & 1u;
+            const uint32_t nv = min(cr, nwin - c * cr), stage = i % g.S, par = (i / g.S) & 1u;
             const long long c0 = trace ? clock64() : 0;
             if (!failed && !mbar_wait(full0 + 8u * stage, par)) failed = true;
             if (trace) { const long long c1 = clock64(); tw += c1 - c0; ta -= c1; }
             if (own) {
               const float* rp = ring + (size_t)stage * g.R * g.stride + (e0 - col0);
-              if (nv == g.R && g.R == 64u) {  // whole chunk: straight-line blocks
+              if (nv == cr && cr == 64u) {  // whole chunk: straight-line blocks
                 chain_block<EPL, 32>(acc, rp, g.stride);
                 chain_block<EPL, 32>(acc, rp + (size_t)32u * g.stride, g.stride);
-              } else if (nv == g.R && g.R == 32u) {
+              } else if (nv == cr && cr == 32u) {
                 chain_block<EPL, 32>(acc, rp, g.stride);
-              } else if (nv == g.R && g.R == 16u) {
+              } else if (nv == cr && cr == 16u) {
                 chain_block<EPL, 16>(acc, rp, g.stride);
-              } else if (nv == g.R && g.R == 8u) {
+              } else if (nv == cr && cr == 8u) {
                 chain_block<EPL, 8>(acc, rp, g.stride);
               } else {  // the item's last chunk (the producer padded it with zero rows to a multiple of four)
                 for (uint32_t r = 0; r < nv; r += 4) chain_block<EPL, 4>(acc, rp + (size_t)r * g.stride, g.stride);
@@ -853,9 +858,9 @@ static void hot_launch(const TableDev& t, const OptimDev& op, const HyperDev& hy
   if (vec && g.R * nvr > 256u) g.vec = 0;  // (rows longer than 64 vectors per pass: element by element)
   g.lean = g.vec && g.vshift <= 5u && t.dim <= HOT_COLS && !a.occ_outrow;
   // every chunk costs the chain a barrier round trip (~500 cycles measured) whatever its size: up to 64 rows per chunk
-  // (parts of R1 rows) where the slot stays within 32 KB
+  // (parts of R1 rows) where the slot stays within 32 KB; the producers' lean loop converts at most four parts
   g.R1 = g.R;
-  while (g.R < 64u && 2u * g.R * g.stride * 4u <= 32768u) g.R *= 2u;
+  while (g.R < 64u && g.R < 4u * g.R1 && 2u * g.R * g.stride * 4u <= 32768u) g.R *= 2u;
   if (g.R * g.stride * 4u > 16384u) g.S = 6;  // 6 x 32 KB (the producers must not outnumber the slots)
   const size_t smem = (size_t)g.S * g.R * g.stride * 4u + (((size_t)t.dim + 3u) & ~(size_t)3u) * 4u;
   auto kern = k_reduce_hot<EPL, F16, SEND>;
