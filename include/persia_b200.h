@@ -120,7 +120,15 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream);
  * number: the union evicts least recently used first, and pb_table_export_signs of both tables merges into the
  * reference's list order.
  * pb_table_clear of the table clears its tier too.  Destroy the table before its tier.  The sharded calls refuse a
- * table with a tier. */
+ * table with a tier.
+ *
+ * Staging (pb_tier_stage): the ids of batch i+1 are known while batch i trains, and moving an entry never changes its
+ * value, so the moves of request i+1 can run one batch ahead, on a stream of their own, beside batch i's dense step and
+ * backward.  The library orders a stage: it starts after every earlier call on the table (pending backwards included),
+ * and every later call on the table or its tier except pb_backward and pb_backward_raw (which run beside it) starts
+ * after it.  In a CUDA graph, a stage and the calls after it work when they are captured into one graph, the stage on
+ * a stream forked from the capturing one; a call captured after a stage issued outside the capture that has not
+ * completed fails with PB_ERR_STATE (synchronise before capturing). */
 int pb_table_create_host(int device, const pb_table_cfg* cfg, pb_table** out);
 /* Both tables need their optimizer registered; checks dim, optimizer kind and row stride. */
 int pb_table_attach_tier(pb_table* t, pb_table* tier);
@@ -128,6 +136,21 @@ int pb_table_attach_tier(pb_table* t, pb_table* tier);
  * restored into HBM, [3] entries dropped: by its own sweep, or because neither table had a row for them (an eviction
  * victim or a pb_set_rows entry), [4] training restores refused for want of a free HBM row.  Synchronises `stream`. */
 int pb_tier_stats(pb_table* t, uint64_t h_out[5], void* stream);
+/* Moves the host-tier traffic of an upcoming training request off its critical path: the eviction check that request
+ * would run (victims out to the tier), then every sign of d_ids the HBM table lacks and its tier holds back into a
+ * free HBM row.  Values never change; only where entries live.  No tier: does nothing.
+ * d_ids, h_slot_occ_off, h_prefix, n_slots and prefix_bit as pb_add_prefix: raw slot ids (hash-stacked where a slot
+ * hash-stacks), prefixed here by slot (prefix 0 = taken as they are).  The check runs whenever the table has an
+ * eviction policy, gated on low water as always, with keep = max(keep_batches, pending batches + 1); it does not count
+ * as one of the request's every-`check_every` calls.  A staged row gets the current batch number (age 0: any check
+ * before the request keeps it).  A sign that finds no free HBM row stays in the tier for the request's own restore.
+ * Never admits a sign, never refreshes an HBM-resident one.  Runs on a fixed, small grid (it shares the GPU). */
+int pb_tier_stage(pb_table* t, const uint64_t* d_ids, uint32_t n, const uint32_t* h_slot_occ_off,
+                  const uint64_t* h_prefix, uint32_t n_slots, uint32_t prefix_bit, void* stream);
+/* [0] signs moved into HBM by stages (also counted in pb_tier_stats[2]), [1] stage restores skipped for want of a
+ * free HBM row (left to the request's own restore; NOT counted in pb_tier_stats[4]).  Since creation / clear; zeros
+ * without a tier.  Synchronises `stream`. */
+int pb_tier_stage_stats(pb_table* t, uint64_t h_out[2], void* stream);
 /* Diagnostic: the state of the hash index's n_cells normal cells (the three cells reserved for the marker-valued signs
  * are not counted): [0] live (a resident sign), [1] tombstones (an evicted sign), [2] EMPTY.  An admission needs an
  * EMPTY cell on its probe path; every eviction check rebuilds the index (tombstones dropped) once fewer than 1/8 of the

@@ -63,6 +63,21 @@ float uniform_scale(float lo, float hi) {
   return scale;
 }
 
+// an event recorded on a caller's stream, and the stream capture it was recorded into (0 = none: a real record)
+struct Mark {
+  cudaEvent_t ev = nullptr;
+  unsigned long long capture = 0;
+  bool set = false;
+};
+
+// Grid of pb_tier_stage's kernels: they run beside the backward and the dense step of the batch before, so they take a
+// fixed share of the GPU rather than the usual grids (8 blocks per SM for the index scans).  One block per SM: measured
+// on an H100 with scripts/host_tier_bench.py (DESIGN.md §4 "Staging"), a step with the stage on 8, 16, 32, 64 and 132
+// blocks took 6.49, 3.97, 2.93, 2.58 and 2.43 ms beside a 1.06 ms dense stand-in: the stage's eviction check moves
+// ~45k entries out per step, and fewer blocks leave too few copies in flight to keep PCIe busy, so the stage outlasts
+// the dense step and the backward and delays the next forward.
+uint32_t g_stage_blocks = PB_NUM_SMS;
+
 }  // namespace
 
 struct pb_table {
@@ -95,6 +110,9 @@ struct pb_table {
   pb_table* tier = nullptr;
   pb_table* tier_of = nullptr;
   uint32_t* move_cells = nullptr;  // the eviction check's victim list (with rebuild_keys / rebuild_rows), `capacity` words
+  // ordering around pb_tier_stage (a table with a tier): `last` is recorded after every call on the table, `staged`
+  // after every stage
+  Mark last, staged;
 };
 
 struct pb_ctx {
@@ -201,10 +219,9 @@ int ensure_evict_ws(pb_table* t) {
   return PB_OK;
 }
 
-// Between two training requests: release the least recently used rows when free storage runs low, and rebuild the
-// index when its EMPTY cells run short.
-int maybe_evict(pb_table* t, cudaStream_t st) {
-  if (!t->evict_every || (++t->train_calls % t->evict_every)) return PB_OK;
+// The eviction check: release the least recently used rows when free storage runs low, and rebuild the index when its
+// EMPTY cells run short.  blocks: grid of its scans (0 = the usual; pb_tier_stage's is small).
+int evict_check(pb_table* t, cudaStream_t st, uint32_t blocks = 0) {
   int rc = ensure_evict_ws(t);
   if (rc) return rc;
   // rows of batches whose gradients are still to come are never released: a row used by a pending batch was
@@ -213,12 +230,98 @@ int maybe_evict(pb_table* t, cudaStream_t st) {
   if (t->tier) {  // the victims move into the tier
     pb_table* h = t->tier;
     launch_evict_tier(t->d, h->d, t->hy, t->op, t->evict_low, t->evict_target, keep, t->evict_ws, t->rebuild_keys,
-                      t->rebuild_rows, h->evict_ws, h->rebuild_keys, h->rebuild_rows, t->move_cells, st);
+                      t->rebuild_rows, h->evict_ws, h->rebuild_keys, h->rebuild_rows, t->move_cells, st, blocks);
     return PB_OK;
   }
   launch_evict(t->d, t->evict_low, t->evict_target, keep, t->evict_ws, t->rebuild_keys, t->rebuild_rows, st);
   return PB_OK;
 }
+
+// between two training requests: every `evict_every`-th one runs the check
+int maybe_evict(pb_table* t, cudaStream_t st) {
+  if (!t->evict_every || (++t->train_calls % t->evict_every)) return PB_OK;
+  return evict_check(t, st);
+}
+
+// ---- ordering around pb_tier_stage ---------------------------------------------------------------------------------
+// A stage runs on a stream of the caller's choosing, beside the backward of the batch before.  The library orders it:
+// the stage waits for all earlier work on the table (Mark `last`), and every later call but the backwards waits for
+// the stage (Mark `staged`).  Waiting on a completed event costs nothing.
+// Stream capture (CUDA 12.9): a capturing stream may wait only on an event recorded into the same capture (a fork/join
+// inside the graph).  Waiting on an event recorded outside it is invalid without cudaEventWaitExternal, and that flag
+// would make every replay wait on whatever the event's latest record is by then: not the dependency meant here.  So an
+// event recorded outside the capture is queried instead: complete, there is nothing to wait for; still running, the
+// call fails with PB_ERR_STATE rather than record a dependency it cannot keep.  The query runs under
+// cudaThreadExchangeStreamCaptureMode(relaxed): a global-mode capture forbids it otherwise; querying an event recorded
+// inside a capture stays forbidden, and is never done.  A mark recorded into another capture is part of that graph,
+// whose launches the caller orders: nothing is waited for.
+
+// the table whose marks a call on `t` uses (a tier's own calls, export and index statistics, use its table's), or
+// null: no tier, no stage, nothing to order
+pb_table* marks_of(pb_table* t) {
+  pb_table* o = t->tier_of ? t->tier_of : t;
+  return o->tier ? o : nullptr;
+}
+
+cudaError_t capture_id(cudaStream_t st, unsigned long long& id) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  id = 0;
+  const cudaError_t e = cudaStreamGetCaptureInfo(st, &cs, &id);
+  if (cs != cudaStreamCaptureStatusActive) id = 0;
+  return e;
+}
+
+int record(Mark& m, cudaStream_t st) {
+  PB_CUDA(capture_id(st, m.capture));
+  PB_CUDA(cudaEventRecord(m.ev, st));
+  m.set = true;
+  return PB_OK;
+}
+
+// `st` waits for the work behind `m`
+int wait_for(const Mark& m, cudaStream_t st) {
+  if (!m.set) return PB_OK;
+  unsigned long long cap = 0;
+  PB_CUDA(capture_id(st, cap));
+  if (m.capture) {  // recorded into a capture: a dependency inside that graph only
+    if (m.capture == cap) PB_CUDA(cudaStreamWaitEvent(st, m.ev, 0));
+    return PB_OK;
+  }
+  if (!cap) {
+    PB_CUDA(cudaStreamWaitEvent(st, m.ev, 0));
+    return PB_OK;
+  }
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  PB_CUDA(cudaThreadExchangeStreamCaptureMode(&mode));
+  const cudaError_t q = cudaEventQuery(m.ev);
+  cudaThreadExchangeStreamCaptureMode(&mode);
+  if (q == cudaSuccess) return PB_OK;
+  if (q == cudaErrorNotReady)
+    return fail(PB_ERR_STATE, "a pb_tier_stage (or a call before one) issued outside this stream capture has not "
+                              "completed: synchronise before capturing, or capture the stage too");
+  return fail(PB_ERR_CUDA, std::string("cudaEventQuery: ") + cudaGetErrorString(q));
+}
+
+// One call on a table: begin() makes `st` wait for the latest stage (not for the backwards, which run beside one), and
+// the call is recorded as the table's latest work when it returns.  Does nothing for a table without a tier.
+struct TableCall {
+  pb_table* m = nullptr;
+  cudaStream_t st = nullptr;
+  int begin(pb_table* t, cudaStream_t s, bool after_stage = true) {
+    pb_table* o = marks_of(t);
+    if (!o) return PB_OK;
+    if (after_stage) {
+      const int rc = wait_for(o->staged, s);
+      if (rc) return rc;
+    }
+    m = o;
+    st = s;
+    return PB_OK;
+  }
+  ~TableCall() {
+    if (m) record(m->last, st);
+  }
+};
 
 // signs the HBM table lacks and its tier holds are moved back into HBM rows before they are probed
 void restore_ids(pb_table* t, bool prefix, const SlotsDev& sl, const uint64_t* ids, uint32_t n, cudaStream_t st) {
@@ -346,6 +449,8 @@ int pb_table_attach_tier(pb_table* t, pb_table* tier) {
   if (t->d.stride != tier->d.stride) return fail(PB_ERR_INVALID, "the tier's row stride differs from the table's");
   if ((rc = ensure_evict_ws(t)) || (rc = ensure_evict_ws(tier))) return rc;
   PB_CUDA(cudaMalloc(&t->move_cells, sizeof(uint32_t) * (size_t)t->d.capacity));
+  PB_CUDA(cudaEventCreateWithFlags(&t->last.ev, cudaEventDisableTiming));
+  PB_CUDA(cudaEventCreateWithFlags(&t->staged.ev, cudaEventDisableTiming));
   t->tier = tier;
   tier->tier_of = t;
   return PB_OK;
@@ -356,6 +461,8 @@ int pb_tier_stats(pb_table* t, uint64_t h_out[5], void* stream) {
   for (int i = 0; i < 5; ++i) h_out[i] = 0;
   if (!t->tier) return PB_OK;
   DeviceGuard g(t->device);
+  TableCall call;
+  if (int rc = call.begin(t, (cudaStream_t)stream)) return rc;
   uint32_t c[CTR_COUNT];
   PB_CUDA(cudaMemcpyAsync(c, t->tier->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
@@ -367,12 +474,65 @@ int pb_tier_stats(pb_table* t, uint64_t h_out[5], void* stream) {
   return PB_OK;
 }
 
+int pb_tier_stage(pb_table* t, const uint64_t* d_ids, uint32_t n, const uint32_t* h_slot_occ_off, const uint64_t* h_prefix,
+                  uint32_t n_slots, uint32_t prefix_bit, void* stream) {
+  if (!t || (n && !d_ids) || !h_slot_occ_off || !h_prefix) return fail(PB_ERR_INVALID, "null argument");
+  if (t->tier_of) return fail(PB_ERR_STATE, "a host tier is not staged directly: use the table it is attached to");
+  if (n_slots == 0 || n_slots > PB_MAX_SLOTS) return fail(PB_ERR_INVALID, "n_slots must be in 1..PB_MAX_SLOTS");
+  if (prefix_bit == 0 || prefix_bit > 63) return fail(PB_ERR_INVALID, "feature_index_prefix_bit must be in 1..63");
+  if (h_slot_occ_off[0] != 0 || h_slot_occ_off[n_slots] != n) return fail(PB_ERR_INVALID, "slot offsets do not span the id array");
+  for (uint32_t s = 0; s < n_slots; ++s)
+    if (h_slot_occ_off[s] > h_slot_occ_off[s + 1]) return fail(PB_ERR_INVALID, "slot offsets must ascend");
+  if (!t->tier) return PB_OK;  // nothing to move
+  int rc = ready_for_training(t);
+  if (rc) return rc;
+  pb_slots_cfg cfg;
+  std::memset(&cfg, 0, sizeof(cfg));
+  cfg.n_slots = n_slots;
+  cfg.prefix_bit = prefix_bit;
+  for (uint32_t i = 0; i < n_slots; ++i) cfg.prefix[i] = h_prefix[i];
+  SlotsDev sl;
+  if ((rc = make_slots(cfg, h_slot_occ_off, sl))) return rc;
+  DeviceGuard g(t->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  // Every earlier call on the table first (enqueued backwards included); every later call but the backwards waits for
+  // this stage.  Why it may run beside a backward: no backward kernel reads index cells, the free-row stack or
+  // row_tick (the only index read outside the forward path is k_raw_table's, in the raw forward, which waits), and a
+  // backward writes only the rows of its own batch, which are never victims here (keep > pending_batches) nor restore
+  // targets (those come off the free stack).  Counters it shares with a backward are updated atomically.
+  if ((rc = wait_for(t->last, st))) return rc;
+  // the check the request would run (not counted in train_calls, so the request's own stays where it was: after a
+  // stage it usually finds enough free rows and does nothing); keep covers the batches pending now
+  if (t->evict_every && (rc = evict_check(t, st, g_stage_blocks))) return rc;
+  launch_tier_stage(t->d, t->tier->d, t->hy, t->op, sl, d_ids, n, g_stage_blocks, st);
+  PB_CUDA(cudaGetLastError());
+  if ((rc = record(t->staged, st))) return rc;
+  return record(t->last, st);
+}
+
+int pb_tier_stage_stats(pb_table* t, uint64_t h_out[2], void* stream) {
+  if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
+  h_out[0] = h_out[1] = 0;
+  if (!t->tier) return PB_OK;
+  DeviceGuard g(t->device);
+  TableCall call;
+  if (int rc = call.begin(t, (cudaStream_t)stream)) return rc;
+  uint32_t c[CTR_COUNT];
+  PB_CUDA(cudaMemcpyAsync(c, t->tier->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  h_out[0] = c[CTR_STAGE_IN];
+  h_out[1] = c[CTR_STAGE_SKIP];
+  return PB_OK;
+}
+
 int pb_table_destroy(pb_table* t) {
   if (!t) return PB_OK;
   DeviceGuard g(t->device);
   if (t->tier) t->tier->tier_of = nullptr;
   if (t->tier_of) t->tier_of->tier = nullptr;
   if (t->move_cells) cudaFree(t->move_cells);
+  if (t->last.ev) cudaEventDestroy(t->last.ev);
+  if (t->staged.ev) cudaEventDestroy(t->staged.ev);
   if (t->allocated) {
     cudaDeviceSynchronize();
     cudaFree(t->d.cells);
@@ -451,6 +611,8 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream) {
   h_out[0] = h_out[1] = h_out[2] = h_out[3] = h_out[4] = 0;
   if (!t->allocated) return PB_OK;
   DeviceGuard g(t->device);
+  TableCall call;
+  if (int rc = call.begin(t, (cudaStream_t)stream)) return rc;
   uint32_t c[CTR_COUNT];
   PB_CUDA(cudaMemcpyAsync(c, t->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
@@ -468,6 +630,8 @@ int pb_table_index_stats(pb_table* t, uint64_t h_out[3], void* stream) {
   if (!t->allocated) return PB_OK;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if (int rc = call.begin(t, st)) return rc;
   if (!t->stats_ws) PB_CUDA(cudaMalloc(&t->stats_ws, 3 * sizeof(uint32_t)));
   launch_index_stats(t->d, t->stats_ws, st);
   uint32_t c[3];
@@ -491,6 +655,8 @@ int pb_table_clear(pb_table* t, void* stream) {
   if (!t->allocated) return PB_OK;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if (int rc = call.begin(t, st)) return rc;
   launch_fill_cells(t->d.cells, (uint64_t)t->d.n_cells + N_SPECIAL, st);
   PB_CUDA(cudaMemsetAsync(t->d.counters, 0, sizeof(uint32_t) * CTR_COUNT, st));
   PB_CUDA(cudaMemsetAsync(t->d.row_tick, 0, sizeof(uint32_t) * (size_t)t->d.capacity, st));
@@ -509,6 +675,8 @@ int pb_lookup(pb_table* t, const uint64_t* d_signs, uint32_t n, int training, fl
   }
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if (int rc = call.begin(t, st)) return rc;
   int rc = ensure_alloc(t);
   if (rc) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
@@ -535,6 +703,8 @@ int pb_update(pb_table* t, const uint64_t* d_signs, const float* d_grads, uint32
   if (rc) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if ((rc = call.begin(t, st))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
   SlotsDev sl = no_slots();
@@ -562,6 +732,8 @@ int pb_set_rows(pb_table* t, const uint64_t* d_signs, const float* d_entries, ui
   if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered: entry length unknown");
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if (int rc = call.begin(t, st)) return rc;
   int rc = ensure_alloc(t);
   if (rc) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
@@ -581,6 +753,8 @@ int pb_get_rows(pb_table* t, const uint64_t* d_signs, uint32_t n, float* d_entri
   if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered: entry length unknown");
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if (int rc = call.begin(t, st)) return rc;
   int rc = ensure_alloc(t);
   if (rc) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
@@ -598,6 +772,8 @@ int pb_table_export_signs(pb_table* t, uint64_t* d_signs, uint32_t* d_recency, u
   if (!t || !d_count || (max_n && (!d_signs || !d_recency))) return fail(PB_ERR_INVALID, "null argument");
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if (int rc = call.begin(t, st)) return rc;
   if (!t->allocated) {
     PB_CUDA(cudaMemsetAsync(d_count, 0, sizeof(uint32_t), st));
     return PB_OK;
@@ -800,6 +976,8 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   }
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if ((rc = call.begin(t, st))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
@@ -857,6 +1035,8 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
   if ((rc = check_grads_aligned(h_grads, S))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;  // runs beside a pb_tier_stage (see there): waits for none
+  if ((rc = call.begin(t, st, false))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, c->occ_off, sl))) return rc;
   GradsDev gr;
@@ -1289,6 +1469,8 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   }
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if ((rc = call.begin(t, st))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_raw(c))) return rc;
   if (training && (rc = ensure_raw_stage(c, t->d.dim, st))) return rc;
@@ -1337,6 +1519,8 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
   if (rc) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;  // runs beside a pb_tier_stage (see there): waits for none
+  if ((rc = call.begin(t, st, false))) return rc;
   drop_raw_pending(c);  // enqueued below: the sweep of the next training call runs after these gradients
   GradsDev gr;
   std::memset(&gr, 0, sizeof(gr));
@@ -1492,3 +1676,5 @@ int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_gr
 // debugging aid (not in include/persia_b200.h): device buffer of 4 u64 per hot item that k_reduce_hot stamps
 namespace pb { void set_hot_trace(unsigned long long* p); }
 extern "C" void pb_debug_hot_trace(void* d_buf) { pb::set_hot_trace(reinterpret_cast<unsigned long long*>(d_buf)); }
+// measuring aid (not in include/persia_b200.h): pb_tier_stage's grid (scripts/host_tier_bench.py --stage-blocks)
+extern "C" void pb_debug_stage_blocks(uint32_t blocks) { g_stage_blocks = blocks ? blocks : PB_NUM_SMS; }

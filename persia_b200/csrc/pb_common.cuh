@@ -94,6 +94,8 @@ enum {
   CTR_TIER_IN = 11,       // entries restored into the HBM table (their tier rows are free again)
   CTR_TIER_REFUSED = 12,  // restores that found no free HBM row (the entry stayed in the tier)
   CTR_TIER_LOST = 13,     // victims of an HBM sweep that found no tier row (dropped, like a plain sweep's)
+  CTR_STAGE_IN = 14,      // of CTR_TIER_IN: restores made by pb_tier_stage
+  CTR_STAGE_SKIP = 15,    // pb_tier_stage restores that found no free HBM row (left to the request's own restore)
   CTR_COUNT = 16
 };
 

@@ -286,11 +286,12 @@ __global__ void __launch_bounds__(256) k_index_stats(TableDev t, uint32_t* __res
 // ------------------------------------------------------------------------------------------------
 // launchers (host)
 // ------------------------------------------------------------------------------------------------
-void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st) {
+void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st, uint32_t blocks) {
+  const uint32_t g = blocks ? blocks : PB_NUM_SMS * 8;
   PB_LAUNCH(k_rebuild_plan, 1, 32, 0, st, t, ev);
-  PB_LAUNCH(k_rebuild_compact, PB_NUM_SMS * 8, 256, 0, st, t, ev, keys, rows);
-  PB_LAUNCH(k_rebuild_clear, PB_NUM_SMS * 8, 256, 0, st, t, ev);
-  PB_LAUNCH(k_rebuild_insert, PB_NUM_SMS * 8, 256, 0, st, t, ev, keys, rows);
+  PB_LAUNCH(k_rebuild_compact, g, 256, 0, st, t, ev, keys, rows);
+  PB_LAUNCH(k_rebuild_clear, g, 256, 0, st, t, ev);
+  PB_LAUNCH(k_rebuild_insert, g, 256, 0, st, t, ev, keys, rows);
 }
 
 void launch_index_stats(const TableDev& t, uint32_t* out, cudaStream_t st) {
@@ -388,17 +389,18 @@ void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, u
 // of being swept.  Every step reads its sizes from the device: no host sync, a captured step stays capturable.
 void launch_evict_tier(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, uint32_t low_water,
                        uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys, uint32_t* rb_rows, uint32_t* tev,
-                       uint64_t* trb_keys, uint32_t* trb_rows, uint32_t* move_cells, cudaStream_t st) {
+                       uint64_t* trb_keys, uint32_t* trb_rows, uint32_t* move_cells, cudaStream_t st, uint32_t blocks) {
+  const uint32_t g = blocks ? blocks : PB_NUM_SMS * 8;
   PB_LAUNCH(k_evict_plan, 1, 256, 0, st, h, low_water, target_free, ev);
-  PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, h, ev);
+  PB_LAUNCH(k_evict_hist, g, 256, 0, st, h, ev);
   PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
   launch_tier_plan(h, t, ev, tev, st);
-  PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, t, tev);
+  PB_LAUNCH(k_evict_hist, g, 256, 0, st, t, tev);
   PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, 0u, tev);  // no batch holds a tier row: only the current batch number's stay
-  PB_LAUNCH(k_evict_sweep, PB_NUM_SMS * 8, 256, 0, st, t, tev);
-  launch_tier_move(h, t, hy, op, ev, tev, rb_keys, rb_rows, move_cells, st);  // (the rebuild buffers are free until below)
-  launch_rebuild(h, ev, rb_keys, rb_rows, st);
-  launch_rebuild(t, tev, trb_keys, trb_rows, st);
+  PB_LAUNCH(k_evict_sweep, g, 256, 0, st, t, tev);
+  launch_tier_move(h, t, hy, op, ev, tev, rb_keys, rb_rows, move_cells, st, blocks);  // (rebuild buffers free until below)
+  launch_rebuild(h, ev, rb_keys, rb_rows, st, blocks);
+  launch_rebuild(t, tev, trb_keys, trb_rows, st, blocks);
 }
 
 void launch_shard_of(const uint64_t* signs, uint32_t n, uint32_t R, uint32_t* shard, uint64_t* hash, cudaStream_t st) {

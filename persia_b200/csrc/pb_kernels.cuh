@@ -253,10 +253,15 @@ void launch_index_stats(const TableDev& t, uint32_t* out, cudaStream_t st);
 // move_cells: `h.capacity` words.
 void launch_evict_tier(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, uint32_t low_water,
                        uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys, uint32_t* rb_rows, uint32_t* tev,
-                       uint64_t* trb_keys, uint32_t* trb_rows, uint32_t* move_cells, cudaStream_t st);
+                       uint64_t* trb_keys, uint32_t* trb_rows, uint32_t* move_cells, cudaStream_t st,
+                       uint32_t blocks = 0);  // blocks: grid of the scans and moves (0 = their usual multiple of the SMs)
 void launch_tier_plan(const TableDev& h, const TableDev& t, const uint32_t* ev, uint32_t* tev, cudaStream_t st);
 void launch_tier_move(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const uint32_t* ev,
-                      uint32_t* tev, uint64_t* keys, uint32_t* rows, uint32_t* cells, cudaStream_t st);
+                      uint32_t* tev, uint64_t* keys, uint32_t* rows, uint32_t* cells, cudaStream_t st, uint32_t blocks = 0);
+// pb_tier_stage: restores of an upcoming request's signs (slot-prefixed), on `blocks` blocks; a moved row gets the current
+// batch number, a sign that finds no free HBM row stays in the tier (counted as a skipped stage)
+void launch_tier_stage(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const SlotsDev& sl,
+                       const uint64_t* ids, uint32_t n, uint32_t blocks, cudaStream_t st);
 // before a probe: every sign the HBM index lacks and the tier holds is moved into a free HBM row (flat ids, prefixed by
 // slot when `prefix`; or the distinct items of a batch)
 void launch_tier_restore(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const SlotsDev& sl,
@@ -280,7 +285,7 @@ void launch_tier_where(const TableDev& h, const TableDev& t, const uint64_t* sig
 // pb_set_rows: entries the HBM table had no row for are stored in the tier
 void launch_tier_set(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const uint64_t* signs,
                      const uint32_t* occ_cell, uint32_t n, const float* entries, cudaStream_t st);
-void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st);
+void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st, uint32_t blocks = 0);
 uint64_t launch_count();
 enum { FAM_PROBE = 0, FAM_DEDUP, FAM_GATHER, FAM_NAN, FAM_HOT, FAM_UPDATE, FAM_OTHER, FAM_WARM, FAM_WAIT, FAM_ROUTE, FAM_OWNER, FAM_COUNT };
 bool profiling();  // a kernel family is being timed: the backward then runs its kernels one after another

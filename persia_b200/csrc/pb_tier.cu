@@ -10,8 +10,13 @@
 //            gets a row from the HBM free pool, its entry is copied back and published (MODE_MOVE), the tier row is freed
 //   in place inference lookups, pb_update and pb_get_rows read (or step) tier-held rows where they are: nothing moves,
 //            so they never depend on free HBM rows
-// A moved entry keeps its row_tick, and the tier ages its rows by the HBM table's batch number: the union of the two
-// tables evicts least recently used first, at batch granularity.  A sign lives in at most one of the two tables.
+//   stage    pb_tier_stage, one batch ahead on a stream of its own: the eviction check the next training request would
+//            run, then the restores of its signs, so that request finds them in HBM and its own check and restore have
+//            (usually) nothing left to do.  A staged row is stamped with the current batch number (age 0), so the next
+//            check keeps it; a stage that finds no free row leaves the entry in the tier for the request's own restore.
+// A moved entry keeps its row_tick (a staged restore excepted), and the tier ages its rows by the HBM table's batch
+// number: the union of the two tables evicts least recently used first, at batch granularity.  A sign lives in at most
+// one of the two tables.
 #include "pb_probe.cuh"
 
 namespace pb {
@@ -38,6 +43,9 @@ __device__ __forceinline__ void free_row(const TableDev& t, uint32_t cell, uint3
 // 32 lanes of a warp.  Duplicates of a sign in one launch: the group whose CAS turns the tier cell into a tombstone
 // restores it, the others leave it (the probe that follows finds it in HBM).  No free HBM row: the tier cell gets its
 // sign back, the entry stays where it is and the refusal is counted; the probe's admission then finds no row either.
+// STAGE (pb_tier_stage): the moved row is stamped with the current batch number instead of keeping its tier recency (age
+// 0: the next check keeps it), and a want of free rows is counted as a skipped stage, not as a refused restore.
+template <bool STAGE>
 __device__ __forceinline__ void restore_group(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op,
                                               uint64_t sign, bool valid, uint32_t tick, uint32_t sub, uint32_t gshift) {
   const ProbeOut in_hbm = probe_group<MODE_FIND>(h, hy, op, sign, valid, tick, sub, gshift);
@@ -55,18 +63,19 @@ __device__ __forceinline__ void restore_group(const TableDev& h, const TableDev&
   if (to.row == ROW_NONE) {
     if (sub == 0) {
       *reinterpret_cast<volatile unsigned long long*>(&t.cells[in_tier.cell].key) = stored;
-      atomicAdd(&t.counters[CTR_TIER_REFUSED], 1u);
+      atomicAdd(&t.counters[STAGE ? CTR_STAGE_SKIP : CTR_TIER_REFUSED], 1u);
     }
     return;
   }
   copy_entry(h.rows + (size_t)to.row * h.stride, t.rows + (size_t)in_tier.row * t.stride, h.stride, sub);
-  if (sub == 0) h.row_tick[to.row] = t.row_tick[in_tier.row];
+  if (sub == 0) h.row_tick[to.row] = STAGE ? tick : t.row_tick[in_tier.row];
   __threadfence();
   __syncwarp(0xFFu << gshift);
   if (sub == 0) {
     *reinterpret_cast<volatile uint32_t*>(&h.cells[to.cell].row) = to.row;  // published: the entry is complete
     free_row(t, in_tier.cell, in_tier.row, true);  // (the CAS above tombstoned the tier cell)
     atomicAdd(&t.counters[CTR_TIER_IN], 1u);
+    if (STAGE) atomicAdd(&t.counters[CTR_STAGE_IN], 1u);
   }
 }
 
@@ -89,7 +98,30 @@ __global__ void __launch_bounds__(256) k_tier_restore(TableDev h, TableDev t, Hy
     }
   }
   sign = __shfl_sync(0xffffffffu, sign, gshift);
-  restore_group(h, t, hy, op, sign, valid, tick, sub, gshift);
+  restore_group<false>(h, t, hy, op, sign, valid, tick, sub, gshift);
+}
+
+// pb_tier_stage: the signs of an upcoming training request (slot-prefixed here, as k_tier_restore<true> does), grid-stride
+// over a fixed number of blocks.  Never admits a sign and never refreshes an HBM-resident one.  (One block per SM is all
+// its small grid needs: the register budget that allows keeps it from spilling.)
+__global__ void __launch_bounds__(256, 1) k_tier_stage(TableDev h, TableDev t, HyperDev hy, OptimDev op, SlotsDev sl,
+                                                    const uint64_t* __restrict__ ids, uint32_t n) {
+  const uint32_t tick = h.counters[CTR_TICK];
+  const uint32_t sub = threadIdx.x % BUCKET;
+  const uint32_t gshift = (threadIdx.x & 31) & ~(BUCKET - 1);
+  constexpr uint32_t PER_BLOCK = 256u / BUCKET;
+  for (uint32_t u0 = blockIdx.x * PER_BLOCK; u0 < n; u0 += gridDim.x * PER_BLOCK) {
+    const uint32_t i = u0 + threadIdx.x / BUCKET;
+    const bool valid = i < n;
+    uint64_t sign = 0ULL;
+    if (valid && sub == 0) {
+      sign = ids[i];
+      const uint64_t p = sl.prefix[slot_of_occ(sl, i)];
+      if (p) sign = mod_mersenne(sign, sl.spacing_bits) + p;
+    }
+    sign = __shfl_sync(0xffffffffu, sign, gshift);
+    restore_group<true>(h, t, hy, op, sign, valid, tick, sub, gshift);
+  }
 }
 
 // pb_forward: over the batch's distinct (slot, sign) items, after k_dedup (their number lives on the device)
@@ -108,7 +140,7 @@ __global__ void __launch_bounds__(256) k_tier_restore_items(TableDev h, TableDev
       sign = (c.item >> 31) ? KEY_EMPTY : c.key;  // the scratch set's reserved cell stores 0 for the sign KEY_EMPTY
     }
     sign = __shfl_sync(0xffffffffu, sign, gshift);
-    restore_group(h, t, hy, op, sign, valid, tick, sub, gshift);
+    restore_group<false>(h, t, hy, op, sign, valid, tick, sub, gshift);
   }
 }
 
@@ -314,9 +346,9 @@ void launch_tier_plan(const TableDev& h, const TableDev& t, const uint32_t* ev, 
 }
 
 void launch_tier_move(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const uint32_t* ev,
-                      uint32_t* tev, uint64_t* keys, uint32_t* rows, uint32_t* cells, cudaStream_t st) {
-  PB_LAUNCH(k_tier_collect, PB_NUM_SMS * 8, 256, 0, st, h, ev, tev, keys, rows, cells);
-  PB_LAUNCH(k_tier_move, PB_NUM_SMS * 4, 256, 0, st, h, t, hy, op, tev, keys, rows, cells);
+                      uint32_t* tev, uint64_t* keys, uint32_t* rows, uint32_t* cells, cudaStream_t st, uint32_t blocks) {
+  PB_LAUNCH(k_tier_collect, blocks ? blocks : PB_NUM_SMS * 8, 256, 0, st, h, ev, tev, keys, rows, cells);
+  PB_LAUNCH(k_tier_move, blocks ? blocks : PB_NUM_SMS * 4, 256, 0, st, h, t, hy, op, tev, keys, rows, cells);
 }
 
 void launch_tier_restore(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const SlotsDev& sl,
@@ -325,6 +357,11 @@ void launch_tier_restore(const TableDev& h, const TableDev& t, const HyperDev& h
   const uint32_t g = cdiv((uint64_t)n * BUCKET, 256);
   if (prefix) PB_LAUNCH(k_tier_restore<true>, g, 256, 0, st, h, t, hy, op, sl, ids, n);
   else PB_LAUNCH(k_tier_restore<false>, g, 256, 0, st, h, t, hy, op, sl, ids, n);
+}
+
+void launch_tier_stage(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const SlotsDev& sl,
+                       const uint64_t* ids, uint32_t n, uint32_t blocks, cudaStream_t st) {
+  if (n) PB_LAUNCH(k_tier_stage, blocks, 256, 0, st, h, t, hy, op, sl, ids, n);
 }
 
 void launch_tier_restore_items(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op,

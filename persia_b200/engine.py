@@ -16,9 +16,12 @@ never touches the GPU and is tested on the CPU with a stand-in lookup.
 """
 import heapq
 import itertools
+import logging
 import queue
 import threading
 import time
+
+_log = logging.getLogger(__name__)
 
 
 class Permit:
@@ -38,9 +41,14 @@ class Permit:
 
 class ForwardEngine:
     def __init__(self, lookup, forward_buffer_size, reproducible, embedding_staleness=None, world_size=1, rank=0,
-                 flush_after_s=1.0):
-        """lookup(batch, permit_or_None) -> training batch.  `is_remote_ref(batch)` decides who needs a permit."""
+                 flush_after_s=1.0, stage=None):
+        """lookup(batch, permit_or_None) -> training batch.  `is_remote_ref(batch)` decides who needs a permit.
+        stage(batch), optional: called by the worker on every batch it takes in, before it waits for the batch's
+        permit, so that work which needs only the batch's ids (persia_core: the host-tier moves of its lookup) runs
+        while the batches before it still train.  An error is logged and the batch goes on: the lookup does the same
+        work anyway."""
         self.lookup = lookup
+        self.stage = stage
         self.reproducible = bool(reproducible)
         self.world_size, self.rank, self.flush_after_s = max(1, int(world_size)), int(rank), float(flush_after_s)
         self._out = queue.Queue(maxsize=max(1, int(forward_buffer_size)))
@@ -132,6 +140,11 @@ class ForwardEngine:
                 batch = src.get(timeout=0.01)
             except queue.Empty:
                 continue
+            if self.stage is not None:
+                try:
+                    self.stage(batch)
+                except Exception:  # noqa: BLE001 — the lookup restores what the stage did not move
+                    _log.exception("staging a batch failed; its lookup moves its entries itself")
             permit = None
             if self._sem is not None and self.is_remote_ref(batch):
                 while not self._sem.acquire(timeout=0.01):

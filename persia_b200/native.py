@@ -61,6 +61,8 @@ SYMBOLS = {
     "pb_table_create_host": (_i32, [_i32, C.POINTER(TableCfg), C.POINTER(_vp)]),
     "pb_table_attach_tier": (_i32, [_vp, _vp]),
     "pb_tier_stats": (_i32, [_vp, C.POINTER(_u64 * 5), _vp]),
+    "pb_tier_stage": (_i32, [_vp, _vp, _u32, C.POINTER(_u32), C.POINTER(_u64), _u32, _u32, _vp]),
+    "pb_tier_stage_stats": (_i32, [_vp, C.POINTER(_u64 * 2), _vp]),
     "pb_lookup": (_i32, [_vp, _vp, _u32, _i32, _vp, _vp]),
     "pb_update": (_i32, [_vp, _vp, _vp, _u32, _vp]),
     "pb_set_rows": (_i32, [_vp, _vp, _vp, _u32, _vp]),

@@ -599,6 +599,56 @@ def _forward_locked(batch, device_id, training):
                                pending if training else None)
 
 
+def _stage(batch):
+    """Forward's stage (ForwardEngine): for every dim group whose table has a host-memory tier, the host-tier moves the
+    batch's training forward will need (pb_tier_stage) are issued now, while the batches before it still train: the
+    signs of the group's summation slots (hash-stacked as _to_device_ids does) and raw slots, on a stream the group owns,
+    under the group's lock.  Results do not change; the forward finds its entries in HBM.  Nothing runs for tables
+    without a tier, inference batches, or on R GPUs (no tier there)."""
+    import torch
+
+    if (_S.replica_size or 1) > 1 or batch.embedding_tensor is None or not _S.slots:
+        return
+    if batch.embedding_tensor[0] == "ref":
+        stored = _S.forward_id_buffer.get(batch.embedding_tensor[1])
+        if stored is None:
+            return
+        requires_grad, feats = stored
+    else:
+        _, requires_grad, feats = batch.embedding_tensor
+    sizes = {len(x) for _, x in feats}
+    if not requires_grad or len(sizes) != 1 or any(n not in _S.by_name for n, _ in feats):
+        return
+    B = sizes.pop()
+    dev = torch.device("cuda", _S.device_id if _S.device_id is not None else 0)
+    for dim in sorted({_S.by_name[n].dim for n, _ in feats}):
+        with _STATE_LOCK:
+            g = _S.groups.get(dim)  # (a group is created by its first forward: nothing is held in a tier before)
+        if g is None or g["shard"].host_tier is None:
+            continue
+        summ = [(n, x) for n, x in feats if _S.by_name[n].dim == dim and _S.by_name[n].embedding_summation]
+        raw = [(n, x) for n, x in feats if _S.by_name[n].dim == dim and not _S.by_name[n].embedding_summation]
+        with g["lock"]:
+            if g.get("stage_stream") is None:
+                g["stage_stream"] = torch.cuda.Stream(dev)
+            with torch.cuda.stream(g["stage_stream"]):
+                parts, off, prefixes = [], [0], []
+                if summ:
+                    ids, row_off, slot_off = _flatten(summ, B)
+                    slots = [_S.by_name[n] for n, _ in summ]
+                    d_ids, _, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
+                    parts.append(d_ids)
+                    off += [int(x) for x in slot_off[1:]]
+                    prefixes += [sc.index_prefix for sc in slots]
+                for n, x in raw:
+                    ids, _, _ = _flatten([(n, x)], B)
+                    parts.append(torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True))
+                    off.append(off[-1] + int(ids.size))
+                    prefixes.append(_S.by_name[n].index_prefix)
+                d = torch.cat(parts) if len(parts) > 1 else parts[0]
+                g["shard"].stage(d, off, prefixes, _S.prefix_bit)
+
+
 def _sharded_worker(g, dim, names, B, ids, row_off, slot_off, dev):
     """The dim group's ShardedEmbeddingWorker (persia_b200/worker.py), created by the first batch: a collective —
     every rank's first lookup of the group must happen in the same step (it does: the ranks train in lockstep)."""
@@ -946,8 +996,11 @@ class Forward:  # forward.rs:833-907 over persia_b200.engine.ForwardEngine (reor
             tb._permit = permit
             return tb
 
+        def stage(batch):
+            _stage(batch)
+
         self._engine = ForwardEngine(lookup, forward_buffer_size, reproducible, embedding_staleness,
-                                     world_size=max(1, _S.replica_size or 1), rank=_S.replica_index or 0)
+                                     world_size=max(1, _S.replica_size or 1), rank=_S.replica_index or 0, stage=stage)
         self._engine.is_remote_ref = lambda b: b.embedding_tensor is not None and b.embedding_tensor[0] == "ref"
 
     def set_input_channel(self, receiver):

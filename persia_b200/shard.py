@@ -108,6 +108,25 @@ class EmbeddingShard:
         N.check(self.lib.pb_tier_stats(self.h, C.byref(out), _stream(self.device)))
         return {"host_rows": out[0], "moved_out": out[1], "restored": out[2], "dropped": out[3], "refused": out[4]}
 
+    def stage(self, ids, slot_off, prefixes, prefix_bit=8):
+        """pb_tier_stage on the current stream: the eviction check and the tier restores of an upcoming training request,
+        one batch ahead.  ids: flat device slot ids (slot-major, hash-stacked where a slot hash-stacks), slot_off: host
+        list of n_slots + 1 offsets, prefixes: each slot's index prefix (0 = ids taken as they are).  Values never
+        change, only where entries live; without a tier nothing runs."""
+        ids = _as_i64_bits(ids)
+        S = len(prefixes)
+        off = (C.c_uint32 * (S + 1))(*[int(x) for x in slot_off])
+        pf = (C.c_uint64 * S)(*[int(p) for p in prefixes])
+        N.check(self.lib.pb_tier_stage(self.h, _ptr(ids), ids.numel(), off, pf, S, int(prefix_bit),
+                                       _stream(self.device)))
+
+    def stage_stats(self):
+        """Stage counters (host sync): signs moved into HBM by stages (also counted in tier_stats()["restored"]), and
+        stage restores skipped for want of a free HBM row (left to the request's own restore)."""
+        out = (C.c_uint64 * 2)()
+        N.check(self.lib.pb_tier_stage_stats(self.h, C.byref(out), _stream(self.device)))
+        return {"staged": out[0], "skipped": out[1]}
+
     def __len__(self):
         """Entries held: the HBM rows plus the host tier's."""
         n = int(self.counters()["admitted"])
