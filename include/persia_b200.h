@@ -151,6 +151,38 @@ int pb_tier_stage(pb_table* t, const uint64_t* d_ids, uint32_t n, const uint32_t
  * free HBM row (left to the request's own restore; NOT counted in pb_tier_stats[4]).  Since creation / clear; zeros
  * without a tier.  Synchronises `stream`. */
 int pb_tier_stage_stats(pb_table* t, uint64_t h_out[2], void* stream);
+/* ---- incremental updates: the signs stepped since the last take ---------------------------------------------------
+ * The reference's parameter server hands every sign update_gradient_mixed stepped to its incremental-update manager,
+ * which dumps the entries of the signs it collected once there are more than incremental_buffer_size of them
+ * (embedding_parameter_service/mod.rs:366-424, persia-incremental-update-manager/src/lib.rs:251-312).  Here the set of
+ * such signs lives on the device and the training calls fill it, after the optimizer step they report and on the same
+ * stream (a captured step stays one graph):
+ *   - pb_backward: every distinct (slot, sign) item of the batch whose slot was applied (d_slot_status 0) and that had a
+ *     row (a gradient miss is not marked), once per call whatever the feature groups;
+ *   - pb_backward_raw: the slot's distinct signs that had a row, if the request was applied;
+ *   - pb_update: the signs it found, in HBM or in the host tier (a tier-held row is stepped in place and marked too);
+ *   - pb_backward_sharded / pb_backward_raw_sharded: on the owner (PB_PHASE_SERVE), every received entry whose gradient
+ *     was applied and that had a row.  Nothing is marked on the requesting side.
+ * Lookups, admissions, pb_set_rows, tier moves and stages mark nothing.  A sign is held once however often it is marked.
+ * A set that holds `capacity` signs drops further new signs and counts them (as the reference's full channel does,
+ * mod.rs:415-423): a mark never blocks and never fails a step.  The set is keyed by sign, so a move between a table and
+ * its tier never touches it; a tier has no set of its own.  A table that never enables one launches no extra kernel. */
+/* Allocates the set (an open-addressing set of next_pow2(2 x capacity) cells of 16 B, counters in HBM, the held count
+ * mirrored into one word of mapped pinned host memory), emptying any set the table had; capacity 0 frees it.
+ * Synchronises the device. */
+int pb_table_enable_incremental(pb_table* t, uint64_t capacity);
+/* If the set holds at most max_n signs, writes them to d_signs (in no particular order) and empties the set, in one pass;
+ * otherwise writes nothing and leaves the set as it is.  Either way *d_count = the signs held (max_n = 0 sizes the
+ * buffer, as pb_table_export_signs).  Ordered like every other call on the table.  A take and the calls that mark must
+ * be ordered by the caller (one stream, or events): a mark running beside a take may be lost, and the take then writes
+ * at most max_n signs. */
+int pb_inc_take(pb_table* t, uint64_t* d_signs, uint32_t max_n, uint32_t* d_count, void* stream);
+/* [0] signs held, [1] signs inserted, [2] signs dropped because the set was full, [3] signs taken; since the set was
+ * enabled.  Zeros without a set.  Synchronises `stream`. */
+int pb_inc_stats(pb_table* t, uint64_t h_out[4], void* stream);
+/* The held count as the last completed mark or take left it, read from host memory without synchronising: it may lag
+ * the stream by the calls still in flight.  0 without a set. */
+int pb_inc_held(pb_table* t, uint64_t* h_out);
 /* Diagnostic: the state of the hash index's n_cells normal cells (the three cells reserved for the marker-valued signs
  * are not counted): [0] live (a resident sign), [1] tombstones (an evicted sign), [2] EMPTY.  An admission needs an
  * EMPTY cell on its probe path; every eviction check rebuilds the index (tombstones dropped) once fewer than 1/8 of the

@@ -30,9 +30,14 @@ DONE_FILE = "embedding_dump_done"
 
 
 # ------------------------------------------------------------------------------------------------ format
+def entry_fields(entry_len):
+    """One HashMapEmbeddingEntry as speedy writes it (emb_entry.rs:17-25): len u32 | f32 x len | embedding_dim u64 |
+    sign u64.  Incremental-update packets (persia_b200/incremental.py) carry the same entries."""
+    return [("len", "<u4"), ("inner", "<f4", (entry_len,)), ("dim", "<u8"), ("sign", "<u8")]
+
+
 def _node_dtype(entry_len):
-    return np.dtype([("next", "<u4"), ("prev", "<u4"), ("flag", "u1"), ("len", "<u4"), ("inner", "<f4", (entry_len,)),
-                     ("dim", "<u8"), ("sign", "<u8")])
+    return np.dtype([("next", "<u4"), ("prev", "<u4"), ("flag", "u1")] + entry_fields(entry_len))
 
 
 def encode_list(signs, entries, dims):

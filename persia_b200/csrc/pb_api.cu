@@ -113,6 +113,9 @@ struct pb_table {
   // ordering around pb_tier_stage (a table with a tier): `last` is recorded after every call on the table, `staged`
   // after every stage
   Mark last, staged;
+  // incremental updates (pb_table_enable_incremental): the set of signs stepped since the last take; cells == null: off
+  IncDev inc{};
+  unsigned long long* inc_host = nullptr;  // host address of inc.mirror (cudaFreeHost)
 };
 
 struct pb_ctx {
@@ -379,6 +382,14 @@ int check_grads_aligned(const void* const* h_grads, uint32_t n_slots) {
   return PB_OK;
 }
 
+void free_incremental(pb_table* t) {
+  if (t->inc.cells) cudaFree(t->inc.cells);
+  if (t->inc.ctr) cudaFree(t->inc.ctr);
+  if (t->inc_host) cudaFreeHost(t->inc_host);
+  t->inc = IncDev{};
+  t->inc_host = nullptr;
+}
+
 void drop_pending(pb_ctx* c) {
   if (c->pending && c->pending_table && c->pending_table->pending_batches) c->pending_table->pending_batches--;
   c->pending = false;
@@ -525,6 +536,72 @@ int pb_tier_stage_stats(pb_table* t, uint64_t h_out[2], void* stream) {
   return PB_OK;
 }
 
+int pb_table_enable_incremental(pb_table* t, uint64_t capacity) {
+  if (!t) return fail(PB_ERR_INVALID, "null argument");
+  if (t->host) return fail(PB_ERR_STATE, "a host tier has no set of its own: enable it on the table the tier is attached to");
+  if (capacity >= (1ull << 30)) return fail(PB_ERR_INVALID, "capacity must be < 2^30 signs");
+  DeviceGuard g(t->device);
+  PB_CUDA(cudaDeviceSynchronize());  // enqueued marks may still use the old set
+  free_incremental(t);
+  if (!capacity) return PB_OK;
+  IncDev& s = t->inc;
+  s.capacity = capacity;
+  s.n_cells = next_pow2(2 * capacity < 1024 ? 1024 : 2 * capacity);
+  s.bucket_mask = s.n_cells / BUCKET - 1;
+  cudaError_t e = cudaMalloc(&s.cells, sizeof(Cell) * ((size_t)s.n_cells + N_SPECIAL));
+  if (e == cudaSuccess) e = cudaMalloc(&s.ctr, sizeof(unsigned long long) * INC_WORDS);
+  if (e == cudaSuccess) e = cudaHostAlloc((void**)&t->inc_host, sizeof(unsigned long long), cudaHostAllocMapped | cudaHostAllocPortable);
+  if (e == cudaSuccess) {
+    *t->inc_host = 0;
+    e = cudaHostGetDevicePointer((void**)&s.mirror, t->inc_host, 0);
+  }
+  if (e == cudaSuccess) {
+    launch_inc_fill(s, 0);
+    e = cudaDeviceSynchronize();
+  }
+  if (e != cudaSuccess) {
+    free_incremental(t);
+    return fail(PB_ERR_CUDA, std::string("pb_table_enable_incremental: ") + cudaGetErrorString(e));
+  }
+  return PB_OK;
+}
+
+int pb_inc_take(pb_table* t, uint64_t* d_signs, uint32_t max_n, uint32_t* d_count, void* stream) {
+  if (!t || !d_count || (max_n && !d_signs)) return fail(PB_ERR_INVALID, "null argument");
+  if (!t->inc.cells) return fail(PB_ERR_STATE, "incremental updates are not enabled on this table");
+  DeviceGuard g(t->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if (int rc = call.begin(t, st)) return rc;
+  launch_inc_take(t->inc, d_signs, max_n, d_count, st);
+  PB_CUDA(cudaGetLastError());
+  return PB_OK;
+}
+
+int pb_inc_stats(pb_table* t, uint64_t h_out[4], void* stream) {
+  if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
+  for (int i = 0; i < 4; ++i) h_out[i] = 0;
+  if (!t->inc.cells) return PB_OK;
+  DeviceGuard g(t->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if (int rc = call.begin(t, st)) return rc;
+  unsigned long long c[INC_WORDS];
+  PB_CUDA(cudaMemcpyAsync(c, t->inc.ctr, sizeof(c), cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  h_out[0] = c[INC_HELD];
+  h_out[1] = c[INC_INSERTED];
+  h_out[2] = c[INC_DROPPED];
+  h_out[3] = c[INC_TAKEN];
+  return PB_OK;
+}
+
+int pb_inc_held(pb_table* t, uint64_t* h_out) {
+  if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
+  *h_out = t->inc_host ? *reinterpret_cast<volatile unsigned long long*>(t->inc_host) : 0;
+  return PB_OK;
+}
+
 int pb_table_destroy(pb_table* t) {
   if (!t) return PB_OK;
   DeviceGuard g(t->device);
@@ -544,6 +621,10 @@ int pb_table_destroy(pb_table* t) {
     if (t->evict_ws) cudaFree(t->evict_ws);
     if (t->rebuild_keys) cudaFree(t->rebuild_keys);
     if (t->rebuild_rows) cudaFree(t->rebuild_rows);
+  }
+  if (t->inc.cells) {
+    cudaDeviceSynchronize();
+    free_incremental(t);
   }
   if (t->stats_ws) cudaFree(t->stats_ws);
   if (t->scratch) cudaFree(t->scratch);
@@ -723,6 +804,9 @@ int pb_update(pb_table* t, const uint64_t* d_signs, const float* d_grads, uint32
   }
   launch_update_direct(t->d, t->op, t->hy, t->scratch, d_grads, n, pair, st);
   if (t->tier) launch_update_direct(t->tier->d, t->op, t->hy, t->tier->scratch, d_grads, n, pair, st);
+  if (t->inc.cells && n)  // the signs just stepped, in HBM or in the tier
+    launch_inc_mark_signs(t->inc, t->d, d_signs, t->scratch, n, t->tier ? t->tier->d : t->d,
+                          t->tier ? t->tier->scratch : nullptr, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -1080,7 +1164,8 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
   // beside the main stream: the scratch set is emptied and, once the NaN marks are known, the hot items are reduced
   PB_CUDA(cudaEventRecord(c->ev_fork, st));
   PB_CUDA(cudaStreamWaitEvent(c->side, c->ev_fork, 0));
-  if (c->set_dirty) {
+  const bool mark = t->inc.cells != nullptr;  // the mark reads the scratch set and empties it after the steps
+  if (c->set_dirty && !mark) {
     launch_clear_items(c->b, c->side);
     c->set_dirty = false;
   }
@@ -1115,6 +1200,15 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
   PB_CUDA(cudaStreamWaitEvent(st, c->ev_join, 0));
   PB_CUDA(cudaEventRecord(c->ev_join2, c->side2));
   PB_CUDA(cudaStreamWaitEvent(st, c->ev_join2, 0));
+  if (mark) {  // every round has stepped: the applied items that had a row
+    IncSlots on{};
+    for (uint32_t s = 0; s < S; ++s)
+      if (h_grads[s]) on.applied[s >> 5] |= 1u << (s & 31);
+    BatchDev b = c->b;
+    b.n = c->n_occ;
+    launch_inc_mark_items(t->inc, b, sl, on, c->dev_tick, c->nan_tick, c->set_dirty, st);
+    c->set_dirty = false;
+  }
   drop_pending(c);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
@@ -1172,6 +1266,7 @@ int owner_backward(pb_table* t, pb_xchg* x, const uint64_t* prefix, uint32_t n_p
     }
     launch_owner_update_all(t->d, t->op, t->hy, x->d, st);
   }
+  if (t->inc.cells) launch_inc_mark_owner(t->inc, x->d, t->d.capacity, st);  // the entries just stepped
   x->u_dirty = false;
   return PB_OK;
 }
@@ -1552,6 +1647,7 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
   launch_raw_stage(d_grad, is_f16 != 0, c->raw.counts, dim, inv, do_scale, c->raw_stage, st);
   launch_update_direct(t->d, t->op, t->hy, c->raw.target, c->raw_stage, c->n_occ, pair, st, c->raw.counts,
                        c->dev_tick, c->nan_tick, true);
+  if (t->inc.cells && c->n_occ) launch_inc_mark_raw(t->inc, c->raw, c->n_occ, c->dev_tick, c->nan_tick, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }

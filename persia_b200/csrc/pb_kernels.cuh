@@ -149,6 +149,30 @@ struct RawWork {
   uint32_t* peer;           // [PB_MAX_RANKS] distinct signs routed to each owner
 };
 
+// the set of signs stepped since the last take (pb_inc.cu, pb_table_enable_incremental): an open-addressing set of
+// n_cells cells keyed by sign (a power of two >= 2 x capacity), BUCKET cells per 128 B line, home bucket from mix64 as in
+// the index; the signs >= KEY_TOMB (equal to a marker) own the N_SPECIAL reserved cells after them (row == 1: held)
+enum { INC_HELD = 0, INC_INSERTED, INC_DROPPED, INC_TAKEN, INC_CURSOR, INC_DONE, INC_WORDS };
+struct IncDev {
+  Cell* cells;                  // n_cells + N_SPECIAL
+  unsigned long long* ctr;      // INC_* words
+  unsigned long long* mirror;   // device address of the mapped pinned host word that mirrors ctr[INC_HELD]
+  unsigned long long capacity;  // signs the set may hold
+  uint32_t n_cells, bucket_mask;
+};
+struct IncSlots {
+  uint32_t applied[PB_MAX_SLOTS / 32];  // slots the request gave a gradient (the NaN rule is read on the device)
+};
+void launch_inc_fill(const IncDev& s, cudaStream_t st);
+void launch_inc_mark_items(const IncDev& s, const BatchDev& b, const SlotsDev& sl, const IncSlots& on,
+                           const uint32_t* tick, const uint32_t* nan_tick, bool clear, cudaStream_t st);
+void launch_inc_mark_raw(const IncDev& s, const RawWork& w, uint32_t n, const uint32_t* tick, const uint32_t* nan_tick,
+                         cudaStream_t st);
+void launch_inc_mark_signs(const IncDev& s, const TableDev& h, const uint64_t* signs, const uint32_t* occ_cell,
+                           uint32_t n, const TableDev& t, const uint32_t* where, cudaStream_t st);
+void launch_inc_mark_owner(const IncDev& s, const XchgDev& x, uint32_t capacity, cudaStream_t st);
+void launch_inc_take(const IncDev& s, uint64_t* out, uint32_t max_n, uint32_t* count, cudaStream_t st);
+
 void launch_fill_cells(Cell* cells, uint64_t n, cudaStream_t st);
 void launch_fill_set(DCell* set, uint64_t n, cudaStream_t st);
 // bump: a training request (advances the table's batch number and the context's request number)

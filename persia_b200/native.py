@@ -63,6 +63,10 @@ SYMBOLS = {
     "pb_tier_stats": (_i32, [_vp, C.POINTER(_u64 * 5), _vp]),
     "pb_tier_stage": (_i32, [_vp, _vp, _u32, C.POINTER(_u32), C.POINTER(_u64), _u32, _u32, _vp]),
     "pb_tier_stage_stats": (_i32, [_vp, C.POINTER(_u64 * 2), _vp]),
+    "pb_table_enable_incremental": (_i32, [_vp, _u64]),
+    "pb_inc_take": (_i32, [_vp, _vp, _u32, _vp, _vp]),
+    "pb_inc_stats": (_i32, [_vp, C.POINTER(_u64 * 4), _vp]),
+    "pb_inc_held": (_i32, [_vp, C.POINTER(_u64)]),
     "pb_lookup": (_i32, [_vp, _vp, _u32, _i32, _vp, _vp]),
     "pb_update": (_i32, [_vp, _vp, _vp, _u32, _vp]),
     "pb_set_rows": (_i32, [_vp, _vp, _vp, _u32, _vp]),

@@ -16,7 +16,9 @@ Their calls are collective, so every rank issues them in one fixed order: the ra
 summation dims in ascending order, in the forward and again in the backward; every batch must carry the same raw
 slots in the same order.  `Forward` prefetches on worker threads with the reference's ordering and
 staleness rules (persia_b200/engine.py), `Backward` applies updates in the caller's thread; `to_bytes()` is a private encoding (the speedy wire format is N4); `dump`/`load`
-write and read the reference's `.emb` checkpoint files (persia_b200/checkpoint.py).
+write and read the reference's `.emb` checkpoint files (persia_b200/checkpoint.py).  With the global config's
+`enable_incremental_update` on a Train job, the signs the tables step are flushed as the reference's `.inc` packets; an
+Infer job loads its checkpoint and applies them as they appear (persia_b200/incremental.py, `set_global_config`).
 """
 import os
 import queue
@@ -108,6 +110,28 @@ class _State:
         self.next_batch_id = 0
         self.forward_id_buffer = {}
         self.raw_order = None  # replica_size > 1: the raw slots of the first batch, in order (every batch must match)
+        self.gcfg = None  # the global config's keys this project reads (incremental.parse_global_config)
+        self.dumper = None  # Train with enable_incremental_update: the writer of this replica's flushes
+        self.loader = None  # Infer: the scanner of this replica's incremental directory
+        self.inc_lock = threading.Lock()
+
+    def global_config(self):
+        """set_global_config's dict, else the PERSIA_GLOBAL_CONFIG yaml, else the reference's defaults."""
+        if self.gcfg is None:
+            from . import incremental as INC
+
+            gc = {}
+            g = os.environ.get("PERSIA_GLOBAL_CONFIG")
+            if g and os.path.isfile(g):
+                import yaml
+
+                gc = yaml.safe_load(open(g)) or {}
+            self.gcfg = INC.parse_global_config(gc)
+        return self.gcfg
+
+    def incremental_on(self):
+        c = self.global_config()
+        return c["job_type"] == "Train" and c["enable_incremental_update"]
 
     def set_config(self, cfg):
         self.prefix_bit, self.slots = parse_embedding_config(cfg)
@@ -145,6 +169,8 @@ class _State:
                 sh.set_optimizer(**self.optimizer)
             if self.hyper is not None:
                 sh.configure(**self.hyper)
+            if self.incremental_on():  # twice the flush threshold: the set fills while a flush is being taken
+                sh.enable_incremental(2 * self.global_config()["incremental_buffer_size"])
             g = self.groups[dim] = {"shard": sh, "ctx": {}, "device": dev, "lock": threading.RLock()}
         return g
 
@@ -162,11 +188,132 @@ def set_embedding_config(cfg):
     _S.set_config(cfg)
 
 
+def set_global_config(cfg):
+    """Programmatic stand-in for the PERSIA_GLOBAL_CONFIG yaml (persia-embedding-config/src/lib.rs:355-447): of it this
+    project reads embedding_parameter_server_config.{enable_incremental_update, incremental_buffer_size,
+    incremental_dir, incremental_channel_capacity} and common_config.{job_type, checkpointing_config.num_workers,
+    infer_config.embedding_checkpoint}.  (capacity keeps coming from PERSIA_B200_CAPACITY or the yaml.)  Set it before
+    the first batch: the tables are created with it."""
+    from . import incremental as INC
+
+    _S.gcfg = INC.parse_global_config(cfg)
+
+
 def reset():
     """Drop every table and configuration (tests)."""
+    if _S.loader is not None:
+        _S.loader.stop()
+    if _S.dumper is not None:
+        _S.dumper.close()
     for g in _S.groups.values():
         g["shard"].close()
     _S.reset()
+
+
+def _maybe_flush_incremental():
+    """After a batch's updates are enqueued: the reference dumps once its set holds more than incremental_buffer_size
+    signs (lib.rs:265-275), one set per parameter server across every dim, so the threshold counts the signs of all of
+    this replica's tables.  The held counts are read without a sync and may lag by the batches still in flight."""
+    if not _S.incremental_on():
+        return
+    groups = [g for g in _S.groups.values()]
+    if sum(g["shard"].incremental_held() for g in groups) > _S.global_config()["incremental_buffer_size"]:
+        _flush_incremental()
+
+
+def _flush_incremental():
+    """Takes every table's set and hands one flush to the dumper.  Only device work is done here, under each group's
+    lock and on the update stream: the take (one pass over the set) and the gather of the taken signs' entries into a
+    device buffer, then one host sync to read how many signs there are.  The copy to the host, the sort and the files
+    are the dumper thread's: it waits for an event recorded after the gathers.  A queued flush keeps its signs and
+    entries in device memory (~1 GB per 10^6 signs at dim 128 with Adagrad) until the dumper has copied them out, so
+    at most MAX_QUEUED_FLUSHES wait: past that the training thread waits for the writer rather than drop updates."""
+    from . import incremental as INC
+
+    c = _S.global_config()
+    with _S.inc_lock:
+        parts = _take_flush(_S.groups, 2 * c["incremental_buffer_size"])
+        if _S.dumper is None:
+            _S.dumper = INC.IncrementalDumper(c["incremental_dir"], _S.replica_index or 0, c["num_workers"],
+                                              c["incremental_channel_capacity"])
+        _S.dumper.wait_queued(MAX_QUEUED_FLUSHES - 1)
+        _S.dumper.submit(parts)
+    return _S.dumper
+
+
+MAX_QUEUED_FLUSHES = 2  # flushes whose device buffers may wait for the dumper thread at once
+
+
+def _take_flush(groups, capacity):
+    """The device half of a flush over `groups` ({dim: group}, each a table of `capacity`-sign set and its lock);
+    returns the host half, a callable that waits for the device work and gives the dumper's parts."""
+    import torch
+
+    from . import shard as SH
+
+    taken = []
+    for dim in sorted(groups):
+        g = groups[dim]
+        with g["lock"]:
+            got = g["shard"].take_incremental_device(capacity)
+        taken.append((dim, got))
+    ready = torch.cuda.Event()
+    ready.record()
+
+    def parts():  # (on the dumper's thread)
+        ready.synchronize()
+        out = []
+        for dim, (signs, ent, found) in taken:
+            s, e, _ = SH.host_entries(signs, ent, found)
+            out.append((s, dim, e))
+        return out
+
+    return parts
+
+
+def _start_infer():
+    """Infer: load infer_config.embedding_checkpoint, then scan incremental_dir/s{replica_index} for flushes
+    (persia-embedding-parameter-server.rs:111-117, lib.rs:163-170).  Runs once the optimizer is registered (the entry
+    layout is known then)."""
+    from . import checkpoint as CK
+    from . import incremental as INC
+
+    c = _S.global_config()
+    if c["job_type"] != "Infer" or _S.loader is not None:
+        return
+    _S.ensure_config()
+    dims = sorted({s.dim for s in _S.slots})
+    if c["embedding_checkpoint"]:
+        CK.load_shards(c["embedding_checkpoint"], {d: _S.group(d)["shard"] for d in dims}, _S.replica_index or 0,
+                       max(1, _S.replica_size or 1))
+    directory = os.path.join(c["incremental_dir"], f"s{_S.replica_index or 0}")
+    _S.loader = INC.IncrementalLoader(directory, _apply_incremental)
+    _S.loader.start()
+
+
+def _apply_incremental(signs, dims, entries, groups=None):
+    """One packet into the tables of its dims (groups: {dim: group}, None = this replica's), through set_entries (HBM
+    first, then the tier); returns the entries neither table had room for."""
+    import torch
+
+    dropped = 0
+    groups = _S.groups if groups is None else groups
+    for dim in np.unique(dims):
+        g = groups.get(int(dim))
+        if g is None:
+            raise RuntimeError(f"incremental packet holds dim-{int(dim)} entries but no slot has that dim")
+        pick = np.flatnonzero(dims == dim)
+        ent = np.stack([entries[i] for i in pick])
+        sh = g["shard"]
+        if ent.shape[1] != sh.entry_len:
+            raise RuntimeError(f"dim-{int(dim)} entries of {ent.shape[1]} floats, the registered optimizer needs "
+                               f"{sh.entry_len}")
+        dev = torch.device("cuda", g["device"])
+        sg = torch.from_numpy(np.ascontiguousarray(signs[pick]).view(np.int64)).to(dev)
+        with g["lock"]:
+            sh.set_entries(sg, torch.from_numpy(ent).to(dev))
+            dropped += int((~sh.get_entries(sg)[1]).sum())
+    return dropped
 
 
 def is_cuda_feature_available():  # lib.rs:452-459
@@ -876,6 +1023,7 @@ class Backward:  # backward.rs:203-405
                         g["worker"].backward_ptrs(ptrs, bool(f16), scales)
                     else:
                         ctx.backward_ptrs(g["shard"], ptrs, bool(f16), scales)
+            _maybe_flush_incremental()
         finally:
             p.release()
             if permit is not None:  # the update is enqueued: the batch no longer counts as in flight (backward.rs:341-343)
@@ -924,6 +1072,7 @@ class OptimizerBase:  # optim.rs:8-66
         _S.optimizer = dict(self._cfg)
         for g in _S.groups.values():
             g["shard"].set_optimizer(**_S.optimizer)
+        _start_infer()  # job_type Infer: the servers load their checkpoint and start scanning for incremental updates
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -1070,6 +1219,25 @@ class PersiaCommonContext:
         dims = sorted({s.dim for s in _S.slots})
         CK.load_shards(src_dir, {d: _S.group(d)["shard"] for d in dims}, _S.replica_index or 0, max(1, _S.replica_size or 1))
 
+    def flush_incremental(self):
+        """Not part of the reference surface (its manager flushes only on the threshold): takes every table's set of
+        updated signs now, writes them as one incremental update and returns once it is on disk — for the end of
+        training and for tests.  Returns the directory written (None when no sign was updated since the last flush)."""
+        if not _S.incremental_on():
+            raise RuntimeError("incremental updates are off: set embedding_parameter_server_config."
+                               "enable_incremental_update on a Train job (set_global_config / PERSIA_GLOBAL_CONFIG)")
+        for b in list(_BACKWARDS):
+            b.flush()
+        n = len(_S.dumper.written) if _S.dumper is not None else 0
+        d = _flush_incremental()
+        d.flush()
+        return d.written[-1] if len(d.written) > n else None
+
+    @property
+    def incremental_loader(self):
+        """Infer: the IncrementalLoader scanning this replica's incremental directory (poll() applies what is new)."""
+        return _S.loader
+
     def wait_for_serving(self):
         return None
 
@@ -1181,7 +1349,8 @@ utils = _submodule("utils", PersiaMessageQueueServer=PersiaMessageQueueServer, P
 nats = _submodule("nats", initialize_dataflow=initialize_dataflow)
 
 
-_PUBLIC = ("PersiaCommonContext", "is_cuda_feature_available", "set_embedding_config", "reset", "parse_embedding_config")
+_PUBLIC = ("PersiaCommonContext", "is_cuda_feature_available", "set_embedding_config", "set_global_config", "reset",
+           "parse_embedding_config")
 _facade = None
 
 

@@ -127,6 +127,59 @@ class EmbeddingShard:
         N.check(self.lib.pb_tier_stage_stats(self.h, C.byref(out), _stream(self.device)))
         return {"staged": out[0], "skipped": out[1]}
 
+    # incremental updates (PerisaIncrementalUpdateManager, persia-incremental-update-manager/src/lib.rs:251-312)
+    def enable_incremental(self, capacity):
+        """Keep the set of signs the optimizer steps from now on (at most `capacity`; further new signs are dropped and
+        counted), for take_incremental().  capacity 0 frees the set.  With a host tier, the set covers both tables."""
+        N.check(self.lib.pb_table_enable_incremental(self.h, int(capacity)))
+
+    def incremental_stats(self):
+        """The set's counters (host sync): signs held now, inserted, dropped because the set was full, and taken."""
+        out = (C.c_uint64 * 4)()
+        N.check(self.lib.pb_inc_stats(self.h, C.byref(out), _stream(self.device)))
+        return {"held": out[0], "inserted": out[1], "dropped": out[2], "taken": out[3]}
+
+    def incremental_held(self):
+        """Signs held, read without a sync: may lag the work still in flight on the stream."""
+        v = C.c_uint64()
+        N.check(self.lib.pb_inc_held(self.h, C.byref(v)))
+        return int(v.value)
+
+    def take_incremental_device(self, capacity):
+        """Empties the set (at most `capacity` signs: the capacity it was enabled with) on the current stream and returns
+        (signs int64 [n], entries f32 [n, entry_len], found bool [n]) on the device, in no particular order; found is
+        False for a held sign no table holds any more.  The only host sync is the read of n.  None (and the set left as
+        it is) when it holds more than `capacity` signs."""
+        buf = torch.empty(max(int(capacity), 1), dtype=torch.int64, device=self.device)
+        count = torch.zeros(1, dtype=torch.int32, device=self.device)
+        N.check(self.lib.pb_inc_take(self.h, _ptr(buf), int(capacity), _ptr(count), _stream(self.device)))
+        n = int(count)
+        if n > capacity:
+            return None
+        signs = buf[:n]
+        if not n:
+            return signs, torch.zeros((0, self.entry_len), dtype=torch.float32, device=self.device), \
+                torch.zeros(0, dtype=torch.bool, device=self.device)
+        ent, found = self.get_entries(signs)
+        return signs, ent, found
+
+    def take_incremental(self, capacity=None):
+        """Empties the set.  Returns (signs, entries, skipped): the held signs that are still resident (HBM or tier),
+        int64 bit patterns sorted ascending as u64, on the host; their entries (f32 [n, entry_len], on the host); and
+        the number of held signs no table holds any more (evicted and dropped since they were marked), which are
+        skipped as the reference skips them (lib.rs:187-192).  capacity: the set's (None: sized by a first call)."""
+        while True:
+            n = capacity
+            if n is None:
+                count = torch.zeros(1, dtype=torch.int32, device=self.device)
+                N.check(self.lib.pb_inc_take(self.h, None, 0, _ptr(count), _stream(self.device)))
+                n = int(count)
+            got = self.take_incremental_device(n)
+            if got is not None:  # (marks enqueued from another thread since the sizing call can grow the set)
+                return host_entries(*got)
+            if capacity is not None:
+                raise RuntimeError("the set holds more signs than the capacity given")
+
     def __len__(self):
         """Entries held: the HBM rows plus the host tier's."""
         n = int(self.counters()["admitted"])
@@ -325,6 +378,18 @@ class BatchContext:
             self.close()
         except Exception:
             pass
+
+
+def host_entries(signs, ent, found):
+    """take_incremental_device's result on the host: (signs int64 sorted ascending as u64, entries, skipped) of the
+    signs found."""
+    import numpy as np
+
+    found = found.cpu().numpy()
+    signs = signs.cpu().numpy()[found]
+    ent = ent.cpu().numpy()[found]
+    order = np.argsort(signs.view(np.uint64), kind="stable")
+    return signs[order], ent[order], int((~found).sum())
 
 
 def add_prefix(ids, slot_occ_off, prefixes, prefix_bit=8):

@@ -134,6 +134,25 @@ class ShardedEmbeddingWorker:
             worst = int(t)
         return (int(worst * margin) + extra + 7) // 8 * 8
 
+    # ---- incremental updates: the owner table's set of stepped signs (EmbeddingShard.enable_incremental) ---------------
+    def _on_stream(self, fn, *args):
+        if self.stream is None:
+            return fn(*args)
+        with torch.cuda.stream(self.stream):
+            return fn(*args)
+
+    def enable_incremental(self, capacity):
+        return self._on_stream(self.shard.enable_incremental, capacity)
+
+    def incremental_stats(self):
+        return self._on_stream(self.shard.incremental_stats)
+
+    def incremental_held(self):
+        return self.shard.incremental_held()
+
+    def take_incremental(self):
+        return self._on_stream(self.shard.take_incremental)
+
     # ---- forward_batched_direct / update_gradient_batched ------------------------------------------------------------
     def _st(self):
         s = self.stream if self.stream is not None else torch.cuda.current_stream(self.device)
