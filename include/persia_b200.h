@@ -16,6 +16,26 @@
  * rule; the Python wrappers pass a copy of such views.)  A "sign" is a prefixed u64 feature id
  * (embedding_worker_service/mod.rs:402-429).  One pb_table is one parameter-server shard resident in
  * one GPU's HBM, fixed embedding dim (the host side keeps one table per distinct dim).
+ *
+ * Several streams on one table (batches in flight, embedding_staleness > 1: one pb_ctx and one stream per batch).
+ * The library orders the calls on one table, whatever their streams, in the order they are issued, in two chains:
+ *   - steps: pb_backward, pb_backward_raw and pb_update (the row steps, Adam's beta-power advance and the incremental
+ *     set's marks).  Two steps never overlap, so no gradient is lost and no entry torn, and every row is stepped in
+ *     issue order, as the reference's entry locks step it in some serial order.
+ *   - index work: the training and inference forms of pb_forward, pb_forward_raw and pb_lookup (probes, admissions,
+ *     eviction checks, index rebuilds, tier restores), plus pb_update.
+ *   A backward is in the step chain only, so it runs beside the next batch's forward: a forward may read rows a backward
+ *   on another stream is stepping (the staleness embedding_staleness allows).  An eviction check also waits for every
+ *   step issued before it, so it never releases a row whose gradients are still to be applied.  pb_set_rows,
+ *   pb_get_rows, pb_table_export_signs, pb_table_clear, the statistics calls and pb_inc_take are in both chains.
+ * Waiting costs a stream-wait on an event per call; a wait on work already complete costs nothing on the device.
+ * Calls on one table must still be issued from one host thread at a time (the persia_core groups hold a lock), and a
+ * pb_ctx holds one batch at a time.  Under CUDA stream capture the ordering becomes edges of the graph when the calls
+ * are captured into one graph (contexts forked onto side streams of one capture); graphs captured separately cannot be
+ * ordered by the library (a capture waits only on events of the same capture): whoever launches them orders them, e.g.
+ * replays on one stream, or events between replays that touch one table.  A call captured while earlier work on the
+ * table issued outside the capture is still running fails with PB_ERR_STATE (synchronise before capturing).  The
+ * sharded calls (pb_*_sharded) are not in these chains: their caller orders them.
  */
 #ifndef PERSIA_B200_H_
 #define PERSIA_B200_H_
@@ -173,9 +193,8 @@ int pb_tier_stage_stats(pb_table* t, uint64_t h_out[2], void* stream);
 int pb_table_enable_incremental(pb_table* t, uint64_t capacity);
 /* If the set holds at most max_n signs, writes them to d_signs (in no particular order) and empties the set, in one pass;
  * otherwise writes nothing and leaves the set as it is.  Either way *d_count = the signs held (max_n = 0 sizes the
- * buffer, as pb_table_export_signs).  Ordered like every other call on the table.  A take and the calls that mark must
- * be ordered by the caller (one stream, or events): a mark running beside a take may be lost, and the take then writes
- * at most max_n signs. */
+ * buffer, as pb_table_export_signs).  Ordered after every mark issued before it and before every mark issued after it,
+ * whatever their streams (the step chain, top of this file); the sharded owners' marks are ordered by the caller. */
 int pb_inc_take(pb_table* t, uint64_t* d_signs, uint32_t max_n, uint32_t* d_count, void* stream);
 /* [0] signs held, [1] signs inserted, [2] signs dropped because the set was full, [3] signs taken; since the set was
  * enabled.  Zeros without a set.  Synchronises `stream`. */

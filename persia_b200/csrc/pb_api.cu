@@ -113,6 +113,9 @@ struct pb_table {
   // ordering around pb_tier_stage (a table with a tier): `last` is recorded after every call on the table, `staged`
   // after every stage
   Mark last, staged;
+  // ordering of calls on several streams (TableCall): `index` after every call that probes or changes the index,
+  // `step` after every call that steps rows, advances Adam's beta powers or marks the incremental set
+  Mark index, step;
   // incremental updates (pb_table_enable_incremental): the set of signs stepped since the last take; cells == null: off
   IncDev inc{};
   unsigned long long* inc_host = nullptr;  // host address of inc.mirror (cudaFreeHost)
@@ -222,11 +225,16 @@ int ensure_evict_ws(pb_table* t) {
   return PB_OK;
 }
 
+int wait_for(const Mark& m, cudaStream_t st);
+
 // The eviction check: release the least recently used rows when free storage runs low, and rebuild the index when its
 // EMPTY cells run short.  blocks: grid of its scans (0 = the usual; pb_tier_stage's is small).
 int evict_check(pb_table* t, cudaStream_t st, uint32_t blocks = 0) {
   int rc = ensure_evict_ws(t);
   if (rc) return rc;
+  // `pending_batches` drops when a backward is enqueued, perhaps on another stream: the check first waits for every
+  // enqueued step, so the rows it may release are those it would release were every call on one stream
+  if ((rc = wait_for(t->step, st))) return rc;
   // rows of batches whose gradients are still to come are never released: a row used by a pending batch was
   // refreshed by its forward, i.e. at most `pending_batches` requests ago
   const uint32_t keep = t->evict_keep > t->pending_batches + 1 ? t->evict_keep : t->pending_batches + 1;
@@ -257,14 +265,7 @@ int maybe_evict(pb_table* t, cudaStream_t st) {
 // call fails with PB_ERR_STATE rather than record a dependency it cannot keep.  The query runs under
 // cudaThreadExchangeStreamCaptureMode(relaxed): a global-mode capture forbids it otherwise; querying an event recorded
 // inside a capture stays forbidden, and is never done.  A mark recorded into another capture is part of that graph,
-// whose launches the caller orders: nothing is waited for.
-
-// the table whose marks a call on `t` uses (a tier's own calls, export and index statistics, use its table's), or
-// null: no tier, no stage, nothing to order
-pb_table* marks_of(pb_table* t) {
-  pb_table* o = t->tier_of ? t->tier_of : t;
-  return o->tier ? o : nullptr;
-}
+// whose launches the caller orders: nothing is waited for.  The marks of TableCall (below) follow the same rules.
 
 cudaError_t capture_id(cudaStream_t st, unsigned long long& id) {
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
@@ -300,29 +301,49 @@ int wait_for(const Mark& m, cudaStream_t st) {
   cudaThreadExchangeStreamCaptureMode(&mode);
   if (q == cudaSuccess) return PB_OK;
   if (q == cudaErrorNotReady)
-    return fail(PB_ERR_STATE, "a pb_tier_stage (or a call before one) issued outside this stream capture has not "
-                              "completed: synchronise before capturing, or capture the stage too");
+    return fail(PB_ERR_STATE, "earlier work on this table issued outside this stream capture has not completed: "
+                              "synchronise before capturing, or capture that work too");
   return fail(PB_ERR_CUDA, std::string("cudaEventQuery: ") + cudaGetErrorString(q));
 }
 
-// One call on a table: begin() makes `st` wait for the latest stage (not for the backwards, which run beside one), and
-// the call is recorded as the table's latest work when it returns.  Does nothing for a table without a tier.
+// ---- ordering of calls on several streams ------------------------------------------------------------------------
+// Batches of different contexts may be in flight on different streams (embedding_staleness > 1).  A call's work falls
+// in two chains, each kept in the order the calls were issued, whatever their streams:
+//   CALL_INDEX  index work: probes (training or not), admissions, eviction checks and rebuilds, row_tick, tier moves;
+//   CALL_STEP   row steps, Adam's beta-power advance and the incremental set's marks.
+// A call waits for the latest call of each chain it belongs to and becomes that chain's latest.  So two steps never
+// overlap (no update is lost or torn; every row is stepped in issue order) and no probe runs beside a rebuild, while a
+// backward (CALL_STEP only) still runs beside the next batch's forward (CALL_INDEX only): no backward kernel reads
+// index cells, the free-row stack or row_tick.  A forward reads rows that a backward beside it may be stepping: a
+// stale read, as staleness allows.  An eviction check also waits for the step chain (evict_check).  Calls that read
+// or write entries or counters outside a batch (set/get rows, export, statistics, takes, clear) are in both chains.
+// Under stream capture the marks follow wait_for: within one capture they become edges of the graph; graphs captured
+// separately are ordered by whoever launches them.
+enum : unsigned { CALL_INDEX = 1, CALL_STEP = 2, CALL_ALL = 3 };
+
+// One call on a table: begin() makes `st` wait for the chains the call is in and, with a tier, for the latest stage
+// (not the backwards, which run beside one); when the call returns it is recorded as the latest of those chains (and,
+// with a tier, as the table's latest work).  A host tier's calls use its table's marks.
 struct TableCall {
   pb_table* m = nullptr;
   cudaStream_t st = nullptr;
-  int begin(pb_table* t, cudaStream_t s, bool after_stage = true) {
-    pb_table* o = marks_of(t);
-    if (!o) return PB_OK;
-    if (after_stage) {
-      const int rc = wait_for(o->staged, s);
-      if (rc) return rc;
-    }
+  unsigned chains = 0;
+  int begin(pb_table* t, cudaStream_t s, unsigned ch, bool after_stage = true) {
+    pb_table* o = t->tier_of ? t->tier_of : t;
+    int rc;
+    if (o->tier && after_stage && (rc = wait_for(o->staged, s))) return rc;
+    if ((ch & CALL_INDEX) && (rc = wait_for(o->index, s))) return rc;
+    if ((ch & CALL_STEP) && (rc = wait_for(o->step, s))) return rc;
     m = o;
     st = s;
+    chains = ch;
     return PB_OK;
   }
   ~TableCall() {
-    if (m) record(m->last, st);
+    if (!m) return;
+    if (chains & CALL_INDEX) record(m->index, st);
+    if (chains & CALL_STEP) record(m->step, st);
+    if (m->tier) record(m->last, st);
   }
 };
 
@@ -432,9 +453,16 @@ int pb_table_create(int device, const pb_table_cfg* cfg, pb_table** out) {
   int ndev = 0;
   PB_CUDA(cudaGetDeviceCount(&ndev));
   if (device < 0 || device >= ndev) return fail(PB_ERR_INVALID, "no such CUDA device");
+  DeviceGuard g(device);
   pb_table* t = new pb_table();
   t->device = device;
   t->cfg = *cfg;
+  cudaError_t e = cudaEventCreateWithFlags(&t->index.ev, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->step.ev, cudaEventDisableTiming);
+  if (e != cudaSuccess) {
+    pb_table_destroy(t);
+    return fail(PB_ERR_CUDA, std::string("pb_table_create: ") + cudaGetErrorString(e));
+  }
   *out = t;
   return PB_OK;
 }
@@ -473,7 +501,7 @@ int pb_tier_stats(pb_table* t, uint64_t h_out[5], void* stream) {
   if (!t->tier) return PB_OK;
   DeviceGuard g(t->device);
   TableCall call;
-  if (int rc = call.begin(t, (cudaStream_t)stream)) return rc;
+  if (int rc = call.begin(t, (cudaStream_t)stream, CALL_ALL)) return rc;
   uint32_t c[CTR_COUNT];
   PB_CUDA(cudaMemcpyAsync(c, t->tier->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
@@ -527,7 +555,7 @@ int pb_tier_stage_stats(pb_table* t, uint64_t h_out[2], void* stream) {
   if (!t->tier) return PB_OK;
   DeviceGuard g(t->device);
   TableCall call;
-  if (int rc = call.begin(t, (cudaStream_t)stream)) return rc;
+  if (int rc = call.begin(t, (cudaStream_t)stream, CALL_ALL)) return rc;
   uint32_t c[CTR_COUNT];
   PB_CUDA(cudaMemcpyAsync(c, t->tier->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
@@ -572,7 +600,7 @@ int pb_inc_take(pb_table* t, uint64_t* d_signs, uint32_t max_n, uint32_t* d_coun
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if (int rc = call.begin(t, st)) return rc;
+  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
   launch_inc_take(t->inc, d_signs, max_n, d_count, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
@@ -585,7 +613,7 @@ int pb_inc_stats(pb_table* t, uint64_t h_out[4], void* stream) {
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if (int rc = call.begin(t, st)) return rc;
+  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
   unsigned long long c[INC_WORDS];
   PB_CUDA(cudaMemcpyAsync(c, t->inc.ctr, sizeof(c), cudaMemcpyDeviceToHost, st));
   PB_CUDA(cudaStreamSynchronize(st));
@@ -610,6 +638,8 @@ int pb_table_destroy(pb_table* t) {
   if (t->move_cells) cudaFree(t->move_cells);
   if (t->last.ev) cudaEventDestroy(t->last.ev);
   if (t->staged.ev) cudaEventDestroy(t->staged.ev);
+  if (t->index.ev) cudaEventDestroy(t->index.ev);
+  if (t->step.ev) cudaEventDestroy(t->step.ev);
   if (t->allocated) {
     cudaDeviceSynchronize();
     cudaFree(t->d.cells);
@@ -693,7 +723,7 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream) {
   if (!t->allocated) return PB_OK;
   DeviceGuard g(t->device);
   TableCall call;
-  if (int rc = call.begin(t, (cudaStream_t)stream)) return rc;
+  if (int rc = call.begin(t, (cudaStream_t)stream, CALL_ALL)) return rc;
   uint32_t c[CTR_COUNT];
   PB_CUDA(cudaMemcpyAsync(c, t->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
@@ -712,7 +742,7 @@ int pb_table_index_stats(pb_table* t, uint64_t h_out[3], void* stream) {
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if (int rc = call.begin(t, st)) return rc;
+  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
   if (!t->stats_ws) PB_CUDA(cudaMalloc(&t->stats_ws, 3 * sizeof(uint32_t)));
   launch_index_stats(t->d, t->stats_ws, st);
   uint32_t c[3];
@@ -737,7 +767,7 @@ int pb_table_clear(pb_table* t, void* stream) {
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if (int rc = call.begin(t, st)) return rc;
+  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
   launch_fill_cells(t->d.cells, (uint64_t)t->d.n_cells + N_SPECIAL, st);
   PB_CUDA(cudaMemsetAsync(t->d.counters, 0, sizeof(uint32_t) * CTR_COUNT, st));
   PB_CUDA(cudaMemsetAsync(t->d.row_tick, 0, sizeof(uint32_t) * (size_t)t->d.capacity, st));
@@ -757,7 +787,7 @@ int pb_lookup(pb_table* t, const uint64_t* d_signs, uint32_t n, int training, fl
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if (int rc = call.begin(t, st)) return rc;
+  if (int rc = call.begin(t, st, CALL_INDEX)) return rc;
   int rc = ensure_alloc(t);
   if (rc) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
@@ -785,7 +815,7 @@ int pb_update(pb_table* t, const uint64_t* d_signs, const float* d_grads, uint32
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if ((rc = call.begin(t, st))) return rc;
+  if ((rc = call.begin(t, st, CALL_ALL))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
   SlotsDev sl = no_slots();
@@ -817,7 +847,7 @@ int pb_set_rows(pb_table* t, const uint64_t* d_signs, const float* d_entries, ui
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if (int rc = call.begin(t, st)) return rc;
+  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
   int rc = ensure_alloc(t);
   if (rc) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
@@ -838,7 +868,7 @@ int pb_get_rows(pb_table* t, const uint64_t* d_signs, uint32_t n, float* d_entri
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if (int rc = call.begin(t, st)) return rc;
+  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
   int rc = ensure_alloc(t);
   if (rc) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
@@ -857,7 +887,7 @@ int pb_table_export_signs(pb_table* t, uint64_t* d_signs, uint32_t* d_recency, u
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if (int rc = call.begin(t, st)) return rc;
+  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
   if (!t->allocated) {
     PB_CUDA(cudaMemsetAsync(d_count, 0, sizeof(uint32_t), st));
     return PB_OK;
@@ -1061,7 +1091,7 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if ((rc = call.begin(t, st))) return rc;
+  if ((rc = call.begin(t, st, CALL_INDEX))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
@@ -1120,7 +1150,7 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;  // runs beside a pb_tier_stage (see there): waits for none
-  if ((rc = call.begin(t, st, false))) return rc;
+  if ((rc = call.begin(t, st, CALL_STEP, false))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, c->occ_off, sl))) return rc;
   GradsDev gr;
@@ -1565,7 +1595,7 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if ((rc = call.begin(t, st))) return rc;
+  if ((rc = call.begin(t, st, CALL_INDEX))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_raw(c))) return rc;
   if (training && (rc = ensure_raw_stage(c, t->d.dim, st))) return rc;
@@ -1615,7 +1645,7 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;  // runs beside a pb_tier_stage (see there): waits for none
-  if ((rc = call.begin(t, st, false))) return rc;
+  if ((rc = call.begin(t, st, CALL_STEP, false))) return rc;
   drop_raw_pending(c);  // enqueued below: the sweep of the next training call runs after these gradients
   GradsDev gr;
   std::memset(&gr, 0, sizeof(gr));
