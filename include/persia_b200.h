@@ -376,6 +376,13 @@ int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_gr
 
 /* Number of kernels the library has launched on behalf of the caller since load (bench bookkeeping). */
 uint64_t pb_launch_count(void);
+/* Diagnostic: the geometry the backward gives its reduce of hot signs (> 32 occurrences) for rows of `dim` columns
+ * (1..4096), f16 or f32 gradients, and a batch with several ids per sample in some slot (ragged) or one id per sample
+ * in every slot.  Host-only, no device needed.  h_out: [0] EPL columns per chain lane, [1] CH chain warps, [2] PW
+ * producer warps, [3] 16-byte producer loads (else element by element), [4] log2 of the 16-byte vectors per row when
+ * that is a power of two (else 32), [5] the producers' lean loop, [6] R1 rows per producer part, [7] R rows per ring
+ * slot, [8] S ring slots, [9] columns per pass, [10] floats per ring row, [11] column passes. */
+int pb_hot_geometry(uint32_t dim, int is_f16, int ragged, uint32_t h_out[12]);
 /* Bench instrumentation: launches of the kernel families selected by the bit mask are bracketed by CUDA events on
  * their stream (0 = off).  pb_profile_read synchronises the device and returns summed milliseconds and launch
  * counts per family: 0 probe/admit, 1 dedup, 2 gather+pool, 3 NaN scan, 4 reduce+update of hot signs (> 32 occurrences),

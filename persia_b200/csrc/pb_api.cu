@@ -431,6 +431,12 @@ extern "C" {
 const char* pb_last_error(void) { return g_err.c_str(); }
 int pb_version(void) { return 100; }
 uint64_t pb_launch_count(void) { return launch_count(); }
+int pb_hot_geometry(uint32_t dim, int is_f16, int ragged, uint32_t h_out[12]) {
+  if (!h_out) return fail(PB_ERR_INVALID, "null argument");
+  if (dim == 0 || dim > 4096) return fail(PB_ERR_INVALID, "dim must be in 1..4096");
+  hot_geometry(dim, is_f16 != 0, ragged != 0, h_out);
+  return PB_OK;
+}
 int pb_profile_enable(int family_mask) {
   profile_enable((uint32_t)family_mask);
   return PB_OK;

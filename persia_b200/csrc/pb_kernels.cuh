@@ -199,6 +199,8 @@ void launch_nan_scan(const GradsDev& gr, uint32_t n_slots, uint32_t elems_per_sl
 void launch_reduce_items(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl,
                          const GradsDev& gr, bool f16, const ReduceArgs& a, cudaStream_t st, cudaStream_t st_hot, cudaStream_t st_warm,
                          bool send = false);
+// diagnostic (pb_hot_geometry): the geometry launch_reduce_items gives k_reduce_hot
+void hot_geometry(uint32_t dim, bool f16, bool ragged, uint32_t out[12]);
 // pb_shard.cu
 void launch_route_items(bool training, const SlotsDev& sl, const BatchDev& b, const XchgDev& x, cudaStream_t st);
 void launch_link_items(const SlotsDev& sl, const BatchDev& b, const XchgDev& x, const GroupLinks& gl, cudaStream_t st);

@@ -421,6 +421,12 @@ struct HotGeom {
   uint32_t vshift;    // log2(vectors per row) when that is a power of two, else 32
 };
 
+// PW producers share S slots: PW <= S keeps a producer from running two rounds ahead of the chain (the parity of a
+// slot's barrier only tells odd rounds from even ones)
+__host__ __device__ __forceinline__ uint32_t hot_producers(uint32_t CH, uint32_t S) {
+  return HOT_WARPS - CH < S ? HOT_WARPS - CH : S;
+}
+
 // one chunk: rows k0 .. k0+nv-1 of the sorted list, columns [col0, col0+cols) -> prepared f32 in the ring slot.
 // Vector mode: R * (vectors per row) <= 256, i.e. at most eight 16-byte loads per lane, all issued before the first
 // conversion; vector v = j * 32 + lane of the chunk is row v / nvr, vector v % nvr of the row (POW2: by shift and
@@ -581,9 +587,7 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
   float* ring = reinterpret_cast<float*>(smem_raw);                     // [S][R][stride] prepared rows
   float* vstage = ring + (size_t)geo.S * geo.R * geo.stride;            // [dim] Adagrad-vectorwise dot
   const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  // PW producers share S slots: PW <= S keeps a producer from running two rounds ahead of the chain (the parity of a
-  // slot's barrier only tells odd rounds from even ones)
-  const uint32_t CH = geo.CH, PW = min(HOT_WARPS - CH, geo.S);
+  const uint32_t CH = geo.CH, PW = hot_producers(CH, geo.S);
   if (tid == 0) {
     for (uint32_t s = 0; s < HOT_MAX_SLOTS; ++s) {
       mbar_init(smem_u32(bars + s), 32u);                       // every lane of the producing warp
@@ -836,16 +840,23 @@ static void items_dispatch(const TableDev& t, const OptimDev& op, const HyperDev
 static unsigned long long* g_hot_trace = nullptr;  // debugging aid: per hot item {start, sorted, summed} globaltimer stamps
 void set_hot_trace(unsigned long long* p) { g_hot_trace = p; }
 
-template <int EPL, bool F16, bool SEND>
-static void hot_launch(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl, const GradsDev& gr,
-                       const ReduceArgs& a, uint32_t vec, cudaStream_t st) {
+// chain lanes own 2 columns (one or two chain warps) up to 128 columns, 4 above
+static uint32_t hot_epl(uint32_t dim) { return dim <= 128u && dim % 2u == 0 ? 2u : 4u; }
+
+// The hot reduce's geometry for rows of `dim` columns: a function of the dim, the gradient dtype and whether the batch
+// has several ids per sample (ragged: the gradient row of an occurrence is looked up, the lean loop does not apply).
+static HotGeom hot_geom(uint32_t dim, bool f16, bool ragged) {
+  const uint32_t EPL = hot_epl(dim);
   HotGeom g;
-  g.cols = t.dim < HOT_COLS ? t.dim : HOT_COLS;
+  g.cols = dim < HOT_COLS ? dim : HOT_COLS;
   g.stride = (g.cols + 3u) & ~3u;
   g.CH = (g.cols + 32u * EPL - 1u) / (32u * EPL);
-  g.rowbytes = t.dim * (F16 ? 2u : 4u);
+  g.rowbytes = dim * (f16 ? 2u : 4u);
+  // the producers' 16-byte loads need whole vectors per row; the rows are then 16-byte aligned, because the ABI
+  // refuses gradient pointers that are not (pb_api.cu)
+  const uint32_t vec = dim % (f16 ? 8u : 4u) == 0 ? 1u : 0u;
   g.vec = vec;
-  const uint32_t nvr = g.cols / (F16 ? 8u : 4u);
+  const uint32_t nvr = g.cols / (f16 ? 8u : 4u);
   g.vshift = 32u;
   if (vec && nvr && !(nvr & (nvr - 1u)))
     for (g.vshift = 0; (1u << g.vshift) < nvr; ++g.vshift) {}
@@ -856,12 +867,26 @@ static void hot_launch(const TableDev& t, const OptimDev& op, const HyperDev& hy
   g.R &= ~3u;  // the chain adds groups of four rows
   if (g.R < 4u) g.R = 4u;
   if (vec && g.R * nvr > 256u) g.vec = 0;  // (rows longer than 64 vectors per pass: element by element)
-  g.lean = g.vec && g.vshift <= 5u && t.dim <= HOT_COLS && !a.occ_outrow;
+  g.lean = g.vec && g.vshift <= 5u && dim <= HOT_COLS && !ragged;
   // every chunk costs the chain a barrier round trip (~500 cycles measured) whatever its size: up to 64 rows per chunk
   // (parts of R1 rows) where the slot stays within 32 KB; the producers' lean loop converts at most four parts
   g.R1 = g.R;
   while (g.R < 64u && g.R < 4u * g.R1 && 2u * g.R * g.stride * 4u <= 32768u) g.R *= 2u;
   if (g.R * g.stride * 4u > 16384u) g.S = 6;  // 6 x 32 KB (the producers must not outnumber the slots)
+  return g;
+}
+
+void hot_geometry(uint32_t dim, bool f16, bool ragged, uint32_t out[12]) {
+  const HotGeom g = hot_geom(dim, f16, ragged);
+  const uint32_t v[12] = {hot_epl(dim), g.CH, hot_producers(g.CH, g.S), g.vec, g.vshift, g.lean,
+                          g.R1, g.R, g.S, g.cols, g.stride, (dim + HOT_COLS - 1u) / HOT_COLS};
+  for (int i = 0; i < 12; ++i) out[i] = v[i];
+}
+
+template <int EPL, bool F16, bool SEND>
+static void hot_launch(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl, const GradsDev& gr,
+                       const ReduceArgs& a, cudaStream_t st) {
+  const HotGeom g = hot_geom(t.dim, F16, a.occ_outrow != nullptr);
   const size_t smem = (size_t)g.S * g.R * g.stride * 4u + (((size_t)t.dim + 3u) & ~(size_t)3u) * 4u;
   auto kern = k_reduce_hot<EPL, F16, SEND>;
   static size_t configured[64] = {0};  // per instantiation and device
@@ -888,20 +913,15 @@ void launch_reduce_items(const TableDev& t, const OptimDev& op, const HyperDev& 
   uint32_t G = (uint32_t)Gi < 4u ? 4u : (uint32_t)Gi;
   // hot items first in time when they have their own stream: they are the long poles
   {
-    // the producers' 16-byte loads need whole vectors per row; the rows are then 16-byte aligned, because the ABI
-    // refuses gradient pointers that are not (pb_api.cu)
-    const uint32_t ev = f16 ? 8u : 4u;
-    const uint32_t hv = t.dim % ev == 0 ? 1u : 0u;
-    // chain lanes own 2 columns (one or two chain warps) up to 128 columns, 4 above
-#define PB_H(E)                                                                 \
-  if (send) {                                                                   \
-    if (f16) hot_launch<E, true, true>(t, op, hy, sl, gr, a, hv, st_hot);       \
-    else hot_launch<E, false, true>(t, op, hy, sl, gr, a, hv, st_hot);          \
-  } else {                                                                      \
-    if (f16) hot_launch<E, true, false>(t, op, hy, sl, gr, a, hv, st_hot);      \
-    else hot_launch<E, false, false>(t, op, hy, sl, gr, a, hv, st_hot);         \
+#define PB_H(E)                                                             \
+  if (send) {                                                               \
+    if (f16) hot_launch<E, true, true>(t, op, hy, sl, gr, a, st_hot);       \
+    else hot_launch<E, false, true>(t, op, hy, sl, gr, a, st_hot);          \
+  } else {                                                                  \
+    if (f16) hot_launch<E, true, false>(t, op, hy, sl, gr, a, st_hot);      \
+    else hot_launch<E, false, false>(t, op, hy, sl, gr, a, st_hot);         \
   }
-    if (t.dim <= 128u && t.dim % 2u == 0) { PB_H(2) } else { PB_H(4) }
+    if (hot_epl(t.dim) == 2u) { PB_H(2) } else { PB_H(4) }
 #undef PB_H
   }
   if (vec == 4) {

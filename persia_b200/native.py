@@ -95,6 +95,7 @@ SYMBOLS = {
     "pb_forward_raw_sharded": (_i32, [_vp, _vp, _vp, _vp, _u32, _vp, _u32, _u32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32]),
     "pb_backward_raw_sharded": (_i32, [_vp, _vp, _vp, _vp, _i32, C.c_float, _vp, _vp, _i32]),
     "pb_launch_count": (_u64, []),
+    "pb_hot_geometry": (_i32, [_u32, _i32, _i32, C.POINTER(_u32 * 12)]),
     "pb_profile_enable": (_i32, [_i32]),
     "pb_profile_read": (_i32, [C.POINTER(C.c_double), C.POINTER(_u64), _i32]),
 }

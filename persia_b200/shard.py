@@ -429,6 +429,17 @@ def farmhash64(x):
     return out
 
 
+HOT_GEOMETRY_FIELDS = ("EPL", "CH", "PW", "vec", "vshift", "lean", "R1", "R", "S", "cols", "stride", "passes")
+
+
+def hot_geometry(dim, f16, ragged=False):
+    """The geometry the backward gives its reduce of hot signs (include/persia_b200.h, pb_hot_geometry) as a dict keyed
+    by HOT_GEOMETRY_FIELDS.  Host-only."""
+    out = (C.c_uint32 * 12)()
+    N.check(N.load().pb_hot_geometry(int(dim), int(bool(f16)), int(bool(ragged)), C.byref(out)))
+    return dict(zip(HOT_GEOMETRY_FIELDS, out))
+
+
 def partition_by_shard(signs, R):
     """Stable partition: returns (perm int32[n], counts int32[R])."""
     lib = N.load()

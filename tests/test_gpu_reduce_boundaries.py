@@ -116,7 +116,7 @@ def _train(torch, s, ctx, w, oracle, pf, slots, B, dim, rng, kind, f32=False, sc
     g = (rng.standard_normal((S, B, dim)) * 1e-2).astype(np.float32 if f32 else np.float16)
     if not f32:
         g[0, 0, 0] = np.inf  # clamps to 65504 (persia-common lib.rs:163-180)
-        g[0, 1, 1] = -np.inf
+        g[0, 1, min(1, dim - 1)] = -np.inf
     if nan is not None:  # at a sample holding the slot's id 0, its most frequent one
         first = int(np.flatnonzero(slots[nan][0] == 0)[0])
         sample = first if slots[nan][1] is None else int(np.searchsorted(slots[nan][1], first, side="right") - 1)
