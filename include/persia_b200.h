@@ -28,6 +28,7 @@
  *   on another stream is stepping (the staleness embedding_staleness allows).  An eviction check also waits for every
  *   step issued before it, so it never releases a row whose gradients are still to be applied.  pb_set_rows,
  *   pb_get_rows, pb_table_export_signs, pb_table_clear, the statistics calls and pb_inc_take are in both chains.
+ *   pb_tier_stage waits for both chains and is in the index chain only.
  * Waiting costs a stream-wait on an event per call; a wait on work already complete costs nothing on the device.
  * Calls on one table must still be issued from one host thread at a time (the persia_core groups hold a lock), and a
  * pb_ctx holds one batch at a time.  Under CUDA stream capture the ordering becomes edges of the graph when the calls
@@ -144,11 +145,12 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream);
  *
  * Staging (pb_tier_stage): the ids of batch i+1 are known while batch i trains, and moving an entry never changes its
  * value, so the moves of request i+1 can run one batch ahead, on a stream of their own, beside batch i's dense step and
- * backward.  The library orders a stage: it starts after every earlier call on the table (pending backwards included),
- * and every later call on the table or its tier except pb_backward and pb_backward_raw (which run beside it) starts
- * after it.  In a CUDA graph, a stage and the calls after it work when they are captured into one graph, the stage on
- * a stream forked from the capturing one; a call captured after a stage issued outside the capture that has not
- * completed fails with PB_ERR_STATE (synchronise before capturing). */
+ * backward.  The library orders a stage through the two chains above: it starts after every earlier call on the table
+ * (pending backwards included, whatever their streams), and every later call on the table or its tier except
+ * pb_backward and pb_backward_raw (in the step chain alone, they run beside it) starts after it.  In a CUDA graph, a
+ * stage and the calls after it work when they are captured into one graph, the stage on a stream forked from the
+ * capturing one; a call captured after a stage issued outside the capture that has not completed fails with
+ * PB_ERR_STATE (synchronise before capturing). */
 int pb_table_create_host(int device, const pb_table_cfg* cfg, pb_table** out);
 /* Both tables need their optimizer registered; checks dim, optimizer kind and row stride. */
 int pb_table_attach_tier(pb_table* t, pb_table* tier);

@@ -110,11 +110,9 @@ struct pb_table {
   pb_table* tier = nullptr;
   pb_table* tier_of = nullptr;
   uint32_t* move_cells = nullptr;  // the eviction check's victim list (with rebuild_keys / rebuild_rows), `capacity` words
-  // ordering around pb_tier_stage (a table with a tier): `last` is recorded after every call on the table, `staged`
-  // after every stage
-  Mark last, staged;
-  // ordering of calls on several streams (TableCall): `index` after every call that probes or changes the index,
-  // `step` after every call that steps rows, advances Adam's beta powers or marks the incremental set
+  // ordering of calls on several streams (TableCall): `index` after every call that probes or changes the index (or
+  // moves entries between the table and its tier), `step` after every call that steps rows, advances Adam's beta
+  // powers or marks the incremental set
   Mark index, step;
   // incremental updates (pb_table_enable_incremental): the set of signs stepped since the last take; cells == null: off
   IncDev inc{};
@@ -254,10 +252,9 @@ int maybe_evict(pb_table* t, cudaStream_t st) {
   return evict_check(t, st);
 }
 
-// ---- ordering around pb_tier_stage ---------------------------------------------------------------------------------
-// A stage runs on a stream of the caller's choosing, beside the backward of the batch before.  The library orders it:
-// the stage waits for all earlier work on the table (Mark `last`), and every later call but the backwards waits for
-// the stage (Mark `staged`).  Waiting on a completed event costs nothing.
+// ---- event marks ---------------------------------------------------------------------------------------------------
+// A Mark is recorded on the stream of one call, and later calls on other streams wait for it (TableCall, below).
+// Waiting on a completed event costs nothing.
 // Stream capture (CUDA 12.9): a capturing stream may wait only on an event recorded into the same capture (a fork/join
 // inside the graph).  Waiting on an event recorded outside it is invalid without cudaEventWaitExternal, and that flag
 // would make every replay wait on whatever the event's latest record is by then: not the dependency meant here.  So an
@@ -265,7 +262,7 @@ int maybe_evict(pb_table* t, cudaStream_t st) {
 // call fails with PB_ERR_STATE rather than record a dependency it cannot keep.  The query runs under
 // cudaThreadExchangeStreamCaptureMode(relaxed): a global-mode capture forbids it otherwise; querying an event recorded
 // inside a capture stays forbidden, and is never done.  A mark recorded into another capture is part of that graph,
-// whose launches the caller orders: nothing is waited for.  The marks of TableCall (below) follow the same rules.
+// whose launches the caller orders: nothing is waited for.
 
 cudaError_t capture_id(cudaStream_t st, unsigned long long& id) {
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
@@ -317,23 +314,23 @@ int wait_for(const Mark& m, cudaStream_t st) {
 // index cells, the free-row stack or row_tick.  A forward reads rows that a backward beside it may be stepping: a
 // stale read, as staleness allows.  An eviction check also waits for the step chain (evict_check).  Calls that read
 // or write entries or counters outside a batch (set/get rows, export, statistics, takes, clear) are in both chains.
+// A stage (pb_tier_stage) waits for both chains and is in the index chain only, so it starts after every earlier call
+// and every later call but a backward starts after it.
 // Under stream capture the marks follow wait_for: within one capture they become edges of the graph; graphs captured
 // separately are ordered by whoever launches them.
 enum : unsigned { CALL_INDEX = 1, CALL_STEP = 2, CALL_ALL = 3 };
 
-// One call on a table: begin() makes `st` wait for the chains the call is in and, with a tier, for the latest stage
-// (not the backwards, which run beside one); when the call returns it is recorded as the latest of those chains (and,
-// with a tier, as the table's latest work).  A host tier's calls use its table's marks.
+// One call on a table: begin() makes `st` wait for the latest call of every chain in `ch | after`; when the call
+// returns it is recorded as the latest of the chains in `ch`.  A host tier's calls use its table's marks.
 struct TableCall {
   pb_table* m = nullptr;
   cudaStream_t st = nullptr;
   unsigned chains = 0;
-  int begin(pb_table* t, cudaStream_t s, unsigned ch, bool after_stage = true) {
+  int begin(pb_table* t, cudaStream_t s, unsigned ch, unsigned after = 0) {
     pb_table* o = t->tier_of ? t->tier_of : t;
     int rc;
-    if (o->tier && after_stage && (rc = wait_for(o->staged, s))) return rc;
-    if ((ch & CALL_INDEX) && (rc = wait_for(o->index, s))) return rc;
-    if ((ch & CALL_STEP) && (rc = wait_for(o->step, s))) return rc;
+    if (((ch | after) & CALL_INDEX) && (rc = wait_for(o->index, s))) return rc;
+    if (((ch | after) & CALL_STEP) && (rc = wait_for(o->step, s))) return rc;
     m = o;
     st = s;
     chains = ch;
@@ -343,9 +340,19 @@ struct TableCall {
     if (!m) return;
     if (chains & CALL_INDEX) record(m->index, st);
     if (chains & CALL_STEP) record(m->step, st);
-    if (m->tier) record(m->last, st);
   }
 };
+
+// a table's counter words (`n` of them at `src`), copied to the host under a call in both chains; synchronises `st`
+template <typename W>
+int read_counters(pb_table* t, const W* src, W* dst, size_t n, cudaStream_t st) {
+  DeviceGuard g(t->device);
+  TableCall call;
+  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
+  PB_CUDA(cudaMemcpyAsync(dst, src, sizeof(W) * n, cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  return PB_OK;
+}
 
 // signs the HBM table lacks and its tier holds are moved back into HBM rows before they are probed
 void restore_ids(pb_table* t, bool prefix, const SlotsDev& sl, const uint64_t* ids, uint32_t n, cudaStream_t st) {
@@ -395,12 +402,66 @@ int make_slots(const pb_slots_cfg& cfg, const uint32_t* h_occ_off, SlotsDev& s) 
   return PB_OK;
 }
 
+// the slots of ids given as pb_add_prefix takes them: one prefix per slot, no sqrt scaling
+int prefix_slots(const uint32_t* h_occ_off, const uint64_t* h_prefix, uint32_t n_slots, uint32_t prefix_bit,
+                 SlotsDev& s) {
+  if (n_slots == 0 || n_slots > PB_MAX_SLOTS) return fail(PB_ERR_INVALID, "n_slots must be in 1..PB_MAX_SLOTS");
+  pb_slots_cfg cfg;
+  std::memset(&cfg, 0, sizeof(cfg));
+  cfg.n_slots = n_slots;
+  cfg.prefix_bit = prefix_bit;
+  for (uint32_t i = 0; i < n_slots; ++i) cfg.prefix[i] = h_prefix[i];
+  return make_slots(cfg, h_occ_off, s);
+}
+
+// a raw context's one slot over n ids (its samples are ragged: never uniform)
+int raw_slots(const pb_ctx* c, uint32_t n, SlotsDev& s) {
+  const uint32_t occ_off[2] = {0, n};
+  int rc = make_slots(c->slots, occ_off, s);
+  s.uniform = 0;
+  return rc;
+}
+
+int check_slot_offsets(const uint32_t* h_occ_off, uint32_t n_slots, uint32_t n) {
+  if (h_occ_off[0] != 0 || h_occ_off[n_slots] != n) return fail(PB_ERR_INVALID, "slot offsets do not span the id array");
+  for (uint32_t s = 0; s < n_slots; ++s)
+    if (h_occ_off[s] > h_occ_off[s + 1]) return fail(PB_ERR_INVALID, "slot offsets must ascend");
+  return PB_OK;
+}
+
 // gradient, output and update buffers are accessed with vector loads and stores of up to 16 bytes
 bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) != 0; }
 int check_grads_aligned(const void* const* h_grads, uint32_t n_slots) {
   for (uint32_t s = 0; s < n_slots; ++s)
     if (h_grads[s] && misaligned(h_grads[s])) return fail(PB_ERR_INVALID, "gradient pointers must be 16-byte aligned");
   return PB_OK;
+}
+
+// A loss scale is applied unless it is within f32::EPSILON of 1 (mod.rs:751); then its inverse must be finite.
+int loss_scale(float sc, uint8_t& on, float& inv) {
+  on = std::fabs(sc - 1.0f) > 1.1920929e-07f;
+  inv = 1.0f / sc;
+  if (on && !std::isfinite(inv)) return fail(PB_ERR_INVALID, "scale on gradient must be finite");
+  return PB_OK;
+}
+
+// the per-slot gradient table of a summation backward (h_scale null: no loss scale)
+int make_grads(const void* const* h_grads, const float* h_scale, uint32_t n_slots, GradsDev& gr) {
+  std::memset(&gr, 0, sizeof(gr));
+  for (uint32_t s = 0; s < n_slots; ++s) {
+    gr.ptr[s] = h_grads[s];
+    if (int rc = loss_scale(h_scale ? h_scale[s] : 1.0f, gr.do_scale[s], gr.inv_scale[s])) return rc;
+  }
+  return PB_OK;
+}
+
+// one beta-power step of Adam's pair k (one request of one feature group, optim.rs:155-197); returns the pair
+const float* advance_adam_pair(pb_table* t, int k, cudaStream_t st) {
+  AdamKeys keys{};
+  keys.idx[0] = (uint8_t)k;
+  keys.n = 1;
+  launch_adam_advance(t->adam_dev, keys, t->op.b1, t->op.b2, st);
+  return t->adam_dev + 2 * k;
 }
 
 void free_incremental(pb_table* t) {
@@ -422,6 +483,145 @@ void drop_raw_pending(pb_ctx* c) {
   if (c->raw_table && c->raw_table->pending_batches) c->raw_table->pending_batches--;
   c->raw_table = nullptr;
   c->raw_pending = false;
+}
+
+// ---- what the local and sharded forms of the forwards and backwards share ------------------------------------------
+int check_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
+                  const uint32_t* h_slot_occ_off, uint32_t batch, void* d_out_f16) {
+  if (!t || !c || !h_slot_occ_off || !d_out_f16 || (n_occ && !d_ids)) return fail(PB_ERR_INVALID, "null argument");
+  if (misaligned(d_out_f16)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
+  if (!c->has_slots) return fail(PB_ERR_STATE, "pb_ctx_set_slots not called");
+  if (t->device != c->device) return fail(PB_ERR_INVALID, "table and context live on different devices");
+  if (batch > 65535) return fail(PB_ERR_BATCH, "batch size cannot be larger than 65535");
+  const uint32_t S = c->slots.n_slots;
+  const uint64_t n_out = (uint64_t)S * batch;
+  if (n_occ > c->max_occ || n_out > c->max_out) return fail(PB_ERR_CAPACITY, "batch exceeds the context's capacity");
+  if (!d_row_off && n_occ != n_out) return fail(PB_ERR_INVALID, "row offsets are required unless every sample has one id per slot");
+  return check_slot_offsets(h_slot_occ_off, S, n_occ);
+}
+
+int check_raw_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
+                      uint32_t batch, uint32_t sample_fixed_size, void* d_table_f16, int64_t* d_index,
+                      int64_t* d_non_empty, uint32_t* d_sample_id_num, uint32_t* d_counts) {
+  if (!t || !c || !d_table_f16 || !d_index || !d_non_empty || !d_sample_id_num || !d_counts || (n_occ && !d_ids))
+    return fail(PB_ERR_INVALID, "null argument");
+  if (misaligned(d_table_f16)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
+  if (!c->has_slots || c->slots.n_slots != 1) return fail(PB_ERR_STATE, "a raw context serves exactly one slot (pb_ctx_set_slots)");
+  if (t->device != c->device) return fail(PB_ERR_INVALID, "table and context live on different devices");
+  if (batch > 65535) return fail(PB_ERR_BATCH, "batch size cannot be larger than 65535");
+  if (sample_fixed_size == 0) return fail(PB_ERR_INVALID, "sample_fixed_size must be positive");
+  if (n_occ > c->max_occ || batch > c->max_out || (uint64_t)batch * sample_fixed_size > (1ull << 31))
+    return fail(PB_ERR_CAPACITY, "batch exceeds the context's capacity");
+  if (!d_row_off && n_occ != batch) return fail(PB_ERR_INVALID, "row offsets are required unless every sample has one id");
+  return PB_OK;
+}
+
+int check_pending(pb_table* t, pb_ctx* c) {
+  if (!c->pending) return fail(PB_ERR_STATE, "no forward batch is pending in this context (backward_ref_id not found)");
+  if (c->pending_table != t) return fail(PB_ERR_INVALID, "the pending batch was looked up in another table");
+  return PB_OK;
+}
+
+int check_raw_pending(pb_table* t, pb_ctx* c) {
+  if (!c->raw_pending) return fail(PB_ERR_STATE, "no raw forward batch is pending in this context (backward_ref_id not found)");
+  if (c->raw_table != t) return fail(PB_ERR_INVALID, "the pending raw batch was looked up in another table");
+  return PB_OK;
+}
+
+// the context's copy of a batch's row offsets (n_rows + 1) and the output row of every id occurrence
+int copy_row_off(pb_ctx* c, const uint32_t* d_row_off, uint32_t n_rows, cudaStream_t st) {
+  PB_CUDA(cudaMemcpyAsync(c->row_off, d_row_off, 4 * ((size_t)n_rows + 1), cudaMemcpyDeviceToDevice, st));
+  launch_expand_rows(c->row_off, n_rows, c->occ_outrow, st);
+  return PB_OK;
+}
+
+// A summation forward's start: the context's previous batch goes (like an expired post_forward_buffer entry,
+// mod.rs:991-1029), then the new batch's distinct items are found.
+int begin_forward(pb_table* t, pb_ctx* c, const SlotsDev& sl, const uint64_t* d_ids, uint32_t n_occ, int training,
+                  cudaStream_t st) {
+  // a batch whose gradients never came (or an inference request) leaves its cells in the scratch set: empty it first
+  if (c->set_dirty) {
+    launch_clear_items(c->b, st);
+    c->set_dirty = false;
+  }
+  if (c->pending) launch_clear_hot_bits(c->b, st);  // its hot items' bitmaps were never consumed
+  drop_pending(c);
+  if (training) {
+    if (int rc = maybe_evict(t, st)) return rc;
+  }
+  launch_begin_batch(t->d, training ? c->dev_tick : nullptr, c->b.cnt, st, training != 0);
+  c->b.n = n_occ;
+  launch_dedup(sl, c->b, d_ids, st);
+  return PB_OK;
+}
+
+// A summation forward's end: a training batch stays in the context, pending, for its backward (its cells are emptied
+// beside the backward, or by the next forward); an inference request's cells are emptied now.
+int end_forward(pb_table* t, pb_ctx* c, const uint32_t* d_row_off, const uint32_t* h_slot_occ_off, uint32_t n_occ,
+                uint32_t batch, int training, cudaStream_t st) {
+  if (!training) {
+    launch_clear_items(c->b, st);
+    return PB_OK;
+  }
+  const uint32_t S = c->slots.n_slots;
+  c->n_occ = n_occ;
+  c->batch = batch;
+  c->multi_id = d_row_off != nullptr;
+  std::memcpy(c->occ_off, h_slot_occ_off, sizeof(uint32_t) * (S + 1));
+  if (d_row_off) {
+    if (int rc = copy_row_off(c, d_row_off, S * batch, st)) return rc;
+  }
+  c->pending = true;
+  c->pending_table = t;
+  t->pending_batches++;
+  c->set_dirty = true;
+  return PB_OK;
+}
+
+// a raw training forward's batch stays pending in the context, its rows spared by eviction, until its backward
+void hold_raw_batch(pb_table* t, pb_ctx* c, uint32_t n_occ, uint32_t batch) {
+  c->n_occ = n_occ;
+  c->batch = batch;
+  c->raw_pending = true;
+  c->raw_table = t;
+  t->pending_batches++;
+}
+
+// what the reduces of a summation backward read of the context's pending batch
+ReduceArgs reduce_args(const pb_ctx* c) {
+  ReduceArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.b = c->b;
+  a.b.n = c->n_occ;
+  a.occ_outrow = c->multi_id ? c->occ_outrow : nullptr;
+  a.row_off = c->multi_id ? c->row_off : nullptr;
+  a.tick_ptr = c->dev_tick;
+  a.nan_tick = c->nan_tick;
+  a.batch = c->batch;
+  return a;
+}
+
+// A summation backward's side streams: `side` follows `st` from fork_side on; `side` and `side2` follow it from
+// fork_after_nan on (the reduces read the NaN scan's marks); join_sides makes `st` wait for both.
+int fork_side(pb_ctx* c, cudaStream_t st) {
+  PB_CUDA(cudaEventRecord(c->ev_fork, st));
+  PB_CUDA(cudaStreamWaitEvent(c->side, c->ev_fork, 0));
+  return PB_OK;
+}
+
+int fork_after_nan(pb_ctx* c, cudaStream_t st) {
+  PB_CUDA(cudaEventRecord(c->ev_nan, st));
+  PB_CUDA(cudaStreamWaitEvent(c->side, c->ev_nan, 0));
+  PB_CUDA(cudaStreamWaitEvent(c->side2, c->ev_nan, 0));
+  return PB_OK;
+}
+
+int join_sides(pb_ctx* c, cudaStream_t st) {
+  PB_CUDA(cudaEventRecord(c->ev_join, c->side));
+  PB_CUDA(cudaStreamWaitEvent(st, c->ev_join, 0));
+  PB_CUDA(cudaEventRecord(c->ev_join2, c->side2));
+  PB_CUDA(cudaStreamWaitEvent(st, c->ev_join2, 0));
+  return PB_OK;
 }
 
 }  // namespace
@@ -494,8 +694,6 @@ int pb_table_attach_tier(pb_table* t, pb_table* tier) {
   if (t->d.stride != tier->d.stride) return fail(PB_ERR_INVALID, "the tier's row stride differs from the table's");
   if ((rc = ensure_evict_ws(t)) || (rc = ensure_evict_ws(tier))) return rc;
   PB_CUDA(cudaMalloc(&t->move_cells, sizeof(uint32_t) * (size_t)t->d.capacity));
-  PB_CUDA(cudaEventCreateWithFlags(&t->last.ev, cudaEventDisableTiming));
-  PB_CUDA(cudaEventCreateWithFlags(&t->staged.ev, cudaEventDisableTiming));
   t->tier = tier;
   tier->tier_of = t;
   return PB_OK;
@@ -505,12 +703,8 @@ int pb_tier_stats(pb_table* t, uint64_t h_out[5], void* stream) {
   if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
   for (int i = 0; i < 5; ++i) h_out[i] = 0;
   if (!t->tier) return PB_OK;
-  DeviceGuard g(t->device);
-  TableCall call;
-  if (int rc = call.begin(t, (cudaStream_t)stream, CALL_ALL)) return rc;
   uint32_t c[CTR_COUNT];
-  PB_CUDA(cudaMemcpyAsync(c, t->tier->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  if (int rc = read_counters(t, t->tier->d.counters, c, CTR_COUNT, (cudaStream_t)stream)) return rc;
   h_out[0] = c[CTR_ADMIT] - c[CTR_EVICT] - c[CTR_TIER_IN];
   h_out[1] = c[CTR_TIER_OUT];
   h_out[2] = c[CTR_TIER_IN];
@@ -525,46 +719,36 @@ int pb_tier_stage(pb_table* t, const uint64_t* d_ids, uint32_t n, const uint32_t
   if (t->tier_of) return fail(PB_ERR_STATE, "a host tier is not staged directly: use the table it is attached to");
   if (n_slots == 0 || n_slots > PB_MAX_SLOTS) return fail(PB_ERR_INVALID, "n_slots must be in 1..PB_MAX_SLOTS");
   if (prefix_bit == 0 || prefix_bit > 63) return fail(PB_ERR_INVALID, "feature_index_prefix_bit must be in 1..63");
-  if (h_slot_occ_off[0] != 0 || h_slot_occ_off[n_slots] != n) return fail(PB_ERR_INVALID, "slot offsets do not span the id array");
-  for (uint32_t s = 0; s < n_slots; ++s)
-    if (h_slot_occ_off[s] > h_slot_occ_off[s + 1]) return fail(PB_ERR_INVALID, "slot offsets must ascend");
-  if (!t->tier) return PB_OK;  // nothing to move
-  int rc = ready_for_training(t);
+  int rc = check_slot_offsets(h_slot_occ_off, n_slots, n);
   if (rc) return rc;
-  pb_slots_cfg cfg;
-  std::memset(&cfg, 0, sizeof(cfg));
-  cfg.n_slots = n_slots;
-  cfg.prefix_bit = prefix_bit;
-  for (uint32_t i = 0; i < n_slots; ++i) cfg.prefix[i] = h_prefix[i];
+  if (!t->tier) return PB_OK;  // nothing to move
+  if ((rc = ready_for_training(t))) return rc;
   SlotsDev sl;
-  if ((rc = make_slots(cfg, h_slot_occ_off, sl))) return rc;
+  if ((rc = prefix_slots(h_slot_occ_off, h_prefix, n_slots, prefix_bit, sl))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
-  // Every earlier call on the table first (enqueued backwards included); every later call but the backwards waits for
-  // this stage.  Why it may run beside a backward: no backward kernel reads index cells, the free-row stack or
-  // row_tick (the only index read outside the forward path is k_raw_table's, in the raw forward, which waits), and a
-  // backward writes only the rows of its own batch, which are never victims here (keep > pending_batches) nor restore
-  // targets (those come off the free stack).  Counters it shares with a backward are updated atomically.
-  if ((rc = wait_for(t->last, st))) return rc;
+  // After both chains, in the index chain only: every earlier call on the table first (enqueued backwards included),
+  // and every later call but the backwards after this stage.  Why it may run beside a backward: no backward kernel
+  // reads index cells, the free-row stack or row_tick (the only index read outside the forward path is k_raw_table's,
+  // in the raw forward, which waits), and a backward writes only the rows of its own batch, which are never victims
+  // here (keep > pending_batches) nor restore targets (those come off the free stack).  Counters it shares with a
+  // backward are updated atomically.
+  TableCall call;
+  if ((rc = call.begin(t, st, CALL_INDEX, CALL_STEP))) return rc;
   // the check the request would run (not counted in train_calls, so the request's own stays where it was: after a
   // stage it usually finds enough free rows and does nothing); keep covers the batches pending now
   if (t->evict_every && (rc = evict_check(t, st, g_stage_blocks))) return rc;
   launch_tier_stage(t->d, t->tier->d, t->hy, t->op, sl, d_ids, n, g_stage_blocks, st);
   PB_CUDA(cudaGetLastError());
-  if ((rc = record(t->staged, st))) return rc;
-  return record(t->last, st);
+  return PB_OK;
 }
 
 int pb_tier_stage_stats(pb_table* t, uint64_t h_out[2], void* stream) {
   if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
   h_out[0] = h_out[1] = 0;
   if (!t->tier) return PB_OK;
-  DeviceGuard g(t->device);
-  TableCall call;
-  if (int rc = call.begin(t, (cudaStream_t)stream, CALL_ALL)) return rc;
   uint32_t c[CTR_COUNT];
-  PB_CUDA(cudaMemcpyAsync(c, t->tier->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  if (int rc = read_counters(t, t->tier->d.counters, c, CTR_COUNT, (cudaStream_t)stream)) return rc;
   h_out[0] = c[CTR_STAGE_IN];
   h_out[1] = c[CTR_STAGE_SKIP];
   return PB_OK;
@@ -616,13 +800,8 @@ int pb_inc_stats(pb_table* t, uint64_t h_out[4], void* stream) {
   if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
   for (int i = 0; i < 4; ++i) h_out[i] = 0;
   if (!t->inc.cells) return PB_OK;
-  DeviceGuard g(t->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  TableCall call;
-  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
   unsigned long long c[INC_WORDS];
-  PB_CUDA(cudaMemcpyAsync(c, t->inc.ctr, sizeof(c), cudaMemcpyDeviceToHost, st));
-  PB_CUDA(cudaStreamSynchronize(st));
+  if (int rc = read_counters(t, t->inc.ctr, c, INC_WORDS, (cudaStream_t)stream)) return rc;
   h_out[0] = c[INC_HELD];
   h_out[1] = c[INC_INSERTED];
   h_out[2] = c[INC_DROPPED];
@@ -642,8 +821,6 @@ int pb_table_destroy(pb_table* t) {
   if (t->tier) t->tier->tier_of = nullptr;
   if (t->tier_of) t->tier_of->tier = nullptr;
   if (t->move_cells) cudaFree(t->move_cells);
-  if (t->last.ev) cudaEventDestroy(t->last.ev);
-  if (t->staged.ev) cudaEventDestroy(t->staged.ev);
   if (t->index.ev) cudaEventDestroy(t->index.ev);
   if (t->step.ev) cudaEventDestroy(t->step.ev);
   if (t->allocated) {
@@ -727,12 +904,8 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream) {
   if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
   h_out[0] = h_out[1] = h_out[2] = h_out[3] = h_out[4] = 0;
   if (!t->allocated) return PB_OK;
-  DeviceGuard g(t->device);
-  TableCall call;
-  if (int rc = call.begin(t, (cudaStream_t)stream, CALL_ALL)) return rc;
   uint32_t c[CTR_COUNT];
-  PB_CUDA(cudaMemcpyAsync(c, t->d.counters, sizeof(c), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-  PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  if (int rc = read_counters(t, t->d.counters, c, CTR_COUNT, (cudaStream_t)stream)) return rc;
   h_out[0] = c[CTR_ADMIT] - c[CTR_EVICT] - c[CTR_TIER_IN];  // resident rows (a tier's restored rows left it)
   h_out[1] = c[CTR_MISS];
   h_out[2] = c[CTR_GRAD_MISS];
@@ -830,14 +1003,8 @@ int pb_update(pb_table* t, const uint64_t* d_signs, const float* d_grads, uint32
     if ((rc = ensure_scratch(t->tier, n))) return rc;
     launch_tier_where(t->d, t->tier->d, d_signs, t->scratch, n, t->tier->scratch, st);
   }
-  const float* pair = nullptr;
-  if (t->op.kind == PB_OPT_ADAM) {  // get_batch_level_state: one power step per request (optim.rs:155-197)
-    AdamKeys k{};
-    k.idx[0] = (uint8_t)(PB_ADAM_KEYS - 1);
-    k.n = 1;
-    launch_adam_advance(t->adam_dev, k, t->op.b1, t->op.b2, st);
-    pair = t->adam_dev + 2 * (PB_ADAM_KEYS - 1);
-  }
+  // get_batch_level_state: one power step per request
+  const float* pair = t->op.kind == PB_OPT_ADAM ? advance_adam_pair(t, PB_ADAM_KEYS - 1, st) : nullptr;
   launch_update_direct(t->d, t->op, t->hy, t->scratch, d_grads, n, pair, st);
   if (t->tier) launch_update_direct(t->tier->d, t->op, t->hy, t->tier->scratch, d_grads, n, pair, st);
   if (t->inc.cells && n)  // the signs just stepped, in HBM or in the tier
@@ -907,14 +1074,8 @@ int pb_add_prefix(const uint64_t* d_ids, uint32_t n, const uint32_t* h_slot_occ_
                   uint32_t n_slots, uint32_t prefix_bit, uint64_t* d_out, void* stream) {
   if (n && (!d_ids || !d_out)) return fail(PB_ERR_INVALID, "null argument");
   if (!h_slot_occ_off || !h_prefix) return fail(PB_ERR_INVALID, "null argument");
-  pb_slots_cfg cfg;
-  std::memset(&cfg, 0, sizeof(cfg));
-  cfg.n_slots = n_slots;
-  cfg.prefix_bit = prefix_bit;
-  if (n_slots == 0 || n_slots > PB_MAX_SLOTS) return fail(PB_ERR_INVALID, "n_slots must be in 1..PB_MAX_SLOTS");
-  for (uint32_t i = 0; i < n_slots; ++i) cfg.prefix[i] = h_prefix[i];
   SlotsDev sl;
-  int rc = make_slots(cfg, h_slot_occ_off, sl);
+  int rc = prefix_slots(h_slot_occ_off, h_prefix, n_slots, prefix_bit, sl);
   if (rc) return rc;
   launch_add_prefix(sl, d_ids, n, d_out, (cudaStream_t)stream);
   PB_CUDA(cudaGetLastError());
@@ -1074,19 +1235,9 @@ int pb_ctx_batch_stats(pb_ctx* c, uint32_t h_out[6], void* stream) {
 
 int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
                const uint32_t* h_slot_occ_off, uint32_t batch, int training, void* d_out_f16, void* stream) {
-  if (!t || !c || !h_slot_occ_off || !d_out_f16 || (n_occ && !d_ids)) return fail(PB_ERR_INVALID, "null argument");
-  if (misaligned(d_out_f16)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
-  if (!c->has_slots) return fail(PB_ERR_STATE, "pb_ctx_set_slots not called");
-  if (t->device != c->device) return fail(PB_ERR_INVALID, "table and context live on different devices");
-  if (batch > 65535) return fail(PB_ERR_BATCH, "batch size cannot be larger than 65535");
-  uint32_t S = c->slots.n_slots;
-  uint64_t n_out = (uint64_t)S * batch;
-  if (n_occ > c->max_occ || n_out > c->max_out) return fail(PB_ERR_CAPACITY, "batch exceeds the context's capacity");
-  if (!d_row_off && n_occ != n_out) return fail(PB_ERR_INVALID, "row offsets are required unless every sample has one id per slot");
-  if (h_slot_occ_off[0] != 0 || h_slot_occ_off[S] != n_occ) return fail(PB_ERR_INVALID, "slot offsets do not span the id array");
-  for (uint32_t s = 0; s < S; ++s)
-    if (h_slot_occ_off[s] > h_slot_occ_off[s + 1]) return fail(PB_ERR_INVALID, "slot offsets must ascend");
-  int rc;
+  int rc = check_forward(t, c, d_ids, n_occ, d_row_off, h_slot_occ_off, batch, d_out_f16);
+  if (rc) return rc;
+  const uint64_t n_out = (uint64_t)c->slots.n_slots * batch;
   if (training) {
     if ((rc = ready_for_training(t))) return rc;
   } else if (!t->has_op) {
@@ -1101,19 +1252,7 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   if ((rc = ensure_alloc(t))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
-  // a batch whose gradients never came (or an inference request) leaves its cells in the scratch set: empty it first
-  if (c->set_dirty) {
-    launch_clear_items(c->b, st);
-    c->set_dirty = false;
-  }
-  if (c->pending) launch_clear_hot_bits(c->b, st);  // its hot items' bitmaps were never consumed
-  drop_pending(c);  // like an expired post_forward_buffer entry (mod.rs:991-1029)
-  if (training) {
-    if ((rc = maybe_evict(t, st))) return rc;
-  }
-  launch_begin_batch(t->d, training ? c->dev_tick : nullptr, c->b.cnt, st, training != 0);
-  c->b.n = n_occ;
-  launch_dedup(sl, c->b, d_ids, st);
+  if ((rc = begin_forward(t, c, sl, d_ids, n_occ, training, st))) return rc;
   // a training batch moves its tier-held signs into HBM rows (each distinct sign once); inference reads them in place
   if (t->tier && training) launch_tier_restore_items(t->d, t->tier->d, t->hy, t->op, c->b, st);
   launch_probe_items(training != 0, t->d, t->hy, t->op, sl, c->b, st);
@@ -1124,22 +1263,7 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   } else {
     launch_gather_items(t->d, sl, c->b, d_row_off, (uint32_t)n_out, batch, training != 0, d_out_f16, st);
   }
-  if (training) {
-    c->n_occ = n_occ;
-    c->batch = batch;
-    c->multi_id = d_row_off != nullptr;
-    std::memcpy(c->occ_off, h_slot_occ_off, sizeof(uint32_t) * (S + 1));
-    if (d_row_off) {
-      PB_CUDA(cudaMemcpyAsync(c->row_off, d_row_off, 4 * (n_out + 1), cudaMemcpyDeviceToDevice, st));
-      launch_expand_rows(c->row_off, (uint32_t)n_out, c->occ_outrow, st);
-    }
-    c->pending = true;
-    c->pending_table = t;
-    t->pending_batches++;
-    c->set_dirty = true;  // emptied beside the backward (or by the next forward)
-  } else {
-    launch_clear_items(c->b, st);
-  }
+  if ((rc = end_forward(t, c, d_row_off, h_slot_occ_off, n_occ, batch, training, st))) return rc;
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -1147,28 +1271,19 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
 int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, const float* h_scale,
                 int32_t* d_slot_status, void* stream) {
   if (!t || !c || !h_grads) return fail(PB_ERR_INVALID, "null argument");
-  if (!c->pending) return fail(PB_ERR_STATE, "no forward batch is pending in this context (backward_ref_id not found)");
-  if (c->pending_table != t) return fail(PB_ERR_INVALID, "the pending batch was looked up in another table");
-  int rc = ready_for_training(t);
+  int rc = check_pending(t, c);
   if (rc) return rc;
+  if ((rc = ready_for_training(t))) return rc;
   uint32_t S = c->slots.n_slots;
   if ((rc = check_grads_aligned(h_grads, S))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
-  TableCall call;  // runs beside a pb_tier_stage (see there): waits for none
-  if ((rc = call.begin(t, st, CALL_STEP, false))) return rc;
+  TableCall call;  // in the step chain only: runs beside the next forward and a pb_tier_stage (see there)
+  if ((rc = call.begin(t, st, CALL_STEP))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, c->occ_off, sl))) return rc;
   GradsDev gr;
-  std::memset(&gr, 0, sizeof(gr));
-  for (uint32_t s = 0; s < S; ++s) {
-    gr.ptr[s] = h_grads[s];
-    float sc = h_scale ? h_scale[s] : 1.0f;
-    gr.do_scale[s] = std::fabs(sc - 1.0f) > 1.1920929e-07f;
-    float inv = 1.0f / sc;
-    if (gr.do_scale[s] && !std::isfinite(inv)) return fail(PB_ERR_INVALID, "scale on gradient must be finite");
-    gr.inv_scale[s] = inv;
-  }
+  if ((rc = make_grads(h_grads, h_scale, S, gr))) return rc;
   AdamKeys adam_keys{};
   if (t->op.kind == PB_OPT_ADAM) {  // get_batch_level_state: one power step per request and feature group
     AdamKeys keys{};
@@ -1198,8 +1313,7 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
     vw = c->vw_stage;
   }
   // beside the main stream: the scratch set is emptied and, once the NaN marks are known, the hot items are reduced
-  PB_CUDA(cudaEventRecord(c->ev_fork, st));
-  PB_CUDA(cudaStreamWaitEvent(c->side, c->ev_fork, 0));
+  if ((rc = fork_side(c, st))) return rc;
   const bool mark = t->inc.cells != nullptr;  // the mark reads the scratch set and empties it after the steps
   if (c->set_dirty && !mark) {
     launch_clear_items(c->b, c->side);
@@ -1208,20 +1322,9 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
   uint32_t elems = c->batch * t->d.dim;
   launch_nan_scan(gr, S, elems, is_f16 != 0, c->dev_tick, c->nan_tick, d_slot_status, st);
   if (adam_keys.n) launch_adam_advance(t->adam_dev, adam_keys, t->op.b1, t->op.b2, st, &gr, S, c->dev_tick, c->nan_tick);
-  PB_CUDA(cudaEventRecord(c->ev_nan, st));
-  PB_CUDA(cudaStreamWaitEvent(c->side, c->ev_nan, 0));
-  PB_CUDA(cudaStreamWaitEvent(c->side2, c->ev_nan, 0));
-  ReduceArgs a;
-  std::memset(&a, 0, sizeof(a));
-  a.b = c->b;
-  a.b.n = c->n_occ;
-  a.occ_outrow = c->multi_id ? c->occ_outrow : nullptr;
-  a.row_off = c->multi_id ? c->row_off : nullptr;
-  a.tick_ptr = c->dev_tick;
-  a.nan_tick = c->nan_tick;
+  if ((rc = fork_after_nan(c, st))) return rc;
+  ReduceArgs a = reduce_args(c);
   a.vw_stage = vw;
-  a.batch = c->batch;
-  a.quiet_miss = 0;
   for (uint32_t r = 0; r < c->n_rounds; ++r) {
     a.round = r;
     std::memset(a.round_mask, 0, sizeof(a.round_mask));
@@ -1232,10 +1335,7 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
     const bool one = c->n_rounds == 1 && !profiling();  // (timed alone when the bench instruments a family)
     launch_reduce_items(t->d, t->op, t->hy, sl, gr, is_f16 != 0, a, st, one ? c->side : st, one ? c->side2 : st, false);
   }
-  PB_CUDA(cudaEventRecord(c->ev_join, c->side));
-  PB_CUDA(cudaStreamWaitEvent(st, c->ev_join, 0));
-  PB_CUDA(cudaEventRecord(c->ev_join2, c->side2));
-  PB_CUDA(cudaStreamWaitEvent(st, c->ev_join2, 0));
+  if ((rc = join_sides(c, st))) return rc;
   if (mark) {  // every round has stepped: the applied items that had a row
     IncSlots on{};
     for (uint32_t s = 0; s < S; ++s)
@@ -1401,22 +1501,14 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
                        int phases) {
   if (phases == 0) phases = PB_PHASE_ALL;
   const bool all = phases == PB_PHASE_ALL;
-  if (!t || !c || !x || !h_slot_occ_off || !d_out_f16 || (n_occ && !d_ids)) return fail(PB_ERR_INVALID, "null argument");
+  if (!x) return fail(PB_ERR_INVALID, "null argument");
+  int rc = check_forward(t, c, d_ids, n_occ, d_row_off, h_slot_occ_off, batch, d_out_f16);
+  if (rc) return rc;
   if (t->tier) return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no sharded calls)");
-  if (misaligned(d_out_f16)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
-  if (!c->has_slots) return fail(PB_ERR_STATE, "pb_ctx_set_slots not called");
-  if (t->device != c->device || t->device != x->device) return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
+  if (t->device != x->device) return fail(PB_ERR_INVALID, "table and exchange live on different devices");
   if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
-  if (batch > 65535) return fail(PB_ERR_BATCH, "batch size cannot be larger than 65535");
   if (d_row_off && !x->d.row_f32) return fail(PB_ERR_INVALID, "ragged layouts need an exchange created with f32 rows");
-  uint32_t S = c->slots.n_slots;
-  uint64_t n_out = (uint64_t)S * batch;
-  if (n_occ > c->max_occ || n_out > c->max_out) return fail(PB_ERR_CAPACITY, "batch exceeds the context's capacity");
-  if (!d_row_off && n_occ != n_out) return fail(PB_ERR_INVALID, "row offsets are required unless every sample has one id per slot");
-  if (h_slot_occ_off[0] != 0 || h_slot_occ_off[S] != n_occ) return fail(PB_ERR_INVALID, "slot offsets do not span the id array");
-  for (uint32_t s = 0; s < S; ++s)
-    if (h_slot_occ_off[s] > h_slot_occ_off[s + 1]) return fail(PB_ERR_INVALID, "slot offsets must ascend");
-  int rc;
+  const uint64_t n_out = (uint64_t)c->slots.n_slots * batch;
   // every rank serves lookups whether or not its own batch trains: the shard must be usable (a collective call)
   if ((rc = ready_for_training(t))) return rc;
   DeviceGuard g(t->device);
@@ -1425,18 +1517,7 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
   if (phases & PB_PHASE_SEND) {
-    if (c->set_dirty) {
-      launch_clear_items(c->b, st);
-      c->set_dirty = false;
-    }
-    if (c->pending) launch_clear_hot_bits(c->b, st);
-    drop_pending(c);
-    if (training) {
-      if ((rc = maybe_evict(t, st))) return rc;
-    }
-    launch_begin_batch(t->d, training ? c->dev_tick : nullptr, c->b.cnt, st, training != 0);
-    c->b.n = n_occ;
-    launch_dedup(sl, c->b, d_ids, st);
+    if ((rc = begin_forward(t, c, sl, d_ids, n_occ, training, st))) return rc;
     launch_route_items(training != 0, sl, c->b, x->d, st);               // requester: signs -> owners' areas
     if (training && c->n_rounds > 1) launch_link_items(sl, c->b, x->d, c->links, st);  // a sign's entries, slot order
     if (all) launch_signal_wait(x->d, XC_FLAG_SIGN, c->b.cnt + BC_PEER, st);  // (one launch when no phase split is asked for)
@@ -1456,22 +1537,7 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
   }
   if (!all) launch_wait(x->d, XC_FLAG_ROW, -1, st);
   launch_expand_items(t->d, sl, c->b, x->d, d_row_off, (uint32_t)n_out, batch, training != 0, d_out_f16, st);
-  if (training) {
-    c->n_occ = n_occ;
-    c->batch = batch;
-    c->multi_id = d_row_off != nullptr;
-    std::memcpy(c->occ_off, h_slot_occ_off, sizeof(uint32_t) * (S + 1));
-    if (d_row_off) {
-      PB_CUDA(cudaMemcpyAsync(c->row_off, d_row_off, 4 * (n_out + 1), cudaMemcpyDeviceToDevice, st));
-      launch_expand_rows(c->row_off, (uint32_t)n_out, c->occ_outrow, st);
-    }
-    c->pending = true;
-    c->pending_table = t;
-    t->pending_batches++;
-    c->set_dirty = true;
-  } else {
-    launch_clear_items(c->b, st);
-  }
+  if ((rc = end_forward(t, c, d_row_off, h_slot_occ_off, n_occ, batch, training, st))) return rc;
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -1480,10 +1546,9 @@ int pb_backward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* const* h
                         int32_t* d_slot_status, void* stream, int phases) {
   if (phases == 0) phases = PB_PHASE_ALL;
   if (!t || !c || !x || !h_grads) return fail(PB_ERR_INVALID, "null argument");
-  if (!c->pending) return fail(PB_ERR_STATE, "no forward batch is pending in this context (backward_ref_id not found)");
-  if (c->pending_table != t) return fail(PB_ERR_INVALID, "the pending batch was looked up in another table");
-  int rc = ready_for_training(t);
+  int rc = check_pending(t, c);
   if (rc) return rc;
+  if ((rc = ready_for_training(t))) return rc;
   uint32_t S = c->slots.n_slots;
   if ((rc = check_grads_aligned(h_grads, S))) return rc;
   DeviceGuard g(t->device);
@@ -1491,47 +1556,23 @@ int pb_backward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* const* h
   SlotsDev sl;
   if ((rc = make_slots(c->slots, c->occ_off, sl))) return rc;
   GradsDev gr;
-  std::memset(&gr, 0, sizeof(gr));
-  for (uint32_t s = 0; s < S; ++s) {
-    gr.ptr[s] = h_grads[s];
-    float sc = h_scale ? h_scale[s] : 1.0f;
-    gr.do_scale[s] = std::fabs(sc - 1.0f) > 1.1920929e-07f;
-    float inv = 1.0f / sc;
-    if (gr.do_scale[s] && !std::isfinite(inv)) return fail(PB_ERR_INVALID, "scale on gradient must be finite");
-    gr.inv_scale[s] = inv;
-  }
+  if ((rc = make_grads(h_grads, h_scale, S, gr))) return rc;
   if (phases & PB_PHASE_SEND) {
-  PB_CUDA(cudaEventRecord(c->ev_fork, st));
-  PB_CUDA(cudaStreamWaitEvent(c->side, c->ev_fork, 0));
-  if (c->set_dirty) {
-    launch_clear_items(c->b, c->side);
-    c->set_dirty = false;
-  }
-  launch_nan_scan(gr, S, c->batch * t->d.dim, is_f16 != 0, c->dev_tick, c->nan_tick, d_slot_status, st);  // per slot, on the requester (mod.rs:731-746)
-  PB_CUDA(cudaEventRecord(c->ev_nan, st));
-  PB_CUDA(cudaStreamWaitEvent(c->side, c->ev_nan, 0));
-  PB_CUDA(cudaStreamWaitEvent(c->side2, c->ev_nan, 0));
-  ReduceArgs a;
-  std::memset(&a, 0, sizeof(a));
-  a.b = c->b;
-  a.b.n = c->n_occ;
-  a.occ_outrow = c->multi_id ? c->occ_outrow : nullptr;
-  a.row_off = c->multi_id ? c->row_off : nullptr;
-  a.tick_ptr = c->dev_tick;
-  a.nan_tick = c->nan_tick;
-  a.batch = c->batch;
-  a.round = 0;
-  for (uint32_t s = 0; s < S; ++s) a.round_mask[s >> 5] |= 1u << (s & 31);
-  a.x = x->d;
-  PB_CUDA(cudaStreamWaitEvent(c->side2, c->ev_nan, 0));
-  launch_reduce_items(t->d, t->op, t->hy, sl, gr, is_f16 != 0, a, st, profiling() ? st : c->side, profiling() ? st : c->side2,
-                      true);  // requester: gradients -> owners' areas
-  PB_CUDA(cudaEventRecord(c->ev_join, c->side));
-  PB_CUDA(cudaStreamWaitEvent(st, c->ev_join, 0));
-  PB_CUDA(cudaEventRecord(c->ev_join2, c->side2));
-  PB_CUDA(cudaStreamWaitEvent(st, c->ev_join2, 0));
-  if (phases == PB_PHASE_ALL && t->op.kind != PB_OPT_ADAGRAD_VW) launch_signal_wait(x->d, XC_FLAG_GRAD, nullptr, st);
-  else launch_signal(x->d, XC_FLAG_GRAD, nullptr, st);
+    if ((rc = fork_side(c, st))) return rc;
+    if (c->set_dirty) {
+      launch_clear_items(c->b, c->side);
+      c->set_dirty = false;
+    }
+    launch_nan_scan(gr, S, c->batch * t->d.dim, is_f16 != 0, c->dev_tick, c->nan_tick, d_slot_status, st);  // per slot, on the requester (mod.rs:731-746)
+    if ((rc = fork_after_nan(c, st))) return rc;
+    ReduceArgs a = reduce_args(c);
+    for (uint32_t s = 0; s < S; ++s) a.round_mask[s >> 5] |= 1u << (s & 31);
+    a.x = x->d;
+    launch_reduce_items(t->d, t->op, t->hy, sl, gr, is_f16 != 0, a, st, profiling() ? st : c->side,
+                        profiling() ? st : c->side2, true);  // requester: gradients -> owners' areas
+    if ((rc = join_sides(c, st))) return rc;
+    if (phases == PB_PHASE_ALL && t->op.kind != PB_OPT_ADAGRAD_VW) launch_signal_wait(x->d, XC_FLAG_GRAD, nullptr, st);
+    else launch_signal(x->d, XC_FLAG_GRAD, nullptr, st);
   }
   if (!(phases & PB_PHASE_SERVE)) {
     PB_CUDA(cudaGetLastError());
@@ -1582,17 +1623,9 @@ static int ensure_raw_stage(pb_ctx* c, uint32_t dim, cudaStream_t st) {
 int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
                    uint32_t batch, uint32_t sample_fixed_size, int training, void* d_table_f16, int64_t* d_index,
                    int64_t* d_non_empty, uint32_t* d_sample_id_num, uint32_t* d_counts, void* stream) {
-  if (!t || !c || !d_table_f16 || !d_index || !d_non_empty || !d_sample_id_num || !d_counts || (n_occ && !d_ids))
-    return fail(PB_ERR_INVALID, "null argument");
-  if (misaligned(d_table_f16)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
-  if (!c->has_slots || c->slots.n_slots != 1) return fail(PB_ERR_STATE, "a raw context serves exactly one slot (pb_ctx_set_slots)");
-  if (t->device != c->device) return fail(PB_ERR_INVALID, "table and context live on different devices");
-  if (batch > 65535) return fail(PB_ERR_BATCH, "batch size cannot be larger than 65535");
-  if (sample_fixed_size == 0) return fail(PB_ERR_INVALID, "sample_fixed_size must be positive");
-  if (n_occ > c->max_occ || batch > c->max_out || (uint64_t)batch * sample_fixed_size > (1ull << 31))
-    return fail(PB_ERR_CAPACITY, "batch exceeds the context's capacity");
-  if (!d_row_off && n_occ != batch) return fail(PB_ERR_INVALID, "row offsets are required unless every sample has one id");
-  int rc;
+  int rc = check_raw_forward(t, c, d_ids, n_occ, d_row_off, batch, sample_fixed_size, d_table_f16, d_index, d_non_empty,
+                             d_sample_id_num, d_counts);
+  if (rc) return rc;
   if (training) {
     if ((rc = ready_for_training(t))) return rc;
   } else if (!t->has_op) {
@@ -1605,10 +1638,8 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   if ((rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_raw(c))) return rc;
   if (training && (rc = ensure_raw_stage(c, t->d.dim, st))) return rc;
-  const uint32_t occ_off[2] = {0, n_occ};
   SlotsDev sl;
-  if ((rc = make_slots(c->slots, occ_off, sl))) return rc;
-  sl.uniform = 0;
+  if ((rc = raw_slots(c, n_occ, sl))) return rc;
   drop_raw_pending(c);  // the numbering below replaces the pending batch's
   if (training) {
     if ((rc = maybe_evict(t, st))) return rc;
@@ -1618,24 +1649,14 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   } else {
     launch_probe(MODE_FIND, true, t->d, t->hy, t->op, sl, d_ids, n_occ, c->occ_cell, st);
   }
-  const uint32_t* occ_sample = nullptr;
-  if (d_row_off) {
-    PB_CUDA(cudaMemcpyAsync(c->row_off, d_row_off, 4 * ((size_t)batch + 1), cudaMemcpyDeviceToDevice, st));
-    launch_expand_rows(c->row_off, batch, c->occ_outrow, st);
-    occ_sample = c->occ_outrow;
-  }
-  launch_raw_forward(t->d, sl, d_ids, n_occ, d_row_off ? c->row_off : nullptr, occ_sample, batch, sample_fixed_size,
-                     c->occ_cell, c->raw, d_table_f16, (long long*)d_index, (long long*)d_non_empty, d_sample_id_num, st);
+  if (d_row_off && (rc = copy_row_off(c, d_row_off, batch, st))) return rc;
+  launch_raw_forward(t->d, sl, d_ids, n_occ, d_row_off ? c->row_off : nullptr, d_row_off ? c->occ_outrow : nullptr,
+                     batch, sample_fixed_size, c->occ_cell, c->raw, d_table_f16, (long long*)d_index,
+                     (long long*)d_non_empty, d_sample_id_num, st);
   if (!training && t->tier)  // inference moves nothing: tier-held signs are read where they are
     launch_tier_raw_fill(t->d, t->tier->d, sl, d_ids, n_occ, c->occ_cell, c->raw, d_table_f16, st);
   PB_CUDA(cudaMemcpyAsync(d_counts, c->raw.counts, 8, cudaMemcpyDeviceToDevice, st));
-  if (training) {
-    c->n_occ = n_occ;
-    c->batch = batch;
-    c->raw_pending = true;
-    c->raw_table = t;
-    t->pending_batches++;
-  }
+  if (training) hold_raw_batch(t, c, n_occ, batch);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -1643,15 +1664,14 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
 int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, float scale, int32_t* d_status,
                     void* stream) {
   if (!t || !c) return fail(PB_ERR_INVALID, "null argument");
-  if (!c->raw_pending) return fail(PB_ERR_STATE, "no raw forward batch is pending in this context (backward_ref_id not found)");
-  if (c->raw_table != t) return fail(PB_ERR_INVALID, "the pending raw batch was looked up in another table");
-  if (d_grad && misaligned(d_grad)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
-  int rc = ready_for_training(t);
+  int rc = check_raw_pending(t, c);
   if (rc) return rc;
+  if (d_grad && misaligned(d_grad)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
+  if ((rc = ready_for_training(t))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
-  TableCall call;  // runs beside a pb_tier_stage (see there): waits for none
-  if ((rc = call.begin(t, st, CALL_STEP, false))) return rc;
+  TableCall call;  // in the step chain only: runs beside the next forward and a pb_tier_stage (see there)
+  if ((rc = call.begin(t, st, CALL_STEP))) return rc;
   drop_raw_pending(c);  // enqueued below: the sweep of the next training call runs after these gradients
   GradsDev gr;
   std::memset(&gr, 0, sizeof(gr));
@@ -1660,18 +1680,14 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
     if (d_status) launch_slot_status(gr, 1, c->dev_tick, c->nan_tick, d_status, st);
     return PB_OK;
   }
-  const bool do_scale = std::fabs(scale - 1.0f) > 1.1920929e-07f;
-  const float inv = 1.0f / scale;
-  if (do_scale && !std::isfinite(inv)) return fail(PB_ERR_INVALID, "scale on gradient must be finite");
+  uint8_t do_scale;
+  float inv;
+  if ((rc = loss_scale(scale, do_scale, inv))) return rc;
   const float* pair = nullptr;
-  if (t->op.kind == PB_OPT_ADAM) {  // one power step per request and feature group (optim.rs:155-197)
+  if (t->op.kind == PB_OPT_ADAM) {  // one power step per request and feature group
     const int k = adam_index(t, c->slots.prefix[0]);
     if (k < 0) return fail(PB_ERR_CAPACITY, "more feature groups than Adam beta-power pairs");
-    AdamKeys keys{};
-    keys.idx[0] = (uint8_t)k;
-    keys.n = 1;
-    launch_adam_advance(t->adam_dev, keys, t->op.b1, t->op.b2, st);
-    pair = t->adam_dev + 2 * k;
+    pair = advance_adam_pair(t, k, st);
   }
   const uint32_t dim = t->d.dim;
   launch_raw_nan(d_grad, is_f16 != 0, c->raw.counts, dim, c->dev_tick, c->nan_tick, st);
@@ -1680,7 +1696,7 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
   // gradient into +0.  pb_update takes its gradients as given, like the PS (PS mod.rs:359-427), so the step does not.
   // The pending training forward allocated the buffer for this table's dim; only another table's larger dim allocates.
   if ((rc = ensure_raw_stage(c, dim, st))) return rc;
-  launch_raw_stage(d_grad, is_f16 != 0, c->raw.counts, dim, inv, do_scale, c->raw_stage, st);
+  launch_raw_stage(d_grad, is_f16 != 0, c->raw.counts, dim, inv, do_scale != 0, c->raw_stage, st);
   launch_update_direct(t->d, t->op, t->hy, c->raw.target, c->raw_stage, c->n_occ, pair, st, c->raw.counts,
                        c->dev_tick, c->nan_tick, true);
   if (t->inc.cells && c->n_occ) launch_inc_mark_raw(t->inc, c->raw, c->n_occ, c->dev_tick, c->nan_tick, st);
@@ -1694,20 +1710,14 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
                            uint32_t* d_counts, void* stream, int phases) {
   if (phases == 0) phases = PB_PHASE_ALL;
   const bool all = phases == PB_PHASE_ALL;
-  if (!t || !c || !x || !d_table_f16 || !d_index || !d_non_empty || !d_sample_id_num || !d_counts || (n_occ && !d_ids))
-    return fail(PB_ERR_INVALID, "null argument");
+  if (!x) return fail(PB_ERR_INVALID, "null argument");
+  int rc = check_raw_forward(t, c, d_ids, n_occ, d_row_off, batch, sample_fixed_size, d_table_f16, d_index, d_non_empty,
+                             d_sample_id_num, d_counts);
+  if (rc) return rc;
   if (t->tier) return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no sharded calls)");
-  if (misaligned(d_table_f16)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
-  if (!c->has_slots || c->slots.n_slots != 1) return fail(PB_ERR_STATE, "a raw context serves exactly one slot (pb_ctx_set_slots)");
-  if (t->device != c->device || t->device != x->device) return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
+  if (t->device != x->device) return fail(PB_ERR_INVALID, "table and exchange live on different devices");
   if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
   if (!x->d.row_f32) return fail(PB_ERR_INVALID, "raw slots need an exchange created with f32 rows (the requester rounds them)");
-  if (batch > 65535) return fail(PB_ERR_BATCH, "batch size cannot be larger than 65535");
-  if (sample_fixed_size == 0) return fail(PB_ERR_INVALID, "sample_fixed_size must be positive");
-  if (n_occ > c->max_occ || batch > c->max_out || (uint64_t)batch * sample_fixed_size > (1ull << 31))
-    return fail(PB_ERR_CAPACITY, "batch exceeds the context's capacity");
-  if (!d_row_off && n_occ != batch) return fail(PB_ERR_INVALID, "row offsets are required unless every sample has one id");
-  int rc;
   // every rank serves lookups whether or not its own batch trains: the shard must be usable (a collective call)
   if ((rc = ready_for_training(t))) return rc;
   DeviceGuard g(t->device);
@@ -1715,23 +1725,17 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
   if ((rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_raw(c))) return rc;
   if (phases & PB_PHASE_SEND) {
-    const uint32_t occ_off[2] = {0, n_occ};
     SlotsDev sl;
-    if ((rc = make_slots(c->slots, occ_off, sl))) return rc;
-    sl.uniform = 0;
+    if ((rc = raw_slots(c, n_occ, sl))) return rc;
     drop_raw_pending(c);  // the numbering below replaces the pending batch's
     if (training) {
       if ((rc = maybe_evict(t, st))) return rc;
       launch_begin_batch(t->d, c->dev_tick, nullptr, st);
     }
-    const uint32_t* occ_sample = nullptr;
-    if (d_row_off) {
-      PB_CUDA(cudaMemcpyAsync(c->row_off, d_row_off, 4 * ((size_t)batch + 1), cudaMemcpyDeviceToDevice, st));
-      launch_expand_rows(c->row_off, batch, c->occ_outrow, st);
-      occ_sample = c->occ_outrow;
-    }
-    launch_raw_number(sl, d_ids, n_occ, d_row_off ? c->row_off : nullptr, occ_sample, batch, sample_fixed_size, nullptr,
-                      c->raw, (long long*)d_index, (long long*)d_non_empty, d_sample_id_num, st);
+    if (d_row_off && (rc = copy_row_off(c, d_row_off, batch, st))) return rc;
+    launch_raw_number(sl, d_ids, n_occ, d_row_off ? c->row_off : nullptr, d_row_off ? c->occ_outrow : nullptr, batch,
+                      sample_fixed_size, nullptr, c->raw, (long long*)d_index, (long long*)d_non_empty, d_sample_id_num,
+                      st);
     PB_CUDA(cudaMemcpyAsync(d_counts, c->raw.counts, 8, cudaMemcpyDeviceToDevice, st));
     PB_CUDA(cudaMemsetAsync(c->raw.peer, 0, 4 * PB_MAX_RANKS, st));
     launch_raw_route(c->raw, n_occ, x->d, st);  // requester: distinct signs -> owners' areas
@@ -1752,13 +1756,7 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
   }
   if (!all) launch_wait(x->d, XC_FLAG_ROW, -1, st);
   launch_raw_fill(c->raw, n_occ, t->d.dim, x->d, d_table_f16, st);  // requester: rows in -> distinct-sign table
-  if (training) {
-    c->n_occ = n_occ;
-    c->batch = batch;
-    c->raw_pending = true;
-    c->raw_table = t;
-    t->pending_batches++;
-  }
+  if (training) hold_raw_batch(t, c, n_occ, batch);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -1770,13 +1768,13 @@ int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_gr
   if (!c->has_slots || c->slots.n_slots != 1) return fail(PB_ERR_STATE, "a raw context serves exactly one slot (pb_ctx_set_slots)");
   if (t->device != c->device || t->device != x->device) return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
   if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
-  if (!c->raw_pending) return fail(PB_ERR_STATE, "no raw forward batch is pending in this context (backward_ref_id not found)");
-  if (d_grad && misaligned(d_grad)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
-  int rc = ready_for_training(t);
+  int rc = check_raw_pending(t, c);
   if (rc) return rc;
-  const bool do_scale = std::fabs(scale - 1.0f) > 1.1920929e-07f;
-  const float inv = 1.0f / scale;
-  if (d_grad && do_scale && !std::isfinite(inv)) return fail(PB_ERR_INVALID, "scale on gradient must be finite");
+  if (d_grad && misaligned(d_grad)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
+  if ((rc = ready_for_training(t))) return rc;
+  uint8_t do_scale = 0;  // (add_skipped_gradient: the send reads no gradient, nor its scale)
+  float inv = 1.0f;
+  if (d_grad && (rc = loss_scale(scale, do_scale, inv))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   const uint32_t dim = t->d.dim;
@@ -1786,7 +1784,7 @@ int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_gr
     gr.ptr[0] = d_grad;
     if (d_grad) launch_raw_nan(d_grad, is_f16 != 0, c->raw.counts, dim, c->dev_tick, c->nan_tick, st);
     if (d_status) launch_slot_status(gr, 1, c->dev_tick, c->nan_tick, d_status, st);
-    launch_raw_send(d_grad, is_f16 != 0, c->raw, c->n_occ, dim, inv, do_scale, c->dev_tick, c->nan_tick, x->d, st);
+    launch_raw_send(d_grad, is_f16 != 0, c->raw, c->n_occ, dim, inv, do_scale != 0, c->dev_tick, c->nan_tick, x->d, st);
     if (phases == PB_PHASE_ALL && t->op.kind != PB_OPT_ADAGRAD_VW) launch_signal_wait(x->d, XC_FLAG_GRAD, nullptr, st);
     else launch_signal(x->d, XC_FLAG_GRAD, nullptr, st);
   }
@@ -1794,9 +1792,8 @@ int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_gr
     PB_CUDA(cudaGetLastError());
     return PB_OK;
   }
-  const uint32_t occ_off[2] = {0, c->n_occ};
   SlotsDev sl;
-  if ((rc = make_slots(c->slots, occ_off, sl))) return rc;
+  if ((rc = raw_slots(c, c->n_occ, sl))) return rc;
   if ((rc = owner_backward(t, x, c->slots.prefix, 1, sl.spacing, phases, st))) return rc;
   drop_raw_pending(c);
   PB_CUDA(cudaGetLastError());
