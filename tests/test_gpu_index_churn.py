@@ -15,6 +15,7 @@ is reset to init_row(sign) ++ initial state at that point.  Tables stay at capac
 import numpy as np
 import pytest
 
+from hash_set_keys import mix64
 from util import full_row_off, to_dev_i32, to_dev_ids
 
 pytestmark = pytest.mark.gpu
@@ -36,18 +37,6 @@ def torch_cuda():
 def n_cells(cap):
     want = max(1024, cap + cap // 2)
     return 1 << (want - 1).bit_length()
-
-
-def mix64(k):
-    """pb_common.cuh mix64, on uint64 numpy arrays (multiplication wraps)."""
-    k = np.asarray(k, np.uint64).copy()
-    with np.errstate(over="ignore"):
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xFF51AFD7ED558CCD)
-        k ^= k >> np.uint64(33)
-        k *= np.uint64(0xC4CEB9FE1A85EC53)
-        k ^= k >> np.uint64(33)
-    return k
 
 
 class IndexModel:
