@@ -856,15 +856,13 @@ def _exchange_cap(slot_ids, dev):
     import torch
     import torch.distributed as dist
 
+    from .worker import distinct_per_owner
+
     cap = int(os.environ.get("PERSIA_B200_XCHG_CAP", 0))
     if cap:
         return cap
-    R = dist.get_world_size()
-    counts = np.zeros(R, np.int64)
-    spacing = np.uint64((1 << (64 - _S.prefix_bit)) - 1)
-    for x, prefix in slot_ids:
-        u = np.unique(x % spacing + np.uint64(prefix) if prefix else x)
-        counts += np.bincount((farmhash64_np(u) % np.uint64(R)).astype(np.int64), minlength=R)
+    ids, prefixes = zip(*slot_ids)
+    counts = distinct_per_owner(ids, prefixes, dist.get_world_size(), _S.prefix_bit)
     t = torch.tensor([int(counts.max())], dtype=torch.int64, device=dev)
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
     return (int(int(t) * 1.5) + 1024 + 7) // 8 * 8

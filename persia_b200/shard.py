@@ -41,6 +41,87 @@ def _as_i64_bits(t):
     return t.contiguous()
 
 
+# Marshalling shared by the local wrappers here and the sharded ones (worker.py): tensors -> the C ABI's arguments.
+def _slot_offsets(slot_off, n_slots):
+    return (C.c_uint32 * (n_slots + 1))(*[int(x) for x in slot_off])
+
+
+def _prefixes(prefixes):
+    return (C.c_uint64 * len(prefixes))(*[int(p) for p in prefixes])
+
+
+def _grad_ptrs(ptrs, n_slots):
+    """Per-slot device pointers (None or 0 = skipped slot) as the backward's c_void_p[n_slots] array."""
+    return (C.c_void_p * n_slots)(*[(int(p) if p else None) for p in ptrs])
+
+
+def _slot_grads(grads, n_slots, stream=None):
+    """Per-slot gradients (device tensors [batch, dim], all f16 or all f32; None = skipped slot) -> (pointer array,
+    is_f16, the tensors to hold through the call).  A misaligned tensor is copied on `stream`, the stream the call runs
+    on (None: the current one; see aligned)."""
+    grads = [aligned(g, stream) for g in grads]
+    is_f16 = None
+    for g in grads:
+        if g is not None:
+            assert g.is_contiguous() and g.dtype in (torch.float16, torch.float32)
+            f16 = g.dtype == torch.float16
+            assert is_f16 is None or is_f16 == f16, "all slot gradients of one request share a dtype"
+            is_f16 = f16
+    return _grad_ptrs([g.data_ptr() if g is not None else None for g in grads], n_slots), bool(is_f16), grads
+
+
+def _scales(scales, n_slots):
+    """Per-slot loss scales as the backward's c_float[n_slots] array; None when none are given."""
+    return (C.c_float * n_slots)(*[float(s) for s in scales]) if scales is not None else None
+
+
+def _raw_grad(grad, is_f16, owner, stream=None):
+    """A raw backward's gradient (tensor, device pointer or None) -> (pointer, is_f16, the tensor to hold through the
+    call).  A misaligned tensor is copied on `stream` (see aligned).  An empty one (U = 0: nothing is read, but the
+    request is not a skipped one) points at `owner._dummy`, made on first use: one per wrapper object."""
+    if grad is None or isinstance(grad, int):
+        return grad, is_f16, None
+    grad = aligned(grad, stream)
+    assert grad.is_contiguous() and grad.dtype in (torch.float16, torch.float32)
+    is_f16 = grad.dtype == torch.float16
+    if not grad.numel():
+        if getattr(owner, "_dummy", None) is None:
+            owner._dummy = torch.zeros(4, dtype=torch.float32, device=owner.device)
+        grad = owner._dummy
+    return grad.data_ptr(), is_f16, grad
+
+
+def _raw_outputs(n, batch, fixed, dim, device):
+    """The five output buffers of a raw forward of n ids (see BatchContext.forward_raw)."""
+    return (torch.empty((n + 1, dim), dtype=torch.float16, device=device),
+            torch.empty(batch * fixed, dtype=torch.int64, device=device),
+            torch.empty(max(batch * fixed, 1), dtype=torch.int64, device=device),
+            torch.empty(max(batch, 1), dtype=torch.int32, device=device),
+            torch.empty(2, dtype=torch.int32, device=device))
+
+
+def _raw_row_off(row_off, batch):
+    """A raw forward's CSR offsets (device int32 [batch + 1]; None: one id per sample), checked, as a pointer."""
+    if row_off is not None:
+        assert row_off.dtype == torch.int32 and row_off.is_contiguous() and row_off.numel() == batch + 1
+    return _ptr(row_off)
+
+
+def _read_block(fields, call, ctype=C.c_uint64):
+    """`call(pointer)` fills len(fields) counters of `ctype` and returns a pb status; the counters keyed by `fields`."""
+    out = (ctype * len(fields))()
+    N.check(call(C.byref(out)))
+    return dict(zip(fields, out))
+
+
+COUNTER_FIELDS = ("admitted", "lookup_miss", "gradient_id_miss", "capacity_refused", "wait_errors")
+INDEX_STATS_FIELDS = ("live", "tomb", "empty")
+TIER_STATS_FIELDS = ("host_rows", "moved_out", "restored", "dropped", "refused")
+STAGE_STATS_FIELDS = ("staged", "skipped")
+INCREMENTAL_STATS_FIELDS = ("held", "inserted", "dropped", "taken")
+BATCH_STATS_FIELDS = ("items", "cold", "warm", "hot", "repeated_occurrences", "occurrences")
+
+
 class EmbeddingShard:
     def __init__(self, dim, capacity, device=0, tier_rows=0, host=False):
         """capacity: rows in HBM.  tier_rows > 0: a host-memory tier of that many rows behind them (include/persia_b200.h,
@@ -91,22 +172,15 @@ class EmbeddingShard:
         return self._entry_len
 
     def counters(self):
-        out = (C.c_uint64 * 5)()
-        N.check(self.lib.pb_table_counters(self.h, C.byref(out), _stream(self.device)))
-        return {"admitted": out[0], "lookup_miss": out[1], "gradient_id_miss": out[2], "capacity_refused": out[3],
-                "wait_errors": out[4]}
+        return _read_block(COUNTER_FIELDS, lambda out: self.lib.pb_table_counters(self.h, out, _stream(self.device)))
 
     def index_stats(self):
         """Cells of the hash index (host sync): live signs, tombstones of evicted signs, and EMPTY cells."""
-        out = (C.c_uint64 * 3)()
-        N.check(self.lib.pb_table_index_stats(self.h, C.byref(out), _stream(self.device)))
-        return {"live": out[0], "tomb": out[1], "empty": out[2]}
+        return _read_block(INDEX_STATS_FIELDS, lambda out: self.lib.pb_table_index_stats(self.h, out, _stream(self.device)))
 
     def tier_stats(self):
         """The host tier's counters (host sync); all zero without a tier."""
-        out = (C.c_uint64 * 5)()
-        N.check(self.lib.pb_tier_stats(self.h, C.byref(out), _stream(self.device)))
-        return {"host_rows": out[0], "moved_out": out[1], "restored": out[2], "dropped": out[3], "refused": out[4]}
+        return _read_block(TIER_STATS_FIELDS, lambda out: self.lib.pb_tier_stats(self.h, out, _stream(self.device)))
 
     def stage(self, ids, slot_off, prefixes, prefix_bit=8):
         """pb_tier_stage on the current stream: the eviction check and the tier restores of an upcoming training request,
@@ -115,17 +189,13 @@ class EmbeddingShard:
         change, only where entries live; without a tier nothing runs."""
         ids = _as_i64_bits(ids)
         S = len(prefixes)
-        off = (C.c_uint32 * (S + 1))(*[int(x) for x in slot_off])
-        pf = (C.c_uint64 * S)(*[int(p) for p in prefixes])
-        N.check(self.lib.pb_tier_stage(self.h, _ptr(ids), ids.numel(), off, pf, S, int(prefix_bit),
-                                       _stream(self.device)))
+        N.check(self.lib.pb_tier_stage(self.h, _ptr(ids), ids.numel(), _slot_offsets(slot_off, S), _prefixes(prefixes), S,
+                                       int(prefix_bit), _stream(self.device)))
 
     def stage_stats(self):
         """Stage counters (host sync): signs moved into HBM by stages (also counted in tier_stats()["restored"]), and
         stage restores skipped for want of a free HBM row (left to the request's own restore)."""
-        out = (C.c_uint64 * 2)()
-        N.check(self.lib.pb_tier_stage_stats(self.h, C.byref(out), _stream(self.device)))
-        return {"staged": out[0], "skipped": out[1]}
+        return _read_block(STAGE_STATS_FIELDS, lambda out: self.lib.pb_tier_stage_stats(self.h, out, _stream(self.device)))
 
     # incremental updates (PerisaIncrementalUpdateManager, persia-incremental-update-manager/src/lib.rs:251-312)
     def enable_incremental(self, capacity):
@@ -135,9 +205,7 @@ class EmbeddingShard:
 
     def incremental_stats(self):
         """The set's counters (host sync): signs held now, inserted, dropped because the set was full, and taken."""
-        out = (C.c_uint64 * 4)()
-        N.check(self.lib.pb_inc_stats(self.h, C.byref(out), _stream(self.device)))
-        return {"held": out[0], "inserted": out[1], "dropped": out[2], "taken": out[3]}
+        return _read_block(INCREMENTAL_STATS_FIELDS, lambda out: self.lib.pb_inc_stats(self.h, out, _stream(self.device)))
 
     def incremental_held(self):
         """Signs held, read without a sync: may lag the work still in flight on the stream."""
@@ -278,10 +346,8 @@ class BatchContext:
 
     def batch_stats(self):
         """Dedup statistics of the last training batch (host sync): distinct items and their multiplicity classes."""
-        out = (C.c_uint32 * 6)()
-        N.check(self.lib.pb_ctx_batch_stats(self.h, C.byref(out), _stream(self.device)))
-        return {"items": out[0], "cold": out[1], "warm": out[2], "hot": out[3], "repeated_occurrences": out[4],
-                "occurrences": out[5]}
+        return _read_block(BATCH_STATS_FIELDS, lambda out: self.lib.pb_ctx_batch_stats(self.h, out, _stream(self.device)),
+                           C.c_uint32)
 
     def forward(self, shard, ids, slot_occ_off, batch, row_off=None, training=True, out=None):
         """ids: flat device int64-bit ids (slot-major); slot_occ_off: host list, n_slots+1;
@@ -290,42 +356,27 @@ class BatchContext:
         ids = _as_i64_bits(ids)
         if out is None:
             out = torch.empty((self.n_slots, batch, shard.dim), dtype=torch.float16, device=self.device)
-        off = (C.c_uint32 * (self.n_slots + 1))(*[int(x) for x in slot_occ_off])
         if row_off is not None:
             assert row_off.dtype == torch.int32 and row_off.is_contiguous()
-        N.check(self.lib.pb_forward(shard.h, self.h, _ptr(ids), ids.numel(), _ptr(row_off), off, int(batch),
-                                    int(training), _ptr(out), _stream(self.device)))
+        N.check(self.lib.pb_forward(shard.h, self.h, _ptr(ids), ids.numel(), _ptr(row_off),
+                                    _slot_offsets(slot_occ_off, self.n_slots), int(batch), int(training), _ptr(out),
+                                    _stream(self.device)))
         return out
 
     def backward(self, shard, grads, scales=None, want_status=False):
-        """grads: list (per slot) of device tensors [batch, dim] (all f16 or all f32) or None (skipped).  A tensor that
-        is not 16-byte aligned is copied first."""
-        ptrs = (C.c_void_p * self.n_slots)()
-        is_f16 = None
-        grads = [aligned(g) for g in grads]  # (kept alive until the call has enqueued its reads)
-        for i, g in enumerate(grads):
-            if g is None:
-                ptrs[i] = None
-                continue
-            assert g.is_contiguous()
-            f16 = g.dtype == torch.float16
-            assert f16 or g.dtype == torch.float32
-            assert is_f16 is None or is_f16 == f16, "all slot gradients of one request share a dtype"
-            is_f16 = f16
-            ptrs[i] = g.data_ptr()
-        sc = None
-        if scales is not None:
-            sc = (C.c_float * self.n_slots)(*[float(s) for s in scales])
+        """grads: list (per slot) of device tensors [batch, dim] (all f16 or all f32) or None (skipped), or an
+        [n_slots, batch, dim] tensor.  A tensor that is not 16-byte aligned is copied first."""
+        ptrs, is_f16, held = _slot_grads(grads, self.n_slots)  # (held through the call)
         status = torch.empty(self.n_slots, dtype=torch.int32, device=self.device) if want_status else None
-        N.check(self.lib.pb_backward(shard.h, self.h, ptrs, int(bool(is_f16)), sc, _ptr(status), _stream(self.device)))
+        N.check(self.lib.pb_backward(shard.h, self.h, ptrs, int(is_f16), _scales(scales, self.n_slots), _ptr(status),
+                                     _stream(self.device)))
         return status
 
     def backward_ptrs(self, shard, ptrs, is_f16, scales=None):
         """GradientBatch form (persia-core/src/backward.rs:86-105): raw device pointers, None = skipped slot.  A pointer
         that is not 16-byte aligned is refused (PersiaB200Error)."""
-        arr = (C.c_void_p * self.n_slots)(*[(int(p) if p else None) for p in ptrs])
-        sc = (C.c_float * self.n_slots)(*[float(x) for x in scales]) if scales is not None else None
-        N.check(self.lib.pb_backward(shard.h, self.h, arr, int(bool(is_f16)), sc, None, _stream(self.device)))
+        N.check(self.lib.pb_backward(shard.h, self.h, _grad_ptrs(ptrs, self.n_slots), int(bool(is_f16)),
+                                     _scales(scales, self.n_slots), None, _stream(self.device)))
 
     def forward_raw(self, shard, ids, batch, sample_fixed_size, row_off=None, training=True):
         """Raw (embedding_summation: false) slot; the context must have been built with ONE prefix.
@@ -335,38 +386,20 @@ class BatchContext:
         assert self.n_slots == 1, "a raw context serves one slot"
         ids = _as_i64_bits(ids)
         n, fixed = ids.numel(), int(sample_fixed_size)
-        table = torch.empty((n + 1, shard.dim), dtype=torch.float16, device=self.device)
-        index = torch.empty(batch * fixed, dtype=torch.int64, device=self.device)
-        non_empty = torch.empty(max(batch * fixed, 1), dtype=torch.int64, device=self.device)
-        sample_id_num = torch.empty(max(batch, 1), dtype=torch.int32, device=self.device)
-        counts = torch.empty(2, dtype=torch.int32, device=self.device)
-        if row_off is not None:
-            assert row_off.dtype == torch.int32 and row_off.is_contiguous() and row_off.numel() == batch + 1
-        N.check(self.lib.pb_forward_raw(shard.h, self.h, _ptr(ids), n, _ptr(row_off), int(batch), fixed, int(training),
-                                        _ptr(table), _ptr(index), _ptr(non_empty), _ptr(sample_id_num), _ptr(counts),
-                                        _stream(self.device)))
+        out = _raw_outputs(n, batch, fixed, shard.dim, self.device)
+        N.check(self.lib.pb_forward_raw(shard.h, self.h, _ptr(ids), n, _raw_row_off(row_off, batch), int(batch), fixed,
+                                        int(training), *map(_ptr, out), _stream(self.device)))
+        table, index, non_empty, sample_id_num, counts = out
         return table, index, non_empty, sample_id_num[:batch], counts
 
     def backward_raw(self, shard, grad, scale=1.0, want_status=False, is_f16=None):
         """grad: device tensor [U, dim] (f32 as persia/ctx.py:970-980 builds it, or f16), a raw device pointer
         (then pass is_f16), or None (add_skipped_gradient)."""
-        ptr = None
-        if grad is not None and not isinstance(grad, int):
-            grad = aligned(grad)
-            assert grad.is_contiguous() and grad.dtype in (torch.float16, torch.float32)
-            is_f16 = grad.dtype == torch.float16
-            ptr = grad.data_ptr() if grad.numel() else self._raw_dummy().data_ptr()
-        elif grad is not None:
-            ptr = grad
+        ptr, is_f16, held = _raw_grad(grad, is_f16, self)  # (held through the call)
         status = torch.empty(1, dtype=torch.int32, device=self.device) if want_status else None
         N.check(self.lib.pb_backward_raw(shard.h, self.h, ptr, int(bool(is_f16)), float(scale), _ptr(status),
                                          _stream(self.device)))
         return status
-
-    def _raw_dummy(self):
-        if not hasattr(self, "_dummy"):
-            self._dummy = torch.zeros(4, dtype=torch.float32, device=self.device)
-        return self._dummy
 
     def close(self):
         if getattr(self, "h", None):
@@ -397,9 +430,8 @@ def add_prefix(ids, slot_occ_off, prefixes, prefix_bit=8):
     ids = _as_i64_bits(ids)
     out = torch.empty_like(ids)
     S = len(prefixes)
-    off = (C.c_uint32 * (S + 1))(*[int(x) for x in slot_occ_off])
-    pf = (C.c_uint64 * S)(*[int(p) for p in prefixes])
-    N.check(lib.pb_add_prefix(_ptr(ids), ids.numel(), off, pf, S, prefix_bit, _ptr(out), _stream(ids.device)))
+    N.check(lib.pb_add_prefix(_ptr(ids), ids.numel(), _slot_offsets(slot_occ_off, S), _prefixes(prefixes), S, prefix_bit,
+                              _ptr(out), _stream(ids.device)))
     return out
 
 
@@ -435,9 +467,8 @@ HOT_GEOMETRY_FIELDS = ("EPL", "CH", "PW", "vec", "vshift", "lean", "R1", "R", "S
 def hot_geometry(dim, f16, ragged=False):
     """The geometry the backward gives its reduce of hot signs (include/persia_b200.h, pb_hot_geometry) as a dict keyed
     by HOT_GEOMETRY_FIELDS.  Host-only."""
-    out = (C.c_uint32 * 12)()
-    N.check(N.load().pb_hot_geometry(int(dim), int(bool(f16)), int(bool(ragged)), C.byref(out)))
-    return dict(zip(HOT_GEOMETRY_FIELDS, out))
+    return _read_block(HOT_GEOMETRY_FIELDS,
+                       lambda out: N.load().pb_hot_geometry(int(dim), int(bool(f16)), int(bool(ragged)), out), C.c_uint32)
 
 
 def partition_by_shard(signs, R):

@@ -29,20 +29,27 @@ from . import native as N
 from . import shard as SH
 
 
-def distinct_per_owner(ids, batch, prefixes, R, prefix_bit=8):
+def distinct_per_owner(slot_ids, prefixes, R, prefix_bit=8):
     """Host-side (numpy) count of the distinct signs one batch requests of every owner: what `cap` must cover.
-    ids: uint64 [n_slots * batch] slot-major.  Mirrors indices_add_prefix + FeatureBatch::new + sign_to_shard_modulo."""
+    slot_ids: each slot's uint64 ids (any lengths).  Mirrors indices_add_prefix + FeatureBatch::new + sign_to_shard_modulo."""
     from .persia_core import farmhash64_np
 
-    S = len(prefixes)
-    ids = np.ascontiguousarray(ids, dtype=np.uint64).reshape(S, batch)
     spacing = np.uint64((1 << (64 - prefix_bit)) - 1)
     counts = np.zeros(R, np.int64)
-    for s in range(S):
-        signs = ids[s] % spacing + np.uint64(prefixes[s]) if prefixes[s] else ids[s]
-        u = np.unique(signs)
+    for x, prefix in zip(slot_ids, prefixes):
+        x = np.asarray(x, dtype=np.uint64)
+        u = np.unique(x % spacing + np.uint64(prefix) if prefix else x)
         counts += np.bincount((farmhash64_np(u) % np.uint64(R)).astype(np.int64), minlength=R)
     return counts
+
+
+XCHG_STATUS_FIELDS = ("overflowed", "wait_gave_up")
+
+
+def _by_phase(workers, *phases):
+    """(rank, worker, phase) in the order one host thread drives the virtual ranks of one GPU: every phase is enqueued
+    for all ranks before the next."""
+    return ((r, w, ph) for ph in phases for r, w in enumerate(workers))
 
 
 class ShardedEmbeddingWorker:
@@ -123,7 +130,8 @@ class ShardedEmbeddingWorker:
         re-runs it on a worker built with a larger cap."""
         worst = 0
         for ids in id_batches:
-            worst = max(worst, int(distinct_per_owner(ids, batch, prefixes, world).max()))
+            slot_ids = np.ascontiguousarray(ids, dtype=np.uint64).reshape(len(prefixes), batch)
+            worst = max(worst, int(distinct_per_owner(slot_ids, prefixes, world).max()))
         if group is not None or (torch.distributed.is_available() and torch.distributed.is_initialized()):
             import torch.distributed as dist
 
@@ -136,9 +144,7 @@ class ShardedEmbeddingWorker:
 
     # ---- incremental updates: the owner table's set of stepped signs (EmbeddingShard.enable_incremental) ---------------
     def _on_stream(self, fn, *args):
-        if self.stream is None:
-            return fn(*args)
-        with torch.cuda.stream(self.stream):
+        with torch.cuda.stream(self._torch_stream()):
             return fn(*args)
 
     def enable_incremental(self, capacity):
@@ -154,9 +160,12 @@ class ShardedEmbeddingWorker:
         return self._on_stream(self.shard.take_incremental)
 
     # ---- forward_batched_direct / update_gradient_batched ------------------------------------------------------------
+    def _torch_stream(self):
+        """The stream this worker's calls run on: its own, else the current one."""
+        return self.stream if self.stream is not None else torch.cuda.current_stream(self.device)
+
     def _st(self):
-        s = self.stream if self.stream is not None else torch.cuda.current_stream(self.device)
-        return C.c_void_p(s.cuda_stream)
+        return C.c_void_p(self._torch_stream().cuda_stream)
 
     def forward(self, ids, batch, training=True, row_off=None, slot_occ_off=None, out=None, phases=0):
         """ids: device int64-bit ids, slot-major; one id per sample per slot unless row_off (device int32 CSR offsets,
@@ -167,9 +176,9 @@ class ShardedEmbeddingWorker:
             slot_occ_off = [s * batch for s in range(self.S + 1)]
         if out is None:
             out = torch.empty((self.S, batch, self.dim), dtype=torch.float16, device=self.device)
-        off = (C.c_uint32 * (self.S + 1))(*[int(v) for v in slot_occ_off])
-        N.check(self.lib.pb_forward_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), ids.numel(), SH._ptr(row_off), off,
-                                            int(batch), int(training), SH._ptr(out), self._st(), int(phases)))
+        N.check(self.lib.pb_forward_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), ids.numel(), SH._ptr(row_off),
+                                            SH._slot_offsets(slot_occ_off, self.S), int(batch), int(training),
+                                            SH._ptr(out), self._st(), int(phases)))
         return out
 
     def backward(self, grads, scales=None, want_status=False, phases=0, status=None):
@@ -178,58 +187,39 @@ class ShardedEmbeddingWorker:
         16) is copied first, on the worker's stream."""
         if torch.is_tensor(grads):
             grads = [grads[i] for i in range(self.S)]
-        st = self.stream if self.stream is not None else torch.cuda.current_stream(self.device)
-        grads = [SH.aligned(g, st) for g in grads]  # (kept alive until the call has enqueued its reads)
-        ptrs = (C.c_void_p * self.S)()
-        is_f16 = None
-        for i, g in enumerate(grads):
-            if g is None:
-                ptrs[i] = None
-                continue
-            assert g.is_contiguous() and g.dtype in (torch.float16, torch.float32)
-            f16 = g.dtype == torch.float16
-            assert is_f16 is None or is_f16 == f16, "all slot gradients of one request share a dtype"
-            is_f16 = f16
-            ptrs[i] = g.data_ptr()
-        sc = (C.c_float * self.S)(*[float(v) for v in scales]) if scales is not None else None
+        ptrs, is_f16, held = SH._slot_grads(grads, self.S, self._torch_stream())  # (held through the call)
         if status is None and want_status:
             status = torch.empty(self.S, dtype=torch.int32, device=self.device)
-        N.check(self.lib.pb_backward_sharded(self.shard.h, self.ctx.h, self.h, ptrs, int(bool(is_f16)), sc, SH._ptr(status),
-                                             self._st(), int(phases)))
+        N.check(self.lib.pb_backward_sharded(self.shard.h, self.ctx.h, self.h, ptrs, int(is_f16), SH._scales(scales, self.S),
+                                             SH._ptr(status), self._st(), int(phases)))
         return status
 
     def backward_ptrs(self, ptrs, is_f16, scales=None):
         """GradientBatch form (persia-core/src/backward.rs:86-105): raw device pointers, None = skipped slot.  A pointer
         that is not 16-byte aligned is refused (PersiaB200Error)."""
-        arr = (C.c_void_p * self.S)(*[(int(p) if p else None) for p in ptrs])
-        sc = (C.c_float * self.S)(*[float(v) for v in scales]) if scales is not None else None
-        N.check(self.lib.pb_backward_sharded(self.shard.h, self.ctx.h, self.h, arr, int(bool(is_f16)), sc, None, self._st(), 0))
+        N.check(self.lib.pb_backward_sharded(self.shard.h, self.ctx.h, self.h, SH._grad_ptrs(ptrs, self.S),
+                                             int(bool(is_f16)), SH._scales(scales, self.S), None, self._st(), 0))
 
     @staticmethod
     def group_forward(workers, ids, batch, training=True, row_offs=None, slot_occ_offs=None, outs=None):
         """Virtual ranks of one GPU, driven by one host thread: every phase is enqueued for all ranks before the next."""
-        R = len(workers)
-        outs = outs if outs is not None else [None] * R
-        for ph in (N.PHASE_SEND, N.PHASE_SERVE, N.PHASE_FINISH):
-            for r, w in enumerate(workers):
-                outs[r] = w.forward(ids[r], batch, training, row_offs[r] if row_offs else None,
-                                    slot_occ_offs[r] if slot_occ_offs else None, outs[r], phases=ph)
+        outs = outs if outs is not None else [None] * len(workers)
+        for r, w, ph in _by_phase(workers, N.PHASE_SEND, N.PHASE_SERVE, N.PHASE_FINISH):
+            outs[r] = w.forward(ids[r], batch, training, row_offs[r] if row_offs else None,
+                                slot_occ_offs[r] if slot_occ_offs else None, outs[r], phases=ph)
         return outs
 
     @staticmethod
     def group_backward(workers, grads, scales=None, want_status=False):
-        R = len(workers)
         sts = [torch.empty(w.S, dtype=torch.int32, device=w.device) if want_status else None for w in workers]
-        for ph in (N.PHASE_SEND, N.PHASE_SERVE):
-            for r, w in enumerate(workers):
-                w.backward(grads[r], scales, want_status, phases=ph, status=sts[r])
+        for r, w, ph in _by_phase(workers, N.PHASE_SEND, N.PHASE_SERVE):
+            w.backward(grads[r], scales, want_status, phases=ph, status=sts[r])
         return sts
 
     def status(self):
         """(overflowed, wait_gave_up) — host sync."""
-        out = (C.c_uint32 * 2)()
-        N.check(self.lib.pb_xchg_status(self.h, C.byref(out), self._st()))
-        return bool(out[0]), bool(out[1])
+        out = SH._read_block(XCHG_STATUS_FIELDS, lambda out: self.lib.pb_xchg_status(self.h, out, self._st()), C.c_uint32)
+        return bool(out["overflowed"]), bool(out["wait_gave_up"])
 
     def close(self):
         if getattr(self, "h", None):
@@ -258,7 +248,6 @@ class ShardedRawWorker(ShardedEmbeddingWorker):
         kw["rows_f32"] = True
         kw.pop("sqrt_scaling", None)  # (a raw slot's sqrt_scaling only matters with hash-stack, which it cannot have)
         super().__init__(1, dim, prefixes, capacity, device, rank, world, cap, area, peer_bases, optimizer, **kw)
-        self._dummy = None
 
     @staticmethod
     def area_bytes(world, cap, dim, rows_f32=True):
@@ -272,37 +261,17 @@ class ShardedRawWorker(ShardedEmbeddingWorker):
         ids = SH._as_i64_bits(ids)
         n, fixed = ids.numel(), int(sample_fixed_size)
         if out is None:
-            out = (torch.empty((n + 1, self.dim), dtype=torch.float16, device=self.device),
-                   torch.empty(batch * fixed, dtype=torch.int64, device=self.device),
-                   torch.empty(max(batch * fixed, 1), dtype=torch.int64, device=self.device),
-                   torch.empty(max(batch, 1), dtype=torch.int32, device=self.device),
-                   torch.empty(2, dtype=torch.int32, device=self.device))
+            out = SH._raw_outputs(n, batch, fixed, self.dim, self.device)
         table, index, non_empty, num, counts = out
-        if row_off is not None:
-            assert row_off.dtype == torch.int32 and row_off.is_contiguous() and row_off.numel() == batch + 1
-        N.check(self.lib.pb_forward_raw_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), n, SH._ptr(row_off),
-                                                int(batch), fixed, int(training), SH._ptr(table), SH._ptr(index),
-                                                SH._ptr(non_empty), SH._ptr(num), SH._ptr(counts), self._st(),
-                                                int(phases)))
+        N.check(self.lib.pb_forward_raw_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), n,
+                                                SH._raw_row_off(row_off, batch), int(batch), fixed, int(training),
+                                                *map(SH._ptr, out), self._st(), int(phases)))
         return table, index, non_empty, num[:batch], counts
 
     def backward_raw(self, grad, scale=1.0, want_status=False, is_f16=None, phases=0, status=None):
         """grad: device tensor [U, dim] (f32 as persia/ctx.py:970-980 builds it, or f16), a raw device pointer (then
         pass is_f16), or None (add_skipped_gradient).  A tensor that is not 16-byte aligned is copied first."""
-        ptr = None
-        if grad is not None and not isinstance(grad, int):
-            st = self.stream if self.stream is not None else torch.cuda.current_stream(self.device)
-            grad = SH.aligned(grad, st)
-            assert grad.is_contiguous() and grad.dtype in (torch.float16, torch.float32)
-            is_f16 = grad.dtype == torch.float16
-            if grad.numel():
-                ptr = grad.data_ptr()
-            else:  # U = 0: nothing is read, but the request is not a skipped one
-                if self._dummy is None:
-                    self._dummy = torch.zeros(4, dtype=torch.float32, device=self.device)
-                ptr = self._dummy.data_ptr()
-        elif grad is not None:
-            ptr = grad
+        ptr, is_f16, held = SH._raw_grad(grad, is_f16, self, self._torch_stream())  # (held through the call)
         if status is None and want_status:
             status = torch.empty(1, dtype=torch.int32, device=self.device)
         N.check(self.lib.pb_backward_raw_sharded(self.shard.h, self.ctx.h, self.h, ptr, int(bool(is_f16)), float(scale),
@@ -313,19 +282,16 @@ class ShardedRawWorker(ShardedEmbeddingWorker):
     def group_forward_raw(workers, ids, batch, sample_fixed_size, training=True, row_offs=None, outs=None):
         """Virtual ranks of one GPU, driven by one host thread: every phase is enqueued for all ranks before the next.
         Returns one forward_raw result per rank."""
-        R = len(workers)
-        outs = list(outs) if outs is not None else [None] * R
-        for ph in (N.PHASE_SEND, N.PHASE_SERVE, N.PHASE_FINISH):
-            for r, w in enumerate(workers):
-                outs[r] = w.forward_raw(ids[r], batch, sample_fixed_size, row_offs[r] if row_offs else None, training,
-                                        out=outs[r], phases=ph)
+        outs = list(outs) if outs is not None else [None] * len(workers)
+        for r, w, ph in _by_phase(workers, N.PHASE_SEND, N.PHASE_SERVE, N.PHASE_FINISH):
+            outs[r] = w.forward_raw(ids[r], batch, sample_fixed_size, row_offs[r] if row_offs else None, training,
+                                    out=outs[r], phases=ph)
         return outs
 
     @staticmethod
     def group_backward_raw(workers, grads, scales=None, want_status=False):
         """grads: per rank a [U_r, dim] tensor or None (add_skipped_gradient); scales: per rank (default 1)."""
         sts = [torch.empty(1, dtype=torch.int32, device=w.device) if want_status else None for w in workers]
-        for ph in (N.PHASE_SEND, N.PHASE_SERVE):
-            for r, w in enumerate(workers):
-                w.backward_raw(grads[r], scales[r] if scales is not None else 1.0, phases=ph, status=sts[r])
+        for r, w, ph in _by_phase(workers, N.PHASE_SEND, N.PHASE_SERVE):
+            w.backward_raw(grads[r], scales[r] if scales is not None else 1.0, phases=ph, status=sts[r])
         return sts

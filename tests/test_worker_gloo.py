@@ -48,7 +48,7 @@ def _run(rank, port, q, R):
         pf = [oracle.index_prefix(i) for i in range(S)]
         mine = [ids[rank] for ids, _ in _batches(R)]
         cap = ShardedEmbeddingWorker.calibrate_cap(mine, B, pf, R, margin=1.0, extra=0)  # collective MAX over the ranks
-        worst = max(int(distinct_per_owner(ids[r], B, pf, R).max()) for ids, _ in _batches(R) for r in range(R))
+        worst = max(int(distinct_per_owner(ids[r].reshape(S, B), pf, R).max()) for ids, _ in _batches(R) for r in range(R))
         assert cap == (worst + 7) // 8 * 8 and cap < S * B
         m = ExchangeModel(oracle, pf, DIM, oracle.Optim(oracle.SGD, lr=0.1, wd=0.0), rank, R, cap)
         outs, sts = [], []
@@ -64,7 +64,7 @@ def _run(rank, port, q, R):
         dist.destroy_process_group()
 
 
-@pytest.mark.parametrize("R", [2, 3])
+@pytest.mark.parametrize("R", [2, 3, 4, 5])
 def test_sharded_protocol_equals_oracle_requests_in_rank_order(R):
     import oracle
 
@@ -103,6 +103,75 @@ def test_sharded_protocol_equals_oracle_requests_in_rank_order(R):
             assert ref is not None and e.tobytes() == ref.tobytes()
             n += 1
     assert n > 100
+
+
+def _exchange_cap_counts(slot_ids, R, prefix_bit):
+    """The per-owner count persia_core._exchange_cap made inline before it called distinct_per_owner."""
+    from persia_b200.persia_core import farmhash64_np
+
+    counts = np.zeros(R, np.int64)
+    spacing = np.uint64((1 << (64 - prefix_bit)) - 1)
+    for x, prefix in slot_ids:
+        u = np.unique(x % spacing + np.uint64(prefix) if prefix else x)
+        counts += np.bincount((farmhash64_np(u) % np.uint64(R)).astype(np.int64), minlength=R)
+    return counts
+
+
+@pytest.mark.parametrize("prefix_bit", [8, 12])
+@pytest.mark.parametrize("R", [1, 2, 3, 8])
+def test_distinct_per_owner_ragged_slots(oracle, R, prefix_bit):
+    """Ragged slots with repeats, an empty one, and slots with and without an index prefix (two share one): per owner,
+    the distinct signs of each slot, summed over the slots."""
+    from persia_b200.worker import distinct_per_owner
+
+    rng = np.random.default_rng(1000 * R + prefix_bit)
+    sizes, cards = [300, 0, 1, 257, 64, 500], [50, 10, 3, 1 << 40, 2**64 - 1, 200]
+    slot_ids = [rng.integers(0, c, size=n, dtype=np.uint64) for n, c in zip(sizes, cards)]
+    slot_ids[4][:3] = [2**64 - 1, 0, 2**64 - 1]  # ids the prefix wraps and leaves
+    pf = [oracle.index_prefix(0, prefix_bit), 0, oracle.index_prefix(1, prefix_bit), 0, oracle.index_prefix(0, prefix_bit),
+          oracle.index_prefix(2, prefix_bit)]
+    got = distinct_per_owner(slot_ids, pf, R, prefix_bit)
+    want = np.zeros(R, np.int64)
+    for x, p in zip(slot_ids, pf):
+        for owner in oracle.shard_of(np.unique(oracle.add_prefix(x, prefix_bit, p)), R):
+            want[owner] += 1
+    assert got.tolist() == want.tolist() and want.sum() > 500
+    assert got.tolist() == _exchange_cap_counts(list(zip(slot_ids, pf)), R, prefix_bit).tolist()
+
+
+def _ragged_slots(rank):
+    rng = np.random.default_rng(5 + rank)
+    return [rng.integers(0, c, size=n, dtype=np.uint64) for n, c in zip([300 * (rank + 1), 0, 40], [2**64 - 1, 9, 25])]
+
+
+def _run_exchange_cap(rank, port, q, R, pf, prefix_bit):
+    from persia_b200 import persia_core as pc
+
+    dist.init_process_group("gloo", init_method=f"tcp://127.0.0.1:{port}", rank=rank, world_size=R)
+    try:
+        pc._S.prefix_bit = prefix_bit
+        q.put((rank, pc._exchange_cap(list(zip(_ragged_slots(rank), pf)), "cpu")))
+    finally:
+        dist.destroy_process_group()
+
+
+def test_exchange_cap_counts_ragged_slots_at_the_prefix_width(oracle):
+    """persia_core's exchange cap: the most distinct signs one rank's first batch asks of one owner, over the ranks, at
+    the configured prefix width, with its own margin."""
+    R, prefix_bit = 2, 12
+    pf = [oracle.index_prefix(0, prefix_bit), 0, oracle.index_prefix(3, prefix_bit)]
+    port = _free_port()
+    ctx = mp.get_context("spawn")
+    q = ctx.Queue()
+    procs = [ctx.Process(target=_run_exchange_cap, args=(r, port, q, R, pf, prefix_bit)) for r in range(R)]
+    for p in procs:
+        p.start()
+    caps = [q.get(timeout=180)[1] for _ in range(R)]
+    for p in procs:
+        p.join(timeout=60)
+        assert p.exitcode == 0
+    worst = max(int(_exchange_cap_counts(list(zip(_ragged_slots(r), pf)), R, prefix_bit).max()) for r in range(R))
+    assert caps == [(int(worst * 1.5) + 1024 + 7) // 8 * 8] * R
 
 
 def test_exchange_area_geometry():
