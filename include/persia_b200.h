@@ -27,7 +27,8 @@
  *   A backward is in the step chain only, so it runs beside the next batch's forward: a forward may read rows a backward
  *   on another stream is stepping (the staleness embedding_staleness allows).  An eviction check also waits for every
  *   step issued before it, so it never releases a row whose gradients are still to be applied.  pb_set_rows,
- *   pb_get_rows, pb_table_export_signs, pb_table_clear, the statistics calls and pb_inc_take are in both chains.
+ *   pb_get_rows, pb_table_export_signs, pb_table_clear, the statistics calls, pb_inc_take, pb_table_dump_part and
+ *   pb_dump_nodes are in both chains.
  *   pb_tier_stage waits for both chains and is in the index chain only.
  * Waiting costs a stream-wait on an event per call; a wait on work already complete costs nothing on the device.
  * Calls on one table must still be issued from one host thread at a time (the persia_core groups hold a lock), and a
@@ -232,6 +233,42 @@ int pb_get_rows(pb_table* t, const uint64_t* d_signs, uint32_t n, float* d_entri
  * Entries are then read with pb_get_rows and restored with pb_set_rows. */
 int pb_table_export_signs(pb_table* t, uint64_t* d_signs, uint32_t* d_recency, uint32_t max_n, uint32_t* d_count,
                           void* stream);
+
+/* ---- checkpoint images on the device ---------------------------------------------------------------------------------
+ * The reference's parameter server dumps each internal shard's entries under that shard's read lock on a thread pool
+ * while training goes on (persia-model-manager/src/lib.rs:286-343).  These calls write the bytes of such a file, the
+ * speedy encoding of an ArrayLinkedList<HashMapEmbeddingEntry> (persia_b200/checkpoint.py), on the device:
+ *   header = count u64 | first u32 | last u32 | free u32 (0) | end u32 (0) | n_nodes u32            (28 bytes)
+ *   node i = next u32 (i + 2, 0 for the last) | prev u32 (i) | flag u8 (1) | len u32 | f32 x len | dim u64 | sign u64
+ * (29 + 4 len bytes, len = embedding ++ optimizer state).  Entries are read in HBM or, through a host tier, in place in
+ * its mapped host rows.  A host tier is dumped with the table it is attached to (calls on the tier itself are refused).
+ * Both calls are in both chains (top of this file), like pb_get_rows: calls issued before them finish first, calls
+ * issued after them start after them.  The sharded calls are outside the chains: on R GPUs the caller orders a dump
+ * call against them (e.g. by issuing it on the stream its sharded calls use).
+ *
+ * The workspace (collection, sort and locations; about 60 B per entry plus the sort's temporary storage) is allocated
+ * by pb_table_dump_reserve for images of up to max_bytes, replacing any earlier one, and freed by
+ * pb_table_dump_release (or pb_table_destroy).  Both synchronise the device, touch nothing but the workspace and may
+ * run on another host thread than the table's other calls (not beside a dump call on the same table). */
+int pb_table_dump_reserve(pb_table* t, uint64_t max_bytes);
+int pb_table_dump_release(pb_table* t);
+/* One part of a background dump: the entries (HBM and tier, the three marker-valued signs included) whose sign has
+ * part(sign) == part, where part(sign) = splitmix64(sign) % n_parts and
+ *   splitmix64(x): z = x + 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
+ *                  z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31).
+ * They are taken as they are at this call's point in the table's order and listed oldest first: last-use request
+ * number ascending, ties by sign compared as an int64 (pb_table_export_signs' order).  Writes the part's whole image
+ * (header and nodes) to d_image (16-byte aligned) and its size to *d_bytes; an image larger than max_bytes is not
+ * written, only *d_bytes is set (as pb_inc_take does).  *d_request = the table's training-request number at that point.
+ * No host synchronisation and no allocation: the entry count stays on the device (a table that was never allocated
+ * gives the empty list without allocating it).  Needs a workspace reserved for max_bytes or more (else PB_ERR_INVALID). */
+int pb_table_dump_part(pb_table* t, uint32_t part, uint32_t n_parts, void* d_image, uint64_t max_bytes,
+                       uint64_t* d_bytes, uint32_t* d_request, void* stream);
+/* The synchronous dump's slices: nodes [lo, lo + n) of a list of the n_list signs d_signs (the list order the caller
+ * chose, e.g. pb_table_export_signs' sorted), without the header, to d_out (16-byte aligned; n * (29 + 4 len) bytes).
+ * A sign no table holds gets zeros.  Needs a workspace reserved for n entries or more. */
+int pb_dump_nodes(pb_table* t, const uint64_t* d_signs, uint32_t n_list, uint32_t lo, uint32_t n, void* d_out,
+                  void* stream);
 
 /* ---- id preprocessing (the EW's lookup_batched_all_slots_preprocess) --------------------------- */
 /* indices_add_prefix (embedding_worker_service/mod.rs:402-429): out[i] = ids[i] % spacing + prefix of

@@ -304,10 +304,15 @@ class EmbeddingCtx(BaseCtx):  # ctx.py:345-652
     def get_embedding_from_bytes(self, data, device_id=None):  # ctx.py:637-652
         return self.common_context.get_embedding_from_bytes(data, device_id if device_id is not None else self.device_id)
 
-    def dump_embedding(self, dst_dir, blocking=True):  # ctx.py:535-553
-        self.common_context.dump(dst_dir)
+    def dump_embedding(self, dst_dir, blocking=True):  # ctx.py:522-537
+        """blocking=False starts a background dump (training may go on; wait_for_dump_embedding waits for it);
+        blocking=True dumps now."""
+        self.common_context.dump(dst_dir, background=not blocking)
         if blocking:
             self.common_context.wait_for_emb_dumping()
+
+    def wait_for_dump_embedding(self):  # ctx.py:604-606
+        self.common_context.wait_for_emb_dumping()
 
     def load_embedding(self, src_dir, blocking=True):  # ctx.py:515-533
         self.common_context.load(src_dir)

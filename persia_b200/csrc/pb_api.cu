@@ -117,6 +117,9 @@ struct pb_table {
   // incremental updates (pb_table_enable_incremental): the set of signs stepped since the last take; cells == null: off
   IncDev inc{};
   unsigned long long* inc_host = nullptr;  // host address of inc.mirror (cudaFreeHost)
+  // checkpoint images (pb_table_dump_reserve): one allocation holding every DumpWs array; null: none reserved
+  DumpWs dump{};
+  void* dump_mem = nullptr;
 };
 
 struct pb_ctx {
@@ -839,6 +842,10 @@ int pb_table_destroy(pb_table* t) {
     cudaDeviceSynchronize();
     free_incremental(t);
   }
+  if (t->dump_mem) {
+    cudaDeviceSynchronize();
+    cudaFree(t->dump_mem);
+  }
   if (t->stats_ws) cudaFree(t->stats_ws);
   if (t->scratch) cudaFree(t->scratch);
   if (t->adam_dev) cudaFree(t->adam_dev);
@@ -1067,6 +1074,112 @@ int pb_table_export_signs(pb_table* t, uint64_t* d_signs, uint32_t* d_recency, u
   }
   launch_export_signs(t->d, d_signs, d_recency, max_n, d_count, st);
   PB_CUDA(cudaGetLastError());
+  return PB_OK;
+}
+
+namespace {
+
+uint64_t dump_items(pb_table* t, uint64_t max_bytes) {
+  uint32_t len = 0;
+  pb_table_entry_len(t, &len);
+  const uint64_t nb = dump_node_bytes(len);
+  return max_bytes > 28 ? (max_bytes - 28) / nb : 0;
+}
+
+void dump_free(pb_table* t) {
+  if (t->dump_mem) cudaFree(t->dump_mem);
+  t->dump_mem = nullptr;
+  t->dump = DumpWs{};
+}
+
+// a dump call on `t`: the table a tier is attached to, with a workspace of at least `items` entries
+int dump_ready(pb_table* t, uint64_t items) {
+  if (t->tier_of) return fail(PB_ERR_INVALID, "dump the table the tier is attached to");
+  if (!t->dump_mem) return fail(PB_ERR_STATE, "no dump workspace: call pb_table_dump_reserve first");
+  if (items > t->dump.max_items)
+    return fail(PB_ERR_INVALID, "the dump workspace holds " + std::to_string(t->dump.max_items) + " entries, the call needs " +
+                                    std::to_string(items) + ": reserve a larger one");
+  return PB_OK;
+}
+
+}  // namespace
+
+int pb_table_dump_reserve(pb_table* t, uint64_t max_bytes) {
+  if (!t) return fail(PB_ERR_INVALID, "null argument");
+  if (t->tier_of) return fail(PB_ERR_INVALID, "dump the table the tier is attached to");
+  if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered: entry length unknown");
+  DeviceGuard g(t->device);
+  uint64_t items = dump_items(t, max_bytes);
+  if (items < 1) items = 1;
+  if (items >= (1ull << 31)) return fail(PB_ERR_INVALID, "a dump image holds fewer than 2^31 entries");
+  PB_CUDA(cudaDeviceSynchronize());  // a part issued on the old workspace may still run
+  dump_free(t);
+  const uint32_t m = (uint32_t)items;
+  auto r = [](uint64_t b) { return (b + 255) & ~255ull; };
+  const uint64_t sort_bytes = dump_sort_bytes(m);
+  const uint64_t sz8 = r(8ull * m), sz4 = r(4ull * m);
+  PB_CUDA(cudaMalloc(&t->dump_mem, 3 * sz8 + 6 * sz4 + 256 + r(sort_bytes)));
+  char* p = static_cast<char*>(t->dump_mem);
+  DumpWs& w = t->dump;
+  w.key = reinterpret_cast<uint64_t*>(p), p += sz8;
+  w.key_s = reinterpret_cast<uint64_t*>(p), p += sz8;
+  w.loc = reinterpret_cast<uint64_t*>(p), p += sz8;
+  uint32_t** u32s[6] = {&w.rec, &w.rec2, &w.rec_s, &w.idx0, &w.idx1, &w.idx2};
+  for (uint32_t** q : u32s) *q = reinterpret_cast<uint32_t*>(p), p += sz4;
+  w.words = reinterpret_cast<uint32_t*>(p), p += 256;
+  w.sort_tmp = p;
+  w.sort_bytes = sort_bytes;
+  w.max_items = m;
+  return PB_OK;
+}
+
+int pb_table_dump_release(pb_table* t) {
+  if (!t) return fail(PB_ERR_INVALID, "null argument");
+  if (!t->dump_mem) return PB_OK;
+  DeviceGuard g(t->device);
+  PB_CUDA(cudaDeviceSynchronize());
+  dump_free(t);
+  return PB_OK;
+}
+
+int pb_table_dump_part(pb_table* t, uint32_t part, uint32_t n_parts, void* d_image, uint64_t max_bytes,
+                       uint64_t* d_bytes, uint32_t* d_request, void* stream) {
+  if (!t || !d_bytes || !d_request || (max_bytes && !d_image)) return fail(PB_ERR_INVALID, "null argument");
+  if (n_parts == 0 || part >= n_parts) return fail(PB_ERR_INVALID, "part must be in 0..n_parts-1");
+  if (misaligned(d_image)) return fail(PB_ERR_INVALID, "image pointer must be 16-byte aligned");
+  if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered: entry length unknown");
+  int rc = dump_ready(t, dump_items(t, max_bytes));
+  if (rc) return rc;
+  DeviceGuard g(t->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if ((rc = call.begin(t, st, CALL_ALL))) return rc;
+  if (!t->allocated) {  // nothing was ever stored (no allocation here: the caller may hold the table's lock)
+    PB_CUDA(launch_dump_empty(static_cast<uint8_t*>(d_image), max_bytes, reinterpret_cast<unsigned long long*>(d_bytes),
+                              d_request, st));
+    return PB_OK;
+  }
+  const TableDev* h = t->tier && t->tier->allocated ? &t->tier->d : nullptr;
+  PB_CUDA(launch_dump_part(t->d, h, part, n_parts, t->dump, static_cast<uint8_t*>(d_image), max_bytes,
+                           reinterpret_cast<unsigned long long*>(d_bytes), d_request, st));
+  return PB_OK;
+}
+
+int pb_dump_nodes(pb_table* t, const uint64_t* d_signs, uint32_t n_list, uint32_t lo, uint32_t n, void* d_out,
+                  void* stream) {
+  if (!t || (n && (!d_signs || !d_out))) return fail(PB_ERR_INVALID, "null argument");
+  if ((uint64_t)lo + n > n_list) return fail(PB_ERR_INVALID, "nodes [lo, lo + n) must lie in the list");
+  if (misaligned(d_out)) return fail(PB_ERR_INVALID, "output pointer must be 16-byte aligned");
+  if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered: entry length unknown");
+  int rc = dump_ready(t, n);
+  if (rc) return rc;
+  DeviceGuard g(t->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if ((rc = call.begin(t, st, CALL_ALL))) return rc;
+  if ((rc = ensure_alloc(t))) return rc;
+  const TableDev* h = t->tier && t->tier->allocated ? &t->tier->d : nullptr;
+  PB_CUDA(launch_dump_nodes(t->d, h, d_signs, n_list, lo, n, t->dump, static_cast<uint8_t*>(d_out), st));
   return PB_OK;
 }
 

@@ -312,6 +312,39 @@ void launch_tier_where(const TableDev& h, const TableDev& t, const uint64_t* sig
 void launch_tier_set(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const uint64_t* signs,
                      const uint32_t* occ_cell, uint32_t n, const float* entries, cudaStream_t st);
 void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st, uint32_t blocks = 0);
+// checkpoint images (pb_dump.cu).  The part of a sign in a background dump: splitmix64(sign) % n_parts, with
+// splitmix64(x): z = x + 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
+// z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31)   (include/persia_b200.h, pb_table_dump_part)
+__host__ __device__ __forceinline__ uint64_t dump_splitmix64(uint64_t x) {
+  uint64_t z = x + 0x9E3779B97F4A7C15ULL;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
+  return z ^ (z >> 31);
+}
+enum { DW_COUNT = 0, DW_NODES, DW_WORDS };
+// a table's dump workspace (pb_table_dump_reserve): `max_items` entries of each array, the sort's temporary storage
+struct DumpWs {
+  uint64_t* key;    // collected: sign ^ 2^63
+  uint64_t* key_s;  // (sorted keys: discarded)
+  uint64_t* loc;    // collected: row | (1 = the tier's row) << 32; pb_dump_nodes: the located rows
+  uint32_t *rec, *rec2, *rec_s;     // last-use request: collected, in sign order, (sorted: discarded)
+  uint32_t *idx0, *idx1, *idx2;     // item numbers: identity, in sign order, in (request, sign) order
+  uint32_t* words;  // DW_* counters
+  void* sort_tmp;
+  uint64_t sort_bytes;
+  uint32_t max_items;
+};
+uint64_t dump_node_bytes(uint32_t entry_len);
+uint64_t dump_sort_bytes(uint32_t max_items);
+// h: the tier behind t (null: none)
+cudaError_t launch_dump_part(const TableDev& t, const TableDev* h, uint32_t part, uint32_t n_parts, const DumpWs& w,
+                             uint8_t* image, uint64_t max_bytes, unsigned long long* d_bytes, uint32_t* d_request,
+                             cudaStream_t st);
+// the part of a table that was never allocated: the empty list
+cudaError_t launch_dump_empty(uint8_t* image, uint64_t max_bytes, unsigned long long* d_bytes, uint32_t* d_request,
+                              cudaStream_t st);
+cudaError_t launch_dump_nodes(const TableDev& t, const TableDev* h, const uint64_t* signs, uint32_t n_list, uint32_t lo,
+                              uint32_t n, const DumpWs& w, uint8_t* out, cudaStream_t st);
 uint64_t launch_count();
 enum { FAM_PROBE = 0, FAM_DEDUP, FAM_GATHER, FAM_NAN, FAM_HOT, FAM_UPDATE, FAM_OTHER, FAM_WARM, FAM_WAIT, FAM_ROUTE, FAM_OWNER, FAM_COUNT };
 bool profiling();  // a kernel family is being timed: the backward then runs its kernels one after another

@@ -72,6 +72,10 @@ SYMBOLS = {
     "pb_set_rows": (_i32, [_vp, _vp, _vp, _u32, _vp]),
     "pb_get_rows": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp]),
     "pb_table_export_signs": (_i32, [_vp, _vp, _vp, _u32, _vp, _vp]),
+    "pb_table_dump_reserve": (_i32, [_vp, _u64]),
+    "pb_table_dump_release": (_i32, [_vp]),
+    "pb_table_dump_part": (_i32, [_vp, _u32, _u32, _vp, _u64, _vp, _vp, _vp]),
+    "pb_dump_nodes": (_i32, [_vp, _vp, _u32, _u32, _u32, _vp, _vp]),
     "pb_add_prefix": (_i32, [_vp, _u32, C.POINTER(_u32), C.POINTER(_u64), _u32, _u32, _vp, _vp]),
     "pb_shard_of": (_i32, [_vp, _u32, _u32, _vp, _vp]),
     "pb_hash_stack": (_i32, [_vp, _u32, _u32, _u64, _vp, _vp]),

@@ -114,6 +114,8 @@ class _State:
         self.dumper = None  # Train with enable_incremental_update: the writer of this replica's flushes
         self.loader = None  # Infer: the scanner of this replica's incremental directory
         self.inc_lock = threading.Lock()
+        self.gcfg_raw = None  # the global config dict itself (keys parse_global_config does not carry)
+        self.emb_dump = None  # the latest background dump (checkpoint.BackgroundDumper)
 
     def global_config(self):
         """set_global_config's dict, else the PERSIA_GLOBAL_CONFIG yaml, else the reference's defaults."""
@@ -127,7 +129,21 @@ class _State:
 
                 gc = yaml.safe_load(open(g)) or {}
             self.gcfg = INC.parse_global_config(gc)
+            self.gcfg_raw = gc
         return self.gcfg
+
+    def internal_shards(self):
+        """num_hashmap_internal_shards of the global config: the least number of parts of a background dump."""
+        from . import checkpoint as CK
+
+        self.global_config()
+        return CK.internal_shards(self.gcfg_raw)
+
+    def wait_dump(self):
+        """Returns once no background dump runs (its outcome stays in emb_dump for wait_for_emb_dumping)."""
+        d = self.emb_dump
+        if d is not None and d.running():
+            d._thread.join()
 
     def incremental_on(self):
         c = self.global_config()
@@ -172,6 +188,10 @@ class _State:
             if self.incremental_on():  # twice the flush threshold: the set fills while a flush is being taken
                 sh.enable_incremental(2 * self.global_config()["incremental_buffer_size"])
             g = self.groups[dim] = {"shard": sh, "ctx": {}, "device": dev, "lock": threading.RLock()}
+            if (self.replica_size or 1) > 1:  # orders dumps against the sharded calls, whatever their streams
+                from . import checkpoint as CK
+
+                g["fence"] = CK.ShardedFence()
         return g
 
     def all_groups(self):
@@ -197,10 +217,13 @@ def set_global_config(cfg):
     from . import incremental as INC
 
     _S.gcfg = INC.parse_global_config(cfg)
+    _S.gcfg_raw = cfg or {}
 
 
 def reset():
-    """Drop every table and configuration (tests)."""
+    """Drop every table and configuration (tests).  A running background dump is stopped first."""
+    if _S.emb_dump is not None:
+        _S.emb_dump.stop()
     if _S.loader is not None:
         _S.loader.stop()
     if _S.dumper is not None:
@@ -601,6 +624,24 @@ _STATE_LOCK = threading.RLock()  # configuration / group creation; GPU work take
 _BACKWARDS = []                   # live Backward engines (direct lookups wait for their queues to drain)
 
 
+class _Sharded:
+    """A sharded call on group g's table through worker wk (under the group's lock): ordered against the group's dumps
+    by its ShardedFence (the table's chains do not order sharded calls)."""
+
+    def __init__(self, g, wk):
+        self.fence, self.wk = g.get("fence"), wk
+
+    def __enter__(self):
+        if self.fence is not None:
+            self.st = self.wk._torch_stream()
+            self.fence.call_begin(self.st)
+        return self.wk
+
+    def __exit__(self, *exc):
+        if self.fence is not None:
+            self.fence.call_end(self.st)
+
+
 def _forward(batch, device_id, training, direct=False):
     if direct:  # forward_directly (forward.rs:782-831) carries no staleness permit: see every update already handed over
         for b in list(_BACKWARDS):
@@ -663,8 +704,9 @@ def _forward_locked(batch, device_id, training):
                 wk = _sharded_raw_worker(g, sc, B, ids, row_off, dev)
                 d_ids = torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True)
                 d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-                table, index, non_empty, num, counts = wk.forward_raw(d_ids, B, sc.sample_fixed_size, row_off=d_off,
-                                                                      training=training)
+                with _Sharded(g, wk):
+                    table, index, non_empty, num, counts = wk.forward_raw(d_ids, B, sc.sample_fixed_size, row_off=d_off,
+                                                                          training=training)
                 if wk.status()[0]:
                     raise RuntimeError("a batch requested more distinct signs of one shard than the exchange holds: raise "
                                        "PERSIA_B200_XCHG_CAP")
@@ -712,7 +754,8 @@ def _forward_locked(batch, device_id, training):
                     ids = d_ids.cpu().numpy().view(np.uint64)  # (the first batch sizes the exchange from its keys)
                 wk = _sharded_worker(g, dim, names, B, ids, row_off, slot_off, dev)
                 d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-                out = wk.forward(d_ids, B, training=training, row_off=d_off, slot_occ_off=slot_off)
+                with _Sharded(g, wk):
+                    out = wk.forward(d_ids, B, training=training, row_off=d_off, slot_occ_off=slot_off)
                 if wk.status()[0]:
                     raise RuntimeError("a batch requested more distinct signs of one shard than the exchange holds: raise "
                                        "PERSIA_B200_XCHG_CAP")
@@ -993,11 +1036,12 @@ class Backward:  # backward.rs:203-405
                         item = grads.get(names[0])
                         if ctx is None:  # R GPUs: the slot's raw worker (a collective, even when skipped)
                             wk = g["raw_workers"][names[0]]
-                            if item is None:
-                                wk.backward_raw(None)
-                            else:
-                                ptr, shape, is16, sc = item
-                                wk.backward_raw(ptr, scale=sc, is_f16=is16)
+                            with _Sharded(g, wk):
+                                if item is None:
+                                    wk.backward_raw(None)
+                                else:
+                                    ptr, shape, is16, sc = item
+                                    wk.backward_raw(ptr, scale=sc, is_f16=is16)
                         elif item is None:
                             ctx.backward_raw(g["shard"], None)
                         else:
@@ -1018,7 +1062,8 @@ class Backward:  # backward.rs:203-405
                         ptrs.append(ptr)
                         scales.append(sc)
                     if g.get("worker") is not None:
-                        g["worker"].backward_ptrs(ptrs, bool(f16), scales)
+                        with _Sharded(g, g["worker"]) as wk:
+                            wk.backward_ptrs(ptrs, bool(f16), scales)
                     else:
                         ctx.backward_ptrs(g["shard"], ptrs, bool(f16), scales)
             _maybe_flush_incremental()
@@ -1199,18 +1244,40 @@ class PersiaCommonContext:
         return [len(g["shard"]) for g in _S.all_groups()]
 
     def clear_embeddings(self):
+        _S.wait_dump()
         for g in _S.all_groups():
             g["shard"].clear()
 
-    def dump(self, dst_dir):  # lib.rs:356-366 -> PS dump (mod.rs:453-458): the reference's .emb files
+    def dump(self, dst_dir, background=None):  # lib.rs:356-366 -> PS dump (mod.rs:453-458): the reference's .emb files
+        """background: True starts a background dump (checkpoint.BackgroundDumper: the tables are dumped part by part
+        while training goes on; wait_for_emb_dumping / dump_status follow it) and returns; False dumps now, one file per
+        dim, each table read under its group's lock; None: background when PERSIA_B200_BACKGROUND_DUMP=1."""
         from . import checkpoint as CK
 
+        if background is None:
+            background = os.environ.get("PERSIA_B200_BACKGROUND_DUMP", "") == "1"
         _S.ensure_config()
-        CK.dump_shards(dst_dir, [g["shard"] for g in _S.all_groups()], _S.replica_index or 0, max(1, _S.replica_size or 1))
+        if _S.emb_dump is not None and _S.emb_dump.running():
+            raise RuntimeError("an embedding dump is already running: wait_for_emb_dumping() first")
+        groups = _S.all_groups()
+        r, R = _S.replica_index or 0, max(1, _S.replica_size or 1)
+        if not background:
+            _S.emb_dump = None  # an earlier background dump's outcome no longer describes the latest dump
+            CK.dump_shards(dst_dir, [g["shard"] for g in groups], r, R, locks=[g["lock"] for g in groups],
+                           fences=[g.get("fence") for g in groups])
+            return
+        tables = [CK.DumpTable(g["shard"], g["lock"], fence=g.get("fence")) for g in groups]
+        _S.emb_dump = CK.BackgroundDumper(dst_dir, tables, r, R, shards=_S.internal_shards()).start()
+
+    def dump_status(self):
+        """Not part of the reference surface (its servers report it through wait_for_emb_dumping's polling, rpc.rs:211-280):
+        ("Idle", 1.0), ("Dumping", fraction done) or ("Failed", message) of this replica's latest background dump."""
+        return _S.emb_dump.status() if _S.emb_dump is not None else ("Idle", 1.0)
 
     def load(self, src_dir):  # lib.rs:368-378 -> PS load (mod.rs:460-466)
         from . import checkpoint as CK
 
+        _S.wait_dump()
         _S.ensure_config()
         if _S.optimizer is None:
             raise RuntimeError("optimizer not registered: the entry layout (embedding ++ state) is unknown")
@@ -1243,7 +1310,10 @@ class PersiaCommonContext:
         return None
 
     def wait_for_emb_dumping(self):
-        return None
+        """Blocks until this replica's background dump is done (on replica 0: until the root marker is written, after
+        every replica's); RuntimeError("emb dump FAILED for server {r}, due to ...") when it failed."""
+        if _S.emb_dump is not None:
+            _S.emb_dump.wait()
 
     def shutdown_servers(self):
         return None
@@ -1305,6 +1375,7 @@ class PersiaCommonContext:
     def set_embedding(self, embeddings):  # lib.rs:433-449: [(sign, emb f32 ndarray, opt f32 ndarray)]
         import torch
 
+        _S.wait_dump()
         _S.ensure_config()
         by_dim = {}
         for sign, emb, opt in embeddings:

@@ -312,6 +312,34 @@ class EmbeddingShard:
             signs, rec = signs[order], rec[order]
         return signs, rec
 
+    # checkpoint images on the device (include/persia_b200.h, pb_table_dump_*)
+    def node_bytes(self):
+        """Bytes of one entry's node in a `.emb` list: 29 + 4 * entry_len."""
+        return 29 + 4 * self.entry_len
+
+    def dump_reserve(self, max_bytes):
+        """Allocates the dump workspace for images of up to max_bytes (synchronises the device)."""
+        N.check(self.lib.pb_table_dump_reserve(self.h, int(max_bytes)))
+
+    def dump_release(self):
+        N.check(self.lib.pb_table_dump_release(self.h))
+
+    def dump_part(self, part, n_parts, image, meta, stream=None):
+        """Enqueues part `part` of `n_parts` on `stream` (None: the current one): its image into `image` (device uint8,
+        16-byte aligned; its size is the image bound), its size into meta[0] and the table's request number into the low
+        word of meta[1] (meta: device int64 [2])."""
+        st = C.c_void_p((stream or torch.cuda.current_stream(self.device)).cuda_stream)
+        base = meta.data_ptr()
+        N.check(self.lib.pb_table_dump_part(self.h, int(part), int(n_parts), _ptr(image), image.numel(), C.c_void_p(base),
+                                            C.c_void_p(base + 8), st))
+
+    def dump_nodes(self, signs, lo, n, out):
+        """Nodes [lo, lo + n) of the list of `signs` (device int64, in list order) into `out` (device uint8, 16-byte
+        aligned, n * node_bytes()), on the current stream."""
+        signs = _as_i64_bits(signs)
+        N.check(self.lib.pb_dump_nodes(self.h, _ptr(signs), signs.numel(), int(lo), int(n), _ptr(out),
+                                       _stream(self.device)))
+
     def close(self):
         if getattr(self, "h", None):
             self.lib.pb_table_destroy(self.h)
