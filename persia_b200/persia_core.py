@@ -7,11 +7,12 @@ process's GPU, `get_embedding_from_data` / `Forward.get_batch` run pb_forward, `
 the raw device pointers `GradientBatch.add_gradient` receives.  `install()` registers it (and its submodules)
 in `sys.modules` as `persia_core`, after which the reference's own `persia` package runs unchanged on top.
 
-Scope: summation and raw slots (no hash-stack on raw slots), one process per GPU.  With `replica_size > 1` every dim
-group is served by a ShardedEmbeddingWorker and every raw slot by its own ShardedRawWorker (persia_b200.worker), all
-of one dim on the rank's one table; summation slots there may share a feature group (each rank's entries of a shared
-sign are applied in slot order, the ranks in rank order), but a raw slot may not share its feature group with another
-slot of the batch.
+Scope: summation and raw slots (no hash-stack on raw slots), one process per GPU.  The summation slots of one dim are
+served by batch contexts of at most PB_MAX_SLOTS slots each, a feature group never split (slot_chunks).  With
+`replica_size > 1` every such chunk is served by a ShardedEmbeddingWorker and every raw slot by its own
+ShardedRawWorker (persia_b200.worker), all of one dim on the rank's one table; summation slots there may share a
+feature group (each rank's entries of a shared sign are applied in slot order, the ranks in rank order), but a raw slot
+may not share its feature group with another slot of the batch.
 Their calls are collective, so every rank issues them in one fixed order: the raw slots in batch order, then the
 summation dims in ascending order, in the forward and again in the backward; every batch must carry the same raw
 slots in the same order.  `Forward` prefetches on worker threads with the reference's ordering and
@@ -524,10 +525,10 @@ class _Pending:
     """What the EW keeps under backward_ref_id (mod.rs:1087-1098): per dim group, the device context."""
 
     def __init__(self):
-        self.parts = []  # (group, ctx, [slot names in order], is_raw)
+        self.parts = []  # (group, ctx, [slot names in order], is_raw, sharded worker or None)
 
     def release(self):
-        for g, ctx, _, _ in self.parts:
+        for g, ctx, _, _, _ in self.parts:
             if ctx is not None:  # sharded groups keep their one context inside the worker
                 g["ctx"].setdefault(ctx._pool_key, []).append(ctx)
         self.parts = []
@@ -618,6 +619,44 @@ def _to_device_ids(ids, row_off, slot_off, slots, B, dev):
     new_row_off = np.zeros(counts.size + 1, np.uint32)
     new_row_off[1:] = np.cumsum(counts)
     return d_out, new_row_off, new_off
+
+
+def slot_chunks(prefixes):
+    """The summation slots of one dim, given by their index prefixes in batch order, split into the batch contexts that
+    serve them (a context holds at most PB_MAX_SLOTS slots): lists of slot indices, each in batch order.  A feature group
+    (the slots of one index prefix) is never split: Adam advances a group's beta powers once per request, so a group
+    served by two backwards would advance twice.  Groups are packed in the order of their first slot, so the split
+    depends on the slots alone and every rank issues the same calls."""
+    from .native import PB_MAX_SLOTS
+
+    members = {}  # (insertion order: the order of each group's first slot)
+    for i, p in enumerate(prefixes):
+        members.setdefault(p, []).append(i)
+    chunks, cur = [], []
+    for idx in members.values():
+        if len(idx) > PB_MAX_SLOTS:
+            raise RuntimeError(f"a feature group of {len(idx)} summation slots of one dim: one batch context serves at "
+                               f"most {PB_MAX_SLOTS} slots and a feature group is not split across contexts")
+        if len(cur) + len(idx) > PB_MAX_SLOTS:
+            chunks.append(sorted(cur))
+            cur = []
+        cur += idx
+    if cur:
+        chunks.append(sorted(cur))
+    return chunks
+
+
+MAX_CTX_OCCURRENCES = 1 << 24  # id occurrences one batch context holds (pb_ctx_create)
+
+
+def ctx_occurrences(n_ids, rows=0):
+    """Id occurrences of a pooled batch context made for a batch of n_ids ids in `rows` output rows (slots x samples):
+    twice the larger of the two, so that later batches fit, but at most what one context holds.  A batch of more ids
+    than that is refused."""
+    if n_ids > MAX_CTX_OCCURRENCES:
+        raise RuntimeError(f"a batch holds {n_ids} ids in the slots one batch context serves: at most "
+                           f"{MAX_CTX_OCCURRENCES} (2^24) fit, split the batch")
+    return min(max(2 * max(n_ids, rows), 1024), MAX_CTX_OCCURRENCES)
 
 
 _STATE_LOCK = threading.RLock()  # configuration / group creation; GPU work takes the lock of the table it touches
@@ -714,7 +753,7 @@ def _forward_locked(batch, device_id, training):
             raw_out[n] = (Tensor(table[:U + 1], n), Tensor(index, f"{n}_index"),
                           Tensor(non_empty[:ne], f"{n}_non_empty_index"), num.tolist())
             if training:
-                pending.parts.append((g, None, [n], True))
+                pending.parts.append((g, None, [n], True, wk))
             continue
         key = ("raw", n)
         pool = g["ctx"].setdefault(key, [])
@@ -723,7 +762,7 @@ def _forward_locked(batch, device_id, training):
         if pool and pool[-1]._cap >= max(len(ids), B):
             ctx = pool.pop()
         else:
-            cap = max(2 * len(ids), 2 * B, 1024)
+            cap = ctx_occurrences(len(ids), B)
             ctx = SH.BatchContext(cap, cap, [sc.index_prefix], None, _S.prefix_bit, dev)
             ctx._pool_key, ctx._cap = key, cap
         d_ids = torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True)
@@ -734,55 +773,58 @@ def _forward_locked(batch, device_id, training):
         raw_out[n] = (Tensor(table[:U + 1], n), Tensor(index, f"{n}_index"),
                       Tensor(non_empty[:ne], f"{n}_non_empty_index"), num.tolist())
         if training:
-            pending.parts.append((g, ctx, [n], True))
+            pending.parts.append((g, ctx, [n], True, None))
         else:
             pool.append(ctx)
         g["lock"].release()
     for dim in sorted({_S.by_name[n].dim for n, _ in feats if _S.by_name[n].embedding_summation}):
-        part = [(n, x) for n, x in feats if _S.by_name[n].dim == dim and _S.by_name[n].embedding_summation]
-        names = [n for n, _ in part]
+        dim_part = [(n, x) for n, x in feats if _S.by_name[n].dim == dim and _S.by_name[n].embedding_summation]
         with _STATE_LOCK:
             g = _S.group(dim)
-        key = tuple(names)
-        pool = g["ctx"].setdefault(key, [])
-        ids, row_off, slot_off = _flatten(part, B)
-        slots = [_S.by_name[n] for n in names]
-        if (_S.replica_size or 1) > 1:  # R GPUs: the embedding worker's fan-out runs inside the sharded worker
+        if sharded and g.setdefault("names", tuple(n for n, _ in dim_part)) != tuple(n for n, _ in dim_part):
+            raise RuntimeError("on R GPUs every batch must carry the same summation slots of a dim, in the same order")
+        for k, chunk in enumerate(slot_chunks([_S.by_name[n].index_prefix for n, _ in dim_part])):
+            part = [dim_part[i] for i in chunk]
+            names = [n for n, _ in part]
+            key = tuple(names)
+            pool = g["ctx"].setdefault(key, [])
+            ids, row_off, slot_off = _flatten(part, B)
+            slots = [_S.by_name[n] for n in names]
+            if sharded:  # R GPUs: the embedding worker's fan-out runs inside the chunk's sharded worker
+                with g["lock"]:
+                    d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
+                    if len(g.get("workers", ())) <= k and any(sc.hash_stack_rounds > 0 for sc in slots):
+                        ids = d_ids.cpu().numpy().view(np.uint64)  # (the first batch sizes the exchange from its keys)
+                    wk = _sharded_worker(g, k, dim, names, B, ids, row_off, slot_off, dev)
+                    d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
+                    with _Sharded(g, wk):
+                        out = wk.forward(d_ids, B, training=training, row_off=d_off, slot_occ_off=slot_off)
+                    if wk.status()[0]:
+                        raise RuntimeError("a batch requested more distinct signs of one shard than the exchange holds: "
+                                           "raise PERSIA_B200_XCHG_CAP")
+                for i, n in enumerate(names):
+                    by_slot[n] = out[i]
+                if training:
+                    pending.parts.append((g, None, names, False, wk))
+                continue
             with g["lock"]:
                 d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
-                if g.get("worker") is None and any(sc.hash_stack_rounds > 0 for sc in slots):
-                    ids = d_ids.cpu().numpy().view(np.uint64)  # (the first batch sizes the exchange from its keys)
-                wk = _sharded_worker(g, dim, names, B, ids, row_off, slot_off, dev)
+                if pool and pool[-1]._cap >= d_ids.numel():
+                    ctx = pool.pop()
+                else:
+                    cap = ctx_occurrences(int(d_ids.numel()), len(names) * B)
+                    ctx = SH.BatchContext(cap, max(len(names) * max(B, 1) * 2, 1024),
+                                          [_S.by_name[n].index_prefix for n in names],
+                                          [_S.by_name[n].sqrt_scaling for n in names], _S.prefix_bit, dev)
+                    ctx._pool_key, ctx._cap = key, cap
                 d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-                with _Sharded(g, wk):
-                    out = wk.forward(d_ids, B, training=training, row_off=d_off, slot_occ_off=slot_off)
-                if wk.status()[0]:
-                    raise RuntimeError("a batch requested more distinct signs of one shard than the exchange holds: raise "
-                                       "PERSIA_B200_XCHG_CAP")
-            for i, n in enumerate(names):
-                by_slot[n] = out[i]
-            if training:
-                pending.parts.append((g, None, names, False))
-            continue
-        g["lock"].acquire()
-        d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
-        if pool and pool[-1]._cap >= d_ids.numel():
-            ctx = pool.pop()
-        else:
-            cap = max(int(d_ids.numel()), len(names) * max(B, 1), 1)
-            ctx = SH.BatchContext(max(cap * 2, 1024), max(len(names) * max(B, 1) * 2, 1024),
-                                  [_S.by_name[n].index_prefix for n in names],
-                                  [_S.by_name[n].sqrt_scaling for n in names], _S.prefix_bit, dev)
-            ctx._pool_key, ctx._cap = key, max(cap * 2, 1024)
-        d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-        out = ctx.forward(g["shard"], d_ids, slot_off, B, row_off=d_off, training=training)
-        for i, n in enumerate(names):
-            by_slot[n] = out[i]
-        if training:
-            pending.parts.append((g, ctx, names, False))
-        else:
-            pool.append(ctx)
-        g["lock"].release()
+                out = ctx.forward(g["shard"], d_ids, slot_off, B, row_off=d_off, training=training)
+                for i, n in enumerate(names):
+                    by_slot[n] = out[i]
+                if training:
+                    pending.parts.append((g, ctx, names, False, None))
+                else:
+                    pool.append(ctx)
     emb = [Embedding(None, raw=raw_out[n]) if n in raw_out else Embedding(Tensor(by_slot[n], n)) for n, _ in feats]
     to_dev = lambda items: [Tensor(torch.from_numpy(a).to(dev), n) for n, a in items]  # noqa: E731
     return PersiaTrainingBatch(to_dev(batch.non_id_type_features), emb, to_dev(batch.labels), batch.meta_data,
@@ -796,6 +838,8 @@ def _stage(batch):
     under the group's lock.  Results do not change; the forward finds its entries in HBM.  Nothing runs for tables
     without a tier, inference batches, or on R GPUs (no tier there)."""
     import torch
+
+    from .native import PB_MAX_SLOTS
 
     if (_S.replica_size or 1) > 1 or batch.embedding_tensor is None or not _S.slots:
         return
@@ -836,17 +880,19 @@ def _stage(batch):
                     off.append(off[-1] + int(ids.size))
                     prefixes.append(_S.by_name[n].index_prefix)
                 d = torch.cat(parts) if len(parts) > 1 else parts[0]
-                g["shard"].stage(d, off, prefixes, _S.prefix_bit)
+                for lo in range(0, len(prefixes), PB_MAX_SLOTS):  # pb_tier_stage takes at most PB_MAX_SLOTS slots
+                    hi = min(lo + PB_MAX_SLOTS, len(prefixes))
+                    g["shard"].stage(d[off[lo]:off[hi]], [o - off[lo] for o in off[lo:hi + 1]], prefixes[lo:hi],
+                                     _S.prefix_bit)
 
 
-def _sharded_worker(g, dim, names, B, ids, row_off, slot_off, dev):
-    """The dim group's ShardedEmbeddingWorker (persia_b200/worker.py), created by the first batch: a collective —
-    every rank's first lookup of the group must happen in the same step (it does: the ranks train in lockstep)."""
-    wk = g.get("worker")
-    if wk is not None:
-        if wk.names != tuple(names):
-            raise RuntimeError("on R GPUs every batch must carry the same summation slots of a dim, in the same order")
-        return wk
+def _sharded_worker(g, k, dim, names, B, ids, row_off, slot_off, dev):
+    """The ShardedEmbeddingWorker (persia_b200/worker.py) of chunk k (slot_chunks) of the dim group, created by the
+    first batch: a collective — every rank's first lookup of the group must happen in the same step (it does: the ranks
+    train in lockstep).  All chunks of a dim serve the rank's one table."""
+    workers = g.setdefault("workers", [])
+    if k < len(workers):
+        return workers[k]
     import torch
     import torch.distributed as dist
 
@@ -864,8 +910,7 @@ def _sharded_worker(g, dim, names, B, ids, row_off, slot_off, dev):
                        hyper=_S.hyper, max_batch=max(B, max_batch), sqrt_scaling=[sc.sqrt_scaling for sc in slots],
                        rows_f32=ragged, prefix_bit=_S.prefix_bit, max_ids_per_sample=2 * per_sample if ragged else 1,
                        shard=g["shard"])
-    wk.names = tuple(names)
-    g["worker"] = wk
+    workers.append(wk)
     return wk
 
 
@@ -1030,12 +1075,11 @@ class Backward:  # backward.rs:203-405
                 import torch
 
                 torch.cuda.current_stream().wait_event(ready)
-            for g, ctx, names, is_raw in p.parts:
+            for g, ctx, names, is_raw, wk in p.parts:
                 with g["lock"]:
                     if is_raw:  # [U, dim] gradient of the distinct-sign table (persia/ctx.py:970-980)
                         item = grads.get(names[0])
-                        if ctx is None:  # R GPUs: the slot's raw worker (a collective, even when skipped)
-                            wk = g["raw_workers"][names[0]]
+                        if wk is not None:  # R GPUs: the slot's raw worker (a collective, even when skipped)
                             with _Sharded(g, wk):
                                 if item is None:
                                     wk.backward_raw(None)
@@ -1061,8 +1105,8 @@ class Backward:  # backward.rs:203-405
                         f16 = is16
                         ptrs.append(ptr)
                         scales.append(sc)
-                    if g.get("worker") is not None:
-                        with _Sharded(g, g["worker"]) as wk:
+                    if wk is not None:  # R GPUs: the chunk's sharded worker
+                        with _Sharded(g, wk):
                             wk.backward_ptrs(ptrs, bool(f16), scales)
                     else:
                         ctx.backward_ptrs(g["shard"], ptrs, bool(f16), scales)

@@ -358,6 +358,8 @@ class BatchContext:
     """Device-side per-batch context + workspace for the batched forward/backward of one shard."""
 
     def __init__(self, max_occurrences, max_out_rows, prefixes, sqrt_scaling=None, prefix_bit=8, device=0):
+        if len(prefixes) > N.PB_MAX_SLOTS:
+            raise ValueError(f"a batch context serves at most PB_MAX_SLOTS = {N.PB_MAX_SLOTS} slots, got {len(prefixes)}")
         self.lib = N.load()
         self.device = torch.device("cuda", device) if not isinstance(device, torch.device) else device
         self.n_slots = len(prefixes)
