@@ -148,8 +148,10 @@ struct pb_ctx {
   uint32_t* nan_tick = nullptr;
   float* vw_stage = nullptr;
   size_t vw_stage_floats = 0;
-  cudaStream_t side = nullptr;  // hot items + scratch-set clearing run beside the main stream during pb_backward
-  cudaStream_t side2 = nullptr;  // the warm items, beside the cold ones
+  float* hot_stage = nullptr;  // the hot items' sums, b.hot_cap x dim floats (allocated by the training pb_forward)
+  size_t hot_stage_floats = 0;
+  cudaStream_t side = nullptr;  // hot items run beside the main stream during pb_backward
+  cudaStream_t side2 = nullptr;  // scratch-set clearing, then the warm items beside the cold ones
   cudaEvent_t ev_fork = nullptr, ev_nan = nullptr, ev_join = nullptr, ev_join2 = nullptr;
   // raw slot (pb_forward_raw / pb_backward_raw): allocated on first use
   uint32_t* occ_cell = nullptr;
@@ -604,11 +606,12 @@ ReduceArgs reduce_args(const pb_ctx* c) {
   return a;
 }
 
-// A summation backward's side streams: `side` follows `st` from fork_side on; `side` and `side2` follow it from
-// fork_after_nan on (the reduces read the NaN scan's marks); join_sides makes `st` wait for both.
+// A summation backward's side streams: `side` and `side2` follow `st` from fork_side on, and again from fork_after_nan
+// on (what comes after reads the NaN scan's marks); join_sides makes `st` wait for both.
 int fork_side(pb_ctx* c, cudaStream_t st) {
   PB_CUDA(cudaEventRecord(c->ev_fork, st));
   PB_CUDA(cudaStreamWaitEvent(c->side, c->ev_fork, 0));
+  PB_CUDA(cudaStreamWaitEvent(c->side2, c->ev_fork, 0));
   return PB_OK;
 }
 
@@ -1291,7 +1294,7 @@ int pb_ctx_destroy(pb_ctx* c) {
   drop_pending(c);
   drop_raw_pending(c);
   void* ptrs[] = {c->b.set,   c->b.occ_set, c->b.item_cell, c->b.seg_occ, c->b.cold, c->b.warm, c->b.hot, c->b.hot_bits, c->b.cnt,
-                  c->occ_cell, c->occ_outrow, c->row_off, c->nan_tick, c->vw_stage, c->dev_tick, c->raw.set,
+                  c->occ_cell, c->occ_outrow, c->row_off, c->nan_tick, c->vw_stage, c->hot_stage, c->dev_tick, c->raw.set,
                   c->raw.occ_set, c->raw.flag, c->raw.rank, c->raw.tiles, c->raw.distinct_cell, c->raw.counts, c->raw.target,
                   c->raw.peer,    c->raw_stage};
   for (void* p : ptrs)
@@ -1346,6 +1349,28 @@ int pb_ctx_batch_stats(pb_ctx* c, uint32_t h_out[6], void* stream) {
   return PB_OK;
 }
 
+// pb_backward's staging buffer of the hot items' sums, hot_cap x dim floats.  The training forward calls this, so the
+// backward that follows neither synchronises nor allocates (and can be captured without a warm-up call).  The first
+// allocation neither synchronises nor enqueues anything, so that a context's first forward can be captured too: the
+// thread's capture mode is relaxed around it (cudaMalloc is refused under a global-mode capture otherwise).
+static int ensure_hot_stage(pb_ctx* c, uint32_t dim, cudaStream_t st) {
+  const size_t cap = (size_t)c->b.hot_cap * dim;
+  if (cap <= c->hot_stage_floats) return PB_OK;
+  if (c->hot_stage) {  // a wider table: the old buffer may still be read by enqueued work
+    PB_CUDA(cudaStreamSynchronize(st));
+    cudaFree(c->hot_stage);
+    c->hot_stage = nullptr;
+    c->hot_stage_floats = 0;
+  }
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  PB_CUDA(cudaThreadExchangeStreamCaptureMode(&mode));
+  const cudaError_t e = cudaMalloc(&c->hot_stage, sizeof(float) * cap);
+  cudaThreadExchangeStreamCaptureMode(&mode);  // the caller's mode again
+  PB_CUDA(e);
+  c->hot_stage_floats = cap;
+  return PB_OK;
+}
+
 int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
                const uint32_t* h_slot_occ_off, uint32_t batch, int training, void* d_out_f16, void* stream) {
   int rc = check_forward(t, c, d_ids, n_occ, d_row_off, h_slot_occ_off, batch, d_out_f16);
@@ -1363,6 +1388,7 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   TableCall call;
   if ((rc = call.begin(t, st, CALL_INDEX))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
+  if (training && (rc = ensure_hot_stage(c, t->d.dim, st))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
   if ((rc = begin_forward(t, c, sl, d_ids, n_occ, training, st))) return rc;
@@ -1425,28 +1451,42 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
     }
     vw = c->vw_stage;
   }
-  // beside the main stream: the scratch set is emptied and, once the NaN marks are known, the hot items are reduced
+  if ((size_t)c->b.hot_cap * t->d.dim > c->hot_stage_floats)
+    return fail(PB_ERR_STATE, "pb_backward: the pending batch did not come from a training pb_forward of this table");
+  ReduceArgs a = reduce_args(c);
+  a.vw_stage = vw;
+  a.hot_stage = c->hot_stage;
+  auto set_round = [&](uint32_t r) {
+    a.round = r;
+    std::memset(a.round_mask, 0, sizeof(a.round_mask));
+    for (uint32_t s = 0; s < S; ++s)
+      if (c->round_of[s] == r) a.round_mask[s >> 5] |= 1u << (s & 31);
+  };
+  // One round (no shared feature groups, the usual case): the hot items' sums need no NaN mark, so their reduce — the
+  // longest kernel of the step — starts on `side` at once, beside the NaN scan; once the marks are known the hot rows
+  // are stepped there, and the cold and warm items are reduced and stepped on `st` and `side2`.  Several rounds (the
+  // items of a round are distinct rows, whatever their list), or a kernel family being timed: everything on `st`,
+  // round after round.
+  const bool beside = c->n_rounds == 1 && !profiling();
   if ((rc = fork_side(c, st))) return rc;
+  if (beside) {
+    set_round(0);
+    launch_reduce_hot(t->d, sl, gr, is_f16 != 0, a, c->side);
+  }
   const bool mark = t->inc.cells != nullptr;  // the mark reads the scratch set and empties it after the steps
   if (c->set_dirty && !mark) {
-    launch_clear_items(c->b, c->side);
+    launch_clear_items(c->b, c->side2);
     c->set_dirty = false;
   }
   uint32_t elems = c->batch * t->d.dim;
   launch_nan_scan(gr, S, elems, is_f16 != 0, c->dev_tick, c->nan_tick, d_slot_status, st);
   if (adam_keys.n) launch_adam_advance(t->adam_dev, adam_keys, t->op.b1, t->op.b2, st, &gr, S, c->dev_tick, c->nan_tick);
   if ((rc = fork_after_nan(c, st))) return rc;
-  ReduceArgs a = reduce_args(c);
-  a.vw_stage = vw;
   for (uint32_t r = 0; r < c->n_rounds; ++r) {
-    a.round = r;
-    std::memset(a.round_mask, 0, sizeof(a.round_mask));
-    for (uint32_t s = 0; s < S; ++s)
-      if (c->round_of[s] == r) a.round_mask[s >> 5] |= 1u << (s & 31);
-    // one round (no shared feature groups, the usual case): hot items run beside the others; several: one after another
-    // the items of a round are distinct rows, whatever their list.
-    const bool one = c->n_rounds == 1 && !profiling();  // (timed alone when the bench instruments a family)
-    launch_reduce_items(t->d, t->op, t->hy, sl, gr, is_f16 != 0, a, st, one ? c->side : st, one ? c->side2 : st, false);
+    set_round(r);
+    if (!beside) launch_reduce_hot(t->d, sl, gr, is_f16 != 0, a, st);
+    launch_step_hot(t->d, t->op, t->hy, sl, gr, a, beside ? c->side : st);
+    launch_reduce_items(t->d, t->op, t->hy, sl, gr, is_f16 != 0, a, st, beside ? c->side2 : st, false);
   }
   if ((rc = join_sides(c, st))) return rc;
   if (mark) {  // every round has stepped: the applied items that had a row
@@ -1681,8 +1721,9 @@ int pb_backward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* const* h
     ReduceArgs a = reduce_args(c);
     for (uint32_t s = 0; s < S; ++s) a.round_mask[s >> 5] |= 1u << (s & 31);
     a.x = x->d;
-    launch_reduce_items(t->d, t->op, t->hy, sl, gr, is_f16 != 0, a, st, profiling() ? st : c->side,
-                        profiling() ? st : c->side2, true);  // requester: gradients -> owners' areas
+    // requester: gradients -> owners' areas
+    launch_reduce_hot(t->d, sl, gr, is_f16 != 0, a, profiling() ? st : c->side, true);
+    launch_reduce_items(t->d, t->op, t->hy, sl, gr, is_f16 != 0, a, st, profiling() ? st : c->side2, true);
     if ((rc = join_sides(c, st))) return rc;
     if (phases == PB_PHASE_ALL && t->op.kind != PB_OPT_ADAGRAD_VW) launch_signal_wait(x->d, XC_FLAG_GRAD, nullptr, st);
     else launch_signal(x->d, XC_FLAG_GRAD, nullptr, st);

@@ -123,6 +123,7 @@ struct ReduceArgs {
   const uint32_t* tick_ptr;
   const uint32_t* nan_tick;
   float* vw_stage;             // Adagrad vectorwise: one reduced gradient per item
+  float* hot_stage;            // [hot_cap][dim]: the sum of every hot item at its entry of b.hot (k_reduce_hot -> k_step_hot)
   uint32_t batch, round, quiet_miss;
   uint32_t round_mask[PB_MAX_SLOTS / 32];  // slots stepped by this launch (slots of one feature group take turns)
   XchgDev x;                   // sharded: the reduced gradient is stored into the owner's receive area instead
@@ -194,12 +195,19 @@ void launch_copy_entries(bool write, const TableDev& t, const uint32_t* occ_cell
                          uint8_t* found, cudaStream_t st);
 void launch_nan_scan(const GradsDev& gr, uint32_t n_slots, uint32_t elems_per_slot, bool f16, const uint32_t* tick,
                      uint32_t* nan_tick, int32_t* status, cudaStream_t st);
-// pb_reduce.cu: cold + warm items on `st`, hot items on `st_hot` (may equal st)
-// send: sharded requester — a.x names the owners' receive areas, no row is touched here
+// pb_reduce.cu, the backward's reduces.  send: sharded requester — a.x names the owners' receive areas, no row is
+// touched here.
+// cold items on `st`, warm items on `st_warm` (may equal st)
 void launch_reduce_items(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl,
-                         const GradsDev& gr, bool f16, const ReduceArgs& a, cudaStream_t st, cudaStream_t st_hot, cudaStream_t st_warm,
+                         const GradsDev& gr, bool f16, const ReduceArgs& a, cudaStream_t st, cudaStream_t st_warm,
                          bool send = false);
-// diagnostic (pb_hot_geometry): the geometry launch_reduce_items gives k_reduce_hot
+// hot items: the ordered sums (to a.hot_stage unless send; reads no NaN mark unless send), then, local path only, the
+// step of their rows (after the NaN scan and the Adam power advance)
+void launch_reduce_hot(const TableDev& t, const SlotsDev& sl, const GradsDev& gr, bool f16, const ReduceArgs& a,
+                       cudaStream_t st, bool send = false);
+void launch_step_hot(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl, const GradsDev& gr,
+                     const ReduceArgs& a, cudaStream_t st);
+// diagnostic (pb_hot_geometry): the geometry launch_reduce_hot gives k_reduce_hot
 void hot_geometry(uint32_t dim, bool f16, bool ragged, uint32_t out[12]);
 // pb_shard.cu
 void launch_route_items(bool training, const SlotsDev& sl, const BatchDev& b, const XchgDev& x, cudaStream_t st);

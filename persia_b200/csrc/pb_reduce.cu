@@ -1,5 +1,5 @@
-// pb_reduce.cu — backward of the batched path: per distinct sign, the in-order gradient segment reduce (A8) fused with
-// the optimizer step and weight bound on the resident row (A9).  SURVEY.md §8a.
+// pb_reduce.cu — backward of the batched path: per distinct sign, the in-order gradient segment reduce (A8) and the
+// optimizer step and weight bound on the resident row (A9), fused except for hot items.  SURVEY.md §8a.
 //
 // Reference: update_all_batched_gradients (embedding_worker_service/mod.rs:703-872) reduces, per slot and distinct
 // sign, the gradients of the samples holding the sign — sequentially, in the order FeatureBatch::new listed them
@@ -19,8 +19,11 @@
 //                   occurrences after another.  Producer warps load the gradient rows with 16-byte (or element-wise)
 //                   loads, prepare them (f16 -> f32, clamp, scale) and store them into a shared-memory ring of chunks
 //                   guarded by mbarriers; chain warps add the chunks' rows in order — a dependent FADD chain fed from
-//                   shared memory, which is the floor for a strictly sequential sum — then perform the optimizer step.
-//                   Rows wider than HOT_COLS columns take several passes.  Details above the kernel.
+//                   shared memory, which is the floor for a strictly sequential sum — and store the sum to a staging
+//                   buffer.  Rows wider than HOT_COLS columns take several passes.  Details above the kernel.  It reads
+//                   no NaN mark, so the backward runs it beside the NaN scan.
+//   k_step_hot      a lane group per hot item, after the NaN scan: the NaN rule, then the optimizer step with the
+//                   staged sum.
 #include "pb_optim.cuh"
 
 namespace pb {
@@ -158,18 +161,27 @@ __device__ __forceinline__ uint32_t* send_gok_ptr(const XchgDev& x, uint32_t tar
   return reinterpret_cast<uint32_t*>(x.base[q] + x.off_gok) + ((size_t)x.rank * x.cap + k);
 }
 
-// slots whose gradient is skipped or holds a NaN (mod.rs:731-746), or that this launch does not step, as a bit mask
-__device__ __forceinline__ void build_dead_mask(uint32_t* dead, const GradsDev& gr, const ReduceArgs& a, uint32_t n_slots) {
+// slots whose gradient is skipped or holds a NaN (mod.rs:731-746), or that this launch does not step, as a bit mask.
+// nan = false: the NaN marks are left out (and not read: the NaN scan may still be writing them)
+__device__ __forceinline__ void build_dead_mask(uint32_t* dead, const GradsDev& gr, const ReduceArgs& a, uint32_t n_slots,
+                                                bool nan = true) {
   if (threadIdx.x < PB_MAX_SLOTS / 32) dead[threadIdx.x] = 0u;
   __syncthreads();
-  const uint32_t tick = *a.tick_ptr;
+  const uint32_t tick = nan ? *a.tick_ptr : 0u;
   for (uint32_t s = threadIdx.x; s < PB_MAX_SLOTS; s += blockDim.x) {
-    const bool off = s >= n_slots || !gr.ptr[s] || a.nan_tick[s] == tick || !((a.round_mask[s >> 5] >> (s & 31)) & 1u);
+    const bool off = s >= n_slots || !gr.ptr[s] || (nan && a.nan_tick[s] == tick) || !((a.round_mask[s >> 5] >> (s & 31)) & 1u);
     if (off) atomicOr(&dead[s >> 5], 1u << (s & 31));
   }
   __syncthreads();
 }
 __device__ __forceinline__ bool slot_dead(const uint32_t* dead, uint32_t slot) { return (dead[slot >> 5] >> (slot & 31)) & 1u; }
+
+// the entry of `hot` that holds the h-th hot item in reducing order: the giants first, then the huge items (both listed
+// from the end of `hot`), then the others
+__device__ __forceinline__ uint32_t hot_entry(const BatchDev& b, uint32_t h, uint32_t n_giant, uint32_t n_huge) {
+  return h < n_giant ? b.hot_cap - 1u - h
+                     : (h < n_giant + n_huge ? b.hot_cap - 1u - b.giant_cap - (h - n_giant) : h - n_giant - n_huge);
+}
 
 // ------------------------------------------------------------------------------------------------
 // cold and warm items
@@ -349,7 +361,7 @@ __global__ void __launch_bounds__(256) k_reduce_cold(TableDev t, OptimDev op, Hy
 //              chunk's ring slot; every lane arrives on the slot's `full` mbarrier.  The common case (one id per
 //              sample, no scaling) has its own lean loop: ~25 instructions per 16 bytes is what bounds a producer.
 //   chain      (CH warps, 32 * EPL columns each) waits for the slot and adds its rows in order: one LDS and EPL
-//              dependent FADDs per row — nothing else — then arrives on `empty`; finally the optimizer step.
+//              dependent FADDs per row — nothing else — then arrives on `empty`; finally it stores the sum.
 // Measured alternatives (scripts/ubench/hot_ubench.cu): cp.async.bulk of the rows into a raw ring + converter warps is
 // bound by the copy engine's issue rate (~60 cycles per 128-byte copy and SM), a single warp doing load + convert + add
 // by the instruction stream (~40 cycles per row).
@@ -575,9 +587,12 @@ __device__ __forceinline__ void chain_block(float (&acc)[EPL], const float* rp, 
   }
 }
 
+// The sum of an item goes to `out` (dim floats per item), not into the row: SEND, the owner's receive area; otherwise
+// a.hot_stage at the item's entry of `hot`, which k_step_hot steps the row with once the NaN marks are known.  The local
+// reduce reads no NaN mark, so it can run beside the NaN scan: the items of a NaN slot are summed too, their sums unused.
 template <int EPL, bool F16, bool SEND>
-__global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, OptimDev op, HyperDev hy, SlotsDev sl, GradsDev gr,
-                                                              ReduceArgs a, HotGeom geo, unsigned long long* trace) {
+__global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, SlotsDev sl, GradsDev gr, ReduceArgs a, HotGeom geo,
+                                                              unsigned long long* trace) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ uint32_t dead[PB_MAX_SLOTS / 32];
   __shared__ uint32_t s_item, s_nwin;
@@ -585,7 +600,6 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
   __shared__ uint16_t sorted[HOT_WIN];
   __shared__ __align__(8) uint64_t bars[2 * HOT_MAX_SLOTS];  // full[0..8), empty[8..16)
   float* ring = reinterpret_cast<float*>(smem_raw);                     // [S][R][stride] prepared rows
-  float* vstage = ring + (size_t)geo.S * geo.R * geo.stride;            // [dim] Adagrad-vectorwise dot
   const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t CH = geo.CH, PW = hot_producers(CH, geo.S);
   if (tid == 0) {
@@ -595,7 +609,7 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  build_dead_mask(dead, gr, a, sl.n_slots);  // ends with __syncthreads
+  build_dead_mask(dead, gr, a, sl.n_slots, SEND);  // ends with __syncthreads
   const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + HOT_MAX_SLOTS);
   const uint32_t n_giant = a.b.cnt[BC_GIANT], n_huge = a.b.cnt[BC_HUGE];  // the longest chains first
   const uint32_t n_hot = a.b.cnt[BC_HOT] + n_huge + n_giant;
@@ -610,8 +624,8 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
     const uint32_t h = s_item;
     if (h >= n_hot) break;
     if (trace && tid == 0) trace[8 * h] = globaltimer_ns();
-    const uint4 d = a.b.hot[h < n_giant ? a.b.hot_cap - 1u - h
-                                        : (h < n_giant + n_huge ? a.b.hot_cap - 1u - a.b.giant_cap - (h - n_giant) : h - n_giant - n_huge)];
+    const uint32_t entry = hot_entry(a.b, h, n_giant, n_huge);
+    const uint4 d = a.b.hot[entry];
     const uint32_t row = d.x, cnt = d.z, slot = d.w;
     const bool bm_mode = d.y >> 31;
     const uint32_t base = d.y & 0x7FFFFFFFu;  // first bitmap word of the item, or first entry of its occurrence list
@@ -621,8 +635,7 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
       skip = row == ROW_NONE || slot_dead(dead, slot);
       if (row != ROW_NONE && tid == 0) *send_gok_ptr(a.x, row) = slot_dead(dead, slot) ? 0u : 1u;
     } else {
-      skip = slot_dead(dead, slot) || row >= t.capacity;
-      if (!slot_dead(dead, slot) && row >= t.capacity && tid == 0 && !a.quiet_miss) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);
+      skip = slot_dead(dead, slot) || row >= t.capacity;  // (k_step_hot counts the rowless items of applied slots)
     }
     if (skip) {  // the item's bits must still go back to zero for the next batch, unless a later round reads them
       const bool other_round = !((a.round_mask[slot >> 5] >> (slot & 31)) & 1u);  // (an earlier one zeroed them already)
@@ -631,10 +644,7 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
       continue;
     }
     const ItemSrc src = item_src(sl, gr, a, slot);
-    float* prow = SEND ? send_grad_ptr(a.x, row, t.dim) : t.rows + (size_t)row * t.stride;
-    StepCtx sc;
-    sc.vw_state = sc.r1 = sc.r2 = 0.0f;
-    if (!SEND) sc = step_ctx(prow, t, op, gr, slot);
+    float* out = SEND ? send_grad_ptr(a.x, row, t.dim) : a.hot_stage + (size_t)entry * t.dim;
     for (uint32_t pass = 0; pass < n_pass; ++pass) {
       const uint32_t col0 = pass * HOT_COLS;
       HotGeom g = geo;
@@ -770,46 +780,61 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Optim
         trace[8 * h + 2] = globaltimer_ns();
         trace[8 * h + 3] = ((unsigned long long)blockIdx.x << 32) | cnt;
       }
-      // ---- the optimizer step on this pass's columns (chain warps).  Columns past dim (dim % EPL != 0) were summed
-      // from the ring's padding and are dropped here.  EPL-wide loads and stores need the optimizer state (at
-      // prow + dim + e0) and the rows of the send area (dim floats each) aligned to EPL floats, i.e. dim % EPL == 0;
-      // otherwise the step goes element by element.
+      // ---- this pass's columns of the sum (chain warps).  Columns past dim (dim % EPL != 0) were summed from the
+      // ring's padding and are dropped here.  EPL-wide stores need the item's rows of `out` (dim floats each) aligned
+      // to EPL floats, i.e. dim % EPL == 0; otherwise they go element by element.
       if (own) {
         const uint32_t nq = min((uint32_t)EPL, t.dim - e0);
-        const bool wide = nq == EPL && t.dim % EPL == 0;
-        if (SEND) {
-          if (wide) RowElems<-1, EPL>::template st<EPL>(prow + e0, acc);
-          else for (uint32_t q = 0; q < nq; ++q) prow[e0 + q] = acc[q];
-        } else if (wide) {
-          RowElems<-1, EPL> rc;
-          rc.load(prow, e0, t, op);
-          if (op.kind == PB_OPT_ADAGRAD_VW) {
-#pragma unroll
-            for (int q = 0; q < EPL; ++q) vstage[e0 + q] = acc[q];
-          }
-          rc.step(e0, acc, t, op, hy, sc);
-          rc.store(prow, e0, t, op);
-        } else {
-          for (uint32_t q = 0; q < nq; ++q) {
-            RowElems<-1, 1> rc;
-            float one[1] = {acc[q]};
-            rc.load(prow, e0 + q, t, op);
-            if (op.kind == PB_OPT_ADAGRAD_VW) vstage[e0 + q] = acc[q];
-            rc.step(e0 + q, one, t, op, hy, sc);
-            rc.store(prow, e0 + q, t, op);
-          }
-        }
-      }
-    }
-    if (!SEND && op.kind == PB_OPT_ADAGRAD_VW) {  // state = state*mom + dot(g,g)/dim (optim.rs:280-283)
-      __syncthreads();                            // every chain warp staged its columns
-      if (tid == 0) {
-        float gs = __fdiv_rn(vw_dot(vstage, t.dim), (float)t.dim);
-        prow[t.dim] = __fadd_rn(__fmul_rn(sc.vw_state, op.mom), gs);
+        if (nq == EPL && t.dim % EPL == 0) RowElems<-1, EPL>::template st<EPL>(out + e0, acc);
+        else for (uint32_t q = 0; q < nq; ++q) out[e0 + q] = acc[q];
       }
     }
   }
   if (failed && lane == 0) atomicAdd(&t.counters[CTR_ERR], 1u);
+}
+
+// ---- hot items, the step (local path): a lane group per item takes the sum k_reduce_hot staged at its entry of `hot`,
+// applies the whole dead mask, NaN marks included, and steps the row.  The step depends on the element index and the
+// summed value only, so the rows come out as they would from a step fused into the reduce.
+template <int VEC>
+__global__ void __launch_bounds__(256) k_step_hot(TableDev t, OptimDev op, HyperDev hy, SlotsDev sl, GradsDev gr,
+                                                  ReduceArgs a, uint32_t G) {
+  __shared__ uint32_t dead[PB_MAX_SLOTS / 32];
+  const uint32_t n_giant = a.b.cnt[BC_GIANT], n_huge = a.b.cnt[BC_HUGE];
+  const uint32_t n_hot = a.b.cnt[BC_HOT] + n_huge + n_giant;
+  if (blockIdx.x * (blockDim.x / G) >= n_hot) return;  // whole block
+  build_dead_mask(dead, gr, a, sl.n_slots);
+  const uint32_t lane = threadIdx.x % G, wl = threadIdx.x & 31;
+  const uint32_t gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (wl / G * G));
+  const uint32_t nvec = t.dim / VEC;
+  for (uint32_t h = blockIdx.x * (blockDim.x / G) + threadIdx.x / G; h < n_hot; h += gridDim.x * (blockDim.x / G)) {
+    const uint32_t entry = hot_entry(a.b, h, n_giant, n_huge);
+    const uint4 d = a.b.hot[entry];
+    const uint32_t row = d.x, slot = d.w;
+    if (slot_dead(dead, slot)) continue;
+    if (row >= t.capacity) {
+      if (lane == 0 && !a.quiet_miss) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);  // gradient_id_miss_count (PS mod.rs:401-403)
+      continue;
+    }
+    const float* sum = a.hot_stage + (size_t)entry * t.dim;
+    float* prow = t.rows + (size_t)row * t.stride;
+    const StepCtx sc = step_ctx(prow, t, op, gr, slot);
+    for (uint32_t c = lane; c < nvec; c += G) {
+      RowElems<-1, VEC> rc;
+      float g[VEC];
+      rc.load(prow, c * VEC, t, op);
+      load_vec<VEC>(sum + c * VEC, g);
+      rc.step(c * VEC, g, t, op, hy, sc);
+      rc.store(prow, c * VEC, t, op);
+    }
+    if (op.kind == PB_OPT_ADAGRAD_VW) {  // state = state*mom + dot(g,g)/dim (optim.rs:280-283)
+      __syncwarp(gmask);                 // every lane of the group read the old state
+      if (lane == 0) {
+        float gs = __fdiv_rn(vw_dot(sum, t.dim), (float)t.dim);
+        prow[t.dim] = __fadd_rn(__fmul_rn(sc.vw_state, op.mom), gs);
+      }
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -884,10 +909,9 @@ void hot_geometry(uint32_t dim, bool f16, bool ragged, uint32_t out[12]) {
 }
 
 template <int EPL, bool F16, bool SEND>
-static void hot_launch(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl, const GradsDev& gr,
-                       const ReduceArgs& a, cudaStream_t st) {
+static void hot_launch(const TableDev& t, const SlotsDev& sl, const GradsDev& gr, const ReduceArgs& a, cudaStream_t st) {
   const HotGeom g = hot_geom(t.dim, F16, a.occ_outrow != nullptr);
-  const size_t smem = (size_t)g.S * g.R * g.stride * 4u + (((size_t)t.dim + 3u) & ~(size_t)3u) * 4u;
+  const size_t smem = (size_t)g.S * g.R * g.stride * 4u;
   auto kern = k_reduce_hot<EPL, F16, SEND>;
   static size_t configured[64] = {0};  // per instantiation and device
   int dev = 0;
@@ -901,29 +925,43 @@ static void hot_launch(const TableDev& t, const OptimDev& op, const HyperDev& hy
   const uint32_t cap_blocks = cdiv(a.b.n, PB_WARM_MAX + 1);  // at most this many hot items exist
   uint32_t grid = PB_NUM_SMS;
   if (grid > cap_blocks) grid = cap_blocks ? cap_blocks : 1;
-  PB_LAUNCH_F(FAM_HOT, kern, grid, HOT_THREADS, smem, st, t, op, hy, sl, gr, a, g, g_hot_trace);
+  PB_LAUNCH_F(FAM_HOT, kern, grid, HOT_THREADS, smem, st, t, sl, gr, a, g, g_hot_trace);
+}
+
+void launch_reduce_hot(const TableDev& t, const SlotsDev& sl, const GradsDev& gr, bool f16, const ReduceArgs& a,
+                       cudaStream_t st, bool send) {
+  if (!a.b.n) return;
+#define PB_H(E)                                              \
+  if (send) {                                                \
+    if (f16) hot_launch<E, true, true>(t, sl, gr, a, st);    \
+    else hot_launch<E, false, true>(t, sl, gr, a, st);       \
+  } else {                                                   \
+    if (f16) hot_launch<E, true, false>(t, sl, gr, a, st);   \
+    else hot_launch<E, false, false>(t, sl, gr, a, st);      \
+  }
+  if (hot_epl(t.dim) == 2u) { PB_H(2) } else { PB_H(4) }
+#undef PB_H
+}
+
+void launch_step_hot(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl, const GradsDev& gr,
+                     const ReduceArgs& a, cudaStream_t st) {
+  if (!a.b.n) return;
+  int vec, Gi;
+  vec_group(t.dim, vec, Gi);
+  const uint32_t G = (uint32_t)Gi < 4u ? 4u : (uint32_t)Gi;
+  // at most this many hot items exist; blocks past their number return at once
+  uint32_t grid = cdiv(cdiv(a.b.n, PB_WARM_MAX + 1), 256u / G);
+  if (grid > PB_NUM_SMS * 2u) grid = PB_NUM_SMS * 2u;  // groups stride over the list
+  if (vec == 4) PB_LAUNCH(k_step_hot<4>, grid, 256, 0, st, t, op, hy, sl, gr, a, G);
+  else PB_LAUNCH(k_step_hot<1>, grid, 256, 0, st, t, op, hy, sl, gr, a, G);
 }
 
 void launch_reduce_items(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl,
-                         const GradsDev& gr, bool f16, const ReduceArgs& a, cudaStream_t st, cudaStream_t st_hot,
-                         cudaStream_t st_warm, bool send) {
+                         const GradsDev& gr, bool f16, const ReduceArgs& a, cudaStream_t st, cudaStream_t st_warm, bool send) {
   if (!a.b.n) return;
   int vec, Gi;
   vec_group(t.dim, vec, Gi);
   uint32_t G = (uint32_t)Gi < 4u ? 4u : (uint32_t)Gi;
-  // hot items first in time when they have their own stream: they are the long poles
-  {
-#define PB_H(E)                                                             \
-  if (send) {                                                               \
-    if (f16) hot_launch<E, true, true>(t, op, hy, sl, gr, a, st_hot);       \
-    else hot_launch<E, false, true>(t, op, hy, sl, gr, a, st_hot);          \
-  } else {                                                                  \
-    if (f16) hot_launch<E, true, false>(t, op, hy, sl, gr, a, st_hot);      \
-    else hot_launch<E, false, false>(t, op, hy, sl, gr, a, st_hot);         \
-  }
-    if (hot_epl(t.dim) == 2u) { PB_H(2) } else { PB_H(4) }
-#undef PB_H
-  }
   if (vec == 4) {
     if (f16) items_dispatch<4, true>(t, op, hy, sl, gr, a, G, st, st_warm, send);
     else items_dispatch<4, false>(t, op, hy, sl, gr, a, G, st, st_warm, send);

@@ -7,35 +7,45 @@ namespace pb {
 // ------------------------------------------------------------------------------------------------
 // A8 (NaN rule): a slot whose gradient holds any NaN is skipped whole (mod.rs:731-746).
 // grid.y = slot.  status[s] = tick when a NaN was seen (no reset needed between batches).
+// The scan runs beside k_reduce_hot, which holds most of every SM's registers and shared memory, so only a few of its
+// warps fit on an SM: each thread has NAN_LOADS independent 16-byte loads in flight before it tests any, and the
+// register cap (__launch_bounds__ below: <= 32 per thread) lets two 256-thread blocks sit beside a hot block of up to
+// 192 registers per thread.  (A 24-register cap would serialise the loads two by two.)
 // ------------------------------------------------------------------------------------------------
+constexpr uint32_t NAN_LOADS = 4;
+constexpr uint32_t NAN_TRIPS = 4;  // loop trips per thread the grid is sized for (up to 4 blocks per SM and slot)
+
 template <bool F16>
-__global__ void __launch_bounds__(256) k_nan_scan(GradsDev gr, uint32_t elems_per_slot,
-                                                  const uint32_t* __restrict__ tick_ptr,
-                                                  uint32_t* __restrict__ nan_tick) {
-  uint32_t s = blockIdx.y;
+__device__ __forceinline__ bool nan_bits(uint32_t w) {
+  if (F16) return ((w & 0x7fffu) > 0x7c00u) | (((w >> 16) & 0x7fffu) > 0x7c00u);
+  return (w & 0x7fffffffu) > 0x7f800000u;
+}
+
+template <bool F16>
+__global__ void __launch_bounds__(256, 8) k_nan_scan(GradsDev gr, uint32_t elems_per_slot,
+                                                      const uint32_t* __restrict__ tick_ptr,
+                                                      uint32_t* __restrict__ nan_tick) {
+  const uint32_t s = blockIdx.y;
   const void* base = gr.ptr[s];
   if (!base) return;
   bool bad = false;
-  uint32_t stride = gridDim.x * blockDim.x;
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (F16) {
-    // 8 halves per 16 B load; the ABI refuses gradient pointers that are not 16-byte aligned
-    const uint4* p = reinterpret_cast<const uint4*>(base);
-    uint32_t nv = elems_per_slot / 8;
-    for (uint32_t j = i; j < nv; j += stride) {
-      uint4 v = p[j];
-      uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  const uint32_t stride = gridDim.x * blockDim.x;
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  // 8 halves or 4 floats per 16-byte load; the ABI refuses gradient pointers that are not 16-byte aligned
+  constexpr uint32_t EV = F16 ? 8u : 4u;
+  const uint4* p = reinterpret_cast<const uint4*>(base);
+  const uint32_t nv = elems_per_slot / EV;
+  for (uint32_t j = i; j < nv; j += NAN_LOADS * stride) {
+    uint4 v[NAN_LOADS];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        uint32_t lo = w[k] & 0x7fffu, hi = (w[k] >> 16) & 0x7fffu;
-        bad |= (lo > 0x7c00u) | (hi > 0x7c00u);
-      }
-    }
-    const uint16_t* q = reinterpret_cast<const uint16_t*>(base);
-    for (uint32_t j = nv * 8 + i; j < elems_per_slot; j += stride) bad |= (q[j] & 0x7fffu) > 0x7c00u;
-  } else {
-    const float* p = reinterpret_cast<const float*>(base);
-    for (uint32_t j = i; j < elems_per_slot; j += stride) bad |= isnan(p[j]);
+    for (uint32_t u = 0; u < NAN_LOADS; ++u) v[u] = j + u * stride < nv ? p[j + u * stride] : make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+    for (uint32_t u = 0; u < NAN_LOADS; ++u)
+      bad |= nan_bits<F16>(v[u].x) | nan_bits<F16>(v[u].y) | nan_bits<F16>(v[u].z) | nan_bits<F16>(v[u].w);
+  }
+  for (uint32_t j = nv * EV + i; j < elems_per_slot; j += stride) {
+    bad |= F16 ? nan_bits<true>(reinterpret_cast<const uint16_t*>(base)[j])
+               : nan_bits<false>(reinterpret_cast<const uint32_t*>(base)[j]);
   }
   if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) nan_tick[s] = *tick_ptr;
 }
@@ -97,8 +107,8 @@ __global__ void __launch_bounds__(256) k_update_direct(TableDev t, OptimDev op, 
 // ------------------------------------------------------------------------------------------------
 void launch_nan_scan(const GradsDev& gr, uint32_t n_slots, uint32_t elems_per_slot, bool f16, const uint32_t* tick,
                      uint32_t* nan_tick, int32_t* status, cudaStream_t st) {
-  uint32_t per = f16 ? elems_per_slot / 8 : elems_per_slot;
-  uint32_t gx = cdiv(per ? per : 1, 256 * 4);
+  const uint32_t per = elems_per_slot / (f16 ? 8u : 4u);  // 16-byte loads per slot
+  uint32_t gx = cdiv(per ? per : 1, 256 * NAN_LOADS * NAN_TRIPS);
   if (gx > PB_NUM_SMS * 4) gx = PB_NUM_SMS * 4;
   dim3 grid(gx, n_slots);
   if (f16) PB_LAUNCH_F(FAM_NAN, k_nan_scan<true>, grid, 256, 0, st, gr, elems_per_slot, tick, nan_tick);
