@@ -56,7 +56,8 @@ typedef enum {
   PB_ERR_CUDA = -2,      /* CUDA runtime error (message in pb_last_error) */
   PB_ERR_STATE = -3,     /* optimizer / hyper-parameters not configured (reference: OptimizerNotFoundError, NotConfiguredError) */
   PB_ERR_CAPACITY = -4,  /* workspace too small for this batch */
-  PB_ERR_BATCH = -5      /* batch size > 65535 (persia-common/src/lib.rs:49-51 panics) */
+  PB_ERR_BATCH = -5,     /* batch size > 65535 (persia-common/src/lib.rs:49-51 panics) */
+  PB_ERR_FORMAT = -6     /* malformed checkpoint image; pb_last_error() = "ExceptionType: message" (pb_image_index) */
 } pb_status;
 
 typedef enum { PB_OPT_SGD = 0, PB_OPT_ADAGRAD = 1, PB_OPT_ADAGRAD_VW = 2, PB_OPT_ADAM = 3 } pb_optim_kind;
@@ -269,6 +270,46 @@ int pb_table_dump_part(pb_table* t, uint32_t part, uint32_t n_parts, void* d_ima
  * A sign no table holds gets zeros.  Needs a workspace reserved for n entries or more. */
 int pb_dump_nodes(pb_table* t, const uint64_t* d_signs, uint32_t n_list, uint32_t lo, uint32_t n, void* d_out,
                   void* stream);
+
+/* ---- checkpoint loads on the device ----------------------------------------------------------------------------------
+ * The reference's server loads every `.emb` of its shard directory, one job per file, each decoded whole
+ * (read_to_end_speedy) and inserted in list order (persia-model-manager/src/lib.rs:259-273, 375-425;
+ * embedding_parameter_service/mod.rs:460-466); a re-sharding load keeps the entries with
+ * farmhash64(sign) % R == rank (embedding_worker_service/mod.rs:1197-1259).  A pb_image indexes one list image (or a
+ * window of whole nodes of one) that lies in pinned host memory (cudaHostAlloc, or any pinned buffer under unified
+ * addressing): the kernels read it in place.  pb_image_insert then gathers selected entries into aligned staging and
+ * stores them with pb_set_rows (so in both chains, HBM first, then the tier).  The image must stay unchanged until
+ * the inserts that read it have run (e.g. an event recorded after them).
+ *
+ * Workspace (about 13 B per list position, the staging of max_chunk entries, and the host pass's 13 B per node) is
+ * allocated by the index calls as they need it, in the order of their stream (cudaMallocAsync), and freed by
+ * pb_image_destroy, which synchronises that stream only. */
+typedef struct pb_image pb_image;
+int pb_image_create(int device, uint32_t max_chunk, pb_image** out);
+int pb_image_destroy(pb_image* im);
+/* A whole image of any layout (free nodes, nodes out of list order, mixed entry lengths): node offsets, links and
+ * list order from one sequential pass over it on the host, with checkpoint.decode_list's checks in its order
+ * (PB_ERR_FORMAT with the first failure).  Then, on the device, the entries at list positions [p_lo, p_hi) with
+ * farmhash64(sign) % R == rank are selected and counted per (dim, entry length): h_summary gets *h_rows rows
+ * (dim, entry length, selected entries), at most max_rows (64 always suffice).  Synchronises `stream` once. */
+int pb_image_index(pb_image* im, const void* h_image, uint64_t nbytes, uint32_t p_lo, uint32_t p_hi, uint32_t R,
+                   uint32_t rank, uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows, void* stream);
+/* A window of the writer layout (every file this library's dumps write): nodes [node0, node0 + n) of a file of n_total
+ * nodes of entry_len floats, the window's bytes starting at its first node.  Each node's header is checked on the
+ * device: next = i + 2 (0 for the last), flag 1, entry_len and dim.  *h_writer = 0 when one is not so (nothing of the
+ * window may then be inserted: index the whole file instead); else the selection and summary as pb_image_index's.
+ * Synchronises `stream` once. */
+int pb_image_window(pb_image* im, const void* h_window, uint64_t node0, uint32_t n, uint64_t n_total, uint32_t entry_len,
+                    uint64_t dim, uint32_t R, uint32_t rank, uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows,
+                    int* h_writer, void* stream);
+/* set_embedding of the indexed image's selected dim-`dim` entries [lo, hi) (counted in list order, or from the end of
+ * the list when newest_first, and offered in that order) into `t`, whose entry length they must have; hi - lo at most
+ * max_chunk.  No host synchronisation. */
+int pb_image_insert(pb_image* im, pb_table* t, uint64_t dim, uint32_t lo, uint32_t hi, int newest_first, void* stream);
+/* Pinned host memory, mapped into every device's address space (cudaHostAlloc mapped | portable), for images; freed
+ * by pb_host_free, not kept by any caching allocator once the load ends. */
+int pb_host_alloc(uint64_t bytes, void** out);
+int pb_host_free(void* p);
 
 /* ---- id preprocessing (the EW's lookup_batched_all_slots_preprocess) --------------------------- */
 /* indices_add_prefix (embedding_worker_service/mod.rs:402-429): out[i] = ids[i] % spacing + prefix of

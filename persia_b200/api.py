@@ -315,7 +315,8 @@ class EmbeddingCtx(BaseCtx):  # ctx.py:345-652
         self.common_context.wait_for_emb_dumping()
 
     def load_embedding(self, src_dir, blocking=True):  # ctx.py:515-533
-        self.common_context.load(src_dir)
+        """blocking=False starts a background load (wait_for_emb_loading waits for it); blocking=True loads now."""
+        self.common_context.load(src_dir, background=not blocking)
         if blocking:
             self.common_context.wait_for_emb_loading()
 

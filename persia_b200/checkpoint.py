@@ -548,6 +548,24 @@ def _farmhash64(x):
         return g * mul
 
 
+def load_files(src_dir, replica_index=0, replica_size=1):
+    """The `.emb` files load_shards reads, in its order, and how it selects: (files, error, R, rank).  error: the
+    exception load_shards raises when it reaches the first incomplete shard directory (after the files before it;
+    None: all complete).  Entries are kept when farmhash64(sign) % R == rank."""
+    num_shards, _ = checkpoint_info(src_dir)
+    reshard = num_shards != replica_size
+    dirs = [os.path.join(src_dir, f"s{k}") for k in range(num_shards)] if reshard else [os.path.join(src_dir, f"s{replica_index}")]
+    files = []
+    for shard_dir in dirs:
+        names = sorted(x for x in os.listdir(shard_dir) if x.endswith(".emb")) if os.path.isdir(shard_dir) else []
+        if not os.path.isfile(os.path.join(shard_dir, DONE_FILE)) or not names:
+            return files, RuntimeError(f"LoadingFromUncompeleteCheckpoint({shard_dir!r})"), 1, 0
+        files += [os.path.join(shard_dir, x) for x in names]
+    if reshard and replica_size > 1:
+        return files, None, int(replica_size), int(replica_index)
+    return files, None, 1, 0
+
+
 def load_shards(src_dir, shards_by_dim, replica_index=0, replica_size=1, chunk=1 << 20):
     """EmbeddingWorker::load (embedding_worker_service/mod.rs:1150-1259).  A checkpoint written by as many shards as there
     are replicas now is loaded shard by shard: replica r reads `s{r}` (load_embedding_via_emb_servers ->
@@ -594,3 +612,425 @@ def load_shards(src_dir, shards_by_dim, replica_index=0, replica_size=1, chunk=1
                     sh.set_entries(sg, ent)
                 total += pick.size
     return total
+
+
+# ------------------------------------------------------------------------------------------------ device load
+# The reference's server loads a checkpoint in the background: one job per file, each decoded whole and inserted in
+# list order, while the server reports Loading(progress) (persia-model-manager/src/lib.rs:375-425,
+# embedding_parameter_service/mod.rs:264-280); the caller polls wait_for_emb_loading (persia-core/src/rpc.rs:154-176,
+# 235-283).  Here the entries are decoded, selected and gathered on the device (pb_image_*, pb_load.cu) and offered to
+# the tables in load_shards' order, so the tables end as load_shards leaves them.
+LOAD_SUMMARY_ROWS = 64  # (dim, entry length) pairs one image may hold (pb_load.cu LOAD_PAIRS)
+_FORMAT_ERRORS = {"ValueError": ValueError, "IndexError": IndexError}
+
+
+def writer_layout(size, head):
+    """(n_nodes, entry_len) when a file of `size` bytes whose first 41 bytes (header and first node's header) are
+    `head` may be in the writer layout: count = n_nodes > 0, the list from node 1, the first node live, size =
+    28 + n_nodes (29 + 4 entry_len).  None: any other layout.  The nodes themselves are checked as their windows are
+    read."""
+    if size < 41 or len(head) < 41:
+        return None
+    count = int(np.frombuffer(head[:8], "<u8")[0])
+    first, _, _, _, n = (int(x) for x in np.frombuffer(head[8:28], "<u4"))
+    L = int(np.frombuffer(head[37:41], "<u4")[0])
+    if not n or count != n or first != 1 or head[36] != 1 or size != 28 + n * (29 + 4 * L):
+        return None
+    return n, L
+
+
+def windows(n_nodes, node_bytes, buffer_bytes, newest_first=False):
+    """Node ranges [lo, hi) of a writer-layout file read through a buffer of buffer_bytes: whole nodes, at least one
+    per window.  newest_first: from the end of the file, cut from the end (so that, as in load_shards' reversed
+    chunks, only the last window offered is short)."""
+    w = max(1, int(buffer_bytes) // int(node_bytes))
+    if newest_first:
+        return [(max(0, hi - w), hi) for hi in range(n_nodes, 0, -w)]
+    return [(lo, min(lo + w, n_nodes)) for lo in range(0, n_nodes, w)]
+
+
+def check_dims(summary, shards_by_dim):
+    """load_shards' checks of one image's selected entries, dims ascending: summary rows (dim, entry length,
+    entries).  Returns [(dim, entries)] of the dims with selected entries."""
+    out = []
+    for dim in sorted({d for d, _, k in summary if k}):
+        sh = shards_by_dim.get(dim)
+        if sh is None:
+            raise RuntimeError(f"checkpoint holds dim-{dim} embeddings but no slot has that dim")
+        lens = sorted({ln for d, ln, k in summary if d == dim and k})
+        if lens != [sh.entry_len]:
+            raise RuntimeError(f"dim-{dim} entries of {lens} floats, the registered optimizer needs {sh.entry_len} "
+                               f"(embedding ++ state)")
+        out.append((dim, sum(k for d, _, k in summary if d == dim)))
+    return out
+
+
+class LoadStatus:
+    """The reference's server status while it loads (embedding_parameter_service/mod.rs:264-280): ("Loading", fraction)
+    as work is done, ("Idle", 1.0) once done, ("Failed", "Type: message") when it failed."""
+
+    def __init__(self, total):
+        self.total, self.done, self.error, self.finished = max(1, int(total)), 0, None, False
+
+    def advance(self, amount):
+        self.done = min(self.total, self.done + int(amount))
+
+    def fail(self, e):
+        self.error = f"{type(e).__name__}: {e}"
+
+    def finish(self):
+        self.finished = True
+
+    def __call__(self):
+        if self.error is not None:
+            return ("Failed", self.error)
+        if self.finished:
+            return ("Idle", 1.0)
+        return ("Loading", min(self.done / self.total, 0.999))
+
+
+class _Pinned:
+    """Pinned host memory of the library's own (pb_host_alloc), mapped into the device's address space and freed on
+    close(): the image buffers of a load, released when the load ends rather than kept by a caching allocator."""
+
+    def __init__(self, nbytes):
+        import ctypes as C
+
+        from . import native as N
+
+        self.N, self.lib = N, N.load()
+        p = C.c_void_p()
+        N.check(self.lib.pb_host_alloc(int(nbytes), C.byref(p)))
+        self.ptr, self.size = p.value, int(nbytes)
+        self.view = np.ctypeslib.as_array((C.c_uint8 * max(1, self.size)).from_address(self.ptr))
+
+    def data_ptr(self):
+        return self.ptr
+
+    def close(self):
+        if self.ptr:
+            self.view = None
+            self.N.check(self.lib.pb_host_free(self.ptr))
+            self.ptr = 0
+
+
+class _Image:
+    """A pb_image: one list image (or writer-layout window) in pinned host memory, indexed, selected and inserted on
+    the device."""
+
+    def __init__(self, device, chunk):
+        import ctypes as C
+
+        from . import native as N
+
+        self.C, self.N, self.lib = C, N, N.load()
+        h = C.c_void_p()
+        N.check(self.lib.pb_image_create(device.index or 0, int(chunk), C.byref(h)))
+        self.h = h
+        self._rows = (C.c_uint64 * (3 * LOAD_SUMMARY_ROWS))()
+
+    def _summary(self, n):
+        return [(int(self._rows[3 * i]), int(self._rows[3 * i + 1]), int(self._rows[3 * i + 2])) for i in range(n)]
+
+    def index(self, buf, nbytes, p_lo, p_hi, R, rank, stream):
+        C = self.C
+        rows = C.c_uint32()
+        rc = self.lib.pb_image_index(self.h, C.c_void_p(buf.data_ptr()), int(nbytes), int(p_lo), int(p_hi), R, rank,
+                                     self._rows, LOAD_SUMMARY_ROWS, C.byref(rows), C.c_void_p(stream.cuda_stream))
+        if rc == self.N.PB_ERR_FORMAT:  # decode_list's exception
+            kind, msg = self.lib.pb_last_error().decode().split(": ", 1)
+            raise _FORMAT_ERRORS[kind](msg)
+        self.N.check(rc)
+        return self._summary(rows.value)
+
+    def window(self, buf, node0, n, n_total, entry_len, dim, R, rank, stream):
+        """The window's summary, or None when a node of it is not in the writer layout."""
+        C = self.C
+        rows, ok = C.c_uint32(), C.c_int()
+        self.N.check(self.lib.pb_image_window(self.h, C.c_void_p(buf.data_ptr()), int(node0), int(n), int(n_total),
+                                              int(entry_len), int(dim), R, rank, self._rows, LOAD_SUMMARY_ROWS,
+                                              C.byref(rows), C.byref(ok), C.c_void_p(stream.cuda_stream)))
+        return self._summary(rows.value) if ok.value else None
+
+    def insert(self, shard, dim, lo, hi, newest_first, stream):
+        self.N.check(self.lib.pb_image_insert(self.h, shard.h, int(dim), int(lo), int(hi), int(bool(newest_first)),
+                                              self.C.c_void_p(stream.cuda_stream)))
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.pb_image_destroy(self.h)
+            self.h = None
+
+
+class DeviceLoader:
+    """load_shards on the device, in the foreground or in the background: the same files, entries, order and errors,
+    and the same tables at the end.
+
+    A file in the writer layout (writer_layout) is read through the pinned buffers a window of whole nodes at a time
+    (windows: from the end of the file for a table with a host tier, whose entries go newest first); each window's
+    nodes are checked on the device before any of it is inserted.  A window that is not in the writer layout sends the
+    loader to the whole file, which then gives decode_list's error, or the entries not yet inserted.  Any other file is
+    read whole.  A reader thread reads window or file k + 1 into one of two alternating pinned buffers while k is
+    decoded.  The entries of each dim go to its table in chunks of at most `chunk`, each under the table's lock
+    (locks: {dim: lock}), on a stream of the loader's own, and at R > 1 between the table's ShardedFence calls
+    (fences: {dim: fence}).  Device workspace lives while the load runs.
+
+    run() loads in the caller's thread and raises what load_shards raises; start() runs it on a thread; step()
+    handles one window or file in the caller's thread (tests interleave training steps); wait() blocks and raises
+    RuntimeError("emb dump FAILED for server {r}, due to ...") (the reference's text) when it failed; status():
+    LoadStatus.  Files and windows inserted before a failure stay."""
+
+    def __init__(self, src_dir, shards_by_dim, replica_index=0, replica_size=1, chunk=1 << 20, buffer_bytes=SLICE_BYTES,
+                 locks=None, fences=None):
+        self.src_dir, self.shards = src_dir, dict(shards_by_dim)
+        self.replica_index, self.replica_size = int(replica_index), int(replica_size)
+        self.chunk, self.buffer_bytes = int(chunk), max(64, int(buffer_bytes))
+        self.locks, self.fences = locks or {}, fences or {}
+        self.loaded = 0
+        self.error = None
+        self._status = LoadStatus(1)
+        self._planned = False
+        self._tasks, self._next = [], 0
+        self._thread = None
+        self._stop = False
+        self._opened = False
+
+    # ---- surface ------------------------------------------------------------------------------------------------------
+    def status(self):
+        return self._status()
+
+    def start(self):
+        import threading
+
+        self._thread = threading.Thread(target=self._run, name="persia-emb-load", daemon=True)
+        self._thread.start()
+        return self
+
+    def running(self):
+        return self._thread is not None and self._thread.is_alive()
+
+    def join(self):
+        if self._thread is not None:
+            self._thread.join()
+
+    def wait(self):
+        self.join()
+        if self.error is not None:
+            raise RuntimeError(f"emb dump FAILED for server {self.replica_index}, due to {self._status.error}")
+
+    def stop(self):
+        """Abandons the load after the window or file in hand (what was inserted stays); a load that had not finished
+        then reports ("Failed", "RuntimeError: the load was stopped")."""
+        self._stop = True
+        self.join()
+        self._close()
+
+    def run(self):
+        """Loads everything in the caller's thread; raises the load's exception.  Returns the entries loaded."""
+        try:
+            self._open()
+            pending = self._submit(0)
+            for i in range(len(self._tasks)):
+                if self._stop:
+                    raise RuntimeError("the load was stopped")
+                got = pending.result()
+                pending = self._submit(i + 1)
+                self._handle(i, got)
+            self._status.finish()
+            return self.loaded
+        except Exception as e:  # noqa: BLE001 — recorded as the load's status, then raised
+            self.error = e
+            self._status.fail(e)
+            raise
+        finally:
+            self._close()
+
+    def step(self):
+        """Handles the next window or file in the caller's thread; returns whether any remain."""
+        try:
+            if not self._opened:
+                self._open()
+            if self._next < len(self._tasks):
+                i = self._next
+                self._handle(i, self._read(i))
+            if self._next >= len(self._tasks):
+                self._status.finish()
+                self._close()
+                return False
+            return True
+        except Exception as e:  # noqa: BLE001
+            self.error = e
+            self._status.fail(e)
+            self._close()
+            raise
+
+    # ---- the load -----------------------------------------------------------------------------------------------------
+    def _run(self):
+        try:
+            self.run()
+        except Exception:  # noqa: BLE001 — recorded as the load's status, raised by wait()
+            pass
+
+    def _open(self):
+        import concurrent.futures
+
+        import torch
+
+        files, self._dir_error, self.R, self.rank = load_files(self.src_dir, self.replica_index, self.replica_size)
+        tasks = []  # (file, kind, lo, hi, info): kind "window" (writer layout, nodes [lo, hi)) or "whole"
+        for f in files:
+            size = os.path.getsize(f)
+            with open(f, "rb") as fh:
+                w = writer_layout(size, fh.read(41))
+                if w is not None:
+                    n, L = w
+                    fh.seek(41 + 4 * L)
+                    dim = int(np.frombuffer(fh.read(8), "<u8")[0])
+            if w is None:
+                tasks.append((f, "whole", 0, 0, size))
+                continue
+            sh = self.shards.get(dim)
+            newest = sh is not None and getattr(sh, "host_tier", None) is not None
+            tasks += [(f, "window", lo, hi, (n, L, dim, newest)) for lo, hi in windows(n, 29 + 4 * L, self.buffer_bytes, newest)]
+        if self._dir_error is not None:
+            tasks.append((None, "error", 0, 0, 0))
+        self._tasks = tasks
+        self._skip = set()  # files loaded whole after a window was not in the writer layout
+        self._status = LoadStatus(sum(self._task_bytes(t) for t in tasks))
+        self.device = next(iter(self.shards.values())).device if self.shards else torch.device("cuda", torch.cuda.current_device())
+        self._stream = torch.cuda.Stream(self.device)
+        self._bufs = [None, None]
+        self._done = [torch.cuda.Event(), torch.cuda.Event()]  # the inserts that read each buffer
+        # where the time goes: file reads (reader thread), index calls (host pass + device selection, wall time), and
+        # the device time of the gathers and inserts (CUDA events, from the end of each index call to its last insert)
+        self.timings = {"read_s": 0.0, "index_s": 0.0, "insert_ms": 0.0}
+        self._events = []
+        self._image = _Image(self.device, self.chunk)
+        self._pool = concurrent.futures.ThreadPoolExecutor(1, thread_name_prefix="persia-emb-read")
+        self._opened = True
+
+    def _close(self):
+        if not self._opened:
+            return
+        self._opened = False
+        self._pool.shutdown(wait=True)
+        self._stream.synchronize()
+        self._image.close()
+        self.timings["insert_ms"] += sum(a.elapsed_time(b) for a, b in self._events)
+        self._events = []
+        for b in self._bufs:
+            if b is not None:
+                b.close()
+        self._bufs = [None, None]
+
+    @staticmethod
+    def _task_bytes(t):
+        f, kind, lo, hi, info = t
+        if kind == "window":
+            return (hi - lo) * (29 + 4 * info[1])
+        return info if kind == "whole" else 0
+
+    def _buffer(self, slot, nbytes):
+        buf = self._bufs[slot]
+        if buf is None or buf.size < nbytes:
+            self._done[slot].synchronize()
+            if buf is not None:
+                buf.close()
+            cap = max(64, min(int(nbytes) * 2, max(int(nbytes), self.buffer_bytes)))
+            buf = self._bufs[slot] = _Pinned(cap)
+        return buf
+
+    def _read(self, i):
+        """Task i's bytes into buffer i % 2 (once the inserts that read that buffer before have run)."""
+        f, kind, lo, hi, info = self._tasks[i]
+        slot = i % 2
+        self._done[slot].synchronize()
+        if kind == "error" or f in self._skip:
+            return slot, 0
+        if kind == "window":
+            nb = 29 + 4 * info[1]
+            start, nbytes = 28 + lo * nb, (hi - lo) * nb
+        else:
+            start, nbytes = 0, info
+        buf = self._buffer(slot, nbytes)
+        t0 = time.perf_counter()
+        with open(f, "rb") as fh:
+            fh.seek(start)
+            got = fh.readinto(memoryview(buf.view)[:nbytes])
+        self.timings["read_s"] += time.perf_counter() - t0
+        if got != nbytes:
+            raise RuntimeError(f"{f} changed while it was loaded")
+        return slot, nbytes
+
+    def _submit(self, i):
+        import concurrent.futures
+
+        if i >= len(self._tasks):
+            done = concurrent.futures.Future()
+            done.set_result(None)
+            return done
+        return self._pool.submit(self._read, i)
+
+    def _insert(self, summary, newest_of=None):
+        """load_shards' checks of the image's dims, then their entries, dims ascending, a chunk at a time."""
+        import contextlib
+
+        for dim, k in check_dims(summary, self.shards):
+            sh = self.shards[dim]
+            newest = getattr(sh, "host_tier", None) is not None if newest_of is None else newest_of
+            fence = self.fences.get(dim)
+            for lo in range(0, k, self.chunk):
+                with self.locks.get(dim) or contextlib.nullcontext():
+                    if fence is not None:
+                        fence.dump_begin(self._stream)
+                    self._image.insert(sh, dim, lo, min(lo + self.chunk, k), newest, self._stream)
+                    if fence is not None:
+                        fence.dump_end(self._stream)
+            self.loaded += k
+
+    def _handle(self, i, got):
+        f, kind, lo, hi, info = self._tasks[i]
+        self._next = i + 1
+        slot, nbytes = got
+        if kind == "error":
+            raise self._dir_error
+        if f not in self._skip:
+            import torch
+
+            buf = self._bufs[slot]
+            t0 = time.perf_counter()
+            if kind == "whole":
+                summary = self._image.index(buf, nbytes, 0, 0xFFFFFFFF, self.R, self.rank, self._stream)
+            else:
+                n, L, dim, newest = info
+                summary = self._image.window(buf, lo, hi - lo, n, L, dim, self.R, self.rank, self._stream)
+            self.timings["index_s"] += time.perf_counter() - t0
+            ev = (torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
+            ev[0].record(self._stream)
+            if kind == "whole":
+                self._insert(summary)
+            elif summary is not None:
+                self._insert(summary, newest)
+            else:
+                self._whole_rest(i)
+            ev[1].record(self._stream)
+            self._events.append(ev)
+            self._done[slot].record(self._stream)
+        self._status.advance(self._task_bytes(self._tasks[i]))
+
+    def _whole_rest(self, i):
+        """Window i of its file is not in the writer layout: the whole file, less the windows already inserted (they
+        hold list positions [0, lo), or [hi, n) newest first, whenever the file is a valid list)."""
+        f, _, lo, hi, (n, _, _, newest) = self._tasks[i]
+        self._skip.add(f)
+        self._stream.synchronize()
+        size = os.path.getsize(f)
+        buf = _Pinned(max(64, size))
+        try:
+            with open(f, "rb") as fh:
+                fh.readinto(memoryview(buf.view)[:size])
+            p_lo, p_hi = (0, hi) if newest else (lo, n)
+            self._insert(self._image.index(buf, size, p_lo, p_hi, self.R, self.rank, self._stream))
+            self._stream.synchronize()  # (the inserts read buf)
+        finally:
+            buf.close()

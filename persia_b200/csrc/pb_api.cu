@@ -1186,6 +1186,237 @@ int pb_dump_nodes(pb_table* t, const uint64_t* d_signs, uint32_t n_list, uint32_
   return PB_OK;
 }
 
+// ---- checkpoint loads (pb_load.cu) ----------------------------------------------------------------------------------
+struct pb_image {
+  int device = 0;
+  uint32_t max_chunk = 0;
+  LoadImg L{};           // the image indexed last
+  bool indexed = false;
+  void* sum_mem = nullptr;  // dims, pairs, counts, flags of L
+  uint64_t* off = nullptr;  // per position (whole images)
+  uint8_t* slot = nullptr;
+  uint32_t* sel = nullptr;  // the selected positions of one dim, in list order
+  uint32_t* d_count = nullptr;
+  uint32_t pos_cap = 0;
+  void* tmp = nullptr;
+  size_t tmp_bytes = 0;
+  int sel_slot = -1;        // the dim slot `sel` holds
+  uint64_t* st_signs = nullptr;  // aligned staging of one insert
+  float* st_ent = nullptr;
+  uint64_t st_entries = 0, st_floats = 0;
+  std::vector<uint64_t> host_off;
+  cudaStream_t st = nullptr;  // the stream of the latest call: workspace is allocated and freed in its order
+  unsigned long long h_dims[LOAD_DIMS], h_pairs[LOAD_PAIRS];
+  uint32_t h_counts[LOAD_PAIRS], h_flags[LOAD_FLAGS];
+};
+
+namespace {
+
+// The workspace is stream-ordered (cudaMallocAsync / cudaFreeAsync on the load's stream): a load beside training never
+// waits for the device as a whole, and a buffer is released only after the inserts issued before that read it.
+void free_on(void* p, cudaStream_t st) {
+  if (p) cudaFreeAsync(p, st);
+}
+
+void image_free(pb_image* im, cudaStream_t st) {
+  free_on(im->off, st), free_on(im->slot, st), free_on(im->sel, st), free_on(im->tmp, st);
+  free_on(im->st_signs, st), free_on(im->st_ent, st), free_on(im->sum_mem, st), free_on(im->d_count, st);
+  im->off = nullptr, im->slot = nullptr, im->sel = nullptr, im->tmp = nullptr;
+  im->st_signs = nullptr, im->st_ent = nullptr, im->sum_mem = nullptr, im->d_count = nullptr;
+  im->pos_cap = 0, im->tmp_bytes = 0, im->st_entries = 0, im->st_floats = 0;
+}
+
+// the summary, on first use
+int image_ready(pb_image* im, cudaStream_t st) {
+  im->st = st;
+  if (im->sum_mem) return PB_OK;
+  const size_t sum_bytes = sizeof(unsigned long long) * (LOAD_DIMS + LOAD_PAIRS) + sizeof(uint32_t) * (LOAD_PAIRS + LOAD_FLAGS);
+  PB_CUDA(cudaMallocAsync(&im->sum_mem, sum_bytes + 16, st));
+  PB_CUDA(cudaMallocAsync((void**)&im->d_count, sizeof(uint32_t), st));
+  LoadImg& L = im->L;
+  L.dims = static_cast<unsigned long long*>(im->sum_mem);
+  L.pairs = L.dims + LOAD_DIMS;
+  L.counts = reinterpret_cast<uint32_t*>(L.pairs + LOAD_PAIRS);
+  L.flags = L.counts + LOAD_PAIRS;
+  return PB_OK;
+}
+
+// workspace for n positions (grown, never shrunk while the load runs)
+int image_room(pb_image* im, uint32_t n, cudaStream_t st) {
+  int rc = image_ready(im, st);
+  if (rc) return rc;
+  if (n <= im->pos_cap && im->pos_cap) return PB_OK;
+  free_on(im->off, st), free_on(im->slot, st), free_on(im->sel, st), free_on(im->tmp, st);
+  im->off = nullptr, im->slot = nullptr, im->sel = nullptr, im->tmp = nullptr, im->pos_cap = 0;
+  const uint32_t cap = n ? n : 1;
+  PB_CUDA(cudaMallocAsync((void**)&im->off, sizeof(uint64_t) * cap, st));
+  PB_CUDA(cudaMallocAsync((void**)&im->slot, cap, st));
+  PB_CUDA(cudaMallocAsync((void**)&im->sel, sizeof(uint32_t) * cap, st));
+  im->tmp_bytes = load_list_bytes(cap);
+  PB_CUDA(cudaMallocAsync(&im->tmp, im->tmp_bytes ? im->tmp_bytes : 16, st));
+  im->pos_cap = cap;
+  return PB_OK;
+}
+
+// the selection and per-dim summary of im->L (positions set up by the caller); one host synchronisation
+int image_select(pb_image* im, uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows, cudaStream_t st) {
+  LoadImg& L = im->L;
+  L.slot = im->slot;
+  PB_CUDA(cudaMemsetAsync(L.dims, 0xFF, sizeof(unsigned long long) * (LOAD_DIMS + LOAD_PAIRS), st));
+  PB_CUDA(cudaMemsetAsync(L.counts, 0, sizeof(uint32_t) * (LOAD_PAIRS + LOAD_FLAGS), st));
+  PB_CUDA(launch_load_select(L, st));
+  PB_CUDA(cudaMemcpyAsync(im->h_dims, L.dims, sizeof(im->h_dims), cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaMemcpyAsync(im->h_pairs, L.pairs, sizeof(im->h_pairs), cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaMemcpyAsync(im->h_counts, L.counts, sizeof(im->h_counts), cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaMemcpyAsync(im->h_flags, L.flags, sizeof(im->h_flags), cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  im->sel_slot = -1;
+  im->indexed = true;
+  if (im->h_flags[LOAD_FLAG_FULL])
+    return fail(PB_ERR_INVALID, "a checkpoint file holds more than " + std::to_string(LOAD_DIMS) + " dims or " +
+                                    std::to_string(LOAD_PAIRS) + " (dim, entry length) pairs");
+  // rows (dim, entry length, entries), and staging for the largest insert they allow
+  uint32_t rows = 0;
+  uint64_t most = 0, widest = 0;
+  for (uint32_t j = 0; j < LOAD_PAIRS; ++j) {
+    if (im->h_pairs[j] == KEY_EMPTY) continue;
+    if (rows >= max_rows) return fail(PB_ERR_CAPACITY, "summary rows: pass room for " + std::to_string(LOAD_PAIRS));
+    const uint64_t len = im->h_pairs[j] & 0xFFFFFFFFu;
+    h_summary[3 * rows] = im->h_dims[im->h_pairs[j] >> 32];
+    h_summary[3 * rows + 1] = len;
+    h_summary[3 * rows + 2] = im->h_counts[j];
+    ++rows;
+    most = most > im->h_counts[j] ? most : im->h_counts[j];
+    widest = widest > len ? widest : len;
+  }
+  *h_rows = rows;
+  const uint64_t ent = most < im->max_chunk ? most : im->max_chunk;
+  if (ent > im->st_entries || ent * widest > im->st_floats) {
+    free_on(im->st_signs, st), free_on(im->st_ent, st);
+    im->st_signs = nullptr, im->st_ent = nullptr, im->st_entries = 0, im->st_floats = 0;
+    PB_CUDA(cudaMallocAsync((void**)&im->st_signs, sizeof(uint64_t) * ent, st));
+    PB_CUDA(cudaMallocAsync((void**)&im->st_ent, sizeof(float) * ent * widest, st));
+    im->st_entries = ent, im->st_floats = ent * widest;
+  }
+  return PB_OK;
+}
+
+int image_device_ptr(const void* h, const uint8_t** d) {
+  void* p = nullptr;
+  PB_CUDA(cudaHostGetDevicePointer(&p, const_cast<void*>(h), 0));
+  *d = static_cast<const uint8_t*>(p);
+  return PB_OK;
+}
+
+}  // namespace
+
+int pb_image_create(int device, uint32_t max_chunk, pb_image** out) {
+  if (!out || !max_chunk) return fail(PB_ERR_INVALID, "null argument or zero max_chunk");
+  pb_image* im = new pb_image();
+  im->device = device;
+  im->max_chunk = max_chunk;
+  *out = im;
+  return PB_OK;
+}
+
+int pb_image_destroy(pb_image* im) {
+  if (!im) return PB_OK;
+  DeviceGuard g(im->device);
+  image_free(im, im->st);  // (after the inserts in flight on the load's stream)
+  cudaStreamSynchronize(im->st);
+  delete im;
+  return PB_OK;
+}
+
+int pb_host_alloc(uint64_t bytes, void** out) {
+  if (!out) return fail(PB_ERR_INVALID, "null argument");
+  *out = nullptr;
+  PB_CUDA(cudaHostAlloc(out, bytes ? bytes : 1, cudaHostAllocMapped | cudaHostAllocPortable));
+  return PB_OK;
+}
+
+int pb_host_free(void* p) {
+  if (p) PB_CUDA(cudaFreeHost(p));
+  return PB_OK;
+}
+
+int pb_image_index(pb_image* im, const void* h_image, uint64_t nbytes, uint32_t p_lo, uint32_t p_hi, uint32_t R,
+                   uint32_t rank, uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows, void* stream) {
+  if (!im || !h_image || !h_summary || !h_rows) return fail(PB_ERR_INVALID, "null argument");
+  if (R == 0 || rank >= R) return fail(PB_ERR_INVALID, "rank must be in 0..R-1");
+  DeviceGuard g(im->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  im->indexed = false;
+  std::string err;
+  try {
+    if (!load_index_host(static_cast<const uint8_t*>(h_image), nbytes, im->host_off, err)) return fail(PB_ERR_FORMAT, err);
+  } catch (const std::bad_alloc&) {
+    return fail(PB_ERR_CAPACITY, "host memory for the node offsets of a " + std::to_string(nbytes) + "-byte image");
+  }
+  const uint32_t n = (uint32_t)im->host_off.size();
+  int rc = image_room(im, n, st);
+  if (rc) return rc;
+  LoadImg& L = im->L;
+  if ((rc = image_device_ptr(h_image, &L.img))) return rc;
+  if (n) PB_CUDA(cudaMemcpyAsync(im->off, im->host_off.data(), sizeof(uint64_t) * n, cudaMemcpyHostToDevice, st));
+  L.off = im->off;
+  L.nb = 0, L.n = n, L.p_lo = p_lo, L.p_hi = p_hi < n ? p_hi : n;
+  L.node0 = 0, L.n_total = n, L.dim = 0, L.len = 0, L.R = R, L.rank = rank;
+  return image_select(im, h_summary, max_rows, h_rows, st);
+}
+
+int pb_image_window(pb_image* im, const void* h_window, uint64_t node0, uint32_t n, uint64_t n_total, uint32_t entry_len,
+                    uint64_t dim, uint32_t R, uint32_t rank, uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows,
+                    int* h_writer, void* stream) {
+  if (!im || !h_window || !h_summary || !h_rows || !h_writer) return fail(PB_ERR_INVALID, "null argument");
+  if (R == 0 || rank >= R) return fail(PB_ERR_INVALID, "rank must be in 0..R-1");
+  if (node0 + n > n_total || n_total >= (1ull << 32)) return fail(PB_ERR_INVALID, "nodes [node0, node0 + n) must lie in the file");
+  DeviceGuard g(im->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  im->indexed = false;
+  int rc = image_room(im, n, st);
+  if (rc) return rc;
+  LoadImg& L = im->L;
+  if ((rc = image_device_ptr(h_window, &L.img))) return rc;
+  L.off = nullptr;
+  L.nb = dump_node_bytes(entry_len), L.n = n, L.p_lo = 0, L.p_hi = n;
+  L.node0 = node0, L.n_total = n_total, L.dim = dim, L.len = entry_len, L.R = R, L.rank = rank;
+  if ((rc = image_select(im, h_summary, max_rows, h_rows, st))) return rc;
+  *h_writer = im->h_flags[LOAD_FLAG_BAD] ? 0 : 1;
+  if (!*h_writer) im->indexed = false;
+  return PB_OK;
+}
+
+int pb_image_insert(pb_image* im, pb_table* t, uint64_t dim, uint32_t lo, uint32_t hi, int newest_first, void* stream) {
+  if (!im || !t) return fail(PB_ERR_INVALID, "null argument");
+  if (!im->indexed) return fail(PB_ERR_STATE, "no image indexed: call pb_image_index or pb_image_window first");
+  if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered: entry length unknown");
+  uint32_t len = 0;
+  pb_table_entry_len(t, &len);
+  int j = -1;
+  for (uint32_t k = 0; k < LOAD_DIMS; ++k)
+    if (im->h_dims[k] == dim) j = (int)k;
+  uint64_t K = 0;
+  for (uint32_t k = 0; j >= 0 && k < LOAD_PAIRS; ++k) {
+    if (im->h_pairs[k] == KEY_EMPTY || (int)(im->h_pairs[k] >> 32) != j) continue;
+    if ((im->h_pairs[k] & 0xFFFFFFFFu) != len)
+      return fail(PB_ERR_INVALID, "the image's dim-" + std::to_string(dim) + " entries are not of the table's length");
+    K += im->h_counts[k];
+  }
+  if (lo > hi || hi > K) return fail(PB_ERR_INVALID, "entries [lo, hi) must lie in the image's entries of `dim`");
+  const uint32_t n = hi - lo;
+  if (n > im->st_entries) return fail(PB_ERR_INVALID, "at most max_chunk entries per insert");
+  if (!n) return PB_OK;
+  DeviceGuard g(im->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (im->sel_slot != j) {
+    PB_CUDA(launch_load_list(im->L, (uint32_t)j, im->tmp, im->tmp_bytes, im->sel, im->d_count, st));
+    im->sel_slot = j;
+  }
+  PB_CUDA(launch_load_gather(im->L, im->sel, (uint32_t)K, lo, n, newest_first, len, im->st_signs, im->st_ent, st));
+  return pb_set_rows(t, im->st_signs, im->st_ent, n, stream);
+}
+
 int pb_add_prefix(const uint64_t* d_ids, uint32_t n, const uint32_t* h_slot_occ_off, const uint64_t* h_prefix,
                   uint32_t n_slots, uint32_t prefix_bit, uint64_t* d_out, void* stream) {
   if (n && (!d_ids || !d_out)) return fail(PB_ERR_INVALID, "null argument");

@@ -1,6 +1,8 @@
 // pb_kernels.cuh — kernel-side parameter blocks and launcher prototypes (internal).
 #pragma once
 #include <atomic>
+#include <string>
+#include <vector>
 
 #include "pb_common.cuh"
 
@@ -353,6 +355,32 @@ cudaError_t launch_dump_empty(uint8_t* image, uint64_t max_bytes, unsigned long 
                               cudaStream_t st);
 cudaError_t launch_dump_nodes(const TableDev& t, const TableDev* h, const uint64_t* signs, uint32_t n_list, uint32_t lo,
                               uint32_t n, const DumpWs& w, uint8_t* out, cudaStream_t st);
+// checkpoint loads (pb_load.cu): one list image, read in place (mapped pinned host memory), and its per-dim summary
+constexpr uint32_t LOAD_DIMS = 32, LOAD_PAIRS = 64;  // distinct dims, distinct (dim, entry length) pairs of one image
+constexpr uint32_t LOAD_NONE = 0xFF;                  // slot of a position not selected
+enum { LOAD_FLAG_BAD = 0, LOAD_FLAG_FULL, LOAD_FLAGS };
+struct LoadImg {
+  const uint8_t* img;   // device address of the image's bytes (a window: its first node's)
+  const uint64_t* off;  // byte offset of each list position's node; null: a writer-layout window (pos * nb)
+  uint64_t nb;          // writer layout: node bytes
+  uint32_t n;           // list positions
+  uint32_t p_lo, p_hi;  // positions offered (the others are not selected)
+  uint64_t node0, n_total, dim;  // writer layout: the window's first node, the file's nodes, its dim
+  uint32_t len;                  // writer layout: its entry length
+  uint32_t R, rank;              // selection: farmhash64(sign) % R == rank
+  uint8_t* slot;                 // per position: summary slot of its dim, LOAD_NONE = not selected
+  unsigned long long* dims;      // LOAD_DIMS, KEY_EMPTY = unused
+  unsigned long long* pairs;     // LOAD_PAIRS: slot << 32 | entry length, KEY_EMPTY = unused
+  uint32_t* counts;              // LOAD_PAIRS: selected entries of each pair
+  uint32_t* flags;               // LOAD_FLAGS
+};
+bool load_index_host(const uint8_t* image, uint64_t nbytes, std::vector<uint64_t>& pos_off, std::string& err);
+cudaError_t launch_load_select(const LoadImg& L, cudaStream_t st);
+size_t load_list_bytes(uint32_t n);
+cudaError_t launch_load_list(const LoadImg& L, uint32_t slot, void* tmp, size_t tmp_bytes, uint32_t* sel,
+                             uint32_t* d_count, cudaStream_t st);
+cudaError_t launch_load_gather(const LoadImg& L, const uint32_t* sel, uint32_t K, uint32_t lo, uint32_t n, int rev,
+                               uint32_t len, uint64_t* signs, float* ent, cudaStream_t st);
 uint64_t launch_count();
 enum { FAM_PROBE = 0, FAM_DEDUP, FAM_GATHER, FAM_NAN, FAM_HOT, FAM_UPDATE, FAM_OTHER, FAM_WARM, FAM_WAIT, FAM_ROUTE, FAM_OWNER, FAM_COUNT };
 bool profiling();  // a kernel family is being timed: the backward then runs its kernels one after another

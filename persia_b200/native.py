@@ -13,7 +13,7 @@ PB_MAX_SLOTS = 128
 OPT_SGD, OPT_ADAGRAD, OPT_ADAGRAD_VW, OPT_ADAM = 0, 1, 2, 3
 
 PHASE_SEND, PHASE_SERVE, PHASE_FINISH, PHASE_ALL = 1, 2, 4, 7
-PB_OK, PB_ERR_INVALID, PB_ERR_CUDA, PB_ERR_STATE, PB_ERR_CAPACITY, PB_ERR_BATCH = 0, -1, -2, -3, -4, -5
+PB_OK, PB_ERR_INVALID, PB_ERR_CUDA, PB_ERR_STATE, PB_ERR_CAPACITY, PB_ERR_BATCH, PB_ERR_FORMAT = 0, -1, -2, -3, -4, -5, -6
 
 
 class PersiaB200Error(RuntimeError):
@@ -76,6 +76,14 @@ SYMBOLS = {
     "pb_table_dump_release": (_i32, [_vp]),
     "pb_table_dump_part": (_i32, [_vp, _u32, _u32, _vp, _u64, _vp, _vp, _vp]),
     "pb_dump_nodes": (_i32, [_vp, _vp, _u32, _u32, _u32, _vp, _vp]),
+    "pb_image_create": (_i32, [_i32, _u32, C.POINTER(_vp)]),
+    "pb_image_destroy": (_i32, [_vp]),
+    "pb_image_index": (_i32, [_vp, _vp, _u64, _u32, _u32, _u32, _u32, _vp, _u32, C.POINTER(_u32), _vp]),
+    "pb_image_window": (_i32, [_vp, _vp, _u64, _u32, _u64, _u32, _u64, _u32, _u32, _vp, _u32, C.POINTER(_u32),
+                               C.POINTER(_i32), _vp]),
+    "pb_image_insert": (_i32, [_vp, _vp, _u64, _u32, _u32, _i32, _vp]),
+    "pb_host_alloc": (_i32, [_u64, C.POINTER(_vp)]),
+    "pb_host_free": (_i32, [_vp]),
     "pb_add_prefix": (_i32, [_vp, _u32, C.POINTER(_u32), C.POINTER(_u64), _u32, _u32, _vp, _vp]),
     "pb_shard_of": (_i32, [_vp, _u32, _u32, _vp, _vp]),
     "pb_hash_stack": (_i32, [_vp, _u32, _u32, _u64, _vp, _vp]),

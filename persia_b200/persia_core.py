@@ -117,6 +117,7 @@ class _State:
         self.inc_lock = threading.Lock()
         self.gcfg_raw = None  # the global config dict itself (keys parse_global_config does not carry)
         self.emb_dump = None  # the latest background dump (checkpoint.BackgroundDumper)
+        self.emb_load = None  # the latest load (checkpoint.DeviceLoader)
 
     def global_config(self):
         """set_global_config's dict, else the PERSIA_GLOBAL_CONFIG yaml, else the reference's defaults."""
@@ -145,6 +146,20 @@ class _State:
         d = self.emb_dump
         if d is not None and d.running():
             d._thread.join()
+
+    def wait_load(self):
+        """Returns once no background load runs (its outcome stays in emb_load for wait_for_emb_loading)."""
+        if self.emb_load is not None:
+            self.emb_load.join()
+
+    def device_loader(self, src_dir):
+        """A checkpoint.DeviceLoader of src_dir into this replica's tables, under their groups' locks and fences."""
+        from . import checkpoint as CK
+
+        groups = {d: self.group(d) for d in sorted({s.dim for s in self.slots})}
+        return CK.DeviceLoader(src_dir, {d: g["shard"] for d, g in groups.items()}, self.replica_index or 0,
+                               max(1, self.replica_size or 1), locks={d: g["lock"] for d, g in groups.items()},
+                               fences={d: g["fence"] for d, g in groups.items() if g.get("fence") is not None})
 
     def incremental_on(self):
         c = self.global_config()
@@ -225,6 +240,8 @@ def reset():
     """Drop every table and configuration (tests).  A running background dump is stopped first."""
     if _S.emb_dump is not None:
         _S.emb_dump.stop()
+    if _S.emb_load is not None:
+        _S.emb_load.stop()
     if _S.loader is not None:
         _S.loader.stop()
     if _S.dumper is not None:
@@ -306,10 +323,8 @@ def _start_infer():
     if c["job_type"] != "Infer" or _S.loader is not None:
         return
     _S.ensure_config()
-    dims = sorted({s.dim for s in _S.slots})
     if c["embedding_checkpoint"]:
-        CK.load_shards(c["embedding_checkpoint"], {d: _S.group(d)["shard"] for d in dims}, _S.replica_index or 0,
-                       max(1, _S.replica_size or 1))
+        _S.device_loader(c["embedding_checkpoint"]).run()
     directory = os.path.join(c["incremental_dir"], f"s{_S.replica_index or 0}")
     _S.loader = INC.IncrementalLoader(directory, _apply_incremental)
     _S.loader.start()
@@ -1289,6 +1304,7 @@ class PersiaCommonContext:
 
     def clear_embeddings(self):
         _S.wait_dump()
+        _S.wait_load()
         for g in _S.all_groups():
             g["shard"].clear()
 
@@ -1301,6 +1317,7 @@ class PersiaCommonContext:
         if background is None:
             background = os.environ.get("PERSIA_B200_BACKGROUND_DUMP", "") == "1"
         _S.ensure_config()
+        _S.wait_load()
         if _S.emb_dump is not None and _S.emb_dump.running():
             raise RuntimeError("an embedding dump is already running: wait_for_emb_dumping() first")
         groups = _S.all_groups()
@@ -1318,15 +1335,28 @@ class PersiaCommonContext:
         ("Idle", 1.0), ("Dumping", fraction done) or ("Failed", message) of this replica's latest background dump."""
         return _S.emb_dump.status() if _S.emb_dump is not None else ("Idle", 1.0)
 
-    def load(self, src_dir):  # lib.rs:368-378 -> PS load (mod.rs:460-466)
-        from . import checkpoint as CK
-
+    def load(self, src_dir, background=None):  # lib.rs:368-378 -> PS load (mod.rs:460-466)
+        """Loads the checkpoint on the device (checkpoint.DeviceLoader: the tables end as load_shards leaves them).
+        background: True starts the load and returns (wait_for_emb_loading / load_status follow it, as the reference's
+        load_embedding_from_dir spawns one job per file, lib.rs:375-425); False loads now and raises what load_shards
+        raises; None: background when PERSIA_B200_BACKGROUND_LOAD=1."""
+        if background is None:
+            background = os.environ.get("PERSIA_B200_BACKGROUND_LOAD", "") == "1"
         _S.wait_dump()
+        _S.wait_load()
         _S.ensure_config()
         if _S.optimizer is None:
             raise RuntimeError("optimizer not registered: the entry layout (embedding ++ state) is unknown")
-        dims = sorted({s.dim for s in _S.slots})
-        CK.load_shards(src_dir, {d: _S.group(d)["shard"] for d in dims}, _S.replica_index or 0, max(1, _S.replica_size or 1))
+        _S.emb_load = _S.device_loader(src_dir)
+        if background:
+            _S.emb_load.start()
+        else:
+            _S.emb_load.run()
+
+    def load_status(self):
+        """The reference's server status of this replica's latest load (embedding_parameter_service/mod.rs:264-280):
+        ("Loading", fraction done), ("Idle", 1.0) or ("Failed", "Type: message")."""
+        return _S.emb_load.status() if _S.emb_load is not None else ("Idle", 1.0)
 
     def flush_incremental(self):
         """Not part of the reference surface (its manager flushes only on the threshold): takes every table's set of
@@ -1348,10 +1378,14 @@ class PersiaCommonContext:
         return _S.loader
 
     def wait_for_serving(self):
-        return None
+        """Blocks while a load runs (the reference's server is not ready_for_serving while it loads)."""
+        _S.wait_load()
 
     def wait_for_emb_loading(self):
-        return None
+        """Blocks until this replica's load is done; RuntimeError("emb dump FAILED for server {r}, due to ...") (the
+        reference's text, persia-core/src/rpc.rs:154-176) when it failed."""
+        if _S.emb_load is not None:
+            _S.emb_load.wait()
 
     def wait_for_emb_dumping(self):
         """Blocks until this replica's background dump is done (on replica 0: until the root marker is written, after
