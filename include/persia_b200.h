@@ -341,6 +341,12 @@ typedef struct {
   uint8_t sqrt_scaling[PB_MAX_SLOTS];
 } pb_slots_cfg;
 
+/* A context holds up to 2^24 id occurrences.  It allocates about 105 bytes per occurrence of max_occurrences and 4 per
+ * output row when created (1.8 GB at 2^24), then, on first use, max_occurrences / 33 x dim f32 of hot-sign staging (a
+ * training pb_forward) or 52 to 84 bytes per occurrence of raw scratch (pb_forward_raw).  A training pb_forward_raw
+ * also keeps n_occ x dim f32 of gradient staging, sized by its batch and grown when a larger batch or dim comes; growing
+ * synchronises the stream and frees the old buffer, so a raw step is capturable (and its graph replayable) only after a
+ * batch at least as large has run on the context. */
 int pb_ctx_create(int device, uint32_t max_occurrences, uint32_t max_out_rows, pb_ctx** out);
 int pb_ctx_destroy(pb_ctx* c);
 int pb_ctx_set_slots(pb_ctx* c, const pb_slots_cfg* cfg);

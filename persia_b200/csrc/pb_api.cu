@@ -1991,16 +1991,27 @@ static int ensure_raw(pb_ctx* c) {
   return PB_OK;
 }
 
-// pb_backward_raw's f32 staging buffer, max_occ x dim floats.  The training forward calls this, so the backward that
-// follows neither synchronises nor allocates (and can be captured without a warm-up call).
-static int ensure_raw_stage(pb_ctx* c, uint32_t dim, cudaStream_t st) {
-  const size_t cap = (size_t)c->max_occ * dim;
+// pb_backward_raw's f32 staging buffer: one row per distinct sign of the batch, so n_occ x dim floats bound it.  Sized
+// by the batch, not by max_occ: a context made at twice a batch's ids (persia_core) would otherwise ask for twice the
+// staging, 64 GB at 2^24 occurrences and dim 1024.  It grows when a larger batch or dim comes.  The training forward
+// calls this, so the backward that follows neither synchronises nor allocates; the first allocation neither synchronises
+// nor enqueues anything (see ensure_hot_stage).  Growing synchronises the stream and frees the old buffer: a forward
+// captured with more ids than any batch before it fails its capture, and a graph captured earlier must not be replayed
+// after a larger batch ran eagerly (warm up with the largest batch, as for vw_stage).
+static int ensure_raw_stage(pb_ctx* c, uint32_t n_occ, uint32_t dim, cudaStream_t st) {
+  const size_t cap = (size_t)(n_occ ? n_occ : 1) * dim;
   if (cap <= c->raw_stage_floats) return PB_OK;
-  PB_CUDA(cudaStreamSynchronize(st));  // the old buffer may still be read by enqueued work
-  if (c->raw_stage) cudaFree(c->raw_stage);
-  c->raw_stage = nullptr;
-  c->raw_stage_floats = 0;
-  PB_CUDA(cudaMalloc(&c->raw_stage, sizeof(float) * cap));
+  if (c->raw_stage) {  // the old buffer may still be read by enqueued work
+    PB_CUDA(cudaStreamSynchronize(st));
+    cudaFree(c->raw_stage);
+    c->raw_stage = nullptr;
+    c->raw_stage_floats = 0;
+  }
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  PB_CUDA(cudaThreadExchangeStreamCaptureMode(&mode));
+  const cudaError_t e = cudaMalloc(&c->raw_stage, sizeof(float) * cap);
+  cudaThreadExchangeStreamCaptureMode(&mode);  // the caller's mode again
+  PB_CUDA(e);
   c->raw_stage_floats = cap;
   return PB_OK;
 }
@@ -2022,7 +2033,7 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   if ((rc = call.begin(t, st, CALL_INDEX))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_raw(c))) return rc;
-  if (training && (rc = ensure_raw_stage(c, t->d.dim, st))) return rc;
+  if (training && (rc = ensure_raw_stage(c, n_occ, t->d.dim, st))) return rc;
   SlotsDev sl;
   if ((rc = raw_slots(c, n_occ, sl))) return rc;
   drop_raw_pending(c);  // the numbering below replaces the pending batch's
@@ -2080,7 +2091,7 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
   // Always staged, f32 without a loss scale included: the EW adds each row into zeros (mod.rs:780-798), which turns a -0
   // gradient into +0.  pb_update takes its gradients as given, like the PS (PS mod.rs:359-427), so the step does not.
   // The pending training forward allocated the buffer for this table's dim; only another table's larger dim allocates.
-  if ((rc = ensure_raw_stage(c, dim, st))) return rc;
+  if ((rc = ensure_raw_stage(c, c->n_occ, dim, st))) return rc;
   launch_raw_stage(d_grad, is_f16 != 0, c->raw.counts, dim, inv, do_scale != 0, c->raw_stage, st);
   launch_update_direct(t->d, t->op, t->hy, c->raw.target, c->raw_stage, c->n_occ, pair, st, c->raw.counts,
                        c->dev_tick, c->nan_tick, true);

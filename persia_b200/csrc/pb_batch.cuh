@@ -45,8 +45,10 @@ __device__ __forceinline__ ItemSlots block_item_slots(const BatchDev& b, bool he
   bool bitmap = false;
   uint32_t bm_off = 0;
   if (r.cls == 3 && hot_nwords && hot_nwords <= b.hot_words) {  // a few hundred per batch: one global atomic each
-    bm_off = atomicAdd(&b.cnt[BC_HOTW], hot_nwords);
-    bitmap = bm_off + hot_nwords <= b.hot_words;
+    // 64-bit: a 32-bit sum of the words asked for wraps past 2^32 and would hand out offsets again
+    const unsigned long long at = atomicAdd(hot_words_asked(b), (unsigned long long)hot_nwords);
+    bitmap = at + hot_nwords <= b.hot_words;
+    bm_off = bitmap ? (uint32_t)at : 0u;
   }
   if (r.cls >= 2 && !bitmap) seg = atomicAdd(&s_n[5], cnt);
   __syncthreads();

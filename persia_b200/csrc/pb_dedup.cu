@@ -254,7 +254,8 @@ __global__ void __launch_bounds__(256) k_clear_items(BatchDev b) {
 
 // a batch whose gradients never came leaves the bits its forward set in the hot-item bitmap pool
 __global__ void __launch_bounds__(256) k_clear_hot_bits(BatchDev b) {
-  const uint32_t used = min(b.cnt[BC_HOTW], b.hot_words);
+  const unsigned long long asked = *hot_words_asked(b);
+  const uint32_t used = asked < b.hot_words ? (uint32_t)asked : b.hot_words;
   for (uint32_t w = blockIdx.x * blockDim.x + threadIdx.x; w < used; w += gridDim.x * blockDim.x) b.hot_bits[w] = 0u;
 }
 

@@ -42,12 +42,15 @@ enum {
   BC_HOT,        // items of more
   BC_SEG,        // entries of seg_occ handed out
   BC_HUGE,       // hot items of more than PB_HUGE_MIN occurrences: listed from the END of `hot`, reduced first
-  BC_HOTW,       // words of the hot-item bitmap pool handed out
   BC_GIANT,      // hot items of more than PB_GIANT_MIN occurrences: the very first to be reduced
   BC_PEER = 8,
   BC_NEXT = 24,  // work cursors of the reducing kernels: [round] warm, [PB_MAX_SLOTS + round] hot
-  BC_COUNT = BC_NEXT + 2 * PB_MAX_SLOTS
+  // words of the hot-item bitmap pool asked for, a u64 over two words (8-byte aligned): every hot item adds its slot's
+  // bitmap words, also once the pool is used up, and a batch can ask for up to n / 33 x n / 32 words (2^38 at 2^24)
+  BC_HOTW = BC_NEXT + 2 * PB_MAX_SLOTS,
+  BC_COUNT = BC_HOTW + 2
 };
+static_assert(BC_HOTW % 2 == 0, "BC_HOTW is a u64");
 struct BatchDev {
   DCell* set;           // scratch set: region of slot s = [2*occ_off[s] + 2*s, +2*n_s + 1), then its reserved cell
   uint32_t* occ_set;    // [n] set cell of every occurrence
@@ -63,6 +66,9 @@ struct BatchDev {
   uint32_t* cnt;        // BC_* words
   uint32_t n;           // id occurrences of the batch
 };
+__device__ __forceinline__ unsigned long long* hot_words_asked(const BatchDev& b) {
+  return reinterpret_cast<unsigned long long*>(b.cnt + BC_HOTW);
+}
 
 // ---- the shard exchange (pb_shard.cu): one endpoint per rank, buffers in peer-mapped memory -----------------------
 // Every rank is an embedding worker for its own batches (requester) and parameter server `rank` (owner).  Rank r owns

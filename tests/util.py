@@ -149,19 +149,26 @@ def pool_model(rows, ids, row_off, batch, sqrt, dim=None, order="sample", per_ro
     sums the rows of its sample's signs into +0 in ascending occurrence order, skipping signs without a row; a slot with
     sqrt scaling then multiplies by f32(1 / f32(sqrt(max(n, 1)))); the result rounds to f16 (RNE).  One-id layouts
     (row_off None) give f16(0 + row).
-      rows     {sign: f32 [dim]}: what the table held at forward time
+      rows     {sign: f32 [dim]}: what the table held at forward time, or (signs u64 [n] ascending, f32 [n, >= dim])
+               for batches of millions of distinct signs
       ids      u64 [N] signs (prefixed), slot-major;  row_off  u32 [S*B+1] or None;  sqrt  per-slot bools or None
     Variants that the kernels must NOT match (tests use them to show their inputs discriminate):
       order    "reversed" / "sorted" (by sign) within each sample;  per_row  scale every row before adding it;
       factor   n (int array) -> f32 sqrt factor, instead of the double-rounded one.
     Returns f16 [S, B, dim]."""
     ids = np.asarray(ids, np.uint64)
-    keys = np.array(sorted(rows), np.uint64)
-    if dim is None:
-        dim = len(next(iter(rows.values())))
-    table = np.zeros((keys.size + 1, dim), np.float32)  # the last row stands for "no row" (never added)
-    for k, x in enumerate(keys):
-        table[k] = np.asarray(rows[int(x)], np.float32)[:dim]
+    if isinstance(rows, tuple):
+        keys, held = np.asarray(rows[0], np.uint64), np.asarray(rows[1], np.float32)
+        dim = held.shape[1] if dim is None else dim
+        table = np.zeros((keys.size + 1, dim), np.float32)  # the last row stands for "no row" (never added)
+        table[:-1] = held[:, :dim]
+    else:
+        keys = np.array(sorted(rows), np.uint64)
+        if dim is None:
+            dim = len(next(iter(rows.values())))
+        table = np.zeros((keys.size + 1, dim), np.float32)
+        for k, x in enumerate(keys):
+            table[k] = np.asarray(rows[int(x)], np.float32)[:dim]
     pos = np.searchsorted(keys, ids)
     hit = pos < keys.size
     hit[hit] = keys[pos[hit]] == ids[hit]
