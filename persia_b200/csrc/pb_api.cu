@@ -152,7 +152,9 @@ struct pb_ctx {
   size_t hot_stage_floats = 0;
   cudaStream_t side = nullptr;  // hot items run beside the main stream during pb_backward
   cudaStream_t side2 = nullptr;  // scratch-set clearing, then the warm items beside the cold ones
+  cudaStream_t side3 = nullptr;  // the short hot items' sums beside everything else (one round, large batches)
   cudaEvent_t ev_fork = nullptr, ev_nan = nullptr, ev_join = nullptr, ev_join2 = nullptr;
+  cudaEvent_t ev_short = nullptr;  // `side3` staged the short hot items' sums (k_step_hot on `side` waits for it)
   // raw slot (pb_forward_raw / pb_backward_raw): allocated on first use
   uint32_t* occ_cell = nullptr;
   RawWork raw{};
@@ -1506,10 +1508,12 @@ int pb_ctx_create(int device, uint32_t max_occurrences, uint32_t max_out_rows, p
   }
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->side2, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->side3, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_join2, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_nan, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_short, cudaEventDisableTiming);
   if (e != cudaSuccess) {
     pb_ctx_destroy(c);
     return fail(PB_ERR_CUDA, std::string("pb_ctx_create: ") + cudaGetErrorString(e));
@@ -1532,10 +1536,12 @@ int pb_ctx_destroy(pb_ctx* c) {
     if (p) cudaFree(p);
   if (c->side) cudaStreamDestroy(c->side);
   if (c->side2) cudaStreamDestroy(c->side2);
+  if (c->side3) cudaStreamDestroy(c->side3);
   if (c->ev_join2) cudaEventDestroy(c->ev_join2);
   if (c->ev_fork) cudaEventDestroy(c->ev_fork);
   if (c->ev_nan) cudaEventDestroy(c->ev_nan);
   if (c->ev_join) cudaEventDestroy(c->ev_join);
+  if (c->ev_short) cudaEventDestroy(c->ev_short);
   delete c;
   return PB_OK;
 }
@@ -1687,22 +1693,29 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
   ReduceArgs a = reduce_args(c);
   a.vw_stage = vw;
   a.hot_stage = c->hot_stage;
+  a.short_max = hot_short_max(c->batch);
   auto set_round = [&](uint32_t r) {
     a.round = r;
     std::memset(a.round_mask, 0, sizeof(a.round_mask));
     for (uint32_t s = 0; s < S; ++s)
       if (c->round_of[s] == r) a.round_mask[s >> 5] |= 1u << (s & 31);
   };
-  // One round (no shared feature groups, the usual case): the hot items' sums need no NaN mark, so their reduce — the
-  // longest kernel of the step — starts on `side` at once, beside the NaN scan; once the marks are known the hot rows
-  // are stepped there, and the cold and warm items are reduced and stepped on `st` and `side2`.  Several rounds (the
-  // items of a round are distinct rows, whatever their list), or a kernel family being timed: everything on `st`,
-  // round after round.
+  // One round (no shared feature groups, the usual case): the hot items' sums need no NaN mark, so their reduces — the
+  // longest kernel of the step on `side`, and at large batches the light one for the short items on `side3` — start at
+  // once, beside the NaN scan; once the marks and the short sums are known the hot rows are stepped on `side`,
+  // and the cold and warm items are reduced and stepped on `st` and `side2`.  Several rounds (the items of a round are
+  // distinct rows, whatever their list), or a kernel family being timed: everything on `st`, round after round.
   const bool beside = c->n_rounds == 1 && !profiling();
   if ((rc = fork_side(c, st))) return rc;
   if (beside) {
     set_round(0);
     launch_reduce_hot(t->d, sl, gr, is_f16 != 0, a, c->side);
+    if (a.short_max) {
+      PB_CUDA(cudaStreamWaitEvent(c->side3, c->ev_fork, 0));
+      launch_reduce_hot_short(t->d, sl, gr, is_f16 != 0, a, c->side3);
+      PB_CUDA(cudaEventRecord(c->ev_short, c->side3));
+      PB_CUDA(cudaStreamWaitEvent(c->side, c->ev_short, 0));  // (joins `side3` back; the reduce queued before does not wait)
+    }
   }
   const bool mark = t->inc.cells != nullptr;  // the mark reads the scratch set and empties it after the steps
   if (c->set_dirty && !mark) {
@@ -1715,7 +1728,10 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
   if ((rc = fork_after_nan(c, st))) return rc;
   for (uint32_t r = 0; r < c->n_rounds; ++r) {
     set_round(r);
-    if (!beside) launch_reduce_hot(t->d, sl, gr, is_f16 != 0, a, st);
+    if (!beside) {
+      launch_reduce_hot(t->d, sl, gr, is_f16 != 0, a, st);
+      launch_reduce_hot_short(t->d, sl, gr, is_f16 != 0, a, st);
+    }
     launch_step_hot(t->d, t->op, t->hy, sl, gr, a, beside ? c->side : st);
     launch_reduce_items(t->d, t->op, t->hy, sl, gr, is_f16 != 0, a, st, beside ? c->side2 : st, false);
   }

@@ -133,6 +133,7 @@ struct ReduceArgs {
   float* vw_stage;             // Adagrad vectorwise: one reduced gradient per item
   float* hot_stage;            // [hot_cap][dim]: the sum of every hot item at its entry of b.hot (k_reduce_hot -> k_step_hot)
   uint32_t batch, round, quiet_miss;
+  uint32_t short_max;          // hot items of up to this many occurrences are k_reduce_hot_short's (0: none)
   uint32_t round_mask[PB_MAX_SLOTS / 32];  // slots stepped by this launch (slots of one feature group take turns)
   XchgDev x;                   // sharded: the reduced gradient is stored into the owner's receive area instead
 };
@@ -213,6 +214,11 @@ void launch_reduce_items(const TableDev& t, const OptimDev& op, const HyperDev& 
 // step of their rows (after the NaN scan and the Adam power advance)
 void launch_reduce_hot(const TableDev& t, const SlotsDev& sl, const GradsDev& gr, bool f16, const ReduceArgs& a,
                        cudaStream_t st, bool send = false);
+// local path: the sums of the hot items of up to a.short_max occurrences (k_reduce_hot_short), staged as
+// launch_reduce_hot stages the others'; a.short_max = hot_short_max(batch), 0 when k_reduce_hot takes every hot item
+uint32_t hot_short_max(uint32_t batch);
+void launch_reduce_hot_short(const TableDev& t, const SlotsDev& sl, const GradsDev& gr, bool f16, const ReduceArgs& a,
+                             cudaStream_t st);
 void launch_step_hot(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl, const GradsDev& gr,
                      const ReduceArgs& a, cudaStream_t st);
 // diagnostic (pb_hot_geometry): the geometry launch_reduce_hot gives k_reduce_hot

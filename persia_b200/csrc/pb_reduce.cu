@@ -14,14 +14,18 @@
 //                   whole chip's worth of groups resident.
 //   k_reduce_warm   a lane group per item: the group sorts the item's <= 32 occurrences in shared memory (rank by
 //                   counting), then adds them in order.
-//   k_reduce_hot    persistent; one 256-thread CTA per item at a time.  The occurrences are put in order by a bitmap
-//                   over the slot's occurrence range (a counting sort that costs B/32 words), one window of HOT_WIN
+//   k_reduce_hot    hot items (those above a.short_max occurrences), persistent; one 256-thread CTA per item at a time.
+//                   The occurrences are put in order by a bitmap over the slot's occurrence range (a counting sort that costs B/32 words), one window of HOT_WIN
 //                   occurrences after another.  Producer warps load the gradient rows with 16-byte (or element-wise)
 //                   loads, prepare them (f16 -> f32, clamp, scale) and store them into a shared-memory ring of chunks
 //                   guarded by mbarriers; chain warps add the chunks' rows in order — a dependent FADD chain fed from
 //                   shared memory, which is the floor for a strictly sequential sum — and store the sum to a staging
 //                   buffer.  Rows wider than HOT_COLS columns take several passes.  Details above the kernel.  It reads
 //                   no NaN mark, so the backward runs it beside the NaN scan.
+//   k_reduce_hot_short  local path, batches of SHORT_BATCH samples or more: the hot items of up to SHORT_MAX
+//                   occurrences, a warp per item; orders them from the same bitmap and adds them in the same order into
+//                   the same staging buffer; light enough to share SMs with k_reduce_hot, the NaN scan and the cold
+//                   and warm reduces.
 //   k_step_hot      a lane group per hot item, after the NaN scan: the NaN rule, then the optimizer step with the
 //                   staged sum.
 #include "pb_optim.cuh"
@@ -113,41 +117,41 @@ __device__ __forceinline__ void add_prepared(float (&acc)[N], const float (&g)[N
   }
 }
 
+// occurrences pos(k..k+n-1), n <= M, added to acc in order, elements [e0, e0+N): all loads are issued before the first add
+template <int M, int N, bool F16, typename POS>
+__device__ __forceinline__ void reduce_batch(float (&acc)[N], const ItemSrc& s, const ReduceArgs& a, const TableDev& t,
+                                             uint32_t k, uint32_t n, uint32_t e0, POS pos) {
+  uint32_t orow[M];
+  float g[M][N];
+#pragma unroll
+  for (int u = 0; u < M; ++u) orow[u] = (uint32_t)u < n ? occ_out_row(a, pos(k + u)) : 0u;
+#pragma unroll
+  for (int u = 0; u < M; ++u)
+    if ((uint32_t)u < n) load_grad_elems<N, F16>(g[u], s.gbase, (size_t)(orow[u] - s.slot_row0) * t.dim, e0);
+#pragma unroll
+  for (int u = 0; u < M; ++u)
+    if ((uint32_t)u < n) add_prepared<N>(acc, g[u], grad_prep(s, a, orow[u]), s.plain);
+}
+
 // sum of the gradients of occurrences pos(0..cnt-1) (already in ascending order), elements [e0, e0+N).
-// Batches of 8 / 4 occurrences have all their loads issued together; the adds stay sequential.
-template <int N, bool F16, typename POS>
+// Batches of U occurrences have all their loads issued together; the adds stay sequential.  The rest: U > 8, one
+// batch of what is left; otherwise batches of 4, then one by one.
+template <int N, bool F16, int U = 8, typename POS>
 __device__ __forceinline__ void reduce_sorted(float (&acc)[N], const ItemSrc& s, const ReduceArgs& a, const TableDev& t,
                                               uint32_t cnt, uint32_t e0, POS pos) {
 #pragma unroll
   for (int q = 0; q < N; ++q) acc[q] = 0.0f;
   uint32_t k = 0;
-  for (; k + 8 <= cnt; k += 8) {
-    uint32_t orow[8];
-    float g[8][N];
-#pragma unroll
-    for (int u = 0; u < 8; ++u) orow[u] = occ_out_row(a, pos(k + u));
-#pragma unroll
-    for (int u = 0; u < 8; ++u) load_grad_elems<N, F16>(g[u], s.gbase, (size_t)(orow[u] - s.slot_row0) * t.dim, e0);
-#pragma unroll
-    for (int u = 0; u < 8; ++u) add_prepared<N>(acc, g[u], grad_prep(s, a, orow[u]), s.plain);
+  for (; k + U <= cnt; k += U) reduce_batch<U, N, F16>(acc, s, a, t, k, U, e0, pos);
+  if (U > 8) {
+    if (k < cnt) reduce_batch<U, N, F16>(acc, s, a, t, k, cnt - k, e0, pos);
+    return;
   }
   if (k + 4 <= cnt) {
-    uint32_t orow[4];
-    float g[4][N];
-#pragma unroll
-    for (int u = 0; u < 4; ++u) orow[u] = occ_out_row(a, pos(k + u));
-#pragma unroll
-    for (int u = 0; u < 4; ++u) load_grad_elems<N, F16>(g[u], s.gbase, (size_t)(orow[u] - s.slot_row0) * t.dim, e0);
-#pragma unroll
-    for (int u = 0; u < 4; ++u) add_prepared<N>(acc, g[u], grad_prep(s, a, orow[u]), s.plain);
+    reduce_batch<4, N, F16>(acc, s, a, t, k, 4, e0, pos);
     k += 4;
   }
-  for (; k < cnt; ++k) {
-    const uint32_t orow = occ_out_row(a, pos(k));
-    float g[N];
-    load_grad_elems<N, F16>(g, s.gbase, (size_t)(orow - s.slot_row0) * t.dim, e0);
-    add_prepared<N>(acc, g, grad_prep(s, a, orow), s.plain);
-  }
+  for (; k < cnt; ++k) reduce_batch<1, N, F16>(acc, s, a, t, k, 1, e0, pos);
 }
 
 // sharded requester: where the reduced gradient of the item with target = owner * cap + k goes (the owner's receive
@@ -367,6 +371,13 @@ __global__ void __launch_bounds__(256) k_reduce_cold(TableDev t, OptimDev op, Hy
 // by the instruction stream (~40 cycles per row).
 // ------------------------------------------------------------------------------------------------
 constexpr uint32_t HOT_WIN = 8192;   // samples per bitmap window
+// Hot items of up to SHORT_MAX occurrences go to k_reduce_hot_short when a slot holds at least SHORT_BATCH samples: a
+// warp sums one in at most eight load round trips, which the longest chains of such batches outlast (measured: a
+// 4,080-row chain at batch 8192).  At smaller batches the chains are shorter than the light reduce (2,099 rows at 4096:
+// the step measured 8 us slower with it), so k_reduce_hot takes every hot item there.
+constexpr uint32_t SHORT_MAX = 128;
+constexpr uint32_t SHORT_BATCH = 8192;
+uint32_t hot_short_max(uint32_t batch) { return batch >= SHORT_BATCH ? SHORT_MAX : 0u; }
 constexpr uint32_t HOT_WORDS = HOT_WIN / 32;
 constexpr uint32_t HOT_THREADS = 256;
 constexpr uint32_t HOT_WARPS = HOT_THREADS / 32;
@@ -619,7 +630,12 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Slots
   bool failed = false;
   for (;;) {
     __syncthreads();  // s_item, bitmap and sorted are free again
-    if (tid == 0) s_item = atomicAdd(next, 1u);
+    if (tid == 0) {  // the next item, past those k_reduce_hot_short sums
+      uint32_t h;
+      do h = atomicAdd(next, 1u);
+      while (h >= n_giant + n_huge && h < n_hot && a.b.hot[h - n_giant - n_huge].z <= a.short_max);
+      s_item = h;
+    }
     __syncthreads();
     const uint32_t h = s_item;
     if (h >= n_hot) break;
@@ -793,6 +809,90 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Slots
   if (failed && lane == 0) atomicAdd(&t.counters[CTR_ERR], 1u);
 }
 
+// ---- short hot items (PB_WARM_MAX + 1 .. a.short_max occurrences, among entries [0, cnt[BC_HOT]) of `hot`): one warp
+// per item.  A whole-SM k_reduce_hot block spends most of a short item's time ordering it and on one producer round
+// trip before its chain starts, while the SM could serve the NaN scan and the cold and warm reduces.  Here the warp
+// expands the item's bitmap words (eight per lane in flight) into the ascending list of its occurrences in shared
+// memory, or ranks its occurrence list by counting when the bitmap pool ran out, then each lane sums its columns in
+// that order with U rows' loads in flight: the additions of k_reduce_hot, one row after another from +0 (its zero
+// padding rows add nothing).  Same skip, clear and output rules as k_reduce_hot.
+constexpr uint32_t SHORT_WARPS = 4;  // warps (items) per block; four blocks per SM hold at most 128 registers per thread
+template <int VEC, bool F16>
+__global__ void __launch_bounds__(SHORT_WARPS * 32, 4) k_reduce_hot_short(TableDev t, SlotsDev sl, GradsDev gr, ReduceArgs a) {
+  __shared__ uint32_t dead[PB_MAX_SLOTS / 32];
+  __shared__ uint32_t lists[SHORT_WARPS][2 * SHORT_MAX];  // per warp: unsorted (list mode) | ascending occurrences
+  const uint32_t n_short = a.b.cnt[BC_HOT];
+  if (blockIdx.x * SHORT_WARPS >= n_short) return;  // whole block
+  build_dead_mask(dead, gr, a, sl.n_slots, false);  // (the sums read no NaN mark, like k_reduce_hot's)
+  const uint32_t lane = threadIdx.x & 31;
+  uint32_t* raw = lists[threadIdx.x >> 5];
+  uint32_t* srt = raw + SHORT_MAX;
+  const uint32_t nvec = t.dim / VEC;
+  constexpr int U = 16;  // rows whose loads a lane has in flight together
+  for (uint32_t h = blockIdx.x * SHORT_WARPS + (threadIdx.x >> 5); h < n_short; h += gridDim.x * SHORT_WARPS) {
+    __syncwarp();  // the previous item's list is no longer read
+    const uint4 d = a.b.hot[h];
+    const uint32_t row = d.x, cnt = d.z, slot = d.w;
+    if (cnt > a.short_max) continue;  // k_reduce_hot's
+    const bool bm_mode = d.y >> 31;
+    const uint32_t base = d.y & 0x7FFFFFFFu;  // first bitmap word of the item, or first entry of its occurrence list
+    const uint32_t lo = sl.occ_off[slot], n_words = (sl.occ_off[slot + 1] - lo + 31u) / 32u;
+    if (slot_dead(dead, slot) || row >= t.capacity) {  // (k_step_hot counts the rowless items of applied slots)
+      // the item's bits must still go back to zero for the next batch, unless a later round reads them
+      const bool other_round = !((a.round_mask[slot >> 5] >> (slot & 31)) & 1u);  // (an earlier one zeroed them already)
+      if (bm_mode && !other_round)
+        for (uint32_t w = lane; w < n_words; w += 32u) a.b.hot_bits[base + w] = 0u;
+      continue;
+    }
+    // ---- the item's occurrences, ascending
+    if (bm_mode) {
+      uint32_t* gw = a.b.hot_bits + base;
+      // its cnt bits are the only ones set in its words: the words past the cnt-th bit are zero already
+      for (uint32_t w0 = 0, found = 0; w0 < n_words && found < cnt; w0 += 32u * 8u) {
+        const uint32_t w1 = w0 + lane * 8u;  // this lane's eight consecutive words
+        uint32_t m[8], n = 0;
+#pragma unroll
+        for (uint32_t j = 0; j < 8; ++j) m[j] = w1 + j < n_words ? gw[w1 + j] : 0u;
+#pragma unroll
+        for (uint32_t j = 0; j < 8; ++j) {
+          if (m[j]) gw[w1 + j] = 0u;  // all zero again for the next batch
+          n += __popc(m[j]);
+        }
+        uint32_t inc = n;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o);
+          if (lane >= (uint32_t)o) inc += y;
+        }
+        uint32_t at = found + inc - n;
+#pragma unroll
+        for (uint32_t j = 0; j < 8; ++j)
+          for (uint32_t mm = m[j]; mm; mm &= mm - 1u, ++at)
+            if (at < cnt) srt[at] = lo + (w1 + j) * 32u + __ffs(mm) - 1u;
+        found += __shfl_sync(0xffffffffu, inc, 31);
+      }
+    } else {
+      for (uint32_t l = lane; l < cnt; l += 32u) raw[l] = a.b.seg_occ[base + l];
+      __syncwarp();
+      for (uint32_t l = lane; l < cnt; l += 32u) {  // occurrences are distinct numbers
+        const uint32_t p = raw[l];
+        uint32_t r = 0;
+        for (uint32_t q = 0; q < cnt; ++q) r += raw[q] < p;
+        srt[r] = p;
+      }
+    }
+    __syncwarp();
+    // ---- the sum, VEC columns per lane at a time
+    const ItemSrc src = item_src(sl, gr, a, slot);
+    float* out = a.hot_stage + (size_t)h * t.dim;
+    for (uint32_t c = lane; c < nvec; c += 32u) {
+      float acc[VEC];
+      reduce_sorted<VEC, F16, U>(acc, src, a, t, cnt, c * VEC, [srt](uint32_t k) { return srt[k]; });
+      store_vec<VEC>(out + c * VEC, acc);
+    }
+  }
+}
+
 // ---- hot items, the step (local path): a lane group per item takes the sum k_reduce_hot staged at its entry of `hot`,
 // applies the whole dead mask, NaN marks included, and steps the row.  The step depends on the element index and the
 // summed value only, so the rows come out as they would from a step fused into the reduce.
@@ -941,6 +1041,23 @@ void launch_reduce_hot(const TableDev& t, const SlotsDev& sl, const GradsDev& gr
   }
   if (hot_epl(t.dim) == 2u) { PB_H(2) } else { PB_H(4) }
 #undef PB_H
+}
+
+void launch_reduce_hot_short(const TableDev& t, const SlotsDev& sl, const GradsDev& gr, bool f16, const ReduceArgs& a,
+                             cudaStream_t st) {
+  if (!a.b.n || !a.short_max) return;
+  // at most this many short items exist; blocks past their number return at once, and warps stride over the list
+  uint32_t grid = cdiv(cdiv(a.b.n, PB_WARM_MAX + 1), SHORT_WARPS);
+  if (grid > PB_NUM_SMS * 8u) grid = PB_NUM_SMS * 8u;
+#define PB_S(V, F) PB_LAUNCH_F(FAM_HOT, (k_reduce_hot_short<V, F>), grid, SHORT_WARPS * 32, 0, st, t, sl, gr, a)
+  if (t.dim % 4u == 0) {
+    if (f16) PB_S(4, true);
+    else PB_S(4, false);
+  } else {
+    if (f16) PB_S(1, true);
+    else PB_S(1, false);
+  }
+#undef PB_S
 }
 
 void launch_step_hot(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl, const GradsDev& gr,

@@ -2,11 +2,12 @@
 
 Runs bench.py's metric-leg workload (table, batches and gradients built as run_leg builds them), kernel by kernel, in
 two phases of --steps steps each:
-  beside  the usual stream layout: k_reduce_hot starts on the context's side stream with the backward, beside
-          k_nan_scan; k_step_hot follows the scan there
+  beside  the usual stream layout: k_reduce_hot starts on the context's side stream with the backward and, at 8192
+          samples per slot or more, k_reduce_hot_short (the items of up to 128 occurrences) on its third one, both
+          beside k_nan_scan; k_step_hot follows the scan and the short sums on the first
   alone   a kernel family being timed (pb_profile_enable): the backward runs its kernels one after another on one stream
-and prints, per phase, the mean duration of k_nan_scan, k_reduce_hot and k_step_hot from the CUDA kernel records, and in
-how many steps k_reduce_hot started before k_nan_scan ended.  The chrome traces go to --out.
+and prints, per phase, the mean duration of k_nan_scan, k_reduce_hot, k_reduce_hot_short and k_step_hot from the CUDA
+kernel records, and in how many steps k_reduce_hot started before k_nan_scan ended.  The chrome traces go to --out.
   python scripts/hot_overlap_profile.py [--steps 20] [--out DIR] [bench.py's workload flags: --rows --dim --batch ...]"""
 import argparse
 import json
@@ -24,7 +25,7 @@ from persia_b200 import native as N
 from persia_b200 import shard as SH
 from persia_b200 import workload as W
 
-KERNELS = ("k_nan_scan", "k_reduce_hot", "k_step_hot")
+KERNELS = ("k_nan_scan", "k_reduce_hot_short", "k_reduce_hot", "k_step_hot")  # (a name matches its first entry)
 
 
 def kernel_records(path):
