@@ -40,6 +40,11 @@ __device__ __forceinline__ void store_vec(float* p, const float (&v)[VEC]) {
   else p[0] = v[0];
 }
 
+// the lanes of this thread's group of G lanes (G a power of two <= 32) within its warp
+__device__ __forceinline__ uint32_t group_mask(uint32_t G) {
+  const uint32_t wl = threadIdx.x & 31u;
+  return (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (wl / G * G));
+}
 
 // lanes per row and floats per lane for a given embedding dim
 static inline void vec_group(uint32_t dim, int& vec, int& G) {

@@ -156,22 +156,48 @@ struct RowElems {
   }
 };
 
-__device__ __forceinline__ StepCtx step_ctx(const float* row, const TableDev& t, const OptimDev& op, const GradsDev& gr,
-                                            uint32_t slot) {
+// pair: the (beta1^t, beta2^t) of the row's feature group, read only when the optimizer is Adam
+__device__ __forceinline__ StepCtx step_ctx(const OptimDev& op, float vw_state, const float* pair) {
   StepCtx sc;
-  sc.vw_state = 0.0f;
+  sc.vw_state = vw_state;
   sc.r1 = sc.r2 = 0.0f;
-  if (op.kind == PB_OPT_ADAGRAD_VW) sc.vw_state = row[t.dim];
   if (op.kind == PB_OPT_ADAM) {
-    const float* pw = gr.adam_pow + 2u * gr.pow_idx[slot];
-    sc.r1 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[0]));
-    sc.r2 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[1]));
+    sc.r1 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pair[0]));
+    sc.r2 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pair[1]));
   }
   return sc;
 }
+__device__ __forceinline__ StepCtx step_ctx(const float* row, const TableDev& t, const OptimDev& op, const GradsDev& gr,
+                                            uint32_t slot) {
+  return step_ctx(op, op.kind == PB_OPT_ADAGRAD_VW ? row[t.dim] : 0.0f, gr.adam_pow + 2u * gr.pow_idx[slot]);
+}
+
+// a sign without a row in the table; lane 0 counts it when `count` (gradient_id_miss_count, PS mod.rs:401-403)
+__device__ __forceinline__ bool row_missing(uint32_t row, const TableDev& t, uint32_t lane, bool count) {
+  if (row < t.capacity) return false;
+  if (lane == 0 && count) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);
+  return true;
+}
+
+// one optimizer step on the lane's columns of a resident row, VEC at a time (lane < G lanes per row): the row's
+// elements are loaded first, so that they are in flight while grad(e0, g) fills g with the gradient of columns
+// [e0, e0 + VEC)
+template <int KIND, int VEC, typename GRAD>
+__device__ __forceinline__ void step_row(float* prow, const TableDev& t, const OptimDev& op, const HyperDev& hy,
+                                         const StepCtx& sc, uint32_t lane, uint32_t G, GRAD grad) {
+  const uint32_t nvec = t.dim / VEC;
+  for (uint32_t c = lane; c < nvec; c += G) {
+    RowElems<KIND, VEC> rc;
+    float g[VEC];
+    rc.load(prow, c * VEC, t, op);
+    grad(c * VEC, g);
+    rc.step(c * VEC, g, t, op, hy, sc);
+    rc.store(prow, c * VEC, t, op);
+  }
+}
 
 // ndarray 0.15 unrolled_dot order (8 partial sums, pairwise fold, scalar tail), serial per row: one lane calls it on
-// the reduced gradient staged in memory.  state = state*mom + dot(g,g)/dim (optim.rs:280-283).
+// the reduced gradient in memory
 static __device__ float vw_dot(const float* g, uint32_t n) {
   float p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   uint32_t i = 0;
@@ -185,6 +211,15 @@ static __device__ float vw_dot(const float* g, uint32_t n) {
   sum = __fadd_rn(sum, __fadd_rn(p[3], p[7]));
   for (; i < n; ++i) sum = __fadd_rn(sum, __fmul_rn(g[i], g[i]));
   return sum;
+}
+
+// Adagrad vectorwise, after the group (gmask) stepped the row with the old state sc.vw_state and g, the reduced
+// gradient, is in memory: state = state*mom + dot(g,g)/dim (optim.rs:280-283)
+__device__ __forceinline__ void vw_state_step(float* prow, const float* g, const TableDev& t, const OptimDev& op,
+                                              const StepCtx& sc, uint32_t lane, uint32_t gmask) {
+  __syncwarp(gmask);  // every lane of the group has read the old state, and g is visible to lane 0
+  if (lane == 0) prow[t.dim] = __fadd_rn(__fmul_rn(sc.vw_state, op.mom), __fdiv_rn(vw_dot(g, t.dim), (float)t.dim));
+  __syncwarp(gmask);  // the new state is written before any lane of the group reads it again
 }
 
 // one gradient value as the EW prepares it before summing: f16 -> f32 with +-inf clamped to +-65504

@@ -71,6 +71,13 @@ __device__ __forceinline__ GradPrep grad_prep(const ItemSrc& s, const ReduceArgs
   return p;
 }
 
+// +-inf -> +-65504 (persia-common lib.rs:163-180), two halves per instruction; finite halves are inside already.  A
+// caller that clamps several values may build lim = f16_lim2() once.
+__device__ __forceinline__ __half2 f16_lim2() { return __floats2half2_rn(65504.0f, 65504.0f); }
+__device__ __forceinline__ __half2 clamp_h2(__half2 v, __half2 lim = f16_lim2()) {
+  return __hmin2(__hmax2(v, __hneg2(lim)), lim);
+}
+
 // N consecutive gradient elements of one output row starting at element e0, converted to f32 and clamped
 template <int N, bool F16>
 __device__ __forceinline__ void load_grad_elems(float (&g)[N], const void* gbase, size_t row_elem0, uint32_t e0) {
@@ -80,10 +87,8 @@ __device__ __forceinline__ void load_grad_elems(float (&g)[N], const void* gbase
 #pragma unroll
       for (int q = 0; q < N / 4; ++q) {
         uint2 raw = *reinterpret_cast<const uint2*>(gp + 4 * q);
-        // +-inf -> +-65504 (persia-common lib.rs:163-180), two halves per instruction; finite halves are inside already
-        const __half2 lim = __floats2half2_rn(65504.0f, 65504.0f);
-        __half2 h0 = __hmin2(__hmax2(*reinterpret_cast<__half2*>(&raw.x), __hneg2(lim)), lim);
-        __half2 h1 = __hmin2(__hmax2(*reinterpret_cast<__half2*>(&raw.y), __hneg2(lim)), lim);
+        const __half2 lim = f16_lim2();
+        __half2 h0 = clamp_h2(*reinterpret_cast<__half2*>(&raw.x), lim), h1 = clamp_h2(*reinterpret_cast<__half2*>(&raw.y), lim);
         float2 x = __half22float2(h0), y = __half22float2(h1);
         g[4 * q] = x.x; g[4 * q + 1] = x.y; g[4 * q + 2] = y.x; g[4 * q + 3] = y.y;
       }
@@ -187,6 +192,26 @@ __device__ __forceinline__ uint32_t hot_entry(const BatchDev& b, uint32_t h, uin
                      : (h < n_giant + n_huge ? b.hot_cap - 1u - b.giant_cap - (h - n_giant) : h - n_giant - n_huge);
 }
 
+// a skipped hot item of `slot`, whose occurrences are [lo, hi) (bitmap words from base when bm_mode), thread i of n: its
+// bits must still go back to zero for the next batch, unless a later round reads them (an earlier one zeroed them already)
+__device__ __forceinline__ void release_hot_bits(const ReduceArgs& a, uint32_t slot, bool bm_mode, uint32_t base,
+                                                 uint32_t lo, uint32_t hi, uint32_t i, uint32_t n) {
+  const bool other_round = !((a.round_mask[slot >> 5] >> (slot & 31)) & 1u);
+  if (bm_mode && !other_round)
+    for (uint32_t w = i; w < (hi - lo + 31u) / 32u; w += n) a.b.hot_bits[base + w] = 0u;
+}
+
+// an item's cnt occurrences raw[0..cnt) (distinct numbers) in ascending order into srt, ranked by counting; lane of
+// n_lanes
+__device__ __forceinline__ void rank_sort(const uint32_t* raw, uint32_t* srt, uint32_t cnt, uint32_t lane, uint32_t n_lanes) {
+  for (uint32_t l = lane; l < cnt; l += n_lanes) {
+    const uint32_t p = raw[l];
+    uint32_t r = 0;
+    for (uint32_t m = 0; m < cnt; ++m) r += raw[m] < p;
+    srt[r] = p;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // cold and warm items
 // ------------------------------------------------------------------------------------------------
@@ -212,26 +237,13 @@ __device__ __forceinline__ void step_item(const TableDev& t, const OptimDev& op,
                                           const GradsDev& gr, const ReduceArgs& a, uint32_t row, uint32_t slot,
                                           uint32_t cnt, uint32_t lane, uint32_t G, uint32_t gmask, float* stage, POS pos) {
   float* prow = t.rows + (size_t)row * t.stride;
-  const uint32_t nvec = t.dim / VEC;
   const ItemSrc src = item_src(sl, gr, a, slot);
   const StepCtx sc = step_ctx(prow, t, op, gr, slot);
-  for (uint32_t c = lane; c < nvec; c += G) {
-    RowElems<KIND, VEC> rc;
-    rc.load(prow, c * VEC, t, op);  // in flight while the gradients are fetched and summed
-    float acc[VEC];
-    reduce_sorted<VEC, F16>(acc, src, a, t, cnt, c * VEC, pos);
-    if (KIND == PB_OPT_ADAGRAD_VW) store_vec<VEC>(stage + c * VEC, acc);
-    rc.step(c * VEC, acc, t, op, hy, sc);
-    rc.store(prow, c * VEC, t, op);
-  }
-  if (KIND == PB_OPT_ADAGRAD_VW) {  // state = state*mom + dot(g,g)/dim (optim.rs:280-283)
-    __syncwarp(gmask);              // the staged gradient of every lane of the group is visible to lane 0
-    if (lane == 0) {
-      float gs = __fdiv_rn(vw_dot(stage, t.dim), (float)t.dim);
-      prow[t.dim] = __fadd_rn(__fmul_rn(sc.vw_state, op.mom), gs);
-    }
-    __syncwarp(gmask);
-  }
+  step_row<KIND, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&acc)[VEC]) {
+    reduce_sorted<VEC, F16>(acc, src, a, t, cnt, e0, pos);
+    if (KIND == PB_OPT_ADAGRAD_VW) store_vec<VEC>(stage + e0, acc);
+  });
+  if (KIND == PB_OPT_ADAGRAD_VW) vw_state_step(prow, stage, t, op, sc, lane, gmask);
 }
 
 // ---- warm items: one lane group per item; the group sorts the item's <= 32 occurrences (rank by counting), then adds
@@ -244,8 +256,8 @@ __global__ void __launch_bounds__(256, 3) k_reduce_warm(TableDev t, OptimDev op,
   const uint32_t n_warm = a.b.cnt[BC_WARM], n_cold = a.b.cnt[BC_COLD];
   if (blockIdx.x * (blockDim.x / G) >= n_warm) return;  // whole block
   build_dead_mask(dead, gr, a, sl.n_slots);
-  const uint32_t lane = threadIdx.x % G, grp = threadIdx.x / G, wl = threadIdx.x & 31;
-  const uint32_t gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (wl / G * G));
+  const uint32_t lane = threadIdx.x % G, grp = threadIdx.x / G;
+  const uint32_t gmask = group_mask(G);
   uint32_t* raw = sortbuf[grp];
   uint32_t* srt = raw + PB_WARM_MAX;
   // the grid holds a few blocks per SM; a group strides over the list (its length lives on the device)
@@ -255,12 +267,7 @@ __global__ void __launch_bounds__(256, 3) k_reduce_warm(TableDev t, OptimDev op,
     const uint32_t row = d.x, base = d.y, cnt = d.z;
     for (uint32_t l = lane; l < cnt; l += G) raw[l] = a.b.seg_occ[base + l];
     __syncwarp(gmask);
-    for (uint32_t l = lane; l < cnt; l += G) {  // occurrences are distinct numbers
-      const uint32_t p = raw[l];
-      uint32_t r = 0;
-      for (uint32_t m = 0; m < cnt; ++m) r += raw[m] < p;
-      srt[r] = p;
-    }
+    rank_sort(raw, srt, cnt, lane, G);
     __syncwarp(gmask);
     const uint32_t slot = slot_of_occ(sl, srt[0]);
     if (SEND) {
@@ -272,11 +279,7 @@ __global__ void __launch_bounds__(256, 3) k_reduce_warm(TableDev t, OptimDev op,
       }
       continue;
     }
-    if (slot_dead(dead, slot)) continue;
-    if (row >= t.capacity) {
-      if (lane == 0 && !a.quiet_miss) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);  // gradient_id_miss_count (PS mod.rs:401-403)
-      continue;
-    }
+    if (slot_dead(dead, slot) || row_missing(row, t, lane, !a.quiet_miss)) continue;
     float* stage = a.vw_stage ? a.vw_stage + (size_t)(n_cold + w) * t.dim : nullptr;
     step_item<VEC, F16, KIND>(t, op, hy, sl, gr, a, row, slot, cnt, lane, G, gmask, stage, [&](uint32_t k) { return srt[k]; });
   }
@@ -292,8 +295,7 @@ __global__ void __launch_bounds__(256) k_reduce_cold(TableDev t, OptimDev op, Hy
   const uint32_t n_cold = a.b.cnt[BC_COLD];
   if (blockIdx.x * (blockDim.x / G) >= n_cold) return;  // whole block
   build_dead_mask(dead, gr, a, sl.n_slots);
-  const uint32_t lane = threadIdx.x % G, wl = threadIdx.x & 31;
-  const uint32_t gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (wl / G * G));
+  const uint32_t lane = threadIdx.x % G;
   const uint32_t nvec = t.dim / VEC;
   // the grid holds a few blocks per SM; a group strides over the list (its length lives on the device)
   for (uint32_t w = blockIdx.x * (blockDim.x / G) + threadIdx.x / G; w < n_cold; w += gridDim.x * (blockDim.x / G)) {
@@ -319,32 +321,22 @@ __global__ void __launch_bounds__(256) k_reduce_cold(TableDev t, OptimDev op, Hy
       }
       continue;
     }
-    if (slot_dead(dead, slot)) continue;
-    if (d.x >= t.capacity) {
-      if (lane == 0 && !a.quiet_miss) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);
-      continue;
-    }
+    if (slot_dead(dead, slot) || row_missing(d.x, t, lane, !a.quiet_miss)) continue;
     if (KIND == PB_OPT_ADAGRAD_VW) {  // needs the whole reduced gradient staged for the dot
       const uint32_t occ = d.y;
-      step_item<VEC, F16, KIND>(t, op, hy, sl, gr, a, d.x, slot, 1u, lane, G, gmask, a.vw_stage + (size_t)w * t.dim,
-                                [&](uint32_t) { return occ; });
+      step_item<VEC, F16, KIND>(t, op, hy, sl, gr, a, d.x, slot, 1u, lane, G, group_mask(G),
+                                a.vw_stage + (size_t)w * t.dim, [&](uint32_t) { return occ; });
       continue;
     }
     float* prow = t.rows + (size_t)d.x * t.stride;
-    StepCtx sc;
-    sc.vw_state = sc.r1 = sc.r2 = 0.0f;
-    if (KIND == PB_OPT_ADAM) sc = step_ctx(prow, t, op, gr, slot);
-    for (uint32_t c = lane; c < nvec; c += G) {
-      RowElems<KIND, VEC> rc;
-      float g[VEC], acc[VEC];
-      rc.load(prow, c * VEC, t, op);
-      load_grad_elems<VEC, F16>(g, src.gbase, gelem, c * VEC);
+    const StepCtx sc = KIND == PB_OPT_ADAM ? step_ctx(prow, t, op, gr, slot) : StepCtx{0.0f, 0.0f, 0.0f};
+    step_row<KIND, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&acc)[VEC]) {
+      float g[VEC];
+      load_grad_elems<VEC, F16>(g, src.gbase, gelem, e0);
 #pragma unroll
       for (int q = 0; q < VEC; ++q) acc[q] = 0.0f;  // the reference adds into a zeroed row (-0 -> +0)
       add_prepared<VEC>(acc, g, prep, src.plain);
-      rc.step(c * VEC, acc, t, op, hy, sc);
-      rc.store(prow, c * VEC, t, op);
-    }
+    });
   }
 }
 
@@ -411,24 +403,6 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   unsigned long long now;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
   return now;
-}
-// non-blocking: has the phase with this parity completed?
-__device__ __forceinline__ bool mbar_test(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(done)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return done;
-}
-
-// +-inf -> +-65504 (persia-common lib.rs:163-180), two halves per instruction; finite halves are inside already
-__device__ __forceinline__ __half2 clamp_h2(__half2 v) {
-  const __half2 lim = __floats2half2_rn(65504.0f, 65504.0f);
-  return __hmin2(__hmax2(v, __hneg2(lim)), lim);
 }
 
 struct HotGeom {
@@ -653,10 +627,8 @@ __global__ void __launch_bounds__(HOT_THREADS, 1) k_reduce_hot(TableDev t, Slots
     } else {
       skip = slot_dead(dead, slot) || row >= t.capacity;  // (k_step_hot counts the rowless items of applied slots)
     }
-    if (skip) {  // the item's bits must still go back to zero for the next batch, unless a later round reads them
-      const bool other_round = !((a.round_mask[slot >> 5] >> (slot & 31)) & 1u);  // (an earlier one zeroed them already)
-      if (bm_mode && !other_round)
-        for (uint32_t w = tid; w < (hi - lo + 31u) / 32u; w += HOT_THREADS) a.b.hot_bits[base + w] = 0u;
+    if (skip) {
+      release_hot_bits(a, slot, bm_mode, base, lo, hi, tid, HOT_THREADS);
       continue;
     }
     const ItemSrc src = item_src(sl, gr, a, slot);
@@ -836,12 +808,9 @@ __global__ void __launch_bounds__(SHORT_WARPS * 32, 4) k_reduce_hot_short(TableD
     if (cnt > a.short_max) continue;  // k_reduce_hot's
     const bool bm_mode = d.y >> 31;
     const uint32_t base = d.y & 0x7FFFFFFFu;  // first bitmap word of the item, or first entry of its occurrence list
-    const uint32_t lo = sl.occ_off[slot], n_words = (sl.occ_off[slot + 1] - lo + 31u) / 32u;
+    const uint32_t lo = sl.occ_off[slot], hi = sl.occ_off[slot + 1], n_words = (hi - lo + 31u) / 32u;
     if (slot_dead(dead, slot) || row >= t.capacity) {  // (k_step_hot counts the rowless items of applied slots)
-      // the item's bits must still go back to zero for the next batch, unless a later round reads them
-      const bool other_round = !((a.round_mask[slot >> 5] >> (slot & 31)) & 1u);  // (an earlier one zeroed them already)
-      if (bm_mode && !other_round)
-        for (uint32_t w = lane; w < n_words; w += 32u) a.b.hot_bits[base + w] = 0u;
+      release_hot_bits(a, slot, bm_mode, base, lo, hi, lane, 32u);
       continue;
     }
     // ---- the item's occurrences, ascending
@@ -874,12 +843,7 @@ __global__ void __launch_bounds__(SHORT_WARPS * 32, 4) k_reduce_hot_short(TableD
     } else {
       for (uint32_t l = lane; l < cnt; l += 32u) raw[l] = a.b.seg_occ[base + l];
       __syncwarp();
-      for (uint32_t l = lane; l < cnt; l += 32u) {  // occurrences are distinct numbers
-        const uint32_t p = raw[l];
-        uint32_t r = 0;
-        for (uint32_t q = 0; q < cnt; ++q) r += raw[q] < p;
-        srt[r] = p;
-      }
+      rank_sort(raw, srt, cnt, lane, 32u);
     }
     __syncwarp();
     // ---- the sum, VEC columns per lane at a time
@@ -904,36 +868,18 @@ __global__ void __launch_bounds__(256) k_step_hot(TableDev t, OptimDev op, Hyper
   const uint32_t n_hot = a.b.cnt[BC_HOT] + n_huge + n_giant;
   if (blockIdx.x * (blockDim.x / G) >= n_hot) return;  // whole block
   build_dead_mask(dead, gr, a, sl.n_slots);
-  const uint32_t lane = threadIdx.x % G, wl = threadIdx.x & 31;
-  const uint32_t gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (wl / G * G));
-  const uint32_t nvec = t.dim / VEC;
+  const uint32_t lane = threadIdx.x % G;
+  const uint32_t gmask = group_mask(G);
   for (uint32_t h = blockIdx.x * (blockDim.x / G) + threadIdx.x / G; h < n_hot; h += gridDim.x * (blockDim.x / G)) {
     const uint32_t entry = hot_entry(a.b, h, n_giant, n_huge);
     const uint4 d = a.b.hot[entry];
     const uint32_t row = d.x, slot = d.w;
-    if (slot_dead(dead, slot)) continue;
-    if (row >= t.capacity) {
-      if (lane == 0 && !a.quiet_miss) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);  // gradient_id_miss_count (PS mod.rs:401-403)
-      continue;
-    }
+    if (slot_dead(dead, slot) || row_missing(row, t, lane, !a.quiet_miss)) continue;
     const float* sum = a.hot_stage + (size_t)entry * t.dim;
     float* prow = t.rows + (size_t)row * t.stride;
     const StepCtx sc = step_ctx(prow, t, op, gr, slot);
-    for (uint32_t c = lane; c < nvec; c += G) {
-      RowElems<-1, VEC> rc;
-      float g[VEC];
-      rc.load(prow, c * VEC, t, op);
-      load_vec<VEC>(sum + c * VEC, g);
-      rc.step(c * VEC, g, t, op, hy, sc);
-      rc.store(prow, c * VEC, t, op);
-    }
-    if (op.kind == PB_OPT_ADAGRAD_VW) {  // state = state*mom + dot(g,g)/dim (optim.rs:280-283)
-      __syncwarp(gmask);                 // every lane of the group read the old state
-      if (lane == 0) {
-        float gs = __fdiv_rn(vw_dot(sum, t.dim), (float)t.dim);
-        prow[t.dim] = __fadd_rn(__fmul_rn(sc.vw_state, op.mom), gs);
-      }
-    }
+    step_row<-1, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&g)[VEC]) { load_vec<VEC>(sum + e0, g); });
+    if (op.kind == PB_OPT_ADAGRAD_VW) vw_state_step(prow, sum, t, op, sc, lane, gmask);
   }
 }
 
@@ -1060,12 +1006,19 @@ void launch_reduce_hot_short(const TableDev& t, const SlotsDev& sl, const GradsD
 #undef PB_S
 }
 
+// floats per lane (vec) and lanes per item of the lane-group kernels: vec_group's, but at least 4 lanes (k_reduce_warm
+// has sort buffers for 64 groups of a block)
+static uint32_t item_group(uint32_t dim, int& vec) {
+  int G;
+  vec_group(dim, vec, G);
+  return (uint32_t)G < 4u ? 4u : (uint32_t)G;
+}
+
 void launch_step_hot(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl, const GradsDev& gr,
                      const ReduceArgs& a, cudaStream_t st) {
   if (!a.b.n) return;
-  int vec, Gi;
-  vec_group(t.dim, vec, Gi);
-  const uint32_t G = (uint32_t)Gi < 4u ? 4u : (uint32_t)Gi;
+  int vec;
+  const uint32_t G = item_group(t.dim, vec);
   // at most this many hot items exist; blocks past their number return at once
   uint32_t grid = cdiv(cdiv(a.b.n, PB_WARM_MAX + 1), 256u / G);
   if (grid > PB_NUM_SMS * 2u) grid = PB_NUM_SMS * 2u;  // groups stride over the list
@@ -1076,9 +1029,8 @@ void launch_step_hot(const TableDev& t, const OptimDev& op, const HyperDev& hy, 
 void launch_reduce_items(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl,
                          const GradsDev& gr, bool f16, const ReduceArgs& a, cudaStream_t st, cudaStream_t st_warm, bool send) {
   if (!a.b.n) return;
-  int vec, Gi;
-  vec_group(t.dim, vec, Gi);
-  uint32_t G = (uint32_t)Gi < 4u ? 4u : (uint32_t)Gi;
+  int vec;
+  const uint32_t G = item_group(t.dim, vec);
   if (vec == 4) {
     if (f16) items_dispatch<4, true>(t, op, hy, sl, gr, a, G, st, st_warm, send);
     else items_dispatch<4, false>(t, op, hy, sl, gr, a, G, st, st_warm, send);

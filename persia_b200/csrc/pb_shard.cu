@@ -403,6 +403,10 @@ __device__ __forceinline__ uint32_t adam_key_of(const XchgDev& x, uint64_t sign)
     if (x.akeys[g] == m) return g;
   return PB_ADAM_KEYS - 1u;  // (a group the table has never seen in a forward: cannot hold rows)
 }
+// request src's (beta1^t, beta2^t) of feature group akey
+__device__ __forceinline__ const float* owner_adam_pair(const XchgDev& x, uint32_t src, uint32_t akey) {
+  return x.apow + ((size_t)src * PB_ADAM_KEYS + akey) * 2u;
+}
 __global__ void __launch_bounds__(256) k_owner_adam_present(XchgDev x) {
   __shared__ uint32_t bits[PB_MAX_RANKS][PB_ADAM_KEYS / 32];
   for (uint32_t i = threadIdx.x; i < PB_MAX_RANKS * (PB_ADAM_KEYS / 32); i += blockDim.x) (&bits[0][0])[i] = 0u;
@@ -464,7 +468,7 @@ __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(Tabl
   if (threadIdx.x == 0) s_chained = *x.chained;
   __syncthreads();
   const uint32_t wl = threadIdx.x & 31u, lane = wl % G, gi = wl / G, n_g = 32u / G;
-  const uint32_t gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (gi * G));
+  const uint32_t gmask = group_mask(G);
   const uint32_t total = x.R * x.cap;
   const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = (gridDim.x * blockDim.x) >> 5;
   const float* grads = reinterpret_cast<const float*>(x.base[x.rank] + x.off_grad);
@@ -497,16 +501,10 @@ __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(Tabl
       const uint32_t j = j0 + mine, me = j / x.cap;
       UCell* cell = x.ucell + idx;
       float* prow = t.rows + (size_t)row * t.stride;
-      StepCtx sc;
-      sc.vw_state = sc.r1 = sc.r2 = 0.0f;
       uint32_t akey = 0;
       if (op.kind == PB_OPT_ADAM) akey = adam_key_of(x, x_sign(x, x.rank)[j]);  // the row's feature group
-#define PB_ADAM_CTX(SRC)                                                                     \
-  if (op.kind == PB_OPT_ADAM) {                                                              \
-    const float* pw = x.apow + ((size_t)(SRC) * PB_ADAM_KEYS + akey) * 2u;                   \
-    sc.r1 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[0]));                                         \
-    sc.r2 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[1]));                                         \
-  }
+      // the step of request s's gradient
+      auto ctx = [&](uint32_t s) { return step_ctx(op, 0.0f, owner_adam_pair(x, s, akey)); };
       // the holder mask, the row and the opener's gradient: one round trip
       const uint32_t mask = cell->mask;
       RowElems<KIND, VEC> rc[CPL];
@@ -520,7 +518,7 @@ __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(Tabl
       const uint32_t chained = mask & s_chained;  // holders whose request may hold the row more than once
       if (mask == (1u << me) && !chained) {  // the opener is the only holder, with one entry (the rule)
         if (ok1) {
-          PB_ADAM_CTX(me)
+          const StepCtx sc = ctx(me);
 #pragma unroll
           for (int u = 0; u < CPL; ++u) {
             const uint32_t e = ((uint32_t)u * G + lane) * VEC;
@@ -540,7 +538,7 @@ __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(Tabl
               float g[CPL][VEC];
 #pragma unroll
               for (int u = 0; u < CPL; ++u) load_vec<VEC>(grads + (size_t)at * t.dim + ((uint32_t)u * G + lane) * VEC, g[u]);
-              PB_ADAM_CTX(s)
+              const StepCtx sc = ctx(s);
 #pragma unroll
               for (int u = 0; u < CPL; ++u) rc[u].step(((uint32_t)u * G + lane) * VEC, g[u], t, op, hy, sc);
             }
@@ -573,7 +571,7 @@ __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(Tabl
 #pragma unroll
           for (int v = 0; v < 2; ++v)
             if (v < n && ok[v]) {
-              PB_ADAM_CTX(src[v])
+              const StepCtx sc = ctx(src[v]);
 #pragma unroll
               for (int u = 0; u < CPL; ++u) rc[u].step(((uint32_t)u * G + lane) * VEC, g[v][u], t, op, hy, sc);
             }
@@ -581,7 +579,6 @@ __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(Tabl
 #pragma unroll
         for (int u = 0; u < CPL; ++u) rc[u].store(prow, ((uint32_t)u * G + lane) * VEC, t, op);
       }
-#undef PB_ADAM_CTX
       __syncwarp(gmask);
       if (lane == 0) {  // every lane of the group has read the cell: it goes back to empty
         cell->row = ROW_NONE;
@@ -606,7 +603,7 @@ __global__ void k_uclear(XchgDev x) {
 template <int VEC>
 __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, HyperDev hy, XchgDev x, uint32_t src,
                                                       uint32_t G) {
-  const uint32_t lane = threadIdx.x % G;
+  const uint32_t lane = threadIdx.x % G, gmask = group_mask(G);
   const uint32_t n = x.own_cnt[src];
   const uint32_t nvec = t.dim / VEC;
   const uint32_t n_groups = gridDim.x * (blockDim.x / G);
@@ -617,41 +614,20 @@ __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, H
     // slots sharing a feature group: a lane group takes a chain's head and steps the sign's entries one after another in
     // slot order (so no two groups hold one row); the entries after the head only count their misses here
     const uint32_t* link = x.own_link + (size_t)src * x.cap;
-    const uint32_t wl = threadIdx.x & 31u;
-    const uint32_t gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (wl / G * G));
     for (uint32_t k0 = blockIdx.x * (blockDim.x / G) + threadIdx.x / G; k0 < n; k0 += n_groups) {
       const uint32_t row = own_row[k0];
-      if (row >= t.capacity) {
-        if (lane == 0 && gok[k0] != 0u) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);
-        continue;
-      }
-      if (link[k0] & CHAIN_CONT) continue;
+      if (row_missing(row, t, lane, gok[k0] != 0u) || (link[k0] & CHAIN_CONT)) continue;
       float* prow = t.rows + (size_t)row * t.stride;
-      StepCtx sc;
-      sc.r1 = sc.r2 = 0.0f;
-      if (op.kind == PB_OPT_ADAM) {  // this request's (beta1^t, beta2^t) of the row's feature group
-        const float* pw = x.apow + ((size_t)src * PB_ADAM_KEYS + adam_key_of(x, x_sign(x, x.rank)[(size_t)src * x.cap + k0])) * 2u;
-        sc.r1 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[0]));
-        sc.r2 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[1]));
-      }
+      // this request's (beta1^t, beta2^t) of the row's feature group
+      const uint32_t akey = op.kind == PB_OPT_ADAM ? adam_key_of(x, x_sign(x, x.rank)[(size_t)src * x.cap + k0]) : 0u;
+      StepCtx sc = step_ctx(op, 0.0f, owner_adam_pair(x, src, akey));
       uint32_t k = k0;
       for (uint32_t d = 0; d < PB_MAX_SLOTS; ++d) {  // (a chain holds at most one entry per slot)
         if (gok[k] != 0u) {
           const float* g0 = grads + (size_t)k * t.dim;
           sc.vw_state = op.kind == PB_OPT_ADAGRAD_VW ? prow[t.dim] : 0.0f;
-          for (uint32_t c = lane; c < nvec; c += G) {
-            RowElems<-1, VEC> rc;
-            float g[VEC];
-            rc.load(prow, c * VEC, t, op);
-            load_vec<VEC>(g0 + c * VEC, g);
-            rc.step(c * VEC, g, t, op, hy, sc);
-            rc.store(prow, c * VEC, t, op);
-          }
-          if (op.kind == PB_OPT_ADAGRAD_VW) {  // every lane has read the state before lane 0 writes the next one
-            __syncwarp(gmask);
-            if (lane == 0) prow[t.dim] = __fadd_rn(__fmul_rn(sc.vw_state, op.mom), __fdiv_rn(vw_dot(g0, t.dim), (float)t.dim));
-            __syncwarp(gmask);
-          }
+          step_row<-1, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&g)[VEC]) { load_vec<VEC>(g0 + e0, g); });
+          if (op.kind == PB_OPT_ADAGRAD_VW) vw_state_step(prow, g0, t, op, sc, lane, gmask);
         }
         k = link[k] & CHAIN_END;
         if (k >= n) break;  // CHAIN_END
@@ -670,19 +646,12 @@ __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, H
       const uint32_t k = k0 + u;
       act[u] = k < n && gok[k < n ? k : 0] != 0u;
       uint32_t row = act[u] ? own_row[k] : ROW_NONE;
-      if (act[u] && row >= t.capacity) {
-        if (lane == 0) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);
-        act[u] = false;
-      }
+      if (act[u] && row_missing(row, t, lane, true)) act[u] = false;
       prow[u] = t.rows + (size_t)(act[u] ? row : 0u) * t.stride;
       g0[u] = grads + (size_t)(act[u] ? k : 0u) * t.dim;
-      sc[u].vw_state = (act[u] && op.kind == PB_OPT_ADAGRAD_VW) ? prow[u][t.dim] : 0.0f;
-      sc[u].r1 = sc[u].r2 = 0.0f;
-      if (act[u] && op.kind == PB_OPT_ADAM) {  // this request's (beta1^t, beta2^t) of the row's feature group
-        const float* pw = x.apow + ((size_t)src * PB_ADAM_KEYS + adam_key_of(x, x_sign(x, x.rank)[(size_t)src * x.cap + k])) * 2u;
-        sc[u].r1 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[0]));
-        sc[u].r2 = __fdiv_rn(1.0f, __fsub_rn(1.0f, pw[1]));
-      }
+      // this request's (beta1^t, beta2^t) of the row's feature group
+      const uint32_t akey = act[u] && op.kind == PB_OPT_ADAM ? adam_key_of(x, x_sign(x, x.rank)[(size_t)src * x.cap + k]) : 0u;
+      sc[u] = step_ctx(op, (act[u] && op.kind == PB_OPT_ADAGRAD_VW) ? prow[u][t.dim] : 0.0f, owner_adam_pair(x, src, akey));
     }
     for (uint32_t c = lane; c < nvec; c += G) {
       RowElems<-1, VEC> rc[2];
@@ -700,13 +669,10 @@ __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, H
           rc[u].store(prow[u], c * VEC, t, op);
         }
     }
-    if (op.kind == PB_OPT_ADAGRAD_VW && lane == 0) {
+    if (op.kind == PB_OPT_ADAGRAD_VW) {
 #pragma unroll
       for (int u = 0; u < 2; ++u)
-        if (act[u]) {
-          float gs = __fdiv_rn(vw_dot(g0[u], t.dim), (float)t.dim);
-          prow[u][t.dim] = __fadd_rn(__fmul_rn(sc[u].vw_state, op.mom), gs);
-        }
+        if (act[u]) vw_state_step(prow[u], g0[u], t, op, sc[u], lane, gmask);
     }
   }
 }

@@ -74,32 +74,12 @@ __global__ void __launch_bounds__(256) k_update_direct(TableDev t, OptimDev op, 
   if (nan_tick && nan_tick[0] == *tick_ptr) return;  // NaN rule: the whole gradient is dropped
   uint32_t h = occ_cell[gid];
   uint32_t row = by_row ? h : (h < t.n_cells + N_SPECIAL) ? t.cells[h].row : ROW_NONE;
-  if (row >= t.capacity) {
-    if (lane == 0) atomicAdd(&t.counters[CTR_GRAD_MISS], 1u);
-    return;
-  }
+  if (row_missing(row, t, lane, true)) return;
   float* prow = t.rows + (size_t)row * t.stride;
-  const uint32_t nvec = t.dim / VEC;
-  StepCtx sc;
-  sc.vw_state = (op.kind == PB_OPT_ADAGRAD_VW) ? prow[t.dim] : 0.0f;
-  sc.r1 = sc.r2 = 0.0f;
-  if (op.kind == PB_OPT_ADAM) {
-    sc.r1 = __fdiv_rn(1.0f, __fsub_rn(1.0f, adam_pair[0]));
-    sc.r2 = __fdiv_rn(1.0f, __fsub_rn(1.0f, adam_pair[1]));
-  }
+  const StepCtx sc = step_ctx(op, op.kind == PB_OPT_ADAGRAD_VW ? prow[t.dim] : 0.0f, adam_pair);
   const float* g0 = grads + (size_t)gid * t.dim;
-  for (uint32_t c = lane; c < nvec; c += G) {
-    float g[VEC];
-    load_vec<VEC>(g0 + c * VEC, g);
-    RowElems<-1, VEC> rc;
-    rc.load(prow, c * VEC, t, op);
-    rc.step(c * VEC, g, t, op, hy, sc);
-    rc.store(prow, c * VEC, t, op);
-  }
-  if (op.kind == PB_OPT_ADAGRAD_VW && lane == 0) {
-    float gs = __fdiv_rn(vw_dot(g0, t.dim), (float)t.dim);
-    prow[t.dim] = __fadd_rn(__fmul_rn(sc.vw_state, op.mom), gs);
-  }
+  step_row<-1, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&g)[VEC]) { load_vec<VEC>(g0 + e0, g); });
+  if (op.kind == PB_OPT_ADAGRAD_VW) vw_state_step(prow, g0, t, op, sc, lane, group_mask(G));
 }
 
 // ------------------------------------------------------------------------------------------------
