@@ -123,6 +123,27 @@ struct pb_table {
 };
 
 struct pb_ctx {
+  // A training forward's batch, pending in the context until its backward: counted in its table's pending_batches, so
+  // that eviction spares its rows.
+  struct Pending {
+    bool on = false;
+    pb_table* table = nullptr;
+    void hold(pb_table* t) {
+      on = true;
+      table = t;
+      t->pending_batches++;
+    }
+    int check(const pb_table* t, const char* not_pending_msg, const char* other_table_msg) const {
+      if (!on) return fail(PB_ERR_STATE, not_pending_msg);
+      if (table != t) return fail(PB_ERR_INVALID, other_table_msg);
+      return PB_OK;
+    }
+    void drop() {
+      if (table && table->pending_batches) table->pending_batches--;
+      on = false;
+      table = nullptr;
+    }
+  };
   int device = 0;
   uint32_t max_occ = 0, max_out = 0;
   pb_slots_cfg slots{};
@@ -138,8 +159,7 @@ struct pb_ctx {
   uint32_t n_occ = 0, batch = 0;
   uint32_t* dev_tick = nullptr;  // request number of the pending forward (device side, CUDA-graph safe)
   uint32_t occ_off[PB_MAX_SLOTS + 1];
-  bool pending = false;
-  pb_table* pending_table = nullptr;  // the table whose rows the pending batch refers to (eviction spares them)
+  Pending pending;  // a summation batch awaiting its backward
   // slots of one feature group take turns in the backward (mod.rs:720-822): round of every slot
   uint32_t n_rounds = 1;
   uint8_t round_of[PB_MAX_SLOTS];
@@ -158,8 +178,8 @@ struct pb_ctx {
   // raw slot (pb_forward_raw / pb_backward_raw): allocated on first use
   uint32_t* occ_cell = nullptr;
   RawWork raw{};
-  bool raw_ready = false, raw_pending = false;
-  pb_table* raw_table = nullptr;  // raw forward pending on this table: counted in its pending_batches
+  bool raw_ready = false;
+  Pending raw_pending;  // a raw batch awaiting its backward
   float* raw_stage = nullptr;
   size_t raw_stage_floats = 0;
 };
@@ -479,19 +499,6 @@ void free_incremental(pb_table* t) {
   t->inc_host = nullptr;
 }
 
-void drop_pending(pb_ctx* c) {
-  if (c->pending && c->pending_table && c->pending_table->pending_batches) c->pending_table->pending_batches--;
-  c->pending = false;
-  c->pending_table = nullptr;
-}
-
-// a raw forward's rows stay protected from eviction until its gradients are applied, like a summation batch's
-void drop_raw_pending(pb_ctx* c) {
-  if (c->raw_table && c->raw_table->pending_batches) c->raw_table->pending_batches--;
-  c->raw_table = nullptr;
-  c->raw_pending = false;
-}
-
 // ---- what the local and sharded forms of the forwards and backwards share ------------------------------------------
 int check_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
                   const uint32_t* h_slot_occ_off, uint32_t batch, void* d_out_f16) {
@@ -523,16 +530,21 @@ int check_raw_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_
   return PB_OK;
 }
 
-int check_pending(pb_table* t, pb_ctx* c) {
-  if (!c->pending) return fail(PB_ERR_STATE, "no forward batch is pending in this context (backward_ref_id not found)");
-  if (c->pending_table != t) return fail(PB_ERR_INVALID, "the pending batch was looked up in another table");
-  return PB_OK;
+int check_backward(pb_table* t, pb_ctx* c, const void* const* h_grads) {
+  if (!t || !c || !h_grads) return fail(PB_ERR_INVALID, "null argument");
+  int rc = c->pending.check(t, "no forward batch is pending in this context (backward_ref_id not found)",
+                            "the pending batch was looked up in another table");
+  if (rc || (rc = ready_for_training(t))) return rc;
+  return check_grads_aligned(h_grads, c->slots.n_slots);
 }
 
-int check_raw_pending(pb_table* t, pb_ctx* c) {
-  if (!c->raw_pending) return fail(PB_ERR_STATE, "no raw forward batch is pending in this context (backward_ref_id not found)");
-  if (c->raw_table != t) return fail(PB_ERR_INVALID, "the pending raw batch was looked up in another table");
-  return PB_OK;
+// (t and c not null: each caller checks them with its own arguments)
+int check_raw_backward(pb_table* t, pb_ctx* c, const void* d_grad) {
+  int rc = c->raw_pending.check(t, "no raw forward batch is pending in this context (backward_ref_id not found)",
+                                "the pending raw batch was looked up in another table");
+  if (rc) return rc;
+  if (d_grad && misaligned(d_grad)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
+  return ready_for_training(t);
 }
 
 // the context's copy of a batch's row offsets (n_rows + 1) and the output row of every id occurrence
@@ -551,8 +563,8 @@ int begin_forward(pb_table* t, pb_ctx* c, const SlotsDev& sl, const uint64_t* d_
     launch_clear_items(c->b, st);
     c->set_dirty = false;
   }
-  if (c->pending) launch_clear_hot_bits(c->b, st);  // its hot items' bitmaps were never consumed
-  drop_pending(c);
+  if (c->pending.on) launch_clear_hot_bits(c->b, st);  // its hot items' bitmaps were never consumed
+  c->pending.drop();
   if (training) {
     if (int rc = maybe_evict(t, st)) return rc;
   }
@@ -578,9 +590,7 @@ int end_forward(pb_table* t, pb_ctx* c, const uint32_t* d_row_off, const uint32_
   if (d_row_off) {
     if (int rc = copy_row_off(c, d_row_off, S * batch, st)) return rc;
   }
-  c->pending = true;
-  c->pending_table = t;
-  t->pending_batches++;
+  c->pending.hold(t);
   c->set_dirty = true;
   return PB_OK;
 }
@@ -589,9 +599,7 @@ int end_forward(pb_table* t, pb_ctx* c, const uint32_t* d_row_off, const uint32_
 void hold_raw_batch(pb_table* t, pb_ctx* c, uint32_t n_occ, uint32_t batch) {
   c->n_occ = n_occ;
   c->batch = batch;
-  c->raw_pending = true;
-  c->raw_table = t;
-  t->pending_batches++;
+  c->raw_pending.hold(t);
 }
 
 // what the reduces of a summation backward read of the context's pending batch
@@ -1526,8 +1534,8 @@ int pb_ctx_destroy(pb_ctx* c) {
   if (!c) return PB_OK;
   DeviceGuard g(c->device);
   cudaDeviceSynchronize();
-  drop_pending(c);
-  drop_raw_pending(c);
+  c->pending.drop();
+  c->raw_pending.drop();
   void* ptrs[] = {c->b.set,   c->b.occ_set, c->b.item_cell, c->b.seg_occ, c->b.cold, c->b.warm, c->b.hot, c->b.hot_bits, c->b.cnt,
                   c->occ_cell, c->occ_outrow, c->row_off, c->nan_tick, c->vw_stage, c->hot_stage, c->dev_tick, c->raw.set,
                   c->raw.occ_set, c->raw.flag, c->raw.rank, c->raw.tiles, c->raw.distinct_cell, c->raw.counts, c->raw.target,
@@ -1586,25 +1594,27 @@ int pb_ctx_batch_stats(pb_ctx* c, uint32_t h_out[6], void* stream) {
   return PB_OK;
 }
 
-// pb_backward's staging buffer of the hot items' sums, hot_cap x dim floats.  The training forward calls this, so the
+// A backward's staging buffer `buf` of `floats` floats, grown to hold `need`.  The training forward grows it, so the
 // backward that follows neither synchronises nor allocates (and can be captured without a warm-up call).  The first
 // allocation neither synchronises nor enqueues anything, so that a context's first forward can be captured too: the
-// thread's capture mode is relaxed around it (cudaMalloc is refused under a global-mode capture otherwise).
-static int ensure_hot_stage(pb_ctx* c, uint32_t dim, cudaStream_t st) {
-  const size_t cap = (size_t)c->b.hot_cap * dim;
-  if (cap <= c->hot_stage_floats) return PB_OK;
-  if (c->hot_stage) {  // a wider table: the old buffer may still be read by enqueued work
+// thread's capture mode is relaxed around it (cudaMalloc is refused under a global-mode capture otherwise).  Growing
+// synchronises the stream and frees the old buffer: a forward captured with a larger need than any call before it fails
+// its capture, and a graph captured earlier must not be replayed after a larger call ran eagerly (warm up with the
+// largest batch, as for vw_stage).
+static int grow_stage(float*& buf, size_t& floats, size_t need, cudaStream_t st) {
+  if (need <= floats) return PB_OK;
+  if (buf) {  // the old buffer may still be read by enqueued work
     PB_CUDA(cudaStreamSynchronize(st));
-    cudaFree(c->hot_stage);
-    c->hot_stage = nullptr;
-    c->hot_stage_floats = 0;
+    cudaFree(buf);
+    buf = nullptr;
+    floats = 0;
   }
   cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
   PB_CUDA(cudaThreadExchangeStreamCaptureMode(&mode));
-  const cudaError_t e = cudaMalloc(&c->hot_stage, sizeof(float) * cap);
+  const cudaError_t e = cudaMalloc(&buf, sizeof(float) * need);
   cudaThreadExchangeStreamCaptureMode(&mode);  // the caller's mode again
   PB_CUDA(e);
-  c->hot_stage_floats = cap;
+  floats = need;
   return PB_OK;
 }
 
@@ -1625,7 +1635,8 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   TableCall call;
   if ((rc = call.begin(t, st, CALL_INDEX))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
-  if (training && (rc = ensure_hot_stage(c, t->d.dim, st))) return rc;
+  // pb_backward's staging of the hot items' sums, hot_cap x dim floats (a wider table grows it)
+  if (training && (rc = grow_stage(c->hot_stage, c->hot_stage_floats, (size_t)c->b.hot_cap * t->d.dim, st))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
   if ((rc = begin_forward(t, c, sl, d_ids, n_occ, training, st))) return rc;
@@ -1646,12 +1657,9 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
 
 int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, const float* h_scale,
                 int32_t* d_slot_status, void* stream) {
-  if (!t || !c || !h_grads) return fail(PB_ERR_INVALID, "null argument");
-  int rc = check_pending(t, c);
+  int rc = check_backward(t, c, h_grads);
   if (rc) return rc;
-  if ((rc = ready_for_training(t))) return rc;
   uint32_t S = c->slots.n_slots;
-  if ((rc = check_grads_aligned(h_grads, S))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;  // in the step chain only: runs beside the next forward and a pb_tier_stage (see there)
@@ -1745,7 +1753,7 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
     launch_inc_mark_items(t->inc, b, sl, on, c->dev_tick, c->nan_tick, c->set_dirty, st);
     c->set_dirty = false;
   }
-  drop_pending(c);
+  c->pending.drop();
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -1775,11 +1783,51 @@ void xchg_layout(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32, uint64_t 
   off[5] = off[4] + round256((uint64_t)R * cap * 4);                               // end
 }
 
+// The phases a sharded call runs (PB_PHASE_*; 0 = all).  Each phase ends by signalling a flag of the exchange that a
+// later phase of every peer waits for: a call that runs every phase waits for its peers' flags in the signal's launch
+// (post); a phase-split call signals only, and its next phase starts by waiting (await).  wait_peers = false: the
+// reader waits for each peer itself (the vectorwise Adagrad owner, owner_backward).
+struct Phases {
+  int mask;
+  explicit Phases(int phases) : mask(phases ? phases : PB_PHASE_ALL) {}
+  bool has(int phase) const { return (mask & phase) != 0; }
+  void post(const pb_xchg* x, int flag, const uint32_t* counts, cudaStream_t st, bool wait_peers = true) const {
+    if (mask == PB_PHASE_ALL && wait_peers) launch_signal_wait(x->d, flag, counts, st);
+    else launch_signal(x->d, flag, counts, st);
+  }
+  void await(const pb_xchg* x, int flag, cudaStream_t st) const {
+    if (mask != PB_PHASE_ALL) launch_wait(x->d, flag, -1, st);
+  }
+};
+
+// What a sharded call needs of its exchange: the table's device and dim, and f32 rows where `need_f32_rows` (refused
+// with `f32_message`).  A backward passes its context, whose device it has not checked yet; a forward passes none
+// (check_forward has checked it), and refuses a table with a host tier as well.
+int check_exchange(const pb_table* t, const pb_ctx* c, const pb_xchg* x, bool need_f32_rows, const char* f32_message) {
+  if (!c && t->tier) return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no sharded calls)");
+  if (c && (t->device != c->device || t->device != x->device))
+    return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
+  if (t->device != x->device) return fail(PB_ERR_INVALID, "table and exchange live on different devices");
+  if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
+  if (need_f32_rows && !x->d.row_f32) return fail(PB_ERR_INVALID, f32_message);
+  return PB_OK;
+}
+
+// The owner's part of a sharded forward (PB_PHASE_SERVE), shared by the summation and the raw calls: the rows of the
+// signs sent to this shard, into the requesters' areas.
+void serve_lookup(pb_table* t, pb_xchg* x, int training, const Phases& ph, cudaStream_t st) {
+  ph.await(x, XC_FLAG_SIGN, st);
+  if (training && x->u_dirty) launch_uclear(x->d, st);  // a training batch whose gradients never came left its rows noted
+  launch_owner_lookup(training != 0, t->d, t->hy, t->op, x->d, st);
+  if (training) x->u_dirty = true;
+  ph.post(x, XC_FLAG_ROW, nullptr, st);
+}
+
 // The owner's part of a sharded backward (PB_PHASE_SERVE), shared by the summation and the raw calls: the step's R
 // gradient requests, every row stepped once per request in rank order.  prefix[n_prefix]: the feature groups of the
 // slots the exchange serves (Adam beta powers).
-int owner_backward(pb_table* t, pb_xchg* x, const uint64_t* prefix, uint32_t n_prefix, uint64_t spacing, int phases,
-                   cudaStream_t st) {
+int owner_backward(pb_table* t, pb_xchg* x, const uint64_t* prefix, uint32_t n_prefix, uint64_t spacing,
+                   const Phases& ph, cudaStream_t st) {
   if (t->op.kind == PB_OPT_ADAGRAD_VW) {  // (needs the whole gradient's dot per step) one request after another
     for (uint32_t src = 0; src < x->d.R; ++src) {
       launch_wait(x->d, XC_FLAG_GRAD, (int)src, st);
@@ -1787,7 +1835,7 @@ int owner_backward(pb_table* t, pb_xchg* x, const uint64_t* prefix, uint32_t n_p
     }
     launch_uclear(x->d, st);
   } else {  // owner: the R requests in one launch, every row stepped in rank order
-    if (phases != PB_PHASE_ALL) launch_wait(x->d, XC_FLAG_GRAD, -1, st);
+    ph.await(x, XC_FLAG_GRAD, st);
     if (t->op.kind == PB_OPT_ADAM) {  // every request advances the beta powers of the feature groups it holds here
       for (uint32_t s = 0; s < n_prefix; ++s)
         if (adam_index(t, prefix[s]) < 0) return fail(PB_ERR_CAPACITY, "more feature groups than Adam beta-power pairs");
@@ -1899,15 +1947,12 @@ int pb_xchg_status(pb_xchg* x, uint32_t h_out[2], void* stream) {
 int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
                        const uint32_t* h_slot_occ_off, uint32_t batch, int training, void* d_out_f16, void* stream,
                        int phases) {
-  if (phases == 0) phases = PB_PHASE_ALL;
-  const bool all = phases == PB_PHASE_ALL;
+  const Phases ph(phases);
   if (!x) return fail(PB_ERR_INVALID, "null argument");
   int rc = check_forward(t, c, d_ids, n_occ, d_row_off, h_slot_occ_off, batch, d_out_f16);
-  if (rc) return rc;
-  if (t->tier) return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no sharded calls)");
-  if (t->device != x->device) return fail(PB_ERR_INVALID, "table and exchange live on different devices");
-  if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
-  if (d_row_off && !x->d.row_f32) return fail(PB_ERR_INVALID, "ragged layouts need an exchange created with f32 rows");
+  if (rc || (rc = check_exchange(t, nullptr, x, d_row_off != nullptr,
+                                 "ragged layouts need an exchange created with f32 rows")))
+    return rc;
   const uint64_t n_out = (uint64_t)c->slots.n_slots * batch;
   // every rank serves lookups whether or not its own batch trains: the shard must be usable (a collective call)
   if ((rc = ready_for_training(t))) return rc;
@@ -1916,48 +1961,36 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
   if ((rc = ensure_alloc(t))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
-  if (phases & PB_PHASE_SEND) {
+  if (ph.has(PB_PHASE_SEND)) {
     if ((rc = begin_forward(t, c, sl, d_ids, n_occ, training, st))) return rc;
     launch_route_items(training != 0, sl, c->b, x->d, st);               // requester: signs -> owners' areas
     if (training && c->n_rounds > 1) launch_link_items(sl, c->b, x->d, c->links, st);  // a sign's entries, slot order
-    if (all) launch_signal_wait(x->d, XC_FLAG_SIGN, c->b.cnt + BC_PEER, st);  // (one launch when no phase split is asked for)
-    else launch_signal(x->d, XC_FLAG_SIGN, c->b.cnt + BC_PEER, st);
+    ph.post(x, XC_FLAG_SIGN, c->b.cnt + BC_PEER, st);
   }
-  if (phases & PB_PHASE_SERVE) {
-    if (!all) launch_wait(x->d, XC_FLAG_SIGN, -1, st);
-    if (training && x->u_dirty) launch_uclear(x->d, st);  // a training batch whose gradients never came left its rows noted
-    launch_owner_lookup(training != 0, t->d, t->hy, t->op, x->d, st);    // owner: rows -> requesters' areas
-    if (training) x->u_dirty = true;
-    if (all) launch_signal_wait(x->d, XC_FLAG_ROW, nullptr, st);
-    else launch_signal(x->d, XC_FLAG_ROW, nullptr, st);
+  if (ph.has(PB_PHASE_SERVE)) serve_lookup(t, x, training, ph, st);
+  if (ph.has(PB_PHASE_FINISH)) {
+    ph.await(x, XC_FLAG_ROW, st);
+    launch_expand_items(t->d, sl, c->b, x->d, d_row_off, (uint32_t)n_out, batch, training != 0, d_out_f16, st);
+    if ((rc = end_forward(t, c, d_row_off, h_slot_occ_off, n_occ, batch, training, st))) return rc;
   }
-  if (!(phases & PB_PHASE_FINISH)) {
-    PB_CUDA(cudaGetLastError());
-    return PB_OK;
-  }
-  if (!all) launch_wait(x->d, XC_FLAG_ROW, -1, st);
-  launch_expand_items(t->d, sl, c->b, x->d, d_row_off, (uint32_t)n_out, batch, training != 0, d_out_f16, st);
-  if ((rc = end_forward(t, c, d_row_off, h_slot_occ_off, n_occ, batch, training, st))) return rc;
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
 
 int pb_backward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* const* h_grads, int is_f16, const float* h_scale,
                         int32_t* d_slot_status, void* stream, int phases) {
-  if (phases == 0) phases = PB_PHASE_ALL;
-  if (!t || !c || !x || !h_grads) return fail(PB_ERR_INVALID, "null argument");
-  int rc = check_pending(t, c);
-  if (rc) return rc;
-  if ((rc = ready_for_training(t))) return rc;
+  const Phases ph(phases);
+  if (!x) return fail(PB_ERR_INVALID, "null argument");
+  int rc = check_backward(t, c, h_grads);
+  if (rc || (rc = check_exchange(t, c, x, false, nullptr))) return rc;
   uint32_t S = c->slots.n_slots;
-  if ((rc = check_grads_aligned(h_grads, S))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, c->occ_off, sl))) return rc;
   GradsDev gr;
   if ((rc = make_grads(h_grads, h_scale, S, gr))) return rc;
-  if (phases & PB_PHASE_SEND) {
+  if (ph.has(PB_PHASE_SEND)) {
     if ((rc = fork_side(c, st))) return rc;
     if (c->set_dirty) {
       launch_clear_items(c->b, c->side);
@@ -1972,15 +2005,12 @@ int pb_backward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* const* h
     launch_reduce_hot(t->d, sl, gr, is_f16 != 0, a, profiling() ? st : c->side, true);
     launch_reduce_items(t->d, t->op, t->hy, sl, gr, is_f16 != 0, a, st, profiling() ? st : c->side2, true);
     if ((rc = join_sides(c, st))) return rc;
-    if (phases == PB_PHASE_ALL && t->op.kind != PB_OPT_ADAGRAD_VW) launch_signal_wait(x->d, XC_FLAG_GRAD, nullptr, st);
-    else launch_signal(x->d, XC_FLAG_GRAD, nullptr, st);
+    ph.post(x, XC_FLAG_GRAD, nullptr, st, t->op.kind != PB_OPT_ADAGRAD_VW);
   }
-  if (!(phases & PB_PHASE_SERVE)) {
-    PB_CUDA(cudaGetLastError());
-    return PB_OK;
+  if (ph.has(PB_PHASE_SERVE)) {
+    if ((rc = owner_backward(t, x, c->slots.prefix, S, sl.spacing, ph, st))) return rc;
+    c->pending.drop();
   }
-  if ((rc = owner_backward(t, x, c->slots.prefix, S, sl.spacing, phases, st))) return rc;
-  drop_pending(c);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -2009,27 +2039,9 @@ static int ensure_raw(pb_ctx* c) {
 
 // pb_backward_raw's f32 staging buffer: one row per distinct sign of the batch, so n_occ x dim floats bound it.  Sized
 // by the batch, not by max_occ: a context made at twice a batch's ids (persia_core) would otherwise ask for twice the
-// staging, 64 GB at 2^24 occurrences and dim 1024.  It grows when a larger batch or dim comes.  The training forward
-// calls this, so the backward that follows neither synchronises nor allocates; the first allocation neither synchronises
-// nor enqueues anything (see ensure_hot_stage).  Growing synchronises the stream and frees the old buffer: a forward
-// captured with more ids than any batch before it fails its capture, and a graph captured earlier must not be replayed
-// after a larger batch ran eagerly (warm up with the largest batch, as for vw_stage).
+// staging, 64 GB at 2^24 occurrences and dim 1024.  It grows when a larger batch or dim comes.
 static int ensure_raw_stage(pb_ctx* c, uint32_t n_occ, uint32_t dim, cudaStream_t st) {
-  const size_t cap = (size_t)(n_occ ? n_occ : 1) * dim;
-  if (cap <= c->raw_stage_floats) return PB_OK;
-  if (c->raw_stage) {  // the old buffer may still be read by enqueued work
-    PB_CUDA(cudaStreamSynchronize(st));
-    cudaFree(c->raw_stage);
-    c->raw_stage = nullptr;
-    c->raw_stage_floats = 0;
-  }
-  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
-  PB_CUDA(cudaThreadExchangeStreamCaptureMode(&mode));
-  const cudaError_t e = cudaMalloc(&c->raw_stage, sizeof(float) * cap);
-  cudaThreadExchangeStreamCaptureMode(&mode);  // the caller's mode again
-  PB_CUDA(e);
-  c->raw_stage_floats = cap;
-  return PB_OK;
+  return grow_stage(c->raw_stage, c->raw_stage_floats, (size_t)(n_occ ? n_occ : 1) * dim, st);
 }
 
 int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
@@ -2052,7 +2064,7 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   if (training && (rc = ensure_raw_stage(c, n_occ, t->d.dim, st))) return rc;
   SlotsDev sl;
   if ((rc = raw_slots(c, n_occ, sl))) return rc;
-  drop_raw_pending(c);  // the numbering below replaces the pending batch's
+  c->raw_pending.drop();  // the numbering below replaces the pending batch's
   if (training) {
     if ((rc = maybe_evict(t, st))) return rc;
     launch_begin_batch(t->d, c->dev_tick, nullptr, st);
@@ -2076,15 +2088,13 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
 int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, float scale, int32_t* d_status,
                     void* stream) {
   if (!t || !c) return fail(PB_ERR_INVALID, "null argument");
-  int rc = check_raw_pending(t, c);
+  int rc = check_raw_backward(t, c, d_grad);
   if (rc) return rc;
-  if (d_grad && misaligned(d_grad)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
-  if ((rc = ready_for_training(t))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;  // in the step chain only: runs beside the next forward and a pb_tier_stage (see there)
   if ((rc = call.begin(t, st, CALL_STEP))) return rc;
-  drop_raw_pending(c);  // enqueued below: the sweep of the next training call runs after these gradients
+  c->raw_pending.drop();  // enqueued below: the sweep of the next training call runs after these gradients
   GradsDev gr;
   std::memset(&gr, 0, sizeof(gr));
   gr.ptr[0] = d_grad;
@@ -2120,26 +2130,23 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
                            const uint32_t* d_row_off, uint32_t batch, uint32_t sample_fixed_size, int training,
                            void* d_table_f16, int64_t* d_index, int64_t* d_non_empty, uint32_t* d_sample_id_num,
                            uint32_t* d_counts, void* stream, int phases) {
-  if (phases == 0) phases = PB_PHASE_ALL;
-  const bool all = phases == PB_PHASE_ALL;
+  const Phases ph(phases);
   if (!x) return fail(PB_ERR_INVALID, "null argument");
   int rc = check_raw_forward(t, c, d_ids, n_occ, d_row_off, batch, sample_fixed_size, d_table_f16, d_index, d_non_empty,
                              d_sample_id_num, d_counts);
-  if (rc) return rc;
-  if (t->tier) return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no sharded calls)");
-  if (t->device != x->device) return fail(PB_ERR_INVALID, "table and exchange live on different devices");
-  if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
-  if (!x->d.row_f32) return fail(PB_ERR_INVALID, "raw slots need an exchange created with f32 rows (the requester rounds them)");
+  if (rc || (rc = check_exchange(t, nullptr, x, true,
+                                 "raw slots need an exchange created with f32 rows (the requester rounds them)")))
+    return rc;
   // every rank serves lookups whether or not its own batch trains: the shard must be usable (a collective call)
   if ((rc = ready_for_training(t))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   if ((rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_raw(c))) return rc;
-  if (phases & PB_PHASE_SEND) {
+  if (ph.has(PB_PHASE_SEND)) {
     SlotsDev sl;
     if ((rc = raw_slots(c, n_occ, sl))) return rc;
-    drop_raw_pending(c);  // the numbering below replaces the pending batch's
+    c->raw_pending.drop();  // the numbering below replaces the pending batch's
     if (training) {
       if ((rc = maybe_evict(t, st))) return rc;
       launch_begin_batch(t->d, c->dev_tick, nullptr, st);
@@ -2151,63 +2158,46 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
     PB_CUDA(cudaMemcpyAsync(d_counts, c->raw.counts, 8, cudaMemcpyDeviceToDevice, st));
     PB_CUDA(cudaMemsetAsync(c->raw.peer, 0, 4 * PB_MAX_RANKS, st));
     launch_raw_route(c->raw, n_occ, x->d, st);  // requester: distinct signs -> owners' areas
-    if (all) launch_signal_wait(x->d, XC_FLAG_SIGN, c->raw.peer, st);
-    else launch_signal(x->d, XC_FLAG_SIGN, c->raw.peer, st);
+    ph.post(x, XC_FLAG_SIGN, c->raw.peer, st);
   }
-  if (phases & PB_PHASE_SERVE) {
-    if (!all) launch_wait(x->d, XC_FLAG_SIGN, -1, st);
-    if (training && x->u_dirty) launch_uclear(x->d, st);  // a training batch whose gradients never came left its rows noted
-    launch_owner_lookup(training != 0, t->d, t->hy, t->op, x->d, st);  // owner: f32 rows -> requesters' areas
-    if (training) x->u_dirty = true;
-    if (all) launch_signal_wait(x->d, XC_FLAG_ROW, nullptr, st);
-    else launch_signal(x->d, XC_FLAG_ROW, nullptr, st);
+  if (ph.has(PB_PHASE_SERVE)) serve_lookup(t, x, training, ph, st);
+  if (ph.has(PB_PHASE_FINISH)) {
+    ph.await(x, XC_FLAG_ROW, st);
+    launch_raw_fill(c->raw, n_occ, t->d.dim, x->d, d_table_f16, st);  // requester: rows in -> distinct-sign table
+    if (training) hold_raw_batch(t, c, n_occ, batch);
   }
-  if (!(phases & PB_PHASE_FINISH)) {
-    PB_CUDA(cudaGetLastError());
-    return PB_OK;
-  }
-  if (!all) launch_wait(x->d, XC_FLAG_ROW, -1, st);
-  launch_raw_fill(c->raw, n_occ, t->d.dim, x->d, d_table_f16, st);  // requester: rows in -> distinct-sign table
-  if (training) hold_raw_batch(t, c, n_occ, batch);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
 
 int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_grad, int is_f16, float scale,
                             int32_t* d_status, void* stream, int phases) {
-  if (phases == 0) phases = PB_PHASE_ALL;
+  const Phases ph(phases);
   if (!t || !c || !x) return fail(PB_ERR_INVALID, "null argument");
   if (!c->has_slots || c->slots.n_slots != 1) return fail(PB_ERR_STATE, "a raw context serves exactly one slot (pb_ctx_set_slots)");
-  if (t->device != c->device || t->device != x->device) return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
-  if (x->dim != t->cfg.dim) return fail(PB_ERR_INVALID, "the exchange was sized for another embedding dim");
-  int rc = check_raw_pending(t, c);
-  if (rc) return rc;
-  if (d_grad && misaligned(d_grad)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
-  if ((rc = ready_for_training(t))) return rc;
+  int rc = check_exchange(t, c, x, false, nullptr);
+  if (rc || (rc = check_raw_backward(t, c, d_grad))) return rc;
   uint8_t do_scale = 0;  // (add_skipped_gradient: the send reads no gradient, nor its scale)
   float inv = 1.0f;
   if (d_grad && (rc = loss_scale(scale, do_scale, inv))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   const uint32_t dim = t->d.dim;
-  if (phases & PB_PHASE_SEND) {  // the NaN rule, add_skipped_gradient, the clamp and 1/scale: on the requester
+  if (ph.has(PB_PHASE_SEND)) {  // the NaN rule, add_skipped_gradient, the clamp and 1/scale: on the requester
     GradsDev gr;
     std::memset(&gr, 0, sizeof(gr));
     gr.ptr[0] = d_grad;
     if (d_grad) launch_raw_nan(d_grad, is_f16 != 0, c->raw.counts, dim, c->dev_tick, c->nan_tick, st);
     if (d_status) launch_slot_status(gr, 1, c->dev_tick, c->nan_tick, d_status, st);
     launch_raw_send(d_grad, is_f16 != 0, c->raw, c->n_occ, dim, inv, do_scale != 0, c->dev_tick, c->nan_tick, x->d, st);
-    if (phases == PB_PHASE_ALL && t->op.kind != PB_OPT_ADAGRAD_VW) launch_signal_wait(x->d, XC_FLAG_GRAD, nullptr, st);
-    else launch_signal(x->d, XC_FLAG_GRAD, nullptr, st);
+    ph.post(x, XC_FLAG_GRAD, nullptr, st, t->op.kind != PB_OPT_ADAGRAD_VW);
   }
-  if (!(phases & PB_PHASE_SERVE)) {
-    PB_CUDA(cudaGetLastError());
-    return PB_OK;
+  if (ph.has(PB_PHASE_SERVE)) {
+    SlotsDev sl;
+    if ((rc = raw_slots(c, c->n_occ, sl))) return rc;
+    if ((rc = owner_backward(t, x, c->slots.prefix, 1, sl.spacing, ph, st))) return rc;
+    c->raw_pending.drop();
   }
-  SlotsDev sl;
-  if ((rc = raw_slots(c, c->n_occ, sl))) return rc;
-  if ((rc = owner_backward(t, x, c->slots.prefix, 1, sl.spacing, phases, st))) return rc;
-  drop_raw_pending(c);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
