@@ -416,6 +416,12 @@ typedef struct pb_xchg pb_xchg;
 uint64_t pb_xchg_bytes(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32);
 int pb_xchg_create(int device, uint32_t R, uint32_t rank, uint32_t cap, uint32_t dim, int rows_f32,
                    const uint64_t* h_peer_base, pb_xchg** out);
+/* Replacing an exchange (e.g. by one of a larger cap, or with f32 rows): an exchange keeps nothing across steps but its
+ * phase epochs, which live in it and in its area, and a cache of the table's feature-group prefixes; the Adam beta powers,
+ * the rows and the incremental set live in the pb_table.  So the ranks may destroy their exchanges and create new ones
+ * (zero-initialised areas) collectively, at a step boundary — after the last step that used the old ones has completed
+ * on every rank and before any rank calls the next — and the table, its Adam powers and its incremental set are
+ * unaffected.  A context's prepared batch (PB_PHASE_PREPARE) survives the replacement. */
 int pb_xchg_destroy(pb_xchg* x);
 /* h_out[0] != 0: a batch needed more than cap slots for one pair (its excess signs read as zeros and took no
  * gradient: re-run it with a larger cap); h_out[1] != 0: a wait for a peer gave up.  Synchronises `stream`. */
@@ -428,6 +434,18 @@ int pb_xchg_status(pb_xchg* x, uint32_t h_out[2], void* stream);
 #define PB_PHASE_SERVE 2  /* owner: forward lookups + rows out; backward optimizer steps */
 #define PB_PHASE_FINISH 4 /* requester, forward only: rows in -> output */
 #define PB_PHASE_ALL 7
+/* Forwards only, never part of phases = 0: requester, local work only — the forward's per-slot dedup (summation call)
+ * or the slot's distinct-sign numbering (raw call), then the batch's distinct (slot, sign) items per owner
+ * farmhash64(sign) % R, for pb_xchg_need.  Raises no flag, stores into no peer's area and reads or writes no table
+ * state (no eviction check, no request number, no probe); the context's previous batch goes, as in SEND.  A ragged
+ * batch may be prepared on an f16 exchange.  A later call with PB_PHASE_SEND on the same context and the same ids
+ * reuses the prepared work and then runs SEND's table part as always: eviction check, request number, route, link,
+ * signal (a different n_occ or batch: PB_ERR_STATE).  Between the two the caller may replace the exchange (see
+ * pb_xchg_destroy) so that its cap covers pb_xchg_need; that is how a step is sized from its own batch. */
+#define PB_PHASE_PREPARE 8
+/* h_out[0] = the most items the context's prepared batch sends to one owner (what cap must hold).  Synchronises
+ * `stream`.  PB_ERR_STATE without a prepared batch (its SEND consumes it). */
+int pb_xchg_need(pb_xchg* x, pb_ctx* c, uint32_t h_out[1], void* stream);
 /* forward_batched_direct over R shards: arguments as pb_forward (raw slots: pb_forward_raw_sharded below).  Slots that
  * share a feature group (equal prefixes) are supported: a sign held by several of them is one entry per slot of the
  * request, and the owner steps a row rank by rank, each rank's entries in slot order, as the reference does. */

@@ -182,7 +182,13 @@ struct pb_ctx {
   Pending raw_pending;  // a raw batch awaiting its backward
   float* raw_stage = nullptr;
   size_t raw_stage_floats = 0;
+  // sharded path, PB_PHASE_PREPARE: the batch deduplicated ahead of its SEND (PREP_SUM / PREP_RAW: which call's, with
+  // its ids) and its distinct items per owner
+  int prepared = 0;
+  uint32_t prepared_n = 0, prepared_batch = 0;
+  uint32_t* need = nullptr;  // [PB_MAX_RANKS]
 };
+enum { PREP_NONE = 0, PREP_SUM = 1, PREP_RAW = 2 };
 
 namespace {
 
@@ -554,10 +560,9 @@ int copy_row_off(pb_ctx* c, const uint32_t* d_row_off, uint32_t n_rows, cudaStre
   return PB_OK;
 }
 
-// A summation forward's start: the context's previous batch goes (like an expired post_forward_buffer entry,
-// mod.rs:991-1029), then the new batch's distinct items are found.
-int begin_forward(pb_table* t, pb_ctx* c, const SlotsDev& sl, const uint64_t* d_ids, uint32_t n_occ, int training,
-                  cudaStream_t st) {
+// The context's previous batch goes (like an expired post_forward_buffer entry, mod.rs:991-1029), and with it any
+// batch prepared and never sent.
+void drop_batch(pb_ctx* c, cudaStream_t st) {
   // a batch whose gradients never came (or an inference request) leaves its cells in the scratch set: empty it first
   if (c->set_dirty) {
     launch_clear_items(c->b, st);
@@ -565,13 +570,41 @@ int begin_forward(pb_table* t, pb_ctx* c, const SlotsDev& sl, const uint64_t* d_
   }
   if (c->pending.on) launch_clear_hot_bits(c->b, st);  // its hot items' bitmaps were never consumed
   c->pending.drop();
+  c->prepared = PREP_NONE;
+}
+
+// A summation forward's start: the context's previous batch goes, then the new batch's distinct items are found.
+// `prepared`: PB_PHASE_PREPARE found them already (prepare_batch); only the table's part is left.
+int begin_forward(pb_table* t, pb_ctx* c, const SlotsDev& sl, const uint64_t* d_ids, uint32_t n_occ, int training,
+                  cudaStream_t st, bool prepared = false) {
+  if (!prepared) drop_batch(c, st);
   if (training) {
     if (int rc = maybe_evict(t, st)) return rc;
+  }
+  if (prepared) {  // the request number only: the dedup's counters hold the prepared batch
+    if (training) launch_begin_batch(t->d, c->dev_tick, nullptr, st, true);
+    c->prepared = PREP_NONE;
+    return PB_OK;
   }
   launch_begin_batch(t->d, training ? c->dev_tick : nullptr, c->b.cnt, st, training != 0);
   c->b.n = n_occ;
   launch_dedup(sl, c->b, d_ids, st);
   return PB_OK;
+}
+
+// PB_PHASE_PREPARE of a summation forward: begin_forward's dedup alone.  It reads no table state (k_dedup works in the
+// context's scratch set), so the eviction check and the request number stay with SEND.  The set holds the batch from
+// here on: a batch prepared and never sent is emptied by the context's next forward.
+void prepare_batch(const pb_table* t, pb_ctx* c, const SlotsDev& sl, const uint64_t* d_ids, uint32_t n_occ,
+                   uint32_t batch, cudaStream_t st) {
+  drop_batch(c, st);
+  launch_begin_batch(t->d, nullptr, c->b.cnt, st, false);  // (no bump: the table's counters are not touched)
+  c->b.n = n_occ;
+  launch_dedup(sl, c->b, d_ids, st);
+  c->set_dirty = true;
+  c->prepared = PREP_SUM;
+  c->prepared_n = n_occ;
+  c->prepared_batch = batch;
 }
 
 // A summation forward's end: a training batch stays in the context, pending, for its backward (its cells are emptied
@@ -580,6 +613,7 @@ int end_forward(pb_table* t, pb_ctx* c, const uint32_t* d_row_off, const uint32_
                 uint32_t batch, int training, cudaStream_t st) {
   if (!training) {
     launch_clear_items(c->b, st);
+    c->set_dirty = false;  // (a prepared batch marked it)
     return PB_OK;
   }
   const uint32_t S = c->slots.n_slots;
@@ -1506,6 +1540,8 @@ int pb_ctx_create(int device, uint32_t max_occurrences, uint32_t max_out_rows, p
   A((void**)&c->row_off, 4 * ((size_t)max_out_rows + 1));
   A((void**)&c->nan_tick, 4 * PB_MAX_SLOTS);
   A((void**)&c->dev_tick, 4);
+  A((void**)&c->need, 4 * PB_MAX_RANKS);
+  if (e == cudaSuccess) e = cudaMemset(c->need, 0, 4 * PB_MAX_RANKS);
   if (e == cudaSuccess) e = cudaMemset(c->nan_tick, 0, 4 * PB_MAX_SLOTS);
   if (e == cudaSuccess) e = cudaMemset(c->dev_tick, 0, 4);
   if (e == cudaSuccess) e = cudaMemset(c->b.cnt, 0, 4 * BC_COUNT);
@@ -1539,7 +1575,7 @@ int pb_ctx_destroy(pb_ctx* c) {
   void* ptrs[] = {c->b.set,   c->b.occ_set, c->b.item_cell, c->b.seg_occ, c->b.cold, c->b.warm, c->b.hot, c->b.hot_bits, c->b.cnt,
                   c->occ_cell, c->occ_outrow, c->row_off, c->nan_tick, c->vw_stage, c->hot_stage, c->dev_tick, c->raw.set,
                   c->raw.occ_set, c->raw.flag, c->raw.rank, c->raw.tiles, c->raw.distinct_cell, c->raw.counts, c->raw.target,
-                  c->raw.peer,    c->raw_stage};
+                  c->raw.peer,    c->raw_stage, c->need};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   if (c->side) cudaStreamDestroy(c->side);
@@ -1786,19 +1822,31 @@ void xchg_layout(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32, uint64_t 
 // The phases a sharded call runs (PB_PHASE_*; 0 = all).  Each phase ends by signalling a flag of the exchange that a
 // later phase of every peer waits for: a call that runs every phase waits for its peers' flags in the signal's launch
 // (post); a phase-split call signals only, and its next phase starts by waiting (await).  wait_peers = false: the
-// reader waits for each peer itself (the vectorwise Adagrad owner, owner_backward).
+// reader waits for each peer itself (the vectorwise Adagrad owner, owner_backward).  PB_PHASE_PREPARE signals nothing
+// and is not part of that choice.
 struct Phases {
   int mask;
   explicit Phases(int phases) : mask(phases ? phases : PB_PHASE_ALL) {}
   bool has(int phase) const { return (mask & phase) != 0; }
+  bool exchanges() const { return (mask & PB_PHASE_ALL) != 0; }  // any phase beyond PREPARE
+  bool all() const { return (mask & PB_PHASE_ALL) == PB_PHASE_ALL; }
   void post(const pb_xchg* x, int flag, const uint32_t* counts, cudaStream_t st, bool wait_peers = true) const {
-    if (mask == PB_PHASE_ALL && wait_peers) launch_signal_wait(x->d, flag, counts, st);
+    if (all() && wait_peers) launch_signal_wait(x->d, flag, counts, st);
     else launch_signal(x->d, flag, counts, st);
   }
   void await(const pb_xchg* x, int flag, cudaStream_t st) const {
-    if (mask != PB_PHASE_ALL) launch_wait(x->d, flag, -1, st);
+    if (!all()) launch_wait(x->d, flag, -1, st);
   }
 };
+
+// A SEND after a PREPARE must bring the batch that was prepared (`kind` PREP_SUM or PREP_RAW): refused before anything
+// is enqueued otherwise.
+int check_prepared(const pb_ctx* c, const Phases& ph, int kind, uint32_t n_occ, uint32_t batch) {
+  if (ph.has(PB_PHASE_PREPARE) || !ph.has(PB_PHASE_SEND) || c->prepared != kind) return PB_OK;
+  if (c->prepared_n != n_occ || c->prepared_batch != batch)
+    return fail(PB_ERR_STATE, "PB_PHASE_SEND after PB_PHASE_PREPARE must pass the prepared batch");
+  return PB_OK;
+}
 
 // What a sharded call needs of its exchange: the table's device and dim, and f32 rows where `need_f32_rows` (refused
 // with `f32_message`).  A backward passes its context, whose device it has not checked yet; a forward passes none
@@ -1936,6 +1984,20 @@ int pb_xchg_destroy(pb_xchg* x) {
   return PB_OK;
 }
 
+int pb_xchg_need(pb_xchg* x, pb_ctx* c, uint32_t h_out[1], void* stream) {
+  if (!x || !c || !h_out) return fail(PB_ERR_INVALID, "null argument");
+  if (x->device != c->device) return fail(PB_ERR_INVALID, "context and exchange live on different devices");
+  if (c->prepared == PREP_NONE) return fail(PB_ERR_STATE, "no batch of this context is prepared (PB_PHASE_PREPARE)");
+  DeviceGuard g(x->device);
+  uint32_t n[PB_MAX_RANKS];
+  PB_CUDA(cudaMemcpyAsync(n, c->need, 4 * (size_t)x->d.R, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  PB_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
+  uint32_t most = 0;
+  for (uint32_t q = 0; q < x->d.R; ++q) most = n[q] > most ? n[q] : most;
+  h_out[0] = most;
+  return PB_OK;
+}
+
 int pb_xchg_status(pb_xchg* x, uint32_t h_out[2], void* stream) {
   if (!x || !h_out) return fail(PB_ERR_INVALID, "null argument");
   DeviceGuard g(x->device);
@@ -1950,19 +2012,26 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
   const Phases ph(phases);
   if (!x) return fail(PB_ERR_INVALID, "null argument");
   int rc = check_forward(t, c, d_ids, n_occ, d_row_off, h_slot_occ_off, batch, d_out_f16);
-  if (rc || (rc = check_exchange(t, nullptr, x, d_row_off != nullptr,
-                                 "ragged layouts need an exchange created with f32 rows")))
+  // (a PREPARE alone may meet a ragged batch on an f16 exchange: finding that out is what it is for)
+  if (rc || (rc = check_exchange(t, nullptr, x, d_row_off != nullptr && ph.exchanges(),
+                                 "ragged layouts need an exchange created with f32 rows")) ||
+      (rc = check_prepared(c, ph, PREP_SUM, n_occ, batch)))
     return rc;
   const uint64_t n_out = (uint64_t)c->slots.n_slots * batch;
   // every rank serves lookups whether or not its own batch trains: the shard must be usable (a collective call)
   if ((rc = ready_for_training(t))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
-  if ((rc = ensure_alloc(t))) return rc;
+  if (ph.exchanges() && (rc = ensure_alloc(t))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
+  if (ph.has(PB_PHASE_PREPARE)) {  // requester, local: the dedup and its items per owner
+    prepare_batch(t, c, sl, d_ids, n_occ, batch, st);
+    PB_CUDA(cudaMemsetAsync(c->need, 0, 4 * PB_MAX_RANKS, st));
+    launch_count_owners(false, c->b, c->raw, n_occ, x->d.R, c->need, st);
+  }
   if (ph.has(PB_PHASE_SEND)) {
-    if ((rc = begin_forward(t, c, sl, d_ids, n_occ, training, st))) return rc;
+    if ((rc = begin_forward(t, c, sl, d_ids, n_occ, training, st, c->prepared == PREP_SUM))) return rc;
     launch_route_items(training != 0, sl, c->b, x->d, st);               // requester: signs -> owners' areas
     if (training && c->n_rounds > 1) launch_link_items(sl, c->b, x->d, c->links, st);  // a sign's entries, slot order
     ph.post(x, XC_FLAG_SIGN, c->b.cnt + BC_PEER, st);
@@ -1981,6 +2050,7 @@ int pb_backward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* const* h
                         int32_t* d_slot_status, void* stream, int phases) {
   const Phases ph(phases);
   if (!x) return fail(PB_ERR_INVALID, "null argument");
+  if (ph.has(PB_PHASE_PREPARE)) return fail(PB_ERR_INVALID, "PB_PHASE_PREPARE is a phase of the sharded forwards");
   int rc = check_backward(t, c, h_grads);
   if (rc || (rc = check_exchange(t, c, x, false, nullptr))) return rc;
   uint32_t S = c->slots.n_slots;
@@ -2065,6 +2135,7 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   SlotsDev sl;
   if ((rc = raw_slots(c, n_occ, sl))) return rc;
   c->raw_pending.drop();  // the numbering below replaces the pending batch's
+  c->prepared = PREP_NONE;
   if (training) {
     if ((rc = maybe_evict(t, st))) return rc;
     launch_begin_batch(t->d, c->dev_tick, nullptr, st);
@@ -2134,28 +2205,45 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
   if (!x) return fail(PB_ERR_INVALID, "null argument");
   int rc = check_raw_forward(t, c, d_ids, n_occ, d_row_off, batch, sample_fixed_size, d_table_f16, d_index, d_non_empty,
                              d_sample_id_num, d_counts);
-  if (rc || (rc = check_exchange(t, nullptr, x, true,
-                                 "raw slots need an exchange created with f32 rows (the requester rounds them)")))
+  if (rc || (rc = check_exchange(t, nullptr, x, ph.exchanges(),
+                                 "raw slots need an exchange created with f32 rows (the requester rounds them)")) ||
+      (rc = check_prepared(c, ph, PREP_RAW, n_occ, batch)))
     return rc;
   // every rank serves lookups whether or not its own batch trains: the shard must be usable (a collective call)
   if ((rc = ready_for_training(t))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
-  if ((rc = ensure_alloc(t))) return rc;
+  if (ph.exchanges() && (rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_raw(c))) return rc;
-  if (ph.has(PB_PHASE_SEND)) {
-    SlotsDev sl;
-    if ((rc = raw_slots(c, n_occ, sl))) return rc;
-    c->raw_pending.drop();  // the numbering below replaces the pending batch's
-    if (training) {
-      if ((rc = maybe_evict(t, st))) return rc;
-      launch_begin_batch(t->d, c->dev_tick, nullptr, st);
-    }
+  SlotsDev sl;
+  if ((rc = raw_slots(c, n_occ, sl))) return rc;
+  // the slot's distinct signs numbered, index / non_empty / sample_id_num written: no table state is read
+  auto number = [&]() -> int {
     if (d_row_off && (rc = copy_row_off(c, d_row_off, batch, st))) return rc;
     launch_raw_number(sl, d_ids, n_occ, d_row_off ? c->row_off : nullptr, d_row_off ? c->occ_outrow : nullptr, batch,
                       sample_fixed_size, nullptr, c->raw, (long long*)d_index, (long long*)d_non_empty, d_sample_id_num,
                       st);
     PB_CUDA(cudaMemcpyAsync(d_counts, c->raw.counts, 8, cudaMemcpyDeviceToDevice, st));
+    return PB_OK;
+  };
+  if (ph.has(PB_PHASE_PREPARE)) {  // requester, local: the numbering and its distinct signs per owner
+    c->raw_pending.drop();  // the numbering below replaces the pending batch's
+    if ((rc = number())) return rc;
+    PB_CUDA(cudaMemsetAsync(c->need, 0, 4 * PB_MAX_RANKS, st));
+    launch_count_owners(true, c->b, c->raw, n_occ, x->d.R, c->need, st);
+    c->prepared = PREP_RAW;
+    c->prepared_n = n_occ;
+    c->prepared_batch = batch;
+  }
+  if (ph.has(PB_PHASE_SEND)) {
+    const bool prepared = c->prepared == PREP_RAW;
+    c->prepared = PREP_NONE;
+    if (!prepared) c->raw_pending.drop();
+    if (training) {
+      if ((rc = maybe_evict(t, st))) return rc;
+      launch_begin_batch(t->d, c->dev_tick, nullptr, st);
+    }
+    if (!prepared && (rc = number())) return rc;
     PB_CUDA(cudaMemsetAsync(c->raw.peer, 0, 4 * PB_MAX_RANKS, st));
     launch_raw_route(c->raw, n_occ, x->d, st);  // requester: distinct signs -> owners' areas
     ph.post(x, XC_FLAG_SIGN, c->raw.peer, st);
@@ -2174,6 +2262,7 @@ int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_gr
                             int32_t* d_status, void* stream, int phases) {
   const Phases ph(phases);
   if (!t || !c || !x) return fail(PB_ERR_INVALID, "null argument");
+  if (ph.has(PB_PHASE_PREPARE)) return fail(PB_ERR_INVALID, "PB_PHASE_PREPARE is a phase of the sharded forwards");
   if (!c->has_slots || c->slots.n_slots != 1) return fail(PB_ERR_STATE, "a raw context serves exactly one slot (pb_ctx_set_slots)");
   int rc = check_exchange(t, c, x, false, nullptr);
   if (rc || (rc = check_raw_backward(t, c, d_grad))) return rc;

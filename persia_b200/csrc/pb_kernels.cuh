@@ -259,6 +259,10 @@ void launch_raw_number(const SlotsDev& sl, const uint64_t* ids, uint32_t n, cons
                        const uint32_t* occ_sample, uint32_t batch, uint32_t fixed, const uint32_t* occ_cell,
                        const RawWork& w, long long* index, long long* non_empty, uint32_t* sample_id_num,
                        cudaStream_t st);
+// pb_shard.cu, PB_PHASE_PREPARE: need[q] += the prepared batch's distinct items owned by q (the dedup's items of `b`, or
+// the raw numbering's distinct signs of `w` when raw; n: worst-case U)
+void launch_count_owners(bool raw, const BatchDev& b, const RawWork& w, uint32_t n, uint32_t R, uint32_t* need,
+                         cudaStream_t st);
 // pb_shard.cu, raw slot over R shards: requester's route, table fill and gradient send (n: worst-case U)
 void launch_raw_route(const RawWork& w, uint32_t n, const XchgDev& x, cudaStream_t st);
 void launch_raw_fill(const RawWork& w, uint32_t n, uint32_t dim, const XchgDev& x, void* table_f16, cudaStream_t st);

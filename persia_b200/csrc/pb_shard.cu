@@ -100,6 +100,42 @@ __global__ void __launch_bounds__(256) k_route_items(SlotsDev sl, BatchDev b, Xc
 }
 
 // ------------------------------------------------------------------------------------------------
+// requester, PB_PHASE_PREPARE: how many of the batch's distinct items go to each owner — what `cap` must cover — read
+// from the context alone (the dedup's set, or the raw numbering's), before anything is sent.  Counted per block in
+// shared memory, one global atomic per block and owner.
+// ------------------------------------------------------------------------------------------------
+template <bool RAW>
+__global__ void __launch_bounds__(256) k_count_owners(BatchDev b, RawWork w, uint32_t R, uint32_t* __restrict__ need) {
+  __shared__ uint32_t s_n[PB_MAX_RANKS];
+  if (threadIdx.x < PB_MAX_RANKS) s_n[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t n_items = RAW ? w.counts[0] : b.cnt[BC_ITEMS];
+  for (uint32_t u = blockIdx.x * blockDim.x + threadIdx.x; u < n_items; u += gridDim.x * blockDim.x) {
+    uint64_t sign;
+    if (RAW) {
+      sign = w.set[w.distinct_cell[u]].key;  // (as k_raw_route reads it)
+    } else {
+      const uint32_t cell = b.item_cell[u];  // (as k_route_items reads it)
+      const uint4 lo = *reinterpret_cast<const uint4*>(&b.set[cell]);
+      const uint4 hi = *(reinterpret_cast<const uint4*>(&b.set[cell]) + 1);
+      sign = (hi.w >> 31) ? KEY_EMPTY : ((uint64_t)lo.x | ((uint64_t)lo.y << 32));
+    }
+    atomicAdd(&s_n[(uint32_t)(farmhash64_u64(sign) % R)], 1u);  // sign_to_shard_modulo, mod.rs:341-345
+  }
+  __syncthreads();
+  if (threadIdx.x < R && s_n[threadIdx.x]) atomicAdd(&need[threadIdx.x], s_n[threadIdx.x]);
+}
+
+void launch_count_owners(bool raw, const BatchDev& b, const RawWork& w, uint32_t n, uint32_t R, uint32_t* need,
+                         cudaStream_t st) {
+  if (!n) return;
+  const uint32_t full = cdiv(n, 256);  // worst case U = N; the blocks stride over the items
+  const uint32_t grid = full < PB_NUM_SMS * 4u ? full : PB_NUM_SMS * 4u;
+  if (raw) PB_LAUNCH_F(FAM_ROUTE, k_count_owners<true>, grid, 256, 0, st, b, w, R, need);
+  else PB_LAUNCH_F(FAM_ROUTE, k_count_owners<false>, grid, 256, 0, st, b, w, R, need);
+}
+
+// ------------------------------------------------------------------------------------------------
 // requester, forward, slots sharing a feature group (launched only then): a sign that several slots of one group hold
 // is one entry per slot in its owner's request, and the reference steps them one after another in slot order
 // (mod.rs:703-872).  Every routed item looks for its sign in the regions of the other slots of its group, nearest

@@ -12,7 +12,7 @@ SO_PATH = os.environ.get("PERSIA_B200_LIB") or os.path.join(_HERE, "libpersia_b2
 PB_MAX_SLOTS = 128
 OPT_SGD, OPT_ADAGRAD, OPT_ADAGRAD_VW, OPT_ADAM = 0, 1, 2, 3
 
-PHASE_SEND, PHASE_SERVE, PHASE_FINISH, PHASE_ALL = 1, 2, 4, 7
+PHASE_SEND, PHASE_SERVE, PHASE_FINISH, PHASE_ALL, PHASE_PREPARE = 1, 2, 4, 7, 8
 PB_OK, PB_ERR_INVALID, PB_ERR_CUDA, PB_ERR_STATE, PB_ERR_CAPACITY, PB_ERR_BATCH, PB_ERR_FORMAT = 0, -1, -2, -3, -4, -5, -6
 
 
@@ -102,6 +102,7 @@ SYMBOLS = {
     "pb_xchg_create": (_i32, [_i32, _u32, _u32, _u32, _u32, _i32, C.POINTER(_u64), C.POINTER(_vp)]),
     "pb_xchg_destroy": (_i32, [_vp]),
     "pb_xchg_status": (_i32, [_vp, C.POINTER(_u32 * 2), _vp]),
+    "pb_xchg_need": (_i32, [_vp, _vp, C.POINTER(_u32 * 1), _vp]),
     "pb_forward_sharded": (_i32, [_vp, _vp, _vp, _vp, _u32, _vp, C.POINTER(_u32), _u32, _i32, _vp, _vp, _i32]),
     "pb_backward_sharded": (_i32, [_vp, _vp, _vp, C.POINTER(_vp), _i32, C.POINTER(C.c_float), _vp, _vp, _i32]),
     "pb_forward_raw_sharded": (_i32, [_vp, _vp, _vp, _vp, _u32, _vp, _u32, _u32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32]),

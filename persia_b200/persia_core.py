@@ -15,7 +15,9 @@ feature group (each rank's entries of a shared sign are applied in slot order, t
 may not share its feature group with another slot of the batch.
 Their calls are collective, so every rank issues them in one fixed order: the raw slots in batch order, then the
 summation dims in ascending order, in the forward and again in the backward; every batch must carry the same raw
-slots in the same order.  `Forward` prefetches on worker threads with the reference's ordering and
+slots in the same order.  Every step on R GPUs is sized from its own batch (_sharded_step): each worker prepares its
+batch locally (PB_PHASE_PREPARE), one all_reduce(MAX) agrees on every worker's need, and the exchanges that do not cover
+it are replaced before any rank sends; an exchange overflow or a wait that gave up is then an internal error.  `Forward` prefetches on worker threads with the reference's ordering and
 staleness rules (persia_b200/engine.py), `Backward` applies updates in the caller's thread; `to_bytes()` is a private encoding (the speedy wire format is N4); `dump`/`load`
 write and read the reference's `.emb` checkpoint files (persia_b200/checkpoint.py).  With the global config's
 `enable_incremental_update` on a Train job, the signs the tables step are flushed as the reference's `.inc` packets; an
@@ -743,6 +745,7 @@ def _forward_locked(batch, device_id, training):
             _S.raw_order = raw_names
         elif _S.raw_order != raw_names:
             raise RuntimeError("on R GPUs every batch must carry the same raw slots, in the same order")
+    step = _sharded_step(feats, B, training, dev) if sharded else {}
     pending = _Pending()
     by_slot = {}
     raw_out = {}
@@ -752,18 +755,13 @@ def _forward_locked(batch, device_id, training):
             continue
         with _STATE_LOCK:
             g = _S.group(sc.dim)
-        if sharded:  # R GPUs: one request per owner, through the slot's raw worker
+        if sharded:  # R GPUs: one request per owner, through the slot's raw worker (prepared and sized above)
+            wk, kw = step[("raw", n)]
             with g["lock"]:
-                ids, row_off, _ = _flatten([(n, x)], B)
-                wk = _sharded_raw_worker(g, sc, B, ids, row_off, dev)
-                d_ids = torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True)
-                d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
                 with _Sharded(g, wk):
-                    table, index, non_empty, num, counts = wk.forward_raw(d_ids, B, sc.sample_fixed_size, row_off=d_off,
-                                                                          training=training)
-                if wk.status()[0]:
-                    raise RuntimeError("a batch requested more distinct signs of one shard than the exchange holds: raise "
-                                       "PERSIA_B200_XCHG_CAP")
+                    table, index, non_empty, num, counts = wk.forward_raw(kw["ids"], B, sc.sample_fixed_size,
+                                                                          row_off=kw["row_off"], training=training)
+                _check_exchange(wk)
                 U, ne = counts.tolist()
             raw_out[n] = (Tensor(table[:U + 1], n), Tensor(index, f"{n}_index"),
                           Tensor(non_empty[:ne], f"{n}_non_empty_index"), num.tolist())
@@ -796,32 +794,25 @@ def _forward_locked(batch, device_id, training):
         dim_part = [(n, x) for n, x in feats if _S.by_name[n].dim == dim and _S.by_name[n].embedding_summation]
         with _STATE_LOCK:
             g = _S.group(dim)
-        if sharded and g.setdefault("names", tuple(n for n, _ in dim_part)) != tuple(n for n, _ in dim_part):
-            raise RuntimeError("on R GPUs every batch must carry the same summation slots of a dim, in the same order")
         for k, chunk in enumerate(slot_chunks([_S.by_name[n].index_prefix for n, _ in dim_part])):
             part = [dim_part[i] for i in chunk]
             names = [n for n, _ in part]
             key = tuple(names)
-            pool = g["ctx"].setdefault(key, [])
-            ids, row_off, slot_off = _flatten(part, B)
-            slots = [_S.by_name[n] for n in names]
-            if sharded:  # R GPUs: the embedding worker's fan-out runs inside the chunk's sharded worker
+            if sharded:  # R GPUs: the embedding worker's fan-out runs inside the chunk's sharded worker (sized above)
+                wk, kw = step[(dim, k)]
                 with g["lock"]:
-                    d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
-                    if len(g.get("workers", ())) <= k and any(sc.hash_stack_rounds > 0 for sc in slots):
-                        ids = d_ids.cpu().numpy().view(np.uint64)  # (the first batch sizes the exchange from its keys)
-                    wk = _sharded_worker(g, k, dim, names, B, ids, row_off, slot_off, dev)
-                    d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
                     with _Sharded(g, wk):
-                        out = wk.forward(d_ids, B, training=training, row_off=d_off, slot_occ_off=slot_off)
-                    if wk.status()[0]:
-                        raise RuntimeError("a batch requested more distinct signs of one shard than the exchange holds: "
-                                           "raise PERSIA_B200_XCHG_CAP")
+                        out = wk.forward(kw["ids"], B, training=training, row_off=kw["row_off"],
+                                         slot_occ_off=kw["slot_occ_off"])
+                    _check_exchange(wk)
                 for i, n in enumerate(names):
                     by_slot[n] = out[i]
                 if training:
                     pending.parts.append((g, None, names, False, wk))
                 continue
+            pool = g["ctx"].setdefault(key, [])
+            ids, row_off, slot_off = _flatten(part, B)
+            slots = [_S.by_name[n] for n in names]
             with g["lock"]:
                 d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
                 if pool and pool[-1]._cap >= d_ids.numel():
@@ -844,6 +835,88 @@ def _forward_locked(batch, device_id, training):
     to_dev = lambda items: [Tensor(torch.from_numpy(a).to(dev), n) for n, a in items]  # noqa: E731
     return PersiaTrainingBatch(to_dev(batch.non_id_type_features), emb, to_dev(batch.labels), batch.meta_data,
                                pending if training else None)
+
+
+def _sharded_step(feats, B, training, dev):
+    """R GPUs: sizes this step's exchanges from its own batch, agreed by every rank before any rank sends.  Every worker
+    the step calls is prepared (its batch context grown if need be, the batch deduplicated: local work) in the
+    collective order — the raw slots in batch order, then the summation dims ascending, chunk by chunk — and then
+    _agree_and_resize sizes them all with one all-reduce.  Returns {("raw", name) | (dim, chunk): (worker, the
+    forward's arguments)}.  PERSIA_B200_XCHG_CAP and PERSIA_B200_MAX_BATCH size a worker's first exchange and
+    context only."""
+    import torch
+
+    plan, step = [], {}
+
+    def add(key, g, wk, need, **kw):
+        plan.append((g, wk, need))
+        step[key] = (wk, kw)
+
+    for n, x in feats:
+        sc = _S.by_name[n]
+        if sc.embedding_summation:
+            continue
+        with _STATE_LOCK:
+            g = _S.group(sc.dim)
+        with g["lock"]:
+            ids, row_off, _ = _flatten([(n, x)], B)
+            wk = _sharded_raw_worker(g, sc, B, ids, row_off, dev)
+            d_ids = torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True)
+            d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
+            need = wk.prepare_raw(d_ids, B, sc.sample_fixed_size, row_off=d_off, training=training)
+        add(("raw", n), g, wk, need, ids=d_ids, row_off=d_off)
+    for dim in sorted({_S.by_name[n].dim for n, _ in feats if _S.by_name[n].embedding_summation}):
+        dim_part = [(n, x) for n, x in feats if _S.by_name[n].dim == dim and _S.by_name[n].embedding_summation]
+        with _STATE_LOCK:
+            g = _S.group(dim)
+        if g.setdefault("names", tuple(n for n, _ in dim_part)) != tuple(n for n, _ in dim_part):
+            raise RuntimeError("on R GPUs every batch must carry the same summation slots of a dim, in the same order")
+        for k, chunk in enumerate(slot_chunks([_S.by_name[n].index_prefix for n, _ in dim_part])):
+            part = [dim_part[i] for i in chunk]
+            names = [n for n, _ in part]
+            ids, row_off, slot_off = _flatten(part, B)
+            slots = [_S.by_name[n] for n in names]
+            with g["lock"]:
+                d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
+                if len(g.get("workers", ())) <= k and any(sc.hash_stack_rounds > 0 for sc in slots):
+                    ids = d_ids.cpu().numpy().view(np.uint64)  # (the first batch sizes the exchange from its keys)
+                wk = _sharded_worker(g, k, dim, names, B, ids, row_off, slot_off, dev)
+                d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
+                need = wk.prepare(d_ids, B, row_off=d_off, slot_occ_off=slot_off, training=training)
+            add((dim, k), g, wk, need, ids=d_ids, row_off=d_off, slot_occ_off=slot_off)
+    _agree_and_resize(plan, dev)
+    return step
+
+
+def _agree_and_resize(plan, dev):
+    """plan: [(group, worker, (need, rows_f32))] of one step, in the collective order.  Every rank's needs are packed into
+    one tensor and reduced by ONE all_reduce(MAX), so every rank gets the same agreed (need, rows_f32) per worker; then,
+    in that order, each worker resizes where the agreed need exceeds its exchange (a collective of its own, which every
+    rank enters alike: the decision depends only on agreed values and the exchange every rank shares).  Returns the
+    agreed pairs."""
+    import torch
+    import torch.distributed as dist
+
+    if not plan:
+        return []
+    packed = [v for _, _, (need, f32) in plan for v in (int(need), int(bool(f32)))]
+    t = torch.tensor(packed, dtype=torch.int64, device=dev if dist.get_backend() == "nccl" else "cpu")
+    dist.all_reduce(t, op=dist.ReduceOp.MAX)
+    v = t.tolist()
+    agreed = [(v[2 * i], bool(v[2 * i + 1])) for i in range(len(plan))]
+    for (g, wk, _), (need, f32) in zip(plan, agreed):
+        with g["lock"]:
+            wk.resize(need, f32)
+    return agreed
+
+
+def _check_exchange(wk):
+    """After a sharded forward: a step sized by _agree_and_resize never overflows its exchange and never waits in vain,
+    so either status flag is an internal error."""
+    overflowed, gave_up = wk.status()
+    if overflowed or gave_up:
+        raise RuntimeError("internal error in the sharded exchange: " + ("a batch overflowed the size every rank agreed on"
+                           if overflowed else "a wait for a peer gave up"))
 
 
 def _stage(batch):

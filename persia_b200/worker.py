@@ -70,11 +70,21 @@ class ShardedEmbeddingWorker:
             shard.configure(**(hyper or {}))
         assert shard.dim == dim, "the shard holds another embedding dim"
         self.shard = shard
-        n = n_slots * max_batch * max_ids_per_sample
-        self.ctx = SH.BatchContext(n, n_slots * max_batch, prefixes, sqrt_scaling, prefix_bit, self.device)
-        bases = (C.c_uint64 * world)(*[int(p) for p in peer_bases])
+        self._ctx_args = (prefixes, sqrt_scaling, prefix_bit)
+        self._new_ctx(n_slots * max_batch * max_ids_per_sample, n_slots * max_batch)
+        self.rows_f32 = bool(rows_f32)
+        self.h = None
+        self._create_xchg(self.cap, self.rows_f32, peer_bases)
+
+    def _new_ctx(self, max_occurrences, max_out_rows):
+        self.ctx = SH.BatchContext(max_occurrences, max_out_rows, *self._ctx_args, self.device)
+        self.ctx_occ, self.ctx_rows = int(max_occurrences), int(max_out_rows)
+
+    def _create_xchg(self, cap, rows_f32, peer_bases):
+        bases = (C.c_uint64 * self.R)(*[int(p) for p in peer_bases])
         h = C.c_void_p()
-        N.check(self.lib.pb_xchg_create(self.device.index or 0, world, rank, self.cap, dim, int(rows_f32), bases, C.byref(h)))
+        N.check(self.lib.pb_xchg_create(self.device.index or 0, self.R, self.rank, int(cap), self.dim, int(rows_f32), bases,
+                                        C.byref(h)))
         self.h = h
 
     # ---- set-up helpers --------------------------------------------------------------------------------------------
@@ -89,28 +99,41 @@ class ShardedEmbeddingWorker:
         """R virtual ranks on one GPU (tests; also a way to exercise the protocol without a multi-GPU box).
         shards: the R ranks' existing EmbeddingShards (e.g. `[w.shard for w in group]` of another group of this dim)."""
         dev = torch.device("cuda", device)
-        nbytes = cls.area_bytes(world, cap, dim, kw.get("rows_f32", False))
-        areas = [torch.zeros(nbytes + 256, dtype=torch.uint8, device=dev) for _ in range(world)]
-        bases = [(a.data_ptr() + 255) // 256 * 256 for a in areas]
-        torch.cuda.synchronize(dev)
+        areas, bases = cls._local_areas(world, cls.area_bytes(world, cap, dim, kw.get("rows_f32", False)), dev)
         return [cls(n_slots, dim, prefixes, capacity, dev, r, world, cap, areas[r], bases, optimizer,
                     stream=torch.cuda.Stream(device=dev), shard=shards[r] if shards else None, **kw)
                 for r in range(world)]
+
+    @staticmethod
+    def _local_areas(world, nbytes, dev):
+        """The zeroed receive areas of `world` virtual ranks on one GPU, in plain device memory, and their bases."""
+        areas = [torch.zeros(nbytes + 256, dtype=torch.uint8, device=dev) for _ in range(world)]
+        torch.cuda.synchronize(dev)
+        return areas, [(a.data_ptr() + 255) // 256 * 256 for a in areas]
 
     @classmethod
     def distributed(cls, n_slots, dim, prefixes, capacity, cap, optimizer, device, group=None, **kw):
         """One process per GPU: the receive areas live in torch symmetric memory (every peer's area mapped here)."""
         import torch.distributed as dist
-        import torch.distributed._symmetric_memory as symm
 
         grp = group if group is not None else dist.group.WORLD
         world, rank = dist.get_world_size(grp), dist.get_rank(grp)
         dev = device if isinstance(device, torch.device) else torch.device("cuda", device)
-        nbytes = cls.area_bytes(world, cap, dim, kw.get("rows_f32", False))
-        if world == 1:
+        area, bases = cls._symmetric_area(cls.area_bytes(world, cap, dim, kw.get("rows_f32", False)), dev, grp)
+        w = cls(n_slots, dim, prefixes, capacity, dev, rank, world, cap, area, bases, optimizer, **kw)
+        w.group = grp
+        return w
+
+    @staticmethod
+    def _symmetric_area(nbytes, dev, grp):
+        """A zeroed receive area of nbytes in symmetric memory and every rank's base (collective over grp); a plain
+        device area when the group has one rank."""
+        import torch.distributed as dist
+        import torch.distributed._symmetric_memory as symm
+
+        if dist.get_world_size(grp) == 1:
             area = torch.zeros(nbytes + 256, dtype=torch.uint8, device=dev)
-            bases = [(area.data_ptr() + 255) // 256 * 256]
-            return cls(n_slots, dim, prefixes, capacity, dev, 0, 1, cap, area, bases, optimizer, **kw)
+            return area, [(area.data_ptr() + 255) // 256 * 256]
         area = symm.empty(nbytes, dtype=torch.uint8, device=dev)
         area.zero_()
         hdl = symm.rendezvous(area, grp)
@@ -118,9 +141,7 @@ class ShardedEmbeddingWorker:
         assert all(b % 256 == 0 for b in bases)
         torch.cuda.synchronize(dev)
         dist.barrier(group=grp)
-        w = cls(n_slots, dim, prefixes, capacity, dev, rank, world, cap, (area, hdl), bases, optimizer, **kw)
-        w.group = grp
-        return w
+        return (area, hdl), bases
 
     @staticmethod
     def calibrate_cap(id_batches, batch, prefixes, world, margin=1.15, extra=64, group=None):
@@ -216,6 +237,103 @@ class ShardedEmbeddingWorker:
             w.backward(grads[r], scales, want_status, phases=ph, status=sts[r])
         return sts
 
+    # ---- sizing each step from its own batch (PB_PHASE_PREPARE, pb_xchg_need) ---------------------------------------
+    def _fit_ctx(self, n_occ, rows):
+        """Grows the batch context when a batch of n_occ ids in `rows` output rows does not fit: with
+        persia_core.ctx_occurrences' headroom and 2^24 limit (local to this rank; the context holds one batch)."""
+        if n_occ <= self.ctx_occ and rows <= self.ctx_rows:
+            return
+        from .persia_core import ctx_occurrences
+
+        occ = max(ctx_occurrences(n_occ, rows), self.ctx_occ)
+        self._torch_stream().synchronize()
+        self.ctx.close()
+        self._new_ctx(occ, max(2 * rows, 1024, self.ctx_rows))
+
+    def _need(self):
+        out = (C.c_uint32 * 1)()
+        N.check(self.lib.pb_xchg_need(self.h, self.ctx.h, out, self._st()))
+        return int(out[0])
+
+    def prepare(self, ids, batch, row_off=None, slot_occ_off=None, training=True):
+        """Local part of a forward, run before it: grows this rank's batch context if the batch needs it, then
+        deduplicates the batch (PB_PHASE_PREPARE: no table state, no peer).  Returns (need, rows_f32): the most distinct
+        items it sends one owner, and whether it needs f32 rows (ragged).  The forward of the same batch follows, after
+        every rank has agreed on the exchange's size (resize)."""
+        ids = SH._as_i64_bits(ids)
+        self._fit_ctx(ids.numel(), self.S * batch)
+        if slot_occ_off is None:
+            slot_occ_off = [s * batch for s in range(self.S + 1)]
+        if getattr(self, "_dummy_out", None) is None:  # (PREPARE writes no output; the call wants an aligned pointer)
+            self._dummy_out = torch.empty(8, dtype=torch.float16, device=self.device)
+        N.check(self.lib.pb_forward_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), ids.numel(), SH._ptr(row_off),
+                                            SH._slot_offsets(slot_occ_off, self.S), int(batch), int(training),
+                                            SH._ptr(self._dummy_out), self._st(), N.PHASE_PREPARE))
+        return self._need(), row_off is not None
+
+    @staticmethod
+    def grown_cap(need, cap):
+        """The cap an exchange of `cap` slots grows to for an agreed need: never smaller, and with headroom over the
+        need (1.5x + 1024, a multiple of 8) so that drift does not resize every step."""
+        return cap if need <= cap else max(cap, (need * 3 // 2 + 1024 + 7) // 8 * 8)
+
+    def _resize_to(self, need, rows_f32):
+        """(cap, rows_f32) of the exchange this worker needs for the agreed (need, rows_f32), or None when its own
+        suffices.  Every rank holds the same exchange geometry, so every rank reaches the same answer."""
+        cap, f32 = self.grown_cap(int(need), self.cap), self.rows_f32 or bool(rows_f32)
+        return None if (cap, f32) == (self.cap, self.rows_f32) else (cap, f32)
+
+    def _replace_xchg(self, cap, rows_f32, area, bases):
+        """The exchange replaced by one of (cap, rows_f32) over `area` (include/persia_b200.h, pb_xchg_destroy): the
+        table, its Adam powers and its incremental set stay; a prepared batch stays in the context."""
+        self._torch_stream().synchronize()
+        old = self.h
+        self._create_xchg(cap, rows_f32, bases)  # (sets self.h once created: a failure leaves the old one in place)
+        self.lib.pb_xchg_destroy(old)
+        self.cap, self.rows_f32, self.area = int(cap), bool(rows_f32), area
+
+    def resize(self, need, rows_f32):
+        """Collective over the worker's group: every rank passes the same agreed (need, rows_f32).  When this exchange
+        does not cover them, every rank drains its stream and passes a barrier (no peer still writes the old areas),
+        then a new symmetric area is rendezvoused and a new exchange created; the old area is released after that.
+        Grows only.  Returns whether it resized."""
+        to = self._resize_to(need, rows_f32)
+        if to is None:
+            return False
+        import torch.distributed as dist
+
+        grp = getattr(self, "group", None)
+        if grp is None:
+            assert self.R == 1, "a virtual rank resizes through group_resize"
+            area, bases = self._local_areas(1, self.area_bytes(1, to[0], self.dim, to[1]), self.device)
+            self._replace_xchg(*to, area[0], bases)
+            return True
+        self._torch_stream().synchronize()
+        dist.barrier(group=grp)
+        area, bases = self._symmetric_area(self.area_bytes(self.R, to[0], self.dim, to[1]), self.device, grp)
+        self._replace_xchg(*to, area, bases)
+        return True
+
+    @staticmethod
+    def group_prepare(workers, ids, batch, training=True, row_offs=None, slot_occ_offs=None):
+        """Virtual ranks of one GPU: every rank's prepare, and their agreement (the max over the ranks, as the
+        all-reduce of persia_core computes it over processes)."""
+        needs = [w.prepare(ids[r], batch, row_offs[r] if row_offs else None, slot_occ_offs[r] if slot_occ_offs else None,
+                           training) for r, w in enumerate(workers)]
+        return max(n for n, _ in needs), any(f for _, f in needs)
+
+    @staticmethod
+    def group_resize(workers, need, rows_f32):
+        """Virtual ranks of one GPU: resize (same rule) with plain device areas for all ranks.  Returns whether it did."""
+        to = workers[0]._resize_to(need, rows_f32)
+        if to is None:
+            return False
+        w0 = workers[0]
+        areas, bases = w0._local_areas(len(workers), w0.area_bytes(len(workers), to[0], w0.dim, to[1]), w0.device)
+        for r, w in enumerate(workers):
+            w._replace_xchg(*to, areas[r], bases)
+        return True
+
     def status(self):
         """(overflowed, wait_gave_up) — host sync."""
         out = SH._read_block(XCHG_STATUS_FIELDS, lambda out: self.lib.pb_xchg_status(self.h, out, self._st()), C.c_uint32)
@@ -260,8 +378,10 @@ class ShardedRawWorker(ShardedEmbeddingWorker):
         captured calls reuse them)."""
         ids = SH._as_i64_bits(ids)
         n, fixed = ids.numel(), int(sample_fixed_size)
-        if out is None:
-            out = SH._raw_outputs(n, batch, fixed, self.dim, self.device)
+        if out is None:  # (after prepare_raw: the buffers it numbered the batch into)
+            out = getattr(self, "_prepared_out", None) or SH._raw_outputs(n, batch, fixed, self.dim, self.device)
+        if phases == 0 or phases & N.PHASE_FINISH:
+            self._prepared_out = None
         table, index, non_empty, num, counts = out
         N.check(self.lib.pb_forward_raw_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), n,
                                                 SH._raw_row_off(row_off, batch), int(batch), fixed, int(training),
@@ -277,6 +397,27 @@ class ShardedRawWorker(ShardedEmbeddingWorker):
         N.check(self.lib.pb_backward_raw_sharded(self.shard.h, self.ctx.h, self.h, ptr, int(bool(is_f16)), float(scale),
                                                  SH._ptr(status), self._st(), int(phases)))
         return status
+
+    def prepare_raw(self, ids, batch, sample_fixed_size, row_off=None, training=True):
+        """prepare() of a raw slot: grows the context if needed, numbers the slot's distinct signs (PB_PHASE_PREPARE) into
+        the output buffers the next forward_raw of this batch takes over.  Returns (need, True): raw exchanges carry f32
+        rows always."""
+        ids = SH._as_i64_bits(ids)
+        n, fixed = ids.numel(), int(sample_fixed_size)
+        self._fit_ctx(n, batch)
+        out = SH._raw_outputs(n, batch, fixed, self.dim, self.device)
+        N.check(self.lib.pb_forward_raw_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), n,
+                                                SH._raw_row_off(row_off, batch), int(batch), fixed, int(training),
+                                                *map(SH._ptr, out), self._st(), N.PHASE_PREPARE))
+        self._prepared_out = out
+        return self._need(), True
+
+    @staticmethod
+    def group_prepare_raw(workers, ids, batch, sample_fixed_size, training=True, row_offs=None):
+        """Virtual ranks of one GPU: every rank's prepare_raw, and their agreement (max over the ranks)."""
+        needs = [w.prepare_raw(ids[r], batch, sample_fixed_size, row_offs[r] if row_offs else None, training)
+                 for r, w in enumerate(workers)]
+        return max(n for n, _ in needs), True
 
     @staticmethod
     def group_forward_raw(workers, ids, batch, sample_fixed_size, training=True, row_offs=None, outs=None):
