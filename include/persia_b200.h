@@ -57,7 +57,8 @@ typedef enum {
   PB_ERR_STATE = -3,     /* optimizer / hyper-parameters not configured (reference: OptimizerNotFoundError, NotConfiguredError) */
   PB_ERR_CAPACITY = -4,  /* workspace too small for this batch */
   PB_ERR_BATCH = -5,     /* batch size > 65535 (persia-common/src/lib.rs:49-51 panics) */
-  PB_ERR_FORMAT = -6     /* malformed checkpoint image; pb_last_error() = "ExceptionType: message" (pb_image_index) */
+  PB_ERR_FORMAT = -6     /* malformed checkpoint image or packet; pb_last_error() = "ExceptionType: message"
+                            (pb_image_index, pb_image_packet) */
 } pb_status;
 
 typedef enum { PB_OPT_SGD = 0, PB_OPT_ADAGRAD = 1, PB_OPT_ADAGRAD_VW = 2, PB_OPT_ADAM = 3 } pb_optim_kind;
@@ -302,6 +303,18 @@ int pb_image_index(pb_image* im, const void* h_image, uint64_t nbytes, uint32_t 
 int pb_image_window(pb_image* im, const void* h_window, uint64_t node0, uint32_t n, uint64_t n_total, uint32_t entry_len,
                     uint64_t dim, uint32_t R, uint32_t rank, uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows,
                     int* h_writer, void* stream);
+/* One incremental-update packet (persia_b200/incremental.py): count u32 | entry x count | unix seconds u64, each entry
+ * len u32 | f32 x len | dim u64 | sign u64, lying in pinned host memory (as pb_image_index's image).  Its list positions
+ * are the packet's entry order.  Checks, and their first failure, are decode_packet's: PB_ERR_FORMAT with
+ * pb_last_error() = "ValueError: truncated packet" / "...: truncated packet: entry" / "...: packet length does not
+ * match its entries".  Then the selection (farmhash64(sign) % R == rank) and the per-(dim, entry length) summary as
+ * pb_image_index; *h_timestamp = the packet's timestamp.  Synchronises `stream` once; touches no table.  A well-formed
+ * packet of more than 32 dims or 64 (dim, entry length) pairs gives PB_ERR_CAPACITY (nothing of it may be inserted).
+ * A packet whose size is that of `count` entries of its first entry's length (every packet this library's flushes
+ * write for one dim) is read at arithmetic offsets, each entry's `len` checked on the device; any other packet, or one
+ * that fails that check, takes one sequential host pass over its length fields (and then twice the synchronisation). */
+int pb_image_packet(pb_image* im, const void* h_packet, uint64_t nbytes, uint32_t R, uint32_t rank,
+                    uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows, uint64_t* h_timestamp, void* stream);
 /* set_embedding of the indexed image's selected dim-`dim` entries [lo, hi) (counted in list order, or from the end of
  * the list when newest_first, and offered in that order) into `t`, whose entry length they must have; hi - lo at most
  * max_chunk.  No host synchronisation. */

@@ -715,8 +715,8 @@ class _Pinned:
 
 
 class _Image:
-    """A pb_image: one list image (or writer-layout window) in pinned host memory, indexed, selected and inserted on
-    the device."""
+    """A pb_image: one list image (or writer-layout window, or incremental-update packet) in pinned host memory,
+    indexed, selected and inserted on the device."""
 
     def __init__(self, device, chunk):
         import ctypes as C
@@ -732,16 +732,28 @@ class _Image:
     def _summary(self, n):
         return [(int(self._rows[3 * i]), int(self._rows[3 * i + 1]), int(self._rows[3 * i + 2])) for i in range(n)]
 
-    def index(self, buf, nbytes, p_lo, p_hi, R, rank, stream):
-        C = self.C
-        rows = C.c_uint32()
-        rc = self.lib.pb_image_index(self.h, C.c_void_p(buf.data_ptr()), int(nbytes), int(p_lo), int(p_hi), R, rank,
-                                     self._rows, LOAD_SUMMARY_ROWS, C.byref(rows), C.c_void_p(stream.cuda_stream))
-        if rc == self.N.PB_ERR_FORMAT:  # decode_list's exception
+    def _check(self, rc):
+        if rc == self.N.PB_ERR_FORMAT:  # decode_list's (decode_packet's) exception
             kind, msg = self.lib.pb_last_error().decode().split(": ", 1)
             raise _FORMAT_ERRORS[kind](msg)
         self.N.check(rc)
+
+    def index(self, buf, nbytes, p_lo, p_hi, R, rank, stream):
+        C = self.C
+        rows = C.c_uint32()
+        self._check(self.lib.pb_image_index(self.h, C.c_void_p(buf.data_ptr()), int(nbytes), int(p_lo), int(p_hi), R,
+                                            rank, self._rows, LOAD_SUMMARY_ROWS, C.byref(rows),
+                                            C.c_void_p(stream.cuda_stream)))
         return self._summary(rows.value)
+
+    def packet(self, buf, nbytes, R, rank, stream):
+        """An incremental-update packet's (summary, timestamp); decode_packet's exception when it is malformed."""
+        C = self.C
+        rows, ts = C.c_uint32(), C.c_uint64()
+        self._check(self.lib.pb_image_packet(self.h, C.c_void_p(buf.data_ptr()), int(nbytes), R, rank, self._rows,
+                                             LOAD_SUMMARY_ROWS, C.byref(rows), C.byref(ts),
+                                             C.c_void_p(stream.cuda_stream)))
+        return self._summary(rows.value), int(ts.value)
 
     def window(self, buf, node0, n, n_total, entry_len, dim, R, rank, stream):
         """The window's summary, or None when a node of it is not in the writer layout."""

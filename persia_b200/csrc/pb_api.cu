@@ -1302,8 +1302,8 @@ int image_room(pb_image* im, uint32_t n, cudaStream_t st) {
   return PB_OK;
 }
 
-// the selection and per-dim summary of im->L (positions set up by the caller); one host synchronisation
-int image_select(pb_image* im, uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows, cudaStream_t st) {
+// the selection of im->L (positions set up by the caller), its flags and summary read back; one host synchronisation
+int image_select(pb_image* im, cudaStream_t st) {
   LoadImg& L = im->L;
   L.slot = im->slot;
   PB_CUDA(cudaMemsetAsync(L.dims, 0xFF, sizeof(unsigned long long) * (LOAD_DIMS + LOAD_PAIRS), st));
@@ -1316,6 +1316,11 @@ int image_select(pb_image* im, uint64_t* h_summary, uint32_t max_rows, uint32_t*
   PB_CUDA(cudaStreamSynchronize(st));
   im->sel_slot = -1;
   im->indexed = true;
+  return PB_OK;
+}
+
+// the per-dim summary of the selection image_select made, and staging for its largest insert
+int image_summary(pb_image* im, uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows, cudaStream_t st) {
   if (im->h_flags[LOAD_FLAG_FULL])
     return fail(PB_ERR_INVALID, "a checkpoint file holds more than " + std::to_string(LOAD_DIMS) + " dims or " +
                                     std::to_string(LOAD_PAIRS) + " (dim, entry length) pairs");
@@ -1404,9 +1409,10 @@ int pb_image_index(pb_image* im, const void* h_image, uint64_t nbytes, uint32_t 
   if ((rc = image_device_ptr(h_image, &L.img))) return rc;
   if (n) PB_CUDA(cudaMemcpyAsync(im->off, im->host_off.data(), sizeof(uint64_t) * n, cudaMemcpyHostToDevice, st));
   L.off = im->off;
-  L.nb = 0, L.n = n, L.p_lo = p_lo, L.p_hi = p_hi < n ? p_hi : n;
+  L.nb = 0, L.hdr = LOAD_NODE_HDR, L.n = n, L.p_lo = p_lo, L.p_hi = p_hi < n ? p_hi : n;
   L.node0 = 0, L.n_total = n, L.dim = 0, L.len = 0, L.R = R, L.rank = rank;
-  return image_select(im, h_summary, max_rows, h_rows, st);
+  if ((rc = image_select(im, st))) return rc;
+  return image_summary(im, h_summary, max_rows, h_rows, st);
 }
 
 int pb_image_window(pb_image* im, const void* h_window, uint64_t node0, uint32_t n, uint64_t n_total, uint32_t entry_len,
@@ -1423,17 +1429,69 @@ int pb_image_window(pb_image* im, const void* h_window, uint64_t node0, uint32_t
   LoadImg& L = im->L;
   if ((rc = image_device_ptr(h_window, &L.img))) return rc;
   L.off = nullptr;
-  L.nb = dump_node_bytes(entry_len), L.n = n, L.p_lo = 0, L.p_hi = n;
+  L.nb = dump_node_bytes(entry_len), L.hdr = LOAD_NODE_HDR, L.n = n, L.p_lo = 0, L.p_hi = n;
   L.node0 = node0, L.n_total = n_total, L.dim = dim, L.len = entry_len, L.R = R, L.rank = rank;
-  if ((rc = image_select(im, h_summary, max_rows, h_rows, st))) return rc;
+  if ((rc = image_select(im, st)) || (rc = image_summary(im, h_summary, max_rows, h_rows, st))) return rc;
   *h_writer = im->h_flags[LOAD_FLAG_BAD] ? 0 : 1;
   if (!*h_writer) im->indexed = false;
   return PB_OK;
 }
 
+int pb_image_packet(pb_image* im, const void* h_packet, uint64_t nbytes, uint32_t R, uint32_t rank,
+                    uint64_t* h_summary, uint32_t max_rows, uint32_t* h_rows, uint64_t* h_timestamp, void* stream) {
+  if (!im || !h_packet || !h_summary || !h_rows || !h_timestamp) return fail(PB_ERR_INVALID, "null argument");
+  if (R == 0 || rank >= R) return fail(PB_ERR_INVALID, "rank must be in 0..R-1");
+  DeviceGuard g(im->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  im->indexed = false;
+  const uint8_t* b = static_cast<const uint8_t*>(h_packet);
+  if (nbytes < 12) return fail(PB_ERR_FORMAT, "ValueError: truncated packet");
+  uint32_t count, len0;
+  std::memcpy(&count, b, 4);
+  std::memcpy(&len0, b + 4, 4);
+  LoadImg& L = im->L;
+  const uint8_t* d_packet = nullptr;
+  int rc = image_device_ptr(h_packet, &d_packet);
+  if (rc) return rc;
+  L.hdr = 0, L.node0 = 0, L.dim = 0, L.R = R, L.rank = rank;
+  // uniform: the size of `count` entries of the first one's length (every packet this project writes with one dim)
+  const uint64_t nb = 20 + 4ull * len0;  // (entries of 2^31 bytes or more are errors: packet_index_host)
+  bool arithmetic = count && nb <= INT32_MAX && (nbytes - 12) % nb == 0 && (nbytes - 12) / nb == count;
+  if (arithmetic) {
+    if ((rc = image_room(im, count, st))) return rc;
+    L.img = d_packet + 4, L.off = nullptr, L.nb = nb, L.len = len0;
+    L.n = count, L.p_lo = 0, L.p_hi = count, L.n_total = count;
+    if ((rc = image_select(im, st))) return rc;
+    arithmetic = !im->h_flags[LOAD_FLAG_BAD];  // an entry of another length: the host walk finds out what it is
+  }
+  if (!arithmetic) {
+    im->indexed = false;
+    std::string err;
+    try {
+      if (!packet_index_host(b, nbytes, im->host_off, err)) return fail(PB_ERR_FORMAT, err);
+    } catch (const std::bad_alloc&) {
+      return fail(PB_ERR_CAPACITY, "host memory for the entry offsets of a " + std::to_string(nbytes) + "-byte packet");
+    }
+    const uint32_t n = (uint32_t)im->host_off.size();
+    if ((rc = image_room(im, n, st))) return rc;
+    if (n) PB_CUDA(cudaMemcpyAsync(im->off, im->host_off.data(), sizeof(uint64_t) * n, cudaMemcpyHostToDevice, st));
+    L.img = d_packet, L.off = im->off, L.nb = 0, L.len = 0;
+    L.n = n, L.p_lo = 0, L.p_hi = n, L.n_total = n;
+    if ((rc = image_select(im, st))) return rc;
+  }
+  if (im->h_flags[LOAD_FLAG_FULL]) {
+    im->indexed = false;
+    return fail(PB_ERR_CAPACITY, "an incremental-update packet holds more than " + std::to_string(LOAD_DIMS) +
+                                     " dims or " + std::to_string(LOAD_PAIRS) + " (dim, entry length) pairs");
+  }
+  if ((rc = image_summary(im, h_summary, max_rows, h_rows, st))) return rc;
+  std::memcpy(h_timestamp, b + nbytes - 8, 8);
+  return PB_OK;
+}
+
 int pb_image_insert(pb_image* im, pb_table* t, uint64_t dim, uint32_t lo, uint32_t hi, int newest_first, void* stream) {
   if (!im || !t) return fail(PB_ERR_INVALID, "null argument");
-  if (!im->indexed) return fail(PB_ERR_STATE, "no image indexed: call pb_image_index or pb_image_window first");
+  if (!im->indexed) return fail(PB_ERR_STATE, "no image indexed: call pb_image_index, pb_image_window or pb_image_packet first");
   if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered: entry length unknown");
   uint32_t len = 0;
   pb_table_entry_len(t, &len);

@@ -371,18 +371,22 @@ cudaError_t launch_dump_empty(uint8_t* image, uint64_t max_bytes, unsigned long 
                               cudaStream_t st);
 cudaError_t launch_dump_nodes(const TableDev& t, const TableDev* h, const uint64_t* signs, uint32_t n_list, uint32_t lo,
                               uint32_t n, const DumpWs& w, uint8_t* out, cudaStream_t st);
-// checkpoint loads (pb_load.cu): one list image, read in place (mapped pinned host memory), and its per-dim summary
+// checkpoint loads (pb_load.cu): one list image or incremental-update packet, read in place (mapped pinned host
+// memory), and its per-dim summary
 constexpr uint32_t LOAD_DIMS = 32, LOAD_PAIRS = 64;  // distinct dims, distinct (dim, entry length) pairs of one image
 constexpr uint32_t LOAD_NONE = 0xFF;                  // slot of a position not selected
+constexpr uint32_t LOAD_NODE_HDR = 9;                 // bytes before an entry's `len`: a `.emb` node's next, prev, flag
 enum { LOAD_FLAG_BAD = 0, LOAD_FLAG_FULL, LOAD_FLAGS };
 struct LoadImg {
-  const uint8_t* img;   // device address of the image's bytes (a window: its first node's)
-  const uint64_t* off;  // byte offset of each list position's node; null: a writer-layout window (pos * nb)
-  uint64_t nb;          // writer layout: node bytes
+  const uint8_t* img;   // device address of the image's bytes (a window: its first node's; a packet: its first entry's
+                        // when off is null)
+  const uint64_t* off;  // byte offset of each list position's record; null: arithmetic offsets (pos * nb)
+  uint64_t nb;          // arithmetic offsets: record bytes
+  uint32_t hdr;         // bytes before each record's `len`: LOAD_NODE_HDR (a `.emb` node), 0 (a packet entry)
   uint32_t n;           // list positions
   uint32_t p_lo, p_hi;  // positions offered (the others are not selected)
-  uint64_t node0, n_total, dim;  // writer layout: the window's first node, the file's nodes, its dim
-  uint32_t len;                  // writer layout: its entry length
+  uint64_t node0, n_total, dim;  // writer-layout window (hdr != 0): the window's first node, the file's nodes, its dim
+  uint32_t len;                  // arithmetic offsets: every record's entry length
   uint32_t R, rank;              // selection: farmhash64(sign) % R == rank
   uint8_t* slot;                 // per position: summary slot of its dim, LOAD_NONE = not selected
   unsigned long long* dims;      // LOAD_DIMS, KEY_EMPTY = unused
@@ -391,6 +395,7 @@ struct LoadImg {
   uint32_t* flags;               // LOAD_FLAGS
 };
 bool load_index_host(const uint8_t* image, uint64_t nbytes, std::vector<uint64_t>& pos_off, std::string& err);
+bool packet_index_host(const uint8_t* packet, uint64_t nbytes, std::vector<uint64_t>& pos_off, std::string& err);
 cudaError_t launch_load_select(const LoadImg& L, cudaStream_t st);
 size_t load_list_bytes(uint32_t n);
 cudaError_t launch_load_list(const LoadImg& L, uint32_t slot, void* tmp, size_t tmp_bytes, uint32_t* sel,

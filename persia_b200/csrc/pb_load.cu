@@ -9,6 +9,10 @@
 //                  whose node offsets, links and list order come from one sequential pass on the host
 //                  (load_index_host: 13 bytes read per node and a walk over a 4-byte array), with exactly the checks,
 //                  and the first failure, of checkpoint.decode_list.
+// An incremental-update packet (persia_b200/incremental.py) holds the same entries without a node header (LoadImg.hdr
+// = 0), in packet order from byte 4.  When its size says every entry has the first one's length, offsets are arithmetic
+// and k_load_select checks each entry's `len` on the device; any other packet takes one host pass over its length
+// fields (packet_index_host, with incremental.decode_packet's checks and first failure).
 // Selection (farmhash64(sign) % R == rank, the re-sharding load) and the per-dim counts run on the device.
 #include <thrust/iterator/counting_iterator.h>
 
@@ -56,22 +60,23 @@ __device__ bool count_pair(const LoadImg& L, uint32_t slot, uint32_t len) {
   return false;
 }
 
-// per list position: the writer layout's header checks (window images), the selection, the dim's summary slot
+// per list position: the checks of arithmetic offsets (every record of the one entry length; a writer-layout window's
+// node headers too), the selection, the dim's summary slot
 __global__ void __launch_bounds__(256) k_load_select(LoadImg L) {
   for (uint32_t pos = blockIdx.x * blockDim.x + threadIdx.x; pos < L.n; pos += gridDim.x * blockDim.x) {
     const uint8_t* p = node_at(L, pos);
-    const uint32_t len = ld_u32(p + 9);
+    const uint32_t len = ld_u32(p + L.hdr);
     uint8_t slot = LOAD_NONE;
-    if (!L.off) {  // writer layout: node node0 + pos of n_total, live, of the window's entry length and dim
+    if (!L.off) {  // of the one entry length; a window's node also node0 + pos of n_total, live, of the window's dim
       const uint64_t g = L.node0 + pos;
       const uint32_t next = g + 1 < L.n_total ? (uint32_t)(g + 2) : 0u;
-      if (ld_u32(p) != next || p[8] != 1 || len != L.len || ld_u64(p + 13 + 4ull * L.len) != L.dim) {
+      if (len != L.len || (L.hdr && (ld_u32(p) != next || p[8] != 1 || ld_u64(p + L.hdr + 4 + 4ull * L.len) != L.dim))) {
         atomicOr(&L.flags[LOAD_FLAG_BAD], 1u);
         L.slot[pos] = LOAD_NONE;
         continue;
       }
     }
-    const uint8_t* q = p + 13 + 4ull * len;
+    const uint8_t* q = p + L.hdr + 4 + 4ull * len;
     const uint64_t dim = ld_u64(q), sign = ld_u64(q + 8);
     const bool keep = pos >= L.p_lo && pos < L.p_hi && (L.R <= 1 || farmhash64_u64(sign) % L.R == L.rank);
     if (keep) {
@@ -92,13 +97,13 @@ __global__ void __launch_bounds__(256) k_load_gather(LoadImg L, const uint32_t* 
   for (uint32_t e = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; e < n; e += warps) {
     const uint32_t r = rev ? K - 1 - (lo + e) : lo + e;
     const uint8_t* p = node_at(L, sel[r]);
-    // the entry's floats start at p + 13, at any byte alignment: aligned words, shifted into place
-    const uint8_t* f = p + 13;
+    // the entry's floats start after its `len`, at any byte alignment: aligned words, shifted into place
+    const uint8_t* f = p + L.hdr + 4;
     const uint32_t a = (uint32_t)((uintptr_t)f & 3u);
     const uint32_t* w = reinterpret_cast<const uint32_t*>(f - a);
     float* out = ent + (size_t)e * len;
     for (uint32_t k = lane; k < len; k += 32) {
-      const uint32_t v = a ? __funnelshift_r(w[k], w[k + 1], 8 * a) : w[k];  // (w[k + 1] stays inside the node)
+      const uint32_t v = a ? __funnelshift_r(w[k], w[k + 1], 8 * a) : w[k];  // (w[k + 1] stays inside the record)
       out[k] = __uint_as_float(v);
     }
     if (lane == 0) signs[e] = ld_u64(f + 4ull * len + 8);
@@ -200,6 +205,33 @@ bool load_index_host(const uint8_t* b, uint64_t nbytes, std::vector<uint64_t>& p
   }
   if (cur != 0) return err = "ValueError: broken list: it continues past `count` entries", false;
   if (unused) return err = "ValueError: the list runs through an unused node", false;
+  return true;
+}
+
+// incremental.decode_packet's checks over a whole packet, in its order (its runs of one length fail exactly where their
+// first entry that does not fit with the timestamp after it would); the byte offset of each entry in pos_off
+bool packet_index_host(const uint8_t* b, uint64_t nbytes, std::vector<uint64_t>& pos_off, std::string& err) {
+  if (nbytes < 12) return err = "ValueError: truncated packet", false;
+  uint32_t count;
+  std::memcpy(&count, b, 4);
+  // grown entry by entry: every entry takes at least 20 bytes, so they never outgrow the packet whatever count says
+  pos_off.clear();
+  pos_off.reserve(count < nbytes / 20 ? count : nbytes / 20);
+  uint64_t o = 4;
+  for (uint32_t k = 0; k < count; ++k) {
+    if (nbytes < o + 4) return err = "ValueError: truncated packet: entry", false;
+    uint32_t L;
+    std::memcpy(&L, b + o, 4);
+    // (numpy's own errors for an entry dtype beyond a C int; one of 2^31 bytes or more has a negative itemsize there,
+    // so no run of it fits)
+    if (L > INT32_MAX) return err = "ValueError: invalid shape in fixed-type tuple: dimension does not fit into a C int.", false;
+    if (4ull * L > INT32_MAX)
+      return err = "ValueError: invalid shape in fixed-type tuple: dtype size in bytes must fit into a C int.", false;
+    if (20 + 4ull * L > INT32_MAX || nbytes < o + 28 + 4ull * L) return err = "ValueError: truncated packet: entry", false;
+    pos_off.push_back(o);
+    o += 20 + 4ull * L;
+  }
+  if (o + 8 != nbytes) return err = "ValueError: packet length does not match its entries", false;
   return true;
 }
 

@@ -242,11 +242,15 @@ _INC_FILE = re.compile(r"^(\d+)_(\d+)\.inc$")
 
 class IncrementalLoader:
     """Applies the flushes that appear under `directory` (incremental_dir/s{replica_index}).  apply(signs u64 [n],
-    dims u64 [n], entries list) stores one packet's entries and returns how many it could not store.  A file that cannot
-    be read or applied is logged and counted (failed_files) and the scan goes on, as the reference's scanner does."""
+    dims u64 [n], entries list) stores one packet's entries, decoded here, and returns how many it could not store;
+    apply_file(path), when given instead, reads, decodes and stores one packet file itself (persia_core: on the device)
+    and returns (how many it could not store, how many entries the packet held).  A file that cannot be read or applied is logged and counted (failed_files) and the scan goes
+    on, as the reference's scanner does."""
 
-    def __init__(self, directory, apply, interval=SCAN_INTERVAL_S):
-        self.dir, self.apply, self.interval = directory, apply, interval
+    def __init__(self, directory, apply=None, interval=SCAN_INTERVAL_S, apply_file=None):
+        if (apply is None) == (apply_file is None):
+            raise ValueError("give one of apply and apply_file")
+        self.dir, self.apply, self.apply_file, self.interval = directory, apply, apply_file, interval
         self.seen = set(self._dirs())  # present at start: not applied (lib.rs:324-333)
         self.applied = []
         self.entries_applied = 0
@@ -273,10 +277,14 @@ class IncrementalLoader:
                 files = sorted((int(m.group(2)), f) for f in os.listdir(path) for m in [_INC_FILE.match(f)] if m)
                 for _, f in files:
                     try:
-                        with open(os.path.join(path, f), "rb") as fh:
-                            signs, dims, entries, _ = decode_packet(fh.read())
-                        self.entries_dropped += int(self.apply(signs, dims, entries))
-                        self.entries_applied += signs.size
+                        if self.apply_file is not None:
+                            dropped, n = (int(x) for x in self.apply_file(os.path.join(path, f)))
+                        else:
+                            with open(os.path.join(path, f), "rb") as fh:
+                                signs, dims, entries, _ = decode_packet(fh.read())
+                            dropped, n = int(self.apply(signs, dims, entries)), signs.size
+                        self.entries_dropped += dropped
+                        self.entries_applied += n
                     except Exception as e:  # noqa: BLE001 — a bad packet does not stop the catch-up (lib.rs:216-227)
                         self.failed_files += 1
                         sys.stderr.write(f"[persia_b200] failed to load incremental packet {os.path.join(path, f)}: {e!r}\n")

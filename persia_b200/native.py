@@ -81,6 +81,7 @@ SYMBOLS = {
     "pb_image_index": (_i32, [_vp, _vp, _u64, _u32, _u32, _u32, _u32, _vp, _u32, C.POINTER(_u32), _vp]),
     "pb_image_window": (_i32, [_vp, _vp, _u64, _u32, _u64, _u32, _u64, _u32, _u32, _vp, _u32, C.POINTER(_u32),
                                C.POINTER(_i32), _vp]),
+    "pb_image_packet": (_i32, [_vp, _vp, _u64, _u32, _u32, _vp, _u32, C.POINTER(_u32), C.POINTER(_u64), _vp]),
     "pb_image_insert": (_i32, [_vp, _vp, _u64, _u32, _u32, _i32, _vp]),
     "pb_host_alloc": (_i32, [_u64, C.POINTER(_vp)]),
     "pb_host_free": (_i32, [_vp]),

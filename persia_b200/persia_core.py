@@ -117,6 +117,8 @@ class _State:
         self.dumper = None  # Train with enable_incremental_update: the writer of this replica's flushes
         self.loader = None  # Infer: the scanner of this replica's incremental directory
         self.inc_lock = threading.Lock()
+        self.packet_readers = {}  # device index -> _PacketReader (_apply_packet_file)
+        self.packet_lock = threading.Lock()
         self.gcfg_raw = None  # the global config dict itself (keys parse_global_config does not carry)
         self.emb_dump = None  # the latest background dump (checkpoint.BackgroundDumper)
         self.emb_load = None  # the latest load (checkpoint.DeviceLoader)
@@ -248,6 +250,8 @@ def reset():
         _S.loader.stop()
     if _S.dumper is not None:
         _S.dumper.close()
+    for rd in _S.packet_readers.values():
+        rd.close()
     for g in _S.groups.values():
         g["shard"].close()
     _S.reset()
@@ -328,8 +332,112 @@ def _start_infer():
     if c["embedding_checkpoint"]:
         _S.device_loader(c["embedding_checkpoint"]).run()
     directory = os.path.join(c["incremental_dir"], f"s{_S.replica_index or 0}")
-    _S.loader = INC.IncrementalLoader(directory, _apply_incremental)
+    _S.loader = INC.IncrementalLoader(directory, apply_file=_apply_packet_file)
     _S.loader.start()
+
+
+PACKET_CHUNK = 1 << 16  # entries of one pb_image_insert of a packet (device staging: PACKET_CHUNK x entry length floats)
+
+
+class _PacketReader:
+    """What _apply_packet_file keeps across the files it applies on one device: the pinned buffer a file is read into
+    (grown when a file needs more), the pb_image that indexes it, the stream its inserts run on, and an event recorded
+    after them, which the next file waits for before it overwrites the buffer."""
+
+    def __init__(self, device):
+        import torch
+
+        from . import checkpoint as CK
+
+        self.CK = CK
+        self.stream = torch.cuda.Stream(device)
+        self.done = torch.cuda.Event()
+        self.image = CK._Image(device, PACKET_CHUNK)
+        self.buf = None
+
+    def read(self, path):
+        """The file's bytes into the buffer; returns their count."""
+        size = os.path.getsize(path)
+        self.done.synchronize()
+        if self.buf is None or self.buf.size < size:
+            if self.buf is not None:
+                self.buf.close()
+            self.buf = self.CK._Pinned(max(64, size))
+        with open(path, "rb") as fh:
+            got = fh.readinto(memoryview(self.buf.view)[:size])
+        if got != size:
+            raise RuntimeError(f"{path} changed while it was read")
+        return size
+
+    def close(self):
+        self.stream.synchronize()
+        self.image.close()
+        if self.buf is not None:
+            self.buf.close()
+            self.buf = None
+
+
+def _dropped_so_far(sh, stream):
+    """Entries the table and its tier have refused since creation: admissions the HBM table refused for capacity (with
+    a tier, pb_set_rows gives each back when the tier stores the entry) plus the tier's drops.  Statistics calls are
+    table calls: the caller holds the table's group lock.  Synchronises `stream`."""
+    import torch
+
+    with torch.cuda.stream(stream):
+        return int(sh.counters()["capacity_refused"]) + int(sh.tier_stats()["dropped"])
+
+
+def _apply_packet_file(path, groups=None, chunk=PACKET_CHUNK):
+    """One packet file into the tables of its dims (groups: {dim: group}, None = this replica's), as
+    _apply_incremental(*decode_packet(bytes)[:3], groups) applies it — the same checks and errors, dims ascending, each
+    dim's entries in packet order through pb_set_rows, what was applied before an error kept — but decoded, selected and
+    gathered on the device (pb_image_packet, pb_load.cu).  The file is read into a pinned buffer and indexed outside
+    every lock; a group's lock is held while its dim's inserts (chunk entries each) are enqueued and the table's counters
+    are read before and after them.  Returns (entries neither the HBM table nor its tier had room for, from those
+    counters; entries the packet holds).  A packet of more dims or (dim, entry length) pairs than one device summary
+    holds (pb_image_packet's PB_ERR_CAPACITY) is decoded on the host and applied by _apply_incremental instead."""
+    import torch
+
+    from . import incremental as INC
+    from . import native as N
+
+    groups = _S.groups if groups is None else groups
+    dev = torch.device("cuda", next(iter(groups.values()))["device"] if groups else torch.cuda.current_device())
+    chunk = max(1, min(int(chunk), PACKET_CHUNK))
+    with _S.packet_lock:
+        rd = _S.packet_readers.get(dev.index)
+        if rd is None:
+            rd = _S.packet_readers[dev.index] = _PacketReader(dev)
+        nbytes = rd.read(path)
+        try:
+            try:
+                summary, _ = rd.image.packet(rd.buf, nbytes, 1, 0, rd.stream)
+            except N.PersiaB200Error as e:
+                if e.code != N.PB_ERR_CAPACITY:
+                    raise
+                signs, dims, entries, _ = INC.decode_packet(rd.buf.view[:nbytes].tobytes())
+                return _apply_incremental(signs, dims, entries, groups), int(signs.size)
+            dropped = 0
+            for dim in sorted({d for d, _, k in summary if k}):
+                g = groups.get(dim)
+                if g is None:
+                    raise RuntimeError(f"incremental packet holds dim-{dim} entries but no slot has that dim")
+                lens = {ln for d, ln, k in summary if d == dim and k}
+                if len(lens) > 1:  # (np.stack's error in _apply_incremental)
+                    raise ValueError("all input arrays must have the same shape")
+                sh = g["shard"]
+                if lens != {sh.entry_len}:
+                    raise RuntimeError(f"dim-{dim} entries of {lens.pop()} floats, the registered optimizer needs "
+                                       f"{sh.entry_len}")
+                k = sum(n for d, _, n in summary if d == dim)
+                with g["lock"]:
+                    before = _dropped_so_far(sh, rd.stream)
+                    for lo in range(0, k, chunk):
+                        rd.image.insert(sh, dim, lo, min(lo + chunk, k), False, rd.stream)
+                    dropped += (_dropped_so_far(sh, rd.stream) - before) % (1 << 32)  # (32-bit device counters)
+            return dropped, sum(n for _, _, n in summary)
+        finally:
+            rd.done.record(rd.stream)
 
 
 def _apply_incremental(signs, dims, entries, groups=None):
