@@ -491,6 +491,59 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
 int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_grad, int is_f16, float scale,
                             int32_t* d_status, void* stream, int phases);
 
+/* ---- inference on R GPUs one rank at a time: reading the owners' shards in place --------------------------------------
+ * The reference's Infer handlers each call get_embedding_from_bytes on their own requests, and the embedding servers
+ * answer each request alone (persia/ctx.py:1077-1135, embedding_parameter_service/mod.rs:162-262).  The sharded calls
+ * above are collective instead: every rank must call them in the same step.  For inference the requesting GPU does the
+ * owner's part itself: it probes each owner's index and reads its rows through a peer mapping (CUDA IPC or, in one
+ * process, the pointers themselves).  No flag, no collective, no kernel on the owner: one rank serves its request
+ * while its peers are idle.
+ *
+ * Read-only rule: from pb_table_export_view on, for the rest of its life, the table refuses with PB_ERR_STATE, before
+ * enqueuing anything, every call that moves index cells or steps rows: training forms of pb_forward, pb_forward_raw,
+ * pb_lookup and the sharded forwards; pb_backward, pb_backward_raw and the sharded backwards; pb_update; pb_table_clear;
+ * pb_tier_stage (an eviction check) and pb_table_attach_tier.  pb_set_rows and pb_image_insert stay allowed (an Infer
+ * job applies checkpoint loads and incremental packets with them), as do inference forwards, reads, statistics and
+ * dumps.  The owner cannot know when a peer closes its view, so there is no way back: export a table only to serve it.
+ * Consistency rule: the exported table keeps a write-sequence word in its HBM.  pb_set_rows raises it to odd before its
+ * writes and back to even after them (one-thread kernels with system-scope fences, on the call's stream).  A remote
+ * read checks each owner's word before and after it probes and copies an item, and reads the item again while the
+ * word is odd or if it changed (a row still being published counts the same).  So a returned row is an entry as it
+ * was before an insert or after it, never a mix, as the reference's entry lock gives.  A read that is still waiting
+ * after the sharded calls' wait budget gives up and counts in the reader's pb_table_counters[4].
+ * Ownership rule: the owner outlives every view of its table (destroy views first; a view of a destroyed table reads
+ * freed memory).  A table with a host tier, and a tier, cannot be exported (no peer can reach the tier's rows). */
+/* Bytes of a view blob (fixed: the exporting pid and a random number drawn once per process, the device pointers and CUDA IPC handles of the index cells, rows,
+ * counters and write-sequence word, and the table's geometry). */
+uint64_t pb_table_view_bytes(void);
+/* Writes t's view blob to h_blob (pb_table_view_bytes() bytes) and makes t read-only (above).  Allocates the table if
+ * needed (so the optimizer must be registered) and synchronises the device the first time. */
+int pb_table_export_view(pb_table* t, void* h_blob);
+typedef struct pb_view pb_view;
+/* A view of an exported table for reads issued on `device`.  A blob of another process: each handle is opened with
+ * cudaIpcOpenMemHandle(cudaIpcMemLazyEnablePeerAccess); of this process: its pointers are used as they are (peer access
+ * is enabled when the table lives on another device); a blob is this process's own when both its pid and its random number
+ * are this process's (pids alone repeat across PID namespaces).  pb_view_close synchronises `device` and closes the handles. */
+int pb_view_open(int device, const void* h_blob, pb_view** out);
+int pb_view_close(pb_view* v);
+/* The inference form (training == 0) of pb_forward_sharded, served by this rank alone: arguments as pb_forward, plus
+ * views[R] (owner q's table; views[rank] may be NULL: `own`, this rank's table, is probed directly), R and rank.  The
+ * batch's distinct (slot, sign) items are read from their owners farmhash64(sign) % R into staging the context owns
+ * (n_occ x dim f32 at most, grown like pb_forward_raw's staging: a call is capturable in a CUDA graph, and no host sync
+ * or allocation happens, once a batch at least as large ran on the context), then pooled by the sharded path's own
+ * kernels.  Outputs are bit for bit pb_forward_sharded(training = 0)'s on the same tables and batch; a sign no owner
+ * holds reads as zeros and counts as a lookup miss on its owner (pb_table_counters[1], a system-scope atomic through the
+ * view).  `own` is in its own index chain; the owners' calls are ordered only by the consistency rule. */
+int pb_forward_remote(pb_table* own, pb_view* const* views, uint32_t R, uint32_t rank, pb_ctx* c, const uint64_t* d_ids,
+                      uint32_t n_occ, const uint32_t* d_row_off, const uint32_t* h_slot_occ_off, uint32_t batch,
+                      void* d_out_f16, void* stream);
+/* The same for a raw slot: arguments and outputs as pb_forward_raw plus views, R and rank; bit for bit
+ * pb_forward_raw_sharded(training = 0)'s: row u+1 is f16(row), rounded once. */
+int pb_forward_raw_remote(pb_table* own, pb_view* const* views, uint32_t R, uint32_t rank, pb_ctx* c,
+                          const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off, uint32_t batch,
+                          uint32_t sample_fixed_size, void* d_table_f16, int64_t* d_index, int64_t* d_non_empty,
+                          uint32_t* d_sample_id_num, uint32_t* d_counts, void* stream);
+
 /* Number of kernels the library has launched on behalf of the caller since load (bench bookkeeping). */
 uint64_t pb_launch_count(void);
 /* Diagnostic: the geometry the backward gives its reduce of hot signs (> 32 occurrences) for rows of `dim` columns

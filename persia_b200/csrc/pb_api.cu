@@ -4,9 +4,12 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <random>
 #include <string>
 #include <utility>
 #include <vector>
+
+#include <unistd.h>
 
 #include "pb_kernels.cuh"
 
@@ -120,6 +123,10 @@ struct pb_table {
   // checkpoint images (pb_table_dump_reserve): one allocation holding every DumpWs array; null: none reserved
   DumpWs dump{};
   void* dump_mem = nullptr;
+  // pb_table_export_view: peers read the index and rows in place from then on, so nothing may move cells or step rows
+  // (writable); `seq` is the write-sequence word pb_set_rows keeps odd while it writes
+  bool exported = false;
+  uint32_t* seq = nullptr;
 };
 
 struct pb_ctx {
@@ -187,6 +194,9 @@ struct pb_ctx {
   int prepared = 0;
   uint32_t prepared_n = 0, prepared_batch = 0;
   uint32_t* need = nullptr;  // [PB_MAX_RANKS]
+  // pb_forward_remote / pb_forward_raw_remote: the rows read from their owners, one per distinct item (grow_stage)
+  float* remote_stage = nullptr;
+  size_t remote_stage_floats = 0;
 };
 enum { PREP_NONE = 0, PREP_SUM = 1, PREP_RAW = 2 };
 
@@ -392,6 +402,14 @@ void restore_ids(pb_table* t, bool prefix, const SlotsDev& sl, const uint64_t* i
   if (t->tier) launch_tier_restore(t->d, t->tier->d, t->hy, t->op, sl, prefix, ids, n, st);
 }
 
+// Calls that move index cells or step rows: refused once peers read the table in place (pb_table_export_view).
+int writable(const pb_table* t) {
+  if (t->exported)
+    return fail(PB_ERR_STATE, "the table was exported for remote reads (pb_table_export_view): it is read-only for the "
+                              "rest of its life (pb_set_rows and pb_image_insert stay allowed)");
+  return PB_OK;
+}
+
 int ready_for_training(pb_table* t) {
   if (t->tier_of) return fail(PB_ERR_STATE, "a host tier is not trained directly: use the table it is attached to");
   if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered (OptimizerNotFoundError)");
@@ -538,6 +556,7 @@ int check_raw_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_
 
 int check_backward(pb_table* t, pb_ctx* c, const void* const* h_grads) {
   if (!t || !c || !h_grads) return fail(PB_ERR_INVALID, "null argument");
+  if (int rc = writable(t)) return rc;
   int rc = c->pending.check(t, "no forward batch is pending in this context (backward_ref_id not found)",
                             "the pending batch was looked up in another table");
   if (rc || (rc = ready_for_training(t))) return rc;
@@ -546,6 +565,7 @@ int check_backward(pb_table* t, pb_ctx* c, const void* const* h_grads) {
 
 // (t and c not null: each caller checks them with its own arguments)
 int check_raw_backward(pb_table* t, pb_ctx* c, const void* d_grad) {
+  if (int rc = writable(t)) return rc;
   int rc = c->raw_pending.check(t, "no raw forward batch is pending in this context (backward_ref_id not found)",
                                 "the pending raw batch was looked up in another table");
   if (rc) return rc;
@@ -732,6 +752,7 @@ int pb_table_create_host(int device, const pb_table_cfg* cfg, pb_table** out) {
 
 int pb_table_attach_tier(pb_table* t, pb_table* tier) {
   if (!t || !tier) return fail(PB_ERR_INVALID, "null argument");
+  if (int rc = writable(t)) return rc;  // (an exported table can have no tier: peers could not read its host rows)
   if (t->host || !tier->host) return fail(PB_ERR_INVALID, "the tier must be a host table (pb_table_create_host) behind an HBM table");
   if (t->tier || t->tier_of || tier->tier_of || tier->tier) return fail(PB_ERR_STATE, "one of the tables already has a tier or is one");
   if (t->device != tier->device) return fail(PB_ERR_INVALID, "the tables live on different devices");
@@ -770,7 +791,7 @@ int pb_tier_stage(pb_table* t, const uint64_t* d_ids, uint32_t n, const uint32_t
   if (n_slots == 0 || n_slots > PB_MAX_SLOTS) return fail(PB_ERR_INVALID, "n_slots must be in 1..PB_MAX_SLOTS");
   if (prefix_bit == 0 || prefix_bit > 63) return fail(PB_ERR_INVALID, "feature_index_prefix_bit must be in 1..63");
   int rc = check_slot_offsets(h_slot_occ_off, n_slots, n);
-  if (rc) return rc;
+  if (rc || (rc = writable(t))) return rc;  // (its eviction check)
   if (!t->tier) return PB_OK;  // nothing to move
   if ((rc = ready_for_training(t))) return rc;
   SlotsDev sl;
@@ -894,6 +915,7 @@ int pb_table_destroy(pb_table* t) {
     cudaFree(t->dump_mem);
   }
   if (t->stats_ws) cudaFree(t->stats_ws);
+  if (t->seq) cudaFree(t->seq);
   if (t->scratch) cudaFree(t->scratch);
   if (t->adam_dev) cudaFree(t->adam_dev);
   delete t;
@@ -996,6 +1018,7 @@ int pb_table_size(pb_table* t, uint64_t* h_out, void* stream) {
 
 int pb_table_clear(pb_table* t, void* stream) {
   if (!t) return fail(PB_ERR_INVALID, "null argument");
+  if (int rc = writable(t)) return rc;
   if (!t->allocated) return PB_OK;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
@@ -1010,8 +1033,8 @@ int pb_table_clear(pb_table* t, void* stream) {
 int pb_lookup(pb_table* t, const uint64_t* d_signs, uint32_t n, int training, float* d_out, void* stream) {
   if (!t || (n && (!d_signs || !d_out))) return fail(PB_ERR_INVALID, "null argument");
   if (training) {
-    int rc = ready_for_training(t);
-    if (rc) return rc;
+    int rc = writable(t);
+    if (rc || (rc = ready_for_training(t))) return rc;
   } else if (!t->has_op) {  // nothing can be resident yet: zeros
     DeviceGuard g(t->device);
     PB_CUDA(cudaMemsetAsync(d_out, 0, sizeof(float) * (size_t)n * t->cfg.dim, (cudaStream_t)stream));
@@ -1043,8 +1066,8 @@ int pb_lookup(pb_table* t, const uint64_t* d_signs, uint32_t n, int training, fl
 int pb_update(pb_table* t, const uint64_t* d_signs, const float* d_grads, uint32_t n, void* stream) {
   if (!t || (n && (!d_signs || !d_grads))) return fail(PB_ERR_INVALID, "null argument");
   if (n && misaligned(d_grads)) return fail(PB_ERR_INVALID, "gradient pointer must be 16-byte aligned");
-  int rc = ready_for_training(t);
-  if (rc) return rc;
+  int rc = writable(t);
+  if (rc || (rc = ready_for_training(t))) return rc;
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
@@ -1082,8 +1105,12 @@ int pb_set_rows(pb_table* t, const uint64_t* d_signs, const float* d_entries, ui
   // with a tier: a tier-held sign is first moved back (it then lives in one table), and an entry the HBM table has no
   // row for goes to the tier
   restore_ids(t, false, sl, d_signs, n, st);
+  // an exported table: peers reading it in place see the write-sequence word odd from before the first cell it may
+  // claim to after the last entry it writes (pb_remote.cu), and read those items again
+  if (t->exported) launch_seq_bump(t->seq, true, st);
   launch_probe(MODE_SET, false, t->d, t->hy, t->op, sl, d_signs, n, t->scratch, st);
   launch_copy_entries(true, t->d, t->scratch, n, const_cast<float*>(d_entries), nullptr, st);
+  if (t->exported) launch_seq_bump(t->seq, false, st);
   if (t->tier) launch_tier_set(t->d, t->tier->d, t->hy, t->op, d_signs, t->scratch, n, d_entries, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
@@ -1633,7 +1660,7 @@ int pb_ctx_destroy(pb_ctx* c) {
   void* ptrs[] = {c->b.set,   c->b.occ_set, c->b.item_cell, c->b.seg_occ, c->b.cold, c->b.warm, c->b.hot, c->b.hot_bits, c->b.cnt,
                   c->occ_cell, c->occ_outrow, c->row_off, c->nan_tick, c->vw_stage, c->hot_stage, c->dev_tick, c->raw.set,
                   c->raw.occ_set, c->raw.flag, c->raw.rank, c->raw.tiles, c->raw.distinct_cell, c->raw.counts, c->raw.target,
-                  c->raw.peer,    c->raw_stage, c->need};
+                  c->raw.peer,    c->raw_stage, c->need,     c->remote_stage};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   if (c->side) cudaStreamDestroy(c->side);
@@ -1718,7 +1745,7 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   if (rc) return rc;
   const uint64_t n_out = (uint64_t)c->slots.n_slots * batch;
   if (training) {
-    if ((rc = ready_for_training(t))) return rc;
+    if ((rc = writable(t)) || (rc = ready_for_training(t))) return rc;
   } else if (!t->has_op) {
     DeviceGuard g(t->device);
     PB_CUDA(cudaMemsetAsync(d_out_f16, 0, 2 * n_out * t->cfg.dim, (cudaStream_t)stream));
@@ -1875,6 +1902,11 @@ void xchg_layout(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32, uint64_t 
   off[3] = off[2] + round256((uint64_t)R * cap * dim * 4);                         // gok
   off[4] = off[3] + round256((uint64_t)R * cap * 4);                               // chain
   off[5] = off[4] + round256((uint64_t)R * cap * 4);                               // end
+}
+
+// the rows this rank's receive area holds, returned by the owners (the requester's FINISH reads them)
+const void* received_rows(const pb_xchg* x) {
+  return reinterpret_cast<const void*>(x->d.base[x->d.rank] + x->d.off_row);
 }
 
 // The phases a sharded call runs (PB_PHASE_*; 0 = all).  Each phase ends by signalling a flag of the exchange that a
@@ -2073,7 +2105,7 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
   // (a PREPARE alone may meet a ragged batch on an f16 exchange: finding that out is what it is for)
   if (rc || (rc = check_exchange(t, nullptr, x, d_row_off != nullptr && ph.exchanges(),
                                  "ragged layouts need an exchange created with f32 rows")) ||
-      (rc = check_prepared(c, ph, PREP_SUM, n_occ, batch)))
+      (rc = check_prepared(c, ph, PREP_SUM, n_occ, batch)) || (training && (rc = writable(t))))
     return rc;
   const uint64_t n_out = (uint64_t)c->slots.n_slots * batch;
   // every rank serves lookups whether or not its own batch trains: the shard must be usable (a collective call)
@@ -2097,7 +2129,8 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
   if (ph.has(PB_PHASE_SERVE)) serve_lookup(t, x, training, ph, st);
   if (ph.has(PB_PHASE_FINISH)) {
     ph.await(x, XC_FLAG_ROW, st);
-    launch_expand_items(t->d, sl, c->b, x->d, d_row_off, (uint32_t)n_out, batch, training != 0, d_out_f16, st);
+    launch_expand_items(t->d, sl, c->b, received_rows(x), x->d.row_f32 != 0, d_row_off, (uint32_t)n_out, batch,
+                        training != 0, d_out_f16, st);
     if ((rc = end_forward(t, c, d_row_off, h_slot_occ_off, n_occ, batch, training, st))) return rc;
   }
   PB_CUDA(cudaGetLastError());
@@ -2179,7 +2212,7 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
                              d_sample_id_num, d_counts);
   if (rc) return rc;
   if (training) {
-    if ((rc = ready_for_training(t))) return rc;
+    if ((rc = writable(t)) || (rc = ready_for_training(t))) return rc;
   } else if (!t->has_op) {
     return fail(PB_ERR_STATE, "optimizer not registered (OptimizerNotFoundError)");
   }
@@ -2265,7 +2298,7 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
                              d_sample_id_num, d_counts);
   if (rc || (rc = check_exchange(t, nullptr, x, ph.exchanges(),
                                  "raw slots need an exchange created with f32 rows (the requester rounds them)")) ||
-      (rc = check_prepared(c, ph, PREP_RAW, n_occ, batch)))
+      (rc = check_prepared(c, ph, PREP_RAW, n_occ, batch)) || (training && (rc = writable(t))))
     return rc;
   // every rank serves lookups whether or not its own batch trains: the shard must be usable (a collective call)
   if ((rc = ready_for_training(t))) return rc;
@@ -2309,7 +2342,7 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
   if (ph.has(PB_PHASE_SERVE)) serve_lookup(t, x, training, ph, st);
   if (ph.has(PB_PHASE_FINISH)) {
     ph.await(x, XC_FLAG_ROW, st);
-    launch_raw_fill(c->raw, n_occ, t->d.dim, x->d, d_table_f16, st);  // requester: rows in -> distinct-sign table
+    launch_raw_fill(c->raw, n_occ, t->d.dim, static_cast<const float*>(received_rows(x)), d_table_f16, st);  // rows in -> table
     if (training) hold_raw_batch(t, c, n_occ, batch);
   }
   PB_CUDA(cudaGetLastError());
@@ -2345,6 +2378,229 @@ int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_gr
     if ((rc = owner_backward(t, x, c->slots.prefix, 1, sl.spacing, ph, st))) return rc;
     c->raw_pending.drop();
   }
+  PB_CUDA(cudaGetLastError());
+  return PB_OK;
+}
+
+// ---- inference on R GPUs one rank at a time: views of the owners' tables --------------------------------------------
+namespace {
+// The bytes pb_table_export_view writes: what a peer needs to read the table in place.
+constexpr uint32_t VIEW_MAGIC = 0x57564250u;  // "PBVW"
+constexpr uint32_t VIEW_VERSION = 1;
+enum { VA_CELLS = 0, VA_ROWS, VA_COUNTERS, VA_SEQ, VA_COUNT };  // the allocations a reader touches
+struct ViewBlob {
+  uint32_t magic, version;
+  uint64_t pid;                                // the exporting process ...
+  uint64_t nonce;                              // ... and its random number (pids repeat across PID namespaces)
+  int32_t device;                              // its device ordinal, in the exporting process
+  uint32_t ipc;                                // 1: the handles below are valid
+  uint64_t ptr[VA_COUNT];                      // device pointers in the exporting process
+  cudaIpcMemHandle_t handle[VA_COUNT];         // the same allocations for other processes
+  uint32_t dim, stride, state_floats, n_cells, capacity, pad;
+};
+// A random number drawn once per process: a blob is this process's own only when both its pid and this number match.
+uint64_t process_nonce() {
+  static const uint64_t n = [] {
+    std::random_device rd;
+    uint64_t v = ((uint64_t)rd() << 32) ^ rd();
+    return v ? v : 1;
+  }();
+  return n;
+}
+}  // namespace
+
+struct pb_view {
+  int device = 0;
+  TableDev d{};
+  uint32_t* seq = nullptr;
+  bool ipc = false;  // the pointers were opened with cudaIpcOpenMemHandle (closed by pb_view_close)
+  void* opened[VA_COUNT] = {};
+};
+
+namespace {
+// The owners' tables of a remote read as this GPU reaches them: views[q] for q != rank, `own` itself for `rank`.
+int remote_views(pb_table* own, pb_view* const* views, uint32_t R, uint32_t rank, RemoteDev& rv) {
+  if (R == 0 || R > PB_MAX_RANKS || rank >= R) return fail(PB_ERR_INVALID, "need 1 <= R <= 16 and rank < R");
+  if (R > 1 && !views) return fail(PB_ERR_INVALID, "null argument");
+  if (own->tier || own->host || own->tier_of)
+    return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no remote reads)");
+  if (!own->has_op) return fail(PB_ERR_STATE, "optimizer not registered (OptimizerNotFoundError)");
+  std::memset(&rv, 0, sizeof(rv));
+  rv.R = R;
+  for (uint32_t q = 0; q < R; ++q) {
+    if (q == rank) continue;
+    const pb_view* v = views[q];
+    if (!v) return fail(PB_ERR_INVALID, "every owner but this rank needs a view (views[q] null)");
+    if (v->device != own->device) return fail(PB_ERR_INVALID, "a view was opened on another device than the table's");
+    if (v->d.dim != own->cfg.dim) return fail(PB_ERR_INVALID, "a view's table holds another embedding dim");
+    rv.t[q] = v->d;
+    rv.seq[q] = v->seq;
+  }
+  return PB_OK;
+}
+
+// The start of a remote call, after its argument checks: `own` allocated and in its index chain, this rank's entry of
+// `rv`, and the staging of `floats` floats.
+int begin_remote(pb_table* own, pb_ctx* c, RemoteDev& rv, uint32_t rank, size_t floats, TableCall& call, cudaStream_t st) {
+  if (int rc = call.begin(own, st, CALL_INDEX)) return rc;
+  if (int rc = ensure_alloc(own)) return rc;
+  rv.t[rank] = own->d;
+  rv.seq[rank] = own->seq;  // (null unless exported: then only calls ordered with this one write it)
+  return grow_stage(c->remote_stage, c->remote_stage_floats, floats ? floats : 1, st);
+}
+}  // namespace
+
+uint64_t pb_table_view_bytes(void) { return sizeof(ViewBlob); }
+
+int pb_table_export_view(pb_table* t, void* h_blob) {
+  if (!t || !h_blob) return fail(PB_ERR_INVALID, "null argument");
+  if (t->host || t->tier_of)
+    return fail(PB_ERR_STATE, "a host tier cannot be exported: its rows are pinned host memory no peer process can map");
+  if (t->tier)
+    return fail(PB_ERR_STATE, "a table with a host tier cannot be exported: peers could not read its tier's rows");
+  DeviceGuard g(t->device);
+  if (int rc = ensure_alloc(t)) return rc;
+  if (!t->seq) {
+    PB_CUDA(cudaMalloc(&t->seq, sizeof(uint32_t)));
+    PB_CUDA(cudaMemset(t->seq, 0, sizeof(uint32_t)));
+    PB_CUDA(cudaDeviceSynchronize());
+  }
+  ViewBlob b;
+  std::memset(&b, 0, sizeof(b));
+  b.magic = VIEW_MAGIC;
+  b.version = VIEW_VERSION;
+  b.pid = (uint64_t)getpid();
+  b.nonce = process_nonce();
+  b.device = t->device;
+  void* p[VA_COUNT] = {t->d.cells, t->d.rows, t->d.counters, t->seq};
+  b.ipc = 1;
+  for (int i = 0; i < VA_COUNT; ++i) {
+    b.ptr[i] = reinterpret_cast<uint64_t>(p[i]);
+    if (b.ipc && cudaIpcGetMemHandle(&b.handle[i], p[i]) != cudaSuccess) b.ipc = 0;  // same-process views still work
+  }
+  if (!b.ipc) {
+    cudaGetLastError();  // (the failed handle request is not this call's error)
+    std::memset(b.handle, 0, sizeof(b.handle));
+  }
+  b.dim = t->d.dim;
+  b.stride = t->d.stride;
+  b.state_floats = t->d.state_floats;
+  b.n_cells = t->d.n_cells;
+  b.capacity = t->d.capacity;
+  std::memcpy(h_blob, &b, sizeof(b));
+  t->exported = true;
+  return PB_OK;
+}
+
+int pb_view_open(int device, const void* h_blob, pb_view** out) {
+  if (!h_blob || !out) return fail(PB_ERR_INVALID, "null argument");
+  ViewBlob b;
+  std::memcpy(&b, h_blob, sizeof(b));
+  if (b.magic != VIEW_MAGIC || b.version != VIEW_VERSION) return fail(PB_ERR_INVALID, "not a table view (pb_table_export_view)");
+  if (!b.n_cells || (b.n_cells & (b.n_cells - 1)) || !b.dim || b.stride < b.dim)
+    return fail(PB_ERR_INVALID, "the view's table geometry is malformed");
+  DeviceGuard g(device);
+  pb_view* v = new pb_view();
+  v->device = device;
+  void* p[VA_COUNT];
+  if (b.pid == (uint64_t)getpid() && b.nonce == process_nonce()) {  // CUDA IPC cannot open a handle in its own process: the pointers are valid here
+    for (int i = 0; i < VA_COUNT; ++i) p[i] = reinterpret_cast<void*>(b.ptr[i]);
+    if (b.device != device) {
+      const cudaError_t e = cudaDeviceEnablePeerAccess(b.device, 0);
+      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) {
+        delete v;
+        return fail(PB_ERR_CUDA, std::string("cudaDeviceEnablePeerAccess: ") + cudaGetErrorString(e));
+      }
+      cudaGetLastError();
+    }
+  } else {
+    if (!b.ipc) {
+      delete v;
+      return fail(PB_ERR_STATE, "the exporting process could not make CUDA IPC handles for this table");
+    }
+    for (int i = 0; i < VA_COUNT; ++i) {
+      const cudaError_t e = cudaIpcOpenMemHandle(&p[i], b.handle[i], cudaIpcMemLazyEnablePeerAccess);
+      if (e != cudaSuccess) {
+        for (int k = 0; k < i; ++k) cudaIpcCloseMemHandle(v->opened[k]);
+        delete v;
+        return fail(PB_ERR_CUDA, std::string("cudaIpcOpenMemHandle: ") + cudaGetErrorString(e));
+      }
+      v->opened[i] = p[i];
+    }
+    v->ipc = true;
+  }
+  TableDev& d = v->d;
+  d.cells = static_cast<Cell*>(p[VA_CELLS]);
+  d.rows = static_cast<float*>(p[VA_ROWS]);
+  d.counters = static_cast<uint32_t*>(p[VA_COUNTERS]);
+  d.n_cells = b.n_cells;
+  d.cell_mask = b.n_cells - 1;
+  d.bucket_mask = b.n_cells / BUCKET - 1;
+  d.capacity = b.capacity;
+  d.dim = b.dim;
+  d.stride = b.stride;
+  d.state_floats = b.state_floats;
+  v->seq = static_cast<uint32_t*>(p[VA_SEQ]);
+  *out = v;
+  return PB_OK;
+}
+
+int pb_view_close(pb_view* v) {
+  if (!v) return PB_OK;
+  DeviceGuard g(v->device);
+  cudaDeviceSynchronize();  // (remote reads through it may still run)
+  if (v->ipc)
+    for (int i = 0; i < VA_COUNT; ++i) cudaIpcCloseMemHandle(v->opened[i]);
+  delete v;
+  return PB_OK;
+}
+
+int pb_forward_remote(pb_table* own, pb_view* const* views, uint32_t R, uint32_t rank, pb_ctx* c, const uint64_t* d_ids,
+                      uint32_t n_occ, const uint32_t* d_row_off, const uint32_t* h_slot_occ_off, uint32_t batch,
+                      void* d_out_f16, void* stream) {
+  int rc = check_forward(own, c, d_ids, n_occ, d_row_off, h_slot_occ_off, batch, d_out_f16);
+  RemoteDev rv;
+  if (rc || (rc = remote_views(own, views, R, rank, rv))) return rc;
+  const uint64_t n_out = (uint64_t)c->slots.n_slots * batch;
+  const bool row_f32 = d_row_off != nullptr;  // ragged layouts pool f32 rows, as on an exchange of f32 rows
+  DeviceGuard g(own->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  const size_t elems = (size_t)n_occ * own->cfg.dim;  // at most one row per id occurrence
+  if ((rc = begin_remote(own, c, rv, rank, row_f32 ? elems : (elems + 1) / 2, call, st))) return rc;
+  SlotsDev sl;
+  if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
+  if ((rc = begin_forward(own, c, sl, d_ids, n_occ, 0, st))) return rc;  // the dedup (an inference request)
+  launch_remote_lookup(false, row_f32, rv, c->b, c->raw, n_occ, c->remote_stage, own->d.dim, own->d.counters + CTR_ERR, st);
+  launch_expand_items(own->d, sl, c->b, c->remote_stage, row_f32, d_row_off, (uint32_t)n_out, batch, false, d_out_f16, st);
+  if ((rc = end_forward(own, c, d_row_off, h_slot_occ_off, n_occ, batch, 0, st))) return rc;
+  PB_CUDA(cudaGetLastError());
+  return PB_OK;
+}
+
+int pb_forward_raw_remote(pb_table* own, pb_view* const* views, uint32_t R, uint32_t rank, pb_ctx* c,
+                          const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off, uint32_t batch,
+                          uint32_t sample_fixed_size, void* d_table_f16, int64_t* d_index, int64_t* d_non_empty,
+                          uint32_t* d_sample_id_num, uint32_t* d_counts, void* stream) {
+  int rc = check_raw_forward(own, c, d_ids, n_occ, d_row_off, batch, sample_fixed_size, d_table_f16, d_index, d_non_empty,
+                             d_sample_id_num, d_counts);
+  RemoteDev rv;
+  if (rc || (rc = remote_views(own, views, R, rank, rv))) return rc;
+  DeviceGuard g(own->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  TableCall call;
+  if ((rc = begin_remote(own, c, rv, rank, (size_t)n_occ * own->cfg.dim, call, st))) return rc;
+  if ((rc = ensure_raw(c))) return rc;
+  SlotsDev sl;
+  if ((rc = raw_slots(c, n_occ, sl))) return rc;
+  c->raw_pending.drop();  // the numbering below replaces the pending batch's
+  c->prepared = PREP_NONE;
+  if (d_row_off && (rc = copy_row_off(c, d_row_off, batch, st))) return rc;
+  launch_raw_number(sl, d_ids, n_occ, d_row_off ? c->row_off : nullptr, d_row_off ? c->occ_outrow : nullptr, batch,
+                    sample_fixed_size, nullptr, c->raw, (long long*)d_index, (long long*)d_non_empty, d_sample_id_num, st);
+  PB_CUDA(cudaMemcpyAsync(d_counts, c->raw.counts, 8, cudaMemcpyDeviceToDevice, st));
+  launch_remote_lookup(true, true, rv, c->b, c->raw, n_occ, c->remote_stage, own->d.dim, own->d.counters + CTR_ERR, st);
+  launch_raw_fill(c->raw, n_occ, own->d.dim, c->remote_stage, d_table_f16, st);  // row u + 1 = f16(row), rounded once
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }

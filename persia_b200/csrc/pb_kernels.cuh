@@ -123,6 +123,14 @@ struct XchgDev {
   float* apow;            // [R][PB_ADAM_KEYS][2]
 };
 
+// a remote read (pb_remote.cu): every owner's index and rows as this GPU reaches them (its own table directly, a peer's
+// through a pb_view), and the owner's write-sequence word (null: no insert can run beside the read)
+struct RemoteDev {
+  TableDev t[PB_MAX_RANKS];
+  const uint32_t* seq[PB_MAX_RANKS];
+  uint32_t R;
+};
+
 // arguments of the backward kernels (pb_reduce.cu)
 struct ReduceArgs {
   BatchDev b;
@@ -231,7 +239,8 @@ void launch_wait(const XchgDev& x, int phase, int src /* -1: every source */, cu
 void launch_signal_wait(const XchgDev& x, int phase, const uint32_t* counts, cudaStream_t st);
 void launch_owner_lookup(bool training, const TableDev& t, const HyperDev& hy, const OptimDev& op, const XchgDev& x,
                          cudaStream_t st);
-void launch_expand_items(const TableDev& t, const SlotsDev& sl, const BatchDev& b, const XchgDev& x,
+// rows: the f16 or f32 (row_f32) rows the items' set-cell targets index (the receive area, or a remote read's staging)
+void launch_expand_items(const TableDev& t, const SlotsDev& sl, const BatchDev& b, const void* rows, bool row_f32,
                          const uint32_t* row_off, uint32_t n_out, uint32_t batch, bool training, void* out_f16,
                          cudaStream_t st);
 void launch_hash_stack(const uint64_t* ids, uint32_t n, uint32_t rounds, uint64_t size, uint64_t* out, cudaStream_t st);
@@ -263,9 +272,16 @@ void launch_raw_number(const SlotsDev& sl, const uint64_t* ids, uint32_t n, cons
 // the raw numbering's distinct signs of `w` when raw; n: worst-case U)
 void launch_count_owners(bool raw, const BatchDev& b, const RawWork& w, uint32_t n, uint32_t R, uint32_t* need,
                          cudaStream_t st);
+// pb_remote.cu: the distinct items of the context's batch (raw: its numbered distinct signs) read from their owners into
+// `stage` at the item's number, f16(0 + row) or f32 rows (raw: f32), targets set to the item's number; err counts the
+// items whose read gave up (n: worst-case U)
+void launch_remote_lookup(bool raw, bool row_f32, const RemoteDev& rv, const BatchDev& b, const RawWork& w, uint32_t n,
+                          void* stage, uint32_t dim, uint32_t* err, cudaStream_t st);
+// an exported table's write-sequence word: odd from `begin` to the end of the writes that follow
+void launch_seq_bump(uint32_t* seq, bool begin, cudaStream_t st);
 // pb_shard.cu, raw slot over R shards: requester's route, table fill and gradient send (n: worst-case U)
 void launch_raw_route(const RawWork& w, uint32_t n, const XchgDev& x, cudaStream_t st);
-void launch_raw_fill(const RawWork& w, uint32_t n, uint32_t dim, const XchgDev& x, void* table_f16, cudaStream_t st);
+void launch_raw_fill(const RawWork& w, uint32_t n, uint32_t dim, const float* rows, void* table_f16, cudaStream_t st);
 void launch_raw_send(const void* grad, bool f16, const RawWork& w, uint32_t n, uint32_t dim, float inv_scale,
                      bool do_scale, const uint32_t* tick, const uint32_t* nan_tick, const XchgDev& x, cudaStream_t st);
 void launch_raw_forward(const TableDev& t, const SlotsDev& sl, const uint64_t* ids, uint32_t n,

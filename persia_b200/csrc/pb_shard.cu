@@ -368,10 +368,12 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_owner_lookup(TableDev 
 // requester, forward: received rows -> batch order (lookup_batched_all_slots_postprocess, mod.rs:486-629).
 // One-id layouts: a pure copy of the f16 row.  Ragged layouts: f32 rows summed in sample order, sqrt scaling, RNE.
 // TRAIN: files every occurrence of a repeated sign into the sign's list, like k_gather_items.
+// `rows`: the rows an item's set cell `target` indexes — this rank's receive area (target = owner * cap + slot), or the
+// context's staging of a remote read (pb_remote.cu, target = the item's number).
 // ------------------------------------------------------------------------------------------------
 template <bool TRAIN>
-__global__ void __launch_bounds__(256) k_expand_copy(uint32_t dim, SlotsDev sl, BatchDev b, XchgDev x, uint32_t n_out,
-                                                     __half* __restrict__ out, uint32_t lanes) {
+__global__ void __launch_bounds__(256) k_expand_copy(uint32_t dim, SlotsDev sl, BatchDev b, const void* __restrict__ rows,
+                                                     uint32_t n_out, __half* __restrict__ out, uint32_t lanes) {
   // `lanes` lanes per output row, 16 bytes per lane and step
   if (TRAIN) {  // one occurrence per thread first (the grid has at least n_out threads), one atomic per warp and sign
     const uint32_t gt = blockIdx.x * blockDim.x + threadIdx.x;
@@ -383,13 +385,13 @@ __global__ void __launch_bounds__(256) k_expand_copy(uint32_t dim, SlotsDev sl, 
   const uint32_t cell = b.occ_set[g];
   const uint32_t target = (reinterpret_cast<const uint4*>(&b.set[cell]) + 1)->x;
   const uint32_t words = dim / 8;  // 16-byte words per f16 row (dim % 8 == 0 on this path)
-  const uint4* src = reinterpret_cast<const uint4*>(x_row(x, x.rank)) + (size_t)(target == ROW_NONE ? 0u : target) * words;
+  const uint4* src = reinterpret_cast<const uint4*>(rows) + (size_t)(target == ROW_NONE ? 0u : target) * words;
   uint4* dst = reinterpret_cast<uint4*>(out) + (size_t)g * words;
   for (uint32_t w = l; w < words; w += lanes) dst[w] = target == ROW_NONE ? make_uint4(0u, 0u, 0u, 0u) : src[w];
 }
 
 template <bool TRAIN, bool ROW_F32>
-__global__ void __launch_bounds__(256) k_expand_pool(uint32_t dim, SlotsDev sl, BatchDev b, XchgDev x,
+__global__ void __launch_bounds__(256) k_expand_pool(uint32_t dim, SlotsDev sl, BatchDev b, const void* __restrict__ rows,
                                                      const uint32_t* __restrict__ row_off, uint32_t n_out, uint32_t batch,
                                                      __half* __restrict__ out, uint32_t G) {
   const uint32_t gid = (blockIdx.x * blockDim.x + threadIdx.x) / G;
@@ -409,7 +411,7 @@ __global__ void __launch_bounds__(256) k_expand_pool(uint32_t dim, SlotsDev sl, 
   }
   if (!ROW_F32 && end - beg == 1) {  // one id: the owner already rounded 0 + row to f16 (a copy keeps the sign of a -0)
     const uint32_t target = b.set[b.occ_set[beg]].target;
-    const __half* src = reinterpret_cast<const __half*>(x_row(x, x.rank)) + (size_t)(target == ROW_NONE ? 0u : target) * dim;
+    const __half* src = reinterpret_cast<const __half*>(rows) + (size_t)(target == ROW_NONE ? 0u : target) * dim;
     for (uint32_t e = lane; e < dim; e += G) out[(size_t)gid * dim + e] = target == ROW_NONE ? __float2half_rn(0.0f) : src[e];
     return;
   }
@@ -419,8 +421,8 @@ __global__ void __launch_bounds__(256) k_expand_pool(uint32_t dim, SlotsDev sl, 
       const uint32_t target = b.set[b.occ_set[j]].target;
       if (target == ROW_NONE) continue;
       float v;
-      if (ROW_F32) v = reinterpret_cast<const float*>(x_row(x, x.rank))[(size_t)target * dim + e];
-      else v = __half2float(reinterpret_cast<const __half*>(x_row(x, x.rank))[(size_t)target * dim + e]);
+      if (ROW_F32) v = reinterpret_cast<const float*>(rows)[(size_t)target * dim + e];
+      else v = __half2float(reinterpret_cast<const __half*>(rows)[(size_t)target * dim + e]);
       acc = __fadd_rn(acc, v);
     }
     out[(size_t)gid * dim + e] = __float2half_rn(__fmul_rn(acc, scale));
@@ -718,6 +720,7 @@ __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, H
 // signs like pb_forward_raw (pb_raw.cu), then every distinct sign is one entry of its owner's request:
 //   k_raw_route  sign -> owner's area; target[u] = owner * cap + slot, kept for the fill and the backward
 //   k_raw_fill   received f32 row -> table row u + 1, rounded once (f16(row): a -0 stays -0); row 0 and misses zeros
+//                (rows: the receive area, or a remote read's staging, pb_remote.cu; target[u] indexes it either way)
 //   k_raw_send   the [U, dim] gradient, +-inf clamped and unscaled, -> owner's gradient area with its apply word
 // The owner's side is the summation path's: k_owner_lookup, then k_owner_update_all / k_owner_update.
 // ------------------------------------------------------------------------------------------------
@@ -757,12 +760,13 @@ __global__ void __launch_bounds__(256) k_raw_route(RawWork w, XchgDev x) {
 }
 
 __global__ void __launch_bounds__(256) k_raw_fill(const uint32_t* __restrict__ counts, const uint32_t* __restrict__ target,
-                                                  uint32_t dim, XchgDev x, __half* __restrict__ out, uint32_t G) {
+                                                  uint32_t dim, const float* __restrict__ rows, __half* __restrict__ out,
+                                                  uint32_t G) {
   const uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) / G;  // table row
   const uint32_t lane = threadIdx.x % G;
   if (r > counts[0]) return;
   const uint32_t tg = r ? target[r - 1] : ROW_NONE;
-  const float* src = reinterpret_cast<const float*>(x_row(x, x.rank)) + (size_t)(tg == ROW_NONE ? 0u : tg) * dim;
+  const float* src = rows + (size_t)(tg == ROW_NONE ? 0u : tg) * dim;
   __half* o = out + (size_t)r * dim;
   for (uint32_t e = lane; e < dim; e += G) o[e] = __float2half_rn(tg == ROW_NONE ? 0.0f : src[e]);  // ndarray_f32_to_f16: RNE
 }
@@ -814,9 +818,9 @@ void launch_raw_route(const RawWork& w, uint32_t n, const XchgDev& x, cudaStream
   PB_LAUNCH_F(FAM_ROUTE, k_raw_route, cdiv(n, 256), 256, 0, st, w, x);
 }
 
-void launch_raw_fill(const RawWork& w, uint32_t n, uint32_t dim, const XchgDev& x, void* table_f16, cudaStream_t st) {
+void launch_raw_fill(const RawWork& w, uint32_t n, uint32_t dim, const float* rows, void* table_f16, cudaStream_t st) {
   const uint32_t G = lanes_for(dim);
-  PB_LAUNCH_F(FAM_GATHER, k_raw_fill, cdiv((uint64_t)(n + 1) * G, 256), 256, 0, st, w.counts, w.target, dim, x,
+  PB_LAUNCH_F(FAM_GATHER, k_raw_fill, cdiv((uint64_t)(n + 1) * G, 256), 256, 0, st, w.counts, w.target, dim, rows,
               reinterpret_cast<__half*>(table_f16), G);
 }
 
@@ -870,29 +874,29 @@ void launch_owner_lookup(bool training, const TableDev& t, const HyperDev& hy, c
   }
 }
 
-void launch_expand_items(const TableDev& t, const SlotsDev& sl, const BatchDev& b, const XchgDev& x,
+void launch_expand_items(const TableDev& t, const SlotsDev& sl, const BatchDev& b, const void* rows, bool row_f32,
                          const uint32_t* row_off, uint32_t n_out, uint32_t batch, bool training, void* out_f16,
                          cudaStream_t st) {
   if (!n_out) return;
   __half* out = reinterpret_cast<__half*>(out_f16);
-  if (!row_off && !x.row_f32 && t.dim % 8 == 0) {
+  if (!row_off && !row_f32 && t.dim % 8 == 0) {
     uint32_t words = t.dim / 8, lanes = 1;
     while (lanes < words && lanes < 32) lanes <<= 1;
     uint32_t grid = cdiv((uint64_t)n_out * lanes, 256);
     if (grid < cdiv(n_out, 256)) grid = cdiv(n_out, 256);
-    if (training) PB_LAUNCH_F(FAM_GATHER, (k_expand_copy<true>), grid, 256, 0, st, t.dim, sl, b, x, n_out, out, lanes);
-    else PB_LAUNCH_F(FAM_GATHER, (k_expand_copy<false>), grid, 256, 0, st, t.dim, sl, b, x, n_out, out, lanes);
+    if (training) PB_LAUNCH_F(FAM_GATHER, (k_expand_copy<true>), grid, 256, 0, st, t.dim, sl, b, rows, n_out, out, lanes);
+    else PB_LAUNCH_F(FAM_GATHER, (k_expand_copy<false>), grid, 256, 0, st, t.dim, sl, b, rows, n_out, out, lanes);
     return;
   }
   uint32_t G = 1;
   while (G < t.dim && G < 32) G <<= 1;
   const uint32_t grid = cdiv((uint64_t)n_out * G, 256);
-#define PB_E(TR, F32) PB_LAUNCH_F(FAM_GATHER, (k_expand_pool<TR, F32>), grid, 256, 0, st, t.dim, sl, b, x, row_off, n_out, batch, out, G)
+#define PB_E(TR, F32) PB_LAUNCH_F(FAM_GATHER, (k_expand_pool<TR, F32>), grid, 256, 0, st, t.dim, sl, b, rows, row_off, n_out, batch, out, G)
   if (training) {
-    if (x.row_f32) PB_E(true, true);
+    if (row_f32) PB_E(true, true);
     else PB_E(true, false);
   } else {
-    if (x.row_f32) PB_E(false, true);
+    if (row_f32) PB_E(false, true);
     else PB_E(false, false);
   }
 #undef PB_E

@@ -108,6 +108,13 @@ SYMBOLS = {
     "pb_backward_sharded": (_i32, [_vp, _vp, _vp, C.POINTER(_vp), _i32, C.POINTER(C.c_float), _vp, _vp, _i32]),
     "pb_forward_raw_sharded": (_i32, [_vp, _vp, _vp, _vp, _u32, _vp, _u32, _u32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32]),
     "pb_backward_raw_sharded": (_i32, [_vp, _vp, _vp, _vp, _i32, C.c_float, _vp, _vp, _i32]),
+    "pb_table_view_bytes": (_u64, []),
+    "pb_table_export_view": (_i32, [_vp, _vp]),
+    "pb_view_open": (_i32, [_i32, _vp, C.POINTER(_vp)]),
+    "pb_view_close": (_i32, [_vp]),
+    "pb_forward_remote": (_i32, [_vp, C.POINTER(_vp), _u32, _u32, _vp, _vp, _u32, _vp, C.POINTER(_u32), _u32, _vp, _vp]),
+    "pb_forward_raw_remote": (_i32, [_vp, C.POINTER(_vp), _u32, _u32, _vp, _vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp,
+                                     _vp, _vp]),
     "pb_launch_count": (_u64, []),
     "pb_hot_geometry": (_i32, [_u32, _i32, _i32, C.POINTER(_u32 * 12)]),
     "pb_profile_enable": (_i32, [_i32]),

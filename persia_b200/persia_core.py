@@ -22,6 +22,8 @@ staleness rules (persia_b200/engine.py), `Backward` applies updates in the calle
 write and read the reference's `.emb` checkpoint files (persia_b200/checkpoint.py).  With the global config's
 `enable_incremental_update` on a Train job, the signs the tables step are flushed as the reference's `.inc` packets; an
 Infer job loads its checkpoint and applies them as they appear (persia_b200/incremental.py, `set_global_config`).
+An Infer job with `replica_size > 1` exports every table once its checkpoint is loaded and serves each forward that does
+not train on its rank alone, reading the owners' shards in place (_start_remote, worker.RemoteReader): no collective.
 """
 import os
 import queue
@@ -122,6 +124,7 @@ class _State:
         self.gcfg_raw = None  # the global config dict itself (keys parse_global_config does not carry)
         self.emb_dump = None  # the latest background dump (checkpoint.BackgroundDumper)
         self.emb_load = None  # the latest load (checkpoint.DeviceLoader)
+        self.remote = None  # Infer at replica_size > 1: dim -> RemoteReader (_start_remote): one rank serves alone
 
     def global_config(self):
         """set_global_config's dict, else the PERSIA_GLOBAL_CONFIG yaml, else the reference's defaults."""
@@ -252,9 +255,21 @@ def reset():
         _S.dumper.close()
     for rd in _S.packet_readers.values():
         rd.close()
+    _close_remote()  # (the views before the tables)
     for g in _S.groups.values():
         g["shard"].close()
     _S.reset()
+
+
+def _close_remote():
+    """Closes the Infer job's remote readers (their contexts and views of the peers' tables), if any: by reset(), and at
+    interpreter exit before any table (an atexit hook, so that the views never outlive this process's tables whatever
+    order the objects are collected in).  A peer's table must outlive this rank's views of it, so the ranks of an Infer
+    job stop serving together: end with a barrier (or dist.destroy_process_group after one) before any rank exits."""
+    if _S.remote is not None:
+        for rd in _S.remote.values():
+            rd.close()
+        _S.remote = None
 
 
 def _maybe_flush_incremental():
@@ -331,9 +346,50 @@ def _start_infer():
     _S.ensure_config()
     if c["embedding_checkpoint"]:
         _S.device_loader(c["embedding_checkpoint"]).run()
+    if (_S.replica_size or 1) > 1:  # before the first packet: from the export on, inserts are bracketed for readers
+        _start_remote()
     directory = os.path.join(c["incremental_dir"], f"s{_S.replica_index or 0}")
     _S.loader = INC.IncrementalLoader(directory, apply_file=_apply_packet_file)
     _S.loader.start()
+
+
+def _start_remote():
+    """Infer on R GPUs: every dim group exports its table and the ranks exchange the blobs once (collective: every rank
+    registers its optimizer, hence starts its Infer job, alike).  From then on a forward that does not train is served
+    by the dim's RemoteReader (persia_b200/worker.py) on this rank alone: no _sharded_step, no all_reduce, so each rank
+    answers its own requests whatever its peers do, as the reference's servers answer each request alone.  The tables
+    are then read-only but for checkpoint loads and incremental packets, which the readers see whole or not at all."""
+    import torch.distributed as dist
+
+    from .worker import RemoteReader
+
+    if not dist.is_initialized():
+        raise RuntimeError("replica_size > 1 needs torch.distributed (TrainCtx initialises it; else call init_process_group)")
+    groups = {d: _S.group(d) for d in sorted({s.dim for s in _S.slots})}
+    blobs = {}
+    for d, g in groups.items():
+        with g["lock"]:
+            blobs[d] = g["shard"].export_view()
+    got = [None] * dist.get_world_size()
+    dist.all_gather_object(got, blobs)  # one exchange for every dim
+    rank = dist.get_rank()
+    from . import shard as SH
+
+    readers = {}
+    for d, g in groups.items():
+        views = [SH.TableView(got[q][d], g["shard"].device) if q != rank else None for q in range(len(got))]
+        readers[d] = RemoteReader(g["shard"], views, rank)
+    dist.barrier()  # (no rank reads before every view is open)
+    _S.remote = readers
+    global _CLOSE_AT_EXIT
+    if not _CLOSE_AT_EXIT:
+        import atexit
+
+        atexit.register(_close_remote)
+        _CLOSE_AT_EXIT = True
+
+
+_CLOSE_AT_EXIT = False  # _close_remote is registered to run at interpreter exit
 
 
 PACKET_CHUNK = 1 << 16  # entries of one pb_image_insert of a packet (device staging: PACKET_CHUNK x entry length floats)
@@ -853,7 +909,9 @@ def _forward_locked(batch, device_id, training):
             _S.raw_order = raw_names
         elif _S.raw_order != raw_names:
             raise RuntimeError("on R GPUs every batch must carry the same raw slots, in the same order")
-    step = _sharded_step(feats, B, training, dev) if sharded else {}
+    # Infer on R GPUs: this rank alone reads the owners' shards (_start_remote); a Train job keeps the collective path
+    remote = _S.remote if sharded and not training else None
+    step = _sharded_step(feats, B, training, dev) if sharded and remote is None else {}
     pending = _Pending()
     by_slot = {}
     raw_out = {}
@@ -863,6 +921,18 @@ def _forward_locked(batch, device_id, training):
             continue
         with _STATE_LOCK:
             g = _S.group(sc.dim)
+        if remote is not None:
+            ids, row_off, _ = _flatten([(n, x)], B)
+            d_ids = torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True)
+            d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
+            with g["lock"]:
+                table, index, non_empty, num, counts = remote[sc.dim].forward_raw(d_ids, B, sc.sample_fixed_size,
+                                                                                  sc.index_prefix, _S.prefix_bit,
+                                                                                  row_off=d_off)
+                U, ne = counts.tolist()
+            raw_out[n] = (Tensor(table[:U + 1], n), Tensor(index, f"{n}_index"),
+                          Tensor(non_empty[:ne], f"{n}_non_empty_index"), num.tolist())
+            continue
         if sharded:  # R GPUs: one request per owner, through the slot's raw worker (prepared and sized above)
             wk, kw = step[("raw", n)]
             with g["lock"]:
@@ -906,6 +976,17 @@ def _forward_locked(batch, device_id, training):
             part = [dim_part[i] for i in chunk]
             names = [n for n, _ in part]
             key = tuple(names)
+            if remote is not None:
+                ids, row_off, slot_off = _flatten(part, B)
+                slots = [_S.by_name[n] for n in names]
+                with g["lock"]:
+                    d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
+                    d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
+                    out = remote[dim].forward(d_ids, B, [sc.index_prefix for sc in slots], [sc.sqrt_scaling for sc in slots],
+                                              _S.prefix_bit, row_off=d_off, slot_occ_off=slot_off)
+                for i, n in enumerate(names):
+                    by_slot[n] = out[i]
+                continue
             if sharded:  # R GPUs: the embedding worker's fan-out runs inside the chunk's sharded worker (sized above)
                 wk, kw = step[(dim, k)]
                 with g["lock"]:

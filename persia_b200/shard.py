@@ -340,12 +340,44 @@ class EmbeddingShard:
         N.check(self.lib.pb_dump_nodes(self.h, _ptr(signs), signs.numel(), int(lo), int(n), _ptr(out),
                                        _stream(self.device)))
 
+    def export_view(self):
+        """The table's view blob (bytes) for peers that read it in place (pb_table_export_view).  From now on the table
+        is read-only but for set_entries and checkpoint / packet inserts, and it must outlive every view of it."""
+        buf = C.create_string_buffer(int(self.lib.pb_table_view_bytes()))
+        N.check(self.lib.pb_table_export_view(self.h, buf))
+        return buf.raw
+
     def close(self):
         if getattr(self, "h", None):
             self.lib.pb_table_destroy(self.h)
             self.h = None
         if getattr(self, "host_tier", None) is not None:  # after the table it stands behind
             self.host_tier.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class TableView:
+    """Another rank's exported table as this process reads it on `device` (pb_view_open / pb_view_close): through CUDA
+    IPC when the blob comes from another process, through its own pointers when from this one."""
+
+    def __init__(self, blob, device=0):
+        self.lib = N.load()
+        self.device = torch.device("cuda", device) if not isinstance(device, torch.device) else device
+        blob = bytes(blob)
+        assert len(blob) == int(self.lib.pb_table_view_bytes()), "not a table view blob"
+        h = C.c_void_p()
+        N.check(self.lib.pb_view_open(self.device.index or 0, blob, C.byref(h)))
+        self.h = h
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.pb_view_close(self.h)
+            self.h = None
 
     def __del__(self):
         try:

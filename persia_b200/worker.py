@@ -436,3 +436,128 @@ class ShardedRawWorker(ShardedEmbeddingWorker):
         for r, w, ph in _by_phase(workers, N.PHASE_SEND, N.PHASE_SERVE):
             w.backward_raw(grads[r], scales[r] if scales is not None else 1.0, phases=ph, status=sts[r])
         return sts
+
+
+class RemoteReader:
+    """Inference on R GPUs one rank at a time (pb_forward_remote / pb_forward_raw_remote): this rank's requests are
+    served alone, whatever its peers do.  The requesting GPU probes each owner's index and reads its rows in place,
+    through views of the owners' exported tables (EmbeddingShard.export_view, TableView); no flag, no collective, no
+    kernel on the owner.  Outputs are bit for bit the collective path's inference forwards (ShardedEmbeddingWorker /
+    ShardedRawWorker with training=False).
+
+    Exporting makes every table read-only but for set_entries and checkpoint / incremental-packet inserts, which the
+    reads see whole or not at all (include/persia_b200.h).  So a reader serves Infer jobs; a training job's tables stay
+    on the collective path.  The views close before the tables (close() first), and every owner outlives its peers'
+    views.
+
+    One batch context per slot chunk (the slots one call serves, keyed by their prefixes), grown when a larger batch
+    comes.  Two ways to build the readers of a box, like ShardedEmbeddingWorker's:
+      * `RemoteReader.distributed(shard, group)`: one process per GPU; the blobs are exchanged with one all_gather_object.
+      * `RemoteReader.local_group(shards)`: R virtual ranks on one GPU in one process (views from blobs of this pid)."""
+
+    def __init__(self, shard, views, rank, stream=None):
+        """shard: this rank's EmbeddingShard (exported); views: one TableView per rank (None at `rank`: its own table is
+        probed directly)."""
+        self.lib = N.load()
+        self.shard, self.views, self.rank, self.R = shard, list(views), int(rank), len(views)
+        self.device, self.dim, self.stream = shard.device, shard.dim, stream
+        self._views = (C.c_void_p * self.R)(*[(v.h.value if v is not None else None) for v in self.views])
+        self._ctxs = {}  # (kind, prefixes, sqrt_scaling, prefix_bit) -> [BatchContext, max occurrences, max rows]
+
+    @classmethod
+    def local_group(cls, shards, streams=None):
+        """R virtual ranks on one GPU: every shard is exported and viewed by the others (same process).  streams: one per
+        rank (default: a new stream each)."""
+        blobs = [s.export_view() for s in shards]
+        return [cls(s, [SH.TableView(b, s.device) if q != r else None for q, b in enumerate(blobs)], r,
+                    stream=streams[r] if streams else torch.cuda.Stream(device=s.device))
+                for r, s in enumerate(shards)]
+
+    @classmethod
+    def distributed(cls, shard, group=None, stream=None):
+        """One process per GPU: exports this rank's shard and exchanges the blobs with one all_gather_object over the
+        group (collective); the peers' tables are then opened through CUDA IPC."""
+        import torch.distributed as dist
+
+        grp = group if group is not None else dist.group.WORLD
+        world, rank = dist.get_world_size(grp), dist.get_rank(grp)
+        blobs = [None] * world
+        dist.all_gather_object(blobs, shard.export_view(), group=grp)
+        views = [SH.TableView(b, shard.device) if q != rank else None for q, b in enumerate(blobs)]
+        dist.barrier(group=grp)  # (no rank reads before every view is open)
+        return cls(shard, views, rank, stream=stream)
+
+    def _torch_stream(self):
+        return self.stream if self.stream is not None else torch.cuda.current_stream(self.device)
+
+    def _st(self):
+        return C.c_void_p(self._torch_stream().cuda_stream)
+
+    def _ctx(self, key, n_occ, rows):
+        """The batch context of `key`, grown (persia_core.ctx_occurrences' rule) when n_occ ids in `rows` rows do not fit."""
+        from .persia_core import ctx_occurrences
+
+        got = self._ctxs.get(key)
+        if got is not None and n_occ <= got[1] and rows <= got[2]:
+            return got[0]
+        occ = max(ctx_occurrences(n_occ, rows), got[1] if got else 0)
+        out_rows = max(2 * rows, 1024, got[2] if got else 0)
+        if got is not None:
+            self._torch_stream().synchronize()
+            got[0].close()
+        _, prefixes, sqrt, prefix_bit = key
+        ctx = SH.BatchContext(occ, out_rows, list(prefixes), list(sqrt) if sqrt else None, prefix_bit, self.device)
+        self._ctxs[key] = [ctx, occ, out_rows]
+        return ctx
+
+    def forward(self, ids, batch, prefixes, sqrt_scaling=None, prefix_bit=8, row_off=None, slot_occ_off=None, out=None):
+        """ShardedEmbeddingWorker.forward(training=False) of this rank alone: ids slot-major (device int64 bits), one id
+        per sample per slot unless row_off (device int32 CSR offsets) and slot_occ_off (host list) are given; the slots'
+        index prefixes and sqrt scaling.  Returns f16 [n_slots, batch, dim]."""
+        ids = SH._as_i64_bits(ids)
+        S = len(prefixes)
+        if slot_occ_off is None:
+            slot_occ_off = [s * batch for s in range(S + 1)]
+        key = ("sum", tuple(int(p) for p in prefixes), tuple(bool(x) for x in sqrt_scaling) if sqrt_scaling else None,
+               int(prefix_bit))
+        ctx = self._ctx(key, ids.numel(), S * batch)
+        if out is None:
+            out = torch.empty((S, batch, self.dim), dtype=torch.float16, device=self.device)
+        if row_off is not None:
+            assert row_off.dtype == torch.int32 and row_off.is_contiguous()
+        N.check(self.lib.pb_forward_remote(self.shard.h, self._views, self.R, self.rank, ctx.h, SH._ptr(ids), ids.numel(),
+                                           SH._ptr(row_off), SH._slot_offsets(slot_occ_off, S), int(batch), SH._ptr(out),
+                                           self._st()))
+        return out
+
+    def forward_raw(self, ids, batch, sample_fixed_size, prefix, prefix_bit=8, row_off=None, out=None):
+        """ShardedRawWorker.forward_raw(training=False) of this rank alone, for the raw slot of index prefix `prefix`:
+        (table f16 [n_occ+1, dim] of which rows [0, U] are valid, index i64 [batch*fixed], non_empty i64 of which
+        counts[1] entries are valid, sample_id_num i32 [batch], counts i32 [2] = (U, non-empty entries)), on the device.
+        out: those five buffers from an earlier call of the same sizes (captured calls reuse them)."""
+        ids = SH._as_i64_bits(ids)
+        n, fixed = ids.numel(), int(sample_fixed_size)
+        ctx = self._ctx(("raw", (int(prefix),), None, int(prefix_bit)), n, batch)
+        if out is None:
+            out = SH._raw_outputs(n, batch, fixed, self.dim, self.device)
+        N.check(self.lib.pb_forward_raw_remote(self.shard.h, self._views, self.R, self.rank, ctx.h, SH._ptr(ids), n,
+                                               SH._raw_row_off(row_off, batch), int(batch), fixed, *map(SH._ptr, out),
+                                               self._st()))
+        table, index, non_empty, num, counts = out
+        return table, index, non_empty, num[:batch], counts
+
+    def close(self):
+        """Closes the contexts and the views (before the tables they view: their owners close those)."""
+        for ctx, _, _ in self._ctxs.values():
+            ctx.close()
+        self._ctxs = {}
+        for v in self.views:
+            if v is not None:
+                v.close()
+        self.views = [None] * self.R
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
