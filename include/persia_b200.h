@@ -519,6 +519,20 @@ uint64_t pb_table_view_bytes(void);
 /* Writes t's view blob to h_blob (pb_table_view_bytes() bytes) and makes t read-only (above).  Allocates the table if
  * needed (so the optimizer must be registered) and synchronises the device the first time. */
 int pb_table_export_view(pb_table* t, void* h_blob);
+/* The live export: the same blob, opened by pb_view_open and read by pb_forward_remote / pb_forward_raw_remote as they
+ * are, but t stays writable: training forwards and backwards, pb_update, eviction checks, pb_set_rows, pb_table_clear,
+ * dumps and loads all run.  So a training job serves its forwards that do not train one rank at a time.
+ * Live consistency rule: the write-sequence word is odd from before the first cell to after the last row each of these
+ * changes: a capacity sweep (tombstones cells, frees rows the next admission gives to another sign), an index rebuild
+ * (cells go EMPTY and are re-inserted), pb_table_clear and pb_set_rows.  The sweep and the rebuild move it inside the
+ * eviction check's own kernels (no launch is added; a captured step stays one graph with no host sync).  So a read never
+ * returns another sign's row, and a sign resident before and after the read is never a false miss.  The word does not
+ * cover an admission (the index publishes a row only once it is initialised; a reader waits on an unpublished one) nor
+ * an optimizer step on a resident row: a read beside a step returns, per element, the value before or after that step,
+ * the stale read a forward beside a backward on one GPU may give too.  A read that waits out the budget counts in
+ * the reader's pb_table_counters[4] and reads zeros.  A table is exported one way only (the other call: PB_ERR_STATE);
+ * the host-tier refusals and the ownership rule are the frozen export's, and a live table refuses pb_table_attach_tier. */
+int pb_table_export_live_view(pb_table* t, void* h_blob);
 typedef struct pb_view pb_view;
 /* A view of an exported table for reads issued on `device`.  A blob of another process: each handle is opened with
  * cudaIpcOpenMemHandle(cudaIpcMemLazyEnablePeerAccess); of this process: its pointers are used as they are (peer access

@@ -368,6 +368,9 @@ class TrainCtx(EmbeddingCtx):  # ctx.py:655-1055
         self.backward_engine.launch(self.backward_workers_size)
 
     def _exit(self):
+        """On R GPUs every rank reads its peers' tables in place for forwards that do not train (persia_core
+        _start_remote), so a peer's table must outlive this rank's views of it: the ranks stop together, ending with a
+        barrier before any rank resets or exits (the views close first, persia_core._close_remote)."""
         super()._exit()
         self.backward_engine.shutdown()
 

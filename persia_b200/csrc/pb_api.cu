@@ -127,6 +127,9 @@ struct pb_table {
   // (writable); `seq` is the write-sequence word pb_set_rows keeps odd while it writes
   bool exported = false;
   uint32_t* seq = nullptr;
+  // pb_table_export_live_view: peers read in place while the table keeps training; sweeps, rebuilds, pb_set_rows and
+  // pb_table_clear keep `seq` odd while they move cells or reuse rows (one table, one export mode)
+  bool live = false;
 };
 
 struct pb_ctx {
@@ -285,7 +288,8 @@ int evict_check(pb_table* t, cudaStream_t st, uint32_t blocks = 0) {
                       t->rebuild_rows, h->evict_ws, h->rebuild_keys, h->rebuild_rows, t->move_cells, st, blocks);
     return PB_OK;
   }
-  launch_evict(t->d, t->evict_low, t->evict_target, keep, t->evict_ws, t->rebuild_keys, t->rebuild_rows, st);
+  launch_evict(t->d, t->evict_low, t->evict_target, keep, t->evict_ws, t->rebuild_keys, t->rebuild_rows,
+               t->live ? t->seq : nullptr, st);
   return PB_OK;
 }
 
@@ -753,6 +757,7 @@ int pb_table_create_host(int device, const pb_table_cfg* cfg, pb_table** out) {
 int pb_table_attach_tier(pb_table* t, pb_table* tier) {
   if (!t || !tier) return fail(PB_ERR_INVALID, "null argument");
   if (int rc = writable(t)) return rc;  // (an exported table can have no tier: peers could not read its host rows)
+  if (t->live) return fail(PB_ERR_STATE, "a live-exported table cannot take a host tier: peers could not read its host rows");
   if (t->host || !tier->host) return fail(PB_ERR_INVALID, "the tier must be a host table (pb_table_create_host) behind an HBM table");
   if (t->tier || t->tier_of || tier->tier_of || tier->tier) return fail(PB_ERR_STATE, "one of the tables already has a tier or is one");
   if (t->device != tier->device) return fail(PB_ERR_INVALID, "the tables live on different devices");
@@ -1024,9 +1029,11 @@ int pb_table_clear(pb_table* t, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
   if (int rc = call.begin(t, st, CALL_ALL)) return rc;
+  if (t->live) launch_seq_bump(t->seq, true, st);  // peers reading in place wait until every cell is EMPTY again
   launch_fill_cells(t->d.cells, (uint64_t)t->d.n_cells + N_SPECIAL, st);
   PB_CUDA(cudaMemsetAsync(t->d.counters, 0, sizeof(uint32_t) * CTR_COUNT, st));
   PB_CUDA(cudaMemsetAsync(t->d.row_tick, 0, sizeof(uint32_t) * (size_t)t->d.capacity, st));
+  if (t->live) launch_seq_bump(t->seq, false, st);
   return t->tier ? pb_table_clear(t->tier, stream) : PB_OK;
 }
 
@@ -1105,12 +1112,13 @@ int pb_set_rows(pb_table* t, const uint64_t* d_signs, const float* d_entries, ui
   // with a tier: a tier-held sign is first moved back (it then lives in one table), and an entry the HBM table has no
   // row for goes to the tier
   restore_ids(t, false, sl, d_signs, n, st);
-  // an exported table: peers reading it in place see the write-sequence word odd from before the first cell it may
-  // claim to after the last entry it writes (pb_remote.cu), and read those items again
-  if (t->exported) launch_seq_bump(t->seq, true, st);
+  // an exported table, frozen or live: peers reading it in place see the write-sequence word odd from before the first
+  // cell it may claim to after the last entry it writes (pb_remote.cu), and read those items again
+  const bool bracket = t->exported || t->live;
+  if (bracket) launch_seq_bump(t->seq, true, st);
   launch_probe(MODE_SET, false, t->d, t->hy, t->op, sl, d_signs, n, t->scratch, st);
   launch_copy_entries(true, t->d, t->scratch, n, const_cast<float*>(d_entries), nullptr, st);
-  if (t->exported) launch_seq_bump(t->seq, false, st);
+  if (bracket) launch_seq_bump(t->seq, false, st);
   if (t->tier) launch_tier_set(t->d, t->tier->d, t->hy, t->op, d_signs, t->scratch, n, d_entries, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
@@ -2445,15 +2453,20 @@ int begin_remote(pb_table* own, pb_ctx* c, RemoteDev& rv, uint32_t rank, size_t 
   if (int rc = call.begin(own, st, CALL_INDEX)) return rc;
   if (int rc = ensure_alloc(own)) return rc;
   rv.t[rank] = own->d;
-  rv.seq[rank] = own->seq;  // (null unless exported: then only calls ordered with this one write it)
+  rv.seq[rank] = own->seq;  // (null unless exported; a live table's training calls need not be ordered with this one)
   return grow_stage(c->remote_stage, c->remote_stage_floats, floats ? floats : 1, st);
 }
 }  // namespace
 
 uint64_t pb_table_view_bytes(void) { return sizeof(ViewBlob); }
 
-int pb_table_export_view(pb_table* t, void* h_blob) {
+namespace {
+// pb_table_export_view (live = false) and pb_table_export_live_view (live = true): one blob layout, one reader
+int export_blob(pb_table* t, void* h_blob, bool live) {
   if (!t || !h_blob) return fail(PB_ERR_INVALID, "null argument");
+  if (live ? t->exported : t->live)
+    return fail(PB_ERR_STATE, live ? "the table was exported frozen (pb_table_export_view): one table, one export mode"
+                                   : "the table was exported live (pb_table_export_live_view): one table, one export mode");
   if (t->host || t->tier_of)
     return fail(PB_ERR_STATE, "a host tier cannot be exported: its rows are pinned host memory no peer process can map");
   if (t->tier)
@@ -2488,9 +2501,15 @@ int pb_table_export_view(pb_table* t, void* h_blob) {
   b.n_cells = t->d.n_cells;
   b.capacity = t->d.capacity;
   std::memcpy(h_blob, &b, sizeof(b));
-  t->exported = true;
+  if (live) t->live = true;
+  else t->exported = true;
   return PB_OK;
 }
+}  // namespace
+
+int pb_table_export_view(pb_table* t, void* h_blob) { return export_blob(t, h_blob, false); }
+
+int pb_table_export_live_view(pb_table* t, void* h_blob) { return export_blob(t, h_blob, true); }
 
 int pb_view_open(int device, const void* h_blob, pb_view** out) {
   if (!h_blob || !out) return fail(PB_ERR_INVALID, "null argument");
@@ -2612,3 +2631,12 @@ namespace pb { void set_hot_trace(unsigned long long* p); }
 extern "C" void pb_debug_hot_trace(void* d_buf) { pb::set_hot_trace(reinterpret_cast<unsigned long long*>(d_buf)); }
 // measuring aid (not in include/persia_b200.h): pb_tier_stage's grid (scripts/host_tier_bench.py --stage-blocks)
 extern "C" void pb_debug_stage_blocks(uint32_t blocks) { g_stage_blocks = blocks ? blocks : PB_NUM_SMS; }
+// measuring aid (not in include/persia_b200.h): an exported table's write-sequence word, read after the device is idle
+// (scripts/live_remote_bench.py: how many owner write windows a reader's requests overlapped)
+extern "C" int pb_debug_table_seq(pb_table* t, uint32_t* h_out) {
+  if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
+  if (!t->seq) return fail(PB_ERR_STATE, "the table was not exported");
+  DeviceGuard g(t->device);
+  PB_CUDA(cudaMemcpy(h_out, t->seq, sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  return PB_OK;
+}

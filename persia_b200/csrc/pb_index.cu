@@ -140,6 +140,22 @@ __global__ void k_fill_cells(Cell* cells, uint64_t n) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// A live-exported table (pb_table_export_live_view) keeps training while peers read its index and rows in place
+// (pb_remote.cu).  A sweep tombstones cells and frees rows the next admission hands to another sign; a rebuild empties
+// the index and fills it again.  So the table's write-sequence word `seq` is odd from before the first cell either
+// changes to after the last, and a reader whose probe or row read overlapped that window reads the item again.  The
+// word moves inside kernels the check launches anyway, so a live table's step launches what any other table's does and
+// stays one graph: the one-thread plan kernels that decide the sweep and the rebuild raise it (a grid's first block is
+// not ordered before its other blocks, the kernel before the grid is), and the last block of the rebuild's re-insert
+// lowers it.  seq null (every other table): none of this runs.
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void seq_step(uint32_t* seq) {
+  __threadfence_system();  // (lowering: every cell and row written before)
+  *reinterpret_cast<volatile uint32_t*>(seq) = *seq + 1u;
+  __threadfence_system();  // (raising: before any cell or row is written)
+}
+
+// ------------------------------------------------------------------------------------------------
 // Capacity: the reference's EvictionMap drops the least recently used entry whenever an insert pushes it over
 // capacity (eviction_map.rs:76-97).  Here recency is the batch number kept in row_tick and
 // eviction is a sweep run between batches when free storage is low: (1) histogram of row ages over the occupied
@@ -172,7 +188,7 @@ __global__ void __launch_bounds__(256) k_evict_hist(TableDev t, uint32_t* __rest
   }
 }
 
-__global__ void k_evict_threshold(uint32_t keep, uint32_t* __restrict__ ev) {
+__global__ void k_evict_threshold(uint32_t keep, uint32_t* __restrict__ ev, uint32_t* __restrict__ seq) {
   if (threadIdx.x || !ev[2]) return;
   uint32_t want = ev[1], got = 0, thr = 0xFFFFFFFFu;
   for (uint32_t a = EV_BINS; a-- > 0 && a > keep;) {  // oldest first; ages <= keep are protected
@@ -181,6 +197,7 @@ __global__ void k_evict_threshold(uint32_t keep, uint32_t* __restrict__ ev) {
     if (got >= want) break;
   }
   ev[0] = got ? thr : 0xFFFFFFFFu;
+  if (seq && got) seq_step(seq);  // the sweep below runs: odd (k_rebuild_plan or the rebuild lowers it)
 }
 
 __global__ void __launch_bounds__(256) k_evict_sweep(TableDev t, uint32_t* __restrict__ ev) {
@@ -212,10 +229,16 @@ __global__ void __launch_bounds__(256) k_evict_sweep(TableDev t, uint32_t* __res
 // ------------------------------------------------------------------------------------------------
 static_assert(EV_RB + 2 <= EVICT_WS_WORDS, "eviction workspace too small");
 
-__global__ void k_rebuild_plan(TableDev t, uint32_t* __restrict__ ev) {
+__global__ void k_rebuild_plan(TableDev t, uint32_t* __restrict__ ev, uint32_t* __restrict__ seq) {
   if (threadIdx.x) return;
-  ev[EV_RB] = t.counters[CTR_USED] > t.n_cells - t.n_cells / 8 ? 1u : 0u;
+  const uint32_t rb = t.counters[CTR_USED] > t.n_cells - t.n_cells / 8 ? 1u : 0u;
+  ev[EV_RB] = rb;
   ev[EV_RB + 1] = 0u;
+  if (!seq) return;
+  ev[EV_DONE] = 0u;
+  // the word is odd iff a sweep ran (k_evict_threshold): a rebuild keeps it odd or raises it, else the sweep is over
+  const bool swept = ev[2] && ev[0] != 0xFFFFFFFFu;
+  if (swept != (rb != 0u)) seq_step(seq);
 }
 
 __global__ void __launch_bounds__(256) k_rebuild_compact(TableDev t, uint32_t* __restrict__ ev, uint64_t* __restrict__ keys,
@@ -242,8 +265,9 @@ __global__ void __launch_bounds__(256) k_rebuild_clear(TableDev t, const uint32_
 }
 
 // keys are distinct and no cell is a tombstone: a CAS on EMPTY is all an insertion needs
-__global__ void __launch_bounds__(256) k_rebuild_insert(TableDev t, const uint32_t* __restrict__ ev,
-                                                        const uint64_t* __restrict__ keys, const uint32_t* __restrict__ rows) {
+__global__ void __launch_bounds__(256) k_rebuild_insert(TableDev t, uint32_t* __restrict__ ev,
+                                                        const uint64_t* __restrict__ keys, const uint32_t* __restrict__ rows,
+                                                        uint32_t* __restrict__ seq) {
   if (!ev[EV_RB]) return;
   const uint32_t n = min(ev[EV_RB + 1], t.capacity);
   if (blockIdx.x == 0 && threadIdx.x == 0) t.counters[CTR_USED] = n;
@@ -258,6 +282,13 @@ __global__ void __launch_bounds__(256) k_rebuild_insert(TableDev t, const uint32
           done = true;
         }
       }
+    }
+  }
+  if (seq) {  // the last block to finish lowers the word once every block's cells are written
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      __threadfence();
+      if (atomicAdd(&ev[EV_DONE], 1u) == gridDim.x - 1) seq_step(seq);
     }
   }
 }
@@ -286,12 +317,13 @@ __global__ void __launch_bounds__(256) k_index_stats(TableDev t, uint32_t* __res
 // ------------------------------------------------------------------------------------------------
 // launchers (host)
 // ------------------------------------------------------------------------------------------------
-void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st, uint32_t blocks) {
+void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st, uint32_t blocks,
+                    uint32_t* seq) {
   const uint32_t g = blocks ? blocks : PB_NUM_SMS * 8;
-  PB_LAUNCH(k_rebuild_plan, 1, 32, 0, st, t, ev);
+  PB_LAUNCH(k_rebuild_plan, 1, 32, 0, st, t, ev, seq);
   PB_LAUNCH(k_rebuild_compact, g, 256, 0, st, t, ev, keys, rows);
   PB_LAUNCH(k_rebuild_clear, g, 256, 0, st, t, ev);
-  PB_LAUNCH(k_rebuild_insert, g, 256, 0, st, t, ev, keys, rows);
+  PB_LAUNCH(k_rebuild_insert, g, 256, 0, st, t, ev, keys, rows, seq);
 }
 
 void launch_index_stats(const TableDev& t, uint32_t* out, cudaStream_t st) {
@@ -376,12 +408,12 @@ void launch_export_signs(const TableDev& t, uint64_t* signs, uint32_t* recency, 
 }
 
 void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys,
-                  uint32_t* rb_rows, cudaStream_t st) {
+                  uint32_t* rb_rows, uint32_t* seq, cudaStream_t st) {
   PB_LAUNCH(k_evict_plan, 1, 256, 0, st, t, low_water, target_free, ev);
   PB_LAUNCH(k_evict_hist, PB_NUM_SMS * 8, 256, 0, st, t, ev);
-  PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
+  PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev, seq);
   PB_LAUNCH(k_evict_sweep, PB_NUM_SMS * 8, 256, 0, st, t, ev);
-  launch_rebuild(t, ev, rb_keys, rb_rows, st);
+  launch_rebuild(t, ev, rb_keys, rb_rows, st, 0, seq);
 }
 
 // The HBM table's plan and threshold count its victims; the tier's own sweep (gated on the flag launch_tier_plan sets)
@@ -393,10 +425,10 @@ void launch_evict_tier(const TableDev& h, const TableDev& t, const HyperDev& hy,
   const uint32_t g = blocks ? blocks : PB_NUM_SMS * 8;
   PB_LAUNCH(k_evict_plan, 1, 256, 0, st, h, low_water, target_free, ev);
   PB_LAUNCH(k_evict_hist, g, 256, 0, st, h, ev);
-  PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev);
+  PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, keep, ev, nullptr);
   launch_tier_plan(h, t, ev, tev, st);
   PB_LAUNCH(k_evict_hist, g, 256, 0, st, t, tev);
-  PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, 0u, tev);  // no batch holds a tier row: only the current batch number's stay
+  PB_LAUNCH(k_evict_threshold, 1, 32, 0, st, 0u, tev, nullptr);  // no batch holds a tier row: only the current batch number's stay
   PB_LAUNCH(k_evict_sweep, g, 256, 0, st, t, tev);
   launch_tier_move(h, t, hy, op, ev, tev, rb_keys, rb_rows, move_cells, st, blocks);  // (rebuild buffers free until below)
   launch_rebuild(h, ev, rb_keys, rb_rows, st, blocks);

@@ -311,9 +311,13 @@ void launch_export_signs(const TableDev& t, uint64_t* signs, uint32_t* recency, 
 constexpr uint32_t EV_BINS = 1024;        // ev[3..]: age histogram (last bin = older)
 constexpr uint32_t EV_RB = 3 + EV_BINS;   // ev[EV_RB] rebuild flag, ev[EV_RB + 1] pairs compacted
 constexpr uint32_t EV_MOVE = EV_RB + 2;   // a tier's ev[EV_MOVE]: HBM victims listed for the move (pb_tier.cu)
-constexpr uint32_t EVICT_WS_WORDS = EV_MOVE + 1;
+constexpr uint32_t EV_DONE = EV_MOVE + 1;  // ev[EV_DONE]: blocks of the rebuild's re-insert that finished (seq != null)
+constexpr uint32_t EVICT_WS_WORDS = EV_DONE + 1;
+// seq: a live-exported table's write-sequence word (pb_table_export_live_view), null otherwise.  The plan kernels and
+// the rebuild's last block keep it odd from before the first cell the sweep or the rebuild changes to after the last;
+// no kernel is added, and with seq null nothing new runs.
 void launch_evict(const TableDev& t, uint32_t low_water, uint32_t target_free, uint32_t keep, uint32_t* ev, uint64_t* rb_keys,
-                  uint32_t* rb_rows, cudaStream_t st);
+                  uint32_t* rb_rows, uint32_t* seq, cudaStream_t st);
 void launch_index_stats(const TableDev& t, uint32_t* out, cudaStream_t st);
 // host-memory tier (pb_tier.cu).  h: the HBM table, t: its tier (rows in mapped pinned host memory).
 // The eviction check of a table with a tier: the HBM sweep's victims move into the tier (whose own sweep first drops its
@@ -353,7 +357,8 @@ void launch_tier_where(const TableDev& h, const TableDev& t, const uint64_t* sig
 // pb_set_rows: entries the HBM table had no row for are stored in the tier
 void launch_tier_set(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op, const uint64_t* signs,
                      const uint32_t* occ_cell, uint32_t n, const float* entries, cudaStream_t st);
-void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st, uint32_t blocks = 0);
+void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st, uint32_t blocks = 0,
+                    uint32_t* seq = nullptr);
 // checkpoint images (pb_dump.cu).  The part of a sign in a background dump: splitmix64(sign) % n_parts, with
 // splitmix64(x): z = x + 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
 // z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31)   (include/persia_b200.h, pb_table_dump_part)

@@ -10,8 +10,9 @@
 // then the collective path's own pooling (k_expand_copy / k_expand_pool, or k_raw_fill for a raw slot) reads the
 // staging.  No flag, no peer kernel, no collective.
 //
-// Consistency with inserts (pb_set_rows on an exported table): the owner keeps a write-sequence word, odd while an
-// insert runs.  A lane group reads it before its probe and copy and again after them; while it is odd, or if it
+// Consistency with writes: the owner keeps a write-sequence word, odd while an insert runs (pb_set_rows on an exported
+// table) and, on a table exported live that keeps training, while a capacity sweep, an index rebuild (pb_index.cu) or a
+// clear runs.  A lane group reads it before its probe and copy and again after them; while it is odd, or if it
 // changed, the item is read again.  A returned row is therefore the entry before an insert or after it, never a mix.
 // A row still ROW_PENDING in the index is an insert in flight: the word has moved, so it is read again as well.
 #include "pb_device.cuh"

@@ -110,6 +110,7 @@ SYMBOLS = {
     "pb_backward_raw_sharded": (_i32, [_vp, _vp, _vp, _vp, _i32, C.c_float, _vp, _vp, _i32]),
     "pb_table_view_bytes": (_u64, []),
     "pb_table_export_view": (_i32, [_vp, _vp]),
+    "pb_table_export_live_view": (_i32, [_vp, _vp]),
     "pb_view_open": (_i32, [_i32, _vp, C.POINTER(_vp)]),
     "pb_view_close": (_i32, [_vp]),
     "pb_forward_remote": (_i32, [_vp, C.POINTER(_vp), _u32, _u32, _vp, _vp, _u32, _vp, C.POINTER(_u32), _u32, _vp, _vp]),

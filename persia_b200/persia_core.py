@@ -22,8 +22,10 @@ staleness rules (persia_b200/engine.py), `Backward` applies updates in the calle
 write and read the reference's `.emb` checkpoint files (persia_b200/checkpoint.py).  With the global config's
 `enable_incremental_update` on a Train job, the signs the tables step are flushed as the reference's `.inc` packets; an
 Infer job loads its checkpoint and applies them as they appear (persia_b200/incremental.py, `set_global_config`).
-An Infer job with `replica_size > 1` exports every table once its checkpoint is loaded and serves each forward that does
-not train on its rank alone, reading the owners' shards in place (_start_remote, worker.RemoteReader): no collective.
+At `replica_size > 1` every forward that does not train is served by its rank alone, reading the owners' shards in place
+(_start_remote, worker.RemoteReader): no collective.  An Infer job exports its tables frozen once its checkpoint is
+loaded; a Train job exports them live when its optimizer is registered, and its training forwards and backwards stay
+collective.
 """
 import os
 import queue
@@ -124,7 +126,7 @@ class _State:
         self.gcfg_raw = None  # the global config dict itself (keys parse_global_config does not carry)
         self.emb_dump = None  # the latest background dump (checkpoint.BackgroundDumper)
         self.emb_load = None  # the latest load (checkpoint.DeviceLoader)
-        self.remote = None  # Infer at replica_size > 1: dim -> RemoteReader (_start_remote): one rank serves alone
+        self.remote = None  # replica_size > 1: dim -> RemoteReader (_start_remote): one rank serves alone
 
     def global_config(self):
         """set_global_config's dict, else the PERSIA_GLOBAL_CONFIG yaml, else the reference's defaults."""
@@ -262,10 +264,10 @@ def reset():
 
 
 def _close_remote():
-    """Closes the Infer job's remote readers (their contexts and views of the peers' tables), if any: by reset(), and at
-    interpreter exit before any table (an atexit hook, so that the views never outlive this process's tables whatever
-    order the objects are collected in).  A peer's table must outlive this rank's views of it, so the ranks of an Infer
-    job stop serving together: end with a barrier (or dist.destroy_process_group after one) before any rank exits."""
+    """Closes the remote readers (their contexts and views of the peers' tables), if any: by reset(), and at interpreter
+    exit before any table (an atexit hook, so that the views never outlive this process's tables whatever order the
+    objects are collected in).  A peer's table must outlive this rank's views of it, so the ranks of an Infer or a Train
+    job stop together: end with a barrier (or dist.destroy_process_group after one) before any rank exits."""
     if _S.remote is not None:
         for rd in _S.remote.values():
             rd.close()
@@ -353,12 +355,15 @@ def _start_infer():
     _S.loader.start()
 
 
-def _start_remote():
-    """Infer on R GPUs: every dim group exports its table and the ranks exchange the blobs once (collective: every rank
-    registers its optimizer, hence starts its Infer job, alike).  From then on a forward that does not train is served
-    by the dim's RemoteReader (persia_b200/worker.py) on this rank alone: no _sharded_step, no all_reduce, so each rank
-    answers its own requests whatever its peers do, as the reference's servers answer each request alone.  The tables
-    are then read-only but for checkpoint loads and incremental packets, which the readers see whole or not at all."""
+def _start_remote(live=False):
+    """R GPUs: every dim group exports its table and the ranks exchange the blobs once (collective: every rank registers
+    its optimizer alike, an Infer job once its checkpoint is loaded, a Train job as its TrainCtx enters).  From then on a
+    forward that does not train is served by the dim's RemoteReader (persia_b200/worker.py) on this rank alone: no
+    _sharded_step, no all_reduce, so each rank answers its own requests whatever its peers do, as the reference's servers
+    answer each request alone.  Infer (live = False): the tables are then read-only but for checkpoint loads and
+    incremental packets, which the readers see whole or not at all.  Train (live = True): the tables keep training
+    through the collective path; a read never returns another sign's row, and beside an optimizer step it may see each
+    element before or after that step (include/persia_b200.h, pb_table_export_live_view)."""
     import torch.distributed as dist
 
     from .worker import RemoteReader
@@ -369,7 +374,7 @@ def _start_remote():
     blobs = {}
     for d, g in groups.items():
         with g["lock"]:
-            blobs[d] = g["shard"].export_view()
+            blobs[d] = g["shard"].export_live_view() if live else g["shard"].export_view()
     got = [None] * dist.get_world_size()
     dist.all_gather_object(got, blobs)  # one exchange for every dim
     rank = dist.get_rank()
@@ -390,6 +395,20 @@ def _start_remote():
 
 
 _CLOSE_AT_EXIT = False  # _close_remote is registered to run at interpreter exit
+
+
+def _start_train_remote():
+    """Train on R GPUs: once the optimizer is registered (every rank's TrainCtx registers it as it enters, in step), the
+    tables are exported live and the views exchanged (_start_remote), once.  Where torch.distributed is not initialised
+    nothing starts: the collective path, which needs it as well, then raises at the first forward, as before."""
+    import torch.distributed as dist
+
+    if _S.global_config()["job_type"] != "Train" or (_S.replica_size or 1) <= 1 or _S.remote is not None:
+        return
+    if not dist.is_initialized():
+        return
+    _S.ensure_config()
+    _start_remote(live=True)
 
 
 PACKET_CHUNK = 1 << 16  # entries of one pb_image_insert of a packet (device staging: PACKET_CHUNK x entry length floats)
@@ -909,7 +928,8 @@ def _forward_locked(batch, device_id, training):
             _S.raw_order = raw_names
         elif _S.raw_order != raw_names:
             raise RuntimeError("on R GPUs every batch must carry the same raw slots, in the same order")
-    # Infer on R GPUs: this rank alone reads the owners' shards (_start_remote); a Train job keeps the collective path
+    # R GPUs: a forward that does not train is read from the owners' shards by this rank alone (_start_remote), in Infer
+    # and Train jobs; a training forward takes the collective path
     remote = _S.remote if sharded and not training else None
     step = _sharded_step(feats, B, training, dev) if sharded and remote is None else {}
     pending = _Pending()
@@ -1437,6 +1457,7 @@ class OptimizerBase:  # optim.rs:8-66
         for g in _S.groups.values():
             g["shard"].set_optimizer(**_S.optimizer)
         _start_infer()  # job_type Infer: the servers load their checkpoint and start scanning for incremental updates
+        _start_train_remote()  # job_type Train on R GPUs: export the tables live for forwards that do not train
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -1681,6 +1702,10 @@ class PersiaCommonContext:
             g["shard"].configure(**_S.hyper)
 
     def get_embedding_from_data(self, batch, device_id=None):  # forward_directly (forward.rs:782-831)
+        """forward_directly: this rank's pending backwards are flushed first.  On R GPUs a batch that does not train is
+        then read from the owners' shards by this rank alone (_start_remote): it sees every update this rank handed
+        over, but updates its peers' owners have not applied yet may still be missing, the staleness the reference's
+        asynchronous backward workers give too."""
         return _forward(batch, device_id, training=True, direct=True)
 
     def get_embedding_from_bytes(self, data, device_id=None):

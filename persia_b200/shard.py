@@ -347,6 +347,16 @@ class EmbeddingShard:
         N.check(self.lib.pb_table_export_view(self.h, buf))
         return buf.raw
 
+    def export_live_view(self):
+        """The table's view blob (bytes) for peers that read it in place while it keeps training
+        (pb_table_export_live_view): the blob export_view gives, read by the same TableView and RemoteReader, but the
+        table stays writable.  Sweeps, index rebuilds, set_entries and clear are bracketed for the readers; a read beside
+        an optimizer step may see each element before or after it.  One table, one export mode; the table must outlive
+        every view of it."""
+        buf = C.create_string_buffer(int(self.lib.pb_table_view_bytes()))
+        N.check(self.lib.pb_table_export_live_view(self.h, buf))
+        return buf.raw
+
     def close(self):
         if getattr(self, "h", None):
             self.lib.pb_table_destroy(self.h)

@@ -445,10 +445,11 @@ class RemoteReader:
     kernel on the owner.  Outputs are bit for bit the collective path's inference forwards (ShardedEmbeddingWorker /
     ShardedRawWorker with training=False).
 
-    Exporting makes every table read-only but for set_entries and checkpoint / incremental-packet inserts, which the
-    reads see whole or not at all (include/persia_b200.h).  So a reader serves Infer jobs; a training job's tables stay
-    on the collective path.  The views close before the tables (close() first), and every owner outlives its peers'
-    views.
+    export_view makes every table read-only but for set_entries and checkpoint / incremental-packet inserts, which the
+    reads see whole or not at all (include/persia_b200.h): an Infer job's export.  A training job's tables are exported
+    live instead (EmbeddingShard.export_live_view, built into readers with this class's constructor): they keep training
+    collectively, and a read never returns another sign's row.  The views close before the tables (close() first), and
+    every owner outlives its peers' views.
 
     One batch context per slot chunk (the slots one call serves, keyed by their prefixes), grown when a larger batch
     comes.  Two ways to build the readers of a box, like ShardedEmbeddingWorker's:
