@@ -116,7 +116,7 @@ int pb_table_entry_len(pb_table* t, uint32_t* h_out);
  * refused because the shard is full, [4] in-kernel waits that gave up (must stay 0: a non-zero value voids the batch
  * that raised it).  Synchronises `stream`. */
 int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream);
-/* ---- host-memory tier: a table larger than HBM on one GPU ----------------------------------------------------------
+/* ---- host-memory tier: a table larger than HBM, on one GPU or behind each of R ------------------------------------
  * The reference's parameter server keeps every entry in host DRAM, bounded by `capacity`.  A tier is a second table
  * whose rows (embedding ++ optimizer state) live in mapped pinned host memory (cudaHostAllocMapped | Portable, not
  * write-combined); its index cells, row recency, free-row stack and counters live in HBM like any table's.  So HBM
@@ -143,8 +143,8 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream);
  * entry stays as it was.  A moved entry keeps its recency, and the tier ages rows by the HBM table's training-request
  * number: the union evicts least recently used first, and pb_table_export_signs of both tables merges into the
  * reference's list order.
- * pb_table_clear of the table clears its tier too.  Destroy the table before its tier.  The sharded calls refuse a
- * table with a tier.
+ * pb_table_clear of the table clears its tier too.  Destroy the table before its tier.  The sharded calls serve a
+ * table with a tier on its owner rank by the same rules (see the R-GPU calls below); exporting it stays refused.
  *
  * Staging (pb_tier_stage): the ids of batch i+1 are known while batch i trains, and moving an entry never changes its
  * value, so the moves of request i+1 can run one batch ahead, on a stream of their own, beside batch i's dense step and
@@ -424,7 +424,15 @@ int pb_backward_raw(pb_table* t, pb_ctx* c, const void* d_grad, int is_f16, floa
  * step.  A rank's receive area is pb_xchg_bytes() bytes of zero-initialised device memory that all ranks can store
  * to (CUDA peer access / symmetric memory); h_peer_base[q] is rank q's area as mapped in this process, 256-byte
  * aligned; cap = slots per (source, owner) pair, i.e. the most distinct signs one rank may request of one owner in one
- * batch; rows_f32 != 0 returns f32 rows (needed for ragged layouts, which pool on the requester; f16 otherwise). */
+ * batch; rows_f32 != 0 returns f32 rows (needed for ragged layouts, which pool on the requester; f16 otherwise).
+ *
+ * A shard may have a host tier (pb_table_attach_tier): R GPUs then hold R x (HBM + tier) entries.  Its owner serves the
+ * requests it receives as one GPU serves its own (PB_PHASE_SERVE of the summation and raw forwards alike): a training
+ * request's tier-held signs are first moved into free HBM rows (a sign that finds none stays in the tier, reads zeros,
+ * takes no gradient and counts in pb_tier_stats[4]); an inference request (training == 0) reads them in place and moves
+ * nothing.  The eviction check in each rank's SEND moves its own shard's victims into its tier, and the backwards step
+ * only HBM rows: the rows of pending requests are never victims.  Nothing else changes: no host synchronisation, and a
+ * step stays capturable.  A requester cannot tell a tiered owner from an untiered one. */
 typedef struct pb_xchg pb_xchg;
 uint64_t pb_xchg_bytes(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32);
 int pb_xchg_create(int device, uint32_t R, uint32_t rank, uint32_t cap, uint32_t dim, int rows_f32,

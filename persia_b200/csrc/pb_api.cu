@@ -1948,9 +1948,8 @@ int check_prepared(const pb_ctx* c, const Phases& ph, int kind, uint32_t n_occ, 
 
 // What a sharded call needs of its exchange: the table's device and dim, and f32 rows where `need_f32_rows` (refused
 // with `f32_message`).  A backward passes its context, whose device it has not checked yet; a forward passes none
-// (check_forward has checked it), and refuses a table with a host tier as well.
+// (check_forward has checked it).
 int check_exchange(const pb_table* t, const pb_ctx* c, const pb_xchg* x, bool need_f32_rows, const char* f32_message) {
-  if (!c && t->tier) return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no sharded calls)");
   if (c && (t->device != c->device || t->device != x->device))
     return fail(PB_ERR_INVALID, "table, context and exchange live on different devices");
   if (t->device != x->device) return fail(PB_ERR_INVALID, "table and exchange live on different devices");
@@ -1960,11 +1959,14 @@ int check_exchange(const pb_table* t, const pb_ctx* c, const pb_xchg* x, bool ne
 }
 
 // The owner's part of a sharded forward (PB_PHASE_SERVE), shared by the summation and the raw calls: the rows of the
-// signs sent to this shard, into the requesters' areas.
+// signs sent to this shard, into the requesters' areas.  With a host tier, as on one GPU: a training request's tier-held
+// signs move into HBM rows first (a sign that finds no free row stays in the tier, counted, and reads zeros), so the
+// backward, the eviction check and the incremental marks see only HBM rows; an inference request reads them in place.
 void serve_lookup(pb_table* t, pb_xchg* x, int training, const Phases& ph, cudaStream_t st) {
   ph.await(x, XC_FLAG_SIGN, st);
   if (training && x->u_dirty) launch_uclear(x->d, st);  // a training batch whose gradients never came left its rows noted
-  launch_owner_lookup(training != 0, t->d, t->hy, t->op, x->d, st);
+  if (training && t->tier) launch_tier_restore_recv(t->d, t->tier->d, t->hy, t->op, x->d, st);
+  launch_owner_lookup(training != 0, t->d, t->tier ? &t->tier->d : nullptr, t->hy, t->op, x->d, st);
   if (training) x->u_dirty = true;
   ph.post(x, XC_FLAG_ROW, nullptr, st);
 }

@@ -237,8 +237,9 @@ void launch_link_items(const SlotsDev& sl, const BatchDev& b, const XchgDev& x, 
 void launch_signal(const XchgDev& x, int phase, const uint32_t* counts, cudaStream_t st);
 void launch_wait(const XchgDev& x, int phase, int src /* -1: every source */, cudaStream_t st);
 void launch_signal_wait(const XchgDev& x, int phase, const uint32_t* counts, cudaStream_t st);
-void launch_owner_lookup(bool training, const TableDev& t, const HyperDev& hy, const OptimDev& op, const XchgDev& x,
-                         cudaStream_t st);
+// tier: the table's host tier (null: none); an inference request then reads the signs it holds in place
+void launch_owner_lookup(bool training, const TableDev& t, const TableDev* tier, const HyperDev& hy, const OptimDev& op,
+                         const XchgDev& x, cudaStream_t st);
 // rows: the f16 or f32 (row_f32) rows the items' set-cell targets index (the receive area, or a remote read's staging)
 void launch_expand_items(const TableDev& t, const SlotsDev& sl, const BatchDev& b, const void* rows, bool row_f32,
                          const uint32_t* row_off, uint32_t n_out, uint32_t batch, bool training, void* out_f16,
@@ -340,6 +341,10 @@ void launch_tier_restore(const TableDev& h, const TableDev& t, const HyperDev& h
                          bool prefix, const uint64_t* ids, uint32_t n, cudaStream_t st);
 void launch_tier_restore_items(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op,
                                const BatchDev& b, cudaStream_t st);
+// sharded training forward (PB_PHASE_SERVE): the signs the R requests of the step brought this owner (its receive area,
+// each source's count), before k_owner_lookup probes them
+void launch_tier_restore_recv(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op,
+                              const XchgDev& x, cudaStream_t st);
 // Reads in place (no move): signs the HBM probe missed (occ_cell = none) that the tier holds.
 //   pb_get_rows: whole entries (len = entry length) + found;  inference pb_lookup: embeddings (len = dim), and the
 //   HBM table's CTR_MISS gives back the misses it counted for them (miss_ctr = that counter)

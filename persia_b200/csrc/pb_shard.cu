@@ -242,8 +242,12 @@ __global__ void k_signal_wait(XchgDev x, int phase, const uint32_t* __restrict__
 // store it, converted, into the requester's area.  f16 rows serve one-id-per-sample layouts (the EW's result is
 // f16(0 + row) there, bit for bit); f32 rows serve ragged layouts, which pool on the requester.
 // ------------------------------------------------------------------------------------------------
-template <int MODE, bool ROW_F32>
-__global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_owner_lookup(TableDev t, HyperDev hy, OptimDev op, XchgDev x) {
+// TIER (inference, MODE_FIND, on a table with a host tier `tier`): a sign the HBM index lacks is probed in the tier and
+// read from its mapped host row where it is, converted as an HBM row is; only a sign neither table holds is a miss.
+// Training requests never take this path: their tier-held signs were moved into HBM rows first (k_tier_restore_recv).
+template <int MODE, bool ROW_F32, bool TIER>
+__device__ __forceinline__ void owner_lookup(const TableDev& t, const TableDev& tier, const HyperDev& hy, const OptimDev& op,
+                                             const XchgDev& x) {
   const uint32_t tick = t.counters[CTR_TICK];
   const uint32_t sub = threadIdx.x % BUCKET;
   const uint32_t lane = threadIdx.x & 31;
@@ -275,12 +279,14 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_owner_lookup(TableDev 
     if (valid && sub == 0) sign = x_sign(x, x.rank)[j];
     sign = __shfl_sync(0xffffffffu, sign, gshift);
     const ProbeOut r = probe_group<MODE>(t, hy, op, sign, valid, tick, sub, gshift);
+    uint32_t trow = ROW_NONE;  // TIER: the sign's tier row
+    if (TIER) trow = probe_group<MODE_FIND>(tier, HyperDev{}, OptimDev{}, sign, valid && r.row == ROW_NONE, 0u, sub, gshift).row;
     // a row admitted just now was initialised by this very group (fenced before its number was published); rows are
     // read through L2 below, never from a stale L1 line
     if (!valid) continue;
     if (sub == 0) {
       x.own_row[j] = r.row;
-      if (r.row == ROW_NONE) atomicAdd(&t.counters[CTR_MISS], 1u);
+      if (r.row == ROW_NONE && (!TIER || trow == ROW_NONE)) atomicAdd(&t.counters[CTR_MISS], 1u);
       if (MODE == MODE_TRAIN) {
         // the backward steps every row ONCE for all the requests that hold it (in rank order): note who asked.  A
         // chained request notes the head of each sign's chain; the other entries are reached through the links.
@@ -303,8 +309,9 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_owner_lookup(TableDev 
         x.uwin[j] = r.row < t.capacity ? won : UWIN_MISS;
       }
     }
-    const float* row = t.rows + (size_t)(r.row < t.capacity ? r.row : 0u) * t.stride;
-    const bool have = r.row < t.capacity;
+    const float* row = (!TIER || r.row < t.capacity) ? t.rows + (size_t)(r.row < t.capacity ? r.row : 0u) * t.stride
+                                                     : tier.rows + (size_t)(trow < tier.capacity ? trow : 0u) * tier.stride;
+    const bool have = r.row < t.capacity || (TIER && trow < tier.capacity);
     const size_t slot = (size_t)x.rank * x.cap + k;  // this owner's segment in the requester's area
     if (ROW_F32) {
       float* dst = reinterpret_cast<float*>(x_row(x, src)) + slot * t.dim;
@@ -362,6 +369,17 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_owner_lookup(TableDev 
       }
     }
   }
+}
+
+template <int MODE, bool ROW_F32>
+__global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_owner_lookup(TableDev t, HyperDev hy, OptimDev op, XchgDev x) {
+  owner_lookup<MODE, ROW_F32, false>(t, t, hy, op, x);
+}
+
+template <bool ROW_F32>
+__global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_owner_lookup_tier(TableDev t, TableDev tier, HyperDev hy,
+                                                                            OptimDev op, XchgDev x) {
+  owner_lookup<MODE_FIND, ROW_F32, true>(t, tier, hy, op, x);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -861,11 +879,14 @@ void launch_wait(const XchgDev& x, int phase, int src, cudaStream_t st) {
   PB_LAUNCH_F(FAM_WAIT, k_wait, 1, 32, 0, st, x, phase, src);
 }
 
-void launch_owner_lookup(bool training, const TableDev& t, const HyperDev& hy, const OptimDev& op, const XchgDev& x,
-                         cudaStream_t st) {
+void launch_owner_lookup(bool training, const TableDev& t, const TableDev* tier, const HyperDev& hy, const OptimDev& op,
+                         const XchgDev& x, cudaStream_t st) {
   const uint32_t full = cdiv((uint64_t)x.R * x.cap * BUCKET, 256);
   const uint32_t grid = full < PB_NUM_SMS * PB_PROBE_BLOCKS ? full : PB_NUM_SMS * PB_PROBE_BLOCKS;
-  if (training) {
+  if (tier && !training) {  // inference reads tier-held signs in place
+    if (x.row_f32) PB_LAUNCH_F(FAM_PROBE, k_owner_lookup_tier<true>, grid, 256, 0, st, t, *tier, hy, op, x);
+    else PB_LAUNCH_F(FAM_PROBE, k_owner_lookup_tier<false>, grid, 256, 0, st, t, *tier, hy, op, x);
+  } else if (training) {
     if (x.row_f32) PB_LAUNCH_F(FAM_PROBE, (k_owner_lookup<MODE_TRAIN, true>), grid, 256, 0, st, t, hy, op, x);
     else PB_LAUNCH_F(FAM_PROBE, (k_owner_lookup<MODE_TRAIN, false>), grid, 256, 0, st, t, hy, op, x);
   } else {

@@ -6,10 +6,11 @@
 // whole entries (embedding ++ optimizer state) between the two tables, eight lanes per sign with 16-byte accesses:
 //   out      an eviction check's victims: tier row + cell claimed (MODE_MOVE), entry copied, tier cell published, and
 //            only then the HBM cell tombstoned and its row freed
-//   restore  before the probe of a training request (and of pb_set_rows): a sign the HBM index lacks and the tier holds
-//            gets a row from the HBM free pool, its entry is copied back and published (MODE_MOVE), the tier row is freed
-//   in place inference lookups, pb_update and pb_get_rows read (or step) tier-held rows where they are: nothing moves,
-//            so they never depend on free HBM rows
+//   restore  before the probe of a training request (and of pb_set_rows; on R GPUs, before the owner's probe of the
+//            signs its peers sent): a sign the HBM index lacks and the tier holds gets a row from the HBM free pool, its
+//            entry is copied back and published (MODE_MOVE), the tier row is freed
+//   in place inference lookups (on R GPUs too: k_owner_lookup_tier, pb_shard.cu), pb_update and pb_get_rows read (or
+//            step) tier-held rows where they are: nothing moves, so they never depend on free HBM rows
 //   stage    pb_tier_stage, one batch ahead on a stream of its own: the eviction check the next training request would
 //            run, then the restores of its signs, so that request finds them in HBM and its own check and restore have
 //            (usually) nothing left to do.  A staged row is stamped with the current batch number (age 0), so the next
@@ -139,6 +140,28 @@ __global__ void __launch_bounds__(256) k_tier_restore_items(TableDev h, TableDev
       const DCell& c = b.set[b.item_cell[u]];
       sign = (c.item >> 31) ? KEY_EMPTY : c.key;  // the scratch set's reserved cell stores 0 for the sign KEY_EMPTY
     }
+    sign = __shfl_sync(0xffffffffu, sign, gshift);
+    restore_group<false>(h, t, hy, op, sign, valid, tick, sub, gshift);
+  }
+}
+
+// sharded training forward (PB_PHASE_SERVE), before k_owner_lookup: the R x cap signs of this owner's receive area, each
+// source's up to its count.  A sign that several sources sent is restored once (the tier cell's CAS); one that finds no
+// free HBM row stays in the tier, counted, and the probe that follows reads zeros for it (its gradient is a miss).
+__global__ void __launch_bounds__(256) k_tier_restore_recv(TableDev h, TableDev t, HyperDev hy, OptimDev op, XchgDev x) {
+  const uint32_t tick = h.counters[CTR_TICK];
+  const uint32_t sub = threadIdx.x % BUCKET;
+  const uint32_t gshift = (threadIdx.x & 31) & ~(BUCKET - 1);
+  const uint32_t total = x.R * x.cap;
+  const uint32_t* ctrl = reinterpret_cast<const uint32_t*>(x.base[x.rank]);
+  const uint64_t* signs = reinterpret_cast<const uint64_t*>(x.base[x.rank] + x.off_sign);
+  constexpr uint32_t PER_BLOCK = 256u / BUCKET;
+  for (uint32_t j0 = blockIdx.x * PER_BLOCK; j0 < total; j0 += gridDim.x * PER_BLOCK) {
+    const uint32_t j = j0 + threadIdx.x / BUCKET;
+    const bool valid = j < total && j % x.cap < ctrl[XC_COUNT * PB_MAX_RANKS + j / x.cap];
+    if (!__any_sync(0xffffffffu, valid)) continue;  // (warp-uniform)
+    uint64_t sign = 0ULL;
+    if (valid && sub == 0) sign = signs[j];
     sign = __shfl_sync(0xffffffffu, sign, gshift);
     restore_group<false>(h, t, hy, op, sign, valid, tick, sub, gshift);
   }
@@ -370,6 +393,13 @@ void launch_tier_restore_items(const TableDev& h, const TableDev& t, const Hyper
   uint32_t grid = cdiv((uint64_t)b.n * BUCKET, 256);  // worst case U = N
   if (grid > PB_NUM_SMS * 4u) grid = PB_NUM_SMS * 4u;
   PB_LAUNCH(k_tier_restore_items, grid, 256, 0, st, h, t, hy, op, b);
+}
+
+void launch_tier_restore_recv(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op,
+                              const XchgDev& x, cudaStream_t st) {
+  uint32_t grid = cdiv((uint64_t)x.R * x.cap * BUCKET, 256);
+  if (grid > PB_NUM_SMS * 4u) grid = PB_NUM_SMS * 4u;
+  PB_LAUNCH(k_tier_restore_recv, grid, 256, 0, st, h, t, hy, op, x);
 }
 
 void launch_tier_get(const TableDev& h, const TableDev& t, const uint64_t* signs, const uint32_t* occ_cell, uint32_t n,
