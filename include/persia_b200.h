@@ -499,6 +499,50 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
 int pb_backward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* d_grad, int is_f16, float scale,
                             int32_t* d_status, void* stream, int phases);
 
+/* ---- staging on R GPUs: the next batch's host-tier moves one step early --------------------------------------------
+ * pb_tier_stage on R GPUs.  A rank's next batch asks for signs that its owners hold, so its stage needs those signs at
+ * the owners a step early.  A stage exchange carries them: an exchange with a ctrl and a sign part only (no rows,
+ * gradients or chain words; no owner-side set or Adam arrays).  Its area is pb_xchg_stage_bytes(R, cap) bytes of
+ * zero-initialised device memory that all ranks can store to, mapped as for pb_xchg_create:
+ *   [0, 512)          ctrl: XC_WORDS (5) x 16 u32 flag and count words (as a batch exchange's)
+ *   [512, 512 + S)    sign: R x cap u64, the signs each source stages here, by source; S = R x cap x 8 rounded up to 256
+ * pb_xchg_stage_bytes returns 0 for R = 0, R > 16, cap = 0 or R x cap >= 2^32 - 16.  cap: the most signs one rank sends
+ * one owner in one stage.  pb_xchg_destroy frees a stage exchange and pb_xchg_status reads it: h_out[0] != 0 when a
+ * stage had more than cap signs for one owner (the excess was not sent; the forward restores it as unstaged), h_out[1]
+ * as for a batch exchange.  The sharded forwards and backwards refuse a stage exchange (PB_ERR_INVALID), and
+ * pb_tier_stage_sharded refuses a batch exchange (PB_ERR_INVALID).
+ *
+ * pb_tier_stage_sharded: arguments as pb_tier_stage (raw slot ids, slot offsets, per-slot prefixes, 0 = taken as they
+ * are) plus the stage exchange and `phases`: PB_PHASE_SEND, PB_PHASE_SERVE or both (0 = both; PB_PHASE_FINISH and
+ * PB_PHASE_PREPARE are refused, PB_ERR_INVALID).  Virtual ranks of one GPU enqueue SEND for every rank, then SERVE.
+ *   SEND (requester)  every id slot-prefixed, its owner farmhash64 % R, duplicates inside a warp dropped, the sign
+ *                     stored into the owner's stage area; then the flag.
+ *   SERVE (owner)     waits for the R flags; with a host tier, runs the eviction check pb_tier_stage runs (not counted
+ *                     as one of the every-`check_every` calls; keep = max(keep_batches, pending batches + 1); victims
+ *                     out to the tier), then moves every received sign the HBM table lacks and its tier holds into a
+ *                     free HBM row, stamped with the current batch number.  Never admits a sign.  A sign that finds no
+ *                     free row is counted as a skipped stage and left to the forward.  Counters: pb_tier_stage_stats of
+ *                     the owner's table.  An owner without a tier waits for and consumes the flags and moves nothing.
+ * Values never change, only where entries live, and a sign the stage did not move is restored by the forward exactly
+ * as unstaged: a staged run equals the unstaged one bit for bit.
+ * Rules: the call is collective, like the other sharded calls, and outside the table's chains: the caller orders it.
+ *   - A rank's stage starts after its previous training forward (every phase) has completed, and its next sharded
+ *     forward on the table starts after the stage has completed.  Refused on a host tier (PB_ERR_STATE) and on a table
+ *     exported for remote reads (pb_table_export_view: PB_ERR_STATE).
+ *   - It may run beside the sharded backwards, summation and raw alike, on another stream: no owner-side backward kernel
+ *     (k_owner_update_all, k_owner_update, the raw owner path, which is the same, and the Adam beta-power advance)
+ *     reads index cells, the free-row stack or row_tick.  They step only the rows their forward found, by the row
+ *     numbers it stored; those rows are never victims (their age is below keep) nor restore targets (those come off
+ *     the free stack), and the incremental marks read the exchange, not the index.
+ *   - A stage area is never rewritten while its owner still reads the previous stage: rank r's stage i+1 starts after
+ *     r's forward i, which waited for every owner's SERVE of forward i, and each owner's forward i started after its
+ *     own stage i had completed.  One area per rank therefore suffices.
+ *   - No host synchronisation: a step with a stage, the stage forked onto a side stream, is capturable in one graph. */
+uint64_t pb_xchg_stage_bytes(uint32_t R, uint32_t cap);
+int pb_xchg_create_stage(int device, uint32_t R, uint32_t rank, uint32_t cap, const uint64_t* h_peer_base, pb_xchg** out);
+int pb_tier_stage_sharded(pb_table* t, pb_xchg* xs, const uint64_t* d_ids, uint32_t n, const uint32_t* h_slot_occ_off,
+                          const uint64_t* h_prefix, uint32_t n_slots, uint32_t prefix_bit, void* stream, int phases);
+
 /* ---- inference on R GPUs one rank at a time: reading the owners' shards in place --------------------------------------
  * The reference's Infer handlers each call get_embedding_from_bytes on their own requests, and the embedding servers
  * answer each request alone (persia/ctx.py:1077-1135, embedding_parameter_service/mod.rs:162-262).  The sharded calls

@@ -1899,6 +1899,10 @@ struct pb_xchg {
   float* apow = nullptr;
   size_t akeys_uploaded = 0;
   bool u_dirty = false;     // a training lookup filled ucell and its update has not run (abandoned batch)
+  // a stage exchange (pb_xchg_create_stage): ctrl and sign areas only, dim 0 (so check_exchange refuses it); `sent`:
+  // [PB_MAX_RANKS] signs of this rank's stage per owner (in `mem`, after the phase words)
+  bool stage = false;
+  uint32_t* sent = nullptr;
 };
 
 namespace {
@@ -1910,6 +1914,12 @@ void xchg_layout(uint32_t R, uint32_t cap, uint32_t dim, int rows_f32, uint64_t 
   off[3] = off[2] + round256((uint64_t)R * cap * dim * 4);                         // gok
   off[4] = off[3] + round256((uint64_t)R * cap * 4);                               // chain
   off[5] = off[4] + round256((uint64_t)R * cap * 4);                               // end
+}
+
+// a stage exchange's area: ctrl, then the R x cap signs sent to this rank (off[0] sign, off[1] end)
+void xchg_stage_layout(uint32_t R, uint32_t cap, uint64_t off[2]) {
+  off[0] = round256((uint64_t)XC_WORDS * PB_MAX_RANKS * 4);
+  off[1] = off[0] + round256((uint64_t)R * cap * 8);
 }
 
 // the rows this rank's receive area holds, returned by the owners (the requester's FINISH reads them)
@@ -2081,6 +2091,91 @@ int pb_xchg_destroy(pb_xchg* x) {
   if (x->apresent) cudaFree(x->apresent);
   if (x->apow) cudaFree(x->apow);
   delete x;
+  return PB_OK;
+}
+
+uint64_t pb_xchg_stage_bytes(uint32_t R, uint32_t cap) {
+  if (R == 0 || R > PB_MAX_RANKS || cap == 0 || (uint64_t)R * cap >= 0xFFFFFFF0ull) return 0;
+  uint64_t off[2];
+  xchg_stage_layout(R, cap, off);
+  return off[1];
+}
+
+int pb_xchg_create_stage(int device, uint32_t R, uint32_t rank, uint32_t cap, const uint64_t* h_peer_base, pb_xchg** out) {
+  if (!out || !h_peer_base || R == 0 || R > PB_MAX_RANKS || rank >= R || cap == 0)
+    return fail(PB_ERR_INVALID, "bad argument");
+  if ((uint64_t)R * cap >= 0xFFFFFFF0ull) return fail(PB_ERR_INVALID, "R * cap must stay below 2^32 - 16");
+  for (uint32_t q = 0; q < R; ++q)
+    if (!h_peer_base[q] || (h_peer_base[q] & 255u)) return fail(PB_ERR_INVALID, "stage areas must be mapped and 256-byte aligned");
+  DeviceGuard g(device);
+  pb_xchg* x = new pb_xchg();
+  x->device = device;
+  x->stage = true;  // dim 0: no row, gradient or chain area, no ucell set, no Adam arrays
+  uint64_t off[2];
+  xchg_stage_layout(R, cap, off);
+  XchgDev& d = x->d;
+  std::memset(&d, 0, sizeof(d));
+  for (uint32_t q = 0; q < R; ++q) d.base[q] = h_peer_base[q];
+  d.off_sign = off[0];
+  d.off_row = d.off_grad = d.off_gok = d.off_chain = off[1];
+  d.R = R;
+  d.rank = rank;
+  d.cap = cap;
+  const size_t words = XC_WORDS + (size_t)XC_WORDS * PB_MAX_RANKS + PB_MAX_RANKS + 4;  // epoch | waited | sent | err
+  cudaError_t e = cudaMalloc(&x->mem, 4 * words);
+  if (e == cudaSuccess) e = cudaMemset(x->mem, 0, 4 * words);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) {
+    if (x->mem) cudaFree(x->mem);
+    delete x;
+    return fail(PB_ERR_CUDA, std::string("pb_xchg_create_stage: ") + cudaGetErrorString(e));
+  }
+  d.epoch = x->mem;
+  d.waited = d.epoch + XC_WORDS;
+  x->sent = d.waited + (size_t)XC_WORDS * PB_MAX_RANKS;
+  d.err = x->sent + PB_MAX_RANKS;
+  *out = x;
+  return PB_OK;
+}
+
+int pb_tier_stage_sharded(pb_table* t, pb_xchg* xs, const uint64_t* d_ids, uint32_t n, const uint32_t* h_slot_occ_off,
+                          const uint64_t* h_prefix, uint32_t n_slots, uint32_t prefix_bit, void* stream, int phases) {
+  if (!t || !xs || (n && !d_ids) || !h_slot_occ_off || !h_prefix) return fail(PB_ERR_INVALID, "null argument");
+  if (!xs->stage)
+    return fail(PB_ERR_INVALID, "a batch exchange carries no stage: create a stage exchange (pb_xchg_create_stage)");
+  if (phases & ~(PB_PHASE_SEND | PB_PHASE_SERVE))
+    return fail(PB_ERR_INVALID, "a stage has the phases PB_PHASE_SEND and PB_PHASE_SERVE only");
+  if (t->tier_of) return fail(PB_ERR_STATE, "a host tier is not staged directly: use the table it is attached to");
+  if (n_slots == 0 || n_slots > PB_MAX_SLOTS) return fail(PB_ERR_INVALID, "n_slots must be in 1..PB_MAX_SLOTS");
+  if (prefix_bit == 0 || prefix_bit > 63) return fail(PB_ERR_INVALID, "feature_index_prefix_bit must be in 1..63");
+  if (t->device != xs->device) return fail(PB_ERR_INVALID, "table and exchange live on different devices");
+  int rc = check_slot_offsets(h_slot_occ_off, n_slots, n);
+  if (rc || (rc = writable(t))) return rc;  // (its eviction check)
+  if (t->tier && (rc = ready_for_training(t))) return rc;
+  SlotsDev sl;
+  if ((rc = prefix_slots(h_slot_occ_off, h_prefix, n_slots, prefix_bit, sl))) return rc;
+  DeviceGuard g(t->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  // a stage has no FINISH: SEND and SERVE together are the whole call (one process per GPU: one signal-and-wait launch)
+  const int mask = phases ? phases : PB_PHASE_SEND | PB_PHASE_SERVE;
+  const Phases ph(mask == (PB_PHASE_SEND | PB_PHASE_SERVE) ? PB_PHASE_ALL : mask);
+  if (ph.has(PB_PHASE_SEND)) {  // requester: the next batch's signs -> their owners' stage areas
+    PB_CUDA(cudaMemsetAsync(xs->sent, 0, 4 * PB_MAX_RANKS, st));
+    launch_stage_route(sl, d_ids, n, xs->d, xs->sent, st);
+    ph.post(xs, XC_FLAG_SIGN, xs->sent, st);
+  }
+  if (ph.has(PB_PHASE_SERVE)) {  // owner: the check the next request would run, then the received signs' restores
+    ph.await(xs, XC_FLAG_SIGN, st);
+    if (t->tier) {
+      // Outside the table's chains, like every sharded call (the caller orders it; see include/persia_b200.h).  Not
+      // counted in train_calls; keep covers the batches pending now.  Beside a sharded backward: no owner-side backward
+      // kernel reads index cells, the free-row stack or row_tick, and the rows they step are never victims here (keep >
+      // pending_batches) nor restore targets (those come off the free stack).
+      if (t->evict_every && (rc = evict_check(t, st, g_stage_blocks))) return rc;
+      launch_tier_restore_recv(t->d, t->tier->d, t->hy, t->op, xs->d, st, g_stage_blocks);
+    }
+  }
+  PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
 

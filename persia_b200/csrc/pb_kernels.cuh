@@ -80,6 +80,8 @@ __device__ __forceinline__ unsigned long long* hot_words_asked(const BatchDev& b
 //   gok    [R][cap] u32         1 = apply the gradient, 0 = the slot was skipped / held a NaN
 //   chain  [R][cap] u32         requests with slots sharing a feature group: CHAIN_CONT | the sign's next entry
 // ctrl word XC_CHAIN of a source equals its XC_FLAG_SIGN word when that source's request of the step carries chain words.
+// A stage exchange (pb_xchg_create_stage) has the ctrl and sign parts only: XC_FLAG_SIGN and XC_COUNT carry the signs
+// of the next batch that each source sends the owner a step early (pb_tier_stage_sharded).
 enum { XC_FLAG_SIGN = 0, XC_FLAG_ROW, XC_FLAG_GRAD, XC_COUNT, XC_CHAIN, XC_WORDS };
 // chain word of an entry: a sign that several slots of one feature group hold is one entry per slot; the first (the
 // head, in slot order) carries the step, the others follow it.  CHAIN_CONT: not a head; low bits: the request's next
@@ -342,9 +344,14 @@ void launch_tier_restore(const TableDev& h, const TableDev& t, const HyperDev& h
 void launch_tier_restore_items(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op,
                                const BatchDev& b, cudaStream_t st);
 // sharded training forward (PB_PHASE_SERVE): the signs the R requests of the step brought this owner (its receive area,
-// each source's count), before k_owner_lookup probes them
+// each source's count), before k_owner_lookup probes them.  stage_blocks != 0: pb_tier_stage_sharded's SERVE, on that
+// many blocks: the signs of a stage exchange's area, restored as pb_tier_stage restores (age 0, skips counted as such)
 void launch_tier_restore_recv(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op,
-                              const XchgDev& x, cudaStream_t st);
+                              const XchgDev& x, cudaStream_t st, uint32_t stage_blocks = 0);
+// pb_tier_stage_sharded's SEND (pb_shard.cu): every id slot-prefixed as k_tier_stage does, sent once per warp to its
+// owner's stage area (farmhash64 % R); sent[q] counts the signs for owner q (zeroed by the caller; over cap: x.err[0])
+void launch_stage_route(const SlotsDev& sl, const uint64_t* ids, uint32_t n, const XchgDev& x, uint32_t* sent,
+                        cudaStream_t st);
 // Reads in place (no move): signs the HBM probe missed (occ_cell = none) that the tier holds.
 //   pb_get_rows: whole entries (len = entry length) + found;  inference pb_lookup: embeddings (len = dim), and the
 //   HBM table's CTR_MISS gives back the misses it counted for them (miss_ctr = that counter)

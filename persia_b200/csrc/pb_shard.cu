@@ -100,6 +100,50 @@ __global__ void __launch_bounds__(256) k_route_items(SlotsDev sl, BatchDev b, Xc
 }
 
 // ------------------------------------------------------------------------------------------------
+// requester, pb_tier_stage_sharded's SEND: the next batch's ids, slot-prefixed as k_tier_stage prefixes them, each sent
+// to its owner's stage area.  One thread per id; a sign that several lanes of a warp hold is sent once (the owner's
+// restore is idempotent, so duplicates across warps only cost slots).  Slots per owner as in k_route_items: counted per
+// block in shared memory, one global atomic per block and owner.  A sign over `cap` is not sent (x.err[0]): its
+// forward restores it as it would unstaged.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_stage_route(SlotsDev sl, const uint64_t* __restrict__ ids, uint32_t n, XchgDev x,
+                                                     uint32_t* __restrict__ sent) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  bool valid = i < n;
+  uint64_t sign = 0;
+  if (valid) {
+    sign = ids[i];
+    const uint64_t p = sl.prefix[slot_of_occ(sl, i)];
+    if (p) sign = mod_mersenne(sign, sl.spacing_bits) + p;
+  }
+  const uint32_t live = __ballot_sync(0xffffffffu, valid);
+  const uint32_t same = __match_any_sync(0xffffffffu, (unsigned long long)sign) & live;
+  valid = valid && (uint32_t)(__ffs(same) - 1) == lane;  // the warp's first lane of the sign sends it
+  const uint32_t owner = valid ? (uint32_t)(farmhash64_u64(sign) % x.R) : 0xFFFFFFFFu;  // sign_to_shard_modulo
+  __shared__ uint32_t s_n[PB_MAX_RANKS], s_g[PB_MAX_RANKS];
+  if (threadIdx.x < PB_MAX_RANKS) s_n[threadIdx.x] = 0;
+  __syncthreads();
+  const uint32_t peers = __match_any_sync(0xffffffffu, owner);
+  const uint32_t leader = __ffs(peers) - 1;
+  uint32_t k = 0;
+  if (valid && lane == leader) k = atomicAdd(&s_n[owner], (uint32_t)__popc(peers));
+  k = __shfl_sync(0xffffffffu, k, leader) + __popc(peers & ((1u << lane) - 1u));
+  __syncthreads();
+  if (threadIdx.x < x.R && s_n[threadIdx.x]) s_g[threadIdx.x] = atomicAdd(&sent[threadIdx.x], s_n[threadIdx.x]);
+  __syncthreads();
+  if (!valid) return;
+  k += s_g[owner];
+  if (k < x.cap) x_sign(x, owner)[(size_t)x.rank * x.cap + k] = sign;  // over NVLink when owner != rank
+  else x.err[0] = 1u;
+}
+
+void launch_stage_route(const SlotsDev& sl, const uint64_t* ids, uint32_t n, const XchgDev& x, uint32_t* sent,
+                        cudaStream_t st) {
+  if (n) PB_LAUNCH_F(FAM_ROUTE, k_stage_route, cdiv(n, 256), 256, 0, st, sl, ids, n, x, sent);
+}
+
+// ------------------------------------------------------------------------------------------------
 // requester, PB_PHASE_PREPARE: how many of the batch's distinct items go to each owner — what `cap` must cover — read
 // from the context alone (the dedup's set, or the raw numbering's), before anything is sent.  Counted per block in
 // shared memory, one global atomic per block and owner.

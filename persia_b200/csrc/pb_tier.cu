@@ -13,7 +13,9 @@
 //            step) tier-held rows where they are: nothing moves, so they never depend on free HBM rows
 //   stage    pb_tier_stage, one batch ahead on a stream of its own: the eviction check the next training request would
 //            run, then the restores of its signs, so that request finds them in HBM and its own check and restore have
-//            (usually) nothing left to do.  A staged row is stamped with the current batch number (age 0), so the next
+//            (usually) nothing left to do.  On R GPUs (pb_tier_stage_sharded) every rank first sends the next batch's
+//            signs to their owners' stage areas (k_stage_route, pb_shard.cu); each owner runs the check and restores
+//            what it received (k_tier_restore_recv<true>).  A staged row is stamped with the current batch number (age 0), so the next
 //            check keeps it; a stage that finds no free row leaves the entry in the tier for the request's own restore.
 // A moved entry keeps its row_tick (a staged restore excepted), and the tier ages its rows by the HBM table's batch
 // number: the union of the two tables evicts least recently used first, at batch granularity.  A sign lives in at most
@@ -148,6 +150,9 @@ __global__ void __launch_bounds__(256) k_tier_restore_items(TableDev h, TableDev
 // sharded training forward (PB_PHASE_SERVE), before k_owner_lookup: the R x cap signs of this owner's receive area, each
 // source's up to its count.  A sign that several sources sent is restored once (the tier cell's CAS); one that finds no
 // free HBM row stays in the tier, counted, and the probe that follows reads zeros for it (its gradient is a miss).
+// STAGE (pb_tier_stage_sharded's SERVE): the same walk over a stage exchange's area, whose signs the sources sent one
+// batch ahead; restored as k_tier_stage restores (age 0; no free row: a skipped stage, left to the forward's restore).
+template <bool STAGE>
 __global__ void __launch_bounds__(256) k_tier_restore_recv(TableDev h, TableDev t, HyperDev hy, OptimDev op, XchgDev x) {
   const uint32_t tick = h.counters[CTR_TICK];
   const uint32_t sub = threadIdx.x % BUCKET;
@@ -163,7 +168,7 @@ __global__ void __launch_bounds__(256) k_tier_restore_recv(TableDev h, TableDev 
     uint64_t sign = 0ULL;
     if (valid && sub == 0) sign = signs[j];
     sign = __shfl_sync(0xffffffffu, sign, gshift);
-    restore_group<false>(h, t, hy, op, sign, valid, tick, sub, gshift);
+    restore_group<STAGE>(h, t, hy, op, sign, valid, tick, sub, gshift);
   }
 }
 
@@ -396,10 +401,14 @@ void launch_tier_restore_items(const TableDev& h, const TableDev& t, const Hyper
 }
 
 void launch_tier_restore_recv(const TableDev& h, const TableDev& t, const HyperDev& hy, const OptimDev& op,
-                              const XchgDev& x, cudaStream_t st) {
+                              const XchgDev& x, cudaStream_t st, uint32_t stage_blocks) {
   uint32_t grid = cdiv((uint64_t)x.R * x.cap * BUCKET, 256);
+  if (stage_blocks) {
+    PB_LAUNCH(k_tier_restore_recv<true>, grid < stage_blocks ? grid : stage_blocks, 256, 0, st, h, t, hy, op, x);
+    return;
+  }
   if (grid > PB_NUM_SMS * 4u) grid = PB_NUM_SMS * 4u;
-  PB_LAUNCH(k_tier_restore_recv, grid, 256, 0, st, h, t, hy, op, x);
+  PB_LAUNCH(k_tier_restore_recv<false>, grid, 256, 0, st, h, t, hy, op, x);
 }
 
 void launch_tier_get(const TableDev& h, const TableDev& t, const uint64_t* signs, const uint32_t* occ_cell, uint32_t n,

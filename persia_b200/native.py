@@ -104,6 +104,9 @@ SYMBOLS = {
     "pb_xchg_destroy": (_i32, [_vp]),
     "pb_xchg_status": (_i32, [_vp, C.POINTER(_u32 * 2), _vp]),
     "pb_xchg_need": (_i32, [_vp, _vp, C.POINTER(_u32 * 1), _vp]),
+    "pb_xchg_stage_bytes": (_u64, [_u32, _u32]),
+    "pb_xchg_create_stage": (_i32, [_i32, _u32, _u32, _u32, C.POINTER(_u64), C.POINTER(_vp)]),
+    "pb_tier_stage_sharded": (_i32, [_vp, _vp, _vp, _u32, C.POINTER(_u32), C.POINTER(_u64), _u32, _u32, _vp, _i32]),
     "pb_forward_sharded": (_i32, [_vp, _vp, _vp, _vp, _u32, _vp, C.POINTER(_u32), _u32, _i32, _vp, _vp, _i32]),
     "pb_backward_sharded": (_i32, [_vp, _vp, _vp, C.POINTER(_vp), _i32, C.POINTER(C.c_float), _vp, _vp, _i32]),
     "pb_forward_raw_sharded": (_i32, [_vp, _vp, _vp, _vp, _u32, _vp, _u32, _u32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _i32]),

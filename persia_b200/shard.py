@@ -122,6 +122,31 @@ INCREMENTAL_STATS_FIELDS = ("held", "inserted", "dropped", "taken")
 BATCH_STATS_FIELDS = ("items", "cold", "warm", "hot", "repeated_occurrences", "occurrences")
 
 
+def _capturing(stream):
+    with torch.cuda.stream(stream):
+        return torch.cuda.is_current_stream_capturing()
+
+
+class StreamMark:
+    """An event recorded on one stream for work on another to wait for, as the library's table marks do it: a wait never
+    crosses a stream-capture boundary.  Work recorded outside a capture must have completed before the capture starts
+    (synchronise first); work recorded inside one graph is ordered within it, and graphs among themselves by whoever
+    launches them."""
+
+    def __init__(self):
+        self.ev, self.captured = None, False
+
+    def record(self, stream):
+        if self.ev is None:
+            self.ev = torch.cuda.Event()
+        self.captured = _capturing(stream)
+        self.ev.record(stream)
+
+    def wait(self, stream):
+        if self.ev is not None and self.captured == _capturing(stream):
+            stream.wait_event(self.ev)
+
+
 class EmbeddingShard:
     def __init__(self, dim, capacity, device=0, tier_rows=0, host=False):
         """capacity: rows in HBM.  tier_rows > 0: a host-memory tier of that many rows behind them (include/persia_b200.h,
@@ -138,6 +163,10 @@ class EmbeddingShard:
         self._entry_len = None
         self.host_tier = EmbeddingShard(dim, tier_rows, device, host=True) if tier_rows else None
         self._tier_attached = False
+        # R GPUs (worker.TierStager): the sharded forwards of this shard's workers, keyed by worker, and its stager's
+        # last stage.  A stage waits for the forwards before it; a forward waits for the stage before it.
+        self._forward_marks = {}
+        self._stage_mark = StreamMark()
 
     # register_optimizer (PS mod.rs:429-438)
     def set_optimizer(self, kind, lr=0.01, wd=0.0, g_square_momentum=1.0, initialization=0.01, eps=1e-10,

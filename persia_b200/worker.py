@@ -203,10 +203,21 @@ class ShardedEmbeddingWorker:
             slot_occ_off = [s * batch for s in range(self.S + 1)]
         if out is None:
             out = torch.empty((self.S, batch, self.dim), dtype=torch.float16, device=self.device)
+        self._after_stage()
         N.check(self.lib.pb_forward_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), ids.numel(), SH._ptr(row_off),
                                             SH._slot_offsets(slot_occ_off, self.S), int(batch), int(training),
                                             SH._ptr(out), self._st(), int(phases)))
+        self._forward_done(phases)
         return out
+
+    def _after_stage(self):
+        """A forward starts after the last stage of this rank's shard (TierStager); nothing without one."""
+        self.shard._stage_mark.wait(self._torch_stream())
+
+    def _forward_done(self, phases):
+        """Once a forward's last phase is enqueued, the shard's next stage starts after it (TierStager)."""
+        if phases == 0 or phases & N.PHASE_FINISH:
+            self.shard._forward_marks.setdefault(id(self), SH.StreamMark()).record(self._torch_stream())
 
     def backward(self, grads, scales=None, want_status=False, phases=0, status=None):
         """grads: f16/f32 tensor [n_slots, batch, dim] or a list of per-slot tensors (None = skipped slot).  A slot
@@ -349,6 +360,8 @@ class ShardedEmbeddingWorker:
         if getattr(self, "h", None):
             self.lib.pb_xchg_destroy(self.h)
             self.h = None
+        if getattr(self, "shard", None) is not None:
+            self.shard._forward_marks.pop(id(self), None)
         self.ctx.close()
         if self._own_shard:
             self.shard.close()
@@ -389,9 +402,11 @@ class ShardedRawWorker(ShardedEmbeddingWorker):
         if phases == 0 or phases & N.PHASE_FINISH:
             self._prepared_out = None
         table, index, non_empty, num, counts = out
+        self._after_stage()
         N.check(self.lib.pb_forward_raw_sharded(self.shard.h, self.ctx.h, self.h, SH._ptr(ids), n,
                                                 SH._raw_row_off(row_off, batch), int(batch), fixed, int(training),
                                                 *map(SH._ptr, out), self._st(), int(phases)))
+        self._forward_done(phases)
         return table, index, non_empty, num[:batch], counts
 
     def backward_raw(self, grad, scale=1.0, want_status=False, is_f16=None, phases=0, status=None):
@@ -442,6 +457,105 @@ class ShardedRawWorker(ShardedEmbeddingWorker):
         for r, w, ph in _by_phase(workers, N.PHASE_SEND, N.PHASE_SERVE):
             w.backward_raw(grads[r], scales[r] if scales is not None else 1.0, phases=ph, status=sts[r])
         return sts
+
+
+class TierStager:
+    """The next batch's host-tier moves on R GPUs, one step early (pb_tier_stage_sharded): every rank sends the signs of
+    its next training batch to their owners, and each owner runs the eviction check that batch would run and moves the
+    tier-held signs it received back into HBM, on a stream of its own, beside the current batch's backward and dense
+    step.  One stager per rank and table, shared by the summation and raw workers of that dim (they serve its shard).
+    Values never change: a staged run equals the unstaged one bit for bit.
+
+    Ordering is kept on the EmbeddingShard, so callers handle no events: stage() waits for the last forward of every
+    worker of the shard, and their next forward / forward_raw waits for the stage.  Each call is collective, like the
+    workers' (one process per GPU: `distributed`; virtual ranks of one GPU: `local_group` and `group_stage`).
+
+    cap: the most signs one rank stages one owner in one call; the stage area holds R x cap signs.  Pass the most ids one
+    stage() call brings and no sign is ever over cap.  Signs over it are not staged (status()[0]): the forward restores
+    them as it would unstaged."""
+
+    def __init__(self, shard, rank, world, cap, area, peer_bases, stream=None):
+        self.lib = N.load()
+        self.shard, self.rank, self.R, self.cap = shard, int(rank), int(world), int(cap)
+        self.device = shard.device
+        self.area = area  # keeps the stage area alive
+        self.stream = stream if stream is not None else torch.cuda.Stream(device=self.device)
+        bases = (C.c_uint64 * self.R)(*[int(p) for p in peer_bases])
+        h = C.c_void_p()
+        N.check(self.lib.pb_xchg_create_stage(self.device.index or 0, self.R, self.rank, self.cap, bases, C.byref(h)))
+        self.h = h
+
+    @staticmethod
+    def area_bytes(world, cap):
+        b = int(N.load().pb_xchg_stage_bytes(world, int(cap)))
+        assert b > 0, "bad stage geometry"
+        return b
+
+    @classmethod
+    def local_group(cls, shards, cap, streams=None):
+        """One stager per virtual rank of one GPU, over the ranks' shards (e.g. `[w.shard for w in workers]`)."""
+        dev = shards[0].device
+        areas, bases = ShardedEmbeddingWorker._local_areas(len(shards), cls.area_bytes(len(shards), cap), dev)
+        return [cls(s, r, len(shards), cap, areas[r], bases, stream=streams[r] if streams else None)
+                for r, s in enumerate(shards)]
+
+    @classmethod
+    def distributed(cls, shard, cap, group=None, stream=None):
+        """One process per GPU: the stage area lives in symmetric memory, like the workers' receive areas (collective)."""
+        import torch.distributed as dist
+
+        grp = group if group is not None else dist.group.WORLD
+        world, rank = dist.get_world_size(grp), dist.get_rank(grp)
+        area, bases = ShardedEmbeddingWorker._symmetric_area(cls.area_bytes(world, cap), shard.device, grp)
+        st = cls(shard, rank, world, cap, area, bases, stream=stream)
+        st.group = grp
+        return st
+
+    def stage(self, ids, slot_occ_off, prefixes, prefix_bit=8, phases=0):
+        """Stages the next training batch of this rank: ids flat device slot ids (slot-major, hash-stacked where a slot
+        hash-stacks; the summation and raw slots of the table may come in one call), slot_occ_off host list of
+        n_slots + 1 offsets, prefixes each slot's index prefix (0 = ids taken as they are).  Runs on the stager's
+        stream.  phases: PHASE_SEND, PHASE_SERVE or 0 = both (virtual ranks: group_stage)."""
+        ids = SH._as_i64_bits(ids)
+        S = len(prefixes)
+        st = self.stream
+        if phases == 0 or phases & N.PHASE_SEND:
+            for m in self.shard._forward_marks.values():
+                m.wait(st)
+        N.check(self.lib.pb_tier_stage_sharded(self.shard.h, self.h, SH._ptr(ids), ids.numel(),
+                                               SH._slot_offsets(slot_occ_off, S), SH._prefixes(prefixes), S,
+                                               int(prefix_bit), C.c_void_p(st.cuda_stream), int(phases)))
+        if phases == 0 or phases & N.PHASE_SERVE:
+            self.shard._stage_mark.record(st)
+
+    @staticmethod
+    def group_stage(stagers, ids, slot_occ_offs, prefixes, prefix_bit=8):
+        """Virtual ranks of one GPU, driven by one host thread: SEND for every rank, then SERVE for every rank."""
+        for r, s, ph in _by_phase(stagers, N.PHASE_SEND, N.PHASE_SERVE):
+            s.stage(ids[r], slot_occ_offs[r], prefixes, prefix_bit, phases=ph)
+
+    def stage_stats(self):
+        """This rank's owner counters (host sync): signs staged into HBM, and stage restores skipped for want of a free
+        row."""
+        return self.shard.stage_stats()
+
+    def status(self):
+        """(overflowed, wait_gave_up) — host sync.  overflowed: a stage had more than cap signs for one owner."""
+        out = SH._read_block(XCHG_STATUS_FIELDS, lambda out: self.lib.pb_xchg_status(self.h, out,
+                                                                                     C.c_void_p(self.stream.cuda_stream)),
+                             C.c_uint32)
+        return bool(out["overflowed"]), bool(out["wait_gave_up"])
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.pb_xchg_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 class RemoteReader:
