@@ -7,14 +7,14 @@ process's GPU, `get_embedding_from_data` / `Forward.get_batch` run pb_forward, `
 the raw device pointers `GradientBatch.add_gradient` receives.  `install()` registers it (and its submodules)
 in `sys.modules` as `persia_core`, after which the reference's own `persia` package runs unchanged on top.
 
-Scope: summation and raw slots (no hash-stack on raw slots), one process per GPU.  The summation slots of one dim are
-served by batch contexts of at most PB_MAX_SLOTS slots each, a feature group never split (slot_chunks).  With
-`replica_size > 1` every such chunk is served by a ShardedEmbeddingWorker and every raw slot by its own
-ShardedRawWorker (persia_b200.worker), all of one dim on the rank's one table; summation slots there may share a
-feature group (each rank's entries of a shared sign are applied in slot order, the ranks in rank order), but a raw slot
-may not share its feature group with another slot of the batch.
-Their calls are collective, so every rank issues them in one fixed order: the raw slots in batch order, then the
-summation dims in ascending order, in the forward and again in the backward; every batch must carry the same raw
+Scope: summation and raw slots (no hash-stack on raw slots), one process per GPU.  A batch's units (_units) are its raw
+slots and its summation slots of each dim in chunks of at most PB_MAX_SLOTS slots, a feature group never split
+(slot_chunks); each unit is served by one placement (forward, backward, release): a pooled batch context (_Local) or,
+with `replica_size > 1`, its ShardedEmbeddingWorker or ShardedRawWorker (_ShardedPart, persia_b200.worker), all of one
+dim on the rank's one table; summation slots there may share a feature group (each rank's entries of a shared sign are
+applied in slot order, the ranks in rank order), but a raw slot may not share its feature group with another slot.
+Their calls are collective, so every rank issues them in one fixed order (_units): the raw slots in batch order, then
+the summation dims in ascending order, in the forward and again in the backward; every batch must carry the same raw
 slots in the same order.  Every step on R GPUs is sized from its own batch (_sharded_step): each worker prepares its
 batch locally (PB_PHASE_PREPARE), one all_reduce(MAX) agrees on every worker's need, and the exchanges that do not cover
 it are replaced before any rank sends; an exchange overflow or a wait that gave up is then an internal error.  `Forward` prefetches on worker threads with the reference's ordering and
@@ -23,7 +23,7 @@ write and read the reference's `.emb` checkpoint files (persia_b200/checkpoint.p
 `enable_incremental_update` on a Train job, the signs the tables step are flushed as the reference's `.inc` packets; an
 Infer job loads its checkpoint and applies them as they appear (persia_b200/incremental.py, `set_global_config`).
 At `replica_size > 1` every forward that does not train is served by its rank alone, reading the owners' shards in place
-(_start_remote, worker.RemoteReader): no collective.  An Infer job exports its tables frozen once its checkpoint is
+(_start_remote, _Remote): no collective.  An Infer job exports its tables frozen once its checkpoint is
 loaded; a Train job exports them live when its optimizer is registered, and its training forwards and backwards stay
 collective.
 """
@@ -722,15 +722,15 @@ class PersiaBatch:  # data.rs:142-266
 # the forward itself: LIL id features -> pb_forward per dim group -> PersiaTrainingBatch
 # ---------------------------------------------------------------------------------------------------------
 class _Pending:
-    """What the EW keeps under backward_ref_id (mod.rs:1087-1098): per dim group, the device context."""
+    """What the EW keeps under backward_ref_id (mod.rs:1087-1098): the placement of each of the batch's units
+    (_Local or _ShardedPart), in the order of its forward."""
 
     def __init__(self):
-        self.parts = []  # (group, ctx, [slot names in order], is_raw, sharded worker or None)
+        self.parts = []
 
     def release(self):
-        for g, ctx, _, _, _ in self.parts:
-            if ctx is not None:  # sharded groups keep their one context inside the worker
-                g["ctx"].setdefault(ctx._pool_key, []).append(ctx)
+        for part in self.parts:
+            part.release()
         self.parts = []
 
 
@@ -859,6 +859,13 @@ def ctx_occurrences(n_ids, rows=0):
     return min(max(2 * max(n_ids, rows), 1024), MAX_CTX_OCCURRENCES)
 
 
+def ctx_size(n_ids, rows, held=(0, 0)):
+    """(occurrences, output rows) of a batch context for n_ids ids in `rows` output rows, never less than the `held`
+    (occurrences, rows) of the context it replaces: ctx_occurrences for the ids, twice the rows (at least 1024) for the
+    outputs.  Every batch context persia_core and its workers make is sized by it."""
+    return max(ctx_occurrences(n_ids, rows), held[0]), max(2 * rows, 1024, held[1])
+
+
 _STATE_LOCK = threading.RLock()  # configuration / group creation; GPU work takes the lock of the table it touches
 _BACKWARDS = []                   # live Backward engines (direct lookups wait for their queues to drain)
 
@@ -890,8 +897,6 @@ def _forward(batch, device_id, training, direct=False):
 
 def _forward_locked(batch, device_id, training):
     import torch
-
-    from . import shard as SH
 
     _S.ensure_config()
     if batch.embedding_tensor is None:
@@ -928,173 +933,198 @@ def _forward_locked(batch, device_id, training):
             _S.raw_order = raw_names
         elif _S.raw_order != raw_names:
             raise RuntimeError("on R GPUs every batch must carry the same raw slots, in the same order")
+    units = _units(feats, B)
     # R GPUs: a forward that does not train is read from the owners' shards by this rank alone (_start_remote), in Infer
     # and Train jobs; a training forward takes the collective path
-    remote = _S.remote if sharded and not training else None
-    step = _sharded_step(feats, B, training, dev) if sharded and remote is None else {}
+    if sharded and not training and _S.remote is not None:
+        parts = [_Remote(u, dev) for u in units]
+    elif sharded:
+        parts = _sharded_step(units, training, dev)
+    else:
+        parts = [_Local(u, dev) for u in units]
     pending = _Pending()
-    by_slot = {}
-    raw_out = {}
-    for n, x in feats:  # raw slots: one request each (FeatureRawEmbeddingBatch, mod.rs:586-623)
-        sc = _S.by_name[n]
-        if sc.embedding_summation:
-            continue
-        with _STATE_LOCK:
-            g = _S.group(sc.dim)
-        if remote is not None:
-            ids, row_off, _ = _flatten([(n, x)], B)
-            d_ids = torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True)
-            d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-            with g["lock"]:
-                table, index, non_empty, num, counts = remote[sc.dim].forward_raw(d_ids, B, sc.sample_fixed_size,
-                                                                                  sc.index_prefix, _S.prefix_bit,
-                                                                                  row_off=d_off)
-                U, ne = counts.tolist()
+    by_slot, raw_out = {}, {}
+    for u, part in zip(units, parts):
+        with u.g["lock"]:
+            out = part.forward(training)
+            if u.raw:  # the distinct-sign table is sized on the host, like the reference's CPU tensors
+                U, ne = out[4].tolist()
+            if not training:
+                part.release()
+        if u.raw:  # one request per raw slot (FeatureRawEmbeddingBatch, mod.rs:586-623)
+            (n,), (table, index, non_empty, num, _) = u.names, out
             raw_out[n] = (Tensor(table[:U + 1], n), Tensor(index, f"{n}_index"),
                           Tensor(non_empty[:ne], f"{n}_non_empty_index"), num.tolist())
-            continue
-        if sharded:  # R GPUs: one request per owner, through the slot's raw worker (prepared and sized above)
-            wk, kw = step[("raw", n)]
-            with g["lock"]:
-                with _Sharded(g, wk):
-                    table, index, non_empty, num, counts = wk.forward_raw(kw["ids"], B, sc.sample_fixed_size,
-                                                                          row_off=kw["row_off"], training=training)
-                _check_exchange(wk)
-                U, ne = counts.tolist()
-            raw_out[n] = (Tensor(table[:U + 1], n), Tensor(index, f"{n}_index"),
-                          Tensor(non_empty[:ne], f"{n}_non_empty_index"), num.tolist())
-            if training:
-                pending.parts.append((g, None, [n], True, wk))
-            continue
-        key = ("raw", n)
-        pool = g["ctx"].setdefault(key, [])
-        ids, row_off, _ = _flatten([(n, x)], B)
-        g["lock"].acquire()
-        if pool and pool[-1]._cap >= max(len(ids), B):
-            ctx = pool.pop()
         else:
-            cap = ctx_occurrences(len(ids), B)
-            ctx = SH.BatchContext(cap, cap, [sc.index_prefix], None, _S.prefix_bit, dev)
-            ctx._pool_key, ctx._cap = key, cap
-        d_ids = torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True)
-        d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-        table, index, non_empty, num, counts = ctx.forward_raw(g["shard"], d_ids, B, sc.sample_fixed_size, row_off=d_off,
-                                                               training=training)
-        U, ne = counts.tolist()  # the distinct-sign table is sized on the host, like the reference's CPU tensors
-        raw_out[n] = (Tensor(table[:U + 1], n), Tensor(index, f"{n}_index"),
-                      Tensor(non_empty[:ne], f"{n}_non_empty_index"), num.tolist())
+            by_slot.update(zip(u.names, out))
         if training:
-            pending.parts.append((g, ctx, [n], True, None))
-        else:
-            pool.append(ctx)
-        g["lock"].release()
-    for dim in sorted({_S.by_name[n].dim for n, _ in feats if _S.by_name[n].embedding_summation}):
-        dim_part = [(n, x) for n, x in feats if _S.by_name[n].dim == dim and _S.by_name[n].embedding_summation]
-        with _STATE_LOCK:
-            g = _S.group(dim)
-        for k, chunk in enumerate(slot_chunks([_S.by_name[n].index_prefix for n, _ in dim_part])):
-            part = [dim_part[i] for i in chunk]
-            names = [n for n, _ in part]
-            key = tuple(names)
-            if remote is not None:
-                ids, row_off, slot_off = _flatten(part, B)
-                slots = [_S.by_name[n] for n in names]
-                with g["lock"]:
-                    d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
-                    d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-                    out = remote[dim].forward(d_ids, B, [sc.index_prefix for sc in slots], [sc.sqrt_scaling for sc in slots],
-                                              _S.prefix_bit, row_off=d_off, slot_occ_off=slot_off)
-                for i, n in enumerate(names):
-                    by_slot[n] = out[i]
-                continue
-            if sharded:  # R GPUs: the embedding worker's fan-out runs inside the chunk's sharded worker (sized above)
-                wk, kw = step[(dim, k)]
-                with g["lock"]:
-                    with _Sharded(g, wk):
-                        out = wk.forward(kw["ids"], B, training=training, row_off=kw["row_off"],
-                                         slot_occ_off=kw["slot_occ_off"])
-                    _check_exchange(wk)
-                for i, n in enumerate(names):
-                    by_slot[n] = out[i]
-                if training:
-                    pending.parts.append((g, None, names, False, wk))
-                continue
-            pool = g["ctx"].setdefault(key, [])
-            ids, row_off, slot_off = _flatten(part, B)
-            slots = [_S.by_name[n] for n in names]
-            with g["lock"]:
-                d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
-                if pool and pool[-1]._cap >= d_ids.numel():
-                    ctx = pool.pop()
-                else:
-                    cap = ctx_occurrences(int(d_ids.numel()), len(names) * B)
-                    ctx = SH.BatchContext(cap, max(len(names) * max(B, 1) * 2, 1024),
-                                          [_S.by_name[n].index_prefix for n in names],
-                                          [_S.by_name[n].sqrt_scaling for n in names], _S.prefix_bit, dev)
-                    ctx._pool_key, ctx._cap = key, cap
-                d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-                out = ctx.forward(g["shard"], d_ids, slot_off, B, row_off=d_off, training=training)
-                for i, n in enumerate(names):
-                    by_slot[n] = out[i]
-                if training:
-                    pending.parts.append((g, ctx, names, False, None))
-                else:
-                    pool.append(ctx)
+            pending.parts.append(part)
     emb = [Embedding(None, raw=raw_out[n]) if n in raw_out else Embedding(Tensor(by_slot[n], n)) for n, _ in feats]
     to_dev = lambda items: [Tensor(torch.from_numpy(a).to(dev), n) for n, a in items]  # noqa: E731
     return PersiaTrainingBatch(to_dev(batch.non_id_type_features), emb, to_dev(batch.labels), batch.meta_data,
                                pending if training else None)
 
 
-def _sharded_step(feats, B, training, dev):
-    """R GPUs: sizes this step's exchanges from its own batch, agreed by every rank before any rank sends.  Every worker
-    the step calls is prepared (its batch context grown if need be, the batch deduplicated: local work) in the
-    collective order — the raw slots in batch order, then the summation dims ascending, chunk by chunk — and then
-    _agree_and_resize sizes them all with one all-reduce.  Returns {("raw", name) | (dim, chunk): (worker, the
-    forward's arguments)}.  PERSIA_B200_XCHG_CAP and PERSIA_B200_MAX_BATCH size a worker's first exchange and
-    context only."""
-    import torch
+class _Unit:
+    """One lookup of a batch: a raw slot, or a chunk of one dim's summation slots (slot_chunks), with the dim's group.
+    k: the chunk's index among its dim's chunks; dim_names: the dim's summation slots in batch order."""
 
-    plan, step = [], {}
-
-    def add(key, g, wk, need, **kw):
-        plan.append((g, wk, need))
-        step[key] = (wk, kw)
-
-    for n, x in feats:
-        sc = _S.by_name[n]
-        if sc.embedding_summation:
-            continue
+    def __init__(self, feats, B, raw, k=0, dim_names=()):
+        self.names = [n for n, _ in feats]
+        self.slots = [_S.by_name[n] for n in self.names]
+        self.dim, self.B, self.raw, self.k, self.dim_names = self.slots[0].dim, B, raw, k, dim_names
+        self.key = ("raw", self.names[0]) if raw else tuple(self.names)  # (of its contexts in the group's pool)
+        self.prefixes = [sc.index_prefix for sc in self.slots]
+        self.sqrt = None if raw else [sc.sqrt_scaling for sc in self.slots]
         with _STATE_LOCK:
-            g = _S.group(sc.dim)
-        with g["lock"]:
-            ids, row_off, _ = _flatten([(n, x)], B)
-            wk = _sharded_raw_worker(g, sc, B, ids, row_off, dev)
-            d_ids = torch.from_numpy(ids.view(np.int64)).to(dev, non_blocking=True)
-            d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-            need = wk.prepare_raw(d_ids, B, sc.sample_fixed_size, row_off=d_off, training=training)
-        add(("raw", n), g, wk, need, ids=d_ids, row_off=d_off)
+            self.g = _S.group(self.dim)
+        self.ids, self.row_off, self.slot_off = _flatten(feats, B)
+
+    def device_ids(self, dev):
+        """(device ids, device CSR offsets or None, slot offsets, host CSR offsets or None), hash stack applied."""
+        import torch
+
+        d_ids, row_off, slot_off = _to_device_ids(self.ids, self.row_off, self.slot_off, self.slots, self.B, dev)
+        d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
+        return d_ids, d_off, slot_off, row_off
+
+
+def _units(feats, B):
+    """A batch's lookups (_Unit) in the order every rank issues them on R GPUs: the raw slots in batch order, then the
+    summation dims ascending, each chunk by chunk."""
+    units = [_Unit([(n, x)], B, True) for n, x in feats if not _S.by_name[n].embedding_summation]
     for dim in sorted({_S.by_name[n].dim for n, _ in feats if _S.by_name[n].embedding_summation}):
-        dim_part = [(n, x) for n, x in feats if _S.by_name[n].dim == dim and _S.by_name[n].embedding_summation]
-        with _STATE_LOCK:
-            g = _S.group(dim)
-        if g.setdefault("names", tuple(n for n, _ in dim_part)) != tuple(n for n, _ in dim_part):
+        part = [(n, x) for n, x in feats if _S.by_name[n].dim == dim and _S.by_name[n].embedding_summation]
+        names = tuple(n for n, _ in part)
+        for k, chunk in enumerate(slot_chunks([_S.by_name[n].index_prefix for n in names])):
+            units.append(_Unit([part[i] for i in chunk], B, False, k, names))
+    return units
+
+
+# A unit's placement: forward(training), under the group's lock, returns the outputs (summation) or forward_raw's five
+# tensors (raw); backward(grad, is_f16, scale) steps a training forward's batch (_grad_args); release() follows the
+# backward, or the forward at once when it does not train.
+class _Local:
+    """replica_size 1: a batch context from the group's pool on the group's own table, given back by release."""
+
+    def __init__(self, u, dev):
+        self.u, self.dev, self.ctx = u, dev, None
+
+    def forward(self, training):
+        from . import shard as SH
+
+        u = self.u
+        ids, off, slot_off, _ = u.device_ids(self.dev)
+        n, rows = int(ids.numel()), len(u.names) * u.B
+        pool = u.g["ctx"].setdefault(u.key, [])
+        if pool and n <= pool[-1]._size[0] and rows <= pool[-1]._size[1]:
+            self.ctx = pool.pop()
+        else:  # (covers the pool's top as well: batches of alternating shapes end up reusing one context)
+            size = ctx_size(n, rows, pool[-1]._size if pool else (0, 0))
+            self.ctx = SH.BatchContext(*size, u.prefixes, u.sqrt, _S.prefix_bit, self.dev)
+            self.ctx._size = size
+        try:
+            if u.raw:
+                return self.ctx.forward_raw(u.g["shard"], ids, u.B, u.slots[0].sample_fixed_size, row_off=off,
+                                            training=training)
+            return self.ctx.forward(u.g["shard"], ids, slot_off, u.B, row_off=off, training=training)
+        except Exception:
+            self.release()  # (a refused forward gives its context back)
+            raise
+
+    def backward(self, grad, is_f16, scale):
+        if self.u.raw:
+            self.ctx.backward_raw(self.u.g["shard"], grad, scale=scale, is_f16=is_f16)
+        else:
+            self.ctx.backward_ptrs(self.u.g["shard"], grad, is_f16, scale)
+
+    def release(self):
+        self.u.g["ctx"][self.u.key].append(self.ctx)
+
+
+class _ShardedPart:
+    """R GPUs: the unit's ShardedEmbeddingWorker or ShardedRawWorker (created by the first batch), its batch prepared
+    here (local work: _sharded_step sizes the exchange after every unit is prepared).  Every later call is collective
+    and ordered against the group's dumps (_Sharded); the worker keeps its one context."""
+
+    def __init__(self, u, training, dev):
+        g, self.u = u.g, u
+        if u.k == 0 and not u.raw and g.setdefault("names", u.dim_names) != u.dim_names:
             raise RuntimeError("on R GPUs every batch must carry the same summation slots of a dim, in the same order")
-        for k, chunk in enumerate(slot_chunks([_S.by_name[n].index_prefix for n, _ in dim_part])):
-            part = [dim_part[i] for i in chunk]
-            names = [n for n, _ in part]
-            ids, row_off, slot_off = _flatten(part, B)
-            slots = [_S.by_name[n] for n in names]
-            with g["lock"]:
-                d_ids, row_off, slot_off = _to_device_ids(ids, row_off, slot_off, slots, B, dev)
-                if len(g.get("workers", ())) <= k and any(sc.hash_stack_rounds > 0 for sc in slots):
-                    ids = d_ids.cpu().numpy().view(np.uint64)  # (the first batch sizes the exchange from its keys)
-                wk = _sharded_worker(g, k, dim, names, B, ids, row_off, slot_off, dev)
-                d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-                need = wk.prepare(d_ids, B, row_off=d_off, slot_occ_off=slot_off, training=training)
-            add((dim, k), g, wk, need, ids=d_ids, row_off=d_off, slot_occ_off=slot_off)
-    _agree_and_resize(plan, dev)
-    return step
+        with g["lock"]:
+            self.ids, self.off, self.slot_off, row_off = u.device_ids(dev)
+            if u.raw:
+                self.wk = _sharded_raw_worker(u, row_off, dev)
+                self.need = self.wk.prepare_raw(self.ids, u.B, u.slots[0].sample_fixed_size, row_off=self.off,
+                                                training=training)
+            else:
+                self.wk = _sharded_worker(u, self.ids, row_off, self.slot_off, dev)
+                self.need = self.wk.prepare(self.ids, u.B, row_off=self.off, slot_occ_off=self.slot_off,
+                                            training=training)
+
+    def forward(self, training):
+        u = self.u
+        with _Sharded(u.g, self.wk) as wk:
+            if u.raw:
+                out = wk.forward_raw(self.ids, u.B, u.slots[0].sample_fixed_size, row_off=self.off, training=training)
+            else:
+                out = wk.forward(self.ids, u.B, training=training, row_off=self.off, slot_occ_off=self.slot_off)
+        _check_exchange(self.wk)
+        return out
+
+    def backward(self, grad, is_f16, scale):
+        with _Sharded(self.u.g, self.wk) as wk:
+            if self.u.raw:  # (a collective, even when skipped)
+                wk.backward_raw(grad, scale=scale, is_f16=is_f16)
+            else:
+                wk.backward_ptrs(grad, is_f16, scale)
+
+    def release(self):
+        pass
+
+
+class _Remote:
+    """R GPUs, a forward that does not train: the dim's RemoteReader reads the owners' shards, for this rank alone."""
+
+    def __init__(self, u, dev):
+        self.u, self.dev, self.rd = u, dev, _S.remote[u.dim]
+        self.raw_ids = u.device_ids(dev) if u.raw else None  # (a raw slot's ids are copied before the lock is taken)
+
+    def forward(self, training):
+        u = self.u
+        if u.raw:
+            ids, off, _, _ = self.raw_ids
+            return self.rd.forward_raw(ids, u.B, u.slots[0].sample_fixed_size, u.prefixes[0], _S.prefix_bit,
+                                       row_off=off)
+        ids, off, slot_off, _ = u.device_ids(self.dev)
+        return self.rd.forward(ids, u.B, u.prefixes, u.sqrt, _S.prefix_bit, row_off=off, slot_occ_off=slot_off)
+
+    def release(self):
+        pass
+
+
+def _grad_args(u, grads):
+    """(gradient, is_f16, scale) of unit u's backward from the GradientBatch's items ((ptr, shape, is_f16, scale), or
+    None when skipped): a raw slot's pointer to its [U, dim] gradient of the distinct-sign table (persia/ctx.py:970-980)
+    or None, or a pointer (or None) and a scale per summation slot."""
+    items = [grads.get(n) for n in u.names]
+    dtypes = {it[2] for it in items if it is not None}
+    if len(dtypes) > 1:
+        raise RuntimeError("gradients of one batch must share a dtype")
+    ptrs = [it[0] if it else None for it in items]
+    scales = [it[3] if it else 1.0 for it in items]
+    is16 = dtypes.pop() if dtypes else None
+    return (ptrs[0], is16, scales[0]) if u.raw else (ptrs, bool(is16), scales)
+
+
+def _sharded_step(units, training, dev):
+    """R GPUs: sizes this step's exchanges from its own batch, agreed by every rank before any rank sends.  Every unit's
+    worker is prepared (its batch context grown if need be, the batch deduplicated: local work) in the collective
+    order (_units), and then _agree_and_resize sizes them all with one all-reduce.  Returns the units' placements
+    (_ShardedPart).  PERSIA_B200_XCHG_CAP and PERSIA_B200_MAX_BATCH size a worker's first exchange and context only."""
+    parts = [_ShardedPart(u, training, dev) for u in units]
+    _agree_and_resize([(p.u.g, p.wk, p.need) for p in parts], dev)
+    return parts
 
 
 def _agree_and_resize(plan, dev):
@@ -1183,37 +1213,37 @@ def _stage(batch):
                                      _S.prefix_bit)
 
 
-def _sharded_worker(g, k, dim, names, B, ids, row_off, slot_off, dev):
-    """The ShardedEmbeddingWorker (persia_b200/worker.py) of chunk k (slot_chunks) of the dim group, created by the
-    first batch: a collective — every rank's first lookup of the group must happen in the same step (it does: the ranks
-    train in lockstep).  All chunks of a dim serve the rank's one table."""
-    workers = g.setdefault("workers", [])
-    if k < len(workers):
-        return workers[k]
-    import torch
+def _sharded_worker(u, d_ids, row_off, slot_off, dev):
+    """The ShardedEmbeddingWorker (persia_b200/worker.py) of summation unit u (chunk u.k of its dim group), created by
+    the first batch: a collective — every rank's first lookup of the group must happen in the same step (it does: the
+    ranks train in lockstep).  All chunks of a dim serve the rank's one table.  d_ids, row_off, slot_off: u.device_ids."""
+    workers = u.g.setdefault("workers", [])
+    if u.k < len(workers):
+        return workers[u.k]
     import torch.distributed as dist
 
     from .worker import ShardedEmbeddingWorker as W
 
     if not dist.is_initialized():
         raise RuntimeError("replica_size > 1 needs torch.distributed (TrainCtx initialises it; else call init_process_group)")
-    slots = [_S.by_name[n] for n in names]
-    cap = _exchange_cap([(ids[slot_off[i]:slot_off[i + 1]], sc.index_prefix) for i, sc in enumerate(slots)], dev)
-    ragged = row_off is not None
-    per_sample = max(1, -(-len(ids) // max(1, len(names) * B)))
+    # the exchange is sized from this first batch's keys: hash-stacked ones are read back from the device
+    ids = d_ids.cpu().numpy().view(np.uint64) if any(sc.hash_stack_rounds > 0 for sc in u.slots) else u.ids
+    cap = _exchange_cap([(ids[slot_off[i]:slot_off[i + 1]], sc.index_prefix) for i, sc in enumerate(u.slots)], dev)
+    ragged, B = row_off is not None, u.B
+    per_sample = max(1, -(-len(ids) // max(1, len(u.names) * B)))
     max_batch = int(os.environ.get("PERSIA_B200_MAX_BATCH", B))
     # the group's table is the rank's shard: raw workers of this dim serve it too
-    wk = W.distributed(len(names), dim, [sc.index_prefix for sc in slots], _S.capacity, cap, _S.optimizer or {}, dev,
-                       hyper=_S.hyper, max_batch=max(B, max_batch), sqrt_scaling=[sc.sqrt_scaling for sc in slots],
-                       rows_f32=ragged, prefix_bit=_S.prefix_bit, max_ids_per_sample=2 * per_sample if ragged else 1,
-                       shard=g["shard"])
+    wk = W.distributed(len(u.names), u.dim, u.prefixes, _S.capacity, cap, _S.optimizer or {}, dev, hyper=_S.hyper,
+                       max_batch=max(B, max_batch), sqrt_scaling=u.sqrt, rows_f32=ragged, prefix_bit=_S.prefix_bit,
+                       max_ids_per_sample=2 * per_sample if ragged else 1, shard=u.g["shard"])
     workers.append(wk)
     return wk
 
 
-def _sharded_raw_worker(g, sc, B, ids, row_off, dev):
-    """Raw slot `sc`'s ShardedRawWorker (persia_b200/worker.py) over the rank's table of its dim, created by the first
-    batch that carries the slot: a collective, like _sharded_worker."""
+def _sharded_raw_worker(u, row_off, dev):
+    """Raw unit u's ShardedRawWorker (persia_b200/worker.py) over the rank's table of its dim, created by the first
+    batch that carries the slot: a collective, like _sharded_worker.  row_off: the host CSR offsets or None."""
+    (sc,), g, B, ids = u.slots, u.g, u.B, u.ids
     wk = g.setdefault("raw_workers", {}).get(sc.name)
     if wk is not None:
         return wk
@@ -1372,41 +1402,9 @@ class Backward:  # backward.rs:203-405
                 import torch
 
                 torch.cuda.current_stream().wait_event(ready)
-            for g, ctx, names, is_raw, wk in p.parts:
-                with g["lock"]:
-                    if is_raw:  # [U, dim] gradient of the distinct-sign table (persia/ctx.py:970-980)
-                        item = grads.get(names[0])
-                        if wk is not None:  # R GPUs: the slot's raw worker (a collective, even when skipped)
-                            with _Sharded(g, wk):
-                                if item is None:
-                                    wk.backward_raw(None)
-                                else:
-                                    ptr, shape, is16, sc = item
-                                    wk.backward_raw(ptr, scale=sc, is_f16=is16)
-                        elif item is None:
-                            ctx.backward_raw(g["shard"], None)
-                        else:
-                            ptr, shape, is16, sc = item
-                            ctx.backward_raw(g["shard"], ptr, scale=sc, is_f16=is16)
-                        continue
-                    ptrs, scales, f16 = [], [], None
-                    for n in names:
-                        item = grads.get(n)
-                        if item is None:
-                            ptrs.append(None)
-                            scales.append(1.0)
-                            continue
-                        ptr, shape, is16, sc = item
-                        if f16 is not None and f16 != is16:
-                            raise RuntimeError("gradients of one batch must share a dtype")
-                        f16 = is16
-                        ptrs.append(ptr)
-                        scales.append(sc)
-                    if wk is not None:  # R GPUs: the chunk's sharded worker
-                        with _Sharded(g, wk):
-                            wk.backward_ptrs(ptrs, bool(f16), scales)
-                    else:
-                        ctx.backward_ptrs(g["shard"], ptrs, bool(f16), scales)
+            for part in p.parts:
+                with part.u.g["lock"]:
+                    part.backward(*_grad_args(part.u, grads))
             _maybe_flush_incremental()
         finally:
             p.release()

@@ -256,16 +256,16 @@ class ShardedEmbeddingWorker:
 
     # ---- sizing each step from its own batch (PB_PHASE_PREPARE, pb_xchg_need) ---------------------------------------
     def _fit_ctx(self, n_occ, rows):
-        """Grows the batch context when a batch of n_occ ids in `rows` output rows does not fit: with
-        persia_core.ctx_occurrences' headroom and 2^24 limit (local to this rank; the context holds one batch)."""
+        """Grows the batch context when a batch of n_occ ids in `rows` output rows does not fit, as persia_core.ctx_size
+        sizes it (local to this rank; the context holds one batch)."""
         if n_occ <= self.ctx_occ and rows <= self.ctx_rows:
             return
-        from .persia_core import ctx_occurrences
+        from .persia_core import ctx_size
 
-        occ = max(ctx_occurrences(n_occ, rows), self.ctx_occ)
+        size = ctx_size(n_occ, rows, (self.ctx_occ, self.ctx_rows))
         self._torch_stream().synchronize()
         self.ctx.close()
-        self._new_ctx(occ, max(2 * rows, 1024, self.ctx_rows))
+        self._new_ctx(*size)
 
     def _need(self):
         out = (C.c_uint32 * 1)()
@@ -615,14 +615,13 @@ class RemoteReader:
         return C.c_void_p(self._torch_stream().cuda_stream)
 
     def _ctx(self, key, n_occ, rows):
-        """The batch context of `key`, grown (persia_core.ctx_occurrences' rule) when n_occ ids in `rows` rows do not fit."""
-        from .persia_core import ctx_occurrences
+        """The batch context of `key`, grown (persia_core.ctx_size) when n_occ ids in `rows` rows do not fit."""
+        from .persia_core import ctx_size
 
         got = self._ctxs.get(key)
         if got is not None and n_occ <= got[1] and rows <= got[2]:
             return got[0]
-        occ = max(ctx_occurrences(n_occ, rows), got[1] if got else 0)
-        out_rows = max(2 * rows, 1024, got[2] if got else 0)
+        occ, out_rows = ctx_size(n_occ, rows, got[1:] if got else (0, 0))
         if got is not None:
             self._torch_stream().synchronize()
             got[0].close()

@@ -436,13 +436,13 @@ def test_raw_slot_past_one_spine_trip(torch_cuda, pb, oracle, n):
 # ---------------------------------------------------------------------------------------------- 6. raw staging
 @pytest.mark.parametrize("dim", [128, 1024])
 def test_raw_staging_at_persia_core_sizes(torch_cuda, pb, oracle, dim):
-    """A raw batch of 2^23 - 7 ids in a context made as persia_core makes it (ctx_occurrences: twice the ids, here
+    """A raw batch of 2^23 - 7 ids in a context made as persia_core makes it (ctx_size: twice the ids, here
     2^24 - 14 occurrences).  The backward stages the [U, dim] gradient in f32.  Sized by the context that staging was
     2^24 x 1024 x 4 bytes = 64 GB at dim 1024, beside the 17 GB f16 table of the forward: more than the GPU holds.
     Sized by the batch it is half that.  Outputs against the oracle on the distinct ids in first-occurrence order (the
     same numbering, the same table rows) and the index against the numbering; entries after one f32 step with a loss
     scale against the oracle (a raw gradient row steps its own sign only)."""
-    from persia_b200.persia_core import ctx_occurrences
+    from persia_b200.persia_core import ctx_size
 
     torch = torch_cuda
     m = Meter(torch, f"raw staging dim={dim}")
@@ -450,12 +450,12 @@ def test_raw_staging_at_persia_core_sizes(torch_cuda, pb, oracle, dim):
     fixed = 4
     ids, row_off = SC.stage_case(6)
     n, B = ids.size, row_off.size - 1
-    cap = ctx_occurrences(n, B)
+    cap, rows = ctx_size(n, B)
     pf = oracle.index_prefix(0)
     s = pb.EmbeddingShard(dim, 1 << 13, 0)
     s.set_optimizer(SGD, lr=OPT[SGD]["lr"])
     s.configure()
-    ctx = pb.BatchContext(cap, cap, [pf])
+    ctx = pb.BatchContext(cap, rows, [pf])
     try:
         table, index, non_empty, num, counts = ctx.forward_raw(s, to_dev_ids(ids, DEV), B, fixed,
                                                                row_off=to_dev_i32(row_off, DEV))

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 from persia_b200.native import PB_MAX_SLOTS
-from persia_b200.persia_core import MAX_CTX_OCCURRENCES, ctx_occurrences, parse_embedding_config, slot_chunks
+from persia_b200.persia_core import MAX_CTX_OCCURRENCES, ctx_occurrences, ctx_size, parse_embedding_config, slot_chunks
 
 
 def _check(prefixes, chunks):
@@ -102,6 +102,10 @@ def test_context_sizing_is_clamped():
     assert ctx_occurrences(1000, 128 * 65535) == 2 * 128 * 65535  # rows alone never refuse a batch
     with pytest.raises(RuntimeError, match=f"holds {(1 << 24) + 1} ids.*2\\^24"):
         ctx_occurrences((1 << 24) + 1)
+    # (occurrences, output rows): twice the rows, at least 1024, never less than the context being replaced holds
+    assert ctx_size(1600, 8) == (3200, 1024)
+    assert ctx_size(2048, 2048) == (4096, 4096)
+    assert ctx_size(10, 3, held=(5000, 2000)) == (5000, 2000)
 
 
 def test_batch_context_refuses_more_than_128_slots():
