@@ -8,7 +8,9 @@
  * i.e. a cudaStream_t), never synchronises the device unless its comment says so, and returns 0 or a
  * negative pb_status; pb_last_error() gives the message for the calling thread.
  *
- * Conventions: `d_` = device pointer, `h_` = host pointer.  Gradient, output and update buffers (the gradients of
+ * Conventions: `d_` = device pointer, `h_` = host pointer.  A create or call that returns an error leaves nothing
+ * allocated by it, but for what the steps it completed before the error acquired (a context's first-use buffers, say),
+ * which the object keeps and its next call uses instead of acquiring them again.  Gradient, output and update buffers (the gradients of
  * pb_backward, pb_backward_sharded, pb_backward_raw(_sharded) and pb_update; d_out_f16 of pb_forward and
  * pb_forward_sharded; d_table_f16 of pb_forward_raw(_sharded)) must be 16-byte aligned: the kernels access them with vector loads and stores.  A
  * call given a pointer that is not returns PB_ERR_INVALID before it enqueues anything.  (A contiguous tensor view at

@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <random>
 #include <string>
 #include <utility>
@@ -12,24 +13,11 @@
 #include <unistd.h>
 
 #include "pb_kernels.cuh"
+#include "pb_own.cuh"
 
 using namespace pb;
 
 namespace {
-
-thread_local std::string g_err;
-
-int fail(int code, const std::string& msg) {
-  g_err = msg;
-  return code;
-}
-
-#define PB_CUDA(expr)                                                                              \
-  do {                                                                                             \
-    cudaError_t e__ = (expr);                                                                      \
-    if (e__ != cudaSuccess)                                                                        \
-      return fail(PB_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e__));               \
-  } while (0)
 
 struct DeviceGuard {
   int prev = -1;
@@ -109,7 +97,7 @@ struct pb_table {
   // host-memory tier (pb_tier.cu): `host` = this table's rows are mapped pinned host memory (pb_table_create_host);
   // `tier` = the host table attached behind this one, `tier_of` = the table this one is attached behind
   bool host = false;
-  float* host_rows = nullptr;  // host address of d.rows (cudaFreeHost)
+  float* host_rows = nullptr;  // host address of d.rows
   pb_table* tier = nullptr;
   pb_table* tier_of = nullptr;
   uint32_t* move_cells = nullptr;  // the eviction check's victim list (with rebuild_keys / rebuild_rows), `capacity` words
@@ -119,7 +107,7 @@ struct pb_table {
   Mark index, step;
   // incremental updates (pb_table_enable_incremental): the set of signs stepped since the last take; cells == null: off
   IncDev inc{};
-  unsigned long long* inc_host = nullptr;  // host address of inc.mirror (cudaFreeHost)
+  unsigned long long* inc_host = nullptr;  // host address of inc.mirror
   // checkpoint images (pb_table_dump_reserve): one allocation holding every DumpWs array; null: none reserved
   DumpWs dump{};
   void* dump_mem = nullptr;
@@ -130,6 +118,7 @@ struct pb_table {
   // pb_table_export_live_view: peers read in place while the table keeps training; sweeps, rebuilds, pb_set_rows and
   // pb_table_clear keep `seq` odd while they move cells or reuse rows (one table, one export mode)
   bool live = false;
+  Owned own;  // every CUDA resource above
 };
 
 struct pb_ctx {
@@ -200,13 +189,14 @@ struct pb_ctx {
   // pb_forward_remote / pb_forward_raw_remote: the rows read from their owners, one per distinct item (grow_stage)
   float* remote_stage = nullptr;
   size_t remote_stage_floats = 0;
+  Owned own;  // every CUDA resource above
 };
 enum { PREP_NONE = 0, PREP_SUM = 1, PREP_RAW = 2 };
 
 namespace {
 
-int ensure_alloc(pb_table* t) {
-  if (t->allocated) return PB_OK;
+// The table's index, rows, counters and row_tick, acquired into `o`: the caller adopts `o`, then sets `allocated`.
+int acquire_storage(pb_table* t, Owned& o) {
   if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered (OptimizerNotFoundError)");
   uint32_t dim = t->cfg.dim;
   uint32_t state = 0;
@@ -228,44 +218,57 @@ int ensure_alloc(pb_table* t) {
   d.n_cells = next_pow2(want);
   d.cell_mask = d.n_cells - 1;
   d.bucket_mask = d.n_cells / BUCKET - 1;
-  PB_CUDA(cudaMalloc(&d.cells, sizeof(Cell) * ((size_t)d.n_cells + N_SPECIAL)));
-  if (t->host) {  // not write-combined: the host reads these rows back (checkpoints)
-    PB_CUDA(cudaHostAlloc((void**)&t->host_rows, sizeof(float) * (size_t)d.capacity * d.stride,
-                          cudaHostAllocMapped | cudaHostAllocPortable));
-    PB_CUDA(cudaHostGetDevicePointer((void**)&d.rows, t->host_rows, 0));
-  } else {
-    PB_CUDA(cudaMalloc(&d.rows, sizeof(float) * (size_t)d.capacity * d.stride));
-  }
-  PB_CUDA(cudaMalloc(&d.counters, sizeof(uint32_t) * CTR_COUNT));
-  PB_CUDA(cudaMalloc(&d.row_tick, sizeof(uint32_t) * (size_t)d.capacity));
+  const size_t rows_bytes = sizeof(float) * (size_t)d.capacity * d.stride;
+  int rc;
+  if ((rc = o.dev(d.cells, sizeof(Cell) * ((size_t)d.n_cells + N_SPECIAL))) ||
+      // a host table's rows are not write-combined: the host reads them back (checkpoints)
+      (rc = t->host ? o.mapped(t->host_rows, d.rows, rows_bytes) : o.dev(d.rows, rows_bytes)) ||
+      (rc = o.dev(d.counters, sizeof(uint32_t) * CTR_COUNT)) || (rc = o.dev(d.row_tick, sizeof(uint32_t) * (size_t)d.capacity)))
+    return rc;
   PB_CUDA(cudaMemset(d.row_tick, 0, sizeof(uint32_t) * (size_t)d.capacity));
   PB_CUDA(cudaMemset(d.counters, 0, sizeof(uint32_t) * CTR_COUNT));
   launch_fill_cells(d.cells, (uint64_t)d.n_cells + N_SPECIAL, 0);
   d.free_rows = nullptr;
   PB_CUDA(cudaDeviceSynchronize());
+  return PB_OK;
+}
+
+int ensure_alloc(pb_table* t) {
+  if (t->allocated) return PB_OK;
+  Owned o;
+  if (int rc = acquire_storage(t, o)) return rc;
+  t->own.adopt(o);
   t->allocated = true;
   return PB_OK;
 }
 
 int ensure_scratch(pb_table* t, uint32_t n) {
   if (n <= t->scratch_cap) return PB_OK;
-  if (t->scratch) cudaFree(t->scratch);
-  t->scratch = nullptr;
+  t->own.release(t->scratch);
   t->scratch_cap = 0;
   uint32_t cap = next_pow2(n);
-  PB_CUDA(cudaMalloc(&t->scratch, sizeof(uint32_t) * (size_t)cap));
+  if (int rc = t->own.dev(t->scratch, sizeof(uint32_t) * (size_t)cap)) return rc;
   t->scratch_cap = cap;
   return PB_OK;
 }
 
-// the free-row stack, the sweep's workspace and the rebuild's pair buffer, allocated by the first sweep
+// the free-row stack (into `free_rows`, the gate, once the rest is held), the sweep's workspace and the rebuild's
+// pair buffer, acquired into `o`
+int acquire_evict_ws(pb_table* t, Owned& o, uint32_t*& free_rows) {
+  const size_t cap = t->d.capacity;
+  int rc;
+  if ((rc = o.dev(t->evict_ws, sizeof(uint32_t) * EVICT_WS_WORDS)) || (rc = o.dev(t->rebuild_keys, sizeof(uint64_t) * cap)) ||
+      (rc = o.dev(t->rebuild_rows, sizeof(uint32_t) * cap)))
+    return rc;
+  return o.dev(free_rows, sizeof(uint32_t) * cap);
+}
+
+// allocated by the first sweep
 int ensure_evict_ws(pb_table* t) {
   if (t->d.free_rows) return PB_OK;
-  const size_t cap = t->d.capacity;
-  PB_CUDA(cudaMalloc(&t->evict_ws, sizeof(uint32_t) * EVICT_WS_WORDS));
-  PB_CUDA(cudaMalloc(&t->rebuild_keys, sizeof(uint64_t) * cap));
-  PB_CUDA(cudaMalloc(&t->rebuild_rows, sizeof(uint32_t) * cap));
-  PB_CUDA(cudaMalloc(&t->d.free_rows, sizeof(uint32_t) * cap));
+  Owned o;
+  if (int rc = acquire_evict_ws(t, o, t->d.free_rows)) return rc;
+  t->own.adopt(o);
   return PB_OK;
 }
 
@@ -519,14 +522,6 @@ const float* advance_adam_pair(pb_table* t, int k, cudaStream_t st) {
   return t->adam_dev + 2 * k;
 }
 
-void free_incremental(pb_table* t) {
-  if (t->inc.cells) cudaFree(t->inc.cells);
-  if (t->inc.ctr) cudaFree(t->inc.ctr);
-  if (t->inc_host) cudaFreeHost(t->inc_host);
-  t->inc = IncDev{};
-  t->inc_host = nullptr;
-}
-
 // ---- what the local and sharded forms of the forwards and backwards share ------------------------------------------
 int check_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
                   const uint32_t* h_slot_occ_off, uint32_t batch, void* d_out_f16) {
@@ -734,16 +729,12 @@ int pb_table_create(int device, const pb_table_cfg* cfg, pb_table** out) {
   PB_CUDA(cudaGetDeviceCount(&ndev));
   if (device < 0 || device >= ndev) return fail(PB_ERR_INVALID, "no such CUDA device");
   DeviceGuard g(device);
-  pb_table* t = new pb_table();
+  std::unique_ptr<pb_table> t(new pb_table());
   t->device = device;
   t->cfg = *cfg;
-  cudaError_t e = cudaEventCreateWithFlags(&t->index.ev, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&t->step.ev, cudaEventDisableTiming);
-  if (e != cudaSuccess) {
-    pb_table_destroy(t);
-    return fail(PB_ERR_CUDA, std::string("pb_table_create: ") + cudaGetErrorString(e));
-  }
-  *out = t;
+  int rc;
+  if ((rc = t->own.event(t->index.ev)) || (rc = t->own.event(t->step.ev))) return rc;
+  *out = t.release();
   return PB_OK;
 }
 
@@ -765,11 +756,24 @@ int pb_table_attach_tier(pb_table* t, pb_table* tier) {
   if (t->cfg.dim != tier->cfg.dim || t->op.kind != tier->op.kind)
     return fail(PB_ERR_INVALID, "the tier must have the table's dim and optimizer (one entry layout)");
   DeviceGuard g(t->device);
-  int rc;
-  if ((rc = ensure_alloc(t)) || (rc = ensure_alloc(tier))) return rc;
-  if (t->d.stride != tier->d.stride) return fail(PB_ERR_INVALID, "the tier's row stride differs from the table's");
-  if ((rc = ensure_evict_ws(t)) || (rc = ensure_evict_ws(tier))) return rc;
-  PB_CUDA(cudaMalloc(&t->move_cells, sizeof(uint32_t) * (size_t)t->d.capacity));
+  // both tables' storage and sweep workspace, and the victim list: committed together once all are held
+  pb_table* tt[2] = {t, tier};
+  Owned o[2];
+  uint32_t* free_rows[2] = {t->d.free_rows, tier->d.free_rows};
+  uint32_t* move_cells = nullptr;
+  int rc = 0;
+  for (int i = 0; i < 2 && !rc; ++i)
+    if (!tt[i]->allocated) rc = acquire_storage(tt[i], o[i]);
+  if (!rc && t->d.stride != tier->d.stride) rc = fail(PB_ERR_INVALID, "the tier's row stride differs from the table's");
+  for (int i = 0; i < 2 && !rc; ++i)
+    if (!free_rows[i]) rc = acquire_evict_ws(tt[i], o[i], free_rows[i]);
+  if (rc || (rc = o[0].dev(move_cells, sizeof(uint32_t) * (size_t)t->d.capacity))) return rc;
+  for (int i = 0; i < 2; ++i) {
+    tt[i]->own.adopt(o[i]);
+    tt[i]->allocated = true;
+    tt[i]->d.free_rows = free_rows[i];
+  }
+  t->move_cells = move_cells;
   t->tier = tier;
   tier->tier_of = t;
   return PB_OK;
@@ -836,27 +840,27 @@ int pb_table_enable_incremental(pb_table* t, uint64_t capacity) {
   if (capacity >= (1ull << 30)) return fail(PB_ERR_INVALID, "capacity must be < 2^30 signs");
   DeviceGuard g(t->device);
   PB_CUDA(cudaDeviceSynchronize());  // enqueued marks may still use the old set
-  free_incremental(t);
+  t->own.release(t->inc.cells);
+  t->own.release(t->inc.ctr);
+  t->own.release(t->inc_host);
+  t->inc = IncDev{};
   if (!capacity) return PB_OK;
-  IncDev& s = t->inc;
+  IncDev s{};
   s.capacity = capacity;
   s.n_cells = next_pow2(2 * capacity < 1024 ? 1024 : 2 * capacity);
   s.bucket_mask = s.n_cells / BUCKET - 1;
-  cudaError_t e = cudaMalloc(&s.cells, sizeof(Cell) * ((size_t)s.n_cells + N_SPECIAL));
-  if (e == cudaSuccess) e = cudaMalloc(&s.ctr, sizeof(unsigned long long) * INC_WORDS);
-  if (e == cudaSuccess) e = cudaHostAlloc((void**)&t->inc_host, sizeof(unsigned long long), cudaHostAllocMapped | cudaHostAllocPortable);
-  if (e == cudaSuccess) {
-    *t->inc_host = 0;
-    e = cudaHostGetDevicePointer((void**)&s.mirror, t->inc_host, 0);
-  }
-  if (e == cudaSuccess) {
-    launch_inc_fill(s, 0);
-    e = cudaDeviceSynchronize();
-  }
-  if (e != cudaSuccess) {
-    free_incremental(t);
-    return fail(PB_ERR_CUDA, std::string("pb_table_enable_incremental: ") + cudaGetErrorString(e));
-  }
+  Owned o;
+  unsigned long long* host = nullptr;
+  int rc;
+  if ((rc = o.dev(s.cells, sizeof(Cell) * ((size_t)s.n_cells + N_SPECIAL))) ||
+      (rc = o.dev(s.ctr, sizeof(unsigned long long) * INC_WORDS)) || (rc = o.mapped(host, s.mirror, sizeof(unsigned long long))))
+    return rc;
+  *host = 0;
+  launch_inc_fill(s, 0);
+  PB_CUDA(cudaDeviceSynchronize());
+  t->own.adopt(o);
+  t->inc = s;
+  t->inc_host = host;
   return PB_OK;
 }
 
@@ -896,33 +900,7 @@ int pb_table_destroy(pb_table* t) {
   DeviceGuard g(t->device);
   if (t->tier) t->tier->tier_of = nullptr;
   if (t->tier_of) t->tier_of->tier = nullptr;
-  if (t->move_cells) cudaFree(t->move_cells);
-  if (t->index.ev) cudaEventDestroy(t->index.ev);
-  if (t->step.ev) cudaEventDestroy(t->step.ev);
-  if (t->allocated) {
-    cudaDeviceSynchronize();
-    cudaFree(t->d.cells);
-    if (t->host) cudaFreeHost(t->host_rows);
-    else cudaFree(t->d.rows);
-    cudaFree(t->d.counters);
-    cudaFree(t->d.row_tick);
-    if (t->d.free_rows) cudaFree(t->d.free_rows);
-    if (t->evict_ws) cudaFree(t->evict_ws);
-    if (t->rebuild_keys) cudaFree(t->rebuild_keys);
-    if (t->rebuild_rows) cudaFree(t->rebuild_rows);
-  }
-  if (t->inc.cells) {
-    cudaDeviceSynchronize();
-    free_incremental(t);
-  }
-  if (t->dump_mem) {
-    cudaDeviceSynchronize();
-    cudaFree(t->dump_mem);
-  }
-  if (t->stats_ws) cudaFree(t->stats_ws);
-  if (t->seq) cudaFree(t->seq);
-  if (t->scratch) cudaFree(t->scratch);
-  if (t->adam_dev) cudaFree(t->adam_dev);
+  if (t->allocated || t->inc.cells || t->dump_mem) cudaDeviceSynchronize();  // (enqueued work may still use them)
   delete t;
   return PB_OK;
 }
@@ -932,6 +910,7 @@ int pb_table_set_optimizer(pb_table* t, const pb_optim_cfg* c) {
   if (c->kind < PB_OPT_SGD || c->kind > PB_OPT_ADAM) return fail(PB_ERR_INVALID, "unknown optimizer kind");
   if (t->allocated && c->kind != t->op.kind)
     return fail(PB_ERR_STATE, "optimizer kind cannot change once rows are resident (row layout is fixed)");
+  int rc;
   t->op.kind = c->kind;
   t->op.lr = c->lr;
   t->op.wd = c->wd;
@@ -943,9 +922,13 @@ int pb_table_set_optimizer(pb_table* t, const pb_optim_cfg* c) {
   if (!t->has_op && c->kind == PB_OPT_ADAM) {  // AdamPowerOfBetas starts at (beta1, beta2) for every feature group (optim.rs:118-124)
     DeviceGuard g(t->device);
     t->adam_keys.clear();
-    if (!t->adam_dev) PB_CUDA(cudaMalloc(&t->adam_dev, sizeof(float) * 2 * PB_ADAM_KEYS));
-    launch_adam_fill(t->adam_dev, c->beta1, c->beta2, 0);
+    Owned o;
+    float* pairs = t->adam_dev;
+    if (!pairs && (rc = o.dev(pairs, sizeof(float) * 2 * PB_ADAM_KEYS))) return rc;
+    launch_adam_fill(pairs, c->beta1, c->beta2, 0);
     PB_CUDA(cudaDeviceSynchronize());
+    t->own.adopt(o);
+    t->adam_dev = pairs;
   }
   t->has_op = true;
   return PB_OK;
@@ -1002,8 +985,9 @@ int pb_table_index_stats(pb_table* t, uint64_t h_out[3], void* stream) {
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if (int rc = call.begin(t, st, CALL_ALL)) return rc;
-  if (!t->stats_ws) PB_CUDA(cudaMalloc(&t->stats_ws, 3 * sizeof(uint32_t)));
+  int rc;
+  if ((rc = call.begin(t, st, CALL_ALL))) return rc;
+  if (!t->stats_ws && (rc = t->own.dev(t->stats_ws, 3 * sizeof(uint32_t)))) return rc;
   launch_index_stats(t->d, t->stats_ws, st);
   uint32_t c[3];
   PB_CUDA(cudaMemcpyAsync(c, t->stats_ws, sizeof(c), cudaMemcpyDeviceToHost, st));
@@ -1168,12 +1152,6 @@ uint64_t dump_items(pb_table* t, uint64_t max_bytes) {
   return max_bytes > 28 ? (max_bytes - 28) / nb : 0;
 }
 
-void dump_free(pb_table* t) {
-  if (t->dump_mem) cudaFree(t->dump_mem);
-  t->dump_mem = nullptr;
-  t->dump = DumpWs{};
-}
-
 // a dump call on `t`: the table a tier is attached to, with a workspace of at least `items` entries
 int dump_ready(pb_table* t, uint64_t items) {
   if (t->tier_of) return fail(PB_ERR_INVALID, "dump the table the tier is attached to");
@@ -1195,12 +1173,13 @@ int pb_table_dump_reserve(pb_table* t, uint64_t max_bytes) {
   if (items < 1) items = 1;
   if (items >= (1ull << 31)) return fail(PB_ERR_INVALID, "a dump image holds fewer than 2^31 entries");
   PB_CUDA(cudaDeviceSynchronize());  // a part issued on the old workspace may still run
-  dump_free(t);
+  t->own.release(t->dump_mem);
+  t->dump = DumpWs{};
   const uint32_t m = (uint32_t)items;
   auto r = [](uint64_t b) { return (b + 255) & ~255ull; };
   const uint64_t sort_bytes = dump_sort_bytes(m);
   const uint64_t sz8 = r(8ull * m), sz4 = r(4ull * m);
-  PB_CUDA(cudaMalloc(&t->dump_mem, 3 * sz8 + 6 * sz4 + 256 + r(sort_bytes)));
+  if (int rc = t->own.dev(t->dump_mem, 3 * sz8 + 6 * sz4 + 256 + r(sort_bytes))) return rc;
   char* p = static_cast<char*>(t->dump_mem);
   DumpWs& w = t->dump;
   w.key = reinterpret_cast<uint64_t*>(p), p += sz8;
@@ -1220,7 +1199,8 @@ int pb_table_dump_release(pb_table* t) {
   if (!t->dump_mem) return PB_OK;
   DeviceGuard g(t->device);
   PB_CUDA(cudaDeviceSynchronize());
-  dump_free(t);
+  t->own.release(t->dump_mem);
+  t->dump = DumpWs{};
   return PB_OK;
 }
 
@@ -1287,31 +1267,22 @@ struct pb_image {
   cudaStream_t st = nullptr;  // the stream of the latest call: workspace is allocated and freed in its order
   unsigned long long h_dims[LOAD_DIMS], h_pairs[LOAD_PAIRS];
   uint32_t h_counts[LOAD_PAIRS], h_flags[LOAD_FLAGS];
+  Owned own;  // the workspace
 };
 
 namespace {
 
-// The workspace is stream-ordered (cudaMallocAsync / cudaFreeAsync on the load's stream): a load beside training never
-// waits for the device as a whole, and a buffer is released only after the inserts issued before that read it.
-void free_on(void* p, cudaStream_t st) {
-  if (p) cudaFreeAsync(p, st);
-}
-
-void image_free(pb_image* im, cudaStream_t st) {
-  free_on(im->off, st), free_on(im->slot, st), free_on(im->sel, st), free_on(im->tmp, st);
-  free_on(im->st_signs, st), free_on(im->st_ent, st), free_on(im->sum_mem, st), free_on(im->d_count, st);
-  im->off = nullptr, im->slot = nullptr, im->sel = nullptr, im->tmp = nullptr;
-  im->st_signs = nullptr, im->st_ent = nullptr, im->sum_mem = nullptr, im->d_count = nullptr;
-  im->pos_cap = 0, im->tmp_bytes = 0, im->st_entries = 0, im->st_floats = 0;
-}
-
-// the summary, on first use
+// The workspace is stream-ordered (Owned::async, released on the load's stream): a load beside training never waits
+// for the device as a whole, and a buffer is released only after the inserts issued before that read it.
+// The summary, on first use.
 int image_ready(pb_image* im, cudaStream_t st) {
   im->st = st;
   if (im->sum_mem) return PB_OK;
   const size_t sum_bytes = sizeof(unsigned long long) * (LOAD_DIMS + LOAD_PAIRS) + sizeof(uint32_t) * (LOAD_PAIRS + LOAD_FLAGS);
-  PB_CUDA(cudaMallocAsync(&im->sum_mem, sum_bytes + 16, st));
-  PB_CUDA(cudaMallocAsync((void**)&im->d_count, sizeof(uint32_t), st));
+  Owned o;
+  int rc;  // (sum_mem, the gate, last)
+  if ((rc = o.async(im->d_count, sizeof(uint32_t), st)) || (rc = o.async(im->sum_mem, sum_bytes + 16, st))) return rc;
+  im->own.adopt(o);
   LoadImg& L = im->L;
   L.dims = static_cast<unsigned long long*>(im->sum_mem);
   L.pairs = L.dims + LOAD_DIMS;
@@ -1325,14 +1296,20 @@ int image_room(pb_image* im, uint32_t n, cudaStream_t st) {
   int rc = image_ready(im, st);
   if (rc) return rc;
   if (n <= im->pos_cap && im->pos_cap) return PB_OK;
-  free_on(im->off, st), free_on(im->slot, st), free_on(im->sel, st), free_on(im->tmp, st);
-  im->off = nullptr, im->slot = nullptr, im->sel = nullptr, im->tmp = nullptr, im->pos_cap = 0;
+  im->own.release(im->off, st), im->own.release(im->slot, st), im->own.release(im->sel, st), im->own.release(im->tmp, st);
+  im->pos_cap = 0;
   const uint32_t cap = n ? n : 1;
-  PB_CUDA(cudaMallocAsync((void**)&im->off, sizeof(uint64_t) * cap, st));
-  PB_CUDA(cudaMallocAsync((void**)&im->slot, cap, st));
-  PB_CUDA(cudaMallocAsync((void**)&im->sel, sizeof(uint32_t) * cap, st));
-  im->tmp_bytes = load_list_bytes(cap);
-  PB_CUDA(cudaMallocAsync(&im->tmp, im->tmp_bytes ? im->tmp_bytes : 16, st));
+  const size_t tmp_bytes = load_list_bytes(cap);
+  Owned o;
+  uint64_t* off;
+  uint8_t* slot;
+  uint32_t* sel;
+  void* tmp;
+  if ((rc = o.async(off, sizeof(uint64_t) * cap, st)) || (rc = o.async(slot, cap, st)) ||
+      (rc = o.async(sel, sizeof(uint32_t) * cap, st)) || (rc = o.async(tmp, tmp_bytes ? tmp_bytes : 16, st)))
+    return rc;
+  im->own.adopt(o);
+  im->off = off, im->slot = slot, im->sel = sel, im->tmp = tmp, im->tmp_bytes = tmp_bytes;
   im->pos_cap = cap;
   return PB_OK;
 }
@@ -1376,11 +1353,15 @@ int image_summary(pb_image* im, uint64_t* h_summary, uint32_t max_rows, uint32_t
   *h_rows = rows;
   const uint64_t ent = most < im->max_chunk ? most : im->max_chunk;
   if (ent > im->st_entries || ent * widest > im->st_floats) {
-    free_on(im->st_signs, st), free_on(im->st_ent, st);
-    im->st_signs = nullptr, im->st_ent = nullptr, im->st_entries = 0, im->st_floats = 0;
-    PB_CUDA(cudaMallocAsync((void**)&im->st_signs, sizeof(uint64_t) * ent, st));
-    PB_CUDA(cudaMallocAsync((void**)&im->st_ent, sizeof(float) * ent * widest, st));
-    im->st_entries = ent, im->st_floats = ent * widest;
+    im->own.release(im->st_signs, st), im->own.release(im->st_ent, st);
+    im->st_entries = 0, im->st_floats = 0;
+    Owned o;
+    uint64_t* signs;
+    float* ent_rows;
+    int rc;
+    if ((rc = o.async(signs, sizeof(uint64_t) * ent, st)) || (rc = o.async(ent_rows, sizeof(float) * ent * widest, st))) return rc;
+    im->own.adopt(o);
+    im->st_signs = signs, im->st_ent = ent_rows, im->st_entries = ent, im->st_floats = ent * widest;
   }
   return PB_OK;
 }
@@ -1406,7 +1387,7 @@ int pb_image_create(int device, uint32_t max_chunk, pb_image** out) {
 int pb_image_destroy(pb_image* im) {
   if (!im) return PB_OK;
   DeviceGuard g(im->device);
-  image_free(im, im->st);  // (after the inserts in flight on the load's stream)
+  im->own.release_all(im->st);  // (after the inserts in flight on the load's stream)
   cudaStreamSynchronize(im->st);
   delete im;
   return PB_OK;
@@ -1605,57 +1586,37 @@ int pb_ctx_create(int device, uint32_t max_occurrences, uint32_t max_out_rows, p
   if (!out || max_occurrences == 0 || max_out_rows == 0) return fail(PB_ERR_INVALID, "bad argument");
   if (max_occurrences > (1u << 24)) return fail(PB_ERR_INVALID, "at most 2^24 id occurrences per batch");
   DeviceGuard g(device);
-  pb_ctx* c = new pb_ctx();
+  std::unique_ptr<pb_ctx> c(new pb_ctx());
   c->device = device;
   c->max_occ = max_occurrences;
   c->max_out = max_out_rows;
   std::memset(c->round_of, 0, sizeof(c->round_of));
   const size_t n = max_occurrences;
   c->set_cells = 2 * n + 2 * PB_MAX_SLOTS;  // region of slot s: 2*n_s + 1 cells and the reserved one
-  cudaError_t e = cudaSuccess;
-  auto A = [&](void** p, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc(p, bytes);
-  };
-  A((void**)&c->b.set, sizeof(DCell) * c->set_cells);
-  A((void**)&c->b.occ_set, 4 * n);
-  A((void**)&c->b.item_cell, 4 * n);
-  A((void**)&c->b.seg_occ, 4 * n);
-  A((void**)&c->b.cold, 8 * n);
-  A((void**)&c->b.warm, 16 * (n / 2 + 1));
   c->b.giant_cap = n / PB_GIANT_MIN + 1;
   c->b.hot_cap = n / (PB_WARM_MAX + 1) + 1 + c->b.giant_cap;
-  A((void**)&c->b.hot, 16 * (size_t)c->b.hot_cap);
   c->b.hot_words = (uint32_t)(n < 4096 ? 4096 : n);  // 32 bits of pool per id occurrence the context can hold
-  A((void**)&c->b.hot_bits, 4 * (size_t)c->b.hot_words);
-  A((void**)&c->b.cnt, 4 * BC_COUNT);
-  A((void**)&c->occ_cell, 4 * n);
-  A((void**)&c->occ_outrow, 4 * n);
-  A((void**)&c->row_off, 4 * ((size_t)max_out_rows + 1));
-  A((void**)&c->nan_tick, 4 * PB_MAX_SLOTS);
-  A((void**)&c->dev_tick, 4);
-  A((void**)&c->need, 4 * PB_MAX_RANKS);
-  if (e == cudaSuccess) e = cudaMemset(c->need, 0, 4 * PB_MAX_RANKS);
-  if (e == cudaSuccess) e = cudaMemset(c->nan_tick, 0, 4 * PB_MAX_SLOTS);
-  if (e == cudaSuccess) e = cudaMemset(c->dev_tick, 0, 4);
-  if (e == cudaSuccess) e = cudaMemset(c->b.cnt, 0, 4 * BC_COUNT);
-  if (e == cudaSuccess) e = cudaMemset(c->b.hot_bits, 0, 4 * (size_t)c->b.hot_words);
-  if (e == cudaSuccess) {
-    launch_fill_set(c->b.set, c->set_cells, 0);
-    e = cudaDeviceSynchronize();
-  }
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->side2, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->side3, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_join2, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_nan, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
-  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_short, cudaEventDisableTiming);
-  if (e != cudaSuccess) {
-    pb_ctx_destroy(c);
-    return fail(PB_ERR_CUDA, std::string("pb_ctx_create: ") + cudaGetErrorString(e));
-  }
-  *out = c;
+  Owned& o = c->own;
+  int rc;
+  if ((rc = o.dev(c->b.set, sizeof(DCell) * c->set_cells)) || (rc = o.dev(c->b.occ_set, 4 * n)) ||
+      (rc = o.dev(c->b.item_cell, 4 * n)) || (rc = o.dev(c->b.seg_occ, 4 * n)) || (rc = o.dev(c->b.cold, 8 * n)) ||
+      (rc = o.dev(c->b.warm, 16 * (n / 2 + 1))) || (rc = o.dev(c->b.hot, 16 * (size_t)c->b.hot_cap)) ||
+      (rc = o.dev(c->b.hot_bits, 4 * (size_t)c->b.hot_words)) || (rc = o.dev(c->b.cnt, 4 * BC_COUNT)) ||
+      (rc = o.dev(c->occ_cell, 4 * n)) || (rc = o.dev(c->occ_outrow, 4 * n)) ||
+      (rc = o.dev(c->row_off, 4 * ((size_t)max_out_rows + 1))) || (rc = o.dev(c->nan_tick, 4 * PB_MAX_SLOTS)) ||
+      (rc = o.dev(c->dev_tick, 4)) || (rc = o.dev(c->need, 4 * PB_MAX_RANKS)))
+    return rc;
+  PB_CUDA(cudaMemset(c->need, 0, 4 * PB_MAX_RANKS));
+  PB_CUDA(cudaMemset(c->nan_tick, 0, 4 * PB_MAX_SLOTS));
+  PB_CUDA(cudaMemset(c->dev_tick, 0, 4));
+  PB_CUDA(cudaMemset(c->b.cnt, 0, 4 * BC_COUNT));
+  PB_CUDA(cudaMemset(c->b.hot_bits, 0, 4 * (size_t)c->b.hot_words));
+  launch_fill_set(c->b.set, c->set_cells, 0);
+  PB_CUDA(cudaDeviceSynchronize());
+  if ((rc = o.stream(c->side)) || (rc = o.stream(c->side2)) || (rc = o.stream(c->side3)) || (rc = o.event(c->ev_join2)) ||
+      (rc = o.event(c->ev_fork)) || (rc = o.event(c->ev_nan)) || (rc = o.event(c->ev_join)) || (rc = o.event(c->ev_short)))
+    return rc;
+  *out = c.release();
   return PB_OK;
 }
 
@@ -1665,20 +1626,6 @@ int pb_ctx_destroy(pb_ctx* c) {
   cudaDeviceSynchronize();
   c->pending.drop();
   c->raw_pending.drop();
-  void* ptrs[] = {c->b.set,   c->b.occ_set, c->b.item_cell, c->b.seg_occ, c->b.cold, c->b.warm, c->b.hot, c->b.hot_bits, c->b.cnt,
-                  c->occ_cell, c->occ_outrow, c->row_off, c->nan_tick, c->vw_stage, c->hot_stage, c->dev_tick, c->raw.set,
-                  c->raw.occ_set, c->raw.flag, c->raw.rank, c->raw.tiles, c->raw.distinct_cell, c->raw.counts, c->raw.target,
-                  c->raw.peer,    c->raw_stage, c->need,     c->remote_stage};
-  for (void* p : ptrs)
-    if (p) cudaFree(p);
-  if (c->side) cudaStreamDestroy(c->side);
-  if (c->side2) cudaStreamDestroy(c->side2);
-  if (c->side3) cudaStreamDestroy(c->side3);
-  if (c->ev_join2) cudaEventDestroy(c->ev_join2);
-  if (c->ev_fork) cudaEventDestroy(c->ev_fork);
-  if (c->ev_nan) cudaEventDestroy(c->ev_nan);
-  if (c->ev_join) cudaEventDestroy(c->ev_join);
-  if (c->ev_short) cudaEventDestroy(c->ev_short);
   delete c;
   return PB_OK;
 }
@@ -1723,26 +1670,25 @@ int pb_ctx_batch_stats(pb_ctx* c, uint32_t h_out[6], void* stream) {
   return PB_OK;
 }
 
-// A backward's staging buffer `buf` of `floats` floats, grown to hold `need`.  The training forward grows it, so the
-// backward that follows neither synchronises nor allocates (and can be captured without a warm-up call).  The first
+// A backward's staging buffer `buf` of `floats` floats, held by `own`, grown to hold `need`.  The training forward grows
+// it, so the backward that follows neither synchronises nor allocates (and can be captured without a warm-up call).  The first
 // allocation neither synchronises nor enqueues anything, so that a context's first forward can be captured too: the
 // thread's capture mode is relaxed around it (cudaMalloc is refused under a global-mode capture otherwise).  Growing
 // synchronises the stream and frees the old buffer: a forward captured with a larger need than any call before it fails
 // its capture, and a graph captured earlier must not be replayed after a larger call ran eagerly (warm up with the
 // largest batch, as for vw_stage).
-static int grow_stage(float*& buf, size_t& floats, size_t need, cudaStream_t st) {
+static int grow_stage(Owned& own, float*& buf, size_t& floats, size_t need, cudaStream_t st) {
   if (need <= floats) return PB_OK;
   if (buf) {  // the old buffer may still be read by enqueued work
     PB_CUDA(cudaStreamSynchronize(st));
-    cudaFree(buf);
-    buf = nullptr;
+    own.release(buf);
     floats = 0;
   }
   cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
   PB_CUDA(cudaThreadExchangeStreamCaptureMode(&mode));
-  const cudaError_t e = cudaMalloc(&buf, sizeof(float) * need);
+  const int rc = own.dev(buf, sizeof(float) * need);
   cudaThreadExchangeStreamCaptureMode(&mode);  // the caller's mode again
-  PB_CUDA(e);
+  if (rc) return rc;
   floats = need;
   return PB_OK;
 }
@@ -1765,7 +1711,7 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   if ((rc = call.begin(t, st, CALL_INDEX))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
   // pb_backward's staging of the hot items' sums, hot_cap x dim floats (a wider table grows it)
-  if (training && (rc = grow_stage(c->hot_stage, c->hot_stage_floats, (size_t)c->b.hot_cap * t->d.dim, st))) return rc;
+  if (training && (rc = grow_stage(c->own, c->hot_stage, c->hot_stage_floats, (size_t)c->b.hot_cap * t->d.dim, st))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
   if ((rc = begin_forward(t, c, sl, d_ids, n_occ, training, st))) return rc;
@@ -1814,15 +1760,7 @@ int pb_backward(pb_table* t, pb_ctx* c, const void* const* h_grads, int is_f16, 
   }
   float* vw = nullptr;
   if (t->op.kind == PB_OPT_ADAGRAD_VW) {
-    size_t need = (size_t)c->n_occ * t->d.dim;
-    if (need > c->vw_stage_floats) {
-      PB_CUDA(cudaStreamSynchronize(st));
-      if (c->vw_stage) cudaFree(c->vw_stage);
-      c->vw_stage = nullptr;
-      c->vw_stage_floats = 0;
-      PB_CUDA(cudaMalloc(&c->vw_stage, sizeof(float) * need));
-      c->vw_stage_floats = need;
-    }
+    if ((rc = grow_stage(c->own, c->vw_stage, c->vw_stage_floats, (size_t)c->n_occ * t->d.dim, st))) return rc;
     vw = c->vw_stage;
   }
   if ((size_t)c->b.hot_cap * t->d.dim > c->hot_stage_floats)
@@ -1903,6 +1841,7 @@ struct pb_xchg {
   // [PB_MAX_RANKS] signs of this rank's stage per owner (in `mem`, after the phase words)
   bool stage = false;
   uint32_t* sent = nullptr;
+  Owned own;  // mem, ucell, akeys, apresent, apow
 };
 
 namespace {
@@ -2030,7 +1969,7 @@ int pb_xchg_create(int device, uint32_t R, uint32_t rank, uint32_t cap, uint32_t
   for (uint32_t q = 0; q < R; ++q)
     if (!h_peer_base[q] || (h_peer_base[q] & 255u)) return fail(PB_ERR_INVALID, "receive areas must be mapped and 256-byte aligned");
   DeviceGuard g(device);
-  pb_xchg* x = new pb_xchg();
+  std::unique_ptr<pb_xchg> x(new pb_xchg());
   x->device = device;
   x->dim = dim;
   uint64_t off[6];
@@ -2048,20 +1987,16 @@ int pb_xchg_create(int device, uint32_t R, uint32_t rank, uint32_t cap, uint32_t
   d.cap = cap;
   d.row_f32 = rows_f32 ? 1 : 0;
   const size_t words = XC_WORDS + (size_t)XC_WORDS * PB_MAX_RANKS + PB_MAX_RANKS + 4 + 3 * (size_t)R * cap + 1;
-  cudaError_t e = cudaMalloc(&x->mem, 4 * words);
-  if (e == cudaSuccess) e = cudaMemset(x->mem, 0, 4 * words);
   uint32_t ucells = 1024;
   while ((size_t)ucells < 2 * (size_t)R * cap) ucells <<= 1;
-  if (e == cudaSuccess) e = cudaMalloc(&x->ucell, sizeof(UCell) * (size_t)ucells);
-  if (e == cudaSuccess) e = cudaMalloc(&x->akeys, sizeof(uint64_t) * PB_ADAM_KEYS);
-  if (e == cudaSuccess) e = cudaMalloc(&x->apresent, sizeof(uint32_t) * PB_MAX_RANKS * (PB_ADAM_KEYS / 32));
-  if (e == cudaSuccess) e = cudaMemset(x->apresent, 0, sizeof(uint32_t) * PB_MAX_RANKS * (PB_ADAM_KEYS / 32));
-  if (e == cudaSuccess) e = cudaMalloc(&x->apow, sizeof(float) * 2 * PB_MAX_RANKS * PB_ADAM_KEYS);
-
-  if (e != cudaSuccess) {
-    delete x;
-    return fail(PB_ERR_CUDA, std::string("pb_xchg_create: ") + cudaGetErrorString(e));
-  }
+  const size_t apresent_bytes = sizeof(uint32_t) * PB_MAX_RANKS * (PB_ADAM_KEYS / 32);
+  int rc;
+  if ((rc = x->own.dev(x->mem, 4 * words)) || (rc = x->own.dev(x->ucell, sizeof(UCell) * (size_t)ucells)) ||
+      (rc = x->own.dev(x->akeys, sizeof(uint64_t) * PB_ADAM_KEYS)) || (rc = x->own.dev(x->apresent, apresent_bytes)) ||
+      (rc = x->own.dev(x->apow, sizeof(float) * 2 * PB_MAX_RANKS * PB_ADAM_KEYS)))
+    return rc;
+  PB_CUDA(cudaMemset(x->mem, 0, 4 * words));
+  PB_CUDA(cudaMemset(x->apresent, 0, apresent_bytes));
   d.epoch = x->mem;
   d.waited = d.epoch + XC_WORDS;
   d.own_cnt = d.waited + (size_t)XC_WORDS * PB_MAX_RANKS;
@@ -2077,7 +2012,7 @@ int pb_xchg_create(int device, uint32_t R, uint32_t rank, uint32_t cap, uint32_t
   d.apow = x->apow;
   launch_uclear(d, nullptr);
   PB_CUDA(cudaDeviceSynchronize());
-  *out = x;
+  *out = x.release();
   return PB_OK;
 }
 
@@ -2085,11 +2020,6 @@ int pb_xchg_destroy(pb_xchg* x) {
   if (!x) return PB_OK;
   DeviceGuard g(x->device);
   cudaDeviceSynchronize();
-  if (x->mem) cudaFree(x->mem);
-  if (x->ucell) cudaFree(x->ucell);
-  if (x->akeys) cudaFree(x->akeys);
-  if (x->apresent) cudaFree(x->apresent);
-  if (x->apow) cudaFree(x->apow);
   delete x;
   return PB_OK;
 }
@@ -2108,7 +2038,7 @@ int pb_xchg_create_stage(int device, uint32_t R, uint32_t rank, uint32_t cap, co
   for (uint32_t q = 0; q < R; ++q)
     if (!h_peer_base[q] || (h_peer_base[q] & 255u)) return fail(PB_ERR_INVALID, "stage areas must be mapped and 256-byte aligned");
   DeviceGuard g(device);
-  pb_xchg* x = new pb_xchg();
+  std::unique_ptr<pb_xchg> x(new pb_xchg());
   x->device = device;
   x->stage = true;  // dim 0: no row, gradient or chain area, no ucell set, no Adam arrays
   uint64_t off[2];
@@ -2122,19 +2052,14 @@ int pb_xchg_create_stage(int device, uint32_t R, uint32_t rank, uint32_t cap, co
   d.rank = rank;
   d.cap = cap;
   const size_t words = XC_WORDS + (size_t)XC_WORDS * PB_MAX_RANKS + PB_MAX_RANKS + 4;  // epoch | waited | sent | err
-  cudaError_t e = cudaMalloc(&x->mem, 4 * words);
-  if (e == cudaSuccess) e = cudaMemset(x->mem, 0, 4 * words);
-  if (e == cudaSuccess) e = cudaDeviceSynchronize();
-  if (e != cudaSuccess) {
-    if (x->mem) cudaFree(x->mem);
-    delete x;
-    return fail(PB_ERR_CUDA, std::string("pb_xchg_create_stage: ") + cudaGetErrorString(e));
-  }
+  if (int rc = x->own.dev(x->mem, 4 * words)) return rc;
+  PB_CUDA(cudaMemset(x->mem, 0, 4 * words));
+  PB_CUDA(cudaDeviceSynchronize());
   d.epoch = x->mem;
   d.waited = d.epoch + XC_WORDS;
   x->sent = d.waited + (size_t)XC_WORDS * PB_MAX_RANKS;
   d.err = x->sent + PB_MAX_RANKS;
-  *out = x;
+  *out = x.release();
   return PB_OK;
 }
 
@@ -2284,21 +2209,21 @@ int pb_backward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const void* const* h
 // ---- raw slots ------------------------------------------------------------------------------------
 static int ensure_raw(pb_ctx* c) {
   if (c->raw_ready) return PB_OK;
-  RawWork& w = c->raw;
+  RawWork w = c->raw;
   size_t n = c->max_occ;
   size_t m = n > c->max_out ? n : c->max_out;
   uint32_t cells = next_pow2(2 * (uint64_t)n < 1024 ? 1024 : 2 * (uint64_t)n);
   w.set_mask = cells - 1;
-  PB_CUDA(cudaMalloc(&w.set, sizeof(RawCell) * ((size_t)cells + 1)));
-  PB_CUDA(cudaMalloc(&w.occ_set, 4 * n));
-  PB_CUDA(cudaMalloc(&w.flag, 4 * m));
-  PB_CUDA(cudaMalloc(&w.rank, 4 * m));
-  PB_CUDA(cudaMalloc(&w.tiles, 4 * (size_t)raw_scan_tiles((uint32_t)m)));
-  PB_CUDA(cudaMalloc(&w.distinct_cell, 4 * n));
-  PB_CUDA(cudaMalloc(&w.counts, 8));
+  Owned o;
+  int rc;
+  if ((rc = o.dev(w.set, sizeof(RawCell) * ((size_t)cells + 1))) || (rc = o.dev(w.occ_set, 4 * n)) ||
+      (rc = o.dev(w.flag, 4 * m)) || (rc = o.dev(w.rank, 4 * m)) ||
+      (rc = o.dev(w.tiles, 4 * (size_t)raw_scan_tiles((uint32_t)m))) || (rc = o.dev(w.distinct_cell, 4 * n)) ||
+      (rc = o.dev(w.counts, 8)) || (rc = o.dev(w.target, 4 * n)) || (rc = o.dev(w.peer, 4 * PB_MAX_RANKS)))
+    return rc;
   PB_CUDA(cudaMemset(w.counts, 0, 8));
-  PB_CUDA(cudaMalloc(&w.target, 4 * n));
-  PB_CUDA(cudaMalloc(&w.peer, 4 * PB_MAX_RANKS));
+  c->own.adopt(o);
+  c->raw = w;
   c->raw_ready = true;
   return PB_OK;
 }
@@ -2307,7 +2232,7 @@ static int ensure_raw(pb_ctx* c) {
 // by the batch, not by max_occ: a context made at twice a batch's ids (persia_core) would otherwise ask for twice the
 // staging, 64 GB at 2^24 occurrences and dim 1024.  It grows when a larger batch or dim comes.
 static int ensure_raw_stage(pb_ctx* c, uint32_t n_occ, uint32_t dim, cudaStream_t st) {
-  return grow_stage(c->raw_stage, c->raw_stage_floats, (size_t)(n_occ ? n_occ : 1) * dim, st);
+  return grow_stage(c->own, c->raw_stage, c->raw_stage_floats, (size_t)(n_occ ? n_occ : 1) * dim, st);
 }
 
 int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, const uint32_t* d_row_off,
@@ -2518,8 +2443,7 @@ struct pb_view {
   int device = 0;
   TableDev d{};
   uint32_t* seq = nullptr;
-  bool ipc = false;  // the pointers were opened with cudaIpcOpenMemHandle (closed by pb_view_close)
-  void* opened[VA_COUNT] = {};
+  Owned own;  // the IPC mappings of another process's table
 };
 
 namespace {
@@ -2551,7 +2475,7 @@ int begin_remote(pb_table* own, pb_ctx* c, RemoteDev& rv, uint32_t rank, size_t 
   if (int rc = ensure_alloc(own)) return rc;
   rv.t[rank] = own->d;
   rv.seq[rank] = own->seq;  // (null unless exported; a live table's training calls need not be ordered with this one)
-  return grow_stage(c->remote_stage, c->remote_stage_floats, floats ? floats : 1, st);
+  return grow_stage(c->own, c->remote_stage, c->remote_stage_floats, floats ? floats : 1, st);
 }
 }  // namespace
 
@@ -2571,9 +2495,13 @@ int export_blob(pb_table* t, void* h_blob, bool live) {
   DeviceGuard g(t->device);
   if (int rc = ensure_alloc(t)) return rc;
   if (!t->seq) {
-    PB_CUDA(cudaMalloc(&t->seq, sizeof(uint32_t)));
-    PB_CUDA(cudaMemset(t->seq, 0, sizeof(uint32_t)));
+    Owned o;
+    uint32_t* seq;
+    if (int rc = o.dev(seq, sizeof(uint32_t))) return rc;
+    PB_CUDA(cudaMemset(seq, 0, sizeof(uint32_t)));
     PB_CUDA(cudaDeviceSynchronize());
+    t->own.adopt(o);
+    t->seq = seq;
   }
   ViewBlob b;
   std::memset(&b, 0, sizeof(b));
@@ -2616,34 +2544,21 @@ int pb_view_open(int device, const void* h_blob, pb_view** out) {
   if (!b.n_cells || (b.n_cells & (b.n_cells - 1)) || !b.dim || b.stride < b.dim)
     return fail(PB_ERR_INVALID, "the view's table geometry is malformed");
   DeviceGuard g(device);
-  pb_view* v = new pb_view();
+  std::unique_ptr<pb_view> v(new pb_view());
   v->device = device;
   void* p[VA_COUNT];
   if (b.pid == (uint64_t)getpid() && b.nonce == process_nonce()) {  // CUDA IPC cannot open a handle in its own process: the pointers are valid here
     for (int i = 0; i < VA_COUNT; ++i) p[i] = reinterpret_cast<void*>(b.ptr[i]);
     if (b.device != device) {
       const cudaError_t e = cudaDeviceEnablePeerAccess(b.device, 0);
-      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) {
-        delete v;
+      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled)
         return fail(PB_ERR_CUDA, std::string("cudaDeviceEnablePeerAccess: ") + cudaGetErrorString(e));
-      }
       cudaGetLastError();
     }
   } else {
-    if (!b.ipc) {
-      delete v;
-      return fail(PB_ERR_STATE, "the exporting process could not make CUDA IPC handles for this table");
-    }
-    for (int i = 0; i < VA_COUNT; ++i) {
-      const cudaError_t e = cudaIpcOpenMemHandle(&p[i], b.handle[i], cudaIpcMemLazyEnablePeerAccess);
-      if (e != cudaSuccess) {
-        for (int k = 0; k < i; ++k) cudaIpcCloseMemHandle(v->opened[k]);
-        delete v;
-        return fail(PB_ERR_CUDA, std::string("cudaIpcOpenMemHandle: ") + cudaGetErrorString(e));
-      }
-      v->opened[i] = p[i];
-    }
-    v->ipc = true;
+    if (!b.ipc) return fail(PB_ERR_STATE, "the exporting process could not make CUDA IPC handles for this table");
+    for (int i = 0; i < VA_COUNT; ++i)
+      if (int rc = v->own.ipc(p[i], b.handle[i])) return rc;
   }
   TableDev& d = v->d;
   d.cells = static_cast<Cell*>(p[VA_CELLS]);
@@ -2657,7 +2572,7 @@ int pb_view_open(int device, const void* h_blob, pb_view** out) {
   d.stride = b.stride;
   d.state_floats = b.state_floats;
   v->seq = static_cast<uint32_t*>(p[VA_SEQ]);
-  *out = v;
+  *out = v.release();
   return PB_OK;
 }
 
@@ -2665,8 +2580,6 @@ int pb_view_close(pb_view* v) {
   if (!v) return PB_OK;
   DeviceGuard g(v->device);
   cudaDeviceSynchronize();  // (remote reads through it may still run)
-  if (v->ipc)
-    for (int i = 0; i < VA_COUNT; ++i) cudaIpcCloseMemHandle(v->opened[i]);
   delete v;
   return PB_OK;
 }
@@ -2737,3 +2650,12 @@ extern "C" int pb_debug_table_seq(pb_table* t, uint32_t* h_out) {
   PB_CUDA(cudaMemcpy(h_out, t->seq, sizeof(uint32_t), cudaMemcpyDeviceToHost));
   return PB_OK;
 }
+// testing aids (not in include/persia_b200.h): the resources every live object holds, [count, device + host bytes];
+// and a refusal: the (n+1)-th acquisition from now fails as if CUDA had refused it, before any CUDA call (-1: none)
+extern "C" int pb_debug_owned(uint64_t h_out[2]) {
+  if (!h_out) return fail(PB_ERR_INVALID, "null argument");
+  h_out[0] = g_owned_count.load();
+  h_out[1] = g_owned_bytes.load();
+  return PB_OK;
+}
+extern "C" void pb_debug_refuse_after(int64_t n) { g_refuse_after = n < 0 ? -1 : n; }

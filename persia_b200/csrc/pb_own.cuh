@@ -1,0 +1,154 @@
+// pb_own.cuh — the C ABI's error reporting and the CUDA resources its objects hold (included by pb_api.cu only).
+// Every buffer, mapped pinned host block, stream-ordered buffer, stream, event and IPC mapping an object acquires is
+// recorded in its Owned, which releases what is still held, in reverse order, when the object is deleted.  A step that
+// acquires several resources acquires them into a local Owned and adopts it once every part has succeeded, then sets
+// its gate: a step that fails leaves nothing allocated and no gate set, and the next call acquires afresh.
+#pragma once
+#include <atomic>
+#include <string>
+#include <vector>
+
+#include <cuda_runtime.h>
+
+#include "persia_b200.h"
+
+namespace {
+
+thread_local std::string g_err;
+
+int fail(int code, const std::string& msg) {
+  g_err = msg;
+  return code;
+}
+
+#define PB_CUDA(expr)                                                                              \
+  do {                                                                                             \
+    cudaError_t e__ = (expr);                                                                      \
+    if (e__ != cudaSuccess)                                                                        \
+      return fail(PB_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e__));               \
+  } while (0)
+
+// what every live object holds (pb_debug_owned), and the acquisitions still granted before one is refused
+// (pb_debug_refuse_after; -1: none is)
+std::atomic<uint64_t> g_owned_count{0}, g_owned_bytes{0};
+std::atomic<int64_t> g_refuse_after{-1};
+
+struct Owned {
+  enum Kind { DEV, HOST, ASYNC, STREAM, EVENT, IPC };
+  struct Res {
+    void* p;
+    Kind kind;
+    size_t bytes;
+    cudaStream_t st;  // ASYNC: the stream it was allocated on (the destructor frees it there)
+  };
+  std::vector<Res> held;
+
+  Owned() = default;
+  Owned(const Owned&) = delete;
+  Owned& operator=(const Owned&) = delete;
+  ~Owned() {
+    while (!held.empty()) drop(held.size() - 1, held.back().st);
+  }
+
+  template <typename T>
+  int dev(T*& p, size_t bytes) {
+    void* q = nullptr;
+    const cudaError_t e = refused() ? cudaErrorMemoryAllocation : cudaMalloc(&q, bytes);
+    return keep(e, "cudaMalloc", q, DEV, bytes, nullptr, p);
+  }
+  // pinned host memory mapped into the device's address space: `h` its host address, `d` its device address
+  template <typename T>
+  int mapped(T*& h, T*& d, size_t bytes) {
+    void *q = nullptr, *dq = nullptr;
+    cudaError_t e =
+        refused() ? cudaErrorMemoryAllocation : cudaHostAlloc(&q, bytes, cudaHostAllocMapped | cudaHostAllocPortable);
+    if (int rc = keep(e, "cudaHostAlloc", q, HOST, bytes, nullptr, q)) return rc;
+    if ((e = cudaHostGetDevicePointer(&dq, q, 0)) != cudaSuccess) {
+      release(q);
+      return fail(PB_ERR_CUDA, std::string("cudaHostGetDevicePointer: ") + cudaGetErrorString(e));
+    }
+    h = static_cast<T*>(q);
+    d = static_cast<T*>(dq);
+    return PB_OK;
+  }
+  // stream-ordered: allocated in `st`'s order
+  template <typename T>
+  int async(T*& p, size_t bytes, cudaStream_t st) {
+    void* q = nullptr;
+    const cudaError_t e = refused() ? cudaErrorMemoryAllocation : cudaMallocAsync(&q, bytes, st);
+    return keep(e, "cudaMallocAsync", q, ASYNC, bytes, st, p);
+  }
+  int stream(cudaStream_t& s) {
+    cudaStream_t q = nullptr;
+    const cudaError_t e = refused() ? cudaErrorMemoryAllocation : cudaStreamCreateWithFlags(&q, cudaStreamNonBlocking);
+    return keep(e, "cudaStreamCreateWithFlags", q, STREAM, 0, nullptr, s);
+  }
+  int event(cudaEvent_t& ev) {
+    cudaEvent_t q = nullptr;
+    const cudaError_t e = refused() ? cudaErrorMemoryAllocation : cudaEventCreateWithFlags(&q, cudaEventDisableTiming);
+    return keep(e, "cudaEventCreateWithFlags", q, EVENT, 0, nullptr, ev);
+  }
+  // another process's allocation, mapped into this one
+  int ipc(void*& p, const cudaIpcMemHandle_t& h) {
+    void* q = nullptr;
+    const cudaError_t e =
+        refused() ? cudaErrorMapBufferObjectFailed : cudaIpcOpenMemHandle(&q, h, cudaIpcMemLazyEnablePeerAccess);
+    return keep(e, "cudaIpcOpenMemHandle", q, IPC, 0, nullptr, p);
+  }
+
+  // Release one resource now and null the caller's pointer (null, or not held here: nothing is released).  A
+  // stream-ordered buffer is freed in `st`'s order.
+  template <typename T>
+  void release(T*& p, cudaStream_t st = nullptr) {
+    for (size_t i = held.size(); p && i--;)
+      if (held[i].p == static_cast<const void*>(p)) {
+        drop(i, st);
+        break;
+      }
+    p = nullptr;
+  }
+  // release everything, stream-ordered buffers in `st`'s order
+  void release_all(cudaStream_t st) {
+    while (!held.empty()) drop(held.size() - 1, st);
+  }
+  // take over what `o` holds (a step that has succeeded)
+  void adopt(Owned& o) {
+    held.insert(held.end(), o.held.begin(), o.held.end());
+    o.held.clear();
+  }
+
+ private:
+  // pb_debug_refuse_after: this acquisition is refused, before its CUDA call is made
+  static bool refused() {
+    int64_t n = g_refuse_after.load();
+    while (n >= 0 && !g_refuse_after.compare_exchange_weak(n, n - 1)) {
+    }
+    return n == 0;
+  }
+  // one acquisition's result (`e`, its CUDA call's or its refusal's): recorded and handed to `out` if it succeeded
+  template <typename P>
+  int keep(cudaError_t e, const char* what, void* q, Kind kind, size_t bytes, cudaStream_t st, P& out) {
+    if (e != cudaSuccess) return fail(PB_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+    held.push_back({q, kind, bytes, st});
+    g_owned_count += 1;
+    g_owned_bytes += bytes;
+    out = static_cast<P>(q);
+    return PB_OK;
+  }
+  void drop(size_t i, cudaStream_t st) {
+    const Res r = held[i];
+    held.erase(held.begin() + i);
+    switch (r.kind) {
+      case DEV: cudaFree(r.p); break;
+      case HOST: cudaFreeHost(r.p); break;
+      case ASYNC: cudaFreeAsync(r.p, st); break;
+      case STREAM: cudaStreamDestroy(static_cast<cudaStream_t>(r.p)); break;
+      case EVENT: cudaEventDestroy(static_cast<cudaEvent_t>(r.p)); break;
+      case IPC: cudaIpcCloseMemHandle(r.p); break;
+    }
+    g_owned_count -= 1;
+    g_owned_bytes -= r.bytes;
+  }
+};
+
+}  // namespace
