@@ -146,7 +146,8 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream);
  * number: the union evicts least recently used first, and pb_table_export_signs of both tables merges into the
  * reference's list order.
  * pb_table_clear of the table clears its tier too.  Destroy the table before its tier.  The sharded calls serve a
- * table with a tier on its owner rank by the same rules (see the R-GPU calls below); exporting it stays refused.
+ * table with a tier on its owner rank by the same rules (see the R-GPU calls below).  A table whose tier came from
+ * pb_table_create_host cannot be exported; one whose tier came from pb_table_create_host_shared can (below).
  *
  * Staging (pb_tier_stage): the ids of batch i+1 are known while batch i trains, and moving an entry never changes its
  * value, so the moves of request i+1 can run one batch ahead, on a stream of their own, beside batch i's dense step and
@@ -157,6 +158,13 @@ int pb_table_counters(pb_table* t, uint64_t h_out[5], void* stream);
  * capturing one; a call captured after a stage issued outside the capture that has not completed fails with
  * PB_ERR_STATE (synchronise before capturing). */
 int pb_table_create_host(int device, const pb_table_cfg* cfg, pb_table** out);
+/* A host tier whose rows another process can map: pb_table_create_host in every way but where the host rows come
+ * from.  They are an anonymous memfd (memfd_create; no named /dev/shm file, whose mount is often 64 MB in containers),
+ * ftruncate'd and mapped MAP_SHARED | MAP_POPULATE, then registered with cudaHostRegister(Mapped | Portable): not
+ * write-combined, like pb_table_create_host's.  A table with such a tier can be exported (pb_table_export_view,
+ * pb_table_export_live_view, then pb_table_export_tier_view), and its peers read the tier in place.  The memory is
+ * shmem: it is charged to the owning process's memory cgroup, and every peer that opens the tier pins it once more. */
+int pb_table_create_host_shared(int device, const pb_table_cfg* cfg, pb_table** out);
 /* Both tables need their optimizer registered; checks dim, optimizer kind and row stride. */
 int pb_table_attach_tier(pb_table* t, pb_table* tier);
 /* The tier behind `t` (zeros without one): [0] entries it holds, [1] entries moved out of HBM into it, [2] entries
@@ -566,7 +574,8 @@ int pb_tier_stage_sharded(pb_table* t, pb_xchg* xs, const uint64_t* d_ids, uint3
  * was before an insert or after it, never a mix, as the reference's entry lock gives.  A read that is still waiting
  * after the sharded calls' wait budget gives up and counts in the reader's pb_table_counters[4].
  * Ownership rule: the owner outlives every view of its table (destroy views first; a view of a destroyed table reads
- * freed memory).  A table with a host tier, and a tier, cannot be exported (no peer can reach the tier's rows). */
+ * freed memory).  A tier cannot be exported on its own, nor a table with a tier from pb_table_create_host (no peer can
+ * reach its rows).  A table with a shared tier (pb_table_create_host_shared) can: see "Shared tiers" below. */
 /* Bytes of a view blob (fixed: the exporting pid and a random number drawn once per process, the device pointers and CUDA IPC handles of the index cells, rows,
  * counters and write-sequence word, and the table's geometry). */
 uint64_t pb_table_view_bytes(void);
@@ -594,6 +603,38 @@ typedef struct pb_view pb_view;
  * are this process's (pids alone repeat across PID namespaces).  pb_view_close synchronises `device` and closes the handles. */
 int pb_view_open(int device, const void* h_blob, pb_view** out);
 int pb_view_close(pb_view* v);
+/* ---- Shared tiers: reading a tiered owner in place ------------------------------------------------------------------
+ * A table with a tier from pb_table_create_host_shared exports, frozen or live, a view blob of the same size and layout
+ * marked as tiered (version 2), which pb_view_open refuses (PB_ERR_STATE): a reader that ignored the tier would read
+ * zeros for every tier-held sign.  The tier's part is a second fixed-size blob, pb_table_export_tier_view's, written
+ * after the table's export: the exporting pid and random number, the device pointer and CUDA IPC handle of the tier's
+ * index cells, the memfd number and byte size of its rows, and its geometry (n_cells, capacity, stride).
+ * pb_view_open_tiered opens both: from this process it uses the pointers as they are; from another it opens the cells'
+ * handle, then /proc/<pid>/fd/<fd>, checks the size with fstat, maps it MAP_SHARED and registers it mapped (read-only,
+ * PROT_READ and cudaHostRegisterReadOnly, where the device supports it: a reader never writes the owner's rows).  Where that
+ * open fails (ranks in other PID namespaces or of other users, an owner that is not dumpable) it returns PB_ERR_STATE
+ * and says why.  pb_forward_remote and pb_forward_raw_remote then probe an owner's tier where its HBM index misses and
+ * read the hit from the host row (a kernel of its own, launched only when some owner has a tier): outputs stay bit for
+ * bit the sharded inference forwards', and only a sign neither table holds counts as a miss, on its owner.  `own` may
+ * have a shared tier too.
+ * Consistency: one write-sequence word covers a table and its tier.  Frozen: pb_set_rows (so pb_image_insert) holds it
+ * odd from before its restores to after its tier inserts.  Live: pb_table_clear holds it odd across the tier's clear
+ * too, and every launch that moves an entry between the two tables or hands a row of either to another sign runs
+ * inside a window of two added one-thread launches (k_seq_begin before it, k_seq_end after it): each eviction check
+ * (threshold, the tier's drop sweep, the move, both rebuilds); each restore (pb_forward, pb_forward_raw and pb_lookup
+ * training requests; an owner's SERVE of a training pb_forward_sharded / pb_forward_raw_sharded); pb_tier_stage's
+ * restores and pb_tier_stage_sharded's SERVE restores, each beside the window of the eviction check it runs.  So a
+ * live tiered training step adds 2 launches per restore it makes and 2 per eviction check it runs, and nothing else;
+ * untiered tables, tables with a private tier and tables not exported launch what they launched before.  Optimizer
+ * steps on tier-held rows stay outside the word: a read beside one sees each element before or after it, as for HBM
+ * rows. */
+/* Bytes of a tier blob (fixed). */
+uint64_t pb_tier_view_bytes(void);
+/* Writes the tier blob of t's shared tier (pb_tier_view_bytes() bytes).  t must have been exported (either way) first;
+ * a table without a tier, or with a tier from pb_table_create_host, and a tier itself: PB_ERR_STATE. */
+int pb_table_export_tier_view(pb_table* t, void* h_blob);
+/* pb_view_open for a tiered view blob and its tier blob (above).  Blobs of different exports: PB_ERR_INVALID. */
+int pb_view_open_tiered(int device, const void* h_blob, const void* h_tier_blob, pb_view** out);
 /* The inference form (training == 0) of pb_forward_sharded, served by this rank alone: arguments as pb_forward, plus
  * views[R] (owner q's table; views[rank] may be NULL: `own`, this rank's table, is probed directly), R and rank.  The
  * batch's distinct (slot, sign) items are read from their owners farmhash64(sign) % R into staging the context owns

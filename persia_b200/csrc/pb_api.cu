@@ -98,6 +98,9 @@ struct pb_table {
   // `tier` = the host table attached behind this one, `tier_of` = the table this one is attached behind
   bool host = false;
   float* host_rows = nullptr;  // host address of d.rows
+  // pb_table_create_host_shared: the host rows are a memfd mapping (`shared_fd`) that peer processes can map too
+  bool shared = false;
+  int shared_fd = -1;
   pb_table* tier = nullptr;
   pb_table* tier_of = nullptr;
   uint32_t* move_cells = nullptr;  // the eviction check's victim list (with rebuild_keys / rebuild_rows), `capacity` words
@@ -222,7 +225,9 @@ int acquire_storage(pb_table* t, Owned& o) {
   int rc;
   if ((rc = o.dev(d.cells, sizeof(Cell) * ((size_t)d.n_cells + N_SPECIAL))) ||
       // a host table's rows are not write-combined: the host reads them back (checkpoints)
-      (rc = t->host ? o.mapped(t->host_rows, d.rows, rows_bytes) : o.dev(d.rows, rows_bytes)) ||
+      (rc = t->shared ? o.shared(t->host_rows, d.rows, rows_bytes, -1, t->shared_fd)
+            : t->host ? o.mapped(t->host_rows, d.rows, rows_bytes)
+                      : o.dev(d.rows, rows_bytes)) ||
       (rc = o.dev(d.counters, sizeof(uint32_t) * CTR_COUNT)) || (rc = o.dev(d.row_tick, sizeof(uint32_t) * (size_t)d.capacity)))
     return rc;
   PB_CUDA(cudaMemset(d.row_tick, 0, sizeof(uint32_t) * (size_t)d.capacity));
@@ -274,6 +279,28 @@ int ensure_evict_ws(pb_table* t) {
 
 int wait_for(const Mark& m, cudaStream_t st);
 
+// A live-exported table with a host tier (a shared one: no other tier can be exported) holds its write-sequence word
+// odd around every launch that moves an entry between the table and its tier or hands a row of either to another sign
+// (the eviction check with its moves, sweeps and rebuilds; every restore): a reader that probed the HBM index before
+// such a move and the tier after it would otherwise find the sign in neither table (pb_remote.cu).  Two one-thread
+// launches (k_seq_begin, k_seq_end) around each; every other table launches nothing here.
+// The two kernels step the word with a plain read and +1, not atomically, so windows on one word must never overlap:
+// they are opened only by calls in the table's index chain (TableCall CALL_INDEX: training forwards, the sharded
+// SERVE, pb_set_rows, pb_table_clear, and the stages, which wait for every earlier call and which every later one but
+// a backward waits for), each on its call's stream, so every window is stream-ordered after the one before it.  The
+// backward (step chain only, beside a stage or the next forward) opens none.  A call outside the index chain must not
+// open one.
+struct TierWindow {
+  uint32_t* seq = nullptr;
+  cudaStream_t st = nullptr;
+  TierWindow(const pb_table* t, cudaStream_t s) : st(s) {
+    if (t->live && t->tier) launch_seq_bump(seq = t->seq, true, st);
+  }
+  ~TierWindow() {
+    if (seq) launch_seq_bump(seq, false, st);
+  }
+};
+
 // The eviction check: release the least recently used rows when free storage runs low, and rebuild the index when its
 // EMPTY cells run short.  blocks: grid of its scans (0 = the usual; pb_tier_stage's is small).
 int evict_check(pb_table* t, cudaStream_t st, uint32_t blocks = 0) {
@@ -287,6 +314,7 @@ int evict_check(pb_table* t, cudaStream_t st, uint32_t blocks = 0) {
   const uint32_t keep = t->evict_keep > t->pending_batches + 1 ? t->evict_keep : t->pending_batches + 1;
   if (t->tier) {  // the victims move into the tier
     pb_table* h = t->tier;
+    TierWindow win(t, st);
     launch_evict_tier(t->d, h->d, t->hy, t->op, t->evict_low, t->evict_target, keep, t->evict_ws, t->rebuild_keys,
                       t->rebuild_rows, h->evict_ws, h->rebuild_keys, h->rebuild_rows, t->move_cells, st, blocks);
     return PB_OK;
@@ -404,9 +432,11 @@ int read_counters(pb_table* t, const W* src, W* dst, size_t n, cudaStream_t st) 
   return PB_OK;
 }
 
-// signs the HBM table lacks and its tier holds are moved back into HBM rows before they are probed
+// a training request's signs the HBM table lacks and its tier holds are moved back into HBM rows before they are probed
 void restore_ids(pb_table* t, bool prefix, const SlotsDev& sl, const uint64_t* ids, uint32_t n, cudaStream_t st) {
-  if (t->tier) launch_tier_restore(t->d, t->tier->d, t->hy, t->op, sl, prefix, ids, n, st);
+  if (!t->tier) return;
+  TierWindow win(t, st);
+  launch_tier_restore(t->d, t->tier->d, t->hy, t->op, sl, prefix, ids, n, st);
 }
 
 // Calls that move index cells or step rows: refused once peers read the table in place (pb_table_export_view).
@@ -745,6 +775,13 @@ int pb_table_create_host(int device, const pb_table_cfg* cfg, pb_table** out) {
   return PB_OK;
 }
 
+int pb_table_create_host_shared(int device, const pb_table_cfg* cfg, pb_table** out) {
+  int rc = pb_table_create_host(device, cfg, out);
+  if (rc) return rc;
+  (*out)->shared = true;
+  return PB_OK;
+}
+
 int pb_table_attach_tier(pb_table* t, pb_table* tier) {
   if (!t || !tier) return fail(PB_ERR_INVALID, "null argument");
   if (int rc = writable(t)) return rc;  // (an exported table can have no tier: peers could not read its host rows)
@@ -818,6 +855,7 @@ int pb_tier_stage(pb_table* t, const uint64_t* d_ids, uint32_t n, const uint32_t
   // the check the request would run (not counted in train_calls, so the request's own stays where it was: after a
   // stage it usually finds enough free rows and does nothing); keep covers the batches pending now
   if (t->evict_every && (rc = evict_check(t, st, g_stage_blocks))) return rc;
+  TierWindow win(t, st);
   launch_tier_stage(t->d, t->tier->d, t->hy, t->op, sl, d_ids, n, g_stage_blocks, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
@@ -1013,12 +1051,14 @@ int pb_table_clear(pb_table* t, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
   if (int rc = call.begin(t, st, CALL_ALL)) return rc;
-  if (t->live) launch_seq_bump(t->seq, true, st);  // peers reading in place wait until every cell is EMPTY again
+  // peers reading in place wait until every cell of the table and of its tier is EMPTY again
+  if (t->live) launch_seq_bump(t->seq, true, st);
   launch_fill_cells(t->d.cells, (uint64_t)t->d.n_cells + N_SPECIAL, st);
   PB_CUDA(cudaMemsetAsync(t->d.counters, 0, sizeof(uint32_t) * CTR_COUNT, st));
   PB_CUDA(cudaMemsetAsync(t->d.row_tick, 0, sizeof(uint32_t) * (size_t)t->d.capacity, st));
+  const int rc = t->tier ? pb_table_clear(t->tier, stream) : PB_OK;
   if (t->live) launch_seq_bump(t->seq, false, st);
-  return t->tier ? pb_table_clear(t->tier, stream) : PB_OK;
+  return rc;
 }
 
 int pb_lookup(pb_table* t, const uint64_t* d_signs, uint32_t n, int training, float* d_out, void* stream) {
@@ -1093,17 +1133,18 @@ int pb_set_rows(pb_table* t, const uint64_t* d_signs, const float* d_entries, ui
   if (rc) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
   SlotsDev sl = no_slots();
-  // with a tier: a tier-held sign is first moved back (it then lives in one table), and an entry the HBM table has no
-  // row for goes to the tier
-  restore_ids(t, false, sl, d_signs, n, st);
   // an exported table, frozen or live: peers reading it in place see the write-sequence word odd from before the first
-  // cell it may claim to after the last entry it writes (pb_remote.cu), and read those items again
+  // cell it may claim (or, with a tier, the first entry it moves back) to after the last entry it writes (pb_remote.cu),
+  // and read those items again
   const bool bracket = t->exported || t->live;
   if (bracket) launch_seq_bump(t->seq, true, st);
+  // with a tier: a tier-held sign is first moved back (it then lives in one table), and an entry the HBM table has no
+  // row for goes to the tier
+  if (t->tier) launch_tier_restore(t->d, t->tier->d, t->hy, t->op, sl, false, d_signs, n, st);
   launch_probe(MODE_SET, false, t->d, t->hy, t->op, sl, d_signs, n, t->scratch, st);
   launch_copy_entries(true, t->d, t->scratch, n, const_cast<float*>(d_entries), nullptr, st);
-  if (bracket) launch_seq_bump(t->seq, false, st);
   if (t->tier) launch_tier_set(t->d, t->tier->d, t->hy, t->op, d_signs, t->scratch, n, d_entries, st);
+  if (bracket) launch_seq_bump(t->seq, false, st);
   PB_CUDA(cudaGetLastError());
   return PB_OK;
 }
@@ -1716,7 +1757,10 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
   if ((rc = begin_forward(t, c, sl, d_ids, n_occ, training, st))) return rc;
   // a training batch moves its tier-held signs into HBM rows (each distinct sign once); inference reads them in place
-  if (t->tier && training) launch_tier_restore_items(t->d, t->tier->d, t->hy, t->op, c->b, st);
+  if (t->tier && training) {
+    TierWindow win(t, st);
+    launch_tier_restore_items(t->d, t->tier->d, t->hy, t->op, c->b, st);
+  }
   launch_probe_items(training != 0, t->d, t->hy, t->op, sl, c->b, st);
   if (t->tier && !training) {
     launch_tier_find_items(t->d, t->tier->d, c->b, st);
@@ -1914,7 +1958,10 @@ int check_exchange(const pb_table* t, const pb_ctx* c, const pb_xchg* x, bool ne
 void serve_lookup(pb_table* t, pb_xchg* x, int training, const Phases& ph, cudaStream_t st) {
   ph.await(x, XC_FLAG_SIGN, st);
   if (training && x->u_dirty) launch_uclear(x->d, st);  // a training batch whose gradients never came left its rows noted
-  if (training && t->tier) launch_tier_restore_recv(t->d, t->tier->d, t->hy, t->op, x->d, st);
+  if (training && t->tier) {
+    TierWindow win(t, st);
+    launch_tier_restore_recv(t->d, t->tier->d, t->hy, t->op, x->d, st);
+  }
   launch_owner_lookup(training != 0, t->d, t->tier ? &t->tier->d : nullptr, t->hy, t->op, x->d, st);
   if (training) x->u_dirty = true;
   ph.post(x, XC_FLAG_ROW, nullptr, st);
@@ -2097,6 +2144,7 @@ int pb_tier_stage_sharded(pb_table* t, pb_xchg* xs, const uint64_t* d_ids, uint3
       // kernel reads index cells, the free-row stack or row_tick, and the rows they step are never victims here (keep >
       // pending_batches) nor restore targets (those come off the free stack).
       if (t->evict_every && (rc = evict_check(t, st, g_stage_blocks))) return rc;
+      TierWindow win(t, st);
       launch_tier_restore_recv(t->d, t->tier->d, t->hy, t->op, xs->d, st, g_stage_blocks);
     }
   }
@@ -2417,6 +2465,7 @@ namespace {
 // The bytes pb_table_export_view writes: what a peer needs to read the table in place.
 constexpr uint32_t VIEW_MAGIC = 0x57564250u;  // "PBVW"
 constexpr uint32_t VIEW_VERSION = 1;
+constexpr uint32_t VIEW_VERSION_TIERED = 2;  // the same layout, of a table with a shared tier: opened with its tier blob
 enum { VA_CELLS = 0, VA_ROWS, VA_COUNTERS, VA_SEQ, VA_COUNT };  // the allocations a reader touches
 struct ViewBlob {
   uint32_t magic, version;
@@ -2427,6 +2476,21 @@ struct ViewBlob {
   uint64_t ptr[VA_COUNT];                      // device pointers in the exporting process
   cudaIpcMemHandle_t handle[VA_COUNT];         // the same allocations for other processes
   uint32_t dim, stride, state_floats, n_cells, capacity, pad;
+};
+// The bytes pb_table_export_tier_view writes: the shared tier behind a table exported with version 2.
+constexpr uint32_t TIER_MAGIC = 0x54564250u;  // "PBVT"
+constexpr uint32_t TIER_VERSION = 1;
+struct TierBlob {
+  uint32_t magic, version;
+  uint64_t pid, nonce;             // the exporting process (as ViewBlob)
+  int32_t device;                  // its device ordinal, in the exporting process
+  uint32_t ipc;                    // 1: `handle` is valid
+  uint64_t cells, rows;            // device pointers of the tier's index cells and (mapped) rows, in the exporter
+  cudaIpcMemHandle_t handle;       // the index cells for other processes
+  int32_t fd;                      // the memfd of the rows in the exporting process (/proc/<pid>/fd/<fd>) ...
+  uint32_t pad0;
+  uint64_t bytes;                  // ... and its size: capacity x stride floats
+  uint32_t n_cells, capacity, stride, dim;
 };
 // A random number drawn once per process: a blob is this process's own only when both its pid and this number match.
 uint64_t process_nonce() {
@@ -2442,19 +2506,22 @@ uint64_t process_nonce() {
 struct pb_view {
   int device = 0;
   TableDev d{};
+  TableDev tier{};  // the owner's shared host tier (pb_view_open_tiered); cells null: none
   uint32_t* seq = nullptr;
-  Owned own;  // the IPC mappings of another process's table
+  Owned own;  // the IPC mappings of another process's table, and the mapping of its tier's rows
 };
 
 namespace {
 // The owners' tables of a remote read as this GPU reaches them: views[q] for q != rank, `own` itself for `rank`.
-int remote_views(pb_table* own, pb_view* const* views, uint32_t R, uint32_t rank, RemoteDev& rv) {
+// tiers[q]: owner q's shared host tier (cells null: none)
+int remote_views(pb_table* own, pb_view* const* views, uint32_t R, uint32_t rank, RemoteDev& rv, TableDev* tiers) {
   if (R == 0 || R > PB_MAX_RANKS || rank >= R) return fail(PB_ERR_INVALID, "need 1 <= R <= 16 and rank < R");
   if (R > 1 && !views) return fail(PB_ERR_INVALID, "null argument");
-  if (own->tier || own->host || own->tier_of)
+  if ((own->tier && !own->tier->shared) || own->host || own->tier_of)
     return fail(PB_ERR_STATE, "a table with a host tier serves one GPU only (no remote reads)");
   if (!own->has_op) return fail(PB_ERR_STATE, "optimizer not registered (OptimizerNotFoundError)");
   std::memset(&rv, 0, sizeof(rv));
+  std::memset(tiers, 0, sizeof(TableDev) * PB_MAX_RANKS);
   rv.R = R;
   for (uint32_t q = 0; q < R; ++q) {
     if (q == rank) continue;
@@ -2464,18 +2531,28 @@ int remote_views(pb_table* own, pb_view* const* views, uint32_t R, uint32_t rank
     if (v->d.dim != own->cfg.dim) return fail(PB_ERR_INVALID, "a view's table holds another embedding dim");
     rv.t[q] = v->d;
     rv.seq[q] = v->seq;
+    tiers[q] = v->tier;
   }
   return PB_OK;
 }
 
 // The start of a remote call, after its argument checks: `own` allocated and in its index chain, this rank's entry of
 // `rv`, and the staging of `floats` floats.
-int begin_remote(pb_table* own, pb_ctx* c, RemoteDev& rv, uint32_t rank, size_t floats, TableCall& call, cudaStream_t st) {
+int begin_remote(pb_table* own, pb_ctx* c, RemoteDev& rv, TableDev* tiers, uint32_t rank, size_t floats, TableCall& call,
+                 cudaStream_t st) {
   if (int rc = call.begin(own, st, CALL_INDEX)) return rc;
   if (int rc = ensure_alloc(own)) return rc;
   rv.t[rank] = own->d;
   rv.seq[rank] = own->seq;  // (null unless exported; a live table's training calls need not be ordered with this one)
+  if (own->tier) tiers[rank] = own->tier->d;
   return grow_stage(c->own, c->remote_stage, c->remote_stage_floats, floats ? floats : 1, st);
+}
+
+// the owners' tiers for launch_remote_lookup: null when no owner has one (the untiered kernels)
+const TableDev* any_tier(const TableDev* tiers, uint32_t R) {
+  for (uint32_t q = 0; q < R; ++q)
+    if (tiers[q].cells) return tiers;
+  return nullptr;
 }
 }  // namespace
 
@@ -2490,7 +2567,7 @@ int export_blob(pb_table* t, void* h_blob, bool live) {
                                    : "the table was exported live (pb_table_export_live_view): one table, one export mode");
   if (t->host || t->tier_of)
     return fail(PB_ERR_STATE, "a host tier cannot be exported: its rows are pinned host memory no peer process can map");
-  if (t->tier)
+  if (t->tier && !t->tier->shared)
     return fail(PB_ERR_STATE, "a table with a host tier cannot be exported: peers could not read its tier's rows");
   DeviceGuard g(t->device);
   if (int rc = ensure_alloc(t)) return rc;
@@ -2506,7 +2583,7 @@ int export_blob(pb_table* t, void* h_blob, bool live) {
   ViewBlob b;
   std::memset(&b, 0, sizeof(b));
   b.magic = VIEW_MAGIC;
-  b.version = VIEW_VERSION;
+  b.version = t->tier ? VIEW_VERSION_TIERED : VIEW_VERSION;
   b.pid = (uint64_t)getpid();
   b.nonce = process_nonce();
   b.device = t->device;
@@ -2536,19 +2613,80 @@ int pb_table_export_view(pb_table* t, void* h_blob) { return export_blob(t, h_bl
 
 int pb_table_export_live_view(pb_table* t, void* h_blob) { return export_blob(t, h_blob, true); }
 
-int pb_view_open(int device, const void* h_blob, pb_view** out) {
-  if (!h_blob || !out) return fail(PB_ERR_INVALID, "null argument");
+uint64_t pb_tier_view_bytes(void) { return sizeof(TierBlob); }
+
+int pb_table_export_tier_view(pb_table* t, void* h_blob) {
+  if (!t || !h_blob) return fail(PB_ERR_INVALID, "null argument");
+  if (t->host || t->tier_of)
+    return fail(PB_ERR_STATE, "a host tier cannot be exported: its rows are pinned host memory no peer process can map");
+  if (!t->tier) return fail(PB_ERR_STATE, "the table has no host tier");
+  if (!t->tier->shared)
+    return fail(PB_ERR_STATE, "a table with a host tier cannot be exported: peers could not read its tier's rows");
+  if (!t->exported && !t->live)
+    return fail(PB_ERR_STATE, "export the table first (pb_table_export_view or pb_table_export_live_view)");
+  const pb_table* h = t->tier;
+  TierBlob b;
+  std::memset(&b, 0, sizeof(b));
+  b.magic = TIER_MAGIC;
+  b.version = TIER_VERSION;
+  b.pid = (uint64_t)getpid();
+  b.nonce = process_nonce();
+  b.device = t->device;
+  b.cells = reinterpret_cast<uint64_t>(h->d.cells);
+  b.rows = reinterpret_cast<uint64_t>(h->d.rows);
+  DeviceGuard g(t->device);
+  b.ipc = cudaIpcGetMemHandle(&b.handle, h->d.cells) == cudaSuccess ? 1u : 0u;
+  if (!b.ipc) {
+    cudaGetLastError();  // (same-process views still work)
+    std::memset(&b.handle, 0, sizeof(b.handle));
+  }
+  b.fd = h->shared_fd;
+  b.bytes = sizeof(float) * (uint64_t)h->d.capacity * h->d.stride;
+  b.n_cells = h->d.n_cells;
+  b.capacity = h->d.capacity;
+  b.stride = h->d.stride;
+  b.dim = h->d.dim;
+  std::memcpy(h_blob, &b, sizeof(b));
+  return PB_OK;
+}
+
+namespace {
+// pb_view_open (tb = null) and pb_view_open_tiered: the table's view and, with tb, its shared tier
+int open_view(int device, const void* h_blob, const void* h_tier_blob, pb_view** out) {
   ViewBlob b;
   std::memcpy(&b, h_blob, sizeof(b));
-  if (b.magic != VIEW_MAGIC || b.version != VIEW_VERSION) return fail(PB_ERR_INVALID, "not a table view (pb_table_export_view)");
+  if (b.magic != VIEW_MAGIC || (b.version != VIEW_VERSION && b.version != VIEW_VERSION_TIERED))
+    return fail(PB_ERR_INVALID, "not a table view (pb_table_export_view)");
   if (!b.n_cells || (b.n_cells & (b.n_cells - 1)) || !b.dim || b.stride < b.dim)
     return fail(PB_ERR_INVALID, "the view's table geometry is malformed");
+  TierBlob tb;
+  if (h_tier_blob) {
+    std::memcpy(&tb, h_tier_blob, sizeof(tb));
+    if (tb.magic != TIER_MAGIC || tb.version != TIER_VERSION)
+      return fail(PB_ERR_INVALID, "not a tier view (pb_table_export_tier_view)");
+    if (!tb.n_cells || (tb.n_cells & (tb.n_cells - 1)) || tb.dim != b.dim || tb.stride != b.stride ||
+        tb.bytes != sizeof(float) * (uint64_t)tb.capacity * tb.stride)
+      return fail(PB_ERR_INVALID, "the tier view's geometry is malformed or not its table's");
+    if (tb.pid != b.pid || tb.nonce != b.nonce || tb.device != b.device)
+      return fail(PB_ERR_INVALID, "the tier view comes from another table's export");
+    if (b.version != VIEW_VERSION_TIERED)
+      return fail(PB_ERR_INVALID, "the table has no shared host tier: open it with pb_view_open");
+  } else if (b.version == VIEW_VERSION_TIERED) {
+    // (a reader that ignored the tier would read zeros for every tier-held sign)
+    return fail(PB_ERR_STATE, "the table has a shared host tier: open it with pb_view_open_tiered and its tier view "
+                              "(pb_table_export_tier_view)");
+  }
   DeviceGuard g(device);
   std::unique_ptr<pb_view> v(new pb_view());
   v->device = device;
   void* p[VA_COUNT];
+  void* tp[2] = {nullptr, nullptr};  // the tier's cells and rows
   if (b.pid == (uint64_t)getpid() && b.nonce == process_nonce()) {  // CUDA IPC cannot open a handle in its own process: the pointers are valid here
     for (int i = 0; i < VA_COUNT; ++i) p[i] = reinterpret_cast<void*>(b.ptr[i]);
+    if (h_tier_blob) {
+      tp[0] = reinterpret_cast<void*>(tb.cells);
+      tp[1] = reinterpret_cast<void*>(tb.rows);
+    }
     if (b.device != device) {
       const cudaError_t e = cudaDeviceEnablePeerAccess(b.device, 0);
       if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled)
@@ -2556,9 +2694,29 @@ int pb_view_open(int device, const void* h_blob, pb_view** out) {
       cudaGetLastError();
     }
   } else {
-    if (!b.ipc) return fail(PB_ERR_STATE, "the exporting process could not make CUDA IPC handles for this table");
+    if (!b.ipc || (h_tier_blob && !tb.ipc))
+      return fail(PB_ERR_STATE, "the exporting process could not make CUDA IPC handles for this table");
     for (int i = 0; i < VA_COUNT; ++i)
       if (int rc = v->own.ipc(p[i], b.handle[i])) return rc;
+    if (h_tier_blob) {
+      if (int rc = v->own.ipc(tp[0], tb.handle)) return rc;
+      // the tier's rows: the exporter's memfd, reached through /proc (one user, one PID namespace, a dumpable owner)
+      // read-only where the device can register read-only host memory: a reader never writes the owner's rows
+      int ro = 0;
+      if (cudaDeviceGetAttribute(&ro, cudaDevAttrHostRegisterReadOnlySupported, device) != cudaSuccess) {
+        cudaGetLastError();
+        ro = 0;
+      }
+      const std::string path = "/proc/" + std::to_string(tb.pid) + "/fd/" + std::to_string(tb.fd);
+      const int fd = open(path.c_str(), (ro ? O_RDONLY : O_RDWR) | O_CLOEXEC);
+      if (fd < 0)
+        return fail(PB_ERR_STATE, "cannot open the exporting process's shared tier (" + path + ": " + strerror(errno) +
+                                      "): its ranks must run as one user in one PID namespace, and it must be dumpable");
+      float *h = nullptr, *dr = nullptr;
+      int kept = -1;
+      if (int rc = v->own.shared(h, dr, tb.bytes, fd, kept, ro != 0)) return rc;
+      tp[1] = dr;
+    }
   }
   TableDev& d = v->d;
   d.cells = static_cast<Cell*>(p[VA_CELLS]);
@@ -2571,9 +2729,32 @@ int pb_view_open(int device, const void* h_blob, pb_view** out) {
   d.dim = b.dim;
   d.stride = b.stride;
   d.state_floats = b.state_floats;
+  if (h_tier_blob) {  // (a find touches only cells and rows)
+    TableDev& h = v->tier;
+    h.cells = static_cast<Cell*>(tp[0]);
+    h.rows = static_cast<float*>(tp[1]);
+    h.n_cells = tb.n_cells;
+    h.cell_mask = tb.n_cells - 1;
+    h.bucket_mask = tb.n_cells / BUCKET - 1;
+    h.capacity = tb.capacity;
+    h.dim = tb.dim;
+    h.stride = tb.stride;
+    h.state_floats = b.state_floats;
+  }
   v->seq = static_cast<uint32_t*>(p[VA_SEQ]);
   *out = v.release();
   return PB_OK;
+}
+}  // namespace
+
+int pb_view_open(int device, const void* h_blob, pb_view** out) {
+  if (!h_blob || !out) return fail(PB_ERR_INVALID, "null argument");
+  return open_view(device, h_blob, nullptr, out);
+}
+
+int pb_view_open_tiered(int device, const void* h_blob, const void* h_tier_blob, pb_view** out) {
+  if (!h_blob || !h_tier_blob || !out) return fail(PB_ERR_INVALID, "null argument");
+  return open_view(device, h_blob, h_tier_blob, out);
 }
 
 int pb_view_close(pb_view* v) {
@@ -2589,18 +2770,20 @@ int pb_forward_remote(pb_table* own, pb_view* const* views, uint32_t R, uint32_t
                       void* d_out_f16, void* stream) {
   int rc = check_forward(own, c, d_ids, n_occ, d_row_off, h_slot_occ_off, batch, d_out_f16);
   RemoteDev rv;
-  if (rc || (rc = remote_views(own, views, R, rank, rv))) return rc;
+  TableDev tiers[PB_MAX_RANKS];
+  if (rc || (rc = remote_views(own, views, R, rank, rv, tiers))) return rc;
   const uint64_t n_out = (uint64_t)c->slots.n_slots * batch;
   const bool row_f32 = d_row_off != nullptr;  // ragged layouts pool f32 rows, as on an exchange of f32 rows
   DeviceGuard g(own->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
   const size_t elems = (size_t)n_occ * own->cfg.dim;  // at most one row per id occurrence
-  if ((rc = begin_remote(own, c, rv, rank, row_f32 ? elems : (elems + 1) / 2, call, st))) return rc;
+  if ((rc = begin_remote(own, c, rv, tiers, rank, row_f32 ? elems : (elems + 1) / 2, call, st))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
   if ((rc = begin_forward(own, c, sl, d_ids, n_occ, 0, st))) return rc;  // the dedup (an inference request)
-  launch_remote_lookup(false, row_f32, rv, c->b, c->raw, n_occ, c->remote_stage, own->d.dim, own->d.counters + CTR_ERR, st);
+  launch_remote_lookup(false, row_f32, rv, any_tier(tiers, R), c->b, c->raw, n_occ, c->remote_stage, own->d.dim,
+                       own->d.counters + CTR_ERR, st);
   launch_expand_items(own->d, sl, c->b, c->remote_stage, row_f32, d_row_off, (uint32_t)n_out, batch, false, d_out_f16, st);
   if ((rc = end_forward(own, c, d_row_off, h_slot_occ_off, n_occ, batch, 0, st))) return rc;
   PB_CUDA(cudaGetLastError());
@@ -2614,11 +2797,12 @@ int pb_forward_raw_remote(pb_table* own, pb_view* const* views, uint32_t R, uint
   int rc = check_raw_forward(own, c, d_ids, n_occ, d_row_off, batch, sample_fixed_size, d_table_f16, d_index, d_non_empty,
                              d_sample_id_num, d_counts);
   RemoteDev rv;
-  if (rc || (rc = remote_views(own, views, R, rank, rv))) return rc;
+  TableDev tiers[PB_MAX_RANKS];
+  if (rc || (rc = remote_views(own, views, R, rank, rv, tiers))) return rc;
   DeviceGuard g(own->device);
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
-  if ((rc = begin_remote(own, c, rv, rank, (size_t)n_occ * own->cfg.dim, call, st))) return rc;
+  if ((rc = begin_remote(own, c, rv, tiers, rank, (size_t)n_occ * own->cfg.dim, call, st))) return rc;
   if ((rc = ensure_raw(c))) return rc;
   SlotsDev sl;
   if ((rc = raw_slots(c, n_occ, sl))) return rc;
@@ -2628,7 +2812,8 @@ int pb_forward_raw_remote(pb_table* own, pb_view* const* views, uint32_t R, uint
   launch_raw_number(sl, d_ids, n_occ, d_row_off ? c->row_off : nullptr, d_row_off ? c->occ_outrow : nullptr, batch,
                     sample_fixed_size, nullptr, c->raw, (long long*)d_index, (long long*)d_non_empty, d_sample_id_num, st);
   PB_CUDA(cudaMemcpyAsync(d_counts, c->raw.counts, 8, cudaMemcpyDeviceToDevice, st));
-  launch_remote_lookup(true, true, rv, c->b, c->raw, n_occ, c->remote_stage, own->d.dim, own->d.counters + CTR_ERR, st);
+  launch_remote_lookup(true, true, rv, any_tier(tiers, R), c->b, c->raw, n_occ, c->remote_stage, own->d.dim,
+                       own->d.counters + CTR_ERR, st);
   launch_raw_fill(c->raw, n_occ, own->d.dim, c->remote_stage, d_table_f16, st);  // row u + 1 = f16(row), rounded once
   PB_CUDA(cudaGetLastError());
   return PB_OK;

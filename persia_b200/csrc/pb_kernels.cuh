@@ -132,6 +132,11 @@ struct RemoteDev {
   const uint32_t* seq[PB_MAX_RANKS];
   uint32_t R;
 };
+// k_remote_lookup<TIER>'s argument: the owners' tables and each owner's shared host tier (cells null: none)
+struct RemoteTierDev {
+  RemoteDev rv;
+  TableDev tier[PB_MAX_RANKS];
+};
 
 // arguments of the backward kernels (pb_reduce.cu)
 struct ReduceArgs {
@@ -278,8 +283,9 @@ void launch_count_owners(bool raw, const BatchDev& b, const RawWork& w, uint32_t
 // pb_remote.cu: the distinct items of the context's batch (raw: its numbered distinct signs) read from their owners into
 // `stage` at the item's number, f16(0 + row) or f32 rows (raw: f32), targets set to the item's number; err counts the
 // items whose read gave up (n: worst-case U)
-void launch_remote_lookup(bool raw, bool row_f32, const RemoteDev& rv, const BatchDev& b, const RawWork& w, uint32_t n,
-                          void* stage, uint32_t dim, uint32_t* err, cudaStream_t st);
+// tiers: the owners' host tiers (null: no owner has one, and the untiered kernels run)
+void launch_remote_lookup(bool raw, bool row_f32, const RemoteDev& rv, const TableDev* tiers, const BatchDev& b,
+                          const RawWork& w, uint32_t n, void* stage, uint32_t dim, uint32_t* err, cudaStream_t st);
 // an exported table's write-sequence word: odd from `begin` to the end of the writes that follow
 void launch_seq_bump(uint32_t* seq, bool begin, cudaStream_t st);
 // pb_shard.cu, raw slot over R shards: requester's route, table fill and gradient send (n: worst-case U)

@@ -1,12 +1,20 @@
 // pb_own.cuh — the C ABI's error reporting and the CUDA resources its objects hold (included by pb_api.cu only).
-// Every buffer, mapped pinned host block, stream-ordered buffer, stream, event and IPC mapping an object acquires is
+// Every buffer, mapped pinned host block, shared host mapping, stream-ordered buffer, stream, event and IPC mapping an
+// object acquires is
 // recorded in its Owned, which releases what is still held, in reverse order, when the object is deleted.  A step that
 // acquires several resources acquires them into a local Owned and adopts it once every part has succeeded, then sets
 // its gate: a step that fails leaves nothing allocated and no gate set, and the next call acquires afresh.
 #pragma once
 #include <atomic>
+#include <cerrno>
+#include <cstring>
 #include <string>
 #include <vector>
+
+#include <fcntl.h>
+#include <sys/mman.h>
+#include <sys/stat.h>
+#include <unistd.h>
 
 #include <cuda_runtime.h>
 
@@ -34,12 +42,13 @@ std::atomic<uint64_t> g_owned_count{0}, g_owned_bytes{0};
 std::atomic<int64_t> g_refuse_after{-1};
 
 struct Owned {
-  enum Kind { DEV, HOST, ASYNC, STREAM, EVENT, IPC };
+  enum Kind { DEV, HOST, ASYNC, STREAM, EVENT, IPC, SHARED };
   struct Res {
     void* p;
     Kind kind;
     size_t bytes;
     cudaStream_t st;  // ASYNC: the stream it was allocated on (the destructor frees it there)
+    int fd = -1;      // SHARED: the file the mapping is of
   };
   std::vector<Res> held;
 
@@ -69,6 +78,52 @@ struct Owned {
     }
     h = static_cast<T*>(q);
     d = static_cast<T*>(dq);
+    return PB_OK;
+  }
+  // Host memory another process can map (pb_table_create_host_shared): `fd` < 0, a new anonymous memfd of `bytes`;
+  // else `fd` itself (a peer's, opened through /proc), whose size must be `bytes`.  The file is mapped MAP_SHARED
+  // (populated, not write-combined) and registered mapped into the device's address space: `h` its host address, `d`
+  // its device address, `fd_out` the descriptor.  read_only (a peer's, where the device can register read-only memory):
+  // mapped PROT_READ and registered cudaHostRegisterReadOnly, so that no stray write of a reader reaches the owner's
+  // rows (`fd` then needs no write access).  Released as unregister, unmap, close; a failed step undoes the ones before
+  // it, and a given `fd` is closed on failure too.
+  template <typename T>
+  int shared(T*& h, T*& d, size_t bytes, int fd, int& fd_out, bool read_only = false) {
+    if (refused()) {
+      if (fd >= 0) close(fd);
+      return fail(PB_ERR_CUDA, "shared host mapping: refused");
+    }
+    const bool created = fd < 0;
+    if (created && (fd = memfd_create("persia_b200_tier", MFD_CLOEXEC)) < 0)
+      return fail(PB_ERR_CUDA, std::string("memfd_create: ") + strerror(errno));
+    struct stat sb;
+    const char* what = nullptr;
+    errno = 0;
+    if (created && ftruncate(fd, (off_t)bytes) != 0) what = "ftruncate";
+    else if (!created && (fstat(fd, &sb) != 0 || (size_t)sb.st_size != bytes)) what = "the shared tier's size";
+    void* q = MAP_FAILED;
+    const int prot = read_only ? PROT_READ : PROT_READ | PROT_WRITE;
+    if (!what && (q = mmap(nullptr, bytes, prot, MAP_SHARED | MAP_POPULATE, fd, 0)) == MAP_FAILED) what = "mmap";
+    if (what) {
+      const std::string msg = std::string(what) + ": " + (errno ? strerror(errno) : "mismatch");
+      close(fd);
+      return fail(PB_ERR_STATE, msg);
+    }
+    cudaError_t e = cudaHostRegister(q, bytes, cudaHostRegisterMapped | cudaHostRegisterPortable |
+                                                   (read_only ? cudaHostRegisterReadOnly : 0u));
+    void* dq = nullptr;
+    if (e == cudaSuccess && (e = cudaHostGetDevicePointer(&dq, q, 0)) != cudaSuccess) cudaHostUnregister(q);
+    if (e != cudaSuccess) {
+      munmap(q, bytes);
+      close(fd);
+      return fail(PB_ERR_CUDA, std::string("cudaHostRegister: ") + cudaGetErrorString(e));
+    }
+    held.push_back({q, SHARED, bytes, nullptr, fd});
+    g_owned_count += 1;
+    g_owned_bytes += bytes;
+    h = static_cast<T*>(q);
+    d = static_cast<T*>(dq);
+    fd_out = fd;
     return PB_OK;
   }
   // stream-ordered: allocated in `st`'s order
@@ -129,7 +184,7 @@ struct Owned {
   template <typename P>
   int keep(cudaError_t e, const char* what, void* q, Kind kind, size_t bytes, cudaStream_t st, P& out) {
     if (e != cudaSuccess) return fail(PB_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-    held.push_back({q, kind, bytes, st});
+    held.push_back({q, kind, bytes, st, -1});
     g_owned_count += 1;
     g_owned_bytes += bytes;
     out = static_cast<P>(q);
@@ -145,6 +200,11 @@ struct Owned {
       case STREAM: cudaStreamDestroy(static_cast<cudaStream_t>(r.p)); break;
       case EVENT: cudaEventDestroy(static_cast<cudaEvent_t>(r.p)); break;
       case IPC: cudaIpcCloseMemHandle(r.p); break;
+      case SHARED:
+        cudaHostUnregister(r.p);
+        munmap(r.p, r.bytes);
+        close(r.fd);
+        break;
     }
     g_owned_count -= 1;
     g_owned_bytes -= r.bytes;

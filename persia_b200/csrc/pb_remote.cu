@@ -15,8 +15,24 @@
 // clear runs.  A lane group reads it before its probe and copy and again after them; while it is odd, or if it
 // changed, the item is read again.  A returned row is therefore the entry before an insert or after it, never a mix.
 // A row still ROW_PENDING in the index is an insert in flight: the word has moved, so it is read again as well.
+//
+// An owner with a shared host tier (pb_table_create_host_shared, pb_view_open_tiered): k_remote_lookup<TIER> probes the
+// tier's index (HBM, through the view) where the owner's HBM probe misses, and reads a hit from the tier's host row (the
+// owner's memfd, mapped into this process and registered with CUDA).  One word covers the table and its tier: the owner
+// holds it odd around every launch that moves an entry between the two or hands a row of either to another sign
+// (pb_api.cu, TierWindow), so a reader never finds a moving sign in neither table, and a tier-held row read between two
+// equal even words is that sign's whole row.  The loads between the two reads of the word are the same for both tables:
+// the word is read with ld.acquire.sys (no later load of this thread is performed before it), the index and row loads
+// are plain weak ld.global.cg (whether the row sits in peer HBM over NVLink or in host memory over PCIe: the PTX memory
+// model orders by address, not by where the address lives), and fence.acq_rel.sys orders every one of them before the
+// second ld.acquire.sys.  The owner's side is the converse: its k_seq_begin store is followed by fence.sc.sys
+// (__threadfence_system) before the kernels that write cells or rows, and k_seq_end puts one between them and its store.
+// At .sys scope those fences and the reader's acquire/fence pair synchronise, whichever GPU or PCIe path carries the
+// data: a reader that reads the same even word twice read no row written inside a window.
 #include "pb_device.cuh"
 #include "pb_probe.cuh"
+
+#include <type_traits>
 
 namespace pb {
 
@@ -32,11 +48,18 @@ __device__ __forceinline__ uint32_t seq_acquire(const uint32_t* p) {
 // the loads of a probe and copy complete before the word is read again (the seqlock reader's read barrier)
 __device__ __forceinline__ void fence_acq_rel_sys() { asm volatile("fence.acq_rel.sys;" ::: "memory"); }
 
+__device__ __forceinline__ const RemoteDev& remote_of(const RemoteDev& a) { return a; }
+__device__ __forceinline__ const RemoteDev& remote_of(const RemoteTierDev& a) { return a.rv; }
+template <bool TIER>
+using RemoteArg = typename std::conditional<TIER, RemoteTierDev, RemoteDev>::type;
+
 // One lane group (BUCKET lanes) per distinct item; the grid strides over the items.  Must be called by whole warps.
-template <bool RAW, bool ROW_F32>
-__global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteDev rv, BatchDev b, RawWork w,
+// TIER: a miss in the owner's HBM index is probed again in the owner's host tier (a.tier[owner]; cells null: it has none).
+template <bool RAW, bool ROW_F32, bool TIER>
+__global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteArg<TIER> a, BatchDev b, RawWork w,
                                                                          void* __restrict__ stage, uint32_t dim,
                                                                          uint32_t* __restrict__ err) {
+  const RemoteDev& rv = remote_of(a);
   const uint32_t sub = threadIdx.x % BUCKET;
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t gshift = lane & ~(BUCKET - 1);
@@ -73,20 +96,33 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteDe
       const uint32_t s0_lead = __shfl_sync(0xffffffffu, s0, gshift);
       const bool go = todo && !(s0_lead & 1u);  // odd: an insert is running on the owner
       const ProbeOut r = probe_group<MODE_FIND>(t, hy, op, sign, go, 0u, sub, gshift);
+      // k_owner_lookup_tier's choice: the HBM row, else the tier row, else zeros
+      const float* src = t.rows;
+      uint32_t src_row = r.row, src_cap = t.capacity, src_stride = t.stride;
+      if constexpr (TIER) {
+        const TableDev& h = a.tier[owner];
+        const ProbeOut tr = probe_group<MODE_FIND>(h, hy, op, sign, go && r.row >= t.capacity && h.cells, 0u, sub, gshift);
+        if (r.row >= t.capacity && h.cells) {
+          src = h.rows;
+          src_row = tr.row;
+          src_cap = h.capacity;
+          src_stride = h.stride;
+        }
+      }
+      const bool have = src_row < src_cap;
       if (go) {
         // k_owner_lookup's conversion: f16(0 + row) for one-id layouts, the f32 row for ragged ones (zeros on a miss)
-        const bool have = r.row < t.capacity;
-        const float* row = t.rows + (size_t)(have ? r.row : 0u) * t.stride;
+        const float* row = src + (size_t)(have ? src_row : 0u) * src_stride;
         if (dim % 4 == 0) {
           for (uint32_t e = sub * 4; e < dim; e += BUCKET * 4) {
             const float4 v = have ? __ldcg(reinterpret_cast<const float4*>(row + e)) : make_float4(0.f, 0.f, 0.f, 0.f);
             if (ROW_F32) {
               *reinterpret_cast<float4*>(static_cast<float*>(stage) + (size_t)u * dim + e) = v;
             } else {
-              __half2 a = __floats2half2_rn(__fadd_rn(0.0f, v.x), __fadd_rn(0.0f, v.y));
+              __half2 a2 = __floats2half2_rn(__fadd_rn(0.0f, v.x), __fadd_rn(0.0f, v.y));
               __half2 c = __floats2half2_rn(__fadd_rn(0.0f, v.z), __fadd_rn(0.0f, v.w));
               uint2 pk;
-              pk.x = *reinterpret_cast<uint32_t*>(&a);
+              pk.x = *reinterpret_cast<uint32_t*>(&a2);
               pk.y = *reinterpret_cast<uint32_t*>(&c);
               *reinterpret_cast<uint2*>(static_cast<__half*>(stage) + (size_t)u * dim + e) = pk;
             }
@@ -108,7 +144,7 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteDe
       const uint32_t same = __ballot_sync(0xffffffffu, !go || (s0 == s0_lead && s1 == s0_lead));
       if (go && ((same >> gshift) & 0xFFu) == 0xFFu) {  // the item read whole by every lane, between two inserts
         if (sub == 0) {
-          if (r.row >= t.capacity) atomicAdd_system(&t.counters[CTR_MISS], 1u);  // counted on its owner, as there
+          if (!have) atomicAdd_system(&t.counters[CTR_MISS], 1u);  // counted on its owner, as there
           if (RAW) w.target[u] = u;
           else b.set[cell].target = u;
         }
@@ -125,15 +161,24 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteDe
   }
 }
 
-void launch_remote_lookup(bool raw, bool row_f32, const RemoteDev& rv, const BatchDev& b, const RawWork& w, uint32_t n,
-                          void* stage, uint32_t dim, uint32_t* err, cudaStream_t st) {
+void launch_remote_lookup(bool raw, bool row_f32, const RemoteDev& rv, const TableDev* tiers, const BatchDev& b,
+                          const RawWork& w, uint32_t n, void* stage, uint32_t dim, uint32_t* err, cudaStream_t st) {
   if (!n) return;
   const uint32_t full = cdiv((uint64_t)n * BUCKET, 256);  // worst case: every id a distinct item
   const uint32_t grid = full < PB_NUM_SMS * PB_PROBE_BLOCKS ? full : PB_NUM_SMS * PB_PROBE_BLOCKS;
-#define PB_R(RW, F32) PB_LAUNCH_F(FAM_PROBE, (k_remote_lookup<RW, F32>), grid, 256, 0, st, rv, b, w, stage, dim, err)
-  if (raw) PB_R(true, true);
-  else if (row_f32) PB_R(false, true);
-  else PB_R(false, false);
+#define PB_R(RW, F32, TR, A) PB_LAUNCH_F(FAM_PROBE, (k_remote_lookup<RW, F32, TR>), grid, 256, 0, st, A, b, w, stage, dim, err)
+  if (tiers) {
+    RemoteTierDev a;
+    a.rv = rv;
+    for (uint32_t q = 0; q < PB_MAX_RANKS; ++q) a.tier[q] = tiers[q];
+    if (raw) PB_R(true, true, true, a);
+    else if (row_f32) PB_R(false, true, true, a);
+    else PB_R(false, false, true, a);
+  } else {
+    if (raw) PB_R(true, true, false, rv);
+    else if (row_f32) PB_R(false, true, false, rv);
+    else PB_R(false, false, false, rv);
+  }
 #undef PB_R
 }
 

@@ -59,6 +59,7 @@ SYMBOLS = {
     "pb_table_counters": (_i32, [_vp, C.POINTER(_u64 * 5), _vp]),
     "pb_table_index_stats": (_i32, [_vp, C.POINTER(_u64 * 3), _vp]),
     "pb_table_create_host": (_i32, [_i32, C.POINTER(TableCfg), C.POINTER(_vp)]),
+    "pb_table_create_host_shared": (_i32, [_i32, C.POINTER(TableCfg), C.POINTER(_vp)]),
     "pb_table_attach_tier": (_i32, [_vp, _vp]),
     "pb_tier_stats": (_i32, [_vp, C.POINTER(_u64 * 5), _vp]),
     "pb_tier_stage": (_i32, [_vp, _vp, _u32, C.POINTER(_u32), C.POINTER(_u64), _u32, _u32, _vp]),
@@ -116,6 +117,9 @@ SYMBOLS = {
     "pb_table_export_live_view": (_i32, [_vp, _vp]),
     "pb_view_open": (_i32, [_i32, _vp, C.POINTER(_vp)]),
     "pb_view_close": (_i32, [_vp]),
+    "pb_tier_view_bytes": (_u64, []),
+    "pb_table_export_tier_view": (_i32, [_vp, _vp]),
+    "pb_view_open_tiered": (_i32, [_i32, _vp, _vp, C.POINTER(_vp)]),
     "pb_forward_remote": (_i32, [_vp, C.POINTER(_vp), _u32, _u32, _vp, _vp, _u32, _vp, C.POINTER(_u32), _u32, _vp, _vp]),
     "pb_forward_raw_remote": (_i32, [_vp, C.POINTER(_vp), _u32, _u32, _vp, _vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp,
                                      _vp, _vp]),

@@ -26,6 +26,15 @@ At `replica_size > 1` every forward that does not train is served by its rank al
 (_start_remote, _Remote): no collective.  An Infer job exports its tables frozen once its checkpoint is
 loaded; a Train job exports them live when its optimizer is registered, and its training forwards and backwards stay
 collective.
+
+Host tiers (PERSIA_B200_HBM_ROWS: a table larger than that keeps the rest of `capacity` in host memory behind each
+rank's HBM rows) serve one GPU only unless PERSIA_B200_SHARED_TIER=1.  With it set, every dim group's shard is created
+with a shared tier (pb_table_create_host_shared) at any replica_size, and at replica_size > 1 both exports carry it: an
+Infer job's frozen one (checkpoint loads and incremental packets included) and a Train job's live one, so a forward that
+does not train reads tier-held signs from their owners' host rows in place.  It is an opt-in because shared host memory
+costs more than private pinned memory: it is shmem charged to the owning rank's memory cgroup, every peer that reads
+it pins it again, and the ranks must run as one user in one PID namespace (a peer maps the owner's memfd through
+/proc/<pid>/fd).  Tier staging (worker.TierStager) stays off at replica_size > 1.
 """
 import os
 import queue
@@ -83,10 +92,12 @@ def parse_embedding_config(cfg):
     return bits, slots
 
 
-def hbm_split(capacity, hbm_rows, replica_size=1):
+def hbm_split(capacity, hbm_rows, replica_size=1, shared=False):
     """(rows in HBM, rows of the host-memory tier behind them) of a table of `capacity` entries.  hbm_rows
     (PERSIA_B200_HBM_ROWS; None or "" = unset): a table larger than that keeps the rest in host memory, moved in and out
-    by the kernels (include/persia_b200.h, pb_table_attach_tier); unset or >= capacity: everything in HBM, no tier."""
+    by the kernels (include/persia_b200.h, pb_table_attach_tier); unset or >= capacity: everything in HBM, no tier.
+    At replica_size > 1 a tier needs `shared` (PERSIA_B200_SHARED_TIER=1): its rows are then shared memory the peers'
+    remote reads map (pb_table_create_host_shared)."""
     capacity = int(capacity)
     if hbm_rows is None or str(hbm_rows).strip() == "":
         return capacity, 0
@@ -95,10 +106,15 @@ def hbm_split(capacity, hbm_rows, replica_size=1):
         raise RuntimeError(f"PERSIA_B200_HBM_ROWS must be positive, got {hbm_rows}")
     if hbm_rows >= capacity:
         return capacity, 0
-    if (replica_size or 1) > 1:
+    if (replica_size or 1) > 1 and not shared:
         raise RuntimeError("PERSIA_B200_HBM_ROWS (a host-memory tier behind the HBM rows) is supported on one GPU only "
                            f"(replica_size = 1, got {replica_size}): unset it or raise it to the capacity ({capacity})")
     return hbm_rows, capacity - hbm_rows
+
+
+def shared_tier_on():
+    """PERSIA_B200_SHARED_TIER=1: host tiers are created in shared memory (see the module docstring)."""
+    return os.environ.get("PERSIA_B200_SHARED_TIER", "").strip() == "1"
 
 
 class _State:
@@ -203,8 +219,9 @@ class _State:
             from . import shard as SH
 
             dev = self.device_id if self.device_id is not None else 0
-            hbm, tier = hbm_split(self.capacity, os.environ.get("PERSIA_B200_HBM_ROWS"), self.replica_size)
-            sh = SH.EmbeddingShard(dim, hbm, dev, tier_rows=tier)
+            shared = shared_tier_on()
+            hbm, tier = hbm_split(self.capacity, os.environ.get("PERSIA_B200_HBM_ROWS"), self.replica_size, shared=shared)
+            sh = SH.EmbeddingShard(dim, hbm, dev, tier_rows=tier, shared_tier=shared)
             sh.set_eviction()  # the reference's holder is an LRU map bounded by `capacity` (eviction_map.rs:76-97)
             if self.optimizer is not None:
                 sh.set_optimizer(**self.optimizer)
@@ -1163,7 +1180,8 @@ def _stage(batch):
     batch's training forward will need (pb_tier_stage) are issued now, while the batches before it still train: the
     signs of the group's summation slots (hash-stacked as _to_device_ids does) and raw slots, on a stream the group owns,
     under the group's lock.  Results do not change; the forward finds its entries in HBM.  Nothing runs for tables
-    without a tier, inference batches, or on R GPUs (no tier there)."""
+    without a tier, inference batches, or on R GPUs (there a shared tier is not staged: on virtual ranks staging did not
+    shorten a step, and it waits for a measurement on R real GPUs)."""
     import torch
 
     from .native import PB_MAX_SLOTS

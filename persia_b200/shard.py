@@ -148,20 +148,24 @@ class StreamMark:
 
 
 class EmbeddingShard:
-    def __init__(self, dim, capacity, device=0, tier_rows=0, host=False):
+    def __init__(self, dim, capacity, device=0, tier_rows=0, host=False, shared_tier=False):
         """capacity: rows in HBM.  tier_rows > 0: a host-memory tier of that many rows behind them (include/persia_b200.h,
         pb_table_attach_tier), attached once the optimizer is registered.  host: this table's rows live in host memory
-        (the tier itself)."""
+        (the tier itself).  shared_tier: the tier's rows are shared memory other processes can map
+        (pb_table_create_host_shared), so that the table can be exported and its peers read the tier in place."""
         self.lib = N.load()
         self.dim, self.capacity = int(dim), int(capacity)
         self.device = torch.device("cuda", device) if not isinstance(device, torch.device) else device
         h = C.c_void_p()
         cfg = N.TableCfg(self.dim, self.capacity)
-        create = self.lib.pb_table_create_host if host else self.lib.pb_table_create
+        create = self.lib.pb_table_create
+        if host:
+            create = self.lib.pb_table_create_host_shared if shared_tier else self.lib.pb_table_create_host
         N.check(create(self.device.index or 0, C.byref(cfg), C.byref(h)))
         self.h = h
         self._entry_len = None
-        self.host_tier = EmbeddingShard(dim, tier_rows, device, host=True) if tier_rows else None
+        self.shared_tier = bool(shared_tier and tier_rows)
+        self.host_tier = EmbeddingShard(dim, tier_rows, device, host=True, shared_tier=shared_tier) if tier_rows else None
         self._tier_attached = False
         # R GPUs (worker.TierStager): the sharded forwards of this shard's workers, keyed by worker, and its stager's
         # last stage.  A stage waits for the forwards before it; a forward waits for the stage before it.
@@ -371,20 +375,26 @@ class EmbeddingShard:
 
     def export_view(self):
         """The table's view blob (bytes) for peers that read it in place (pb_table_export_view).  From now on the table
-        is read-only but for set_entries and checkpoint / packet inserts, and it must outlive every view of it."""
-        buf = C.create_string_buffer(int(self.lib.pb_table_view_bytes()))
-        N.check(self.lib.pb_table_export_view(self.h, buf))
-        return buf.raw
+        is read-only but for set_entries and checkpoint / packet inserts, and it must outlive every view of it.  With a
+        shared tier the tier's blob follows the table's in the same bytes (pb_table_export_tier_view)."""
+        return self._export(self.lib.pb_table_export_view)
 
     def export_live_view(self):
         """The table's view blob (bytes) for peers that read it in place while it keeps training
         (pb_table_export_live_view): the blob export_view gives, read by the same TableView and RemoteReader, but the
-        table stays writable.  Sweeps, index rebuilds, set_entries and clear are bracketed for the readers; a read beside
-        an optimizer step may see each element before or after it.  One table, one export mode; the table must outlive
-        every view of it."""
+        table stays writable.  Sweeps, index rebuilds, set_entries and clear are bracketed for the readers (with a shared
+        tier, every move between the table and its tier too); a read beside an optimizer step may see each element before
+        or after it.  One table, one export mode; the table must outlive every view of it."""
+        return self._export(self.lib.pb_table_export_live_view)
+
+    def _export(self, call):
         buf = C.create_string_buffer(int(self.lib.pb_table_view_bytes()))
-        N.check(self.lib.pb_table_export_live_view(self.h, buf))
-        return buf.raw
+        N.check(call(self.h, buf))
+        if not self.shared_tier:
+            return buf.raw
+        tier = C.create_string_buffer(int(self.lib.pb_tier_view_bytes()))
+        N.check(self.lib.pb_table_export_tier_view(self.h, tier))
+        return buf.raw + tier.raw
 
     def close(self):
         if getattr(self, "h", None):
@@ -402,15 +412,20 @@ class EmbeddingShard:
 
 class TableView:
     """Another rank's exported table as this process reads it on `device` (pb_view_open / pb_view_close): through CUDA
-    IPC when the blob comes from another process, through its own pointers when from this one."""
+    IPC when the blob comes from another process, through its own pointers when from this one.  A blob of a table with a
+    shared tier opens both (pb_view_open_tiered; from another process the tier's rows are mapped through /proc)."""
 
     def __init__(self, blob, device=0):
         self.lib = N.load()
         self.device = torch.device("cuda", device) if not isinstance(device, torch.device) else device
         blob = bytes(blob)
-        assert len(blob) == int(self.lib.pb_table_view_bytes()), "not a table view blob"
+        n = int(self.lib.pb_table_view_bytes())
         h = C.c_void_p()
-        N.check(self.lib.pb_view_open(self.device.index or 0, blob, C.byref(h)))
+        if len(blob) == n + int(self.lib.pb_tier_view_bytes()):  # a table with a shared tier: its blob, then the tier's
+            N.check(self.lib.pb_view_open_tiered(self.device.index or 0, blob[:n], blob[n:], C.byref(h)))
+        else:
+            assert len(blob) == n, "not a table view blob"
+            N.check(self.lib.pb_view_open(self.device.index or 0, blob, C.byref(h)))
         self.h = h
 
     def close(self):
