@@ -998,12 +998,12 @@ class _Unit:
         self.ids, self.row_off, self.slot_off = _flatten(feats, B)
 
     def device_ids(self, dev):
-        """(device ids, device CSR offsets or None, slot offsets, host CSR offsets or None), hash stack applied."""
+        """(device ids, device CSR offsets or None, slot offsets), hash stack applied."""
         import torch
 
         d_ids, row_off, slot_off = _to_device_ids(self.ids, self.row_off, self.slot_off, self.slots, self.B, dev)
         d_off = torch.from_numpy(row_off.view(np.int32)).to(dev, non_blocking=True) if row_off is not None else None
-        return d_ids, d_off, slot_off, row_off
+        return d_ids, d_off, slot_off
 
 
 def _units(feats, B):
@@ -1031,7 +1031,7 @@ class _Local:
         from . import shard as SH
 
         u = self.u
-        ids, off, slot_off, _ = u.device_ids(self.dev)
+        ids, off, slot_off = u.device_ids(self.dev)
         n, rows = int(ids.numel()), len(u.names) * u.B
         pool = u.g["ctx"].setdefault(u.key, [])
         if pool and n <= pool[-1]._size[0] and rows <= pool[-1]._size[1]:
@@ -1069,13 +1069,12 @@ class _ShardedPart:
         if u.k == 0 and not u.raw and g.setdefault("names", u.dim_names) != u.dim_names:
             raise RuntimeError("on R GPUs every batch must carry the same summation slots of a dim, in the same order")
         with g["lock"]:
-            self.ids, self.off, self.slot_off, row_off = u.device_ids(dev)
+            self.ids, self.off, self.slot_off = u.device_ids(dev)
+            self.wk = _worker(u, dev)
             if u.raw:
-                self.wk = _sharded_raw_worker(u, row_off, dev)
                 self.need = self.wk.prepare_raw(self.ids, u.B, u.slots[0].sample_fixed_size, row_off=self.off,
                                                 training=training)
             else:
-                self.wk = _sharded_worker(u, self.ids, row_off, self.slot_off, dev)
                 self.need = self.wk.prepare(self.ids, u.B, row_off=self.off, slot_occ_off=self.slot_off,
                                             training=training)
 
@@ -1110,10 +1109,10 @@ class _Remote:
     def forward(self, training):
         u = self.u
         if u.raw:
-            ids, off, _, _ = self.raw_ids
+            ids, off, _ = self.raw_ids
             return self.rd.forward_raw(ids, u.B, u.slots[0].sample_fixed_size, u.prefixes[0], _S.prefix_bit,
                                        row_off=off)
-        ids, off, slot_off, _ = u.device_ids(self.dev)
+        ids, off, slot_off = u.device_ids(self.dev)
         return self.rd.forward(ids, u.B, u.prefixes, u.sqrt, _S.prefix_bit, row_off=off, slot_occ_off=slot_off)
 
     def release(self):
@@ -1138,7 +1137,7 @@ def _sharded_step(units, training, dev):
     """R GPUs: sizes this step's exchanges from its own batch, agreed by every rank before any rank sends.  Every unit's
     worker is prepared (its batch context grown if need be, the batch deduplicated: local work) in the collective
     order (_units), and then _agree_and_resize sizes them all with one all-reduce.  Returns the units' placements
-    (_ShardedPart).  PERSIA_B200_XCHG_CAP and PERSIA_B200_MAX_BATCH size a worker's first exchange and context only."""
+    (_ShardedPart)."""
     parts = [_ShardedPart(u, training, dev) for u in units]
     _agree_and_resize([(p.u.g, p.wk, p.need) for p in parts], dev)
     return parts
@@ -1231,74 +1230,28 @@ def _stage(batch):
                                      _S.prefix_bit)
 
 
-def _sharded_worker(u, d_ids, row_off, slot_off, dev):
-    """The ShardedEmbeddingWorker (persia_b200/worker.py) of summation unit u (chunk u.k of its dim group), created by
-    the first batch: a collective — every rank's first lookup of the group must happen in the same step (it does: the
-    ranks train in lockstep).  All chunks of a dim serve the rank's one table.  d_ids, row_off, slot_off: u.device_ids."""
-    workers = u.g.setdefault("workers", [])
-    if u.k < len(workers):
-        return workers[u.k]
+def _worker(u, dev):
+    """Unit u's worker (persia_b200/worker.py) over the rank's table of its dim: a ShardedRawWorker for a raw slot
+    (g["raw_workers"], by slot name), a ShardedEmbeddingWorker for a summation chunk (g["workers"], by chunk u.k).  The
+    first batch that carries the unit creates it: a collective — every rank's first lookup of the unit must happen in
+    the same step (it does: the ranks train in lockstep).  It starts with the smallest exchange and context; its first
+    prepare grows the context (ctx_size) and _agree_and_resize sizes the exchange, as they do at every later step."""
+    workers = u.g.setdefault("raw_workers" if u.raw else "workers", {})
+    key = u.names[0] if u.raw else u.k
+    if key in workers:
+        return workers[key]
     import torch.distributed as dist
 
-    from .worker import ShardedEmbeddingWorker as W
+    from .worker import ShardedEmbeddingWorker, ShardedRawWorker
 
     if not dist.is_initialized():
         raise RuntimeError("replica_size > 1 needs torch.distributed (TrainCtx initialises it; else call init_process_group)")
-    # the exchange is sized from this first batch's keys: hash-stacked ones are read back from the device
-    ids = d_ids.cpu().numpy().view(np.uint64) if any(sc.hash_stack_rounds > 0 for sc in u.slots) else u.ids
-    cap = _exchange_cap([(ids[slot_off[i]:slot_off[i + 1]], sc.index_prefix) for i, sc in enumerate(u.slots)], dev)
-    ragged, B = row_off is not None, u.B
-    per_sample = max(1, -(-len(ids) // max(1, len(u.names) * B)))
-    max_batch = int(os.environ.get("PERSIA_B200_MAX_BATCH", B))
-    # the group's table is the rank's shard: raw workers of this dim serve it too
-    wk = W.distributed(len(u.names), u.dim, u.prefixes, _S.capacity, cap, _S.optimizer or {}, dev, hyper=_S.hyper,
-                       max_batch=max(B, max_batch), sqrt_scaling=u.sqrt, rows_f32=ragged, prefix_bit=_S.prefix_bit,
-                       max_ids_per_sample=2 * per_sample if ragged else 1, shard=u.g["shard"])
-    workers.append(wk)
-    return wk
-
-
-def _sharded_raw_worker(u, row_off, dev):
-    """Raw unit u's ShardedRawWorker (persia_b200/worker.py) over the rank's table of its dim, created by the first
-    batch that carries the slot: a collective, like _sharded_worker.  row_off: the host CSR offsets or None."""
-    (sc,), g, B, ids = u.slots, u.g, u.B, u.ids
-    wk = g.setdefault("raw_workers", {}).get(sc.name)
-    if wk is not None:
-        return wk
-    import torch.distributed as dist
-
-    from .worker import ShardedRawWorker
-
-    if not dist.is_initialized():
-        raise RuntimeError("replica_size > 1 needs torch.distributed (TrainCtx initialises it; else call init_process_group)")
-    cap = _exchange_cap([(ids, sc.index_prefix)], dev)
-    ragged = row_off is not None
-    per_sample = max(1, -(-len(ids) // max(1, B)))
-    max_batch = int(os.environ.get("PERSIA_B200_MAX_BATCH", B))
-    wk = ShardedRawWorker.distributed(1, sc.dim, [sc.index_prefix], _S.capacity, cap, _S.optimizer or {}, dev,
-                                      hyper=_S.hyper, max_batch=max(B, max_batch, 1), prefix_bit=_S.prefix_bit,
-                                      max_ids_per_sample=2 * per_sample if ragged else 1, shard=g["shard"])
-    g["raw_workers"][sc.name] = wk
-    return wk
-
-
-def _exchange_cap(slot_ids, dev):
-    """Slots per (source, owner) pair of a new exchange: PERSIA_B200_XCHG_CAP, else from this first batch — the
-    distinct signs it requests of one owner, largest over the ranks (a collective), with a generous margin.
-    slot_ids: [(flat ids of one slot, its index_prefix)]."""
-    import torch
-    import torch.distributed as dist
-
-    from .worker import distinct_per_owner
-
-    cap = int(os.environ.get("PERSIA_B200_XCHG_CAP", 0))
-    if cap:
-        return cap
-    ids, prefixes = zip(*slot_ids)
-    counts = distinct_per_owner(ids, prefixes, dist.get_world_size(), _S.prefix_bit)
-    t = torch.tensor([int(counts.max())], dtype=torch.int64, device=dev)
-    dist.all_reduce(t, op=dist.ReduceOp.MAX)
-    return (int(int(t) * 1.5) + 1024 + 7) // 8 * 8
+    cls = ShardedRawWorker if u.raw else ShardedEmbeddingWorker
+    # the group's table is the rank's shard: every worker of the dim serves it
+    workers[key] = cls.distributed(len(u.names), u.dim, u.prefixes, _S.capacity, 8, _S.optimizer or {}, dev,
+                                   hyper=_S.hyper, max_batch=1, sqrt_scaling=u.sqrt, prefix_bit=_S.prefix_bit,
+                                   shard=u.g["shard"])
+    return workers[key]
 
 
 class PersiaTrainingBatch:  # forward.rs:256-306, #[pyclass(dict)]: python attaches attributes to it

@@ -176,13 +176,23 @@ def one_rank():
 def test_r_gpu_placements_on_one_rank(oracle, one_rank):
     """Training batches take the collective workers and the lookup that does not train takes the remote readers, with
     two dims, a ragged slot, a hash-stacked slot, two slots of one feature group and a raw slot (one gradient skipped).
-    Outputs and entries equal the oracle's with one parameter server."""
+    Outputs and entries equal the oracle's with one parameter server.  Every worker starts at cap 8, and its first
+    step's agreement gives it the cap its own prepared need grows to."""
     import torch
     import torch.utils.dlpack as dl
 
+    from persia_b200.worker import ShardedEmbeddingWorker as W
     from util import to_dev_ids
 
     impl, pc, ctx = _surface(PATH_CFG, replica_size=2)
+    agree, first = impl._agree_and_resize, []  # first: the first step's (worker, its prepare's (need, rows_f32))
+
+    def record(plan, dev):
+        if not first:
+            first.extend((wk, need) for _, wk, need in plan)
+        return agree(plan, dev)
+
+    impl._agree_and_resize = record
     try:
         _register(pc, ctx)  # (the process group is up: the tables are exported live here)
         S = impl._S
@@ -257,6 +267,10 @@ def test_r_gpu_placements_on_one_rank(oracle, one_rank):
                 w_raw.backward_raw(0, rctx, None, skip=True)
             else:
                 w_raw.backward_raw(0, rctx, grad.cpu().numpy(), scale=scale)
+            if step == 0:  # the raw slot, the dim-16 chunk (with the hash-stacked slot) and the dim-32 chunk
+                assert sorted((wk.dim, wk.S) for wk, _ in first) == [(16, 3), (32, 1), (32, 2)]
+                for wk, (need, f32) in first:
+                    assert need > 8 and (wk.cap, wk.rows_f32) == (W.grown_cap(need, 8), f32), (wk.dim, wk.S, need)
         torch.cuda.synchronize()
         # the path the training batches took: the collective workers, no pooled context
         for d in (16, 32):
@@ -297,4 +311,5 @@ def test_r_gpu_placements_on_one_rank(oracle, one_rank):
         held = wi != 0  # the row at every index position, whatever numbering either side chose
         assert table[index[held]].tobytes() == wt[wi[held]].tobytes()
     finally:
+        impl._agree_and_resize = agree
         impl.reset()

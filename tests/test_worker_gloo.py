@@ -105,8 +105,8 @@ def test_sharded_protocol_equals_oracle_requests_in_rank_order(R):
     assert n > 100
 
 
-def _exchange_cap_counts(slot_ids, R, prefix_bit):
-    """The per-owner count persia_core._exchange_cap made inline before it called distinct_per_owner."""
+def _owner_counts(slot_ids, R, prefix_bit):
+    """The per-owner count written out in numpy: each slot's distinct prefixed signs, bucketed by farmhash64 % R."""
     from persia_b200.persia_core import farmhash64_np
 
     counts = np.zeros(R, np.int64)
@@ -136,42 +136,7 @@ def test_distinct_per_owner_ragged_slots(oracle, R, prefix_bit):
         for owner in oracle.shard_of(np.unique(oracle.add_prefix(x, prefix_bit, p)), R):
             want[owner] += 1
     assert got.tolist() == want.tolist() and want.sum() > 500
-    assert got.tolist() == _exchange_cap_counts(list(zip(slot_ids, pf)), R, prefix_bit).tolist()
-
-
-def _ragged_slots(rank):
-    rng = np.random.default_rng(5 + rank)
-    return [rng.integers(0, c, size=n, dtype=np.uint64) for n, c in zip([300 * (rank + 1), 0, 40], [2**64 - 1, 9, 25])]
-
-
-def _run_exchange_cap(rank, port, q, R, pf, prefix_bit):
-    from persia_b200 import persia_core as pc
-
-    dist.init_process_group("gloo", init_method=f"tcp://127.0.0.1:{port}", rank=rank, world_size=R)
-    try:
-        pc._S.prefix_bit = prefix_bit
-        q.put((rank, pc._exchange_cap(list(zip(_ragged_slots(rank), pf)), "cpu")))
-    finally:
-        dist.destroy_process_group()
-
-
-def test_exchange_cap_counts_ragged_slots_at_the_prefix_width(oracle):
-    """persia_core's exchange cap: the most distinct signs one rank's first batch asks of one owner, over the ranks, at
-    the configured prefix width, with its own margin."""
-    R, prefix_bit = 2, 12
-    pf = [oracle.index_prefix(0, prefix_bit), 0, oracle.index_prefix(3, prefix_bit)]
-    port = _free_port()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_run_exchange_cap, args=(r, port, q, R, pf, prefix_bit)) for r in range(R)]
-    for p in procs:
-        p.start()
-    caps = [q.get(timeout=180)[1] for _ in range(R)]
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
-    worst = max(int(_exchange_cap_counts(list(zip(_ragged_slots(r), pf)), R, prefix_bit).max()) for r in range(R))
-    assert caps == [(int(worst * 1.5) + 1024 + 7) // 8 * 8] * R
+    assert got.tolist() == _owner_counts(list(zip(slot_ids, pf)), R, prefix_bit).tolist()
 
 
 def test_exchange_area_geometry():
