@@ -65,6 +65,11 @@ typedef enum {
 
 typedef enum { PB_OPT_SGD = 0, PB_OPT_ADAGRAD = 1, PB_OPT_ADAGRAD_VW = 2, PB_OPT_ADAM = 3 } pb_optim_kind;
 
+/* What Adagrad's fused lanes (elements < 8 * floor(dim / 8)) take for 1 / sqrt(s + eps); the tail is exact either way.
+ * EXACT: the correctly rounded value.  INTEL: _mm256_rsqrt_ps as Intel CPUs compute it (a 2 x 1024-entry table), which
+ * reproduces the reference's Adagrad steps bit for bit as run on an Intel CPU. */
+typedef enum { PB_RSQRT_EXACT = 0, PB_RSQRT_INTEL = 1 } pb_rsqrt_mode;
+
 typedef struct pb_table pb_table; /* one shard: hash index + row store, owned by the library */
 typedef struct pb_ctx pb_ctx;     /* per-batch device context: what the EW keeps in post_forward_buffer */
 
@@ -98,6 +103,11 @@ int pb_table_create(int device, const pb_table_cfg* cfg, pb_table** out);
 int pb_table_destroy(pb_table* t);
 /* register_optimizer (embedding_parameter_service/mod.rs:429-438). Must precede the first insert. */
 int pb_table_set_optimizer(pb_table* t, const pb_optim_cfg* cfg);
+/* Adagrad's rsqrt mode (pb_rsqrt_mode; PB_RSQRT_EXACT until set).  Like pb_table_set_optimizer, it is read when work is
+ * enqueued: it applies to every row step enqueued after the call, and a captured graph keeps the mode it was captured
+ * with.  Any optimizer kind accepts it; only the Adagrad kinds read it.  Rows of an attached host-memory tier are stepped
+ * with the mode of the table they are attached to. */
+int pb_table_set_rsqrt(pb_table* t, int mode);
 /* configure (embedding_parameter_service/mod.rs:440-451). */
 int pb_table_configure(pb_table* t, const pb_hyper_cfg* cfg);
 /* num_total_signs (persia-embedding-holder/src/lib.rs:73-79); synchronises `stream`. */

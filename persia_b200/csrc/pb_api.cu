@@ -972,6 +972,13 @@ int pb_table_set_optimizer(pb_table* t, const pb_optim_cfg* c) {
   return PB_OK;
 }
 
+int pb_table_set_rsqrt(pb_table* t, int mode) {
+  if (!t) return fail(PB_ERR_INVALID, "null argument");
+  if (mode != PB_RSQRT_EXACT && mode != PB_RSQRT_INTEL) return fail(PB_ERR_INVALID, "unknown rsqrt mode");
+  t->op.rsqrt = mode;
+  return PB_OK;
+}
+
 int pb_table_configure(pb_table* t, const pb_hyper_cfg* c) {
   if (!t || !c) return fail(PB_ERR_INVALID, "null argument");
   t->hy.lo = c->init_lower;

@@ -102,6 +102,7 @@ enum {
 struct OptimDev {
   int kind;
   float lr, wd, mom, init_acc, eps, b1, b2;
+  int rsqrt;  // pb_rsqrt_mode (pb_table_set_rsqrt): the launchers pick the INTEL instantiation of a stepping kernel
 };
 
 struct HyperDev {

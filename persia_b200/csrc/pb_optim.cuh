@@ -1,10 +1,16 @@
 // pb_optim.cuh — the optimizer step on resident rows (internal; SURVEY.md §8a row A9).
 // persia-simd/src/lib.rs, persia-common/src/optim.rs:227-307.
 // The reference runs 8-wide AVX2 FMAs on elements [0, 8*floor(len/8)) and an UNFUSED scalar tail after that; both
-// forms are reproduced per element (the library is compiled with --fmad=false) so that SGD is bit-exact and Adagrad
-// differs from the reference only by its _mm256_rsqrt_ps approximation (exact 1/sqrt here, as in the reference's tail).
+// forms are reproduced per element (the library is compiled with --fmad=false) so that SGD is bit-exact.  Adagrad's
+// fused lanes take _mm256_rsqrt_ps(s + eps) there, its tail exact 1/sqrt.  A table's rsqrt mode (pb_table_set_rsqrt)
+// picks what the fused lanes take here: PB_RSQRT_EXACT (default) exact 1/sqrt, as the tail, so that the step differs
+// from the reference by the approximation's error (<= 1.5 * 2^-12 relative); PB_RSQRT_INTEL rsqrt_intel, the
+// instruction as Intel CPUs compute it, so that the step is the reference's bit for bit as run on an Intel CPU (AMD's
+// approximation differs in the low bits and is not reproduced).  The mode is a template argument of every kernel that
+// steps rows, dispatched at launch: the exact instantiations are the code that runs without the mode.
 #pragma once
 #include "pb_device.cuh"
+#include "pb_rsqrt_table.cuh"
 
 namespace pb {
 
@@ -22,9 +28,29 @@ __device__ __forceinline__ void sgd_elem(float& w, float g, bool fused, const Op
   }
 }
 
+// RSQRTPS as Intel CPUs compute it: for x = 2^k * 1.m, p = k & 1, the entry at (p, top 10 bits of m) with its exponent
+// lowered by (k - p) / 2; zeros and denormals give a signed infinity, +inf +0, a negative input the default NaN and a
+// NaN itself, quieted.  The table (scripts/gen_rsqrt_table.py) was read from the instruction, and this model matches
+// it on all 2^32 inputs.  Read through L1: neighbouring lanes take different entries, which constant memory would
+// serialize.
+__device__ __forceinline__ float rsqrt_intel(float x) {
+  const uint32_t u = __float_as_uint(x);
+  if (u - 0x00800000u < 0x7f000000u) {  // positive normal
+    const int k = (int)(u >> 23) - 127, p = k & 1;
+    const uint32_t t = __ldg(&kRsqrtIntel[(p << 10) | ((u >> 13) & 1023u)]);
+    return __uint_as_float((uint32_t)((int)t - ((k - p) >> 1) * (1 << 23)));
+  }
+  const uint32_t e = (u >> 23) & 0xffu, neg = u >> 31;
+  if (e == 0xffu) return __uint_as_float((u & 0x7fffffu) ? (u | 0x400000u) : (neg ? 0xffc00000u : 0u));
+  if (e == 0u) return __uint_as_float(neg ? 0xff800000u : 0x7f800000u);
+  return __uint_as_float(0xffc00000u);  // negative normal or -inf
+}
+
+template <bool INTEL>
 __device__ __forceinline__ void adagrad_elem(float& w, float& s, float g, bool fused, const OptimDev& op) {
   float sq = __fmul_rn(g, g);
-  float r = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(s, op.eps)));
+  const float x = __fadd_rn(s, op.eps);
+  float r = (INTEL && fused) ? rsqrt_intel(x) : __fdiv_rn(1.0f, __fsqrt_rn(x));
   float scaled = __fmul_rn(g, r);
   if (fused) {
     w = __fmaf_rn(-op.lr, scaled, w);
@@ -62,7 +88,8 @@ struct StepCtx {
 
 // N consecutive elements of a resident row starting at element e0: load (issued early so that it overlaps the
 // gradient fetch), optimizer step + weight bound given the reduced gradient, store.  KIND < 0: decided at run time.
-template <int KIND, int N>
+// INTEL: Adagrad's fused lanes take rsqrt_intel (the table's rsqrt mode is PB_RSQRT_INTEL).
+template <int KIND, int N, bool INTEL = false>
 struct RowElems {
   static constexpr bool kRuntime = KIND < 0;
   static constexpr bool kS1 = kRuntime || KIND == PB_OPT_ADAGRAD || KIND == PB_OPT_ADAM;
@@ -125,15 +152,18 @@ struct RowElems {
     } else if (k == PB_OPT_ADAGRAD) {
 #pragma unroll
       for (int q = 0; q < N; ++q) {
-        adagrad_elem(w[q], s1[kS1 ? q : 0], g[q], e0 + q < fused_end, op);
+        adagrad_elem<INTEL>(w[q], s1[kS1 ? q : 0], g[q], e0 + q < fused_end, op);
         w[q] = bound(w[q], hy);
       }
     } else if (k == PB_OPT_ADAGRAD_VW) {  // emb step with the OLD scalar state (lib.rs:81-121)
-      float r = __fdiv_rn(1.0f, __fsqrt_rn(__fadd_rn(sc.vw_state, op.eps)));
+      const float x = __fadd_rn(sc.vw_state, op.eps);
+      const float r = __fdiv_rn(1.0f, __fsqrt_rn(x));
+      const float rf = INTEL ? rsqrt_intel(x) : r;  // the fused lanes' factor
 #pragma unroll
       for (int q = 0; q < N; ++q) {
-        float scaled = __fmul_rn(g[q], r);
-        w[q] = (e0 + q < fused_end) ? __fmaf_rn(-op.lr, scaled, w[q]) : __fadd_rn(__fmul_rn(-op.lr, scaled), w[q]);
+        const bool fused = e0 + q < fused_end;
+        float scaled = __fmul_rn(g[q], fused ? rf : r);
+        w[q] = fused ? __fmaf_rn(-op.lr, scaled, w[q]) : __fadd_rn(__fmul_rn(-op.lr, scaled), w[q]);
         w[q] = bound(w[q], hy);
       }
     } else {  // Adam
@@ -182,12 +212,12 @@ __device__ __forceinline__ bool row_missing(uint32_t row, const TableDev& t, uin
 // one optimizer step on the lane's columns of a resident row, VEC at a time (lane < G lanes per row): the row's
 // elements are loaded first, so that they are in flight while grad(e0, g) fills g with the gradient of columns
 // [e0, e0 + VEC)
-template <int KIND, int VEC, typename GRAD>
+template <int KIND, int VEC, bool INTEL = false, typename GRAD>
 __device__ __forceinline__ void step_row(float* prow, const TableDev& t, const OptimDev& op, const HyperDev& hy,
                                          const StepCtx& sc, uint32_t lane, uint32_t G, GRAD grad) {
   const uint32_t nvec = t.dim / VEC;
   for (uint32_t c = lane; c < nvec; c += G) {
-    RowElems<KIND, VEC> rc;
+    RowElems<KIND, VEC, INTEL> rc;
     float g[VEC];
     rc.load(prow, c * VEC, t, op);
     grad(c * VEC, g);

@@ -232,14 +232,14 @@ __device__ __forceinline__ void send_item(const TableDev& t, const SlotsDev& sl,
   if (lane == 0) *send_gok_ptr(a.x, target) = 1u;
 }
 
-template <int VEC, bool F16, int KIND, typename POS>
+template <int VEC, bool F16, int KIND, bool INTEL, typename POS>
 __device__ __forceinline__ void step_item(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl,
                                           const GradsDev& gr, const ReduceArgs& a, uint32_t row, uint32_t slot,
                                           uint32_t cnt, uint32_t lane, uint32_t G, uint32_t gmask, float* stage, POS pos) {
   float* prow = t.rows + (size_t)row * t.stride;
   const ItemSrc src = item_src(sl, gr, a, slot);
   const StepCtx sc = step_ctx(prow, t, op, gr, slot);
-  step_row<KIND, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&acc)[VEC]) {
+  step_row<KIND, VEC, INTEL>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&acc)[VEC]) {
     reduce_sorted<VEC, F16>(acc, src, a, t, cnt, e0, pos);
     if (KIND == PB_OPT_ADAGRAD_VW) store_vec<VEC>(stage + e0, acc);
   });
@@ -248,7 +248,7 @@ __device__ __forceinline__ void step_item(const TableDev& t, const OptimDev& op,
 
 // ---- warm items: one lane group per item; the group sorts the item's <= 32 occurrences (rank by counting), then adds
 // them in order.  Items are assigned statically (a shared work counter would be thousands of same-address atomics).
-template <int VEC, bool F16, int KIND, bool SEND>
+template <int VEC, bool F16, int KIND, bool SEND, bool INTEL = false>
 __global__ void __launch_bounds__(256, 3) k_reduce_warm(TableDev t, OptimDev op, HyperDev hy, SlotsDev sl, GradsDev gr,
                                                      ReduceArgs a, uint32_t G) {
   __shared__ uint32_t dead[PB_MAX_SLOTS / 32];
@@ -281,14 +281,14 @@ __global__ void __launch_bounds__(256, 3) k_reduce_warm(TableDev t, OptimDev op,
     }
     if (slot_dead(dead, slot) || row_missing(row, t, lane, !a.quiet_miss)) continue;
     float* stage = a.vw_stage ? a.vw_stage + (size_t)(n_cold + w) * t.dim : nullptr;
-    step_item<VEC, F16, KIND>(t, op, hy, sl, gr, a, row, slot, cnt, lane, G, gmask, stage, [&](uint32_t k) { return srt[k]; });
+    step_item<VEC, F16, KIND, INTEL>(t, op, hy, sl, gr, a, row, slot, cnt, lane, G, gmask, stage, [&](uint32_t k) { return srt[k]; });
   }
 }
 
 // ---- cold items (one occurrence — the majority): nothing to reduce.  One lane group per item, nothing but two
 // independent loads (row, gradient), the step and the store; light on registers so that the whole chip's worth of
 // groups is resident and the loads of many rows are in flight.
-template <int VEC, bool F16, int KIND, bool SEND>
+template <int VEC, bool F16, int KIND, bool SEND, bool INTEL = false>
 __global__ void __launch_bounds__(256) k_reduce_cold(TableDev t, OptimDev op, HyperDev hy, SlotsDev sl, GradsDev gr,
                                                      ReduceArgs a, uint32_t G) {
   __shared__ uint32_t dead[PB_MAX_SLOTS / 32];
@@ -324,13 +324,13 @@ __global__ void __launch_bounds__(256) k_reduce_cold(TableDev t, OptimDev op, Hy
     if (slot_dead(dead, slot) || row_missing(d.x, t, lane, !a.quiet_miss)) continue;
     if (KIND == PB_OPT_ADAGRAD_VW) {  // needs the whole reduced gradient staged for the dot
       const uint32_t occ = d.y;
-      step_item<VEC, F16, KIND>(t, op, hy, sl, gr, a, d.x, slot, 1u, lane, G, group_mask(G),
+      step_item<VEC, F16, KIND, INTEL>(t, op, hy, sl, gr, a, d.x, slot, 1u, lane, G, group_mask(G),
                                 a.vw_stage + (size_t)w * t.dim, [&](uint32_t) { return occ; });
       continue;
     }
     float* prow = t.rows + (size_t)d.x * t.stride;
     const StepCtx sc = KIND == PB_OPT_ADAM ? step_ctx(prow, t, op, gr, slot) : StepCtx{0.0f, 0.0f, 0.0f};
-    step_row<KIND, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&acc)[VEC]) {
+    step_row<KIND, VEC, INTEL>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&acc)[VEC]) {
       float g[VEC];
       load_grad_elems<VEC, F16>(g, src.gbase, gelem, e0);
 #pragma unroll
@@ -860,7 +860,7 @@ __global__ void __launch_bounds__(SHORT_WARPS * 32, 4) k_reduce_hot_short(TableD
 // ---- hot items, the step (local path): a lane group per item takes the sum k_reduce_hot staged at its entry of `hot`,
 // applies the whole dead mask, NaN marks included, and steps the row.  The step depends on the element index and the
 // summed value only, so the rows come out as they would from a step fused into the reduce.
-template <int VEC>
+template <int VEC, bool INTEL = false>
 __global__ void __launch_bounds__(256) k_step_hot(TableDev t, OptimDev op, HyperDev hy, SlotsDev sl, GradsDev gr,
                                                   ReduceArgs a, uint32_t G) {
   __shared__ uint32_t dead[PB_MAX_SLOTS / 32];
@@ -878,7 +878,7 @@ __global__ void __launch_bounds__(256) k_step_hot(TableDev t, OptimDev op, Hyper
     const float* sum = a.hot_stage + (size_t)entry * t.dim;
     float* prow = t.rows + (size_t)row * t.stride;
     const StepCtx sc = step_ctx(prow, t, op, gr, slot);
-    step_row<-1, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&g)[VEC]) { load_vec<VEC>(sum + e0, g); });
+    step_row<-1, VEC, INTEL>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&g)[VEC]) { load_vec<VEC>(sum + e0, g); });
     if (op.kind == PB_OPT_ADAGRAD_VW) vw_state_step(prow, sum, t, op, sc, lane, gmask);
   }
 }
@@ -899,12 +899,18 @@ static void items_dispatch(const TableDev& t, const OptimDev& op, const HyperDev
     PB_LAUNCH_F(FAM_UPDATE, (k_reduce_cold<VEC, F16, PB_OPT_SGD, true>), grid_cold, 256, 0, st, t, op, hy, sl, gr, a, G);
     return;
   }
-#define PB_K(KK)                                                                                                   \
-  case KK:                                                                                                         \
-    PB_LAUNCH_F(FAM_WARM, (k_reduce_warm<VEC, F16, KK, false>), grid_warm, 256, 0, st_warm, t, op, hy, sl, gr, a, G); \
-    PB_LAUNCH_F(FAM_UPDATE, (k_reduce_cold<VEC, F16, KK, false>), grid_cold, 256, 0, st, t, op, hy, sl, gr, a, G); \
-    break;
-  switch (op.kind) { PB_K(PB_OPT_SGD) PB_K(PB_OPT_ADAGRAD) PB_K(PB_OPT_ADAGRAD_VW) PB_K(PB_OPT_ADAM) }
+#define PB_K(KK, IN)                                                                                                  \
+  do {                                                                                                                \
+    PB_LAUNCH_F(FAM_WARM, (k_reduce_warm<VEC, F16, KK, false, IN>), grid_warm, 256, 0, st_warm, t, op, hy, sl, gr, a, G); \
+    PB_LAUNCH_F(FAM_UPDATE, (k_reduce_cold<VEC, F16, KK, false, IN>), grid_cold, 256, 0, st, t, op, hy, sl, gr, a, G); \
+  } while (0)
+  const bool intel = op.rsqrt == PB_RSQRT_INTEL;
+  switch (op.kind) {
+    case PB_OPT_SGD: PB_K(PB_OPT_SGD, false); break;
+    case PB_OPT_ADAGRAD: if (intel) PB_K(PB_OPT_ADAGRAD, true); else PB_K(PB_OPT_ADAGRAD, false); break;
+    case PB_OPT_ADAGRAD_VW: if (intel) PB_K(PB_OPT_ADAGRAD_VW, true); else PB_K(PB_OPT_ADAGRAD_VW, false); break;
+    case PB_OPT_ADAM: PB_K(PB_OPT_ADAM, false); break;
+  }
 #undef PB_K
 }
 
@@ -1022,8 +1028,13 @@ void launch_step_hot(const TableDev& t, const OptimDev& op, const HyperDev& hy, 
   // at most this many hot items exist; blocks past their number return at once
   uint32_t grid = cdiv(cdiv(a.b.n, PB_WARM_MAX + 1), 256u / G);
   if (grid > PB_NUM_SMS * 2u) grid = PB_NUM_SMS * 2u;  // groups stride over the list
-  if (vec == 4) PB_LAUNCH(k_step_hot<4>, grid, 256, 0, st, t, op, hy, sl, gr, a, G);
-  else PB_LAUNCH(k_step_hot<1>, grid, 256, 0, st, t, op, hy, sl, gr, a, G);
+  if (op.rsqrt == PB_RSQRT_INTEL) {
+    if (vec == 4) PB_LAUNCH((k_step_hot<4, true>), grid, 256, 0, st, t, op, hy, sl, gr, a, G);
+    else PB_LAUNCH((k_step_hot<1, true>), grid, 256, 0, st, t, op, hy, sl, gr, a, G);
+  } else {
+    if (vec == 4) PB_LAUNCH(k_step_hot<4>, grid, 256, 0, st, t, op, hy, sl, gr, a, G);
+    else PB_LAUNCH(k_step_hot<1>, grid, 256, 0, st, t, op, hy, sl, gr, a, G);
+  }
 }
 
 void launch_reduce_items(const TableDev& t, const OptimDev& op, const HyperDev& hy, const SlotsDev& sl,

@@ -559,7 +559,7 @@ void launch_owner_adam(const XchgDev& x, float* table_pow, float b1, float b2, c
 // request's own index, so the row, the gradient and the cell's holder mask are fetched together, two dependent memory
 // round trips per row in all.  Signs without storage are counted (gradient_id_miss_count).  The cell goes back to empty.
 // ------------------------------------------------------------------------------------------------
-template <int VEC, int CPL, int KIND>
+template <int VEC, int CPL, int KIND, bool INTEL = false>
 __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(TableDev t, OptimDev op, HyperDev hy, XchgDev x, uint32_t G) {
   // G lanes per row, CPL chunks of VEC floats per lane (G * CPL * VEC == dim): few lanes per row keep the per-row
   // bookkeeping off most of the warp, and a lane has CPL independent loads in flight
@@ -607,7 +607,7 @@ __global__ void __launch_bounds__(256, CPL == 1 ? 3 : 2) k_owner_update_all(Tabl
       auto ctx = [&](uint32_t s) { return step_ctx(op, 0.0f, owner_adam_pair(x, s, akey)); };
       // the holder mask, the row and the opener's gradient: one round trip
       const uint32_t mask = cell->mask;
-      RowElems<KIND, VEC> rc[CPL];
+      RowElems<KIND, VEC, INTEL> rc[CPL];
       float g1[CPL][VEC];
 #pragma unroll
       for (int u = 0; u < CPL; ++u) {
@@ -700,7 +700,7 @@ __global__ void k_uclear(XchgDev x) {
 // (sign, gradient) whose apply word is set; signs without storage are counted (gradient_id_miss_count).  The
 // requests of a step are served one launch after another, in rank order.
 // ------------------------------------------------------------------------------------------------
-template <int VEC>
+template <int VEC, bool INTEL = false>
 __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, HyperDev hy, XchgDev x, uint32_t src,
                                                       uint32_t G) {
   const uint32_t lane = threadIdx.x % G, gmask = group_mask(G);
@@ -726,7 +726,7 @@ __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, H
         if (gok[k] != 0u) {
           const float* g0 = grads + (size_t)k * t.dim;
           sc.vw_state = op.kind == PB_OPT_ADAGRAD_VW ? prow[t.dim] : 0.0f;
-          step_row<-1, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&g)[VEC]) { load_vec<VEC>(g0 + e0, g); });
+          step_row<-1, VEC, INTEL>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&g)[VEC]) { load_vec<VEC>(g0 + e0, g); });
           if (op.kind == PB_OPT_ADAGRAD_VW) vw_state_step(prow, g0, t, op, sc, lane, gmask);
         }
         k = link[k] & CHAIN_END;
@@ -754,7 +754,7 @@ __global__ void __launch_bounds__(256) k_owner_update(TableDev t, OptimDev op, H
       sc[u] = step_ctx(op, (act[u] && op.kind == PB_OPT_ADAGRAD_VW) ? prow[u][t.dim] : 0.0f, owner_adam_pair(x, src, akey));
     }
     for (uint32_t c = lane; c < nvec; c += G) {
-      RowElems<-1, VEC> rc[2];
+      RowElems<-1, VEC, INTEL> rc[2];
       float g[2][VEC];
 #pragma unroll
       for (int u = 0; u < 2; ++u)
@@ -975,8 +975,11 @@ void launch_owner_update(const TableDev& t, const OptimDev& op, const HyperDev& 
 template <int VEC, int CPL>
 static void owner_update_all_kind(const TableDev& t, const OptimDev& op, const HyperDev& hy, const XchgDev& x, uint32_t G,
                                   uint32_t grid, cudaStream_t st) {
+  const bool intel = op.rsqrt == PB_RSQRT_INTEL;
   if (op.kind == PB_OPT_SGD) PB_LAUNCH_F(FAM_OWNER, (k_owner_update_all<VEC, CPL, PB_OPT_SGD>), grid, 256, 0, st, t, op, hy, x, G);
+  else if (op.kind == PB_OPT_ADAGRAD && intel) PB_LAUNCH_F(FAM_OWNER, (k_owner_update_all<VEC, CPL, PB_OPT_ADAGRAD, true>), grid, 256, 0, st, t, op, hy, x, G);
   else if (op.kind == PB_OPT_ADAGRAD) PB_LAUNCH_F(FAM_OWNER, (k_owner_update_all<VEC, CPL, PB_OPT_ADAGRAD>), grid, 256, 0, st, t, op, hy, x, G);
+  else if (op.kind == PB_OPT_ADAGRAD_VW && intel) PB_LAUNCH_F(FAM_OWNER, (k_owner_update_all<VEC, CPL, -1, true>), grid, 256, 0, st, t, op, hy, x, G);
   else PB_LAUNCH_F(FAM_OWNER, (k_owner_update_all<VEC, CPL, -1>), grid, 256, 0, st, t, op, hy, x, G);
 }
 
@@ -1002,8 +1005,13 @@ void launch_owner_update(const TableDev& t, const OptimDev& op, const HyperDev& 
   const uint32_t G = (uint32_t)Gi;
   const uint32_t full = cdiv((uint64_t)cdiv(x.cap, 2) * G, 256);
   const uint32_t grid = full < PB_NUM_SMS * 6u ? full : PB_NUM_SMS * 6u;
-  if (vec == 4) PB_LAUNCH_F(FAM_UPDATE, (k_owner_update<4>), grid, 256, 0, st, t, op, hy, x, src, G);
-  else PB_LAUNCH_F(FAM_UPDATE, (k_owner_update<1>), grid, 256, 0, st, t, op, hy, x, src, G);
+  if (op.rsqrt == PB_RSQRT_INTEL) {
+    if (vec == 4) PB_LAUNCH_F(FAM_UPDATE, (k_owner_update<4, true>), grid, 256, 0, st, t, op, hy, x, src, G);
+    else PB_LAUNCH_F(FAM_UPDATE, (k_owner_update<1, true>), grid, 256, 0, st, t, op, hy, x, src, G);
+  } else {
+    if (vec == 4) PB_LAUNCH_F(FAM_UPDATE, (k_owner_update<4>), grid, 256, 0, st, t, op, hy, x, src, G);
+    else PB_LAUNCH_F(FAM_UPDATE, (k_owner_update<1>), grid, 256, 0, st, t, op, hy, x, src, G);
+  }
 }
 
 }  // namespace pb

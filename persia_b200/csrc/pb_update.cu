@@ -59,7 +59,7 @@ __global__ void k_slot_status(GradsDev gr, uint32_t n_slots, const uint32_t* __r
 
 // pb_update: distinct signs with explicit f32 gradients (update_gradient_mixed, PS mod.rs:359-427); the raw backward
 // (by_row: the rows its forward found).
-template <int VEC, int G>
+template <int VEC, int G, bool INTEL = false>
 __global__ void __launch_bounds__(256) k_update_direct(TableDev t, OptimDev op, HyperDev hy, int by_row,
                                                        const uint32_t* __restrict__ occ_cell,
                                                        const float* __restrict__ grads, uint32_t n,
@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(256) k_update_direct(TableDev t, OptimDev op, 
   float* prow = t.rows + (size_t)row * t.stride;
   const StepCtx sc = step_ctx(op, op.kind == PB_OPT_ADAGRAD_VW ? prow[t.dim] : 0.0f, adam_pair);
   const float* g0 = grads + (size_t)gid * t.dim;
-  step_row<-1, VEC>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&g)[VEC]) { load_vec<VEC>(g0 + e0, g); });
+  step_row<-1, VEC, INTEL>(prow, t, op, hy, sc, lane, G, [&](uint32_t e0, float (&g)[VEC]) { load_vec<VEC>(g0 + e0, g); });
   if (op.kind == PB_OPT_ADAGRAD_VW) vw_state_step(prow, g0, t, op, sc, lane, group_mask(G));
 }
 
@@ -142,10 +142,16 @@ void launch_update_direct(const TableDev& t, const OptimDev& op, const HyperDev&
   int vec, G;
   vec_group(t.dim, vec, G);
   uint32_t grid = cdiv((uint64_t)n * G, 256);
-#define PB_U(V, GG)                                                                                          \
-  if (vec == V && G == GG)                                                                                   \
-    PB_LAUNCH_F(FAM_UPDATE, (k_update_direct<V, GG>), grid, 256, 0, st, t, op, hy, by_row ? 1 : 0, where, grads, n,  \
-                adam_pair, n_ptr, tick, nan_tick);
+  const bool intel = op.rsqrt == PB_RSQRT_INTEL;
+#define PB_U(V, GG)                                                                                                 \
+  if (vec == V && G == GG) {                                                                                        \
+    if (intel)                                                                                                      \
+      PB_LAUNCH_F(FAM_UPDATE, (k_update_direct<V, GG, true>), grid, 256, 0, st, t, op, hy, by_row ? 1 : 0, where,   \
+                  grads, n, adam_pair, n_ptr, tick, nan_tick);                                                      \
+    else                                                                                                            \
+      PB_LAUNCH_F(FAM_UPDATE, (k_update_direct<V, GG>), grid, 256, 0, st, t, op, hy, by_row ? 1 : 0, where, grads, n, \
+                  adam_pair, n_ptr, tick, nan_tick);                                                                \
+  }
   PB_U(4, 1) PB_U(4, 2) PB_U(4, 4) PB_U(4, 8) PB_U(4, 16) PB_U(4, 32)
   PB_U(1, 1) PB_U(1, 2) PB_U(1, 4) PB_U(1, 8) PB_U(1, 16) PB_U(1, 32)
 #undef PB_U

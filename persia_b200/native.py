@@ -11,6 +11,7 @@ SO_PATH = os.environ.get("PERSIA_B200_LIB") or os.path.join(_HERE, "libpersia_b2
 
 PB_MAX_SLOTS = 128
 OPT_SGD, OPT_ADAGRAD, OPT_ADAGRAD_VW, OPT_ADAM = 0, 1, 2, 3
+RSQRT_EXACT, RSQRT_INTEL = 0, 1  # pb_rsqrt_mode
 
 PHASE_SEND, PHASE_SERVE, PHASE_FINISH, PHASE_ALL, PHASE_PREPARE = 1, 2, 4, 7, 8
 PB_OK, PB_ERR_INVALID, PB_ERR_CUDA, PB_ERR_STATE, PB_ERR_CAPACITY, PB_ERR_BATCH, PB_ERR_FORMAT = 0, -1, -2, -3, -4, -5, -6
@@ -51,6 +52,7 @@ SYMBOLS = {
     "pb_table_create": (_i32, [_i32, C.POINTER(TableCfg), C.POINTER(_vp)]),
     "pb_table_destroy": (_i32, [_vp]),
     "pb_table_set_optimizer": (_i32, [_vp, C.POINTER(OptimCfg)]),
+    "pb_table_set_rsqrt": (_i32, [_vp, _i32]),
     "pb_table_configure": (_i32, [_vp, C.POINTER(HyperCfg)]),
     "pb_table_size": (_i32, [_vp, C.POINTER(_u64), _vp]),
     "pb_table_clear": (_i32, [_vp, _vp]),

@@ -112,6 +112,16 @@ def hbm_split(capacity, hbm_rows, replica_size=1, shared=False):
     return hbm_rows, capacity - hbm_rows
 
 
+def adagrad_rsqrt():
+    """PERSIA_B200_ADAGRAD_RSQRT: "intel" steps Adagrad's fused lanes with _mm256_rsqrt_ps as Intel CPUs compute it, so
+    that training matches the reference's bit for bit as run on an Intel CPU; unset or "exact": exact 1/sqrt.  Read when
+    the optimizer is registered; every rank must see the same value."""
+    v = os.environ.get("PERSIA_B200_ADAGRAD_RSQRT", "").strip() or "exact"
+    if v not in ("exact", "intel"):
+        raise RuntimeError(f"PERSIA_B200_ADAGRAD_RSQRT must be 'exact' or 'intel', got {v!r}")
+    return v
+
+
 def shared_tier_on():
     """PERSIA_B200_SHARED_TIER=1: host tiers are created in shared memory (see the module docstring)."""
     return os.environ.get("PERSIA_B200_SHARED_TIER", "").strip() == "1"
@@ -126,6 +136,7 @@ class _State:
         self.groups = {}  # dim -> dict(shard, ctx pool, slot indices)
         self.capacity = int(os.environ.get("PERSIA_B200_CAPACITY", 1 << 22))
         self.optimizer = None
+        self.rsqrt = "exact"  # adagrad_rsqrt() when the optimizer was registered
         self.hyper = None
         self.device_id = None
         self.replica_index, self.replica_size = 0, 1
@@ -225,6 +236,7 @@ class _State:
             sh.set_eviction()  # the reference's holder is an LRU map bounded by `capacity` (eviction_map.rs:76-97)
             if self.optimizer is not None:
                 sh.set_optimizer(**self.optimizer)
+                sh.set_rsqrt(self.rsqrt)
             if self.hyper is not None:
                 sh.configure(**self.hyper)
             if self.incremental_on():  # twice the flush threshold: the set fills while a flush is being taken
@@ -1423,8 +1435,10 @@ class OptimizerBase:  # optim.rs:8-66
         if self._cfg is None:
             raise RuntimeError("optimizer is not initialized")
         _S.optimizer = dict(self._cfg)
+        _S.rsqrt = adagrad_rsqrt()
         for g in _S.groups.values():
             g["shard"].set_optimizer(**_S.optimizer)
+            g["shard"].set_rsqrt(_S.rsqrt)  # the R-GPU workers serve this shard: an owner steps with its mode
         _start_infer()  # job_type Infer: the servers load their checkpoint and start scanning for incremental updates
         _start_train_remote()  # job_type Train on R GPUs: export the tables live for forwards that do not train
 

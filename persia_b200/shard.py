@@ -147,6 +147,18 @@ class StreamMark:
             stream.wait_event(self.ev)
 
 
+def rsqrt_mode(mode):
+    """pb_rsqrt_mode of "exact" / "intel" (or of the mode itself)."""
+    modes = {"exact": N.RSQRT_EXACT, "intel": N.RSQRT_INTEL}
+    if isinstance(mode, str):
+        if mode not in modes:
+            raise ValueError(f"unknown rsqrt mode {mode!r}: expected 'exact' or 'intel'")
+        return modes[mode]
+    if mode not in modes.values():
+        raise ValueError(f"unknown rsqrt mode {mode!r}")
+    return int(mode)
+
+
 class EmbeddingShard:
     def __init__(self, dim, capacity, device=0, tier_rows=0, host=False, shared_tier=False):
         """capacity: rows in HBM.  tier_rows > 0: a host-memory tier of that many rows behind them (include/persia_b200.h,
@@ -183,6 +195,16 @@ class EmbeddingShard:
             if not self._tier_attached:
                 N.check(self.lib.pb_table_attach_tier(self.h, self.host_tier.h))
                 self._tier_attached = True
+
+    def set_rsqrt(self, mode):
+        """Adagrad's 1/sqrt(s + eps) on the fused lanes (elements < 8 * (dim // 8)): "exact" (N.RSQRT_EXACT, the
+        default) or "intel" (N.RSQRT_INTEL: _mm256_rsqrt_ps as Intel CPUs compute it, so that steps match the reference's
+        bit for bit as run on an Intel CPU).  Applies to every step enqueued after the call (pb_table_set_rsqrt); the host
+        tier gets the same mode."""
+        m = rsqrt_mode(mode)
+        N.check(self.lib.pb_table_set_rsqrt(self.h, m))
+        if self.host_tier is not None:
+            N.check(self.lib.pb_table_set_rsqrt(self.host_tier.h, m))
 
     # configure (PS mod.rs:440-451)
     def configure(self, init_lower=-0.01, init_upper=0.01, admit_probability=1.0, enable_weight_bound=True,

@@ -55,12 +55,13 @@ def _by_phase(workers, *phases):
 class ShardedEmbeddingWorker:
     def __init__(self, n_slots, dim, prefixes, capacity, device, rank, world, cap, area, peer_bases, optimizer,
                  hyper=None, max_batch=4096, sqrt_scaling=None, rows_f32=False, prefix_bit=8, stream=None,
-                 max_ids_per_sample=1, shard=None, tier_rows=0, shared_tier=False):
+                 max_ids_per_sample=1, shard=None, tier_rows=0, shared_tier=False, rsqrt=None):
         """shard: an existing EmbeddingShard of this rank to serve (configured by its owner, who also closes it), so
         that the workers of one dim — summation slots and raw slots — share one table; None: a new one.  tier_rows > 0:
         the new shard has a host-memory tier of that many rows behind its `capacity` HBM rows (EmbeddingShard; a
         caller's `shard` brings its own tier or none); shared_tier: that tier is shared memory, so the shard can be exported
-        to a RemoteReader (EmbeddingShard).  Statistics: `self.shard.tier_stats()`."""
+        to a RemoteReader (EmbeddingShard).  rsqrt: the new shard's Adagrad rsqrt mode (EmbeddingShard.set_rsqrt; None:
+        exact).  Statistics: `self.shard.tier_stats()`."""
         self.S, self.dim, self.rank, self.R, self.cap = n_slots, dim, rank, world, int(cap)
         self.device = device if isinstance(device, torch.device) else torch.device("cuda", device)
         self.lib = N.load()
@@ -70,6 +71,8 @@ class ShardedEmbeddingWorker:
         if shard is None:
             shard = SH.EmbeddingShard(dim, capacity, self.device, tier_rows=tier_rows, shared_tier=shared_tier)
             shard.set_optimizer(**optimizer)
+            if rsqrt is not None:
+                shard.set_rsqrt(rsqrt)
             shard.configure(**(hyper or {}))
         assert shard.dim == dim, "the shard holds another embedding dim"
         self.shard = shard
