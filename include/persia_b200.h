@@ -232,6 +232,30 @@ int pb_inc_held(pb_table* t, uint64_t* h_out);
  * EMPTY cell on its probe path; every eviction check rebuilds the index (tombstones dropped) once fewer than 1/8 of the
  * cells are EMPTY.  Synchronises `stream`. */
 int pb_table_index_stats(pb_table* t, uint64_t h_out[3], void* stream);
+/* ---- growable storage: `capacity` bounds a table instead of reserving it ----------------------------------------
+ * pb_table_set_growth(t, 1), before the table's first allocation (after it: PB_ERR_STATE; a host table refuses it with
+ * PB_ERR_STATE), makes the table's storage grow with its entries.  Device address space is reserved for `capacity` rows
+ * (rows, row recency, free-row stack, the rebuild's pairs) and for the largest index (next_pow2(1.5 x capacity) cells
+ * + 3) through the driver's virtual memory calls; physical HBM backs it in chunks of the allocation granularity as
+ * admissions reach it.  Before a call that can admit signs launches anything (training pb_forward, pb_forward_raw and
+ * pb_lookup, pb_set_rows and so pb_image_insert, an owner's training PB_PHASE_SERVE: at most R x cap signs), the host
+ * backs every row that call and the calls still in flight could hand out, by a bound it keeps without waiting for the
+ * device (the last row count read back, plus the signs of every call issued since), growing by at least 1/8 of what is
+ * mapped.  When the cells those rows and the used cells could take pass 2/3 of the index, the index is doubled in the
+ * table's index chain: its live entries are re-inserted as an eviction check's rebuild does.  Rows never move, so
+ * pending batches survive growth.  Results are bit for bit those of the same table without growth; the allocator never
+ * hands out a row that is not backed (pb_table_storage_stats [3] counts such refusals and stays 0).  A chunk that
+ * cannot be had fails the call with PB_ERR_CUDA before it launches any kernel or copy (only the event wait and record
+ * that order it among the table's calls reach its stream); the table stays valid and a later call can grow it.  Eviction still works against `capacity`: running out of HBM never evicts.  A call enqueued under stream
+ * capture first backs the whole capacity (a replay never passes through the host's bound).  A growable table cannot be
+ * exported (pb_table_export_view, pb_table_export_live_view) nor take a host tier (pb_table_attach_tier): PB_ERR_STATE.
+ * pb_debug_owned counts the bytes backed, not those reserved.  Memory is not given back before the table is
+ * destroyed (pb_table_clear and eviction keep it). */
+int pb_table_set_growth(pb_table* t, int on);
+/* [0] rows reserved (capacity), [1] rows backed by memory (= capacity on a table without growth), [2] index cells,
+ * [3] admissions refused because their row was not backed (must stay 0).  Before the first allocation [1..3] are 0.
+ * Synchronises `stream`. */
+int pb_table_storage_stats(pb_table* t, uint64_t h_out[4], void* stream);
 
 /* ---- single-request entry points (the PS RPCs) ------------------------------------------------- */
 /* lookup_mixed -> batched_lookup (embedding_parameter_service/mod.rs:162-262, 344-357).

@@ -1,5 +1,7 @@
 // pb_api.cu — the C ABI of libpersia_b200.so (include/persia_b200.h): object lifetime, argument checks,
 // kernel sequencing.  No torch types, no allocation on the hot path after the first call of a given size.
+#include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -121,6 +123,29 @@ struct pb_table {
   // pb_table_export_live_view: peers read in place while the table keeps training; sweeps, rebuilds, pb_set_rows and
   // pb_table_clear keep `seq` odd while they move cells or reuse rows (one table, one export mode)
   bool live = false;
+  // growable storage (pb_table_set_growth): the rows, row_tick, free-row stack, rebuild pairs and index cells each have
+  // address space reserved for `capacity` rows (the index: for its largest size, max_cells), backed by memory from the
+  // start up to `mapped` bytes (grow_for)
+  bool grow = false;
+  struct Region {
+    char* base = nullptr;
+    size_t mapped = 0;
+  };
+  enum { G_ROWS, G_TICK, G_FREE, G_RKEYS, G_RROWS, G_CELLS, G_COUNT };
+  Region region[G_COUNT];
+  uint32_t max_cells = 0;
+  size_t gran = 0;  // every chunk's size is a multiple of it
+  // the host's bound on the rows (CTR_ROWS) and used cells (CTR_USED) of every call enqueued: the last values read back
+  // (base_*) plus every sign an admitting call issued since (issued - base_issued).  A read-back (k_grow_readback into
+  // mapped pinned rb_host, stamped rb_stamp) is enqueued by an admitting call when none is outstanding and read by a
+  // later one once its stamp is there; it covers the calls issued before it (rb_issued), which the index chain orders
+  // before it
+  uint64_t issued = 0, base_issued = 0, rb_issued = 0;
+  uint32_t base_rows = 0, base_used = 0, rb_stamp = 0;
+  bool rb_pending = false;
+  uint32_t* rb_host = nullptr;  // [3]: rows, used cells, stamp
+  uint32_t* rb_dev = nullptr;
+  cudaStream_t grow_st = nullptr;  // growth asked for under stream capture runs here, outside the graph
   Owned own;  // every CUDA resource above
 };
 
@@ -198,6 +223,82 @@ enum { PREP_NONE = 0, PREP_SUM = 1, PREP_RAW = 2 };
 
 namespace {
 
+// ---- growable storage (pb_table_set_growth) --------------------------------------------------------------------------
+// bytes per row of each row-indexed region
+size_t region_row_bytes(const pb_table* t, int r) {
+  switch (r) {
+    case pb_table::G_ROWS: return sizeof(float) * (size_t)t->d.stride;
+    case pb_table::G_RKEYS: return sizeof(uint64_t);
+    default: return sizeof(uint32_t);  // row_tick, free_rows, rebuild_rows
+  }
+}
+
+// The chunks that back `rows` rows and `cells` index cells (+ N_SPECIAL), acquired into `o`; `mapped[r]` receives
+// each region's new extent.  Nothing is enqueued.
+int map_growth(pb_table* t, uint64_t rows, uint64_t cells, Owned& o, size_t mapped[pb_table::G_COUNT]) {
+  for (int r = 0; r < pb_table::G_COUNT; ++r) {
+    const size_t want = r == pb_table::G_CELLS ? sizeof(Cell) * ((size_t)cells + N_SPECIAL) : region_row_bytes(t, r) * rows;
+    const size_t to = (want + t->gran - 1) / t->gran * t->gran;
+    pb_table::Region& g = t->region[r];
+    mapped[r] = g.mapped;
+    if (to <= g.mapped) continue;
+    if (int rc = o.chunk(g.base + g.mapped, to - g.mapped, t->device)) return rc;
+    mapped[r] = to;
+  }
+  return PB_OK;
+}
+
+// largest extent of each region: `capacity` rows, the index at max_cells
+size_t region_reserved(const pb_table* t, int r) {
+  if (r == pb_table::G_CELLS) return sizeof(Cell) * ((size_t)t->max_cells + N_SPECIAL);
+  return region_row_bytes(t, r) * t->d.capacity;
+}
+
+// A growable table's first allocation: every region reserved at its largest extent (rounded to the granularity), the
+// first chunk of rows and the index they need backed, counters, the sweep's workspace, the read-back word and the stream
+// of captured growth; the cells filled, row_tick zeroed.  The index starts at the size an eager table of `mapped`
+// rows would have.
+int acquire_growable(pb_table* t, Owned& o) {
+  TableDev& d = t->d;
+  t->max_cells = d.n_cells;
+  if (!(t->gran = vmm_granularity(t->device))) return fail(PB_ERR_CUDA, "no virtual memory management on this device");
+  int rc;
+  for (int r = 0; r < pb_table::G_COUNT; ++r) {
+    const size_t span = (region_reserved(t, r) + t->gran - 1) / t->gran * t->gran;
+    t->region[r] = pb_table::Region{};
+    if ((rc = o.reserve(t->region[r].base, span))) return rc;
+  }
+  uint64_t rows = t->gran / region_row_bytes(t, pb_table::G_ROWS);
+  rows = rows < 1 ? 1 : rows > d.capacity ? d.capacity : rows;
+  uint64_t want = rows + rows / 2;
+  const uint32_t cells = next_pow2(want < 1024 ? 1024 : want);
+  size_t mapped[pb_table::G_COUNT];
+  if ((rc = map_growth(t, rows, cells, o, mapped)) || (rc = o.dev(d.counters, sizeof(uint32_t) * CTR_COUNT)) ||
+      (rc = o.dev(t->evict_ws, sizeof(uint32_t) * EVICT_WS_WORDS)) ||
+      (rc = o.mapped(t->rb_host, t->rb_dev, 3 * sizeof(uint32_t))) || (rc = o.stream(t->grow_st)))
+    return rc;
+  for (int r = 0; r < pb_table::G_COUNT; ++r) t->region[r].mapped = mapped[r];
+  d.cells = reinterpret_cast<Cell*>(t->region[pb_table::G_CELLS].base);
+  d.rows = reinterpret_cast<float*>(t->region[pb_table::G_ROWS].base);
+  d.row_tick = reinterpret_cast<uint32_t*>(t->region[pb_table::G_TICK].base);
+  d.free_rows = nullptr;  // (the gate: set once adopted)
+  t->rebuild_keys = reinterpret_cast<uint64_t*>(t->region[pb_table::G_RKEYS].base);
+  t->rebuild_rows = reinterpret_cast<uint32_t*>(t->region[pb_table::G_RROWS].base);
+  d.mapped = (uint32_t)rows;
+  d.n_cells = cells;
+  d.cell_mask = cells - 1;
+  d.bucket_mask = cells / BUCKET - 1;
+  t->issued = t->base_issued = t->rb_issued = 0;
+  t->base_rows = t->base_used = 0;
+  t->rb_pending = false;
+  t->rb_host[2] = t->rb_stamp;
+  PB_CUDA(cudaMemset(d.row_tick, 0, sizeof(uint32_t) * rows));
+  PB_CUDA(cudaMemset(d.counters, 0, sizeof(uint32_t) * CTR_COUNT));
+  launch_fill_cells(d.cells, (uint64_t)d.n_cells + N_SPECIAL, 0);
+  PB_CUDA(cudaDeviceSynchronize());
+  return PB_OK;
+}
+
 // The table's index, rows, counters and row_tick, acquired into `o`: the caller adopts `o`, then sets `allocated`.
 int acquire_storage(pb_table* t, Owned& o) {
   if (!t->has_op) return fail(PB_ERR_STATE, "optimizer not registered (OptimizerNotFoundError)");
@@ -222,6 +323,8 @@ int acquire_storage(pb_table* t, Owned& o) {
   d.cell_mask = d.n_cells - 1;
   d.bucket_mask = d.n_cells / BUCKET - 1;
   const size_t rows_bytes = sizeof(float) * (size_t)d.capacity * d.stride;
+  d.mapped = d.capacity;
+  if (t->grow) return acquire_growable(t, o);
   int rc;
   if ((rc = o.dev(d.cells, sizeof(Cell) * ((size_t)d.n_cells + N_SPECIAL))) ||
       // a host table's rows are not write-combined: the host reads them back (checkpoints)
@@ -243,6 +346,7 @@ int ensure_alloc(pb_table* t) {
   Owned o;
   if (int rc = acquire_storage(t, o)) return rc;
   t->own.adopt(o);
+  if (t->grow) t->d.free_rows = reinterpret_cast<uint32_t*>(t->region[pb_table::G_FREE].base);
   t->allocated = true;
   return PB_OK;
 }
@@ -420,6 +524,79 @@ struct TableCall {
     if (chains & CALL_STEP) record(m->step, st);
   }
 };
+
+// Before a call on a growable table launches anything that can admit up to `n` signs (a training forward or lookup,
+// pb_set_rows, an owner's training SERVE), in the index chain: back every row the enqueued calls and this one can hand
+// out, and grow the index so that the cells they can use stay within 2/3 of it.  Rows grow by at least 1/8 of what is
+// mapped (a logarithmic number of mappings), the index by doubling.  A chunk that cannot be had fails the call with
+// PB_ERR_CUDA before any kernel or copy is enqueued (the call's TableCall has made its stream wait for the table's
+// earlier calls and records its mark: ordering only); the table stays as it was.  Under stream capture the whole capacity is
+// backed (a replay never passes here), the work enqueued outside the graph and waited for.  Any other table: nothing.
+int grow_for(pb_table* t, uint64_t n, cudaStream_t st) {
+  if (!t->grow) return PB_OK;
+  unsigned long long cap_id = 0;
+  PB_CUDA(capture_id(st, cap_id));
+  TableDev& d = t->d;
+  if (cap_id && d.mapped == d.capacity && d.n_cells == t->max_cells) return PB_OK;
+  if (t->rb_pending && reinterpret_cast<volatile uint32_t*>(t->rb_host)[2] == t->rb_stamp) {
+    std::atomic_thread_fence(std::memory_order_acquire);
+    t->base_rows = reinterpret_cast<volatile uint32_t*>(t->rb_host)[0];
+    t->base_used = reinterpret_cast<volatile uint32_t*>(t->rb_host)[1];
+    t->base_issued = t->rb_issued;
+    t->rb_pending = false;
+  }
+  const uint64_t since = t->issued - t->base_issued + n;
+  uint64_t rows = std::min<uint64_t>(d.capacity, t->base_rows + since);
+  const uint64_t used = std::max<uint64_t>(rows, t->base_used + since);
+  uint64_t cells = d.n_cells;
+  while (cells < t->max_cells && 3 * used > 2 * cells) cells *= 2;
+  if (cap_id) {
+    rows = d.capacity;
+    cells = t->max_cells;
+  } else if (rows > d.mapped) {
+    rows = std::min<uint64_t>(d.capacity, std::max<uint64_t>(rows, (uint64_t)d.mapped + d.mapped / 8));
+  } else {
+    rows = d.mapped;
+  }
+  if (rows > d.mapped || cells > d.n_cells) {
+    // captured: relaxed mode lets this thread map memory and use an uncaptured stream meanwhile
+    cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+    if (cap_id) PB_CUDA(cudaThreadExchangeStreamCaptureMode(&mode));
+    struct Restore {
+      bool on;
+      cudaStreamCaptureMode& m;
+      ~Restore() {
+        if (on) cudaThreadExchangeStreamCaptureMode(&m);
+      }
+    } restore{cap_id != 0, mode};
+    const cudaStream_t ws = cap_id ? t->grow_st : st;
+    Owned o;
+    size_t mapped[pb_table::G_COUNT];
+    if (int rc = map_growth(t, rows, cells, o, mapped)) return rc;
+    t->own.adopt(o);
+    for (int r = 0; r < pb_table::G_COUNT; ++r) t->region[r].mapped = mapped[r];
+    if (rows > d.mapped)
+      PB_CUDA(cudaMemsetAsync(d.row_tick + d.mapped, 0, sizeof(uint32_t) * (size_t)(rows - d.mapped), ws));
+    d.mapped = (uint32_t)rows;
+    if (cells > d.n_cells) {
+      TableDev to = d;
+      to.n_cells = (uint32_t)cells;
+      to.cell_mask = cells - 1;
+      to.bucket_mask = (uint32_t)(cells / BUCKET - 1);
+      launch_grow_index(d, to, t->evict_ws, t->rebuild_keys, t->rebuild_rows, ws);
+      d = to;
+    }
+    PB_CUDA(cudaGetLastError());
+    if (cap_id) PB_CUDA(cudaStreamSynchronize(ws));
+  }
+  if (!cap_id && !t->rb_pending) {
+    launch_grow_readback(d.counters, t->rb_dev, ++t->rb_stamp, st);
+    t->rb_issued = t->issued;
+    t->rb_pending = true;
+  }
+  t->issued += n;
+  return PB_OK;
+}
 
 // a table's counter words (`n` of them at `src`), copied to the host under a call in both chains; synchronises `st`
 template <typename W>
@@ -786,6 +963,7 @@ int pb_table_attach_tier(pb_table* t, pb_table* tier) {
   if (!t || !tier) return fail(PB_ERR_INVALID, "null argument");
   if (int rc = writable(t)) return rc;  // (an exported table can have no tier: peers could not read its host rows)
   if (t->live) return fail(PB_ERR_STATE, "a live-exported table cannot take a host tier: peers could not read its host rows");
+  if (t->grow) return fail(PB_ERR_STATE, "a growable table cannot take a host tier");
   if (t->host || !tier->host) return fail(PB_ERR_INVALID, "the tier must be a host table (pb_table_create_host) behind an HBM table");
   if (t->tier || t->tier_of || tier->tier_of || tier->tier) return fail(PB_ERR_STATE, "one of the tables already has a tier or is one");
   if (t->device != tier->device) return fail(PB_ERR_INVALID, "the tables live on different devices");
@@ -1041,6 +1219,27 @@ int pb_table_index_stats(pb_table* t, uint64_t h_out[3], void* stream) {
   return PB_OK;
 }
 
+int pb_table_set_growth(pb_table* t, int on) {
+  if (!t) return fail(PB_ERR_INVALID, "null argument");
+  if (t->host) return fail(PB_ERR_STATE, "a host table's storage cannot grow");
+  if (t->allocated) return fail(PB_ERR_STATE, "growth must be chosen before the table's first allocation");
+  t->grow = on != 0;
+  return PB_OK;
+}
+
+int pb_table_storage_stats(pb_table* t, uint64_t h_out[4], void* stream) {
+  if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
+  h_out[0] = t->cfg.capacity;
+  h_out[1] = h_out[2] = h_out[3] = 0;
+  if (!t->allocated) return PB_OK;
+  uint32_t c[CTR_COUNT];
+  if (int rc = read_counters(t, t->d.counters, c, CTR_COUNT, (cudaStream_t)stream)) return rc;
+  h_out[1] = t->d.mapped;
+  h_out[2] = t->d.n_cells;
+  h_out[3] = c[CTR_UNMAPPED];
+  return PB_OK;
+}
+
 int pb_table_size(pb_table* t, uint64_t* h_out, void* stream) {
   if (!t || !h_out) return fail(PB_ERR_INVALID, "null argument");
   uint64_t c[5];
@@ -1062,7 +1261,7 @@ int pb_table_clear(pb_table* t, void* stream) {
   if (t->live) launch_seq_bump(t->seq, true, st);
   launch_fill_cells(t->d.cells, (uint64_t)t->d.n_cells + N_SPECIAL, st);
   PB_CUDA(cudaMemsetAsync(t->d.counters, 0, sizeof(uint32_t) * CTR_COUNT, st));
-  PB_CUDA(cudaMemsetAsync(t->d.row_tick, 0, sizeof(uint32_t) * (size_t)t->d.capacity, st));
+  PB_CUDA(cudaMemsetAsync(t->d.row_tick, 0, sizeof(uint32_t) * (size_t)t->d.mapped, st));
   const int rc = t->tier ? pb_table_clear(t->tier, stream) : PB_OK;
   if (t->live) launch_seq_bump(t->seq, false, st);
   return rc;
@@ -1085,6 +1284,7 @@ int pb_lookup(pb_table* t, const uint64_t* d_signs, uint32_t n, int training, fl
   int rc = ensure_alloc(t);
   if (rc) return rc;
   if ((rc = ensure_scratch(t, n))) return rc;
+  if (training && (rc = grow_for(t, n, st))) return rc;
   SlotsDev sl = no_slots();
   if (training) {
     if ((rc = maybe_evict(t, st))) return rc;
@@ -1138,7 +1338,7 @@ int pb_set_rows(pb_table* t, const uint64_t* d_signs, const float* d_entries, ui
   if (int rc = call.begin(t, st, CALL_ALL)) return rc;
   int rc = ensure_alloc(t);
   if (rc) return rc;
-  if ((rc = ensure_scratch(t, n))) return rc;
+  if ((rc = ensure_scratch(t, n)) || (rc = grow_for(t, n, st))) return rc;
   SlotsDev sl = no_slots();
   // an exported table, frozen or live: peers reading it in place see the write-sequence word odd from before the first
   // cell it may claim (or, with a tier, the first entry it moves back) to after the last entry it writes (pb_remote.cu),
@@ -1757,7 +1957,7 @@ int pb_forward(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ, co
   cudaStream_t st = (cudaStream_t)stream;
   TableCall call;
   if ((rc = call.begin(t, st, CALL_INDEX))) return rc;
-  if ((rc = ensure_alloc(t))) return rc;
+  if ((rc = ensure_alloc(t)) || (training && (rc = grow_for(t, n_occ, st)))) return rc;
   // pb_backward's staging of the hot items' sums, hot_cap x dim floats (a wider table grows it)
   if (training && (rc = grow_stage(c->own, c->hot_stage, c->hot_stage_floats, (size_t)c->b.hot_cap * t->d.dim, st))) return rc;
   SlotsDev sl;
@@ -1972,6 +2172,15 @@ void serve_lookup(pb_table* t, pb_xchg* x, int training, const Phases& ph, cudaS
   launch_owner_lookup(training != 0, t->d, t->tier ? &t->tier->d : nullptr, t->hy, t->op, x->d, st);
   if (training) x->u_dirty = true;
   ph.post(x, XC_FLAG_ROW, nullptr, st);
+}
+
+// A growable owner's training SERVE admits up to R x cap signs (the R requests' receive areas): its table grows first
+// (grow_for), and the call joins the table's index chain, which the read-back that bounds its growth relies on.  Every
+// other sharded call orders nothing here, as before.
+int owner_grow(pb_table* t, pb_xchg* x, int training, const Phases& ph, TableCall& call, cudaStream_t st) {
+  if (!t->grow || !training || !ph.has(PB_PHASE_SERVE)) return PB_OK;
+  if (int rc = call.begin(t, st, CALL_INDEX)) return rc;
+  return grow_for(t, (uint64_t)x->d.R * x->d.cap, st);
 }
 
 // The owner's part of a sharded backward (PB_PHASE_SERVE), shared by the summation and the raw calls: the step's R
@@ -2198,6 +2407,8 @@ int pb_forward_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d_ids
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (ph.exchanges() && (rc = ensure_alloc(t))) return rc;
+  TableCall call;
+  if ((rc = owner_grow(t, x, training, ph, call, st))) return rc;
   SlotsDev sl;
   if ((rc = make_slots(c->slots, h_slot_occ_off, sl))) return rc;
   if (ph.has(PB_PHASE_PREPARE)) {  // requester, local: the dedup and its items per owner
@@ -2307,7 +2518,7 @@ int pb_forward_raw(pb_table* t, pb_ctx* c, const uint64_t* d_ids, uint32_t n_occ
   if ((rc = call.begin(t, st, CALL_INDEX))) return rc;
   if ((rc = ensure_alloc(t))) return rc;
   if ((rc = ensure_raw(c))) return rc;
-  if (training && (rc = ensure_raw_stage(c, n_occ, t->d.dim, st))) return rc;
+  if (training && ((rc = ensure_raw_stage(c, n_occ, t->d.dim, st)) || (rc = grow_for(t, n_occ, st)))) return rc;
   SlotsDev sl;
   if ((rc = raw_slots(c, n_occ, sl))) return rc;
   c->raw_pending.drop();  // the numbering below replaces the pending batch's
@@ -2390,7 +2601,8 @@ int pb_forward_raw_sharded(pb_table* t, pb_ctx* c, pb_xchg* x, const uint64_t* d
   DeviceGuard g(t->device);
   cudaStream_t st = (cudaStream_t)stream;
   if (ph.exchanges() && (rc = ensure_alloc(t))) return rc;
-  if ((rc = ensure_raw(c))) return rc;
+  TableCall call;
+  if ((rc = owner_grow(t, x, training, ph, call, st)) || (rc = ensure_raw(c))) return rc;
   SlotsDev sl;
   if ((rc = raw_slots(c, n_occ, sl))) return rc;
   // the slot's distinct signs numbered, index / non_empty / sample_id_num written: no table state is read
@@ -2576,6 +2788,8 @@ int export_blob(pb_table* t, void* h_blob, bool live) {
     return fail(PB_ERR_STATE, "a host tier cannot be exported: its rows are pinned host memory no peer process can map");
   if (t->tier && !t->tier->shared)
     return fail(PB_ERR_STATE, "a table with a host tier cannot be exported: peers could not read its tier's rows");
+  if (t->grow)
+    return fail(PB_ERR_STATE, "a growable table cannot be exported: its storage is mapped in chunks no export describes");
   DeviceGuard g(t->device);
   if (int rc = ensure_alloc(t)) return rc;
   if (!t->seq) {
@@ -2733,6 +2947,7 @@ int open_view(int device, const void* h_blob, const void* h_tier_blob, pb_view**
   d.cell_mask = b.n_cells - 1;
   d.bucket_mask = b.n_cells / BUCKET - 1;
   d.capacity = b.capacity;
+  d.mapped = b.capacity;
   d.dim = b.dim;
   d.stride = b.stride;
   d.state_floats = b.state_floats;
@@ -2744,6 +2959,7 @@ int open_view(int device, const void* h_blob, const void* h_tier_blob, pb_view**
     h.cell_mask = tb.n_cells - 1;
     h.bucket_mask = tb.n_cells / BUCKET - 1;
     h.capacity = tb.capacity;
+    h.mapped = tb.capacity;
     h.dim = tb.dim;
     h.stride = tb.stride;
     h.state_floats = b.state_floats;

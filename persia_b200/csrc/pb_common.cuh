@@ -75,6 +75,7 @@ struct TableDev {
   uint32_t bucket_mask;  // n_cells / BUCKET - 1
   uint32_t n_cells;
   uint32_t capacity;
+  uint32_t mapped;       // rows backed by memory: `capacity`, or fewer in a growable table (pb_table_set_growth)
   uint32_t dim, stride, state_floats;
 };
 
@@ -96,7 +97,8 @@ enum {
   CTR_TIER_LOST = 13,     // victims of an HBM sweep that found no tier row (dropped, like a plain sweep's)
   CTR_STAGE_IN = 14,      // of CTR_TIER_IN: restores made by pb_tier_stage
   CTR_STAGE_SKIP = 15,    // pb_tier_stage restores that found no free HBM row (left to the request's own restore)
-  CTR_COUNT = 16
+  CTR_UNMAPPED = 16,      // admissions refused because their row is not backed yet (a growable table; must stay 0)
+  CTR_COUNT = 17
 };
 
 struct OptimDev {

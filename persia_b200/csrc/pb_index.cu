@@ -293,6 +293,30 @@ __global__ void __launch_bounds__(256) k_rebuild_insert(TableDev t, uint32_t* __
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// Growth of a growable table's index (launch_grow_index): the rebuild above with a larger target.  k_grow_plan forces
+// the rebuild flag; k_rebuild_compact runs with the old masks; k_grow_specials copies the reserved cells to the new end
+// before k_rebuild_clear (new n_cells) overwrites where they were; k_rebuild_insert re-inserts with the new masks.
+// ------------------------------------------------------------------------------------------------
+__global__ void k_grow_plan(uint32_t* __restrict__ ev) {
+  if (threadIdx.x) return;
+  ev[EV_RB] = 1u;
+  ev[EV_RB + 1] = 0u;
+}
+
+__global__ void k_grow_specials(Cell* cells, uint32_t from_n, uint32_t to_n) {
+  if (threadIdx.x < N_SPECIAL) cells[(size_t)to_n + threadIdx.x] = cells[(size_t)from_n + threadIdx.x];
+}
+
+__global__ void k_grow_readback(const uint32_t* __restrict__ counters, uint32_t* out, uint32_t stamp) {
+  if (threadIdx.x) return;
+  volatile uint32_t* o = out;
+  o[0] = counters[CTR_ROWS];
+  o[1] = counters[CTR_USED];
+  __threadfence_system();
+  o[2] = stamp;
+}
+
 // diagnostic (pb_table_index_stats): live, tombstone and EMPTY cells among the n_cells normal cells
 __global__ void __launch_bounds__(256) k_index_stats(TableDev t, uint32_t* __restrict__ out) {
   uint32_t live = 0, tomb = 0, empty = 0;
@@ -324,6 +348,20 @@ void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* r
   PB_LAUNCH(k_rebuild_compact, g, 256, 0, st, t, ev, keys, rows);
   PB_LAUNCH(k_rebuild_clear, g, 256, 0, st, t, ev);
   PB_LAUNCH(k_rebuild_insert, g, 256, 0, st, t, ev, keys, rows, seq);
+}
+
+void launch_grow_index(const TableDev& from, const TableDev& to, uint32_t* ev, uint64_t* keys, uint32_t* rows,
+                       cudaStream_t st) {
+  const uint32_t g = PB_NUM_SMS * 8;
+  PB_LAUNCH(k_grow_plan, 1, 32, 0, st, ev);
+  PB_LAUNCH(k_rebuild_compact, g, 256, 0, st, from, ev, keys, rows);
+  PB_LAUNCH(k_grow_specials, 1, 32, 0, st, to.cells, from.n_cells, to.n_cells);
+  PB_LAUNCH(k_rebuild_clear, g, 256, 0, st, to, ev);
+  PB_LAUNCH(k_rebuild_insert, g, 256, 0, st, to, ev, keys, rows, nullptr);
+}
+
+void launch_grow_readback(const uint32_t* counters, uint32_t* out, uint32_t stamp, cudaStream_t st) {
+  PB_LAUNCH(k_grow_readback, 1, 32, 0, st, counters, out, stamp);
 }
 
 void launch_index_stats(const TableDev& t, uint32_t* out, cudaStream_t st) {

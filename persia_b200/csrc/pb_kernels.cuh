@@ -377,6 +377,15 @@ void launch_tier_set(const TableDev& h, const TableDev& t, const HyperDev& hy, c
                      const uint32_t* occ_cell, uint32_t n, const float* entries, cudaStream_t st);
 void launch_rebuild(const TableDev& t, uint32_t* ev, uint64_t* keys, uint32_t* rows, cudaStream_t st, uint32_t blocks = 0,
                     uint32_t* seq = nullptr);
+// A growable table's index doubled (or more) in place: the live pairs of `from`'s normal cells are compacted, the
+// N_SPECIAL reserved cells move from from.n_cells to to.n_cells, to's normal cells are filled with EMPTY and every pair
+// is re-inserted with to's masks (CTR_USED = pairs).  `to` differs from `from` in n_cells and the masks only; the cells
+// up to to.n_cells + N_SPECIAL are mapped.  Ordered like a rebuild: nothing that holds cell numbers runs beside it.
+void launch_grow_index(const TableDev& from, const TableDev& to, uint32_t* ev, uint64_t* keys, uint32_t* rows,
+                       cudaStream_t st);
+// counters[CTR_ROWS] and counters[CTR_USED] copied to host-mapped `out` ([0], [1]), then out[2] = stamp: the host's
+// bound on what a growable table's enqueued calls can admit reads them once the stamp is there
+void launch_grow_readback(const uint32_t* counters, uint32_t* out, uint32_t stamp, cudaStream_t st);
 // checkpoint images (pb_dump.cu).  The part of a sign in a background dump: splitmix64(sign) % n_parts, with
 // splitmix64(x): z = x + 0x9E3779B97F4A7C15; z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
 // z = (z ^ (z >> 27)) * 0x94D049BB133111EB; return z ^ (z >> 31)   (include/persia_b200.h, pb_table_dump_part)

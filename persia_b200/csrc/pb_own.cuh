@@ -4,11 +4,14 @@
 // recorded in its Owned, which releases what is still held, in reverse order, when the object is deleted.  A step that
 // acquires several resources acquires them into a local Owned and adopts it once every part has succeeded, then sets
 // its gate: a step that fails leaves nothing allocated and no gate set, and the next call acquires afresh.
+// A growable table's storage (pb_table_set_growth) is device address space reserved for its whole capacity and backed
+// by physical memory chunk by chunk: the reservation and each chunk are resources of their own.
 #pragma once
 #include <atomic>
 #include <cerrno>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include <fcntl.h>
@@ -16,6 +19,7 @@
 #include <sys/stat.h>
 #include <unistd.h>
 
+#include <cuda.h>  // the driver's types only: its virtual-memory calls are reached through cudaGetDriverEntryPoint
 #include <cuda_runtime.h>
 
 #include "persia_b200.h"
@@ -41,14 +45,68 @@ int fail(int code, const std::string& msg) {
 std::atomic<uint64_t> g_owned_count{0}, g_owned_bytes{0};
 std::atomic<int64_t> g_refuse_after{-1};
 
+// The driver's virtual-memory calls, looked up once through the runtime, so that the library links only the shared
+// cudart.  `ok` false: the driver lacks one of them (every growable table is then refused).
+struct Vmm {
+  decltype(&cuMemAddressReserve) reserve = nullptr;
+  decltype(&cuMemAddressFree) free = nullptr;
+  decltype(&cuMemCreate) create = nullptr;
+  decltype(&cuMemRelease) release = nullptr;
+  decltype(&cuMemMap) map = nullptr;
+  decltype(&cuMemUnmap) unmap = nullptr;
+  decltype(&cuMemSetAccess) access = nullptr;
+  decltype(&cuMemGetAllocationGranularity) granularity = nullptr;
+  bool ok = false;
+};
+
+const Vmm& vmm() {
+  static const Vmm v = [] {
+    Vmm w;
+    auto get = [](const char* name, auto& fn) {
+      void* p = nullptr;
+      cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+      if (cudaGetDriverEntryPointByVersion(name, &p, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+          q != cudaDriverEntryPointSuccess)
+        p = nullptr;
+      fn = reinterpret_cast<std::remove_reference_t<decltype(fn)>>(p);
+      return p != nullptr;
+    };
+    w.ok = get("cuMemAddressReserve", w.reserve) & get("cuMemAddressFree", w.free) & get("cuMemCreate", w.create) &
+           get("cuMemRelease", w.release) & get("cuMemMap", w.map) & get("cuMemUnmap", w.unmap) &
+           get("cuMemSetAccess", w.access) & get("cuMemGetAllocationGranularity", w.granularity);
+    return w;
+  }();
+  return v;
+}
+
+CUmemAllocationProp vmm_prop(int device) {
+  CUmemAllocationProp prop;
+  std::memset(&prop, 0, sizeof(prop));
+  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+  prop.location.id = device;
+  return prop;
+}
+
+// the size every chunk of `device` is a multiple of (0: no virtual-memory support)
+size_t vmm_granularity(int device) {
+  const Vmm& v = vmm();
+  size_t g = 0;
+  const CUmemAllocationProp prop = vmm_prop(device);
+  if (!v.ok || v.granularity(&g, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM) != CUDA_SUCCESS) return 0;
+  return g;
+}
+
 struct Owned {
-  enum Kind { DEV, HOST, ASYNC, STREAM, EVENT, IPC, SHARED };
+  enum Kind { DEV, HOST, ASYNC, STREAM, EVENT, IPC, SHARED, VRESERVE, VCHUNK };
   struct Res {
     void* p;
     Kind kind;
-    size_t bytes;
+    size_t bytes;     // counted in pb_debug_owned (a reservation: 0)
     cudaStream_t st;  // ASYNC: the stream it was allocated on (the destructor frees it there)
     int fd = -1;      // SHARED: the file the mapping is of
+    size_t span = 0;  // VRESERVE: the address range reserved
+    unsigned long long handle = 0;  // VCHUNK: the physical allocation mapped at p
   };
   std::vector<Res> held;
 
@@ -143,6 +201,47 @@ struct Owned {
     const cudaError_t e = refused() ? cudaErrorMemoryAllocation : cudaEventCreateWithFlags(&q, cudaEventDisableTiming);
     return keep(e, "cudaEventCreateWithFlags", q, EVENT, 0, nullptr, ev);
   }
+  // `bytes` of device address space, nothing behind it yet (chunk() backs it)
+  template <typename T>
+  int reserve(T*& p, size_t bytes) {
+    const Vmm& v = vmm();
+    CUdeviceptr q = 0;
+    if (!v.ok) return fail(PB_ERR_CUDA, "the driver lacks the virtual memory management calls");
+    if (refused()) return fail(PB_ERR_CUDA, "cuMemAddressReserve: refused");
+    if (CUresult e = v.reserve(&q, bytes, 0, 0, 0))
+      return fail(PB_ERR_CUDA, "cuMemAddressReserve: CUresult " + std::to_string((int)e));
+    held.push_back({reinterpret_cast<void*>(q), VRESERVE, 0, nullptr, -1, bytes, 0});
+    g_owned_count += 1;
+    p = reinterpret_cast<T*>(q);
+    return PB_OK;
+  }
+  // `bytes` (a multiple of vmm_granularity) of `device`'s memory, created and mapped read-write at `at`, inside a
+  // reservation; undone as unmap, release
+  int chunk(void* at, size_t bytes, int device) {
+    const Vmm& v = vmm();
+    const CUmemAllocationProp prop = vmm_prop(device);
+    CUmemGenericAllocationHandle h = 0;
+    if (refused()) return fail(PB_ERR_CUDA, "cuMemCreate: refused");
+    if (CUresult e = v.create(&h, bytes, &prop, 0))
+      return fail(PB_ERR_CUDA, "cuMemCreate: CUresult " + std::to_string((int)e));
+    const CUdeviceptr q = reinterpret_cast<CUdeviceptr>(at);
+    CUresult e = v.map(q, bytes, 0, h, 0);
+    if (e == CUDA_SUCCESS) {
+      CUmemAccessDesc acc;
+      std::memset(&acc, 0, sizeof(acc));
+      acc.location = prop.location;
+      acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+      if ((e = v.access(q, bytes, &acc, 1)) != CUDA_SUCCESS) v.unmap(q, bytes);
+    }
+    if (e != CUDA_SUCCESS) {
+      v.release(h);
+      return fail(PB_ERR_CUDA, "cuMemMap / cuMemSetAccess: CUresult " + std::to_string((int)e));
+    }
+    held.push_back({at, VCHUNK, bytes, nullptr, -1, 0, (unsigned long long)h});
+    g_owned_count += 1;
+    g_owned_bytes += bytes;
+    return PB_OK;
+  }
   // another process's allocation, mapped into this one
   int ipc(void*& p, const cudaIpcMemHandle_t& h) {
     void* q = nullptr;
@@ -184,7 +283,7 @@ struct Owned {
   template <typename P>
   int keep(cudaError_t e, const char* what, void* q, Kind kind, size_t bytes, cudaStream_t st, P& out) {
     if (e != cudaSuccess) return fail(PB_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-    held.push_back({q, kind, bytes, st, -1});
+    held.push_back({q, kind, bytes, st, -1, 0, 0});
     g_owned_count += 1;
     g_owned_bytes += bytes;
     out = static_cast<P>(q);
@@ -204,6 +303,11 @@ struct Owned {
         cudaHostUnregister(r.p);
         munmap(r.p, r.bytes);
         close(r.fd);
+        break;
+      case VRESERVE: vmm().free(reinterpret_cast<CUdeviceptr>(r.p), r.span); break;
+      case VCHUNK:
+        vmm().unmap(reinterpret_cast<CUdeviceptr>(r.p), r.bytes);
+        vmm().release((CUmemGenericAllocationHandle)r.handle);
         break;
     }
     g_owned_count -= 1;

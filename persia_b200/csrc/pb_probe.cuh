@@ -129,9 +129,10 @@ __device__ __forceinline__ ProbeOut probe_group(const TableDev& t, const HyperDe
         atomicAdd(&t.counters[CTR_FREE], 1u);
         row = atomicAdd(&t.counters[CTR_ROWS], 1u);
       }
-      if (row >= t.capacity) {
+      if (row >= t.mapped) {  // (mapped <= capacity) a row past the backed ones is refused like a full shard's
+        if (row < t.capacity) atomicAdd(&t.counters[CTR_UNMAPPED], 1u);
+        else if (MODE != MODE_MOVE) atomicAdd(&t.counters[CTR_FULL], 1u);
         row = ROW_NONE;
-        if (MODE != MODE_MOVE) atomicAdd(&t.counters[CTR_FULL], 1u);
       } else {
         atomicAdd(&t.counters[CTR_ADMIT], 1u);
         t.row_tick[row] = tick;  // recency of a fresh row

@@ -60,6 +60,8 @@ SYMBOLS = {
     "pb_table_set_eviction": (_i32, [_vp, _u32, _u64, _u64, _u32]),
     "pb_table_counters": (_i32, [_vp, C.POINTER(_u64 * 5), _vp]),
     "pb_table_index_stats": (_i32, [_vp, C.POINTER(_u64 * 3), _vp]),
+    "pb_table_set_growth": (_i32, [_vp, _i32]),
+    "pb_table_storage_stats": (_i32, [_vp, C.POINTER(_u64 * 4), _vp]),
     "pb_table_create_host": (_i32, [_i32, C.POINTER(TableCfg), C.POINTER(_vp)]),
     "pb_table_create_host_shared": (_i32, [_i32, C.POINTER(TableCfg), C.POINTER(_vp)]),
     "pb_table_attach_tier": (_i32, [_vp, _vp]),

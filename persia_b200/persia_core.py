@@ -35,6 +35,12 @@ does not train reads tier-held signs from their owners' host rows in place.  It 
 costs more than private pinned memory: it is shmem charged to the owning rank's memory cgroup, every peer that reads
 it pins it again, and the ranks must run as one user in one PID namespace (a peer maps the owner's memfd through
 /proc/<pid>/fd).  Tier staging (worker.TierStager) stays off at replica_size > 1.
+
+PERSIA_B200_GROW=1 (growth_on) makes every dim group's table growable: `capacity` bounds each table instead of
+reserving HBM for it, and HBM backs rows and index cells as entries are admitted, so a config with several dims or the
+reference's default capacity of 1e9 costs what its resident entries cost.  Every dim still has its own `capacity`.  It
+is an opt-in, read when a dim group is created, so that the default stays today's allocation; it is refused at
+replica_size > 1 (tables are exported there) and together with PERSIA_B200_HBM_ROWS, before any table exists.
 """
 import os
 import queue
@@ -120,6 +126,26 @@ def adagrad_rsqrt():
     if v not in ("exact", "intel"):
         raise RuntimeError(f"PERSIA_B200_ADAGRAD_RSQRT must be 'exact' or 'intel', got {v!r}")
     return v
+
+
+def growth_on(grow, replica_size=1, hbm_rows=None):
+    """PERSIA_B200_GROW (`grow`; "1" on, None, "" or "0" off): every dim group's table is growable
+    (pb_table_set_growth): `capacity` bounds it and HBM backs its rows and index as entries are admitted, so the
+    reference's capacities (1e9 by default) can be configured as they are.  Refused at replica_size > 1 (a Train job
+    exports its tables live, an Infer job frozen, and a growable table cannot be exported) and together with
+    PERSIA_B200_HBM_ROWS (`hbm_rows`: a growable table has no host tier)."""
+    v = "" if grow is None else str(grow).strip()
+    if v not in ("", "0", "1"):
+        raise RuntimeError(f"PERSIA_B200_GROW must be '1' or '0', got {v!r}")
+    if v != "1":
+        return False
+    if (replica_size or 1) > 1:
+        raise RuntimeError("PERSIA_B200_GROW (tables that grow with their entries) is supported on one GPU only "
+                           f"(replica_size = 1, got {replica_size}): its tables are exported for remote reads there")
+    if hbm_rows is not None and str(hbm_rows).strip() != "":
+        raise RuntimeError("PERSIA_B200_GROW cannot be combined with PERSIA_B200_HBM_ROWS: a growable table has no "
+                           "host-memory tier")
+    return True
 
 
 def shared_tier_on():
@@ -231,8 +257,10 @@ class _State:
 
             dev = self.device_id if self.device_id is not None else 0
             shared = shared_tier_on()
-            hbm, tier = hbm_split(self.capacity, os.environ.get("PERSIA_B200_HBM_ROWS"), self.replica_size, shared=shared)
-            sh = SH.EmbeddingShard(dim, hbm, dev, tier_rows=tier, shared_tier=shared)
+            hbm_rows = os.environ.get("PERSIA_B200_HBM_ROWS")
+            grow = growth_on(os.environ.get("PERSIA_B200_GROW"), self.replica_size, hbm_rows)
+            hbm, tier = hbm_split(self.capacity, hbm_rows, self.replica_size, shared=shared)
+            sh = SH.EmbeddingShard(dim, hbm, dev, tier_rows=tier, shared_tier=shared, grow=grow)
             sh.set_eviction()  # the reference's holder is an LRU map bounded by `capacity` (eviction_map.rs:76-97)
             if self.optimizer is not None:
                 sh.set_optimizer(**self.optimizer)

@@ -116,6 +116,7 @@ def _read_block(fields, call, ctype=C.c_uint64):
 
 COUNTER_FIELDS = ("admitted", "lookup_miss", "gradient_id_miss", "capacity_refused", "wait_errors")
 INDEX_STATS_FIELDS = ("live", "tomb", "empty")
+STORAGE_STATS_FIELDS = ("reserved_rows", "mapped_rows", "index_cells", "refused_unmapped")
 TIER_STATS_FIELDS = ("host_rows", "moved_out", "restored", "dropped", "refused")
 STAGE_STATS_FIELDS = ("staged", "skipped")
 INCREMENTAL_STATS_FIELDS = ("held", "inserted", "dropped", "taken")
@@ -160,11 +161,15 @@ def rsqrt_mode(mode):
 
 
 class EmbeddingShard:
-    def __init__(self, dim, capacity, device=0, tier_rows=0, host=False, shared_tier=False):
+    def __init__(self, dim, capacity, device=0, tier_rows=0, host=False, shared_tier=False, grow=False):
         """capacity: rows in HBM.  tier_rows > 0: a host-memory tier of that many rows behind them (include/persia_b200.h,
         pb_table_attach_tier), attached once the optimizer is registered.  host: this table's rows live in host memory
         (the tier itself).  shared_tier: the tier's rows are shared memory other processes can map
-        (pb_table_create_host_shared), so that the table can be exported and its peers read the tier in place."""
+        (pb_table_create_host_shared), so that the table can be exported and its peers read the tier in place.
+        grow: capacity bounds the table instead of reserving it: HBM backs rows and index cells as entries are admitted
+        (pb_table_set_growth; no tier, no export)."""
+        if grow and (host or tier_rows):
+            raise ValueError("a growable table has no host tier and is not one")
         self.lib = N.load()
         self.dim, self.capacity = int(dim), int(capacity)
         self.device = torch.device("cuda", device) if not isinstance(device, torch.device) else device
@@ -175,6 +180,9 @@ class EmbeddingShard:
             create = self.lib.pb_table_create_host_shared if shared_tier else self.lib.pb_table_create_host
         N.check(create(self.device.index or 0, C.byref(cfg), C.byref(h)))
         self.h = h
+        self.grow = bool(grow)
+        if self.grow:
+            N.check(self.lib.pb_table_set_growth(h, 1))
         self._entry_len = None
         self.shared_tier = bool(shared_tier and tier_rows)
         self.host_tier = EmbeddingShard(dim, tier_rows, device, host=True, shared_tier=shared_tier) if tier_rows else None
@@ -232,6 +240,11 @@ class EmbeddingShard:
     def index_stats(self):
         """Cells of the hash index (host sync): live signs, tombstones of evicted signs, and EMPTY cells."""
         return _read_block(INDEX_STATS_FIELDS, lambda out: self.lib.pb_table_index_stats(self.h, out, _stream(self.device)))
+
+    def storage_stats(self):
+        """Storage of the table (host sync): rows reserved (capacity) and backed by HBM, index cells, and admissions
+        refused because their row was not backed yet (stays 0).  A table without growth backs its whole capacity."""
+        return _read_block(STORAGE_STATS_FIELDS, lambda out: self.lib.pb_table_storage_stats(self.h, out, _stream(self.device)))
 
     def tier_stats(self):
         """The host tier's counters (host sync); all zero without a tier."""

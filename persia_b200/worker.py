@@ -55,13 +55,14 @@ def _by_phase(workers, *phases):
 class ShardedEmbeddingWorker:
     def __init__(self, n_slots, dim, prefixes, capacity, device, rank, world, cap, area, peer_bases, optimizer,
                  hyper=None, max_batch=4096, sqrt_scaling=None, rows_f32=False, prefix_bit=8, stream=None,
-                 max_ids_per_sample=1, shard=None, tier_rows=0, shared_tier=False, rsqrt=None):
+                 max_ids_per_sample=1, shard=None, tier_rows=0, shared_tier=False, rsqrt=None, grow=False):
         """shard: an existing EmbeddingShard of this rank to serve (configured by its owner, who also closes it), so
         that the workers of one dim — summation slots and raw slots — share one table; None: a new one.  tier_rows > 0:
         the new shard has a host-memory tier of that many rows behind its `capacity` HBM rows (EmbeddingShard; a
         caller's `shard` brings its own tier or none); shared_tier: that tier is shared memory, so the shard can be exported
         to a RemoteReader (EmbeddingShard).  rsqrt: the new shard's Adagrad rsqrt mode (EmbeddingShard.set_rsqrt; None:
-        exact).  Statistics: `self.shard.tier_stats()`."""
+        exact).  grow: the new shard's storage grows with its entries (EmbeddingShard; not with a tier, and a growable
+        shard cannot be exported).  Statistics: `self.shard.tier_stats()`, `self.shard.storage_stats()`."""
         self.S, self.dim, self.rank, self.R, self.cap = n_slots, dim, rank, world, int(cap)
         self.device = device if isinstance(device, torch.device) else torch.device("cuda", device)
         self.lib = N.load()
@@ -69,7 +70,7 @@ class ShardedEmbeddingWorker:
         self.area = area  # keeps the receive area alive
         self._own_shard = shard is None
         if shard is None:
-            shard = SH.EmbeddingShard(dim, capacity, self.device, tier_rows=tier_rows, shared_tier=shared_tier)
+            shard = SH.EmbeddingShard(dim, capacity, self.device, tier_rows=tier_rows, shared_tier=shared_tier, grow=grow)
             shard.set_optimizer(**optimizer)
             if rsqrt is not None:
                 shard.set_rsqrt(rsqrt)
@@ -105,7 +106,8 @@ class ShardedEmbeddingWorker:
                     shared_tier=False, **kw):
         """R virtual ranks on one GPU (tests; also a way to exercise the protocol without a multi-GPU box).
         shards: the R ranks' existing EmbeddingShards (e.g. `[w.shard for w in group]` of another group of this dim).
-        tier_rows: host-tier rows behind each new shard (0: none); shared_tier: those tiers are shared memory."""
+        tier_rows: host-tier rows behind each new shard (0: none); shared_tier: those tiers are shared memory.  grow=True
+        (in **kw): each new shard's storage grows with its entries."""
         dev = torch.device("cuda", device)
         areas, bases = cls._local_areas(world, cls.area_bytes(world, cap, dim, kw.get("rows_f32", False)), dev)
         return [cls(n_slots, dim, prefixes, capacity, dev, r, world, cap, areas[r], bases, optimizer,
@@ -124,7 +126,8 @@ class ShardedEmbeddingWorker:
     def distributed(cls, n_slots, dim, prefixes, capacity, cap, optimizer, device, group=None, tier_rows=0,
                     shared_tier=False, **kw):
         """One process per GPU: the receive areas live in torch symmetric memory (every peer's area mapped here).
-        tier_rows: host-tier rows behind this rank's new shard (0: none); shared_tier: that tier is shared memory."""
+        tier_rows: host-tier rows behind this rank's new shard (0: none); shared_tier: that tier is shared memory.  grow=True
+        (in **kw): the new shard's storage grows with its entries."""
         import torch.distributed as dist
 
         grp = group if group is not None else dist.group.WORLD
