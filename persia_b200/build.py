@@ -7,8 +7,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libpersia_b200.so")
-SOURCES = ["pb_index.cu", "pb_dedup.cu", "pb_reduce.cu", "pb_shard.cu", "pb_remote.cu", "pb_sort.cu", "pb_update.cu", "pb_raw.cu", "pb_tier.cu", "pb_inc.cu", "pb_dump.cu", "pb_load.cu", "pb_launch.cu", "pb_api.cu"]
-HEADERS = ["pb_common.cuh", "pb_kernels.cuh", "pb_device.cuh", "pb_group.cuh", "pb_probe.cuh", "pb_optim.cuh", "pb_rsqrt_table.cuh", "pb_batch.cuh", "pb_own.cuh", os.path.join(ROOT, "include", "persia_b200.h")]
+SOURCES = ["pb_index.cu", "pb_dedup.cu", "pb_reduce.cu", "pb_shard.cu", "pb_remote.cu", "pb_sort.cu", "pb_update.cu", "pb_raw.cu", "pb_tier.cu", "pb_inc.cu", "pb_dump.cu", "pb_load.cu", "pb_launch.cu", "pb_own.cu", "pb_api.cu", "pb_api_ckpt.cu", "pb_api_batch.cu", "pb_api_shard.cu", "pb_api_view.cu"]
+HEADERS = ["pb_common.cuh", "pb_kernels.cuh", "pb_device.cuh", "pb_group.cuh", "pb_probe.cuh", "pb_optim.cuh", "pb_rsqrt_table.cuh", "pb_batch.cuh", "pb_own.cuh", "pb_api.cuh", os.path.join(ROOT, "include", "persia_b200.h")]
 
 
 def nvcc():

@@ -1,4 +1,4 @@
-// pb_own.cuh — the C ABI's error reporting and the CUDA resources its objects hold (included by pb_api.cu only).
+// pb_own.cuh — the C ABI's error reporting and the CUDA resources its objects hold (defined once, in pb_own.cu).
 // Every buffer, mapped pinned host block, shared host mapping, stream-ordered buffer, stream, event and IPC mapping an
 // object acquires is
 // recorded in its Owned, which releases what is still held, in reverse order, when the object is deleted.  A step that
@@ -11,7 +11,6 @@
 #include <cerrno>
 #include <cstring>
 #include <string>
-#include <type_traits>
 #include <vector>
 
 #include <fcntl.h>
@@ -24,26 +23,24 @@
 
 #include "persia_b200.h"
 
-namespace {
+namespace pb {
 
-thread_local std::string g_err;
+// the calling thread's last error message (pb_last_error)
+extern thread_local std::string g_err;
 
-int fail(int code, const std::string& msg) {
-  g_err = msg;
-  return code;
-}
+int fail(int code, const std::string& msg);
 
 #define PB_CUDA(expr)                                                                              \
   do {                                                                                             \
     cudaError_t e__ = (expr);                                                                      \
     if (e__ != cudaSuccess)                                                                        \
-      return fail(PB_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e__));               \
+      return pb::fail(PB_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e__));           \
   } while (0)
 
 // what every live object holds (pb_debug_owned), and the acquisitions still granted before one is refused
 // (pb_debug_refuse_after; -1: none is)
-std::atomic<uint64_t> g_owned_count{0}, g_owned_bytes{0};
-std::atomic<int64_t> g_refuse_after{-1};
+extern std::atomic<uint64_t> g_owned_count, g_owned_bytes;
+extern std::atomic<int64_t> g_refuse_after;
 
 // The driver's virtual-memory calls, looked up once through the runtime, so that the library links only the shared
 // cudart.  `ok` false: the driver lacks one of them (every growable table is then refused).
@@ -59,43 +56,10 @@ struct Vmm {
   bool ok = false;
 };
 
-const Vmm& vmm() {
-  static const Vmm v = [] {
-    Vmm w;
-    auto get = [](const char* name, auto& fn) {
-      void* p = nullptr;
-      cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
-      if (cudaGetDriverEntryPointByVersion(name, &p, 12000, cudaEnableDefault, &q) != cudaSuccess ||
-          q != cudaDriverEntryPointSuccess)
-        p = nullptr;
-      fn = reinterpret_cast<std::remove_reference_t<decltype(fn)>>(p);
-      return p != nullptr;
-    };
-    w.ok = get("cuMemAddressReserve", w.reserve) & get("cuMemAddressFree", w.free) & get("cuMemCreate", w.create) &
-           get("cuMemRelease", w.release) & get("cuMemMap", w.map) & get("cuMemUnmap", w.unmap) &
-           get("cuMemSetAccess", w.access) & get("cuMemGetAllocationGranularity", w.granularity);
-    return w;
-  }();
-  return v;
-}
-
-CUmemAllocationProp vmm_prop(int device) {
-  CUmemAllocationProp prop;
-  std::memset(&prop, 0, sizeof(prop));
-  prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
-  prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-  prop.location.id = device;
-  return prop;
-}
+const Vmm& vmm();
 
 // the size every chunk of `device` is a multiple of (0: no virtual-memory support)
-size_t vmm_granularity(int device) {
-  const Vmm& v = vmm();
-  size_t g = 0;
-  const CUmemAllocationProp prop = vmm_prop(device);
-  if (!v.ok || v.granularity(&g, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM) != CUDA_SUCCESS) return 0;
-  return g;
-}
+size_t vmm_granularity(int device);
 
 struct Owned {
   enum Kind { DEV, HOST, ASYNC, STREAM, EVENT, IPC, SHARED, VRESERVE, VCHUNK };
@@ -113,9 +77,7 @@ struct Owned {
   Owned() = default;
   Owned(const Owned&) = delete;
   Owned& operator=(const Owned&) = delete;
-  ~Owned() {
-    while (!held.empty()) drop(held.size() - 1, held.back().st);
-  }
+  ~Owned();
 
   template <typename T>
   int dev(T*& p, size_t bytes) {
@@ -191,16 +153,8 @@ struct Owned {
     const cudaError_t e = refused() ? cudaErrorMemoryAllocation : cudaMallocAsync(&q, bytes, st);
     return keep(e, "cudaMallocAsync", q, ASYNC, bytes, st, p);
   }
-  int stream(cudaStream_t& s) {
-    cudaStream_t q = nullptr;
-    const cudaError_t e = refused() ? cudaErrorMemoryAllocation : cudaStreamCreateWithFlags(&q, cudaStreamNonBlocking);
-    return keep(e, "cudaStreamCreateWithFlags", q, STREAM, 0, nullptr, s);
-  }
-  int event(cudaEvent_t& ev) {
-    cudaEvent_t q = nullptr;
-    const cudaError_t e = refused() ? cudaErrorMemoryAllocation : cudaEventCreateWithFlags(&q, cudaEventDisableTiming);
-    return keep(e, "cudaEventCreateWithFlags", q, EVENT, 0, nullptr, ev);
-  }
+  int stream(cudaStream_t& s);
+  int event(cudaEvent_t& ev);
   // `bytes` of device address space, nothing behind it yet (chunk() backs it)
   template <typename T>
   int reserve(T*& p, size_t bytes) {
@@ -217,38 +171,9 @@ struct Owned {
   }
   // `bytes` (a multiple of vmm_granularity) of `device`'s memory, created and mapped read-write at `at`, inside a
   // reservation; undone as unmap, release
-  int chunk(void* at, size_t bytes, int device) {
-    const Vmm& v = vmm();
-    const CUmemAllocationProp prop = vmm_prop(device);
-    CUmemGenericAllocationHandle h = 0;
-    if (refused()) return fail(PB_ERR_CUDA, "cuMemCreate: refused");
-    if (CUresult e = v.create(&h, bytes, &prop, 0))
-      return fail(PB_ERR_CUDA, "cuMemCreate: CUresult " + std::to_string((int)e));
-    const CUdeviceptr q = reinterpret_cast<CUdeviceptr>(at);
-    CUresult e = v.map(q, bytes, 0, h, 0);
-    if (e == CUDA_SUCCESS) {
-      CUmemAccessDesc acc;
-      std::memset(&acc, 0, sizeof(acc));
-      acc.location = prop.location;
-      acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
-      if ((e = v.access(q, bytes, &acc, 1)) != CUDA_SUCCESS) v.unmap(q, bytes);
-    }
-    if (e != CUDA_SUCCESS) {
-      v.release(h);
-      return fail(PB_ERR_CUDA, "cuMemMap / cuMemSetAccess: CUresult " + std::to_string((int)e));
-    }
-    held.push_back({at, VCHUNK, bytes, nullptr, -1, 0, (unsigned long long)h});
-    g_owned_count += 1;
-    g_owned_bytes += bytes;
-    return PB_OK;
-  }
+  int chunk(void* at, size_t bytes, int device);
   // another process's allocation, mapped into this one
-  int ipc(void*& p, const cudaIpcMemHandle_t& h) {
-    void* q = nullptr;
-    const cudaError_t e =
-        refused() ? cudaErrorMapBufferObjectFailed : cudaIpcOpenMemHandle(&q, h, cudaIpcMemLazyEnablePeerAccess);
-    return keep(e, "cudaIpcOpenMemHandle", q, IPC, 0, nullptr, p);
-  }
+  int ipc(void*& p, const cudaIpcMemHandle_t& h);
 
   // Release one resource now and null the caller's pointer (null, or not held here: nothing is released).  A
   // stream-ordered buffer is freed in `st`'s order.
@@ -262,23 +187,13 @@ struct Owned {
     p = nullptr;
   }
   // release everything, stream-ordered buffers in `st`'s order
-  void release_all(cudaStream_t st) {
-    while (!held.empty()) drop(held.size() - 1, st);
-  }
+  void release_all(cudaStream_t st);
   // take over what `o` holds (a step that has succeeded)
-  void adopt(Owned& o) {
-    held.insert(held.end(), o.held.begin(), o.held.end());
-    o.held.clear();
-  }
+  void adopt(Owned& o);
 
  private:
   // pb_debug_refuse_after: this acquisition is refused, before its CUDA call is made
-  static bool refused() {
-    int64_t n = g_refuse_after.load();
-    while (n >= 0 && !g_refuse_after.compare_exchange_weak(n, n - 1)) {
-    }
-    return n == 0;
-  }
+  static bool refused();
   // one acquisition's result (`e`, its CUDA call's or its refusal's): recorded and handed to `out` if it succeeded
   template <typename P>
   int keep(cudaError_t e, const char* what, void* q, Kind kind, size_t bytes, cudaStream_t st, P& out) {
@@ -289,30 +204,7 @@ struct Owned {
     out = static_cast<P>(q);
     return PB_OK;
   }
-  void drop(size_t i, cudaStream_t st) {
-    const Res r = held[i];
-    held.erase(held.begin() + i);
-    switch (r.kind) {
-      case DEV: cudaFree(r.p); break;
-      case HOST: cudaFreeHost(r.p); break;
-      case ASYNC: cudaFreeAsync(r.p, st); break;
-      case STREAM: cudaStreamDestroy(static_cast<cudaStream_t>(r.p)); break;
-      case EVENT: cudaEventDestroy(static_cast<cudaEvent_t>(r.p)); break;
-      case IPC: cudaIpcCloseMemHandle(r.p); break;
-      case SHARED:
-        cudaHostUnregister(r.p);
-        munmap(r.p, r.bytes);
-        close(r.fd);
-        break;
-      case VRESERVE: vmm().free(reinterpret_cast<CUdeviceptr>(r.p), r.span); break;
-      case VCHUNK:
-        vmm().unmap(reinterpret_cast<CUdeviceptr>(r.p), r.bytes);
-        vmm().release((CUmemGenericAllocationHandle)r.handle);
-        break;
-    }
-    g_owned_count -= 1;
-    g_owned_bytes -= r.bytes;
-  }
+  void drop(size_t i, cudaStream_t st);
 };
 
-}  // namespace
+}  // namespace pb

@@ -930,7 +930,7 @@ static HotGeom hot_geom(uint32_t dim, bool f16, bool ragged) {
   g.CH = (g.cols + 32u * EPL - 1u) / (32u * EPL);
   g.rowbytes = dim * (f16 ? 2u : 4u);
   // the producers' 16-byte loads need whole vectors per row; the rows are then 16-byte aligned, because the ABI
-  // refuses gradient pointers that are not (pb_api.cu)
+  // refuses gradient pointers that are not (pb_api_batch.cu)
   const uint32_t vec = dim % (f16 ? 8u : 4u) == 0 ? 1u : 0u;
   g.vec = vec;
   const uint32_t nvr = g.cols / (f16 ? 8u : 4u);

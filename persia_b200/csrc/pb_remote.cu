@@ -20,7 +20,7 @@
 // tier's index (HBM, through the view) where the owner's HBM probe misses, and reads a hit from the tier's host row (the
 // owner's memfd, mapped into this process and registered with CUDA).  One word covers the table and its tier: the owner
 // holds it odd around every launch that moves an entry between the two or hands a row of either to another sign
-// (pb_api.cu, TierWindow), so a reader never finds a moving sign in neither table, and a tier-held row read between two
+// (pb_api.cuh, TierWindow), so a reader never finds a moving sign in neither table, and a tier-held row read between two
 // equal even words is that sign's whole row.  The loads between the two reads of the word are the same for both tables:
 // the word is read with ld.acquire.sys (no later load of this thread is performed before it), the index and row loads
 // are plain weak ld.global.cg (whether the row sits in peer HBM over NVLink or in host memory over PCIe: the PTX memory

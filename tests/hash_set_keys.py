@@ -9,7 +9,7 @@ kernels; a change to a set's layout changes them here too.
                       `off = 2 occ_off[s] + 2 s`; the sign 2^64-1 (KEY_EMPTY) owns the reserved cell `off + size` that
                       sits between this region and the next.  Home: `off + umulhi(mix64(sign) >> 32, size)`; linear
                       probing wraps from `off + size - 1` to `off`.
-  raw scratch set     k_raw_insert (pb_raw.cu).  `cells = next_pow2(max(1024, 2 max_occurrences))` (ensure_raw, pb_api.cu:
+  raw scratch set     k_raw_insert (pb_raw.cu).  `cells = next_pow2(max(1024, 2 max_occurrences))` (ensure_raw, pb_api_batch.cu:
                       the context's max_occurrences); home `mix64(sign) & (cells - 1)`, wrapping to 0; the sign 2^64-1 owns
                       the extra cell `cells`.
   incremental set     inc_find / inc_claim (pb_inc.cu).  `n_cells = next_pow2(max(1024, 2 capacity))`
