@@ -247,10 +247,15 @@ int pb_table_index_stats(pb_table* t, uint64_t h_out[3], void* stream);
  * hands out a row that is not backed (pb_table_storage_stats [3] counts such refusals and stays 0).  A chunk that
  * cannot be had fails the call with PB_ERR_CUDA before it launches any kernel or copy (only the event wait and record
  * that order it among the table's calls reach its stream); the table stays valid and a later call can grow it.  Eviction still works against `capacity`: running out of HBM never evicts.  A call enqueued under stream
- * capture first backs the whole capacity (a replay never passes through the host's bound).  A growable table cannot be
- * exported (pb_table_export_view, pb_table_export_live_view) nor take a host tier (pb_table_attach_tier): PB_ERR_STATE.
- * pb_debug_owned counts the bytes backed, not those reserved.  Memory is not given back before the table is
- * destroyed (pb_table_clear and eviction keep it). */
+ * capture first backs the whole capacity (a replay never passes through the host's bound).  A table of mode 1 cannot
+ * be exported (pb_table_export_view, pb_table_export_live_view); no growable table can take a host tier
+ * (pb_table_attach_tier): PB_ERR_STATE.  pb_debug_owned counts the bytes backed, not those reserved.  Memory is not
+ * given back before the table is destroyed (pb_table_clear and eviction keep it).
+ * Mode 2, exportable growth: as mode 1, but every chunk is created exportable as a POSIX file descriptor, and the
+ * table can be exported, frozen or live (below: "Exportable growth").  Where the device does not report
+ * CU_DEVICE_ATTRIBUTE_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR_SUPPORTED, or the driver lacks cuMemExportToShareableHandle /
+ * cuMemImportFromShareableHandle, mode 2 is refused with PB_ERR_STATE and a message that says so.  `on`: 0 (off), 1 or
+ * 2; anything else PB_ERR_INVALID. */
 int pb_table_set_growth(pb_table* t, int on);
 /* [0] rows reserved (capacity), [1] rows backed by memory (= capacity on a table without growth), [2] index cells,
  * [3] admissions refused because their row was not backed (must stay 0).  Before the first allocation [1..3] are 0.
@@ -669,6 +674,39 @@ uint64_t pb_tier_view_bytes(void);
 int pb_table_export_tier_view(pb_table* t, void* h_blob);
 /* pb_view_open for a tiered view blob and its tier blob (above).  Blobs of different exports: PB_ERR_INVALID. */
 int pb_view_open_tiered(int device, const void* h_blob, const void* h_tier_blob, pb_view** out);
+/* ---- Exportable growth: reading a growing owner in place -----------------------------------------------------------
+ * A table of growth mode 2 exports, frozen or live, a view blob of the same size and layout marked version 3: the
+ * handle slots of its cells and rows hold the spans the owner reserved for them instead (no IPC handle describes a
+ * reservation backed chunk by chunk), and its write-sequence word has a second word after it, the index's current cell
+ * count.  pb_view_open opens it.  From the owner's process the view uses the owner's pointers.  From another it opens
+ * the counters and the word through CUDA IPC, reserves the same spans in its own address space, and listens on an
+ * abstract-namespace AF_UNIX socket (pb_view_address).  The owner registers that address (pb_table_add_reader) and
+ * sends over it, with SCM_RIGHTS, the descriptor, region, offset and size of every chunk of its rows and cells mapped so
+ * far, then of each new one, right after mapping it and before any kernel that can use it is enqueued.  Sends never
+ * block: one that would is kept and retried by the table's next call that can grow it.  A reader imports each chunk
+ * and maps it read-only (where the driver allows; else read-write) at the same offset of its reservation, at the start
+ * of every remote call; each descriptor is closed once imported, and pb_view_close unmaps and releases them all.
+ * Geometry: an index doubling moves every cell, so the exported table holds its write-sequence word odd around each
+ * doubling (in both export modes) and publishes the new cell count before the word is even again.  A remote read reads
+ * the count inside its window and probes with it.  It never touches an address its process has not mapped: an item
+ * whose owner's count (and 3 reserved cells) pass the cells mapped here, or whose row is at or above the rows mapped
+ * here, is stale, not read.  The call then copies the count of stale items to the host (one synchronisation of its
+ * stream per call, only when some owner is another process's growable table), imports what has arrived and reads the
+ * stale items again, waiting for a missing chunk for up to 20 s; still stale then, it fails with PB_ERR_STATE, and no
+ * output is written.  That synchronisation rules out stream capture: such a call under capture fails with
+ * PB_ERR_STATE before it launches anything (views in the owner's process and eager owners capture as before).  A kept
+ * send is retried only by the owner's next call that can grow the table (a training forward, an owner's SERVE,
+ * pb_set_rows, pb_image_insert): an owner that makes no such call again (a frozen Infer owner done loading) leaves a
+ * kept chunk unsent, and a reader that needs it fails after the wait.  Outputs are bit for bit those of the same reads
+ * of eager owners.  Owners with exportable growth
+ * and owners with shared tiers cannot be read in one call (PB_ERR_STATE). */
+/* The abstract socket name (without its leading NUL) a view of another process's growable table listens on, as a
+ * string in h_out (cap bytes); "" for every other view (nothing to register). */
+int pb_view_address(const pb_view* v, char* h_out, uint64_t cap);
+/* Registers a reader of t (a table of growth mode 2, exported either way) by its view's address (pb_view_address) and
+ * sends it every chunk mapped so far; "" does nothing.  The view must be open (else PB_ERR_STATE, and why).  A reader
+ * whose view has closed is dropped at the next send. */
+int pb_table_add_reader(pb_table* t, const char* addr);
 /* The inference form (training == 0) of pb_forward_sharded, served by this rank alone: arguments as pb_forward, plus
  * views[R] (owner q's table; views[rank] may be NULL: `own`, this rank's table, is probed directly), R and rank.  The
  * batch's distinct (slot, sign) items are read from their owners farmhash64(sign) % R into staging the context owns

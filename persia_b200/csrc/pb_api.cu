@@ -56,15 +56,24 @@ static size_t region_row_bytes(const pb_table* t, int r) {
 }
 
 // The chunks that back `rows` rows and `cells` index cells (+ N_SPECIAL), acquired into `o`; `mapped[r]` receives
-// each region's new extent.  Nothing is enqueued.
-static int map_growth(pb_table* t, uint64_t rows, uint64_t cells, Owned& o, size_t mapped[pb_table::G_COUNT]) {
+// each region's new extent, and `rec` the new chunks of the rows and the cells (exportable growth: what readers are
+// sent).  Nothing is enqueued.
+static int map_growth(pb_table* t, uint64_t rows, uint64_t cells, Owned& o, size_t mapped[pb_table::G_COUNT],
+                      std::vector<pb_table::Chunk>& rec) {
   for (int r = 0; r < pb_table::G_COUNT; ++r) {
     const size_t want = r == pb_table::G_CELLS ? sizeof(Cell) * ((size_t)cells + N_SPECIAL) : region_row_bytes(t, r) * rows;
     const size_t to = (want + t->gran - 1) / t->gran * t->gran;
     pb_table::Region& g = t->region[r];
     mapped[r] = g.mapped;
     if (to <= g.mapped) continue;
-    if (int rc = o.chunk(g.base + g.mapped, to - g.mapped, t->device)) return rc;
+    unsigned long long h = 0;
+    if (int rc = o.chunk(g.base + g.mapped, to - g.mapped, t->device, t->grow_share, &h)) return rc;
+    if (t->grow_share && (r == pb_table::G_ROWS || r == pb_table::G_CELLS)) {
+      int fd = -1;
+      if (CUresult e = vmm().export_fd(&fd, (CUmemGenericAllocationHandle)h, CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR, 0))
+        return fail(PB_ERR_CUDA, "cuMemExportToShareableHandle: CUresult " + std::to_string((int)e));
+      rec.push_back({(uint32_t)r, g.mapped, to - g.mapped, fd});
+    }
     mapped[r] = to;
   }
   return PB_OK;
@@ -89,16 +98,21 @@ static int acquire_growable(pb_table* t, Owned& o) {
     const size_t span = (region_reserved(t, r) + t->gran - 1) / t->gran * t->gran;
     t->region[r] = pb_table::Region{};
     if ((rc = o.reserve(t->region[r].base, span))) return rc;
+    t->region[r].span = span;
   }
   uint64_t rows = t->gran / region_row_bytes(t, pb_table::G_ROWS);
   rows = rows < 1 ? 1 : rows > d.capacity ? d.capacity : rows;
   uint64_t want = rows + rows / 2;
   const uint32_t cells = next_pow2(want < 1024 ? 1024 : want);
   size_t mapped[pb_table::G_COUNT];
-  if ((rc = map_growth(t, rows, cells, o, mapped)) || (rc = o.dev(d.counters, sizeof(uint32_t) * CTR_COUNT)) ||
+  std::vector<pb_table::Chunk> rec;
+  if ((rc = map_growth(t, rows, cells, o, mapped, rec)) || (rc = o.dev(d.counters, sizeof(uint32_t) * CTR_COUNT)) ||
       (rc = o.dev(t->evict_ws, sizeof(uint32_t) * EVICT_WS_WORDS)) ||
-      (rc = o.mapped(t->rb_host, t->rb_dev, 3 * sizeof(uint32_t))) || (rc = o.stream(t->grow_st)))
+      (rc = o.mapped(t->rb_host, t->rb_dev, 3 * sizeof(uint32_t))) || (rc = o.stream(t->grow_st))) {
+    for (const pb_table::Chunk& c : rec) close(c.fd);
     return rc;
+  }
+  t->readers.chunks = rec;
   for (int r = 0; r < pb_table::G_COUNT; ++r) t->region[r].mapped = mapped[r];
   d.cells = reinterpret_cast<Cell*>(t->region[pb_table::G_CELLS].base);
   d.rows = reinterpret_cast<float*>(t->region[pb_table::G_ROWS].base);
@@ -294,6 +308,7 @@ int wait_for(const Mark& m, cudaStream_t st) {
 // backed (a replay never passes here), the work enqueued outside the graph and waited for.  Any other table: nothing.
 int grow_for(pb_table* t, uint64_t n, cudaStream_t st) {
   if (!t->grow) return PB_OK;
+  if (t->grow_share) send_chunks(t);  // (sends an earlier call had to keep)
   unsigned long long cap_id = 0;
   PB_CUDA(capture_id(st, cap_id));
   TableDev& d = t->d;
@@ -332,9 +347,18 @@ int grow_for(pb_table* t, uint64_t n, cudaStream_t st) {
     const cudaStream_t ws = cap_id ? t->grow_st : st;
     Owned o;
     size_t mapped[pb_table::G_COUNT];
-    if (int rc = map_growth(t, rows, cells, o, mapped)) return rc;
+    std::vector<pb_table::Chunk> rec;
+    if (int rc = map_growth(t, rows, cells, o, mapped, rec)) {
+      for (const pb_table::Chunk& c : rec) close(c.fd);
+      return rc;
+    }
     t->own.adopt(o);
     for (int r = 0; r < pb_table::G_COUNT; ++r) t->region[r].mapped = mapped[r];
+    // readers in other processes get the new chunks before any kernel that can use them is enqueued
+    if (!rec.empty()) {
+      t->readers.chunks.insert(t->readers.chunks.end(), rec.begin(), rec.end());
+      send_chunks(t);
+    }
     if (rows > d.mapped)
       PB_CUDA(cudaMemsetAsync(d.row_tick + d.mapped, 0, sizeof(uint32_t) * (size_t)(rows - d.mapped), ws));
     d.mapped = (uint32_t)rows;
@@ -343,7 +367,11 @@ int grow_for(pb_table* t, uint64_t n, cudaStream_t st) {
       to.n_cells = (uint32_t)cells;
       to.cell_mask = cells - 1;
       to.bucket_mask = (uint32_t)(cells / BUCKET - 1);
+      // an exported table (exportable growth: live or frozen) holds its write-sequence word odd while every cell
+      // moves, and publishes the new cell count to its readers before it is even again (pb_remote.cu)
+      if (t->seq) launch_seq_bump(t->seq, true, ws);
       launch_grow_index(d, to, t->evict_ws, t->rebuild_keys, t->rebuild_rows, ws);
+      if (t->seq) launch_seq_bump(t->seq, false, ws, to.n_cells);
       d = to;
     }
     PB_CUDA(cudaGetLastError());
@@ -787,9 +815,15 @@ int pb_table_index_stats(pb_table* t, uint64_t h_out[3], void* stream) {
 
 int pb_table_set_growth(pb_table* t, int on) {
   if (!t) return fail(PB_ERR_INVALID, "null argument");
+  if (on < 0 || on > 2) return fail(PB_ERR_INVALID, "growth mode must be 0, 1 or 2");
   if (t->host) return fail(PB_ERR_STATE, "a host table's storage cannot grow");
   if (t->allocated) return fail(PB_ERR_STATE, "growth must be chosen before the table's first allocation");
+  if (on == 2 && !vmm_fd_supported(t->device))
+    return fail(PB_ERR_STATE, "exportable growth needs device memory that can be shared as POSIX file descriptors, "
+                              "and this device or driver does not report CU_DEVICE_ATTRIBUTE_HANDLE_TYPE_POSIX_FILE_"
+                              "DESCRIPTOR_SUPPORTED (or lacks cuMemExportToShareableHandle)");
   t->grow = on != 0;
+  t->grow_share = on == 2;
   return PB_OK;
 }
 
@@ -1030,3 +1064,11 @@ extern "C" int pb_debug_owned(uint64_t h_out[2]) {
   return PB_OK;
 }
 extern "C" void pb_debug_refuse_after(int64_t n) { g_refuse_after = n < 0 ? -1 : n; }
+// testing aid (not in include/persia_b200.h): an exportable growable table keeps every chunk it would send its readers
+// while `on` is set; clearing it sends them.  So a reader meets rows or cells it has not mapped yet, deterministically
+extern "C" int pb_debug_defer_sends(pb_table* t, int on) {
+  if (!t) return fail(PB_ERR_INVALID, "null argument");
+  t->readers.defer = on != 0;
+  if (!on) send_chunks(t);
+  return PB_OK;
+}

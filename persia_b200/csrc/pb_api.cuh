@@ -95,6 +95,7 @@ struct pb_table {
   struct Region {
     char* base = nullptr;
     size_t mapped = 0;
+    size_t span = 0;  // reserved
   };
   enum { G_ROWS, G_TICK, G_FREE, G_RKEYS, G_RROWS, G_CELLS, G_COUNT };
   Region region[G_COUNT];
@@ -111,6 +112,26 @@ struct pb_table {
   uint32_t* rb_host = nullptr;  // [3]: rows, used cells, stamp
   uint32_t* rb_dev = nullptr;
   cudaStream_t grow_st = nullptr;  // growth asked for under stream capture runs here, outside the graph
+  // exportable growth (pb_table_set_growth(t, 2)): every chunk is created exportable, and the chunks of the two regions
+  // a reader touches (rows, cells) are listed in mapping order.  Each reader registered in another process
+  // (pb_table_add_reader) is a connected socket and the number of listed chunks it has been sent (send_chunks)
+  // (each chunk's descriptor is exported once, when it is mapped, and kept open for the table's life)
+  bool grow_share = false;
+  struct Chunk {
+    uint32_t region;  // G_ROWS or G_CELLS
+    size_t off, bytes;
+    int fd;
+  };
+  struct Reader {
+    int sock;
+    size_t sent;
+  };
+  struct Readers {
+    std::vector<Chunk> chunks;
+    std::vector<Reader> r;
+    bool defer = false;  // pb_debug_defer_sends: nothing is sent until it is cleared
+    ~Readers();
+  } readers;
   Owned own;  // every CUDA resource above
 };
 
@@ -182,6 +203,10 @@ struct pb_ctx {
   // pb_forward_remote / pb_forward_raw_remote: the rows read from their owners, one per distinct item (grow_stage)
   float* remote_stage = nullptr;
   size_t remote_stage_floats = 0;
+  // ... and, when an owner is an exportable growable table in another process, the count of items its read found in
+  // rows or cells this process has not mapped yet, and its pinned copy
+  uint32_t* stale = nullptr;
+  uint32_t* stale_host = nullptr;
   Owned own;  // every CUDA resource above
 };
 enum { PREP_NONE = 0, PREP_SUM = 1, PREP_RAW = 2 };
@@ -259,6 +284,11 @@ int ensure_alloc(pb_table* t);
 int evict_check(pb_table* t, cudaStream_t st, uint32_t blocks = 0);
 int maybe_evict(pb_table* t, cudaStream_t st);
 int grow_for(pb_table* t, uint64_t n, cudaStream_t st);
+
+// ---- pb_api_view.cu ----------------------------------------------------------------------------------------------
+// an exportable growable table: every listed chunk its registered readers have not been sent yet, sent without
+// blocking (a send that would block is kept for the next call)
+void send_chunks(pb_table* t);
 void restore_ids(pb_table* t, bool prefix, const SlotsDev& sl, const uint64_t* ids, uint32_t n, cudaStream_t st);
 int writable(const pb_table* t);
 int ready_for_training(pb_table* t);

@@ -137,6 +137,19 @@ struct RemoteTierDev {
   RemoteDev rv;
   TableDev tier[PB_MAX_RANKS];
 };
+// k_remote_lookup<GROW>'s argument: owners whose tables are exportable growable ones.  geo[q]: owner q's published
+// index cell count (its write-sequence word's second word; null: the geometry in rv.t[q] holds); rows[q] / cells[q]:
+// the rows and index cell slots (with the N_SPECIAL reserved ones) this process has mapped of owner q.  An item whose
+// owner's index has more cells than are mapped here, or whose row is not mapped here, is stale: not read, its target
+// set to ROW_STALE and counted in *stale.  only_stale: items whose target is not ROW_STALE are skipped (a retry)
+struct RemoteGrowDev {
+  RemoteDev rv;
+  const uint32_t* geo[PB_MAX_RANKS];
+  uint32_t rows[PB_MAX_RANKS], cells[PB_MAX_RANKS];
+  uint32_t* stale;
+  uint32_t only_stale;
+};
+constexpr uint32_t ROW_STALE = 0xFFFFFFFDu;  // an item a remote read must read again once more chunks are mapped
 
 // arguments of the backward kernels (pb_reduce.cu)
 struct ReduceArgs {
@@ -283,11 +296,14 @@ void launch_count_owners(bool raw, const BatchDev& b, const RawWork& w, uint32_t
 // pb_remote.cu: the distinct items of the context's batch (raw: its numbered distinct signs) read from their owners into
 // `stage` at the item's number, f16(0 + row) or f32 rows (raw: f32), targets set to the item's number; err counts the
 // items whose read gave up (n: worst-case U)
-// tiers: the owners' host tiers (null: no owner has one, and the untiered kernels run)
-void launch_remote_lookup(bool raw, bool row_f32, const RemoteDev& rv, const TableDev* tiers, const BatchDev& b,
-                          const RawWork& w, uint32_t n, void* stage, uint32_t dim, uint32_t* err, cudaStream_t st);
-// an exported table's write-sequence word: odd from `begin` to the end of the writes that follow
-void launch_seq_bump(uint32_t* seq, bool begin, cudaStream_t st);
+// tiers: the owners' host tiers (null: no owner has one, and the untiered kernels run); grow: the owners' growth
+// (null: no owner grows, and the kernels without the stale check run; its `rv` is ignored: `rv` is used)
+void launch_remote_lookup(bool raw, bool row_f32, const RemoteDev& rv, const TableDev* tiers, const RemoteGrowDev* grow,
+                          const BatchDev& b, const RawWork& w, uint32_t n, void* stage, uint32_t dim, uint32_t* err,
+                          cudaStream_t st);
+// an exported table's write-sequence word: odd from `begin` to the end of the writes that follow.  cells (at the
+// end, nonzero): the index's new cell count, published in the word after it before it is even again
+void launch_seq_bump(uint32_t* seq, bool begin, cudaStream_t st, uint32_t cells = 0);
 // pb_shard.cu, raw slot over R shards: requester's route, table fill and gradient send (n: worst-case U)
 void launch_raw_route(const RawWork& w, uint32_t n, const XchgDev& x, cudaStream_t st);
 void launch_raw_fill(const RawWork& w, uint32_t n, uint32_t dim, const float* rows, void* table_f16, cudaStream_t st);

@@ -31,18 +31,21 @@ const Vmm& vmm() {
     w.ok = get("cuMemAddressReserve", w.reserve) & get("cuMemAddressFree", w.free) & get("cuMemCreate", w.create) &
            get("cuMemRelease", w.release) & get("cuMemMap", w.map) & get("cuMemUnmap", w.unmap) &
            get("cuMemSetAccess", w.access) & get("cuMemGetAllocationGranularity", w.granularity);
+    w.share = w.ok & get("cuMemExportToShareableHandle", w.export_fd) & get("cuMemImportFromShareableHandle", w.import_fd) &
+              get("cuDeviceGet", w.device_get) & get("cuDeviceGetAttribute", w.attribute);
     return w;
   }();
   return v;
 }
 
 namespace {
-CUmemAllocationProp vmm_prop(int device) {
+CUmemAllocationProp vmm_prop(int device, bool shareable = false) {
   CUmemAllocationProp prop;
   std::memset(&prop, 0, sizeof(prop));
   prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
   prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
   prop.location.id = device;
+  if (shareable) prop.requestedHandleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
   return prop;
 }
 }  // namespace
@@ -53,6 +56,16 @@ size_t vmm_granularity(int device) {
   const CUmemAllocationProp prop = vmm_prop(device);
   if (!v.ok || v.granularity(&g, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM) != CUDA_SUCCESS) return 0;
   return g;
+}
+
+bool vmm_fd_supported(int device) {
+  const Vmm& v = vmm();
+  CUdevice d = 0;
+  int on = 0;
+  if (!v.share || v.device_get(&d, device) != CUDA_SUCCESS ||
+      v.attribute(&on, CU_DEVICE_ATTRIBUTE_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR_SUPPORTED, d) != CUDA_SUCCESS)
+    return false;
+  return on != 0;
 }
 
 Owned::~Owned() {
@@ -71,9 +84,9 @@ int Owned::event(cudaEvent_t& ev) {
   return keep(e, "cudaEventCreateWithFlags", q, EVENT, 0, nullptr, ev);
 }
 
-int Owned::chunk(void* at, size_t bytes, int device) {
+int Owned::chunk(void* at, size_t bytes, int device, bool shareable, unsigned long long* handle) {
   const Vmm& v = vmm();
-  const CUmemAllocationProp prop = vmm_prop(device);
+  const CUmemAllocationProp prop = vmm_prop(device, shareable);
   CUmemGenericAllocationHandle h = 0;
   if (refused()) return fail(PB_ERR_CUDA, "cuMemCreate: refused");
   if (CUresult e = v.create(&h, bytes, &prop, 0))
@@ -90,6 +103,39 @@ int Owned::chunk(void* at, size_t bytes, int device) {
   if (e != CUDA_SUCCESS) {
     v.release(h);
     return fail(PB_ERR_CUDA, "cuMemMap / cuMemSetAccess: CUresult " + std::to_string((int)e));
+  }
+  held.push_back({at, VCHUNK, bytes, nullptr, -1, 0, (unsigned long long)h});
+  g_owned_count += 1;
+  g_owned_bytes += bytes;
+  if (handle) *handle = (unsigned long long)h;
+  return PB_OK;
+}
+
+int Owned::import_chunk(void* at, size_t bytes, int fd, int device) {
+  const Vmm& v = vmm();
+  CUmemGenericAllocationHandle h = 0;
+  if (refused()) {
+    close(fd);
+    return fail(PB_ERR_CUDA, "cuMemImportFromShareableHandle: refused");
+  }
+  CUresult e = v.import_fd(&h, reinterpret_cast<void*>((uintptr_t)fd), CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR);
+  close(fd);  // (the handle holds the allocation from here on)
+  if (e != CUDA_SUCCESS) return fail(PB_ERR_CUDA, "cuMemImportFromShareableHandle: CUresult " + std::to_string((int)e));
+  const CUdeviceptr q = reinterpret_cast<CUdeviceptr>(at);
+  if ((e = v.map(q, bytes, 0, h, 0)) == CUDA_SUCCESS) {
+    CUmemAccessDesc acc;
+    std::memset(&acc, 0, sizeof(acc));
+    acc.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+    acc.location.id = device;
+    acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READ;  // a reader never writes the owner's rows or cells ...
+    if (v.access(q, bytes, &acc, 1) != CUDA_SUCCESS) {
+      acc.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;  // ... where the driver can map device memory read-only
+      if ((e = v.access(q, bytes, &acc, 1)) != CUDA_SUCCESS) v.unmap(q, bytes);
+    }
+  }
+  if (e != CUDA_SUCCESS) {
+    v.release(h);
+    return fail(PB_ERR_CUDA, "cuMemMap / cuMemSetAccess of an imported chunk: CUresult " + std::to_string((int)e));
   }
   held.push_back({at, VCHUNK, bytes, nullptr, -1, 0, (unsigned long long)h});
   g_owned_count += 1;

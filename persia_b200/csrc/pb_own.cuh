@@ -5,7 +5,8 @@
 // acquires several resources acquires them into a local Owned and adopts it once every part has succeeded, then sets
 // its gate: a step that fails leaves nothing allocated and no gate set, and the next call acquires afresh.
 // A growable table's storage (pb_table_set_growth) is device address space reserved for its whole capacity and backed
-// by physical memory chunk by chunk: the reservation and each chunk are resources of their own.
+// by physical memory chunk by chunk: the reservation and each chunk are resources of their own.  A view of an
+// exportable growable table from another process reserves the same spans and maps the owner's chunks as they arrive.
 #pragma once
 #include <atomic>
 #include <cerrno>
@@ -54,12 +55,21 @@ struct Vmm {
   decltype(&cuMemSetAccess) access = nullptr;
   decltype(&cuMemGetAllocationGranularity) granularity = nullptr;
   bool ok = false;
+  // exportable growth (pb_table_set_growth(t, 2)): chunks handed to other processes as POSIX file descriptors.  `share`
+  // false: the driver lacks one of these (that mode is then refused; the others are unaffected)
+  decltype(&cuMemExportToShareableHandle) export_fd = nullptr;
+  decltype(&cuMemImportFromShareableHandle) import_fd = nullptr;
+  decltype(&cuDeviceGet) device_get = nullptr;
+  decltype(&cuDeviceGetAttribute) attribute = nullptr;
+  bool share = false;
 };
 
 const Vmm& vmm();
 
 // the size every chunk of `device` is a multiple of (0: no virtual-memory support)
 size_t vmm_granularity(int device);
+// whether `device` can export its chunks as POSIX file descriptors (CU_DEVICE_ATTRIBUTE_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR_SUPPORTED)
+bool vmm_fd_supported(int device);
 
 struct Owned {
   enum Kind { DEV, HOST, ASYNC, STREAM, EVENT, IPC, SHARED, VRESERVE, VCHUNK };
@@ -170,8 +180,13 @@ struct Owned {
     return PB_OK;
   }
   // `bytes` (a multiple of vmm_granularity) of `device`'s memory, created and mapped read-write at `at`, inside a
-  // reservation; undone as unmap, release
-  int chunk(void* at, size_t bytes, int device);
+  // reservation; undone as unmap, release.  shareable: created exportable as a POSIX file descriptor, its handle
+  // written to `handle`
+  int chunk(void* at, size_t bytes, int device, bool shareable = false, unsigned long long* handle = nullptr);
+  // another process's chunk (`fd`, from cuMemExportToShareableHandle; closed here whatever happens), imported and
+  // mapped at `at`, inside a reservation, for `device` to read (read-only where the driver allows it); undone as
+  // unmap, release
+  int import_chunk(void* at, size_t bytes, int fd, int device);
   // another process's allocation, mapped into this one
   int ipc(void*& p, const cudaIpcMemHandle_t& h);
 

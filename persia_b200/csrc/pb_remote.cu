@@ -29,6 +29,13 @@
 // (__threadfence_system) before the kernels that write cells or rows, and k_seq_end puts one between them and its store.
 // At .sys scope those fences and the reader's acquire/fence pair synchronise, whichever GPU or PCIe path carries the
 // data: a reader that reads the same even word twice read no row written inside a window.
+//
+// An owner with exportable growth (pb_table_set_growth(t, 2)): its rows and cells are chunks this process maps as they
+// arrive (pb_api_view.cu), and its index doubles under the readers.  k_remote_lookup<GROW> reads the owner's cell
+// count from the word after its sequence word, inside the same window (the owner publishes it inside the window that
+// holds the doubling), and probes with that geometry.  It touches no address this process has not mapped: an item is
+// stale, not read, when that count and the reserved cells pass the cells mapped here, or when the row found is at or
+// above the rows mapped here.  The caller imports what has arrived and reads the stale items again.
 #include "pb_device.cuh"
 #include "pb_probe.cuh"
 
@@ -50,15 +57,20 @@ __device__ __forceinline__ void fence_acq_rel_sys() { asm volatile("fence.acq_re
 
 __device__ __forceinline__ const RemoteDev& remote_of(const RemoteDev& a) { return a; }
 __device__ __forceinline__ const RemoteDev& remote_of(const RemoteTierDev& a) { return a.rv; }
-template <bool TIER>
-using RemoteArg = typename std::conditional<TIER, RemoteTierDev, RemoteDev>::type;
+__device__ __forceinline__ const RemoteDev& remote_of(const RemoteGrowDev& a) { return a.rv; }
+template <bool TIER, bool GROW>
+using RemoteArg = typename std::conditional<TIER, RemoteTierDev,
+                                            typename std::conditional<GROW, RemoteGrowDev, RemoteDev>::type>::type;
 
 // One lane group (BUCKET lanes) per distinct item; the grid strides over the items.  Must be called by whole warps.
 // TIER: a miss in the owner's HBM index is probed again in the owner's host tier (a.tier[owner]; cells null: it has none).
-template <bool RAW, bool ROW_F32, bool TIER>
-__global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteArg<TIER> a, BatchDev b, RawWork w,
+// GROW (never with TIER: a growable table has no tier): the owners' geometry and this process's mapped extents
+// (RemoteGrowDev).
+template <bool RAW, bool ROW_F32, bool TIER, bool GROW>
+__global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteArg<TIER, GROW> a, BatchDev b, RawWork w,
                                                                          void* __restrict__ stage, uint32_t dim,
                                                                          uint32_t* __restrict__ err) {
+  static_assert(!(TIER && GROW), "a growable table has no host tier");
   const RemoteDev& rv = remote_of(a);
   const uint32_t sub = threadIdx.x % BUCKET;
   const uint32_t lane = threadIdx.x & 31;
@@ -70,7 +82,7 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteAr
   const OptimDev op{};
   for (uint32_t j0 = warp_first; j0 < n_items; j0 += groups) {  // uniform per warp
     const uint32_t u = j0 + lane / BUCKET;
-    const bool valid = u < n_items;
+    bool valid = u < n_items;
     uint64_t sign = 0;
     uint32_t cell = 0;
     if (valid) {
@@ -82,10 +94,15 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteAr
         const uint4 hi = *(reinterpret_cast<const uint4*>(&b.set[cell]) + 1);
         sign = (hi.w >> 31) ? KEY_EMPTY : ((uint64_t)lo.x | ((uint64_t)lo.y << 32));
       }
+      if constexpr (GROW) {
+        if (a.only_stale) valid = (RAW ? w.target[u] : b.set[cell].target) == ROW_STALE;
+      }
     }
     const uint32_t owner = valid ? (uint32_t)(farmhash64_u64(sign) % rv.R) : 0u;  // sign_to_shard_modulo, mod.rs:341-345
     const TableDev& t = rv.t[owner];
     const uint32_t* seq = rv.seq[owner];
+    TableDev tg;  // GROW: the owner's table at the geometry it published
+    if constexpr (GROW) tg = t;
     bool todo = valid;
     uint32_t spins = 0;
     while (__any_sync(0xffffffffu, todo)) {
@@ -95,7 +112,25 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteAr
       if (todo && seq) s0 = seq_acquire(seq);
       const uint32_t s0_lead = __shfl_sync(0xffffffffu, s0, gshift);
       const bool go = todo && !(s0_lead & 1u);  // odd: an insert is running on the owner
-      const ProbeOut r = probe_group<MODE_FIND>(t, hy, op, sign, go, 0u, sub, gshift);
+      bool stale = false;
+      if constexpr (GROW) {
+        // the cell count the owner published, read after the word (ordered by its acquire); the group probes with
+        // its first lane's, and a doubling between the two reads of the word shows as a changed word
+        const uint32_t* geo = a.geo[owner];
+        uint32_t nc = 0;
+        if (go && geo) nc = *reinterpret_cast<const volatile uint32_t*>(geo);
+        nc = __shfl_sync(0xffffffffu, nc, gshift);
+        if (geo) {
+          stale = (uint64_t)nc + N_SPECIAL > a.cells[owner] || nc < BUCKET || (nc & (nc - 1));
+          if (!stale) {
+            tg.n_cells = nc;
+            tg.cell_mask = nc - 1;
+            tg.bucket_mask = nc / BUCKET - 1;
+          }
+        }
+      }
+      const ProbeOut r = probe_group<MODE_FIND>(GROW ? tg : t, hy, op, sign, go && !stale, 0u, sub, gshift);
+      if constexpr (GROW) stale = stale || (a.geo[owner] && r.row < t.capacity && r.row >= a.rows[owner]);
       // k_owner_lookup_tier's choice: the HBM row, else the tier row, else zeros
       const float* src = t.rows;
       uint32_t src_row = r.row, src_cap = t.capacity, src_stride = t.stride;
@@ -110,7 +145,7 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteAr
         }
       }
       const bool have = src_row < src_cap;
-      if (go) {
+      if (go && !stale) {
         // k_owner_lookup's conversion: f16(0 + row) for one-id layouts, the f32 row for ragged ones (zeros on a miss)
         const float* row = src + (size_t)(have ? src_row : 0u) * src_stride;
         if (dim % 4 == 0) {
@@ -144,9 +179,14 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteAr
       const uint32_t same = __ballot_sync(0xffffffffu, !go || (s0 == s0_lead && s1 == s0_lead));
       if (go && ((same >> gshift) & 0xFFu) == 0xFFu) {  // the item read whole by every lane, between two inserts
         if (sub == 0) {
-          if (!have) atomicAdd_system(&t.counters[CTR_MISS], 1u);  // counted on its owner, as there
-          if (RAW) w.target[u] = u;
-          else b.set[cell].target = u;
+          if (stale) {  // (GROW: read again once this process has mapped more of the owner's chunks)
+            if constexpr (GROW) atomicAdd(a.stale, 1u);
+          } else if (!have) {
+            atomicAdd_system(&t.counters[CTR_MISS], 1u);  // counted on its owner, as there
+          }
+          const uint32_t to = stale ? ROW_STALE : u;
+          if (RAW) w.target[u] = to;
+          else b.set[cell].target = to;
         }
         todo = false;
       } else if (todo && ++spins > PB_WAIT_SPINS) {  // the owner never finished its insert: give up, and say so
@@ -161,23 +201,31 @@ __global__ void __launch_bounds__(256, PB_PROBE_BLOCKS) k_remote_lookup(RemoteAr
   }
 }
 
-void launch_remote_lookup(bool raw, bool row_f32, const RemoteDev& rv, const TableDev* tiers, const BatchDev& b,
-                          const RawWork& w, uint32_t n, void* stage, uint32_t dim, uint32_t* err, cudaStream_t st) {
+void launch_remote_lookup(bool raw, bool row_f32, const RemoteDev& rv, const TableDev* tiers, const RemoteGrowDev* grow,
+                          const BatchDev& b, const RawWork& w, uint32_t n, void* stage, uint32_t dim, uint32_t* err,
+                          cudaStream_t st) {
   if (!n) return;
   const uint32_t full = cdiv((uint64_t)n * BUCKET, 256);  // worst case: every id a distinct item
   const uint32_t grid = full < PB_NUM_SMS * PB_PROBE_BLOCKS ? full : PB_NUM_SMS * PB_PROBE_BLOCKS;
-#define PB_R(RW, F32, TR, A) PB_LAUNCH_F(FAM_PROBE, (k_remote_lookup<RW, F32, TR>), grid, 256, 0, st, A, b, w, stage, dim, err)
+#define PB_R(RW, F32, TR, GR, A) \
+  PB_LAUNCH_F(FAM_PROBE, (k_remote_lookup<RW, F32, TR, GR>), grid, 256, 0, st, A, b, w, stage, dim, err)
   if (tiers) {
     RemoteTierDev a;
     a.rv = rv;
     for (uint32_t q = 0; q < PB_MAX_RANKS; ++q) a.tier[q] = tiers[q];
-    if (raw) PB_R(true, true, true, a);
-    else if (row_f32) PB_R(false, true, true, a);
-    else PB_R(false, false, true, a);
+    if (raw) PB_R(true, true, true, false, a);
+    else if (row_f32) PB_R(false, true, true, false, a);
+    else PB_R(false, false, true, false, a);
+  } else if (grow) {
+    RemoteGrowDev a = *grow;
+    a.rv = rv;
+    if (raw) PB_R(true, true, false, true, a);
+    else if (row_f32) PB_R(false, true, false, true, a);
+    else PB_R(false, false, false, true, a);
   } else {
-    if (raw) PB_R(true, true, false, rv);
-    else if (row_f32) PB_R(false, true, false, rv);
-    else PB_R(false, false, false, rv);
+    if (raw) PB_R(true, true, false, false, rv);
+    else if (row_f32) PB_R(false, true, false, false, rv);
+    else PB_R(false, false, false, false, rv);
   }
 #undef PB_R
 }
@@ -191,8 +239,16 @@ __global__ void k_seq_end(uint32_t* seq) {
   __threadfence_system();  // every entry written before
   *reinterpret_cast<volatile uint32_t*>(seq) = *seq + 1u;  // even again
 }
-void launch_seq_bump(uint32_t* seq, bool begin, cudaStream_t st) {
+// the end of an index doubling's window (exportable growth): the new cell count, then the word even again
+__global__ void k_seq_end_cells(uint32_t* seq, uint32_t cells) {
+  __threadfence_system();  // every cell written before
+  reinterpret_cast<volatile uint32_t*>(seq)[1] = cells;
+  __threadfence_system();
+  *reinterpret_cast<volatile uint32_t*>(seq) = *seq + 1u;
+}
+void launch_seq_bump(uint32_t* seq, bool begin, cudaStream_t st, uint32_t cells) {
   if (begin) PB_LAUNCH(k_seq_begin, 1, 1, 0, st, seq);
+  else if (cells) PB_LAUNCH(k_seq_end_cells, 1, 1, 0, st, seq, cells);
   else PB_LAUNCH(k_seq_end, 1, 1, 0, st, seq);
 }
 

@@ -12,6 +12,7 @@ SO_PATH = os.environ.get("PERSIA_B200_LIB") or os.path.join(_HERE, "libpersia_b2
 PB_MAX_SLOTS = 128
 OPT_SGD, OPT_ADAGRAD, OPT_ADAGRAD_VW, OPT_ADAM = 0, 1, 2, 3
 RSQRT_EXACT, RSQRT_INTEL = 0, 1  # pb_rsqrt_mode
+GROW_OFF, GROW_ON, GROW_SHARED = 0, 1, 2  # pb_table_set_growth modes (2: growable and exportable)
 
 PHASE_SEND, PHASE_SERVE, PHASE_FINISH, PHASE_ALL, PHASE_PREPARE = 1, 2, 4, 7, 8
 PB_OK, PB_ERR_INVALID, PB_ERR_CUDA, PB_ERR_STATE, PB_ERR_CAPACITY, PB_ERR_BATCH, PB_ERR_FORMAT = 0, -1, -2, -3, -4, -5, -6
@@ -124,6 +125,8 @@ SYMBOLS = {
     "pb_tier_view_bytes": (_u64, []),
     "pb_table_export_tier_view": (_i32, [_vp, _vp]),
     "pb_view_open_tiered": (_i32, [_i32, _vp, _vp, C.POINTER(_vp)]),
+    "pb_view_address": (_i32, [_vp, C.c_char_p, _u64]),
+    "pb_table_add_reader": (_i32, [_vp, C.c_char_p]),
     "pb_forward_remote": (_i32, [_vp, C.POINTER(_vp), _u32, _u32, _vp, _vp, _u32, _vp, C.POINTER(_u32), _u32, _vp, _vp]),
     "pb_forward_raw_remote": (_i32, [_vp, C.POINTER(_vp), _u32, _u32, _vp, _vp, _u32, _vp, _u32, _u32, _vp, _vp, _vp, _vp,
                                      _vp, _vp]),

@@ -39,8 +39,12 @@ it pins it again, and the ranks must run as one user in one PID namespace (a pee
 PERSIA_B200_GROW=1 (growth_on) makes every dim group's table growable: `capacity` bounds each table instead of
 reserving HBM for it, and HBM backs rows and index cells as entries are admitted, so a config with several dims or the
 reference's default capacity of 1e9 costs what its resident entries cost.  Every dim still has its own `capacity`.  It
-is an opt-in, read when a dim group is created, so that the default stays today's allocation; it is refused at
-replica_size > 1 (tables are exported there) and together with PERSIA_B200_HBM_ROWS, before any table exists.
+is an opt-in, read when a dim group is created, so that the default stays today's allocation.  At replica_size > 1
+tables are exported for remote reads, which PERSIA_B200_GROW=1's tables cannot be: there PERSIA_B200_GROW=shared is
+needed, which makes them growable and exportable (growth mode 2: each rank's peers receive its chunks as they are
+mapped, over a socket, and read while the table grows, _start_remote).  It works at any replica_size, for Train jobs
+(live exports) and Infer jobs (frozen exports, grown by checkpoint loads and incremental packets).  Both are refused
+together with PERSIA_B200_HBM_ROWS, before any table exists.
 """
 import os
 import queue
@@ -129,23 +133,25 @@ def adagrad_rsqrt():
 
 
 def growth_on(grow, replica_size=1, hbm_rows=None):
-    """PERSIA_B200_GROW (`grow`; "1" on, None, "" or "0" off): every dim group's table is growable
+    """PERSIA_B200_GROW (`grow`; "1" or "shared" on, None, "" or "0" off): every dim group's table is growable
     (pb_table_set_growth): `capacity` bounds it and HBM backs its rows and index as entries are admitted, so the
-    reference's capacities (1e9 by default) can be configured as they are.  Refused at replica_size > 1 (a Train job
-    exports its tables live, an Infer job frozen, and a growable table cannot be exported) and together with
-    PERSIA_B200_HBM_ROWS (`hbm_rows`: a growable table has no host tier)."""
+    reference's capacities (1e9 by default) can be configured as they are.  Returns False, True ("1") or "shared"
+    (EmbeddingShard's `grow`).  "1" is refused at replica_size > 1 (a Train job exports its tables live, an Infer job
+    frozen, and its tables cannot be exported); "shared" makes them exportable and works at any replica_size.  Both are
+    refused together with PERSIA_B200_HBM_ROWS (`hbm_rows`: a growable table has no host tier)."""
     v = "" if grow is None else str(grow).strip()
-    if v not in ("", "0", "1"):
-        raise RuntimeError(f"PERSIA_B200_GROW must be '1' or '0', got {v!r}")
-    if v != "1":
+    if v not in ("", "0", "1", "shared"):
+        raise RuntimeError(f"PERSIA_B200_GROW must be '1', 'shared' or '0', got {v!r}")
+    if v in ("", "0"):
         return False
-    if (replica_size or 1) > 1:
-        raise RuntimeError("PERSIA_B200_GROW (tables that grow with their entries) is supported on one GPU only "
-                           f"(replica_size = 1, got {replica_size}): its tables are exported for remote reads there")
+    if v == "1" and (replica_size or 1) > 1:
+        raise RuntimeError("PERSIA_B200_GROW=1 (tables that grow with their entries) is supported on one GPU only "
+                           f"(replica_size = 1, got {replica_size}): its tables are exported for remote reads there; "
+                           "PERSIA_B200_GROW=shared makes them exportable")
     if hbm_rows is not None and str(hbm_rows).strip() != "":
-        raise RuntimeError("PERSIA_B200_GROW cannot be combined with PERSIA_B200_HBM_ROWS: a growable table has no "
+        raise RuntimeError(f"PERSIA_B200_GROW={v} cannot be combined with PERSIA_B200_HBM_ROWS: a growable table has no "
                            "host-memory tier")
-    return True
+    return True if v == "1" else "shared"
 
 
 def shared_tier_on():
@@ -441,6 +447,13 @@ def _start_remote(live=False):
     for d, g in groups.items():
         views = [SH.TableView(got[q][d], g["shard"].device) if q != rank else None for q in range(len(got))]
         readers[d] = RemoteReader(g["shard"], views, rank)
+    if any(g["shard"].grow_shared for g in groups.values()):  # (PERSIA_B200_GROW=shared: the same on every rank)
+        addrs = [None] * len(got)  # each rank's view addresses, per dim and owner
+        dist.all_gather_object(addrs, {d: [v.address if v is not None else "" for v in r.views]
+                                       for d, r in readers.items()})
+        for d, g in groups.items():
+            with g["lock"]:
+                g["shard"].add_readers([a[d][rank] for a in addrs])
     dist.barrier()  # (no rank reads before every view is open)
     _S.remote = readers
     global _CLOSE_AT_EXIT

@@ -160,6 +160,18 @@ def rsqrt_mode(mode):
     return int(mode)
 
 
+def grow_mode(grow):
+    """EmbeddingShard's `grow` as a pb_table_set_growth mode: False / None / 0 / "0" / "" off, True / 1 / "1" growable,
+    "shared" / 2 growable and exportable."""
+    if grow is None or grow is False or str(grow).strip() in ("", "0"):
+        return N.GROW_OFF
+    if grow is True or str(grow).strip() == "1":
+        return N.GROW_ON
+    if str(grow).strip() in ("shared", "2"):
+        return N.GROW_SHARED
+    raise ValueError(f"unknown growth mode {grow!r}: expected False, True or 'shared'")
+
+
 class EmbeddingShard:
     def __init__(self, dim, capacity, device=0, tier_rows=0, host=False, shared_tier=False, grow=False):
         """capacity: rows in HBM.  tier_rows > 0: a host-memory tier of that many rows behind them (include/persia_b200.h,
@@ -167,9 +179,11 @@ class EmbeddingShard:
         (the tier itself).  shared_tier: the tier's rows are shared memory other processes can map
         (pb_table_create_host_shared), so that the table can be exported and its peers read the tier in place.
         grow: capacity bounds the table instead of reserving it: HBM backs rows and index cells as entries are admitted
-        (pb_table_set_growth; no tier, no export)."""
+        (pb_table_set_growth; no tier).  True or "1": no export; "shared": exportable (growth mode 2), so that peers
+        read it in place while it grows (register their views with add_readers)."""
         if grow and (host or tier_rows):
             raise ValueError("a growable table has no host tier and is not one")
+        mode = grow_mode(grow)
         self.lib = N.load()
         self.dim, self.capacity = int(dim), int(capacity)
         self.device = torch.device("cuda", device) if not isinstance(device, torch.device) else device
@@ -180,9 +194,10 @@ class EmbeddingShard:
             create = self.lib.pb_table_create_host_shared if shared_tier else self.lib.pb_table_create_host
         N.check(create(self.device.index or 0, C.byref(cfg), C.byref(h)))
         self.h = h
-        self.grow = bool(grow)
+        self.grow = mode != N.GROW_OFF
+        self.grow_shared = mode == N.GROW_SHARED
         if self.grow:
-            N.check(self.lib.pb_table_set_growth(h, 1))
+            N.check(self.lib.pb_table_set_growth(h, mode))
         self._entry_len = None
         self.shared_tier = bool(shared_tier and tier_rows)
         self.host_tier = EmbeddingShard(dim, tier_rows, device, host=True, shared_tier=shared_tier) if tier_rows else None
@@ -422,6 +437,16 @@ class EmbeddingShard:
         or after it.  One table, one export mode; the table must outlive every view of it."""
         return self._export(self.lib.pb_table_export_live_view)
 
+    def add_readers(self, addresses):
+        """Registers the views of this exported table opened in other processes (TableView.address of each; "" and
+        None are skipped) so that they receive its chunks as it grows (pb_table_add_reader).  Only a table created with
+        grow="shared" has readers; for any other this does nothing."""
+        if not self.grow_shared:
+            return
+        for a in addresses:
+            if a:
+                N.check(self.lib.pb_table_add_reader(self.h, a.encode() if isinstance(a, str) else bytes(a)))
+
     def _export(self, call):
         buf = C.create_string_buffer(int(self.lib.pb_table_view_bytes()))
         N.check(call(self.h, buf))
@@ -462,6 +487,15 @@ class TableView:
             assert len(blob) == n, "not a table view blob"
             N.check(self.lib.pb_view_open(self.device.index or 0, blob, C.byref(h)))
         self.h = h
+
+    @property
+    def address(self):
+        """The socket address the owner of a growable table (grow="shared") in another process sends its chunks to
+        (EmbeddingShard.add_readers); "" for every other view.  Chunks that have arrived are mapped by each remote
+        call itself."""
+        buf = C.create_string_buffer(108)
+        N.check(self.lib.pb_view_address(self.h, buf, len(buf)))
+        return buf.value.decode()
 
     def close(self):
         if getattr(self, "h", None):

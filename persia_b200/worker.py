@@ -61,8 +61,8 @@ class ShardedEmbeddingWorker:
         the new shard has a host-memory tier of that many rows behind its `capacity` HBM rows (EmbeddingShard; a
         caller's `shard` brings its own tier or none); shared_tier: that tier is shared memory, so the shard can be exported
         to a RemoteReader (EmbeddingShard).  rsqrt: the new shard's Adagrad rsqrt mode (EmbeddingShard.set_rsqrt; None:
-        exact).  grow: the new shard's storage grows with its entries (EmbeddingShard; not with a tier, and a growable
-        shard cannot be exported).  Statistics: `self.shard.tier_stats()`, `self.shard.storage_stats()`."""
+        exact).  grow: the new shard's storage grows with its entries (EmbeddingShard; not with a tier): True, or
+        "shared" so that it can also be exported to a RemoteReader.  Statistics: `self.shard.tier_stats()`, `self.shard.storage_stats()`."""
         self.S, self.dim, self.rank, self.R, self.cap = n_slots, dim, rank, world, int(cap)
         self.device = device if isinstance(device, torch.device) else torch.device("cuda", device)
         self.lib = N.load()
@@ -567,6 +567,22 @@ class TierStager:
             pass
 
 
+def exchange_readers(shard, views, group=None):
+    """R GPUs with exportable growable owners (grow="shared"): every rank's view addresses (TableView.address, one per
+    owner) are exchanged with one all_gather_object, and this rank's shard registers the views of it its peers opened
+    (EmbeddingShard.add_readers), so that they receive its chunks as it grows.  Collective; after every view is open.
+    Skipped on every rank when no rank's shard grows shared (the same on all ranks)."""
+    import torch.distributed as dist
+
+    if not shard.grow_shared:
+        return
+    grp = group if group is not None else dist.group.WORLD
+    rank = dist.get_rank(grp)
+    addrs = [None] * dist.get_world_size(grp)
+    dist.all_gather_object(addrs, [v.address if v is not None else "" for v in views], group=grp)
+    shard.add_readers([a[rank] for a in addrs])
+
+
 class RemoteReader:
     """Inference on R GPUs one rank at a time (pb_forward_remote / pb_forward_raw_remote): this rank's requests are
     served alone, whatever its peers do.  The requesting GPU probes each owner's index and reads its rows in place,
@@ -614,6 +630,7 @@ class RemoteReader:
         blobs = [None] * world
         dist.all_gather_object(blobs, shard.export_view(), group=grp)
         views = [SH.TableView(b, shard.device) if q != rank else None for q, b in enumerate(blobs)]
+        exchange_readers(shard, views, grp)
         dist.barrier(group=grp)  # (no rank reads before every view is open)
         return cls(shard, views, rank, stream=stream)
 
